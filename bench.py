@@ -1,9 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/sec of the marlbase hot path on B200 (BASELINE.json metric) next to the CPU reference loop.
+"""bench.py -- env-steps/sec of the marlbase hot path on H100 (BASELINE.json metric) next to the CPU reference loop.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config idqn|vdn15|ia2c]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config idqn|vdn15|ia2c] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
+`--dump-outputs DIR` writes, after the timed steps, what the timed path computed in its last step as DIR/<name>.npy (float32): parameters,
+optimiser state and metrics after the last update, the last env step's network outputs, the episode lengths / returns and a fixed sample of
+the episodes collected.  Model initialisation, environments and replay sampling are seeded by --seed, so two builds can be compared array by array.
 Default workload (`--config idqn`) = BASELINE.json configs[1], the configuration the metric is quoted on: IDQN on
 Foraging-8x8-2p-3f-v3, 4096 envs per GPU, batch_size 1024.  A "step" is one training iteration of the hot path on every GPU: E envs
 collect one episode each (<= 25 env steps; fused forward + epsilon-greedy + transition + replay write per env step) followed by
@@ -38,11 +41,8 @@ WORKLOADS = {
     "ia2c": dict(algo="ia2c", baseline_config=2, env="lbforaging:Foraging-8x8-2p-3f-v3", lbf=dict(rows=8, cols=8, n_agents=2, max_num_food=3, sight=8),
                  envs=8192, batch=0, buffer=0, wrappers=None),
 }
-# dram__bytes_read.sum + dram__bytes_write.sum of one launch of the idqn workload: ncu --set full, one kernel at a time with ncu's cache flush in
-# front (cold L2; profiles/r1_tc_pipeline.md).  The warm, pipelined figure of the whole update is in profiles/r2_dram_traffic.md.
-TRAFFIC_NCU = {"tc_dqn_fwd_kernel": 9303552, "tc_dh1_kernel": 3705344, "tc_dw_kernel": 92672512,
-               # on-chip pass (round 2): dram__bytes of one launch inside the running pipeline (ncu --cache-control none, profiles/r2_dram_traffic.md)
-               "tc_dqn_fwd3_kernel": 4300000, "tc_dh1w1_kernel": 10300000, "tc_dw2_kernel": 10300000}
+# H100 SXM data sheet (dense, 700 W card): fallbacks when MEASURED_PEAKS.json is absent; a card with a lower power limit reaches less
+H100_HBM_GBS, H100_BF16_TFLOPS, H100_MAX_SM_MHZ = 3350.0, 989.0, 1980.0
 
 
 def parse():
@@ -51,7 +51,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--config", default="idqn", choices=sorted(WORKLOADS), help="idqn = BASELINE configs[1] (default, what the driver runs), vdn15 = configs[3], ia2c = configs[2]")
+    ap.add_argument("--config", default="idqn", choices=sorted(WORKLOADS), help="idqn = BASELINE configs[1] (default), vdn15 = configs[3], ia2c = configs[2]")
     ap.add_argument("--envs", type=int, default=0, help="env instances per GPU (0 = the workload's value)")
     ap.add_argument("--batch", type=int, default=0)
     ap.add_argument("--buffer", type=int, default=0, help="replay ring capacity in episodes (per GPU)")
@@ -61,8 +61,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--collective", default="peer", choices=["peer", "nccl"],
                     help="N > 1: gradient exchange inside the fused reduce + Adam kernel over NVLink peer memory (default), or one NCCL all-reduce per update")
-    ap.add_argument("--tc-backward", type=int, default=1, help="1 = tcgen05 training pipeline (default), 0 = fused FP32 FFMA training kernel")
-    ap.add_argument("--tc-onchip", type=int, default=1, help="1 = training pass with H1 / H2 / dH1 kept on chip (tc_train3.cu, default), 0 = streamed through global memory (tc_train.cu)")
+    ap.add_argument("--tc-backward", type=int, default=1, help="1 = tensor-core (wgmma) training pipeline (default), 0 = fused FP32 FFMA training kernel")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write what the timed path computed in its last step to DIR/<name>.npy")
     a = ap.parse_args()
     wl = WORKLOADS[a.config]
     a.envs = a.envs or wl["envs"]
@@ -137,7 +137,7 @@ def plan_a(args, seconds=120.0):
         import omegaconf  # noqa: F401
     except Exception as e:  # noqa: BLE001
         return None, f"{type(e).__name__}: {e}"
-    marlbase = os.path.join(ROOT, "baseline", "_ref", "marlbase")   # a driver-provided install; /root/reference does not exist on the GPU box
+    marlbase = os.path.join(ROOT, "baseline", "_ref", "marlbase")   # an optional (git-ignored) checkout of the reference project
     if not os.path.exists(os.path.join(marlbase, "run.py")):
         return None, "third-party packages import, but no marlbase/run.py under baseline/_ref"
     wl = WORKLOADS[args.config]
@@ -227,7 +227,37 @@ def load_peaks():
         return {}
 
 
-# ---- B200 arm: shared scaffolding ------------------------------------------------------------------------------------------------
+def gpu_info(torch, dev):
+    """The card the numbers were measured on: name and power limit (a power-capped card runs lower clocks under load)."""
+    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(dev.index)], capture_output=True, text=True, timeout=60)
+        info["power_limit_w"] = float(out.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        pass
+    return info
+
+
+def episode_sample(torch, n, k=512, seed=1234):
+    """A fixed, seeded sample of k of n episode slots (sorted), so that dumps stay small at every workload size."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.randperm(n, generator=g)[:min(k, n)].sort().values
+
+
+def dump_outputs(out_dir, arrays):
+    """name -> tensor, written as DIR/<name>.npy in float32 (64 MB at most in all)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    host = {name: t.detach().float().cpu().numpy() for name, t in arrays.items()}
+    total = sum(a.nbytes for a in host.values())
+    if total > 64 << 20:
+        raise SystemExit(f"bench.py: --dump-outputs would write {total} bytes (> 64 MB)")
+    for name, a in host.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
+# ---- GPU arm: shared scaffolding ------------------------------------------------------------------------------------------------
 class Harness:
     """Process-group set-up, the timed-region protocol (barrier + synchronize on both sides, CUDA events, max over ranks), clocks."""
 
@@ -238,7 +268,7 @@ class Harness:
         self.torch, self.dist, self.args = torch, dist, args
         self.rank, self.world, self.local = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("LOCAL_RANK", "0"))
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py: no CUDA device -- the B200 path has no CPU fallback")
+            raise SystemExit("bench.py: no CUDA device -- the GPU path has no CPU fallback")
         torch.cuda.set_device(self.local)
         self.dev = torch.device("cuda", self.local)
         if self.world > 1:
@@ -299,6 +329,7 @@ def run_dqn_family(args, wl):
     env = make_env(args.seed, name=wl["env"], time_limit=T, parallel_envs=E, env_gid0=rank * E, wrappers=wl["wrappers"])
     cfg = Config(dict(optimizer="Adam", lr=3e-4, gamma=0.99, grad_clip=1.0, double_q=True, target_update_interval_or_tau=200, standardise_returns=False))
     cls = VDNetwork if wl["algo"] == "vdn" else QNetwork
+    torch.manual_seed(args.seed)   # the initial parameters: same arguments, same inputs
     model = cls(env.single_observation_space, env.single_action_space, cfg, [128, 128], False, False, True, "cuda", max_batch=B, max_episode_length=T)
     if world > 1 and args.collective == "peer":
         try:
@@ -318,7 +349,6 @@ def run_dqn_family(args, wl):
     coll = Collector(env, model, T)
     lib = nat.lib()
     nat.check(lib.marl_set_option(b"tensor_core_backward", C.c_int32(int(args.tc_backward))), "marl_set_option")
-    nat.check(lib.marl_set_option(b"tensor_core_onchip", C.c_int32(int(args.tc_onchip))), "marl_set_option")
     state = dict(pos=0, updates=0)
     steps_dev = H.steps_dev
     # pinned host mirrors for the e2e leg
@@ -350,7 +380,7 @@ def run_dqn_family(args, wl):
         slot0 = state["pos"] % args.buffer
         eps = 0.5
         if not host_boundary:
-            final_len, _ = coll.collect(rb, slot0, eps)
+            final_len, final_ret = coll.collect(rb, slot0, eps)
         else:  # every env step's observations enter through pinned host memory and its results return to it
             nat_env.reset(traj=rb, slot0=slot0)
             h_obs.copy_(nat_env.obs, non_blocking=True)
@@ -362,8 +392,9 @@ def run_dqn_family(args, wl):
                 h_obs.copy_(nat_env.obs, non_blocking=True); h_rew.copy_(nat_env.rew, non_blocking=True)      # D2H: this step's results
                 h_done.copy_(nat_env.done, non_blocking=True); h_trunc.copy_(nat_env.trunc, non_blocking=True)
                 torch.cuda.current_stream().synchronize()                                 # the host "sees" the step before the next one
-            final_len = nat_env.final_len
+            final_len, final_ret = nat_env.final_len, nat_env.final_ret
         steps_dev.add_(final_len.sum())
+        state.update(slot0=slot0, final_len=final_len, final_ret=final_ret)
         state["pos"] += E
         do_updates()
         if host_boundary:
@@ -374,10 +405,17 @@ def run_dqn_family(args, wl):
     sampler = ClockSampler(H.local) if rank == 0 else None
     ms, n_steps = H.timed(args.steps, lambda: iteration(False))
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        ep = episode_sample(torch, E).to(dev)
+        slots = (state["slot0"] + ep) % args.buffer
+        dump_outputs(args.dump_outputs, {"theta": model.theta, "theta_tgt": model.theta_tgt, "adam_m": model.adam_m, "adam_v": model.adam_v,
+                                         "metrics": model._metrics, "q_last_env_step": coll.q, "episode_length": state["final_len"],
+                                         "episode_return": state["final_ret"], "episode_index": ep, "replay_obs": rb.obs[slots], "replay_act": rb.act[slots],
+                                         "replay_rew": rb.rew[slots], "replay_done": rb.done[slots], "replay_filled": rb.filled[slots]})
 
-    # ---- multi-GPU correctness, driver visible: replicated parameters must be BIT-identical on every rank after the timed region, and the in-kernel
+    # ---- multi-GPU correctness: replicated parameters must be BIT-identical on every rank after the timed region, and the in-kernel
     # peer-memory exchange must agree with the plain NCCL all-reduce path on one update from the same state (tests/test_peer_exchange_gpu.py asserts
-    # the same; the driver's GPU test box has one GPU, so the evidence is emitted here) ------------------------------------------------------------
+    # the same on a box with several GPUs) ------------------------------------------------------------------------------------------------------
     multi = None
     if world > 1:
         fp = theta_fingerprint(torch, model.theta)
@@ -429,39 +467,31 @@ def run_dqn_family(args, wl):
     FWD = fwd_flop_per_row(obs_dim, n_act)
     train_flop = 3 * rows * FWD             # online forward (1x) + backward (2x) of one update
     train_avg_s = (train_ms / max(train_n, 1)) / 1e3
-    sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
+    sm_mhz = (clocks or {}).get("sm_mhz") or H100_MAX_SM_MHZ
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
     fp32_peak = n_sm * 128 * 2 * sm_mhz * 1e6 / 1e12    # FFMA lanes x 2 flop x clock actually seen during the run
     peaks = load_peaks()
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
-    tensor_peak = peaks.get("bf16_tflops_sustained", 1443.2)   # sustained figure: the kernel is timed inside a long step
+    hbm_peak = peaks.get("hbm_gbs", H100_HBM_GBS)
+    tensor_peak = peaks.get("bf16_tflops_sustained", H100_BF16_TFLOPS)
     per_update_us = 1e3 * (ms / args.steps) / U   # upper bound: includes the rollout's share of the iteration
     if kernel_n:
-        # tensor-core training pass (DESIGN.md section 4.3): three kernels; the roofline object describes the slowest one
+        # tensor-core training pass (tc_train.cu): three kernels; the roofline object describes the slowest one
         P_net = model.n_params // model.n_nets
-        if args.tc_onchip:
-            names = ["tc_dqn_fwd3_kernel", "tc_dh1w1_kernel", "tc_dw2_kernel"]
-            flops = [rows * FWD + rows * 2 * (n_act * HIDDEN + n_act),                  # online forward, dW3 | db3
-                     rows * 2 * HIDDEN * HIDDEN + rows * 2 * HIDDEN * (obs_dim + 1),     # dH1 = dH2 x W2, dW1 | db1
-                     rows * 2 * HIDDEN * (HIDDEN + 1)]                                   # dW2 | db2 (the recomputed layer 1, rows * 2 * obs * 128, is overhead and not counted)
-            # algorithmic HBM bytes: what crosses the kernels is the gathered observation row (stored 32 floats wide) and the 64-byte row record
-            inter = [rows * (obs_dim * 4 + n_act * 4) + rows * (128 + 64) + n_sm * 4 * (n_act * HIDDEN + n_act),
-                     rows * (128 + 64) + n_sm * 4 * HIDDEN * (obs_dim + 1), rows * (128 + 64) + n_sm * 4 * HIDDEN * (HIDDEN + 1)]
-        else:
-            names = ["tc_dqn_fwd_kernel", "tc_dh1_kernel", "tc_dw_kernel"]
-            flops = [rows * FWD,                                                       # online forward
-                     rows * 2 * HIDDEN * HIDDEN,                                       # dH1 = dH2 x W2
-                     rows * 2 * (HIDDEN * HIDDEN + HIDDEN * obs_dim + n_act * HIDDEN + HIDDEN + HIDDEN + n_act)]   # dW2, dW1, dW3 and the bias sums
-            # algorithmic HBM bytes per update: H1, H2 written + read, dH1 written + read (FP32), 64-byte row records written + read twice,
-            # gathered observations, target outputs, per-CTA gradient partials
-            inter = [rows * (2 * 512 + 64) + rows * obs_dim * 4 + rows * n_act * 4, rows * (512 + 64), rows * (3 * 512 + 64 + obs_dim * 4) + n_sm * 4 * P_net]
+        names = ["tc_dqn_fwd_kernel", "tc_dh1_kernel", "tc_dw_kernel"]
+        flops = [rows * FWD,                                                       # online forward
+                 rows * 2 * HIDDEN * HIDDEN,                                       # dH1 = dH2 x W2
+                 rows * 2 * (HIDDEN * HIDDEN + HIDDEN * obs_dim + n_act * HIDDEN + HIDDEN + HIDDEN + n_act)]   # dW2, dW1, dW3 and the bias sums
+        # algorithmic HBM bytes per update: observations read, H1, H2 (FP32, 512 B per row each), observations, outputs and ReLU masks written;
+        # outputs, masks and target outputs read, dH1 written; H1, H2, dH1, observations and row records read, per-CTA gradient partials written
+        inter = [rows * (2 * 512 + obs_dim * 4 + 64) + rows * obs_dim * 4, rows * (512 + 96) + rows * n_act * 4,
+                 rows * (3 * 512 + 8 + obs_dim * 4) + n_sm * 4 * P_net]
         us = [1e3 * m / kernel_n for m in kernel_ms]
         k = max(range(3), key=lambda i: us[i])
         achieved = flops[k] / (us[k] * 1e-6) / 1e12
         roofline = {"bound": "tensor", "kernel": names[k], "achieved": achieved, "peak": tensor_peak, "unit": "TFLOP/s", "frac": achieved / tensor_peak,
-                    "traffic": TRAFFIC_NCU.get(names[k]) if args.config == "idqn" else None,   # dram bytes of one launch (ncu)
-                    "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (dense bf16; TF32 runs at half of it and 3xTF32 needs three MMAs per "
-                                   "FP32-accurate product: the FP32-equivalent ceiling of this arithmetic is peak / 6)",
+                    "traffic": None,
+                    "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet, dense BF16") +
+                                   " (TF32 runs at half of it and 3xTF32 needs three MMAs per FP32-accurate product: the FP32-equivalent ceiling of this arithmetic is peak / 6)",
                     "fp32_equivalent_peak": tensor_peak / 6, "frac_of_fp32_equivalent_peak": achieved / (tensor_peak / 6),
                     "launch_us": us[k], "launches_timed": kernel_n, "flop_per_launch": flops[k],
                     "kernels": {names[i]: {"launch_us": us[i], "flop": flops[i], "tflops": flops[i] / (us[i] * 1e-6) / 1e12,
@@ -473,17 +503,17 @@ def run_dqn_family(args, wl):
                     "whole_update": {"us_upper_bound": per_update_us, "flop": 4 * rows * FWD, "tflops": 4 * rows * FWD / (per_update_us * 1e-6) / 1e12,
                                      "frac_of_fp32_equivalent_peak": 4 * rows * FWD / (per_update_us * 1e-6) / 1e12 / (tensor_peak / 6),
                                      "note": "headline ms_per_step / updates_per_iteration (rollout included): target forward + training pass + reduce/Adam, pipelined"},
-                    "hbm_peak_gbs": hbm_peak, "hbm_peak_source": "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"}
+                    "hbm_peak_gbs": hbm_peak, "hbm_peak_source": "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "H100 SXM data sheet"}
     else:
         train_bytes = B * 3421 + 7 * 4 * model.n_params       # gathered episodes + parameter / Adam traffic (SURVEY section 8d)
         achieved = train_flop / train_avg_s / 1e12 if train_n else None
         roofline = {"bound": "fp32-fma", "kernel": "train_kernel<16, kHeadDqn>", "achieved": achieved, "peak": fp32_peak, "unit": "TFLOP/s",
                     "frac": (achieved / fp32_peak) if achieved else None,
-                    "traffic": 5524224,  # dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full (profiles/r1_train_kernel_final.md)
+                    "traffic": None,
                     "peak_source": f"{n_sm} SMs x 128 FP32 lanes x 2 x {sm_mhz:.0f} MHz median SM clock sampled during the run (MEASURED_PEAKS.json holds no FP32 figure)",
                     "launch_us": 1e6 * train_avg_s, "launches_timed": train_n, "flop_per_launch": train_flop,
                     "hbm": {"achieved_gbs": (train_bytes / train_avg_s / 1e9) if train_n else None, "peak_gbs": hbm_peak,
-                            "peak_source": "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)",
+                            "peak_source": "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "H100 SXM data sheet",
                             "frac": (train_bytes / train_avg_s / 1e9 / hbm_peak) if train_n else None, "bytes_per_launch": train_bytes,
                             "note": "the fused learner is compute-bound (~1 750 FLOP/B, SURVEY F7): the HBM fraction is small by construction"},
                     "bf16_tensor_peak_tflops": peaks.get("bf16_tflops_sustained")}
@@ -494,7 +524,7 @@ def run_dqn_family(args, wl):
     line = {"metric": "env-steps/sec", "value": value, "unit": "env-steps/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": workload_config(args, world), "clocks": clocks, "e2e": e2e, "gpu_launches": launches_per_step * args.steps,
-            "roofline": roofline, "updates_per_sec": U * args.steps * world / (ms / 1e3), "env_steps_timed": n_steps}
+            "roofline": roofline, "updates_per_sec": U * args.steps * world / (ms / 1e3), "env_steps_timed": n_steps, "gpu": gpu_info(torch, dev)}
     if multi is not None:
         line["multi_gpu"] = multi
         line["ranks_bit_identical"] = multi["ranks_bit_identical"]
@@ -520,6 +550,7 @@ def run_ia2c(args, wl):
     cfg = types.SimpleNamespace(optimizer="Adam", lr=3e-4, gamma=0.99, grad_clip=False, n_steps=5, entropy_coef=0.001, value_loss_coef=0.5,
                                 target_update_interval_or_tau=200, standardise_returns=False)
     net = types.SimpleNamespace(layers=[128, 128], parameter_sharing=True, use_rnn=False, use_orthogonal_init=True, centralised=False)
+    torch.manual_seed(args.seed)   # the initial parameters: same arguments, same inputs
     model = A2CNetwork(env.single_observation_space, env.single_action_space, cfg, net, net, "cuda", max_envs=P, max_episode_length=T)
     if world > 1:
         dist.broadcast(model.theta, 0)
@@ -544,7 +575,7 @@ def run_ia2c(args, wl):
 
     def iteration(host_boundary: bool):
         if not host_boundary:
-            final_len, _ = coll.collect()
+            final_len, final_ret = coll.collect()
         else:
             b.obs.zero_(); b.act.zero_(); b.rew.zero_(); b.filled.zero_(); b.done.zero_()
             nat_env.reset(traj=b, slot0=0)
@@ -557,8 +588,9 @@ def run_ia2c(args, wl):
                 h_obs.copy_(nat_env.obs, non_blocking=True); h_rew.copy_(nat_env.rew, non_blocking=True)
                 h_done.copy_(nat_env.done, non_blocking=True); h_trunc.copy_(nat_env.trunc, non_blocking=True)
                 torch.cuda.current_stream().synchronize()
-            final_len = nat_env.final_len
+            final_len, final_ret = nat_env.final_len, nat_env.final_ret
         H.steps_dev.add_(final_len.sum())
+        state.update(final_len=final_len, final_ret=final_ret)
         update()
         state["step"] += T * P
         if host_boundary:
@@ -569,6 +601,11 @@ def run_ia2c(args, wl):
     sampler = ClockSampler(H.local) if rank == 0 else None
     ms, n_steps = H.timed(args.steps, lambda: iteration(False))
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        ep = episode_sample(torch, P).to(dev)
+        dump_outputs(args.dump_outputs, {"theta": model.theta, "metrics": model._metrics, "logits_last_env_step": coll.logits,
+                                         "episode_length": state["final_len"], "episode_return": state["final_ret"], "episode_index": ep,
+                                         "batch_obs": b.obs[ep], "batch_act": b.act[ep], "batch_rew": b.rew[ep], "batch_done": b.done[ep], "batch_filled": b.filled[ep]})
     multi = None
     if world > 1:
         fp = theta_fingerprint(torch, model.theta)
@@ -595,7 +632,7 @@ def run_ia2c(args, wl):
     rows_t1, rows_t = n_agents * (T + 1) * P, n_agents * T * P
     f_actor, f_critic = fwd_flop_per_row(obs_dim, n_act), fwd_flop_per_row(obs_dim, 1)
     flop = rows_t1 * f_critic + 3 * rows_t * (f_actor + f_critic)     # target critic forward + forward/backward of critic and actor
-    sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
+    sm_mhz = (clocks or {}).get("sm_mhz") or H100_MAX_SM_MHZ
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
     fp32_peak = n_sm * 128 * 2 * sm_mhz * 1e6 / 1e12
     peaks = load_peaks()
@@ -607,7 +644,7 @@ def run_ia2c(args, wl):
     line = {"metric": "env-steps/sec", "value": n_steps / (ms / 1e3), "unit": "env-steps/s", "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": workload_config(args, world), "clocks": clocks, "e2e": e2e, "gpu_launches": (1 + 5 + 2 * T + 8) * args.steps,
-            "roofline": roofline, "updates_per_sec": args.steps * world / (ms / 1e3), "env_steps_timed": n_steps}
+            "roofline": roofline, "updates_per_sec": args.steps * world / (ms / 1e3), "env_steps_timed": n_steps, "gpu": gpu_info(torch, dev)}
     if multi is not None:
         line["multi_gpu"] = multi
         line["ranks_bit_identical"] = multi["ranks_bit_identical"]

@@ -1,4 +1,4 @@
-"""Independent actor-critic learner on the B200 path -- drop-in for marlbase/ac/model.py A2CNetwork (22-246).
+"""Independent actor-critic learner on the GPU path -- drop-in for marlbase/ac/model.py A2CNetwork (22-246).
 
 Same constructor signature / Hydra `_target_` role (configs/algorithm/ia2c.yaml:8-26) and the reference's
 `state_dict()` key names (`actor.independent.{i}.network.…`, `critic.…`, `target_critic.…`; shared: `.networks.{k}.`).
@@ -20,14 +20,14 @@ class A2CNetwork:
     def __init__(self, obs_space, action_space, cfg, actor, critic, device, max_envs=None, max_episode_length=None):
         for part, name in ((actor, "actor"), (critic, "critic")):
             if part.use_rnn:
-                raise NotImplementedError(f"{name}.use_rnn=True (GRU) is out of scope of the B200 hot path")
+                raise NotImplementedError(f"{name}.use_rnn=True (GRU) is out of scope of the GPU hot path")
             if list(part.layers) != [HIDDEN, HIDDEN]:
                 raise NotImplementedError(f"{name}.layers={list(part.layers)}: the fused kernels implement the shipped [128, 128] MLP only")
         opt = getattr(cfg, "optimizer", "Adam")
         if (opt if isinstance(opt, str) else opt.__name__) != "Adam":
             raise NotImplementedError("only optimizer=Adam is implemented")
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
-            raise nat.NativeError("the B200 learners need algorithm.model.device=cuda (no CPU fallback)")
+            raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
         self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
         self.n_agents = len(obs_space)
         obs_dims, act_dims = [_dim(o) for o in obs_space], [_dim(a) for a in action_space]

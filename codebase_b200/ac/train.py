@@ -1,4 +1,4 @@
-"""IA2C training driver on the B200 path -- drop-in for marlbase/ac/train.py `main(envs, eval_env, logger, time_limit,
+"""IA2C training driver on the GPU path -- drop-in for marlbase/ac/train.py `main(envs, eval_env, logger, time_limit,
 **cfg)` (`algorithm._target_: ac.train.main`, configs/algorithm/ia2c.yaml:6).
 
 Loop structure of the reference (ac/train.py:170-204) with every stage on the device:
@@ -71,7 +71,7 @@ def main(envs, eval_env, logger, time_limit, **cfg):
             torch.save(model.state_dict(), f"checkpoints/model_s{step}.pt")
             last_save = step
         if cfg.video_interval:
-            raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the B200 hot path")
+            raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the GPU hot path")
         updates += 1
         step += t * P
     envs.close()

@@ -1,4 +1,4 @@
-"""A small Hydra-compatible config composer (hydra / omegaconf are not dependencies of the B200 path).
+"""A small Hydra-compatible config composer (hydra / omegaconf are not dependencies of the GPU path).
 
 Implements the subset of Hydra the reference's command lines use (README.md:80-120, marlbase/run.py:14-47):
   python -m codebase_b200.run +algorithm=idqn env.name="lbforaging:Foraging-8x8-2p-3f-v3" env.time_limit=25 seed=0

@@ -1,4 +1,4 @@
-"""Builds codebase_b200/csrc/libmarlb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds codebase_b200/csrc/libmarlb200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import glob
@@ -8,8 +8,9 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "libmarlb200.so")
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + [
+    "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr",
 ]
 
@@ -45,7 +46,7 @@ def build(force: bool = False, verbose: bool = False, out: str | None = None, de
             return obj
         with cf.ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
             objs = list(ex.map(cc, srcs))
-        subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", target] + objs, cwd=HERE)
+        subprocess.check_call([nvcc] + GENCODE + ["-shared", "-o", target] + objs, cwd=HERE)
     else:
         subprocess.check_call([nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", target] + srcs, cwd=HERE)
     return target

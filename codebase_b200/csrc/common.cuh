@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers of libmarlb200 (sm_100a only).
+// common.cuh -- shared helpers of libmarlb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -73,7 +73,7 @@ __host__ __device__ __forceinline__ float u01(uint32_t u) { return (float)(u >> 
 
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------------------------------------
 // The per-update kernels form one dependency chain on one stream; each is launched with programmatic stream serialization so that
-// its CTAs are scheduled (and run their data-independent setup: TMEM allocation, barrier init) while the previous kernel drains.
+// its CTAs are scheduled (and run their data-independent setup: barrier init) while the previous kernel drains.
 // Contract of every kernel launched through launch_pdl: no global memory access before pdl_wait(); pdl_launch_dependents() right
 // after it (when kernel K starts, K-1 has passed its wait, hence K-2 and everything before it has completed).
 #ifdef __CUDACC__
@@ -94,8 +94,6 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 int check_device(int device);
 int tc_forward_enabled();
 int tc_backward_enabled();
-int tc_pingpong_enabled(int which);   // 0: forward kernels, 1: dH1 kernel
-int tc_onchip_enabled();
 int tc_split_exchange_enabled();
 
 }  // namespace marl

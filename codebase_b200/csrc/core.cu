@@ -14,7 +14,7 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-// No CPU fallback: a missing / non-Blackwell device is an error, never a silent slow path.
+// No CPU fallback: a missing / non-Hopper device is an error, never a silent slow path (sm_90a code loads on compute capability 9.0 only).
 int check_device(int device) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
@@ -25,8 +25,8 @@ int check_device(int device) {
   if (device < 0 || device >= n) { set_error("libmarlb200: device %d out of range (0..%d)", device, n - 1); return MARL_EINVAL; }
   cudaDeviceProp p;
   MARL_CUDA_TRY(cudaGetDeviceProperties(&p, device));
-  if (p.major != 10) {
-    set_error("libmarlb200: device %d is sm_%d%d; this build targets sm_100a (B200) only", device, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    set_error("libmarlb200: device %d is sm_%d%d; this build targets sm_90a (H100) only", device, p.major, p.minor);
     return MARL_ECUDA;
   }
   MARL_CUDA_TRY(cudaSetDevice(device));
@@ -34,56 +34,41 @@ int check_device(int device) {
 }
 
 static int env_int(const char* name, int dflt) { const char* v = getenv(name); return v && *v ? atoi(v) : dflt; }
-// bit 0: forward kernels (tc_forward2_kernel, tc_dqn_fwd2_kernel), bit 1: dH1 kernel (tc_dh12_kernel).  Default 2: with ~3 tiles per CTA the
-// two-accumulator forward kernels do not amortise their pipeline fill (measured slower than the one-tile kernels), the dH1 kernel does.
-static int g_tc_forward = 1, g_tc_backward = 1, g_tc_pingpong = env_int("MARL_TC_PINGPONG", 2);   // the environment variable only moves the default
-int tc_pingpong_enabled(int which) { return (g_tc_pingpong >> which) & 1; }
+static int g_tc_forward = 1, g_tc_backward = 1;
 static int g_split_exchange = env_int("MARL_SPLIT_EXCHANGE", 0);
 int tc_split_exchange_enabled() { return g_split_exchange; }
-static int g_tc_onchip = env_int("MARL_TC_ONCHIP", 1);
-int tc_onchip_enabled() { return g_tc_onchip; }
-static unsigned long long* g_dbg_progress = nullptr;
-unsigned long long* tc_debug_progress_ptr() { return g_dbg_progress; }
 int tc_forward_enabled() { return g_tc_forward; }
 int tc_backward_enabled() { return g_tc_backward; }
 
 }  // namespace marl
 
 extern "C" {
-/* Process-wide options.  "tensor_core_forward": 1 = forward-only passes (act, target networks) run on tcgen05 with the
- * 3xTF32 split (default), 0 = FP32 FFMA kernels. */
+/* Process-wide options.  "tensor_core_forward": 1 = forward-only passes (act, target networks) run on the tensor cores (wgmma) with the
+ * 3xTF32 split (default), 0 = FP32 FFMA kernels.  "tensor_core_backward": 1 = the DQN-family training pass runs as the three-kernel
+ * tensor-core pipeline (tc_train.cu, default), 0 = fused FP32 kernel. */
 int marl_set_option(const char* name, int32_t value) {
   if (name && strcmp(name, "tensor_core_forward") == 0) { marl::g_tc_forward = value ? 1 : 0; return MARL_OK; }
   if (name && strcmp(name, "tensor_core_backward") == 0) { marl::g_tc_backward = value ? 1 : 0; return MARL_OK; }
-  /* bit mask of the tensor-core kernels that use two accumulator buffers in TMEM (the epilogue of one 128-row tile runs under the MMAs of the
-   * next): bit 0 = forward kernels, bit 1 = dH1 kernel; default 2.  0: one tile at a time everywhere */
-  if (name && strcmp(name, "tensor_core_pingpong") == 0) { marl::g_tc_pingpong = value & 3; return MARL_OK; }
-  /* 1 (default): the training pass keeps H1 / H2 / dH1 on chip (tc_train3.cu: 192 bytes per row cross kernels); 0: the previous pipeline, which
-   * streams them through global memory (tc_train.cu) */
   /* several ranks: 0 (default) = the gradient exchange inside one fused reduce + Adam kernel; 1 = split into a push kernel and a finishing kernel with the
-   * next update's target forward between them (hides the NVLink round trip but costs a launch: measured 120.9 vs 116.8 us per update on 2 GPUs) */
+   * next update's target forward between them (hides the peer round trip but costs a launch) */
   if (name && strcmp(name, "split_exchange") == 0) { marl::g_split_exchange = value ? 1 : 0; return MARL_OK; }
-  if (name && strcmp(name, "tensor_core_onchip") == 0) { marl::g_tc_onchip = value ? 1 : 0; return MARL_OK; }
   marl::set_error("marl_set_option: unknown option '%s'", name ? name : "(null)");
   return MARL_EINVAL;
 }
 /* Profiling builds only (MARL_NVCC_DEFINES=-DMARL_TC_TIMESTAMPS, tools/ts_timeline.py): the timeline probes of kernel `which` (0 forward, 1 training
- * forward, 2 dH1, 3 weight gradients, 4 reduce + Adam, 5 dH1 with two accumulators) as [160 CTAs][32 slots][globaltimer ns, clock64] -> host memory;
+ * forward, 2 TD head + dH1, 3 weight gradients, 4 reduce + Adam) as [160 CTAs][32 slots][globaltimer ns, clock64] -> host memory;
  * product builds return MARL_EINVAL. */
 int marl_debug_timestamps(int32_t which, uint64_t* out) {
   int rc = -1;
   unsigned long long* o = reinterpret_cast<unsigned long long*>(out);
   switch (which) {
     case 0: rc = marl::tsg_forward(o); break; case 1: rc = marl::tsg_fwd(o); break; case 2: rc = marl::tsg_dh1(o); break;
-    case 3: rc = marl::tsg_dw(o); break; case 4: rc = marl::tsg_adam(o); break; case 5: rc = marl::tsg_dh12(o); break;
-    case 6: rc = marl::tsg_fwd3(o); break; case 7: rc = marl::tsg_dh1w1(o); break; case 8: rc = marl::tsg_dw2(o); break;
+    case 3: rc = marl::tsg_dw(o); break; case 4: rc = marl::tsg_adam(o); break;
     default: break;
   }
   if (rc != 0) { marl::set_error("marl_debug_timestamps: kernel %d has no probes in this build (build with -DMARL_TC_TIMESTAMPS)", (int)which); return MARL_EINVAL; }
   return MARL_OK;
 }
-/* Profiling builds: host-mapped buffer (cudaHostAlloc'd by the caller, uint64 [3][160][32]) that the on-chip training kernels mark their progress in. */
-int marl_debug_progress(uint64_t* mapped) { marl::g_dbg_progress = reinterpret_cast<unsigned long long*>(mapped); return MARL_OK; }
 int marl_version(void) { return MARL_ABI_VERSION; }
 const char* marl_last_error(void) { return marl::g_err; }
 }

@@ -177,7 +177,7 @@ int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_
   *out = nullptr;
   MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "marl_dqn_create: n_agents out of range");
   MARL_REQUIRE(cfg->n_nets >= 1 && cfg->n_nets <= cfg->n_agents, "marl_dqn_create: n_nets out of range");
-  MARL_REQUIRE(cfg->hidden == kHidden, "marl_dqn_create: only layers=[128,128] is implemented on the B200 path (got hidden=%d)", cfg->hidden);
+  MARL_REQUIRE(cfg->hidden == kHidden, "marl_dqn_create: only layers=[128,128] is implemented on the GPU path (got hidden=%d)", cfg->hidden);
   MARL_REQUIRE(cfg->out_dim >= 1 && cfg->out_dim <= kOutPad, "marl_dqn_create: n_actions %d not supported (1..%d)", cfg->out_dim, kOutPad);
   MARL_REQUIRE(max_batch >= 1 && max_T >= 1, "marl_dqn_create: max_batch/max_T must be >= 1");
   MARL_REQUIRE(hp->mixer >= 0 && hp->mixer <= 2, "marl_dqn_create: mixer must be 0 (independent), 1 (VDN) or 2 (QMIX)");
@@ -481,7 +481,7 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
       const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
       int rc = 0;
       rc |= dqn_alloc(&h->tc_h1, rows * kHidden); rc |= dqn_alloc(&h->tc_h2, rows * kHidden);
-      rc |= dqn_alloc(&h->tc_dh1, rows * kHidden); rc |= dqn_alloc(&h->tc_rec, rows * 16 /* kRowRec */); rc |= dqn_alloc(&h->tc_x, rows * kMaxObsDim);
+      rc |= dqn_alloc(&h->tc_dh1, rows * kHidden); rc |= dqn_alloc(&h->tc_rec, rows * 32 /* kRowRec */); rc |= dqn_alloc(&h->tc_x, rows * kMaxObsDim);
       rc |= dqn_alloc(reinterpret_cast<float**>(&h->image_bwd), (size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4);
       if (rc) return MARL_ENOMEM;
     }

@@ -1,4 +1,4 @@
-// lbf_env.cu -- Level-Based Foraging transition for thousands of env instances per launch (sm_100a).
+// lbf_env.cu -- Level-Based Foraging transition for thousands of env instances per launch (sm_90a).
 //
 // Replaces the gym.make()'d third-party `lbforaging` ForagingEnv.reset/step plus marlbase's wrapper stack
 // (TimeLimit -> RecordEpisodeStatistics -> [CooperativeReward]); reference call sites
@@ -244,8 +244,7 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int G = c.G, EPW = 32 / G, EPC = (kThreads / 32) * EPW;
   // Shared-memory pitch of an env's grid = pitch + 4 bytes, i.e. an ODD number of words: the lanes of a warp work on different envs at the same cell
-  // offset, and with the global pitch (64 B at 8x8: 16 words) every second env fell on the same bank -- 60 % of this kernel's shared wavefronts were
-  // conflicts (profiles/r2_lbf_step.md).
+  // offset, and with the global pitch (64 B at 8x8: 16 words) every second env fell on the same bank.
   const int sp = c.pitch + 4, spw = sp >> 2, p16 = c.pitch >> 4;
   int8_t* field_s = reinterpret_cast<int8_t*>(smem_raw);                                   // [EPC][sp]
   uint32_t* pl_s = reinterpret_cast<uint32_t*>(field_s + (size_t)EPC * sp);                 // [EPC][G]

@@ -286,7 +286,7 @@ inline int check_mlp_cfg(const marl_mlp_cfg* cfg, const char* who) {
   MARL_REQUIRE(cfg != nullptr, "%s: NULL network config", who);
   MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "%s: n_agents out of range", who);
   MARL_REQUIRE(cfg->n_nets >= 1 && cfg->n_nets <= cfg->n_agents, "%s: n_nets out of range", who);
-  MARL_REQUIRE(cfg->hidden == kHidden, "%s: only layers=[128,128] is implemented on the B200 path (got hidden=%d)", who, cfg->hidden);
+  MARL_REQUIRE(cfg->hidden == kHidden, "%s: only layers=[128,128] is implemented on the GPU path (got hidden=%d)", who, cfg->hidden);
   MARL_REQUIRE(cfg->in_dim >= 1 && cfg->in_dim <= kMaxObsDim, "%s: obs dim %d not supported (1..%d)", who, cfg->in_dim, kMaxObsDim);
   MARL_REQUIRE(cfg->out_dim >= 1 && cfg->out_dim <= kOutPad, "%s: output width %d not supported (1..%d)", who, cfg->out_dim, kOutPad);
   for (int a = 0; a < cfg->n_agents; ++a) MARL_REQUIRE(cfg->agent_net[a] >= 0 && cfg->agent_net[a] < cfg->n_nets, "%s: agent_net[%d] out of range", who, a);

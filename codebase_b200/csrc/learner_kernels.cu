@@ -1,4 +1,4 @@
-// learner_kernels.cu -- the fused learner kernels (sm_100a).
+// learner_kernels.cu -- the fused learner kernels (sm_90a).
 //
 //  mlp_forward_kernel   per-agent MLP inference on gathered rows: model.act's critic/actor forward
 //                       (marlbase/dqn/model.py:99, marlbase/ac/model.py:148-149) and the target-network pass of the
@@ -10,7 +10,7 @@
 //  grad_reduce_kernel   deterministic sum of the per-CTA gradient partials (+ loss / filled sums).
 //  adam_kernel          clip_grad_norm_ + Adam.step + update_target (marlbase/dqn/model.py:169-196).
 //
-// Persistent CTAs, one per SM (148 on B200) split across networks; FP32 FFMA register-tiled GEMMs (see mlp.cuh).
+// Persistent CTAs, one per SM (132 on H100) split across networks; FP32 FFMA register-tiled GEMMs (see mlp.cuh).
 #include "tc_common.cuh"
 
 namespace marl {

@@ -1,44 +1,36 @@
-// tc_common.cuh -- tcgen05 / TMEM / mbarrier primitives and the packed weight-image layout shared by the tensor-core kernels.
-// PTX forms and descriptor bit fields follow cute/arch/{mma_sm100_umma,mma_sm100_desc,copy_sm100,tmem_allocator_sm100}.hpp and
-// cutlass/arch/barrier.h (vendored CUTLASS headers, read for reference only); bring-up: tools/tc_probe.cu, tools/tc_probe2.cu.
+// tc_common.cuh -- Hopper (sm_90a) tensor-core primitives shared by the 3xTF32 kernels: warpgroup MMA (wgmma) wrappers, shared-memory
+// matrix descriptors, mbarrier + TMA bulk copies, and the packed weight-image layout.
 #pragma once
 #include "learner.cuh"
 
 namespace marl {
 
-
-constexpr int kTrThreads = 512;   // 16 warps: lane quarter x column quarter
+constexpr int kTcThreads = 256;                    // two warpgroups; warpgroup w owns rows [64 w, 64 w + 64) of every 128-row tile
+constexpr int kWgRows = 64;                        // rows of one wgmma (M)
 constexpr int kPanelBytes = kHidden * 128;         // 128 rows x 32 floats
-constexpr int kHeadRows = 16;                      // head GEMM uses N = 16 (minimum for M = 128)
-constexpr int kHeadPanelBytes = kHeadRows * 128;
-// image layout (bytes): W1 hi | W1 lo | W2 hi (4 panels) | W2 lo | W3 hi (4 panels of 16 rows) | W3 lo | b1 | b2 | b3
+// image layout (bytes): W1 hi | W1 lo | W2 hi (4 panels) | W2 lo | b1 | b2 | b3 | FP32 W3 [8][128]
 constexpr int kOffW1Hi = 0, kOffW1Lo = kOffW1Hi + kPanelBytes, kOffW2Hi = kOffW1Lo + kPanelBytes, kOffW2Lo = kOffW2Hi + 4 * kPanelBytes;
-constexpr int kOffW3Hi = kOffW2Lo + 4 * kPanelBytes, kOffW3Lo = kOffW3Hi + 4 * kHeadPanelBytes;
-constexpr int kOffB1 = kOffW3Lo + 4 * kHeadPanelBytes, kOffB2 = kOffB1 + kHidden * 4, kOffB3 = kOffB2 + kHidden * 4;
-constexpr int kOffW3F = kOffB3 + kHeadRows * 4;           // plain FP32 copy of W3 [8][128] (head gradient dH2 = dq x W3)
+constexpr int kOffB1 = kOffW2Lo + 4 * kPanelBytes, kOffB2 = kOffB1 + kHidden * 4, kOffB3 = kOffB2 + kHidden * 4;
+constexpr int kOffW3F = kOffB3 + kOutPad * 4;      // plain FP32 copy of W3 [8][128]: the head runs on the CUDA cores
 constexpr int kImageBytes = kOffW3F + kOutPad * kHidden * 4;
 // backward image: W2^T as a K-major operand (rows = input features j1, K = output features j2), hi | lo
 constexpr int kBwdImageBytes = 8 * kPanelBytes;
-constexpr int kTcSmemBytes = kImageBytes + 64 + 1024;
-// TMEM columns of the row-per-lane kernels: A hi [0,128), A lo [128,256), D [256,384), head D [384,400)
-constexpr uint32_t kColAHi = 0, kColALo = 128, kColD = 256, kColDHead = 384;  // + mbarrier / TMEM slot, + slack for 1024-byte alignment
+static_assert(kOffB1 % 16 == 0 && kOffW3F % 16 == 0 && kImageBytes % 16 == 0, "TMA bulk copies move multiples of 16 bytes");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-// round to TF32 (10-bit mantissa), nearest with ties away from zero: what cvt.rna.tf32.f32 computes for finite inputs, in two
-// integer instructions instead of the five the compiler emits for the cvt (its extra work is NaN / infinity handling)
+// round to TF32 (10-bit mantissa), nearest with ties away from zero: what cvt.rna.tf32.f32 computes for finite inputs
 __device__ __forceinline__ float tf32_rn(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
-// 3xTF32 operand split: x = hi + lo with both parts representable in TF32 (lo rounded too: leaving it to the tensor core's
-// truncation was measured to make no speed difference)
-#ifdef MARL_TF32_SPLIT_RN
-__device__ __forceinline__ void tf32_split(float x, float& hi, float& lo) { hi = tf32_rn(x); lo = tf32_rn(x - hi); }
-#else
-// two instructions instead of five: hi = x with the 13 low mantissa bits cleared (exactly representable in TF32), lo = x - hi (exact in FP32, same sign
-// as x, < 2^-10 |x|); the tensor core drops the low 13 bits of lo, i.e. at most 2^-20 |x| -- the same order as the lo*lo term that 3xTF32 omits anyway.
-// Measured against the oracle: tests/test_tc_backward_gpu.py (gradient error stays ~1e-6 of the gradient scale, bar 1e-5).
+// 3xTF32 operand split of values produced on the fly: hi = x with the 13 low mantissa bits cleared (exactly representable in TF32), lo = x - hi
+// (exact in FP32, < 2^-10 |x|); the tensor core drops the low 13 bits of lo, i.e. at most 2^-20 |x| -- the order of the lo*lo term 3xTF32 omits.
 __device__ __forceinline__ void tf32_split(float x, float& hi, float& lo) { hi = __uint_as_float(__float_as_uint(x) & 0xffffe000u); lo = x - hi; }
-#endif
+__device__ __forceinline__ void tf32_split_u(float x, uint32_t& hi, uint32_t& lo) { float h, l; tf32_split(x, h, l); hi = __float_as_uint(h); lo = __float_as_uint(l); }
+
 // ---- weight image --------------------------------------------------------------------------------------------------
-// element (row n, feature k) of a [rows][K] K-major SWIZZLE_128B operand -> byte offset inside its panel set
+// The A operand of the forward and dH1 products comes from registers, in the wgmma accumulator layout of the previous layer: a thread holds
+// features 2t and 2t + 1 of every group of 8 where the A fragment wants features t and t + 4.  The K order of every image is permuted to match:
+// within each group of 8 features, the even ones first, then the odd ones.
+__host__ __device__ __forceinline__ int kperm(int k) { return (k & ~7) | ((k & 1) << 2) | ((k & 7) >> 1); }
+// element (row n, K position k) of a [rows][K] K-major SWIZZLE_128B operand -> byte offset inside its panel set (one panel per 32 K positions)
 __device__ __forceinline__ int panel_offset(int n, int k, int panel_bytes) {
   const int p = k >> 5, c = (k >> 2) & 7, w = k & 3;
   return p * panel_bytes + n * 128 + ((c ^ (n & 7)) << 4) + (w << 2);
@@ -48,22 +40,20 @@ __device__ __forceinline__ int panel_offset(int n, int k, int panel_bytes) {
 __device__ __forceinline__ void pack_param(const NetLayout& lay, int j, float x, uint8_t* img, uint8_t* bwd) {
   const float hi = tf32_rn(x), lo = tf32_rn(x - hi);
   if (j < lay.b1) {
-    const int n = (j - lay.w1) / lay.in, k = (j - lay.w1) - n * lay.in, o = panel_offset(n, k, kPanelBytes);
+    const int n = (j - lay.w1) / lay.in, k = (j - lay.w1) - n * lay.in, o = panel_offset(n, kperm(k), kPanelBytes);
     *reinterpret_cast<float*>(img + kOffW1Hi + o) = hi; *reinterpret_cast<float*>(img + kOffW1Lo + o) = lo;
   } else if (j < lay.w2) {
     reinterpret_cast<float*>(img + kOffB1)[j - lay.b1] = x;
   } else if (j < lay.b2) {
-    const int n = (j - lay.w2) >> 7, k = (j - lay.w2) & 127, o = panel_offset(n, k, kPanelBytes);
+    const int n = (j - lay.w2) >> 7, k = (j - lay.w2) & 127, o = panel_offset(n, kperm(k), kPanelBytes);
     *reinterpret_cast<float*>(img + kOffW2Hi + o) = hi; *reinterpret_cast<float*>(img + kOffW2Lo + o) = lo;
     if (bwd != nullptr) {  // W2^T as a K-major operand: row = input feature, K = output feature
-      const int ob = panel_offset(k, n, kPanelBytes);
+      const int ob = panel_offset(k, kperm(n), kPanelBytes);
       *reinterpret_cast<float*>(bwd + ob) = hi; *reinterpret_cast<float*>(bwd + 4 * kPanelBytes + ob) = lo;
     }
   } else if (j < lay.w3) {
     reinterpret_cast<float*>(img + kOffB2)[j - lay.b2] = x;
   } else if (j < lay.b3) {
-    const int n = (j - lay.w3) >> 7, k = (j - lay.w3) & 127, o = panel_offset(n, k, kHeadPanelBytes);
-    *reinterpret_cast<float*>(img + kOffW3Hi + o) = hi; *reinterpret_cast<float*>(img + kOffW3Lo + o) = lo;
     reinterpret_cast<float*>(img + kOffW3F)[j - lay.w3] = x;
   } else if (j < lay.P) {
     reinterpret_cast<float*>(img + kOffB3)[j - lay.b3] = x;
@@ -71,47 +61,27 @@ __device__ __forceinline__ void pack_param(const NetLayout& lay, int j, float x,
 }
 
 // ---- optional phase timestamps (profiling builds: MARL_NVCC_DEFINES=-DMARL_TC_TIMESTAMPS) ------------------------------------------
-// One thread of CTA 5 records clock64() at phase boundaries into shared memory and prints the offsets when the kernel ends.
-#ifdef MARL_TC_TIMESTAMPS
-constexpr int kTsBytes = 1024;
-#define TS_DECL(ptr, thread, slot) long long* ts_ = reinterpret_cast<long long*>(ptr) + 48 * (slot); const bool ts_on_ = (int)threadIdx.x == (thread) && blockIdx.x == 5; \
-  int tsi_ = 1; if (ts_on_) { for (int i_ = 1; i_ < 48; ++i_) ts_[i_] = 0; ts_[0] = clock64(); }
-#define TS() do { if (ts_on_ && tsi_ < 48) ts_[tsi_++] = clock64(); } while (0)
-#define TS_DUMP(name) do { if (ts_on_) { printf("TS %s:", name); for (int i_ = 1; i_ < tsi_; ++i_) printf(" %lld", ts_[i_] - ts_[0]); printf("\n"); } } while (0)
-#else
-constexpr int kTsBytes = 0;
-#define TS_DECL(ptr, thread, slot)
-#define TS()
-#define TS_DUMP(name)
-#endif
-
-// Global timeline probes of the same builds: thread 0 of every CTA stores %globaltimer (ns) and clock64() per probe slot into a per-kernel
-// device buffer; tools/ts_timeline.py reads them back through marl_debug_timestamps (launch gaps, prologues, per-tile phases, tail skew).
+// Thread 0 of every CTA stores %globaltimer (ns) and clock64() per probe slot into a per-kernel device buffer; tools/ts_timeline.py reads
+// them back through marl_debug_timestamps (launch gaps, prologues, per-tile phases, tail skew).
 #ifdef MARL_TC_TIMESTAMPS
 constexpr int kTsgCtas = 160, kTsgSlots = 32;
 #define TSG_DEFINE(name) static __device__ unsigned long long name[kTsgCtas][kTsgSlots][2];
 #define TSG(name, slot) do { if (threadIdx.x == 0 && blockIdx.x < kTsgCtas && (slot) < kTsgSlots) { unsigned long long g_; \
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g_)); name[blockIdx.x][(slot)][0] = g_; name[blockIdx.x][(slot)][1] = (unsigned long long)clock64(); } } while (0)
 #define TSG_GETTER(fn, name) int fn(unsigned long long* out) { return cudaMemcpyFromSymbol(out, name, sizeof(name)) == cudaSuccess ? 0 : -1; }
-// the same probe plus a progress mark per WARP in host-mapped memory (dbg: [3 kernels][160 CTAs][32 warps], slot + 1 of the last probe the warp
-// passed): readable from the host while a kernel hangs (tools/debug_hang.py)
-#define TSGP(name, dbg, kid, slot) do { TSG(name, slot); if ((dbg) != nullptr && (threadIdx.x & 31) == 0 && blockIdx.x < kTsgCtas) { \
-  *reinterpret_cast<volatile unsigned long long*>((dbg) + ((kid) * kTsgCtas + blockIdx.x) * 32 + (threadIdx.x >> 5)) = (unsigned long long)((slot) + 1); } } while (0)
 #else
-#define TSGP(name, dbg, kid, slot)
 #define TSG_DEFINE(name)
 #define TSG(name, slot)
 #define TSG_GETTER(fn, name) int fn(unsigned long long*) { return -1; }
 #endif
 int tsg_forward(unsigned long long* out); int tsg_fwd(unsigned long long* out); int tsg_dh1(unsigned long long* out); int tsg_dw(unsigned long long* out);
-int tsg_dh12(unsigned long long* out); int tsg_adam(unsigned long long* out);
-int tsg_fwd3(unsigned long long* out); int tsg_dh1w1(unsigned long long* out); int tsg_dw2(unsigned long long* out);
+int tsg_adam(unsigned long long* out);
 
 // dynamic shared memory rounded up to 1024 bytes (swizzle atoms), keeping the pointer in the shared address space so that the
 // compiler emits LDS / STS rather than generic loads and stores
 __device__ __forceinline__ uint8_t* align_smem_1024(uint8_t* raw) { return raw + ((1024u - ((uint32_t)__cvta_generic_to_shared(raw) & 1023u)) & 1023u); }
 
-// ---- tcgen05 helpers -------------------------------------------------------------------------------------------------
+// ---- mbarrier + TMA bulk copy ----------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
@@ -126,46 +96,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "DONE:\n"
       "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start >> 4, LBO 1, SBO 1024 B,
-// version 1, layout type 2
-__device__ __forceinline__ uint64_t kmajor_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, both K-major, M = 128
-__device__ __forceinline__ uint32_t idesc_tf32(int n) { return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24); }
-
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-      "}" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// MN-major tf32 operand: SWIZZLE_128B_BASE32B (layout type 1), 4-row swizzle period (SBO 512 B), LBO = byte stride between
-// 32-feature panels.  Element (k, mn) lives at panel mn/32, row k (128 B), 32-byte unit ((mn % 32) / 8) ^ (k & 3), word mn % 8.
-__device__ __forceinline__ uint64_t mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
-}
-__device__ __forceinline__ int mn_offset(int k, int mn, int panel_bytes) {
-  return (mn >> 5) * panel_bytes + k * 128 + ((((mn >> 3) & 3) ^ (k & 3)) << 5) + ((mn & 7) << 2);
-}
-__device__ __forceinline__ uint32_t idesc_tf32_major(int n, int a_mn, int b_mn) { return idesc_tf32(n) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16); }
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// ---- TMA bulk copy (cp.async.bulk, SASS UBLKCP): one thread moves a contiguous, 16-byte aligned block global -> shared; completion is
-// counted in bytes on an mbarrier (expect_tx by the issuing thread).  The packed weight images are byte-for-byte shared-memory images, so
-// an image (or a slice of it) is one instruction instead of a loop of per-thread cp.async, and the writes arrive through the async proxy,
-// the one the tensor core reads operands through.
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// cp.async.bulk: one thread moves a contiguous, 16-byte aligned block global -> shared; completion is counted in bytes on an mbarrier
+// (expect_tx by the issuing thread).  The packed weight images are byte-for-byte shared-memory images, so an image is a few instructions
+// instead of a loop of per-thread copies, and the writes arrive through the async proxy, the one wgmma reads its operands through.
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -178,162 +112,148 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t dst_smem, const void* src,
 __device__ __forceinline__ void tma_image_range(uint32_t smem_base, const uint8_t* src, int begin, int end, uint64_t* bar) {
   for (int o = begin; o < end; o += 32768) tma_bulk_g2s(smem_base + (uint32_t)o, src + o, (uint32_t)min(32768, end - o), bar);
 }
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// the forward image in the order the first tile needs it: bars[0] <- W1 + biases + FP32 W3, bars[1] <- W2, bars[2] <- W3 (one thread)
+// the forward image in the order the first tile needs it (one thread): bars[0] <- W1 + biases + FP32 W3, bars[1] <- W2
 __device__ __forceinline__ void tma_forward_image(uint32_t smem_base, const uint8_t* src, uint64_t* bars) {
   mbar_expect_tx(bars + 0, (uint32_t)(kOffW2Hi + (kImageBytes - kOffB1)));
   tma_image_range(smem_base, src, kOffW1Hi, kOffW2Hi, bars + 0);
   tma_image_range(smem_base, src, kOffB1, kImageBytes, bars + 0);
-  mbar_expect_tx(bars + 1, (uint32_t)(kOffW3Hi - kOffW2Hi));
-  tma_image_range(smem_base, src, kOffW2Hi, kOffW3Hi, bars + 1);
-  mbar_expect_tx(bars + 2, (uint32_t)(kOffB1 - kOffW3Hi));
-  tma_image_range(smem_base, src, kOffW3Hi, kOffB1, bars + 2);
+  mbar_expect_tx(bars + 1, (uint32_t)(kOffB1 - kOffW2Hi));
+  tma_image_range(smem_base, src, kOffW2Hi, kOffB1, bars + 1);
 }
-// the same without the tensor-core operand copies of W3 (head on the CUDA cores): bars[0] <- W1 + biases + FP32 W3, bars[1] <- W2
-__device__ __forceinline__ void tma_forward_image_nohead(uint32_t smem_base, const uint8_t* src, uint64_t* bars) {
-  mbar_expect_tx(bars + 0, (uint32_t)(kOffW2Hi + (kImageBytes - kOffB1)));
-  tma_image_range(smem_base, src, kOffW1Hi, kOffW2Hi, bars + 0);
-  tma_image_range(smem_base, src, kOffB1, kImageBytes, bars + 0);
-  mbar_expect_tx(bars + 1, (uint32_t)(kOffW3Hi - kOffW2Hi));
-  tma_image_range(smem_base, src, kOffW2Hi, kOffW3Hi, bars + 1);
-}
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t addr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                 "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(addr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]),
-                 "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
+// ---- wgmma -----------------------------------------------------------------------------------------------------------
+// K-major SWIZZLE_128B shared-memory matrix descriptor: start >> 4, LBO 16 B (unused by swizzled K-major operands), SBO 1024 B (one 8-row
+// swizzle atom), layout type 1 (128-byte swizzle).  A k-step of 8 TF32 values inside an atom row is start + 32 bytes.
+__device__ __forceinline__ uint64_t sw128_desc(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// registers that an in-flight wgmma reads or writes: keep them where they are, and every use after this point, behind the wait that precedes it
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-// issue only; the caller waits with tmem_ld_wait() before touching r[]
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t addr, uint32_t (&r)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                 "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(addr));
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N][4]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(r[i][j])::"memory");
 }
-// the registers are in/out operands of the wait so that no use of them can be scheduled ahead of it
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]),
-                 "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
+// m64nNk8, D (F32) in registers; A from registers (RS, the tf32 fragment: rows lane/4 and +8 of the warp's 16, K t and t + 4) or from shared
+// memory (SS); B from shared memory; both operands K-major.  scale_d == 0: D = A*B, else D += A*B.
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st16(uint32_t addr, const float (&v)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(addr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])),
-               "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])),
-               "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])),
-               "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-               : "memory");
+__device__ __forceinline__ void wgmma_ss_n136(float (&d)[68], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %70, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n136k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67}, %68, %69, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st8(uint32_t addr, const float (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(addr), "r"(__float_as_uint(v[0])),
-               "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])),
-               "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
+__device__ __forceinline__ void wgmma_ss_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ss_n8(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0, %1, %2, %3}, %4, %5, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 
-// ---- the tensor-core training pass (tc_train.cu: one tile at a time; tc_train2.cu: two accumulators) -----------------------------------------------
-constexpr int kRowRec = 16;  // floats per row record: [0] g, [1] act, [2..3] spare, [4..7] mask1, [8..11] mask2
+// 3xTF32 layer of a warpgroup, A in registers: D = A_lo*B_hi + A_hi*B_lo + A_hi*B_hi over `ksteps` (<= KSTEPS) steps of 8 K positions; B = hi / lo
+// images of 32-position panels.  Waits for the MMAs before it returns.
+template <int KSTEPS>
+__device__ __forceinline__ void layer_rs(float (&d)[64], uint32_t (&ahi)[KSTEPS][4], uint32_t (&alo)[KSTEPS][4], uint32_t b_hi, uint32_t b_lo, int ksteps) {
+  wg_fence();
+#pragma unroll
+  for (int term = 0; term < 3; ++term)
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks)
+      if (ks < ksteps)
+        wgmma_rs_n128(d, term == 0 ? alo[ks] : ahi[ks], sw128_desc((term == 1 ? b_lo : b_hi) + (uint32_t)((ks >> 2) * kPanelBytes + (ks & 3) * 32)),
+                      (term | ks) ? 1u : 0u);
+  wg_commit();
+  wg_wait<0>();
+  fence_regs(d); fence_regs(ahi); fence_regs(alo);
+}
+
+// ---- accumulator fragment of a warpgroup's 64 x 128 tile --------------------------------------------------------------
+// Thread (warp w of the warpgroup, lane): rows 16 w + lane / 4 (element bit 1 clear) and + 8 (set); element i holds column 8 (i / 4) + 2 (lane % 4)
+// + (i & 1).  Element pairs (4 ks, 4 ks + 2) / (4 ks + 1, 4 ks + 3) are exactly the A fragment of K step ks in the permuted K order (kperm).
+__device__ __forceinline__ int frag_col(int i, int quad_lane) { return 8 * (i >> 2) + 2 * quad_lane + (i & 1); }
+// values of a 64 x 128 fragment -> A operand registers (hi / lo) of the next product
+__device__ __forceinline__ void frag_to_a(const float (&v)[64], uint32_t (&hi)[16][4], uint32_t (&lo)[16][4]) {
+#pragma unroll
+  for (int ks = 0; ks < 16; ++ks) {
+    tf32_split_u(v[4 * ks + 0], hi[ks][0], lo[ks][0]); tf32_split_u(v[4 * ks + 2], hi[ks][1], lo[ks][1]);
+    tf32_split_u(v[4 * ks + 1], hi[ks][2], lo[ks][2]); tf32_split_u(v[4 * ks + 3], hi[ks][3], lo[ks][3]);
+  }
+}
+// head on the CUDA cores: q[row][a] = sum_j relu(D + b2)[row][j] W3[a][j] for the thread's two rows over its 32 columns, then over the four
+// threads of the quad in a fixed order (xor 1, then xor 2); on return h holds relu(D + b2)
+__device__ __forceinline__ void head_quad(float (&h)[64], const float* b2, const float* w3f, int out, int quad_lane, float (&q0)[kOutPad], float (&q1)[kOutPad]) {
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const float2 bb = *reinterpret_cast<const float2*>(b2 + frag_col(i, quad_lane));
+    h[i] = fmaxf(h[i] + bb.x, 0.f); h[i + 1] = fmaxf(h[i + 1] + bb.y, 0.f);
+  }
+#pragma unroll
+  for (int a = 0; a < kOutPad; ++a) {
+    float s0 = 0.f, s1 = 0.f;
+    if (a < out) {
+#pragma unroll
+      for (int n = 0; n < 16; ++n) {
+        const float2 w = *reinterpret_cast<const float2*>(w3f + a * kHidden + 8 * n + 2 * quad_lane);
+        s0 = fmaf(h[4 * n + 1], w.y, fmaf(h[4 * n], w.x, s0));
+        s1 = fmaf(h[4 * n + 3], w.y, fmaf(h[4 * n + 2], w.x, s1));
+      }
+      s0 += __shfl_xor_sync(0xFFFFFFFFu, s0, 1); s1 += __shfl_xor_sync(0xFFFFFFFFu, s1, 1);
+      s0 += __shfl_xor_sync(0xFFFFFFFFu, s0, 2); s1 += __shfl_xor_sync(0xFFFFFFFFu, s1, 2);
+    }
+    q0[a] = s0; q1[a] = s1;
+  }
+}
+
+// ---- the tensor-core training pass (tc_train.cu) ---------------------------------------------------------------------
+// Row records [rows][kRowRec] floats: [0, 8) online outputs, [16, 20) / [20, 24) ReLU masks of H1 / H2 (training forward); [8] dLoss/dq[act],
+// [9] act (int bits) (dH1 kernel).  Mask word q holds the columns of the fragment threads with lane % 4 == q: bit 2n + b = column 8n + 2q + b.
+constexpr int kRowRec = 32;
+constexpr int kRecG = 8, kRecAct = 9, kRecMask1 = 16, kRecMask2 = 20;
+// a thread's ReLU mask words of its two fragment rows
+__device__ __forceinline__ void frag_masks(const float (&h)[64], uint32_t& m0, uint32_t& m1) {
+  m0 = 0; m1 = 0;
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const uint32_t bit = (h[i] > 0.f ? 1u : 0u) << (((i >> 2) << 1) | (i & 1));
+    if (i & 2) m1 |= bit; else m0 |= bit;
+  }
+}
 
 struct TcTrainParams {
   RowPlan plan; RowSource src; NetLayout lay;
   const uint8_t* images;      // forward images [n_nets][kImageBytes]
   const uint8_t* bwd_images;  // backward images [n_nets][kBwdImageBytes]
-  float* q_out;               // [rows][out] online outputs (optional)
-  // H1, H2, dH1: [32 float4 column chunks][rows][4] -- chunk-major, so that a warp whose lanes are 32 consecutive rows writes or
-  // reads 512 contiguous bytes per instruction (row-major rows of 512 B cost one cache line per lane and instruction)
+  // H1, H2, dH1: feature-major [128][rows] (the weight-gradient kernel stages 32 consecutive rows of one feature per warp instruction)
   float* h1g; float* h2g; float* dh1g; size_t rows;
   float* rec;                 // [rows][kRowRec] row records
-  float* xg;                  // [rows][kMaxObsDim] gathered observation rows (zero padded to the staged width): the weight-gradient
-                              // kernel reads them without chasing the episode index again
+  float* xg;                  // [rows][kMaxObsDim] gathered observation rows: the weight-gradient kernel reads them without chasing the episode index again
   const float* tq; const float* td_ext; int td_agent_stride; float gamma; int double_q;
   float* scratch; int scratch_pitch; float* loss_part;
-  unsigned long long* dbg;    // profiling builds: host-mapped progress marks (NULL otherwise)
 };
-unsigned long long* tc_debug_progress_ptr();   // core.cu
-
-int tc_train2_init();
-int tc_train3_init();
-int launch_tc_dqn_train3(const TcTrainParams& p, int grid, cudaStream_t st, cudaEvent_t* between);   // tc_train3.cu: activations stay on chip
-int launch_tc_dqn_fwd2(const TcTrainParams& p, int grid, cudaStream_t st);
-int launch_tc_dh12(const TcTrainParams& p, int grid, cudaStream_t st);
-
-// ---- pieces shared by the two-accumulator (ping-pong) kernels: tc_forward2_kernel, tc_dqn_fwd2_kernel, tc_dh12_kernel ---------------------------
-constexpr int kTailBytes = kImageBytes - kOffB1;                    // b1 | b2 | b3 | FP32 W3
-constexpr uint32_t kColD0 = 256, kColD1 = 384;                      // TMEM: A hi [0,128) | A lo [128,256) | D0 | D1
-// a 128 x 128 x 128 product in TS form (A hi | lo in the TMEM A columns, B = K-major SWIZZLE_128B hi / lo images of four 32-feature panels):
-// 3 terms x 16 k-steps, fully unrolled, issued by one thread
-__device__ __forceinline__ void issue_kmajor_ts(uint32_t tmem, uint32_t d_col, uint32_t b_hi, uint32_t b_lo) {
-  const uint32_t idesc = idesc_tf32(kHidden);
-  const uint64_t dhi = kmajor_desc(b_hi), dlo = kmajor_desc(b_lo);
-#pragma unroll
-  for (int term = 0; term < 3; ++term)
-#pragma unroll
-    for (int ks = 0; ks < kHidden / 8; ++ks)
-      mma_tf32_ts(tmem + d_col, tmem + (term == 0 ? kColALo : kColAHi) + ks * 8, (term == 1 ? dlo : dhi) + (uint32_t)(((ks >> 2) * kPanelBytes + (ks & 3) * 32) >> 4), idesc,
-                  (term | ks) ? 1u : 0u);
-}
-// layer 1 in SS form: D = X_lo*W_hi + X_hi*W_lo + X_hi*W_hi, both operands K-major SWIZZLE_128B panels of 32 features (one thread)
-__device__ __forceinline__ void issue_l1_ss(uint32_t d_tmem, uint32_t xs_hi, uint32_t xs_lo, uint32_t w_hi, uint32_t w_lo, int ksteps) {
-  const uint32_t idesc = idesc_tf32(kHidden);
-  const uint64_t ahi = kmajor_desc(xs_hi), alo = kmajor_desc(xs_lo), bhi = kmajor_desc(w_hi), blo = kmajor_desc(w_lo);
-#pragma unroll
-  for (int term = 0; term < 3; ++term)
-#pragma unroll
-    for (int ks = 0; ks < kMaxObsDim / 8; ++ks)
-      if (ks < ksteps) mma_tf32_ss(d_tmem, (term == 0 ? alo : ahi) + (uint32_t)((ks * 32) >> 4), (term == 1 ? blo : bhi) + (uint32_t)((ks * 32) >> 4), idesc, (term | ks) ? 1u : 0u);
-}
-// this thread's 8 observation columns of its row -> the K-major SWIZZLE_128B X tile (hi | lo): 16-byte chunk c of row r sits at chunk c ^ (r & 7)
-__device__ __forceinline__ void stage_x_tile(uint8_t* xs, int r, int cq, const float (&x)[8]) {
-  float4 h0, h1, l0, l1;
-  tf32_split(x[0], h0.x, l0.x); tf32_split(x[1], h0.y, l0.y); tf32_split(x[2], h0.z, l0.z); tf32_split(x[3], h0.w, l0.w);
-  tf32_split(x[4], h1.x, l1.x); tf32_split(x[5], h1.y, l1.y); tf32_split(x[6], h1.z, l1.z); tf32_split(x[7], h1.w, l1.w);
-  const int o0 = r * 128 + (((2 * cq) ^ (r & 7)) << 4), o1 = r * 128 + (((2 * cq + 1) ^ (r & 7)) << 4);
-  *reinterpret_cast<float4*>(xs + o0) = h0; *reinterpret_cast<float4*>(xs + o1) = h1;
-  *reinterpret_cast<float4*>(xs + kPanelBytes + o0) = l0; *reinterpret_cast<float4*>(xs + kPanelBytes + o1) = l1;
-}
-__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
-
-// head on the CUDA cores: this thread's 32 columns of relu(D + b2) against the FP32 copy of W3 -> 8 partial outputs of its row.  Packed FP32
-// (fma.rn.f32x2, sm_100): even and odd columns accumulate in the two halves of a register pair and are added at the end (fixed order).
-__device__ __forceinline__ void head_partial(const uint32_t (&ra)[16], const uint32_t (&rb)[16], const float* b2c, const float4* w3c, int out, float (&q)[kOutPad]) {
-  float2 q2[kOutPad];
-#pragma unroll
-  for (int a = 0; a < kOutPad; ++a) q2[a] = make_float2(0.f, 0.f);
-#pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    const uint32_t (&acc)[16] = g < 4 ? ra : rb;
-    const int o = 4 * (g & 3);
-    const float4 bb = *reinterpret_cast<const float4*>(b2c + 4 * g);
-    float2 h01 = __fadd2_rn(make_float2(__uint_as_float(acc[o]), __uint_as_float(acc[o + 1])), make_float2(bb.x, bb.y));
-    float2 h23 = __fadd2_rn(make_float2(__uint_as_float(acc[o + 2]), __uint_as_float(acc[o + 3])), make_float2(bb.z, bb.w));
-    h01.x = fmaxf(h01.x, 0.f); h01.y = fmaxf(h01.y, 0.f); h23.x = fmaxf(h23.x, 0.f); h23.y = fmaxf(h23.y, 0.f);
-#pragma unroll
-    for (int a = 0; a < kOutPad; ++a) {
-      if (a < out) {
-        const float4 w = w3c[a * (kHidden / 4) + g];
-        q2[a] = __ffma2_rn(h23, make_float2(w.z, w.w), __ffma2_rn(h01, make_float2(w.x, w.y), q2[a]));
-      }
-    }
-  }
-#pragma unroll
-  for (int a = 0; a < kOutPad; ++a) q[a] = q2[a].x + q2[a].y;
-}
-
 
 }  // namespace marl

@@ -1,4 +1,4 @@
-"""IDQN / VDN learners on the B200 path -- drop-in for marlbase/dqn/model.py (QNetwork 14-196, VDNetwork 199-269).
+"""IDQN / VDN learners on the GPU path -- drop-in for marlbase/dqn/model.py (QNetwork 14-196, VDNetwork 199-269).
 
 Same constructor signature and Hydra `_target_` role (configs/algorithm/idqn.yaml:6-14, vdn.yaml:11-13), same
 `state_dict()` key names (`critic.independent.{i}.network.{0,2,4}.{weight,bias}`, `target.…`; shared:
@@ -80,14 +80,14 @@ class QNetwork:
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch=None, max_episode_length=None):
         if use_rnn:
-            raise NotImplementedError("use_rnn=True (GRU) is out of scope of the B200 hot path (every shipped config has use_rnn: False)")
+            raise NotImplementedError("use_rnn=True (GRU) is out of scope of the GPU hot path (every shipped config has use_rnn: False)")
         if list(layers) != [HIDDEN, HIDDEN]:
             raise NotImplementedError(f"layers={list(layers)}: the fused kernels implement the shipped [128, 128] MLP only")
         opt = getattr(cfg, "optimizer", "Adam")
         if (opt if isinstance(opt, str) else opt.__name__) != "Adam":
             raise NotImplementedError("only optimizer=Adam is implemented")
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
-            raise nat.NativeError("the B200 learners need algorithm.model.device=cuda (no CPU fallback)")
+            raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
         self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
         self.n_agents = len(obs_space)
         obs_dims, act_dims = [_dim(o) for o in obs_space], [_dim(a) for a in action_space]

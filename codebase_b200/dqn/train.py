@@ -1,4 +1,4 @@
-"""IDQN / VDN training driver on the B200 path -- drop-in for marlbase/dqn/train.py `main(env, eval_env, logger,
+"""IDQN / VDN training driver on the GPU path -- drop-in for marlbase/dqn/train.py `main(env, eval_env, logger,
 time_limit, **cfg)` (`algorithm._target_: dqn.train.main`, configs/algorithm/idqn.yaml:4).
 
 Same loop structure as the reference (dqn/train.py:298-343), vectorised over E = env.parallel_envs instances:
@@ -127,7 +127,7 @@ def main(env, eval_env, logger, time_limit, **cfg):
             last_eval = step
 
         if cfg.video_interval:
-            raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the B200 hot path")
+            raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the GPU hot path")
 
         if cfg.save_interval and (step - last_save) >= cfg.save_interval:
             Path("checkpoints").mkdir(exist_ok=True)

@@ -4,7 +4,7 @@
 
 Like the reference it reads `<path>/config.yaml`, builds the run's env, picks `checkpoints/model_s<load_step>.pt` (the latest when load_step is
 not given), swaps `algorithm._target_`'s "train" for "eval" and calls it with (env, ckpt_path, **algorithm).  The reference's eval targets record
-a video of `video_frames` steps (dqn/eval.py, ac/eval.py); rendering is out of scope of the B200 path, so ours run `episodes` evaluation episodes on
+a video of `video_frames` steps (dqn/eval.py, ac/eval.py); rendering is out of scope of the GPU path, so ours run `episodes` evaluation episodes on
 the device with the loaded parameters and write their returns to `<path>/eval_s<load_step>.json` instead."""
 from __future__ import annotations
 

@@ -53,9 +53,9 @@ class LbfConfig:
 def parse_env_id(name: str, time_limit: int = 0, **overrides) -> LbfConfig:
     m = _ID.match(name)
     if not m:
-        raise ValueError(f"unsupported environment id {name!r}: the B200 path implements Level-Based Foraging ids only")
+        raise ValueError(f"unsupported environment id {name!r}: the GPU path implements Level-Based Foraging ids only")
     if m["grid"]:
-        raise ValueError("grid observations (Foraging-grid-*) are not implemented on the B200 path")
+        raise ValueError("grid observations (Foraging-grid-*) are not implemented on the GPU path")
     s, s2, p, f, v = int(m["s"]), int(m["s2"]), int(m["p"]), int(m["f"]), int(m["v"])
     cfg = LbfConfig(rows=s, cols=s2, n_agents=p, max_num_food=f, sight=2 if m["po"] else s,
                     max_player_level=2 if v >= 3 else 3, force_coop=int(bool(m["coop"])),
@@ -88,7 +88,7 @@ class TrajStore:
 class NativeLbf:
     def __init__(self, cfg: LbfConfig, n_envs: int, seed: int, env_gid0: int = 0, device: int | None = None):
         if not torch.cuda.is_available():
-            raise nat.NativeError("codebase_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise nat.NativeError("codebase_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.cfg, self.E, self.seed, self.gid0 = cfg, int(n_envs), int(seed), int(env_gid0)
         self.device_index = torch.cuda.current_device() if device is None else int(device)
         self.device = torch.device("cuda", self.device_index)

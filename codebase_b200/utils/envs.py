@@ -1,4 +1,4 @@
-"""Env factory on the B200 path -- drop-in for marlbase/utils/envs.py (`env._target_: utils.envs.make_env`,
+"""Env factory on the GPU path -- drop-in for marlbase/utils/envs.py (`env._target_: utils.envs.make_env`,
 configs/default.yaml:28-35).  Returns a vector env whose transition runs in libmarlb200.so (marl_lbf_*).
 
 `B200VecEnv` speaks the gymnasium<1.0 vector protocol the reference's drivers rely on (marlbase/ac/train.py:30-34,
@@ -93,13 +93,13 @@ def episode_info(returns, length, seconds):
 def make_env(seed, enable_video=False, name=None, time_limit=None, clear_info=False, observe_id=False, standardise_rewards=False,
              wrappers=None, parallel_envs=None, env_gid0=0, device=None, **kwargs):
     """marlbase/utils/envs.py:115-119 with the same config keys.  `parallel_envs` absent -> 1 env (the reference's single-env
-    factory); the B200 overlays set it to thousands."""
+    factory); the GPU overlays set it to thousands."""
     if enable_video:
-        raise NotImplementedError("video recording is out of scope of the B200 hot path (algorithm.video_interval must stay False)")
+        raise NotImplementedError("video recording is out of scope of the GPU hot path (algorithm.video_interval must stay False)")
     wrappers = list(wrappers or [])
     unknown = [w for w in wrappers if w not in SUPPORTED_WRAPPERS]
     if unknown:
-        raise NotImplementedError(f"env.wrappers {unknown} are not implemented on the B200 path (supported: {sorted(SUPPORTED_WRAPPERS)})")
+        raise NotImplementedError(f"env.wrappers {unknown} are not implemented on the GPU path (supported: {sorted(SUPPORTED_WRAPPERS)})")
     cfg = parse_env_id(name, time_limit or 0, **kwargs)
     cfg.cooperative_reward = int("CooperativeReward" in wrappers)
     cfg.observe_id, cfg.standardise_rewards = int(bool(observe_id)), int(bool(standardise_rewards))   # envs.py:97-101, inside the listed wrappers

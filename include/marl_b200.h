@@ -1,17 +1,17 @@
 /*
- * marl_b200.h -- C ABI of libmarlb200.so, the B200 (sm_100a) native hot path behind marlbase's plugin surface.
+ * marl_b200.h -- C ABI of libmarlb200.so, the H100 (sm_90a) native hot path behind marlbase's plugin surface.
  *
  * The reference (marl-book/codebase, `marlbase`) is 100 % Python and has NO FFI boundary of its own: its
  * plugin surface is Hydra `_target_` strings + Python duck typing (SURVEY.md §8b).  This header is therefore
  * the boundary a maintainer would bind (ctypes stub shown in INTEGRATION.md) to replace, one for one, the
- * Python call sites cited on each entry point below.  Citations are path:line under /root/reference/.
+ * Python call sites cited on each entry point below.  Citations are path:line in the reference project (marl-book/codebase).
  *
  * Conventions
  *   - every pointer argument documented "device" is a CUDA device pointer owned by the caller (a torch tensor);
  *     `stream` is a cudaStream_t passed as void*; calls enqueue work and return without synchronising;
  *   - return value 0 = ok, negative = MARL_E*; the message is in marl_last_error() (thread local);
  *   - handles are opaque, one host thread per GPU, not thread safe; no C++ / torch types cross the ABI;
- *   - there is NO CPU fallback: every entry point fails with MARL_ECUDA if no sm_100-class device is present.
+ *   - there is NO CPU fallback: every entry point fails with MARL_ECUDA if no sm_90 (Hopper) device is present.
  */
 #ifndef MARL_B200_H
 #define MARL_B200_H
@@ -32,16 +32,13 @@ extern "C" {
 
 int marl_version(void);
 const char* marl_last_error(void);
-/* Process-wide options: "tensor_core_forward" 1 (default) = forward-only passes on tcgen05 with the 3xTF32 split, 0 = FP32 FFMA;
- * "tensor_core_backward" 1 = the DQN-family training pass runs as the three-kernel tcgen05 pipeline (tc_train.cu), 0 = fused FP32 kernel. */
+/* Process-wide options: "tensor_core_forward" 1 (default) = forward-only passes on the tensor cores (wgmma) with the 3xTF32 split, 0 = FP32 FFMA;
+ * "tensor_core_backward" 1 = the DQN-family training pass runs as the three-kernel wgmma pipeline (tc_train.cu), 0 = fused FP32 kernel;
+ * "split_exchange" (several ranks) 1 = gradient exchange split around the next update's target forward. */
 int marl_set_option(const char* name, int32_t value);
-/* "tensor_core_pingpong": bit mask of the tensor-core kernels that keep two accumulators in TMEM (bit 0 forward kernels, bit 1 dH1 kernel; default 2).
- * Profiling builds (-DMARL_TC_TIMESTAMPS): timeline probes of kernel `which` as uint64 [160 CTAs][32 slots][globaltimer ns, clock64] into HOST
+/* Profiling builds (-DMARL_TC_TIMESTAMPS): timeline probes of kernel `which` as uint64 [160 CTAs][32 slots][globaltimer ns, clock64] into HOST
  * memory; product builds return MARL_EINVAL. */
 int marl_debug_timestamps(int32_t which, uint64_t* out);
-/* Profiling builds: `mapped` = host-mapped (pinned, device-visible) uint64 [3][160][32]: the on-chip training kernels store, per kernel / CTA / warp,
- * 1 + the last probe slot the warp passed -- readable from the host while a kernel hangs.  NULL switches it off. */
-int marl_debug_progress(uint64_t* mapped);
 
 /* ------------------------------------------------------------------------------------------------------
  * Level-Based Foraging, E environments per handle, one transition of all of them per launch.

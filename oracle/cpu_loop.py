@@ -3,7 +3,7 @@ env -> one sampled update), marlbase/dqn/model.py:94-116 (act: per-agent forward
 `random.random()` exploration test per step), 1 torch thread as marlbase/run.py:29 mandates.
 
 TEST / MEASUREMENT INFRASTRUCTURE ONLY: this is what bench.py times as `cpu_baseline` and as `--impl reference`
-(kind "port": /root/reference and the third-party `lbforaging` package do not exist on the GPU box).  The env is the
+(kind "port": the reference project and the third-party `lbforaging` package are not dependencies of this one).  The env is the
 pure-Python restatement (oracle/lbf_ref.py), which has the same cost structure as upstream lbforaging (Python objects +
 small numpy arrays); the learner is oracle/learner_ref.py (PyTorch CPU autograd + the Adam arithmetic of torch.optim).
 """

@@ -5,7 +5,7 @@
  * path (codebase_b200/).  Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
  * reference legs use it, and only as the checker / CPU baseline.
  *
- * PARITY UNPINNED (env half): `ForagingEnv.step/reset` is NOT in /root/reference -- it lives in the
+ * PARITY UNPINNED (env half): `ForagingEnv.step/reset` is NOT in the reference project -- it lives in the
  * third-party, un-vendored, unpinned pip package `lbforaging` (GitHub uoe-agents/lb-foraging, the
  * gymnasium-era 2.x/3.x line that registers the `-v3` ids; reference call sites
  * marlbase/utils/envs.py:27-37,90-92, consumer marlbase/dqn/train.py:203,217, marlbase/ac/train.py:30,79-81).

@@ -1,10 +1,10 @@
 """CPU restatement (PyTorch float32, autograd) of the reference learner arithmetic.  TEST INFRASTRUCTURE ONLY.
 
 Written functionally over FLAT parameter vectors in the device layout ([n_nets][P], reference state_dict order), so
-that it also pins the layout conversion.  Pinned against the live reference classes (tests marked `refsrc`, build
-container only) and against committed golden vectors generated from them (tests/golden/, make_golden.py).
+that it also pins the layout conversion.  Pinned against committed golden vectors that the reference classes produced
+(tests/golden/, make_golden.py).
 
-Restated from (path:line under /root/reference/marlbase):
+Restated from (path:line in the reference project's marlbase/):
   utils/models.py:14-48      FCNetwork = Linear-ReLU-Linear-ReLU-Linear
   utils/models.py:133-300    independent / shared per-agent network containers
   dqn/model.py:118-163       QNetwork._compute_loss (double-Q TD target, MSE summed over agents, masked mean)
@@ -16,6 +16,7 @@ Restated from (path:line under /root/reference/marlbase):
 """
 from __future__ import annotations
 
+import copy
 import math
 from dataclasses import dataclass, field
 
@@ -213,7 +214,8 @@ def kink_risk(loss_fn, theta, near=2e-6):
 
 
 def dqn_kink_risk(st: DqnState, batch, hp: DqnHP):
-    return kink_risk(lambda th: dqn_loss(th, st.theta_tgt, st.agent_net, st.in_dim, st.out_dim, batch, hp), st.theta)
+    # the loss of the update: with standardised returns it reads (and advances) the running statistics, so each evaluation gets a copy of them
+    return kink_risk(lambda th: dqn_loss(th, st.theta_tgt, st.agent_net, st.in_dim, st.out_dim, batch, hp, ret_ms=copy.deepcopy(st.ret_ms)), st.theta)
 
 
 def dqn_update(st: DqnState, batch, hp: DqnHP):

@@ -1,6 +1,6 @@
 """CPU restatement (PyTorch float32, autograd) of the reference's QMIX learner.  TEST INFRASTRUCTURE ONLY.
 
-Restated from (path:line under /root/reference/marlbase):
+Restated from (path:line in the reference project's marlbase/):
   dqn/model.py:272-340   QMixer: hypernetworks |W1(s)|, b1(s), |w_final(s)|, V(s); Q_tot = elu(q W1 + b1) w_final + V
   dqn/model.py:343-384   QMixNetwork.__init__: state = the agents' observations concatenated, one Adam over critic + mixer
   dqn/model.py:386-443   _compute_loss (double-Q target per agent, target mixer on the next state, rewards[0]) and soft / hard updates of the mixer
@@ -9,7 +9,7 @@ Restated from (path:line under /root/reference/marlbase):
 The mixer's parameters are one flat vector in the reference's state_dict order (hypernet_layers == 2):
   hyper_w_1.0.{weight [He,S], bias [He]}, hyper_w_1.2.{weight [N*E,He], bias [N*E]}, hyper_w_final.0.{weight [He,S], bias [He]},
   hyper_w_final.2.{weight [E,He], bias [E]}, hyper_b_1.{weight [E,S], bias [E]}, V.0.{weight [E,S], bias [E]}, V.2.{weight [1,E], bias [1]}
-Pinned against the live reference classes by tests/test_qmix.py (refsrc tests, build container) and the golden vectors it checks.
+Pinned against outputs of the reference classes by tests/test_qmix.py (golden vectors under tests/golden).
 """
 from __future__ import annotations
 

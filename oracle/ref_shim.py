@@ -1,9 +1,9 @@
-"""Import shim for the LIVE reference learner classes under /root/reference (build container only).
+"""Import shim for the reference project's learner classes (a checkout of marl-book/codebase named by MARL_REFERENCE_ROOT).
 
-TEST INFRASTRUCTURE ONLY.  The reference's learner half imports cleanly once `gymnasium.spaces.flatdim`
+FIXTURE GENERATION ONLY.  The reference's learner half imports cleanly once `gymnasium.spaces.flatdim`
 (its only gymnasium use: marlbase/dqn/model.py:4, marlbase/ac/model.py:4) and stub `hydra` / `omegaconf` /
-`imageio` modules exist (imports at marlbase/dqn/train.py:6,8,11).  Nothing here is available on the GPU box:
-tests that use it are marked `refsrc`, and tests/golden/make_golden.py uses it to emit committed fixtures.
+`imageio` modules exist (imports at marlbase/dqn/train.py:6,8,11).  tests/golden/make_golden.py uses it to emit the
+committed fixtures that the tests compare against; no test imports the reference itself.
 """
 from __future__ import annotations
 
@@ -11,11 +11,11 @@ import os
 import sys
 import types
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("MARL_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF_ROOT, "marlbase"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "marlbase"))
 
 
 class Space:
@@ -39,7 +39,7 @@ def _flatdim(space):
 def load():
     """Returns a namespace with the reference modules: dqn_model, dqn_train, ac_model, utils, models."""
     if not available():
-        raise RuntimeError("/root/reference is not present")
+        raise RuntimeError("set MARL_REFERENCE_ROOT to a checkout of the reference project (the directory that holds marlbase/)")
     if "gymnasium" not in sys.modules:
         gym = types.ModuleType("gymnasium")
         spaces = types.ModuleType("gymnasium.spaces")

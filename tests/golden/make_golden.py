@@ -1,7 +1,8 @@
-"""Generates tests/golden/*.npz from the LIVE reference learner classes (build container only; /root/reference does
-not exist on the GPU box).  Run:  python tests/golden/make_golden.py
-Every fixture stores the inputs in the device ("trajectory store") layout plus the reference's outputs, so that both
-the CPU oracle (oracle/learner_ref.py) and the CUDA path are checked against numbers the reference itself produced."""
+"""Generates tests/golden/*.npz from the reference project's learner classes (marl-book/codebase, `marlbase`).  Run with a checkout of it:
+    MARL_REFERENCE_ROOT=<checkout> python tests/golden/make_golden.py
+Every fixture stores the inputs in the device ("trajectory store") layout (or the seeds they are drawn from) plus the reference's outputs, so
+that both the CPU oracle (oracle/learner_ref.py) and the CUDA path are checked against numbers the reference itself produced.  Parameter-sized
+outputs of the two-network cases are stored as every STRIDE-th element (tests/helpers.py), which keeps every fixture under 1 MB."""
 import os
 import sys
 
@@ -12,6 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 from oracle import learner_ref as lr  # noqa: E402
 from oracle import ref_shim  # noqa: E402
+from tests.helpers import STRIDE  # noqa: E402
 
 OUT = os.path.dirname(os.path.abspath(__file__))
 N, D, A, T = 2, 15, 6, 25
@@ -54,7 +56,20 @@ def to_ref_batch(mod, store, idx):
     return mod.Batch(b["obss"], b["actions"], b["rewards"], b["dones"], b["filled"], None)
 
 
-def dqn_case(name, cls_name, sharing, n_updates=3, B=8, **cfgkw):
+def sampled(out, keys, stride):
+    """the parameter-sized outputs `keys` as every stride-th element; `stride` is stored with them"""
+    for k in keys:
+        out[k] = out[k][::stride]
+    out["stride"] = np.int64(stride)
+    return out
+
+
+DQN_OUTPUTS = ("grad0", "grad0_clipped", "adam_m_final", "adam_v_final", "theta_final", "target_final")
+A2C_OUTPUTS = ("actor_grad0_clipped", "critic_grad0_clipped", "actor_adam_m_final", "actor_adam_v_final", "critic_adam_m_final", "critic_adam_v_final",
+               "actor_final", "critic_final", "target_final")
+
+
+def dqn_case(name, cls_name, sharing, n_updates=3, B=8, stride=1, **cfgkw):
     ref = ref_shim.load()
     torch.manual_seed(SEEDS[name])
     rng = np.random.default_rng(SEEDS[name])
@@ -94,11 +109,11 @@ def dqn_case(name, cls_name, sharing, n_updates=3, B=8, **cfgkw):
     sd = model.state_dict()
     out["theta_final"] = lr.flat_from_state_dict(sd, prefix, n_nets).numpy()
     out["target_final"] = lr.flat_from_state_dict(sd, prefix.replace("critic", "target"), n_nets).numpy()
-    np.savez_compressed(os.path.join(OUT, f"{name}.npz"), **out)
+    np.savez_compressed(os.path.join(OUT, f"{name}.npz"), **sampled(out, DQN_OUTPUTS, stride))
     print(name, losses)
 
 
-def a2c_case(name, sharing, n_updates=2, P=6, **cfgkw):
+def a2c_case(name, sharing, n_updates=2, P=6, stride=1, **cfgkw):
     ref = ref_shim.load()
     torch.manual_seed(SEEDS[name])
     rng = np.random.default_rng(SEEDS[name])
@@ -145,7 +160,7 @@ def a2c_case(name, sharing, n_updates=2, P=6, **cfgkw):
     out["actor_final"] = lr.flat_from_state_dict(sd, f"actor.{kind}", n_nets).numpy()
     out["critic_final"] = lr.flat_from_state_dict(sd, f"critic.{kind}", n_nets).numpy()
     out["target_final"] = lr.flat_from_state_dict(sd, f"target_critic.{kind}", n_nets).numpy()
-    np.savez_compressed(os.path.join(OUT, f"{name}.npz"), **out)
+    np.savez_compressed(os.path.join(OUT, f"{name}.npz"), **sampled(out, A2C_OUTPUTS, stride))
     print(name, metrics)
 
 
@@ -166,10 +181,15 @@ def misc_case():
 
 
 if __name__ == "__main__":
-    dqn_case("idqn_indep", "QNetwork", False, target_update_interval_or_tau=2)
-    dqn_case("idqn_single_q_polyak_noclip", "QNetwork", False, double_q=False, grad_clip=False, target_update_interval_or_tau=0.05)
+    dqn_case("idqn_indep", "QNetwork", False, stride=STRIDE, target_update_interval_or_tau=2)
+    dqn_case("idqn_single_q_polyak_noclip", "QNetwork", False, stride=STRIDE, double_q=False, grad_clip=False, target_update_interval_or_tau=0.05)
     dqn_case("idqn_shared", "QNetwork", True, target_update_interval_or_tau=2)
-    dqn_case("vdn_indep", "VDNetwork", False, target_update_interval_or_tau=2)
-    a2c_case("ia2c_indep", False)
+    dqn_case("vdn_indep", "VDNetwork", False, stride=STRIDE, target_update_interval_or_tau=2)
+    a2c_case("ia2c_indep", False, stride=STRIDE)
     a2c_case("ia2c_shared", True, grad_clip=0.5)
     misc_case()
+    from tests import test_oracle_learner, test_ppo, test_qmix, test_standardise_returns_dqn
+
+    test_qmix.make_golden()
+    for mod in (test_qmix, test_ppo, test_oracle_learner, test_standardise_returns_dqn):
+        mod.make_reference_outputs(ref_shim.load(), ref_shim)

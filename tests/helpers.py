@@ -1,8 +1,41 @@
-"""Shared helpers of the GPU parity tests."""
+"""Shared helpers of the parity tests."""
 import functools
+import os
 
+import numpy as np
 import pytest
 import torch
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+# Parameter-sized vectors that the reference project produced are stored as every STRIDE-th element (fixtures stay small); inputs are stored whole
+# or regenerated from seeds.
+STRIDE = 8
+
+
+def reference_outputs(name):
+    """What the reference project (marlbase) computed for a test's seeded inputs: tests/golden/<name>.npz, written by tests/golden/make_golden.py."""
+    return np.load(os.path.join(GOLDEN, f"{name}.npz"))
+
+
+def golden_stride(g):
+    """stride of the parameter-sized outputs of a fixture (1: stored whole)"""
+    return int(g["stride"]) if "stride" in g.files else 1
+
+
+def seeded_params(lr, n_nets, in_dim, out_dim, seed):
+    """Initial weights of a parity case (the reference's orthogonal initialisation, seeded): the tests start the oracle from them, and
+    tests/golden/make_golden.py loaded the same weights into the reference model before recording its outputs."""
+    return lr.init_flat(n_nets, in_dim, out_dim, generator=torch.Generator().manual_seed(seed))
+
+
+def load_params(model, lr, prefixes, flat, n_nets, in_dim, out_dim):
+    """Copy flat weights into the sub-networks `prefixes` of a reference model (fixture generation only)."""
+    sd = {}
+    for prefix in prefixes:
+        sd.update(lr.state_dict_from_flat(flat, prefix, n_nets, in_dim, out_dim))
+    missing = set(sd) - set(model.state_dict())
+    assert not missing, sorted(missing)[:4]
+    model.load_state_dict(sd, strict=False)
 
 TIE = 2e-5   # relative gap of the two best online Q-values under which the double-Q argmax may legitimately differ between two implementations
 

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from oracle import learner_ref as lr
+from tests.helpers import golden_stride
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -80,11 +81,12 @@ def test_update_matches_reference_golden(name):
         if u == 0:
             _, ret, _ = m.scratch(P, T)
             _close(ret.permute(2, 1, 0).cpu().numpy(), g["returns0"])
+    S = golden_stride(g)
     am, av = m.adam_m.cpu().numpy(), m.adam_v.cpu().numpy()   # element-wise against the reference optimiser's state
-    _close_scaled(am[: m.n_actor], g["actor_adam_m_final"]); _close_scaled(am[m.n_actor:], g["critic_adam_m_final"])
-    _close_scaled(av[: m.n_actor], g["actor_adam_v_final"], tol=2e-5); _close_scaled(av[m.n_actor:], g["critic_adam_v_final"], tol=2e-5)
+    _close_scaled(am[: m.n_actor][::S], g["actor_adam_m_final"]); _close_scaled(am[m.n_actor:][::S], g["critic_adam_m_final"])
+    _close_scaled(av[: m.n_actor][::S], g["actor_adam_v_final"], tol=2e-5); _close_scaled(av[m.n_actor:][::S], g["critic_adam_v_final"], tol=2e-5)
     th, tg = m.theta.cpu().numpy(), m.theta_tgt.cpu().numpy()
-    for got, want in ((th[: m.n_actor], g["actor_final"]), (th[m.n_actor:], g["critic_final"]), (tg, g["target_final"])):
+    for got, want in ((th[: m.n_actor][::S], g["actor_final"]), (th[m.n_actor:][::S], g["critic_final"]), (tg[::S], g["target_final"])):
         d = np.abs(got - want)
         assert np.quantile(d, 0.999) < 1e-5 and d.max() < 2 * hp.lr * len(g["steps"]) + 1e-6, (np.quantile(d, 0.999), d.max())
 

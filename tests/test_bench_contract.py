@@ -1,6 +1,6 @@
 """CPU: bench.py's contract, exercised on CODE (not on a committed artefact): the reference arm runs here end to end (it needs no GPU) and must
 print exactly one JSON line with every contract key and consistent timing arithmetic; the workload table matches BASELINE.json's configs; under
-a multi-rank launch only rank 0 speaks.  The B200 arm's line is checked by the same validator in the `-m gpu` suite (tests/test_bench_gpu.py)."""
+a multi-rank launch only rank 0 speaks.  The GPU arm's line is checked by the same validator in the `-m gpu` suite (tests/test_bench_gpu.py)."""
 import json
 import os
 import subprocess
@@ -46,7 +46,7 @@ def test_reference_arm_prints_one_contract_line_whose_clock_fits_the_run():
     d = json.loads(lines[0])
     validate_line(d, reference=True)
     assert d["steps"] == 2 and d["warmup"] == 1
-    # the timed steps are wall clock of the whole pool: they must fit inside the driver's own clock around the run (VERDICT r1 weak #3)
+    # the timed steps are wall clock of the whole pool: they must fit inside the caller's own clock around the run (VERDICT r1 weak #3)
     assert d["ms_per_step"] * d["steps"] / 1e3 <= wall
     assert d["cpu_baseline"]["cores"] == len(os.sched_getaffinity(0))
     # every copy stepped real episodes: 3 iterations x <= 25 steps per copy and step

@@ -1,5 +1,5 @@
 """Opportunistic differential test against UPSTREAM lbforaging (SURVEY.md section 8c): the env transition is third-party code that is
-neither in /root/reference nor in this image, so the C / Python restatements are otherwise pinned only by known-answer boards.  Whenever
+neither in the reference project nor a dependency of this one, so the C / Python restatements are otherwise pinned only by known-answer boards.  Whenever
 `import lbforaging` succeeds (a driver-provided install, a developer machine), this steps upstream's ForagingEnv and the C oracle from
 IDENTICAL injected states with identical actions for >= 10^5 (state, action) pairs and requires the same grid, positions, per-agent
 rewards, game-over flag and observation vectors.  Skipped (not failed) when the package is absent."""

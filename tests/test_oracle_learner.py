@@ -1,6 +1,5 @@
-"""CPU: oracle/learner_ref.py (the torch-CPU restatement that travels to the GPU box) pinned against golden vectors
-produced by the LIVE reference classes (tests/golden/make_golden.py) and, when /root/reference is present, against
-the live classes directly."""
+"""CPU: oracle/learner_ref.py (the torch-CPU restatement of the reference learners) pinned against golden vectors produced by the
+reference classes (tests/golden/make_golden.py)."""
 import os
 
 import numpy as np
@@ -8,6 +7,7 @@ import pytest
 import torch
 
 from oracle import learner_ref as lr
+from tests.helpers import STRIDE, golden_stride, load_params, reference_outputs, seeded_params
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 N, D, A, T = 2, 15, 6, 25
@@ -39,20 +39,21 @@ def test_dqn_update_matches_reference_golden(name):
     g, hp = load_dqn_case(name)
     theta = torch.tensor(g["theta0"])
     st = lr.DqnState(theta.clone(), theta.clone(), [int(x) for x in g["agent_net"]], D, A)
+    S = golden_stride(g)
     for u in range(len(g["losses"])):
         store = {k: g[f"u{u}_{k}"] for k in ("obs", "act", "rew", "done", "filled")}
         out = lr.dqn_update(st, lr.batch_from_store(store, g[f"u{u}_idx"]), hp)
         _close(out["loss"], g["losses"][u])
         if u == 0:
-            _close(out["grad"].numpy(), g["grad0"])
-            _close_scaled(out["grad_clipped"].numpy(), g["grad0_clipped"])   # what Adam consumed (after clip_grad_norm_)
-    _close_scaled(st.m.numpy(), g["adam_m_final"])   # element-wise: the loose bound on theta below cannot hide a defect here
-    _close_scaled(st.v.numpy(), g["adam_v_final"], tol=2e-5)
+            _close(out["grad"].numpy()[::S], g["grad0"])
+            _close_scaled(out["grad_clipped"].numpy()[::S], g["grad0_clipped"])   # what Adam consumed (after clip_grad_norm_)
+    _close_scaled(st.m.numpy()[::S], g["adam_m_final"])   # element-wise: the loose bound on theta below cannot hide a defect here
+    _close_scaled(st.v.numpy()[::S], g["adam_v_final"], tol=2e-5)
     # Adam's first steps move every weight by ~lr regardless of |g|: elements whose gradient is rounding noise may
     # flip sign between two float32 summation orders, so compare the bulk tightly and bound the rest by 2*lr per step.
-    d = np.abs(st.theta.numpy() - g["theta_final"])
+    d = np.abs(st.theta.numpy()[::S] - g["theta_final"])
     assert np.quantile(d, 0.999) < 1e-5 and d.max() < 2 * hp.lr * len(g["losses"]) + 1e-6
-    _close(np.quantile(np.abs(st.theta_tgt.numpy() - g["target_final"]), 0.999), 0, atol=1e-5)
+    _close(np.quantile(np.abs(st.theta_tgt.numpy()[::S] - g["target_final"]), 0.999), 0, atol=1e-5)
 
 
 @pytest.mark.parametrize("name", ["ia2c_indep", "ia2c_shared"])
@@ -62,6 +63,7 @@ def test_a2c_update_matches_reference_golden(name):
                   value_loss_coef=float(g["hp"][5]), target_update_interval_or_tau=float(g["hp"][6]))
     nets = [int(x) for x in g["agent_net"]]
     st = lr.A2CState(torch.tensor(g["actor0"]), torch.tensor(g["critic0"]), torch.tensor(g["target0"]), nets, nets, D, A)
+    S = golden_stride(g)
     for u, step in enumerate(g["steps"]):
         s = {k: torch.as_tensor(g[f"u{u}_{k}"]) for k in ("obs", "act", "rew", "done", "filled")}
         P = s["obs"].shape[0]
@@ -72,12 +74,12 @@ def test_a2c_update_matches_reference_golden(name):
         if u == 0:
             _close(out["returns"].numpy(), g["returns0"])
             for k in ("actor", "critic"):
-                _close_scaled(out["grad_clipped"][k].numpy(), g[f"{k}_grad0_clipped"])
+                _close_scaled(out["grad_clipped"][k].numpy()[::S], g[f"{k}_grad0_clipped"])
     for k in ("actor", "critic"):
-        _close_scaled(st.m[k].numpy(), g[f"{k}_adam_m_final"])
-        _close_scaled(st.v[k].numpy(), g[f"{k}_adam_v_final"], tol=2e-5)
+        _close_scaled(st.m[k].numpy()[::S], g[f"{k}_adam_m_final"])
+        _close_scaled(st.v[k].numpy()[::S], g[f"{k}_adam_v_final"], tol=2e-5)
     for mine, want in ((st.actor, "actor_final"), (st.critic, "critic_final"), (st.target, "target_final")):
-        d = np.abs(mine.numpy() - g[want])
+        d = np.abs(mine.numpy()[::S] - g[want])
         assert np.quantile(d, 0.999) < 1e-5 and d.max() < 2 * hp.lr * len(g["steps"]) + 1e-6
 
 
@@ -92,53 +94,61 @@ def test_epsilon_schedule_and_nstep_returns_golden():
         _close(got.numpy(), g[f"ns_ret_{n}"], rtol=1e-6, atol=1e-6)
 
 
-@pytest.mark.refsrc
-def test_replay_ring_matches_live_reference_buffer():
-    """ReplayRef (episode-major) == reference ReplayBuffer (time-major) incl. the stale tail of re-used slots."""
-    from oracle import ref_shim
-
-    ref = ref_shim.load()
+def _replay_episodes(add):
+    """twelve ragged episodes into a five-slot ring (slots are re-used: their stale tails must survive as in the reference)"""
     rng = np.random.default_rng(1)
-    spaces = [ref_shim.Space(shape=(D,)) for _ in range(N)]
-    rb = ref.dqn_train.ReplayBuffer(5, N, spaces, [ref_shim.Space(n=A)] * N, T, "cpu")
-    mine = lr.ReplayRef(5, N, T, D)
     for ep in range(12):
         L = int(rng.integers(2, T + 1))
-        o = [rng.standard_normal(D).astype(np.float32) for _ in range(N)]
-        rb.init_episode(o); mine.init_episode(o)
+        add(None, [rng.standard_normal(D).astype(np.float32) for _ in range(N)])
         for t in range(L):
             o = [rng.standard_normal(D).astype(np.float32) for _ in range(N)]
-            a, r, d = rng.integers(0, A, N), rng.random(N).astype(np.float32), t == L - 1
-            rb.add(o, a, r, d); mine.add(o, a, r, d)
-    assert len(rb) == len(mine) and rb.cur_pos == mine.cur
-    for i in range(N):
-        assert np.array_equal(rb.observations[i].transpose(1, 0, 2), mine.store["obs"][:, i])
-    assert np.array_equal(rb.actions.transpose(2, 0, 1), mine.store["act"])
-    assert np.array_equal(rb.rewards.transpose(2, 0, 1), mine.store["rew"])
-    assert np.array_equal(rb.dones.T, mine.store["done"].astype(bool)) and np.array_equal(rb.filled.T, mine.store["filled"].astype(bool))
+            add((rng.integers(0, A, N), rng.random(N).astype(np.float32), t == L - 1), o)
 
 
-@pytest.mark.refsrc
-def test_live_reference_update_on_fresh_seed():
-    """Not only the committed vectors: a fresh random case against the live classes."""
-    from oracle import ref_shim
+def test_replay_ring_matches_live_reference_buffer():
+    """ReplayRef (episode-major) == the reference's ReplayBuffer (time-major; recorded from the live class, stored transposed) incl. the stale tail of re-used slots."""
+    g = reference_outputs("replay_reference")
+    mine = lr.ReplayRef(5, N, T, D)
+    _replay_episodes(lambda ard, o: mine.init_episode(o) if ard is None else mine.add(o, *ard))
+    assert len(mine) == int(g["len"]) and mine.cur == int(g["cur_pos"])
+    for k in ("obs", "act", "rew"):
+        assert np.array_equal(g[k], mine.store[k]), k
+    assert np.array_equal(g["done"], mine.store["done"].astype(bool)) and np.array_equal(g["filled"], mine.store["filled"].astype(bool))
 
-    ref = ref_shim.load()
-    torch.manual_seed(123)
-    model = ref.dqn_model.QNetwork([ref_shim.Space(shape=(D,))] * N, [ref_shim.Space(n=A)] * N, ref_shim.dqn_cfg(), [128, 128], False, False, True, "cpu")
-    theta = lr.flat_from_state_dict(model.state_dict(), "critic.independent", N)
-    st = lr.DqnState(theta.clone(), theta.clone(), [0, 1], D, A)
+
+def _fresh_batches():
     rng = np.random.default_rng(4)
     for _ in range(2):
         B = 16
-        b = dict(obss=torch.tensor(rng.standard_normal((N, T + 1, B, D)), dtype=torch.float32), actions=torch.tensor(rng.integers(0, A, (N, T, B))),
-                 rewards=torch.tensor(rng.random((N, T, B)), dtype=torch.float32), dones=torch.tensor(rng.random((T + 1, B)) < 0.05, dtype=torch.float32),
-                 filled=torch.tensor(rng.random((T, B)) < 0.9, dtype=torch.float32))
-        want = model.update(ref.dqn_train.Batch(b["obss"], b["actions"], b["rewards"], b["dones"], b["filled"], None))["loss"]
-        got = lr.dqn_update(st, b, lr.DqnHP())
-        _close(got["loss"], want)
-    d = np.abs(st.theta.numpy() - lr.flat_from_state_dict(model.state_dict(), "critic.independent", N).numpy())
-    assert np.quantile(d, 0.999) < 1e-5
+        yield dict(obss=torch.tensor(rng.standard_normal((N, T + 1, B, D)), dtype=torch.float32), actions=torch.tensor(rng.integers(0, A, (N, T, B))),
+                   rewards=torch.tensor(rng.random((N, T, B)), dtype=torch.float32), dones=torch.tensor(rng.random((T + 1, B)) < 0.05, dtype=torch.float32),
+                   filled=torch.tensor(rng.random((T, B)) < 0.9, dtype=torch.float32))
+
+
+def test_live_reference_update_on_fresh_seed():
+    """Not only the trajectory-store fixtures: time-major batches drawn directly (standard-normal observations), two updates of the reference's
+    QNetwork from the same seeded weights (recorded from the live class)."""
+    g = reference_outputs("qnet_reference")
+    theta = seeded_params(lr, N, D, A, 123)
+    st = lr.DqnState(theta.clone(), theta.clone(), [0, 1], D, A)
+    for u, b in enumerate(_fresh_batches()):
+        _close(lr.dqn_update(st, b, lr.DqnHP())["loss"], g["losses"][u])
+    assert np.quantile(np.abs(st.theta.numpy()[::STRIDE] - g["theta"]), 0.999) < 1e-5
+
+
+def make_reference_outputs(ref, ref_shim):
+    """tests/golden/replay_reference.npz and qnet_reference.npz: the reference's ReplayBuffer and QNetwork on the inputs of the two tests above."""
+    spaces = [ref_shim.Space(shape=(D,)) for _ in range(N)]
+    rb = ref.dqn_train.ReplayBuffer(5, N, spaces, [ref_shim.Space(n=A)] * N, T, "cpu")
+    _replay_episodes(lambda ard, o: rb.init_episode(o) if ard is None else rb.add(o, *ard))
+    np.savez_compressed(os.path.join(GOLD, "replay_reference.npz"), len=len(rb), cur_pos=rb.cur_pos,
+                        obs=np.stack([rb.observations[i].transpose(1, 0, 2) for i in range(N)], 1), act=rb.actions.transpose(2, 0, 1),
+                        rew=rb.rewards.transpose(2, 0, 1), done=rb.dones.T, filled=rb.filled.T)
+    model = ref.dqn_model.QNetwork(spaces, [ref_shim.Space(n=A)] * N, ref_shim.dqn_cfg(), [128, 128], False, False, True, "cpu")
+    load_params(model, lr, ("critic.independent", "target.independent"), seeded_params(lr, N, D, A, 123), N, D, A)
+    losses = [model.update(ref.dqn_train.Batch(b["obss"], b["actions"], b["rewards"], b["dones"], b["filled"], None))["loss"] for b in _fresh_batches()]
+    np.savez_compressed(os.path.join(GOLD, "qnet_reference.npz"), losses=np.array(losses, np.float64),
+                        theta=lr.flat_from_state_dict(model.state_dict(), "critic.independent", N).numpy()[::STRIDE])
 
 
 @pytest.mark.parametrize("alg", ["ia2c", "mappo"])

@@ -1,5 +1,6 @@
-"""IPPO (marlbase/ac/model.py PPONetwork, 249-352): the oracle restatement against the LIVE reference class (build container only, `refsrc`),
-and the B200 path (marl_ppo_update through ac.model.PPONetwork) against the oracle on random on-policy batches; driver test."""
+"""IPPO (marlbase/ac/model.py PPONetwork, 249-352): the oracle restatement against outputs of the reference classes stored under tests/golden,
+and the CUDA path (marl_ppo_update through ac.model.PPONetwork) against the oracle on random on-policy batches; driver test."""
+import os
 import types
 
 import numpy as np
@@ -7,6 +8,7 @@ import pytest
 import torch
 
 from oracle import learner_ref as lr
+from tests.helpers import GOLDEN, STRIDE, load_params, reference_outputs, seeded_params
 
 N, D, A, T = 2, 15, 6, 25
 
@@ -39,93 +41,99 @@ def _oracle_batch(s):
                 rewards=t["rew"].permute(2, 0, 1).float(), dones=t["done"].permute(1, 0).float(), filled=t["filled"].permute(1, 0).float())
 
 
-@pytest.mark.refsrc
+METRICS = ("loss", "actor_loss", "value_loss", "entropy")
+# (fixture key, class, seed, batch seed, envs P, steps, epochs, grad_clip, parameter sharing, centralised critic, standardise_returns)
+REF_CASES = {
+    "std_a2c": ("A2CNetwork", 9, 3, 10, (0, 2, 3), 3, False, False, False, True),
+    "std_ppo": ("PPONetwork", 9, 3, 10, (0, 2, 3), 3, False, False, False, True),
+    "cent_a2c": ("A2CNetwork", 4, 5, 10, (0, 2, 3), 3, False, False, True, False),
+    "cent_ppo": ("PPONetwork", 4, 5, 10, (0, 2, 3), 3, False, False, True, False),
+    "ppo_indep": ("PPONetwork", 5, 11, 12, (0, 2, 5), 4, False, False, False, False),
+    "ppo_shared_clip": ("PPONetwork", 5, 11, 12, (0, 2, 5), 4, 0.5, True, False, False),
+}
+
+
+def _ref_state(key):
+    """The oracle state a case starts from: seeded weights (actor, critic; the target critic is a copy of the critic)."""
+    cls, seed, _, _, _, _, clip, sharing, centralised, std = REF_CASES[key]
+    n_nets, nets = (1, [0, 0]) if sharing else (N, [0, 1])
+    actor, critic = seeded_params(lr, n_nets, D, A, seed), seeded_params(lr, n_nets, N * D if centralised else D, 1, seed + 1)
+    return lr.A2CState(actor, critic.clone(), critic.clone(), nets, nets, D, A, centralised=centralised, ret_ms=lr.RunningMeanStdRef((N,)) if std else None)
+
+
+def _run_oracle(key):
+    cls, _, bseed, P, steps, epochs, clip, _, _, _ = REF_CASES[key]
+    st = _ref_state(key)
+    hp = lr.A2CHP(grad_clip=float(clip or 0.0), target_update_interval_or_tau=2)
+    rng = np.random.default_rng(bseed)
+    metrics = []
+    for step in steps:
+        b = _oracle_batch(_batch_arrays(rng, P, N))
+        got = lr.ppo_update(st, b, hp, step, epochs, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, b, hp, step)
+        metrics.append([got[k] for k in METRICS])
+    return st, metrics
+
+
+def _check_reference_case(key):
+    """oracle.learner_ref from the case's seeded weights and batches vs what the reference's A2CNetwork / PPONetwork computed for them (recorded
+    from the live classes under tests/golden): losses, running return statistics, actor / critic / target parameters"""
+    g = reference_outputs("ac_reference")
+    st, metrics = _run_oracle(key)
+    _close(metrics, g[f"{key}_metrics"])
+    if REF_CASES[key][-1]:
+        _close(st.ret_ms.mean.numpy(), g[f"{key}_ret_mean"]); _close(st.ret_ms.var.numpy(), g[f"{key}_ret_var"])
+        assert abs(st.ret_ms.count - float(g[f"{key}_ret_count"])) < 1e-9
+    for mine, name in ((st.actor, "actor"), (st.critic, "critic"), (st.target, "target")):
+        d = np.abs(mine.numpy()[::STRIDE] - g[f"{key}_{name}"])
+        assert np.quantile(d, 0.999) < 1e-5, (name, d.max())
+
+
 @pytest.mark.parametrize("cls", ["A2CNetwork", "PPONetwork"])
 def test_oracle_standardise_returns_matches_live_reference(cls):
-    """cfg.standardise_returns=True: RunningMeanStd over the n-step returns (ac/model.py:195-204, 272-281) -- oracle vs the live classes"""
-    from collections import namedtuple
-
-    from oracle import ref_shim
-
-    ref = ref_shim.load()
-    torch.manual_seed(9)
-    cfg = ref_shim.a2c_cfg(standardise_returns=True, num_epochs=3, ppo_clip=0.2, target_update_interval_or_tau=2)
-    net = ref_shim.net_cfg()
-    model = getattr(ref.ac_model, cls)([ref_shim.Space(shape=(D,))] * N, [ref_shim.Space(n=A)] * N, cfg, net, net, "cpu")
-    sd = model.state_dict()
-    st = lr.A2CState(lr.flat_from_state_dict(sd, "actor.independent", N), lr.flat_from_state_dict(sd, "critic.independent", N),
-                     lr.flat_from_state_dict(sd, "target_critic.independent", N), [0, 1], [0, 1], D, A, ret_ms=lr.RunningMeanStdRef((N,)))
-    hp = lr.A2CHP(target_update_interval_or_tau=2)
-    Batch = namedtuple("Batch", ["obss", "actions", "rewards", "dones", "filled", "action_masks"])
-    rng = np.random.default_rng(3)
-    for step in (0, 2, 3):
-        b = _oracle_batch(_batch_arrays(rng, 10, N))
-        want = model.update(Batch(b["obss"], b["actions"], b["rewards"], b["dones"].bool(), b["filled"], None), step)
-        got = lr.ppo_update(st, b, hp, step, 3, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, b, hp, step)
-        _close([got[k] for k in ("loss", "actor_loss", "value_loss", "entropy")], [want[k] for k in ("loss", "actor_loss", "value_loss", "entropy")])
-    _close(st.ret_ms.mean.numpy(), model.ret_ms.mean.numpy()); _close(st.ret_ms.var.numpy(), model.ret_ms.var.numpy())
-    assert abs(st.ret_ms.count - model.ret_ms.count) < 1e-9
-    d = np.abs(st.actor.numpy() - lr.flat_from_state_dict(model.state_dict(), "actor.independent", N).numpy())
-    assert np.quantile(d, 0.999) < 1e-5
+    """cfg.standardise_returns=True: RunningMeanStd over the n-step returns (ac/model.py:195-204, 272-281)"""
+    _check_reference_case("std_a2c" if cls == "A2CNetwork" else "std_ppo")
 
 
-@pytest.mark.refsrc
 @pytest.mark.parametrize("cls", ["A2CNetwork", "PPONetwork"])
 def test_oracle_centralised_critic_matches_live_reference(cls):
-    """critic.centralised=True (MAA2C / MAPPO, ac/model.py:62-65,156-157): oracle vs the live classes"""
-    from collections import namedtuple
-
-    from oracle import ref_shim
-
-    ref = ref_shim.load()
-    torch.manual_seed(4)
-    cfg = ref_shim.a2c_cfg(num_epochs=3, ppo_clip=0.2, target_update_interval_or_tau=2)
-    model = getattr(ref.ac_model, cls)([ref_shim.Space(shape=(D,))] * N, [ref_shim.Space(n=A)] * N, cfg, ref_shim.net_cfg(), ref_shim.net_cfg(centralised=True), "cpu")
-    sd = model.state_dict()
-    assert sd["critic.independent.0.network.0.weight"].shape == (128, N * D)
-    st = lr.A2CState(lr.flat_from_state_dict(sd, "actor.independent", N), lr.flat_from_state_dict(sd, "critic.independent", N),
-                     lr.flat_from_state_dict(sd, "target_critic.independent", N), [0, 1], [0, 1], D, A, centralised=True)
-    hp = lr.A2CHP(target_update_interval_or_tau=2)
-    Batch = namedtuple("Batch", ["obss", "actions", "rewards", "dones", "filled", "action_masks"])
-    rng = np.random.default_rng(5)
-    for step in (0, 2, 3):
-        b = _oracle_batch(_batch_arrays(rng, 10, N))
-        want = model.update(Batch(b["obss"], b["actions"], b["rewards"], b["dones"].bool(), b["filled"], None), step)
-        got = lr.ppo_update(st, b, hp, step, 3, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, b, hp, step)
-        _close([got[k] for k in ("loss", "actor_loss", "value_loss", "entropy")], [want[k] for k in ("loss", "actor_loss", "value_loss", "entropy")])
-    d = np.abs(st.critic.numpy() - lr.flat_from_state_dict(model.state_dict(), "critic.independent", N).numpy())
-    assert np.quantile(d, 0.999) < 1e-5
+    """critic.centralised=True (MAA2C / MAPPO, ac/model.py:62-65,156-157)"""
+    _check_reference_case("cent_a2c" if cls == "A2CNetwork" else "cent_ppo")
 
 
-@pytest.mark.refsrc
 @pytest.mark.parametrize("sharing,clip", [(False, False), (True, 0.5)])
 def test_oracle_ppo_matches_live_reference(sharing, clip):
-    """three PPO updates (4 epochs each) of the reference's PPONetwork vs oracle.learner_ref.ppo_update from the same weights and batches"""
+    """three PPO updates (4 epochs each) of the reference's PPONetwork, without and with parameter sharing and gradient clipping"""
+    _check_reference_case("ppo_shared_clip" if sharing else "ppo_indep")
+
+
+def make_reference_outputs(ref, ref_shim):
+    """tests/golden/ac_reference.npz: the reference's A2CNetwork / PPONetwork run on REF_CASES."""
     from collections import namedtuple
 
-    from oracle import ref_shim
-
-    ref = ref_shim.load()
-    torch.manual_seed(5)
-    cfg = ref_shim.a2c_cfg(grad_clip=clip, num_epochs=4, ppo_clip=0.2, target_update_interval_or_tau=2)
-    net = ref_shim.net_cfg(parameter_sharing=sharing)
-    model = ref.ac_model.PPONetwork([ref_shim.Space(shape=(D,))] * N, [ref_shim.Space(n=A)] * N, cfg, net, net, "cpu")
-    kind, n_nets, nets = ("networks", 1, [0, 0]) if sharing else ("independent", N, [0, 1])
-    sd = model.state_dict()
-    st = lr.A2CState(lr.flat_from_state_dict(sd, f"actor.{kind}", n_nets), lr.flat_from_state_dict(sd, f"critic.{kind}", n_nets),
-                     lr.flat_from_state_dict(sd, f"target_critic.{kind}", n_nets), nets, nets, D, A)
-    hp = lr.A2CHP(grad_clip=float(clip or 0.0), target_update_interval_or_tau=2)
     Batch = namedtuple("Batch", ["obss", "actions", "rewards", "dones", "filled", "action_masks"])
-    rng = np.random.default_rng(11)
-    for step in (0, 2, 5):
-        b = _oracle_batch(_batch_arrays(rng, 12, N))
-        want = model.update(Batch(b["obss"], b["actions"], b["rewards"], b["dones"].bool(), b["filled"], None), step)
-        got = lr.ppo_update(st, b, hp, step, 4, 0.2)
-        _close([got[k] for k in ("loss", "actor_loss", "value_loss", "entropy")], [want[k] for k in ("loss", "actor_loss", "value_loss", "entropy")])
-    sd = model.state_dict()
-    for mine, prefix in ((st.actor, f"actor.{kind}"), (st.critic, f"critic.{kind}"), (st.target, f"target_critic.{kind}")):
-        d = np.abs(mine.numpy() - lr.flat_from_state_dict(sd, prefix, n_nets).numpy())
-        assert np.quantile(d, 0.999) < 1e-5, (prefix, d.max())
+    out = {}
+    for key, (cls, _, bseed, P, steps, epochs, clip, sharing, centralised, std) in REF_CASES.items():
+        st = _ref_state(key)
+        cfg = ref_shim.a2c_cfg(grad_clip=clip, num_epochs=epochs, ppo_clip=0.2, target_update_interval_or_tau=2, standardise_returns=std)
+        model = getattr(ref.ac_model, cls)([ref_shim.Space(shape=(D,))] * N, [ref_shim.Space(n=A)] * N, cfg, ref_shim.net_cfg(parameter_sharing=sharing),
+                                           ref_shim.net_cfg(parameter_sharing=sharing, centralised=centralised), "cpu")
+        kind, n_nets = ("networks", 1) if sharing else ("independent", N)
+        load_params(model, lr, (f"actor.{kind}",), st.actor, n_nets, D, A)
+        load_params(model, lr, (f"critic.{kind}", f"target_critic.{kind}"), st.critic, n_nets, N * D if centralised else D, 1)
+        rng = np.random.default_rng(bseed)
+        metrics = []
+        for step in steps:
+            b = _oracle_batch(_batch_arrays(rng, P, N))
+            want = model.update(Batch(b["obss"], b["actions"], b["rewards"], b["dones"].bool(), b["filled"], None), step)
+            metrics.append([float(want[k]) for k in METRICS])
+        out[f"{key}_metrics"] = np.array(metrics, np.float64)
+        if std:
+            out[f"{key}_ret_mean"], out[f"{key}_ret_var"] = model.ret_ms.mean.numpy(), model.ret_ms.var.numpy()
+            out[f"{key}_ret_count"] = np.float64(model.ret_ms.count)
+        sd = model.state_dict()
+        for name, prefix in (("actor", f"actor.{kind}"), ("critic", f"critic.{kind}"), ("target", f"target_critic.{kind}")):
+            out[f"{key}_{name}"] = lr.flat_from_state_dict(sd, prefix, n_nets).numpy()[::STRIDE]
+    np.savez_compressed(os.path.join(GOLDEN, "ac_reference.npz"), **out)
 
 
 def test_oracle_ppo_first_epoch_is_a2c_with_unit_ratio():

@@ -1,5 +1,5 @@
-"""QMIX (marlbase/dqn/model.py:272-443): the oracle restatement against the live reference and a committed golden vector (CPU), the CUDA mixer
-against the oracle (GPU)."""
+"""QMIX (marlbase/dqn/model.py:272-443): the oracle restatement against outputs of the reference project stored under tests/golden (CPU), the
+CUDA mixer against the oracle (GPU)."""
 import os
 
 import numpy as np
@@ -8,10 +8,11 @@ import torch
 
 from oracle import learner_ref as lr
 from oracle import qmix_ref as qr
-from tests.helpers import NearTie, redraw_on_near_tie
+from tests.helpers import STRIDE, NearTie, load_params, redraw_on_near_tie, reference_outputs, seeded_params
 
 N, T, D, A = 2, 6, 9, 6
-GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "qmix_indep.npz")
+GOLDEN_DIR = os.path.join(os.path.dirname(__file__), "golden")
+GOLDEN = os.path.join(GOLDEN_DIR, "qmix_indep.npz")
 
 
 def _batch(rng, B, n=N, t=T, d=D):
@@ -35,32 +36,64 @@ def _state_from(model, sharing=False):
     return qr.QmixState(theta.clone(), theta.clone(), mix.clone(), mix.clone(), [0] * N if sharing else list(range(N)), D, A)
 
 
-@pytest.mark.refsrc
-@pytest.mark.parametrize("tu,sharing", [(2.0, False), (0.05, False), (2.0, True)])
-def test_oracle_matches_live_reference(tu, sharing):
-    from oracle import ref_shim
+CASES = [(2.0, False), (0.05, False), (2.0, True)]
 
-    ref = ref_shim.load()
+
+def _case(tu, sharing):
+    return f"tu{tu:g}_{'shared' if sharing else 'indep'}"
+
+
+def _seeded_state(sharing):
+    n_nets = 1 if sharing else N
+    theta = seeded_params(lr, n_nets, D, A, 11)
     torch.manual_seed(11)
-    model = _ref_model(ref, ref_shim, tu, sharing)
-    st = _state_from(model, sharing)
-    kind, n_nets = ("networks", 1) if sharing else ("independent", N)
+    mix = qr.init_mixer_flat(N, N * D, 64, 32)
+    return qr.QmixState(theta.clone(), theta.clone(), mix.clone(), mix.clone(), [0] * N if sharing else list(range(N)), D, A)
+
+
+@pytest.mark.parametrize("tu,sharing", CASES)
+def test_oracle_matches_live_reference(tu, sharing):
+    """three updates of the reference's QMixNetwork (hard and Polyak target updates, shared agent networks too) from the same weights and
+    batches, as the live classes computed them (recorded under tests/golden): loss and all four parameter sets"""
+    g, c = reference_outputs("qmix_reference"), _case(tu, sharing)
+    st = _seeded_state(sharing)
     assert st.mix.numel() == qr.mixer_size(N, N * D, 64, 32)
     rng = np.random.default_rng(5)
     hp = lr.DqnHP(target_update_interval_or_tau=tu)
-    for _ in range(3):
-        b = _batch(rng, 16)
-        want = model.update(ref.dqn_train.Batch(b["obss"], b["actions"], b["rewards"], b["dones"], b["filled"], None))["loss"]
-        got = qr.qmix_update(st, b, hp)
+    for u in range(3):
+        got = qr.qmix_update(st, _batch(rng, 16), hp)
+        want = float(g[f"{c}_loss"][u])
         assert abs(got["loss"] - want) <= 1e-5 * max(1.0, abs(want))
-    sd = model.state_dict()
-    for mine, theirs in ((st.theta, lr.flat_from_state_dict(sd, f"critic.{kind}", n_nets)), (st.theta_tgt, lr.flat_from_state_dict(sd, f"target.{kind}", n_nets)),
-                         (st.mix, qr.mixer_flat_from_state_dict(sd, "mixer")), (st.mix_tgt, qr.mixer_flat_from_state_dict(sd, "target_mixer"))):
-        assert np.quantile(np.abs(mine.numpy() - theirs.numpy()), 0.999) < 1e-5
+    for mine, key in ((st.theta, "theta"), (st.theta_tgt, "theta_tgt"), (st.mix, "mix"), (st.mix_tgt, "mix_tgt")):
+        assert np.quantile(np.abs(mine.numpy()[::STRIDE] - g[f"{c}_{key}"]), 0.999) < 1e-5, key
+
+
+def make_reference_outputs(ref, ref_shim):
+    """tests/golden/qmix_reference.npz: the reference's QMixNetwork run on the cases of test_oracle_matches_live_reference."""
+    out = {}
+    for tu, sharing in CASES:
+        st, c = _seeded_state(sharing), _case(tu, sharing)
+        kind, n_nets = ("networks", 1) if sharing else ("independent", N)
+        model = _ref_model(ref, ref_shim, tu, sharing)
+        load_params(model, lr, (f"critic.{kind}", f"target.{kind}"), st.theta, n_nets, D, A)
+        msd = {**qr.mixer_state_dict_from_flat(st.mix, "mixer", N, N * D, 64, 32), **qr.mixer_state_dict_from_flat(st.mix, "target_mixer", N, N * D, 64, 32)}
+        model.load_state_dict(msd, strict=False)
+        rng = np.random.default_rng(5)
+        losses = []
+        for _ in range(3):
+            b = _batch(rng, 16)
+            losses.append(model.update(ref.dqn_train.Batch(b["obss"], b["actions"], b["rewards"], b["dones"], b["filled"], None))["loss"])
+        sd = model.state_dict()
+        out[f"{c}_loss"] = np.array(losses, np.float64)
+        out[f"{c}_theta"] = lr.flat_from_state_dict(sd, f"critic.{kind}", n_nets).numpy()[::STRIDE]
+        out[f"{c}_theta_tgt"] = lr.flat_from_state_dict(sd, f"target.{kind}", n_nets).numpy()[::STRIDE]
+        out[f"{c}_mix"] = qr.mixer_flat_from_state_dict(sd, "mixer").numpy()[::STRIDE]
+        out[f"{c}_mix_tgt"] = qr.mixer_flat_from_state_dict(sd, "target_mixer").numpy()[::STRIDE]
+    np.savez_compressed(os.path.join(GOLDEN_DIR, "qmix_reference.npz"), **out)
 
 
 def make_golden():
-    """Regenerates tests/golden/qmix_indep.npz from the live reference (build container): python -c 'import tests.test_qmix as t; t.make_golden()'"""
+    """Regenerates tests/golden/qmix_indep.npz from the reference project (tests/golden/make_golden.py)"""
     from oracle import ref_shim
 
     ref = ref_shim.load()

@@ -1,4 +1,4 @@
-"""GPU: the three-kernel tcgen05 training pipeline (tc_train.cu, option "tensor_core_backward") against the fused FP32 kernel and
+"""GPU: the three-kernel wgmma training pipeline (tc_train.cu, option "tensor_core_backward") against the fused FP32 kernel and
 the CPU oracle: gradients, loss, parameters after the update -- IDQN and VDN, ragged tiles, obs widths 15 / 27, several T."""
 import ctypes as C
 import types
@@ -30,8 +30,6 @@ def _restore():
     yield
     _opt(b"tensor_core_backward", True)   # the library defaults
     _opt(b"tensor_core_forward", True)
-    _opt(b"tensor_core_pingpong", 2)      # bit mask: forward kernels | dH1 kernel; default: dH1 only
-    _opt(b"tensor_core_onchip", True)
 
 
 def _store(rng, cap, N, T, D, coop):
@@ -77,19 +75,16 @@ def test_tc_backward_matches_ffma_and_oracle(mixer, N, D, T, B, sharing):
     n = m.n_params
     scale = max(1.0, float(np.abs(want["grad"].numpy()).max()))
     grads = {}
-    # 0: fused FP32 kernel; tensor-core passes -- 2 / 3: activations streamed through global memory (tc_train.cu), one tile at a time / two accumulators
-    # everywhere; 1: the default (tc_train3.cu: activations stay on chip; applied below)
-    for tc in (0, 2, 3, 1):
-        _opt(b"tensor_core_backward", int(tc > 0))
-        _opt(b"tensor_core_onchip", int(tc == 1))
-        _opt(b"tensor_core_pingpong", {0: 0, 2: 0, 3: 3, 1: 2}[tc])
+    # 0: fused FP32 kernel; 1: the tensor-core pipeline (the default; applied below)
+    for tc in (0, 1):
+        _opt(b"tensor_core_backward", tc)
         m.update_grads(ts, idx_d)
         torch.cuda.synchronize()
         g = m.grad.cpu().numpy()
         grads[tc] = g[:n] / g[n + 1]
         assert abs(g[n] / g[n + 1] - want["loss"]) <= 1e-5 * max(1.0, abs(want["loss"])), (tc, g[n] / g[n + 1], want["loss"])
         assert_grad_close(lr, st0, batch, hp, grads[tc], want["grad"].numpy(), what=f"kernel selection {tc}:")
-    assert all(np.abs(grads[0] - grads[k]).max() / scale < 1e-5 for k in (1, 2, 3))
+    assert np.abs(grads[0] - grads[1]).max() / scale < 1e-5
     met = m.update_apply().cpu().numpy()  # applies the tensor-core gradients
     d = np.abs(m.theta.cpu().numpy() - st.theta.numpy())
     assert np.quantile(d, 0.999) < 1e-5 and abs(met[0] - want["loss"]) <= 1e-5 * max(1.0, abs(want["loss"]))

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Secondary measurements quoted in DESIGN.md / profiles (not the driver's bench contract):
+"""Secondary measurements quoted in DESIGN.md / profiles (not bench.py's contract):
   * lbf_step_kernel alone against its HBM roofline (322 B per env-step at 8x8-2p-3f, SURVEY §8d) for a sweep of env counts;
   * the fused rollout (forward + eps-greedy + transition + replay write) in env-steps/s;
   * IA2C (BASELINE.json configs[2]: 8192 envs, parameter sharing, n_steps=5) iteration throughput.

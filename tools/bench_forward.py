@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Forward-only pass timing: tcgen05 (3xTF32) vs FP32 FFMA kernels on the row count of one IDQN target pass
+"""Forward-only pass timing: wgmma (3xTF32) vs FP32 FFMA kernels on the row count of one IDQN target pass
 (B=1024 episodes x 26 steps x 2 agents = 53 248 rows).  CUDA events, warm; JSON lines."""
 import ctypes as C
 import json
@@ -34,7 +34,7 @@ def main():
             e1.record(); torch.cuda.synchronize()
             us = e0.elapsed_time(e1) / 50 * 1e3
             flop = E * 2 * 38144
-            print(json.dumps({"rows": 2 * E, "impl": "tcgen05_3xtf32" if tc else "ffma_fp32", "us_per_pass_incl_pack": us, "tflops_fp32_equiv": flop / us / 1e6}))
+            print(json.dumps({"rows": 2 * E, "impl": "wgmma_3xtf32" if tc else "ffma_fp32", "us_per_pass_incl_pack": us, "tflops_fp32_equiv": flop / us / 1e6}))
 
 
 if __name__ == "__main__":

@@ -3,7 +3,7 @@
 
 Runs IDQN on Foraging-8x8-2p-3f-v3 (time_limit 25, batch_size 128, the reference's hyper-parameters, idqn.yaml) for the
 same number of environment steps and the same update : episode ratio with
-  * the B200 path: E vectorised envs, E updates per iteration (codebase_b200.dqn.train pieces), S seeds;
+  * the GPU path: E vectorised envs, E updates per iteration (codebase_b200.dqn.train pieces), S seeds;
   * the CPU restatement of the reference loop (oracle/cpu_loop.py: 1 env, one update per episode), S seeds in parallel
     on the host cores,
 and prints evaluation returns (100 greedy-ish episodes, eps 0.05) at the same checkpoints as one JSON document."""
@@ -106,7 +106,7 @@ if __name__ == "__main__":
     ap.add_argument("--total", type=int, default=TOTAL, help="environment-step budget per seed")
     ap.add_argument("--eval-every", type=int, default=EVAL_EVERY)
     ap.add_argument("--arm", default="both", choices=["both", "cpu", "gpu"],
-                    help="cpu: only the CPU restatement of the reference loop (runs without a GPU); gpu: only the B200 path")
+                    help="cpu: only the CPU restatement of the reference loop (runs without a GPU); gpu: only the GPU path")
     ap.add_argument("--out", default=None, help="also write the JSON document here")
     a = ap.parse_args()
     _set_budget(a.total, a.eval_every)

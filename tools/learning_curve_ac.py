@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Returns curves of the actor-critic family on the CPU reference loop (oracle/cpu_loop_ac.py) next to the GPU runs of the same overlays
-(profiles/r2_learning_sanity/<alg>.csv, written by tools/gpurun/learning_sanity.sh): same env, 64 env instances, yaml defaults, 400 k env steps,
+(the results.csv of `python -m codebase_b200.run +algorithm=<alg> ...`): same env, 64 env instances, yaml defaults, 400 k env steps,
 training-episode returns logged every 51 200 steps (ac/train.py:184-186 logs the TRAINING episodes' infos).
 
-    python tools/learning_curve_ac.py --seeds 3 --out profiles/r2_learning_curve_ac_cpu.json     (CPU only, ~1 min per run)"""
+    python tools/learning_curve_ac.py --seeds 3 --out curve_ac_cpu.json     (CPU only, ~1 min per run)"""
 import argparse
 import json
 import os

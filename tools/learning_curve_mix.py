@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""VDN / QMIX on the CPU reference loop next to the GPU runs of the same overlays (profiles/r2_learning_sanity/{vdn,qmix}.csv): idqn.yaml's
+"""VDN / QMIX on the CPU reference loop next to the GPU runs of the same overlays (results.csv of `python -m codebase_b200.run`): idqn.yaml's
 hyper-parameters (batch_size 32, training_start 2000, epsilon 1.0 -> 0.05 over half of the budget, hard target update every 200 updates),
 CooperativeReward, 400 k env steps, evaluation (100 episodes at eps 0.05) and the last update's loss every 50 k steps.
 
 The CPU arm is oracle/cpu_loop.py's one-env loop (dqn/train.py:298-311: one episode, one update) with oracle/learner_ref.py (VDN) or
-oracle/qmix_ref.py (QMIX) as the learner.  CPU only:  python tools/learning_curve_mix.py --seeds 2 --out profiles/r2_learning_curve_mix_cpu.json"""
+oracle/qmix_ref.py (QMIX) as the learner.  CPU only:  python tools/learning_curve_mix.py --seeds 2 --out curve_mix_cpu.json"""
 import argparse
 import json
 import multiprocessing as mp

@@ -12,7 +12,7 @@ from codebase_b200 import _native as nat   # noqa: E402
 from codebase_b200.lbf import TrajStore   # noqa: E402
 import types   # noqa: E402
 
-NAMES = {0: "tc_forward (target)", 1: "tc_dqn_fwd", 2: "tc_dh1", 5: "tc_dh12", 3: "tc_dw", 4: "reduce_adam", 6: "tc_dqn_fwd3", 7: "tc_dh1w1", 8: "tc_dw2"}
+NAMES = {0: "tc_forward (target)", 1: "tc_dqn_fwd", 2: "tc_dh1", 3: "tc_dw", 4: "reduce_adam"}
 
 
 def main():
