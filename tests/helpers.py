@@ -1,6 +1,7 @@
 """Shared helpers of the parity tests."""
 import functools
 import os
+import types
 
 import numpy as np
 import pytest
@@ -37,6 +38,43 @@ def load_params(model, lr, prefixes, flat, n_nets, in_dim, out_dim):
     assert not missing, sorted(missing)[:4]
     model.load_state_dict(sd, strict=False)
 
+def space(shape=None, n=None):
+    """the two gymnasium space kinds the learners read (.shape of a Box, .n of a Discrete)"""
+    return types.SimpleNamespace(shape=shape, n=n)
+
+
+def random_store(rng, cap, N, T, D, coop, A=6):
+    """A trajectory store of `cap` random episodes in the device layout (numpy arrays): ragged lengths, sparse rewards (`coop`: agent 0's reward
+    for every agent, as CooperativeReward leaves it), most episodes ending in a terminal step."""
+    obs = rng.integers(-1, 12, size=(cap, N, T + 1, D)).astype(np.float32)
+    act = rng.integers(0, A, size=(cap, N, T)).astype(np.int32)
+    rew = (rng.random((cap, N, T)) < 0.2).astype(np.float32) * rng.random((cap, N, T)).astype(np.float32)
+    if coop:
+        rew[:] = rew[:, :1]
+    length = rng.integers(1, T + 1, size=cap)
+    done = np.zeros((cap, T + 1), np.uint8); filled = np.zeros((cap, T), np.uint8)
+    for e in range(cap):
+        filled[e, : length[e]] = 1
+        done[e, length[e]] = rng.random() < 0.8
+    return dict(obs=obs, act=act, rew=rew, done=done, filled=filled)
+
+
+def close_scaled(a, b, tol=1e-5):
+    """element-wise, relative to the tensor's own scale (Adam's second moment lives at 1e-6 .. 1e-10).  For v = (1 - beta2) g^2 pass tol=2e-5:
+    a relative gradient error e shows up as 2e in v, so 2e-5 on v is the 1e-5 bar on g."""
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    scale = max(float(np.abs(b).max()), 1e-30)
+    assert np.abs(a - b).max() <= tol * scale, (float(np.abs(a - b).max()), scale)
+
+
+def clipped(grad, max_norm):
+    """clip_grad_norm_ on the host, from the device's normalised gradient: what the fused Adam step consumes"""
+    if not max_norm:
+        return grad
+    norm = float(np.sqrt((grad.astype(np.float64) ** 2).sum()))
+    return grad * min(1.0, max_norm / (norm + 1e-6))
+
+
 TIE = 2e-5   # relative gap of the two best online Q-values under which the double-Q argmax may legitimately differ between two implementations
 
 
@@ -50,11 +88,12 @@ def check_margin(lr, st, batch, hp):
         raise NearTie()
 
 
-def assert_grad_close(lr, st, batch, hp, got, want, tol=1e-5, what=""):
+def assert_grad_close(lr, st, batch, hp, got, want, tol=1e-5, what="", kink_risk=None):
     """max |got - want| <= tol x max(1, max |want|).  A mismatch that a single ReLU unit sitting on its kink explains is a NearTie, not a failure: a
     hidden pre-activation within ~1e-6 of zero may be "on" in one implementation and "off" in the other (they agree to ~5e-7), which moves the
     gradient by up to dL/dh x (the unit's input row) = oracle.learner_ref.dqn_kink_risk -- e.g. 1.3e-3 for VDN at batch 16, T = 127, where the
-    defect-free kernels of two consecutive builds "failed" this way.  The excuse only covers mismatches up to twice that bound."""
+    defect-free kernels of two consecutive builds "failed" this way.  The excuse only covers mismatches up to twice that bound.
+    kink_risk: () -> that bound, for learners other than IDQN / VDN (QMIX: oracle.qmix_ref.qmix_kink_risk)."""
     import numpy as np
 
     got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
@@ -62,7 +101,7 @@ def assert_grad_close(lr, st, batch, hp, got, want, tol=1e-5, what=""):
     err = float(np.abs(got - want).max())
     if err <= tol * scale:
         return
-    risk = lr.dqn_kink_risk(st, batch, hp)
+    risk = kink_risk() if kink_risk is not None else lr.dqn_kink_risk(st, batch, hp)
     if risk >= 0.5 * err:
         raise NearTie()
     raise AssertionError(f"{what} max abs error {err:.3e} > {tol:g} x {scale:.3g} (largest ReLU-kink move of this case: {risk:.3e})")
@@ -79,6 +118,7 @@ def redraw_on_near_tie(fn):
             try:
                 return fn(*args, **kwargs)
             except NearTie:
+                print(f"near-tie: {fn.__name__}{kwargs or args} re-drawn after initialisation {attempt}")   # shown by pytest -rP / -s
                 continue
         pytest.fail("five initialisations in a row hit a double-Q near-tie: not plausible")
 

@@ -10,7 +10,7 @@ import torch
 
 from oracle import learner_ref as lr
 from oracle import policy_ref
-from tests.helpers import NearTie, assert_grad_close, golden_stride
+from tests.helpers import NearTie, assert_grad_close, clipped as _clipped, close_scaled as _close_scaled, golden_stride, space as _space
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -20,26 +20,6 @@ N, D, A, T = 2, 15, 6, 25
 def _close(a, b, rtol=1e-5, atol=1e-5):
     a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
     assert np.allclose(a, b, rtol=rtol, atol=atol), float(np.abs(a - b).max())
-
-
-def _close_scaled(a, b, tol=1e-5):
-    """element-wise, relative to the tensor's own scale (Adam's second moment lives at 1e-6 .. 1e-10).  For v = (1 - beta2) g^2 pass tol=2e-5:
-    a relative gradient error e shows up as 2e in v, so 2e-5 on v is the 1e-5 bar on g."""
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    scale = max(float(np.abs(b).max()), 1e-30)
-    assert np.abs(a - b).max() <= tol * scale, (float(np.abs(a - b).max()), scale)
-
-
-def _clipped(grad, max_norm):
-    """clip_grad_norm_ on the host, from the device's normalised gradient: what the fused Adam step consumes"""
-    if not max_norm:
-        return grad
-    norm = float(np.sqrt((grad.astype(np.float64) ** 2).sum()))
-    return grad * min(1.0, max_norm / (norm + 1e-6))
-
-
-def _space(shape=None, n=None):
-    return types.SimpleNamespace(shape=shape, n=n)
 
 
 def _model(cls_name, sharing, hp, n_agents=N, max_batch=64):

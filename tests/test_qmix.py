@@ -231,7 +231,8 @@ def test_gpu_update_matches_oracle(sharing, double_q, tu, B, n, t):
 
 @pytest.mark.gpu
 def test_gpu_update_n_and_state_dict_round_trip():
-    """update_n (on-device sampling, the driver's path) keeps the mixer training; the state_dict uses the reference's keys."""
+    """A QMIX learner trained through update_n moves its mixer and target mixer, and its state_dict uses the reference's keys and round-trips.
+    (update_n's arithmetic is compared with the single-update loop and the oracle in tests/test_update_chain_gpu.py.)"""
     hp = lr.DqnHP(target_update_interval_or_tau=0.01)
     m = _gpu_model(hp, max_batch=32, t=25)
     rng = np.random.default_rng(9)

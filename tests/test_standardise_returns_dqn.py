@@ -10,6 +10,7 @@ import torch
 
 from oracle import learner_ref as lr
 from tests.helpers import GOLDEN, STRIDE, assert_grad_close, check_margin, load_params, redraw_on_near_tie, reference_outputs, seeded_params
+from tests.helpers import space as _space
 
 N, D, A, T = 2, 15, 6, 25
 
@@ -17,10 +18,6 @@ N, D, A, T = 2, 15, 6, 25
 def _close(a, b, rtol=1e-5, atol=1e-5):
     a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
     assert np.allclose(a, b, rtol=rtol, atol=atol), float(np.abs(a - b).max())
-
-
-def _space(shape=None, n=None):
-    return types.SimpleNamespace(shape=shape, n=n)
 
 
 def _store(rng, cap, coop):
