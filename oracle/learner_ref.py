@@ -373,7 +373,7 @@ def a2c_losses(actor, critic, target, st: A2CState, batch, hp: A2CHP):
     obs = list(torch.split(batch["obss"], D, dim=-1))
     cobs, CD = st.critic_inputs(obs)
     with torch.no_grad():
-        next_value = torch.cat(agents_forward(target, st.critic_net, cobs, CD, 1), dim=-1)                # (T+1,P,N)
+        next_value = raw_next_value = torch.cat(agents_forward(target, st.critic_net, cobs, CD, 1), dim=-1)   # (T+1,P,N)
     if st.ret_ms is not None:                                                                             # ac/model.py:195-196
         next_value = next_value * torch.sqrt(st.ret_ms.var) + st.ret_ms.mean
     done = batch["dones"].float().unsqueeze(-1).repeat(1, 1, N)
@@ -393,20 +393,68 @@ def a2c_losses(actor, critic, target, st: A2CState, batch, hp: A2CHP):
     actor_loss = ((-(logp * adv.detach()).sum(-1) - hp.entropy_coef * entropy) * filled).sum() / filled.sum()
     value_loss = ((returns - values).pow(2).sum(-1) * filled).sum() / filled.sum()
     ent = (entropy * filled).sum() / filled.sum()
-    return actor_loss, value_loss, ent, returns
+    return actor_loss, value_loss, ent, returns, raw_next_value, adv.detach()
 
 
-def ppo_update(st: A2CState, batch, hp: A2CHP, step: int, num_epochs: int = 4, ppo_clip: float = 0.2):
-    """PPONetwork.update (ac/model.py:265-352): returns and the collecting policy's log-probabilities once, then num_epochs steps on the clipped
-    surrogate; target critic after the last epoch; the metrics are the epochs' means.  Returns also the first epoch's raw gradients."""
-    N, D = len(st.actor_net), st.in_dim
+def _concat_loss(st: A2CState, loss_fn):
+    """loss_fn(actor, critic) -> loss, as a function of the concatenated [actor | critic] vector (kink_risk differentiates one vector)"""
+    na = st.actor.numel()
+    return lambda th: loss_fn(th[:na], th[na:])
+
+
+def a2c_kink_risk(st: A2CState, batch, hp: A2CHP):
+    """kink_risk of the A2C loss at the state before the update (the running return statistics are advanced on a copy)"""
+    def loss(actor, critic):
+        s = copy.copy(st)
+        s.ret_ms = copy.deepcopy(st.ret_ms)
+        actor_loss, value_loss, *_ = a2c_losses(actor, critic, st.target, s, batch, hp)
+        return actor_loss + hp.value_loss_coef * value_loss
+    return kink_risk(_concat_loss(st, loss), torch.cat([st.actor, st.critic]))
+
+
+def ppo_losses(actor, critic, st: A2CState, batch, hp: A2CHP, returns, old_logp, ppo_clip):
+    """one epoch's clipped-surrogate loss (ac/model.py:297-330) -> (loss, actor_loss, value_loss, mean entropy, ratio, adv)"""
+    D = st.in_dim
     obs = list(torch.split(batch["obss"], D, dim=-1))
     obs_t = [o[:-1] for o in obs]
     acts, filled = batch["actions"], batch["filled"]
     cobs, CD = st.critic_inputs(obs)
     cobs_t = [o[:-1] for o in cobs]
+    values = torch.cat(agents_forward(critic, st.critic_net, cobs_t, CD, 1), dim=-1)
+    logp_all = [F.log_softmax(l, dim=-1) for l in agents_forward(actor, st.actor_net, obs_t, D, st.n_actions)]
+    logp = torch.cat([lp.gather(-1, acts[..., i:i + 1]) for i, lp in enumerate(logp_all)], dim=-1)
+    entropy = torch.stack([-(lp.exp() * lp).sum(-1) for lp in logp_all], dim=-1).sum(-1)
+    adv = returns - values
+    value_loss = adv.pow(2).sum(-1)
+    ratio = torch.exp(logp - old_logp)
+    surr1, surr2 = ratio * adv.detach(), torch.clamp(ratio, 1.0 - ppo_clip, 1.0 + ppo_clip) * adv.detach()
+    actor_loss = -torch.min(surr1, surr2).sum(-1) - hp.entropy_coef * entropy
+    actor_loss = (actor_loss * filled).sum() / filled.sum()
+    value_loss = (value_loss * filled).sum() / filled.sum()
+    loss = actor_loss + hp.value_loss_coef * value_loss
+    return loss, actor_loss, value_loss, (entropy * filled).sum() / filled.sum(), ratio.detach(), adv.detach()
+
+
+def ppo_kink_risk(st: A2CState, batch, hp: A2CHP, res, ppo_clip, epoch=-1):
+    """kink_risk of one epoch's PPO loss, at the parameters that epoch started from (res: what ppo_update returned for the batch)"""
+    actor, critic = res["epoch_start"][epoch]
+    return kink_risk(_concat_loss(st, lambda a, c: ppo_losses(a, c, st, batch, hp, res["returns"], res["old_logp"], ppo_clip)[0]),
+                     torch.cat([actor, critic]))
+
+
+def ppo_update(st: A2CState, batch, hp: A2CHP, step: int, num_epochs: int = 4, ppo_clip: float = 0.2):
+    """PPONetwork.update (ac/model.py:265-352): returns and the collecting policy's log-probabilities once, then num_epochs steps on the clipped
+    surrogate; target critic after the last epoch; the metrics are the epochs' means.  Returns also, per epoch: the raw gradients (`grads`;
+    `grad` is the first epoch's), the clipped ones, their norms, the parameters the epoch started from, the fraction of filled entries whose
+    gradient the clip blocks (ratio outside the range and the clamped term the minimum) and `clip_margin`, the smallest |ratio - (1 -+ clip)|
+    over filled entries with a non-zero advantage (the surrogate's gradient jumps there)."""
+    N, D = len(st.actor_net), st.in_dim
+    obs = list(torch.split(batch["obss"], D, dim=-1))
+    obs_t = [o[:-1] for o in obs]
+    acts, filled = batch["actions"], batch["filled"]
+    cobs, CD = st.critic_inputs(obs)
     with torch.no_grad():
-        next_value = torch.cat(agents_forward(st.target, st.critic_net, cobs, CD, 1), dim=-1)
+        next_value = raw_next_value = torch.cat(agents_forward(st.target, st.critic_net, cobs, CD, 1), dim=-1)
         if st.ret_ms is not None:                                                                         # ac/model.py:272-273
             next_value = next_value * torch.sqrt(st.ret_ms.var) + st.ret_ms.mean
         done = batch["dones"].float().unsqueeze(-1).repeat(1, 1, N)
@@ -417,33 +465,30 @@ def ppo_update(st: A2CState, batch, hp: A2CHP, step: int, num_epochs: int = 4, p
         old = [F.log_softmax(l, dim=-1) for l in agents_forward(st.actor, st.actor_net, obs_t, D, st.n_actions)]
         old_logp = torch.cat([lp.gather(-1, acts[..., i:i + 1]) for i, lp in enumerate(old)], dim=-1)
     out = dict(loss=[], actor_loss=[], value_loss=[], entropy=[])
-    first = None
+    extra = dict(grads=[], grads_clipped=[], grad_norms=[], epoch_start=[], clip_frac=[], clip_margin=[])
+    live = (filled.unsqueeze(-1) > 0).expand_as(old_logp)
     for _ in range(num_epochs):
+        extra["epoch_start"].append((st.actor.clone(), st.critic.clone()))
         actor = st.actor.clone().requires_grad_(True)
         critic = st.critic.clone().requires_grad_(True)
-        values = torch.cat(agents_forward(critic, st.critic_net, cobs_t, CD, 1), dim=-1)
-        logp_all = [F.log_softmax(l, dim=-1) for l in agents_forward(actor, st.actor_net, obs_t, D, st.n_actions)]
-        logp = torch.cat([lp.gather(-1, acts[..., i:i + 1]) for i, lp in enumerate(logp_all)], dim=-1)
-        entropy = torch.stack([-(lp.exp() * lp).sum(-1) for lp in logp_all], dim=-1).sum(-1)
-        adv = returns - values
-        value_loss = adv.pow(2).sum(-1)
-        ratio = torch.exp(logp - old_logp)
-        surr1, surr2 = ratio * adv.detach(), torch.clamp(ratio, 1.0 - ppo_clip, 1.0 + ppo_clip) * adv.detach()
-        actor_loss = -torch.min(surr1, surr2).sum(-1) - hp.entropy_coef * entropy
-        actor_loss = (actor_loss * filled).sum() / filled.sum()
-        value_loss = (value_loss * filled).sum() / filled.sum()
-        loss = actor_loss + hp.value_loss_coef * value_loss
+        loss, actor_loss, value_loss, entropy, ratio, adv = ppo_losses(actor, critic, st, batch, hp, returns, old_logp, ppo_clip)
         g_actor, g_critic = torch.autograd.grad(loss, (actor, critic))
-        if first is None:
-            first = dict(actor=g_actor.clone(), critic=g_critic.clone())
+        extra["grads"].append(dict(actor=g_actor.clone(), critic=g_critic.clone()))
+        extra["grad_norms"].append(float(torch.linalg.vector_norm(torch.cat([g_actor, g_critic]))))
+        outside = (ratio < 1.0 - ppo_clip) | (ratio > 1.0 + ppo_clip)
+        blocked = outside & (torch.clamp(ratio, 1.0 - ppo_clip, 1.0 + ppo_clip) * adv < ratio * adv)
+        extra["clip_frac"].append(float(blocked[live].float().mean()))
+        edge = torch.minimum((ratio - (1.0 - ppo_clip)).abs(), (ratio - (1.0 + ppo_clip)).abs())[live & (adv != 0)]
+        extra["clip_margin"].append(float(edge.min()) if edge.numel() else float("inf"))
         if hp.grad_clip:
             total = torch.linalg.vector_norm(torch.cat([g_actor, g_critic]))
             coef = torch.clamp(hp.grad_clip / (total + 1e-6), max=1.0)
             g_actor, g_critic = g_actor * coef, g_critic * coef
+        extra["grads_clipped"].append(dict(actor=g_actor.clone(), critic=g_critic.clone()))
         st.steps += 1
         adam_step(st.actor, st.m["actor"], st.v["actor"], g_actor, st.steps, hp.lr)
         adam_step(st.critic, st.m["critic"], st.v["critic"], g_critic, st.steps, hp.lr)
-        for k, v in (("loss", loss), ("actor_loss", actor_loss), ("value_loss", value_loss), ("entropy", (entropy * filled).sum() / filled.sum())):
+        for k, v in (("loss", loss), ("actor_loss", actor_loss), ("value_loss", value_loss), ("entropy", entropy)):
             out[k].append(float(v.detach()))
     tu = hp.target_update_interval_or_tau
     if tu > 1.0 and step % tu == 0:
@@ -451,17 +496,20 @@ def ppo_update(st: A2CState, batch, hp: A2CHP, step: int, num_epochs: int = 4, p
     elif tu < 1.0:
         st.target.copy_((1 - tu) * st.target + tu * st.critic)
     res = {k: sum(v) / len(v) for k, v in out.items()}
-    res.update(grad=first, returns=returns, per_epoch=out)
+    res.update(grad=extra["grads"][0], returns=returns, per_epoch=out, next_value=raw_next_value, old_logp=old_logp, **extra)
     return res
 
 
 def a2c_update(st: A2CState, batch, hp: A2CHP, step: int):
+    """A2CNetwork.update: returns the metrics, the raw and clipped gradients and the raw norm, the n-step returns, the advantages and the target
+    critic's values (before the running statistics' rescaling)."""
     actor = st.actor.clone().requires_grad_(True)
     critic = st.critic.clone().requires_grad_(True)
-    actor_loss, value_loss, ent, returns = a2c_losses(actor, critic, st.target, st, batch, hp)
+    actor_loss, value_loss, ent, returns, next_value, adv = a2c_losses(actor, critic, st.target, st, batch, hp)
     loss = actor_loss + hp.value_loss_coef * value_loss
     g_actor, g_critic = torch.autograd.grad(loss, (actor, critic))
     raw = dict(actor=g_actor.clone(), critic=g_critic.clone())
+    norm = float(torch.linalg.vector_norm(torch.cat([g_actor, g_critic])))
     if hp.grad_clip:
         total = torch.linalg.vector_norm(torch.cat([g_actor, g_critic]))
         coef = torch.clamp(hp.grad_clip / (total + 1e-6), max=1.0)
@@ -475,4 +523,4 @@ def a2c_update(st: A2CState, batch, hp: A2CHP, step: int):
     elif tu < 1.0:
         st.target.copy_((1 - tu) * st.target + tu * st.critic)
     return dict(loss=float(loss.detach()), actor_loss=float(actor_loss.detach()), value_loss=float(value_loss.detach()), entropy=float(ent.detach()), grad=raw, returns=returns.detach(),
-                grad_clipped=dict(actor=g_actor.detach().clone(), critic=g_critic.detach().clone()))
+                grad_clipped=dict(actor=g_actor.detach().clone(), critic=g_critic.detach().clone()), grad_norm=norm, advantages=adv, next_value=next_value)

@@ -1,14 +1,13 @@
 """GPU: the fused IA2C learner (marl_a2c_*) against golden vectors produced by the reference's A2CNetwork and against
 the CPU oracle on random on-policy batches.  Tolerance 1e-5 (rtol + atol) on float learner tensors."""
 import os
-import types
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import learner_ref as lr
-from tests.helpers import golden_stride
+from tests.helpers import ac_batch, ac_model, ac_oracle_batch, clipped, close_scaled, golden_stride, traj_store
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
@@ -20,71 +19,26 @@ def _close(a, b, rtol=1e-5, atol=1e-5):
     assert np.allclose(a, b, rtol=rtol, atol=atol), float(np.abs(a - b).max())
 
 
-def _close_scaled(a, b, tol=1e-5):
-    """element-wise, relative to the tensor's own scale (Adam's second moment lives at 1e-6 .. 1e-10).  For v = (1 - beta2) g^2 pass tol=2e-5:
-    a relative gradient error e shows up as 2e in v, so 2e-5 on v is the 1e-5 bar on g."""
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    scale = max(float(np.abs(b).max()), 1e-30)
-    assert np.abs(a - b).max() <= tol * scale, (float(np.abs(a - b).max()), scale)
-
-
-def _clipped(grad, max_norm):
-    if not max_norm:
-        return grad
-    norm = float(np.sqrt((grad.astype(np.float64) ** 2).sum()))
-    return grad * min(1.0, max_norm / (norm + 1e-6))
-
-
-def _space(shape=None, n=None):
-    return types.SimpleNamespace(shape=shape, n=n)
-
-
-def _model(sharing, hp, P, n_agents=N):
-    from codebase_b200.ac.model import A2CNetwork
-
-    cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, n_steps=hp.n_steps, entropy_coef=hp.entropy_coef,
-                                value_loss_coef=hp.value_loss_coef, target_update_interval_or_tau=hp.target_update_interval_or_tau, standardise_returns=False)
-    net = types.SimpleNamespace(layers=[128, 128], parameter_sharing=sharing, use_rnn=False, use_orthogonal_init=True, centralised=False)
-    return A2CNetwork([_space(shape=(D,))] * n_agents, [_space(n=A)] * n_agents, cfg, net, net, "cuda", max_envs=P, max_episode_length=T)
-
-
-def _to_store(s, device):
-    from codebase_b200.lbf import TrajStore
-
-    P, n_agents = s["obs"].shape[0], s["obs"].shape[1]
-    ts = TrajStore(P, n_agents, T, D, device)
-    for k in ("obs", "act", "rew", "done", "filled"):
-        getattr(ts, k).copy_(torch.as_tensor(s[k]))
-    return ts
-
-
-def _oracle_batch(s):
-    t = {k: torch.as_tensor(v) for k, v in s.items()}
-    P, n_agents = t["obs"].shape[0], t["obs"].shape[1]
-    return dict(obss=t["obs"].permute(2, 0, 1, 3).reshape(T + 1, P, n_agents * D).float(), actions=t["act"].permute(2, 0, 1).long(),
-                rewards=t["rew"].permute(2, 0, 1).float(), dones=t["done"].permute(1, 0).float(), filled=t["filled"].permute(1, 0).float())
-
-
 @pytest.mark.parametrize("name", ["ia2c_indep", "ia2c_shared"])
 def test_update_matches_reference_golden(name):
     g = np.load(os.path.join(GOLD, f"{name}.npz"))
     hp = lr.A2CHP(lr=float(g["hp"][0]), gamma=float(g["hp"][1]), grad_clip=float(g["hp"][2]), n_steps=int(g["hp"][3]), entropy_coef=float(g["hp"][4]),
                   value_loss_coef=float(g["hp"][5]), target_update_interval_or_tau=float(g["hp"][6]))
     P = g["u0_obs"].shape[0]
-    m = _model(bool(int(g["n_nets"]) == 1), hp, P)
+    m = ac_model(hp, N, D, P, T, sharing=bool(int(g["n_nets"]) == 1))
     assert m.n_actor == g["actor0"].size and m.n_critic == g["critic0"].size
     m.theta[: m.n_actor].copy_(torch.tensor(g["actor0"])); m.theta[m.n_actor:].copy_(torch.tensor(g["critic0"])); m.theta_tgt.copy_(torch.tensor(g["target0"]))
     for u, step in enumerate(g["steps"]):
         s = {k: g[f"u{u}_{k}"] for k in ("obs", "act", "rew", "done", "filled")}
-        met = m.metrics_dict(m.update_from_store(_to_store(s, m.device), P, int(step)))
+        met = m.metrics_dict(m.update_from_store(traj_store(s, m.device), P, int(step)))
         _close([met["loss"], met["actor_loss"], met["value_loss"], met["entropy"]], g["metrics"][u])
         if u == 0:
             _, ret, _ = m.scratch(P, T)
             _close(ret.permute(2, 1, 0).cpu().numpy(), g["returns0"])
     S = golden_stride(g)
     am, av = m.adam_m.cpu().numpy(), m.adam_v.cpu().numpy()   # element-wise against the reference optimiser's state
-    _close_scaled(am[: m.n_actor][::S], g["actor_adam_m_final"]); _close_scaled(am[m.n_actor:][::S], g["critic_adam_m_final"])
-    _close_scaled(av[: m.n_actor][::S], g["actor_adam_v_final"], tol=2e-5); _close_scaled(av[m.n_actor:][::S], g["critic_adam_v_final"], tol=2e-5)
+    close_scaled(am[: m.n_actor][::S], g["actor_adam_m_final"]); close_scaled(am[m.n_actor:][::S], g["critic_adam_m_final"])
+    close_scaled(av[: m.n_actor][::S], g["actor_adam_v_final"], tol=2e-5); close_scaled(av[m.n_actor:][::S], g["critic_adam_v_final"], tol=2e-5)
     th, tg = m.theta.cpu().numpy(), m.theta_tgt.cpu().numpy()
     for got, want in ((th[: m.n_actor][::S], g["actor_final"]), (th[m.n_actor:][::S], g["critic_final"]), (tg[::S], g["target_final"])):
         d = np.abs(got - want)
@@ -97,30 +51,22 @@ def test_update_matches_oracle_on_random_batches(sharing, P, n_agents, clip):
 
     rng = np.random.default_rng(P)
     hp = lr.A2CHP(grad_clip=clip)
-    m = _model(sharing, hp, P, n_agents)
+    m = ac_model(hp, n_agents, D, P, T, sharing=sharing)
     nets = sharing_to_nets(sharing, n_agents)
     st = lr.A2CState(m.theta[: m.n_actor].cpu().clone(), m.theta[m.n_actor:].cpu().clone(), m.theta_tgt.cpu().clone(), nets, nets, D, A)
     for u, step in enumerate((0, 3 * P, 200)):
-        obs = rng.integers(-1, 8, size=(P, n_agents, T + 1, D)).astype(np.float32)
-        act = rng.integers(0, A, size=(P, n_agents, T)).astype(np.int32)
-        rew = (rng.random((P, n_agents, T)) < 0.2).astype(np.float32) * rng.random((P, n_agents, T)).astype(np.float32)
-        length = rng.integers(1, T + 1, size=P)
-        done = np.zeros((P, T + 1), np.uint8); filled = np.zeros((P, T), np.uint8)
-        for e in range(P):
-            filled[e, : length[e]] = 1
-            done[e, length[e]] = 1
-        s = dict(obs=obs, act=act, rew=rew, done=done, filled=filled)
-        want = lr.a2c_update(st, _oracle_batch(s), hp, step)
-        m.update_grads(_to_store(s, m.device), P)
+        s = ac_batch(rng, P, n_agents, T, D)
+        want = lr.a2c_update(st, ac_oracle_batch(s), hp, step)
+        m.update_grads(traj_store(s, m.device), P)
         gr = m.grad.cpu().numpy()
         n = m.n_actor + m.n_critic
         wg = np.concatenate([want["grad"]["actor"].numpy(), want["grad"]["critic"].numpy()])
         scale = max(1.0, float(np.abs(wg).max()))
         _close(gr[:n] / gr[n + 1] / scale, wg / scale)
-        _close_scaled(_clipped(gr[:n] / gr[n + 1], clip), np.concatenate([want["grad_clipped"]["actor"].numpy(), want["grad_clipped"]["critic"].numpy()]))
+        close_scaled(clipped(gr[:n] / gr[n + 1], clip), np.concatenate([want["grad_clipped"]["actor"].numpy(), want["grad_clipped"]["critic"].numpy()]))
         met = m.metrics_dict(m.update_apply(step))
-        _close_scaled(m.adam_m.cpu().numpy(), np.concatenate([st.m["actor"].numpy(), st.m["critic"].numpy()]))
-        _close_scaled(m.adam_v.cpu().numpy(), np.concatenate([st.v["actor"].numpy(), st.v["critic"].numpy()]), tol=2e-5)
+        close_scaled(m.adam_m.cpu().numpy(), np.concatenate([st.m["actor"].numpy(), st.m["critic"].numpy()]))
+        close_scaled(m.adam_v.cpu().numpy(), np.concatenate([st.v["actor"].numpy(), st.v["critic"].numpy()]), tol=2e-5)
         _close([met["loss"], met["actor_loss"], met["value_loss"], met["entropy"]], [want["loss"], want["actor_loss"], want["value_loss"], want["entropy"]])
         vt, ret, adv = m.scratch(P, T)
         _close(ret.permute(2, 1, 0).cpu().numpy(), want["returns"].numpy())
@@ -137,7 +83,7 @@ def test_forward_passes_and_reference_style_calls():
     rng = np.random.default_rng(1)
     hp = lr.A2CHP()
     P = 300
-    m = _model(False, hp, P)
+    m = ac_model(hp, N, D, P, T)
     obs = rng.integers(-1, 8, size=(P, N, D)).astype(np.float32)
     xs = [torch.tensor(obs[:, i]) for i in range(N)]
     _close(m.logits(torch.tensor(obs, device="cuda")).cpu().numpy(), torch.stack(lr.agents_forward(m.theta[: m.n_actor].cpu(), [0, 1], xs, D, A), 1).numpy())

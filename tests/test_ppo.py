@@ -1,14 +1,14 @@
 """IPPO (marlbase/ac/model.py PPONetwork, 249-352): the oracle restatement against outputs of the reference classes stored under tests/golden,
 and the CUDA path (marl_ppo_update through ac.model.PPONetwork) against the oracle on random on-policy batches; driver test."""
+import copy
 import os
-import types
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import learner_ref as lr
-from tests.helpers import GOLDEN, STRIDE, load_params, reference_outputs, seeded_params
+from tests.helpers import GOLDEN, STRIDE, ac_batch, ac_model, ac_oracle_batch, load_params, reference_outputs, seeded_params, traj_store
 
 N, D, A, T = 2, 15, 6, 25
 
@@ -16,29 +16,6 @@ N, D, A, T = 2, 15, 6, 25
 def _close(a, b, rtol=1e-5, atol=1e-5):
     a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
     assert np.allclose(a, b, rtol=rtol, atol=atol), float(np.abs(a - b).max())
-
-
-def _space(shape=None, n=None):
-    return types.SimpleNamespace(shape=shape, n=n)
-
-
-def _batch_arrays(rng, P, n_agents):
-    obs = rng.integers(-1, 8, size=(P, n_agents, T + 1, D)).astype(np.float32)
-    act = rng.integers(0, A, size=(P, n_agents, T)).astype(np.int32)
-    rew = (rng.random((P, n_agents, T)) < 0.2).astype(np.float32) * rng.random((P, n_agents, T)).astype(np.float32)
-    length = rng.integers(1, T + 1, size=P)
-    done = np.zeros((P, T + 1), np.uint8); filled = np.zeros((P, T), np.uint8)
-    for e in range(P):
-        filled[e, : length[e]] = 1
-        done[e, length[e]] = 1
-    return dict(obs=obs, act=act, rew=rew, done=done, filled=filled)
-
-
-def _oracle_batch(s):
-    t = {k: torch.as_tensor(v) for k, v in s.items()}
-    P, n_agents = t["obs"].shape[0], t["obs"].shape[1]
-    return dict(obss=t["obs"].permute(2, 0, 1, 3).reshape(T + 1, P, n_agents * D).float(), actions=t["act"].permute(2, 0, 1).long(),
-                rewards=t["rew"].permute(2, 0, 1).float(), dones=t["done"].permute(1, 0).float(), filled=t["filled"].permute(1, 0).float())
 
 
 METRICS = ("loss", "actor_loss", "value_loss", "entropy")
@@ -68,7 +45,7 @@ def _run_oracle(key):
     rng = np.random.default_rng(bseed)
     metrics = []
     for step in steps:
-        b = _oracle_batch(_batch_arrays(rng, P, N))
+        b = ac_oracle_batch(ac_batch(rng, P, N, T, D))
         got = lr.ppo_update(st, b, hp, step, epochs, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, b, hp, step)
         metrics.append([got[k] for k in METRICS])
     return st, metrics
@@ -123,7 +100,7 @@ def make_reference_outputs(ref, ref_shim):
         rng = np.random.default_rng(bseed)
         metrics = []
         for step in steps:
-            b = _oracle_batch(_batch_arrays(rng, P, N))
+            b = ac_oracle_batch(ac_batch(rng, P, N, T, D))
             want = model.update(Batch(b["obss"], b["actions"], b["rewards"], b["dones"].bool(), b["filled"], None), step)
             metrics.append([float(want[k]) for k in METRICS])
         out[f"{key}_metrics"] = np.array(metrics, np.float64)
@@ -140,7 +117,7 @@ def test_oracle_ppo_first_epoch_is_a2c_with_unit_ratio():
     """epoch 0: ratio == 1 exactly, inside the clip range -> the surrogate's gradient is the policy gradient of A2C"""
     rng = np.random.default_rng(2)
     theta_a, theta_c = lr.init_flat(N, D, A), lr.init_flat(N, D, 1)
-    b = _oracle_batch(_batch_arrays(rng, 8, N))
+    b = ac_oracle_batch(ac_batch(rng, 8, N, T, D))
     st1 = lr.A2CState(theta_a.clone(), theta_c.clone(), theta_c.clone(), [0, 1], [0, 1], D, A)
     st2 = lr.A2CState(theta_a.clone(), theta_c.clone(), theta_c.clone(), [0, 1], [0, 1], D, A)
     g_ppo = lr.ppo_update(st1, b, lr.A2CHP(), 0, 1, 0.2)["grad"]
@@ -148,15 +125,43 @@ def test_oracle_ppo_first_epoch_is_a2c_with_unit_ratio():
     _close(g_ppo["actor"].numpy(), g_a2c["actor"].numpy()); _close(g_ppo["critic"].numpy(), g_a2c["critic"].numpy())
 
 
-def _model(sharing, hp, P, n_agents, num_epochs, ppo_clip, standardise=False, cls="PPONetwork", centralised=False):
-    from codebase_b200.ac import model as M
+def test_oracle_per_epoch_outputs_and_kink_risk():
+    """ppo_update's per-epoch outputs keep `grad` as the first epoch's raw gradient; a2c_kink_risk is 0 where no hidden unit sits within 2e-6 of
+    its kink, and positive once one unit's bias puts it 1e-7 from its kink on one row"""
+    rng = np.random.default_rng(4)
+    theta_a, theta_c = lr.init_flat(N, D, A, generator=torch.Generator().manual_seed(1)), lr.init_flat(N, D, 1, generator=torch.Generator().manual_seed(2))
+    b = ac_oracle_batch(ac_batch(rng, 4, N, 6, D))
+    st = lr.A2CState(theta_a.clone(), theta_c.clone(), theta_c.clone(), [0, 1], [0, 1], D, A)
+    res = lr.ppo_update(st, b, lr.A2CHP(lr=3e-3), 0, 3, 0.2)
+    assert len(res["grads"]) == len(res["grad_norms"]) == len(res["clip_frac"]) == len(res["clip_margin"]) == 3
+    for k in ("actor", "critic"):
+        assert torch.equal(res["grads"][0][k], res["grad"][k])
+    assert res["grad_norms"][0] == pytest.approx(float(torch.cat([res["grad"]["actor"], res["grad"]["critic"]]).norm()), rel=1e-6)
+    st = lr.A2CState(theta_a.clone(), theta_c.clone(), theta_c.clone(), [0, 1], [0, 1], D, A)
+    assert lr.a2c_kink_risk(st, b, lr.A2CHP()) == 0.0
+    w1, b1 = lr.split_net(st.actor, D, A)[:2]        # views into agent 0's actor network
+    x = b["obss"][0, 0, :D]                          # step 0 of every episode is filled
+    b1[7] = 1e-7 - float(w1[7] @ x)
+    assert lr.a2c_kink_risk(st, b, lr.A2CHP()) > 0.0
 
-    cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, n_steps=hp.n_steps, entropy_coef=hp.entropy_coef,
-                                value_loss_coef=hp.value_loss_coef, target_update_interval_or_tau=hp.target_update_interval_or_tau, standardise_returns=standardise,
-                                num_epochs=num_epochs, ppo_clip=ppo_clip)
-    net = types.SimpleNamespace(layers=[128, 128], parameter_sharing=sharing, use_rnn=False, use_orthogonal_init=True, centralised=False)
-    cnet = types.SimpleNamespace(layers=[128, 128], parameter_sharing=sharing, use_rnn=False, use_orthogonal_init=True, centralised=centralised)
-    return getattr(M, cls)([_space(shape=(D,))] * n_agents, [_space(n=A)] * n_agents, cfg, net, cnet, "cuda", max_envs=P, max_episode_length=T)
+
+def test_oracle_ppo_kink_risk():
+    """ppo_kink_risk judges an epoch's loss at the parameters that epoch started from: 0 where no hidden unit sits within 2e-6 of its kink, positive
+    once one actor unit is 1e-7 from its kink on a filled row (an all-zero observation row, so that the unit's pre-activation is its bias exactly)"""
+    rng = np.random.default_rng(4)
+    theta_a, theta_c = lr.init_flat(N, D, A, generator=torch.Generator().manual_seed(1)), lr.init_flat(N, D, 1, generator=torch.Generator().manual_seed(2))
+    b = ac_oracle_batch(ac_batch(rng, 4, N, 6, D))
+    b["obss"][0, 0, :D] = 0.0                        # step 0 of every episode is filled
+    hp = lr.A2CHP(lr=3e-3)
+    st = lr.A2CState(theta_a.clone(), theta_c.clone(), theta_c.clone(), [0, 1], [0, 1], D, A)
+    st0 = copy.deepcopy(st)
+    res = lr.ppo_update(st, b, hp, 0, 2, 0.2)
+    assert torch.equal(res["epoch_start"][0][0], theta_a) and torch.equal(res["epoch_start"][0][1], theta_c)
+    for epoch in (0, -1):
+        assert lr.ppo_kink_risk(st0, b, hp, res, 0.2, epoch) == 0.0
+    b1 = lr.split_net(res["epoch_start"][0][0], D, A)[1]   # agent 0's actor biases of layer 1 (zero-initialised)
+    b1[7] = 1e-7
+    assert lr.ppo_kink_risk(st0, b, hp, res, 0.2, 0) > 0.0
 
 
 @pytest.mark.gpu
@@ -164,20 +169,15 @@ def _model(sharing, hp, P, n_agents, num_epochs, ppo_clip, standardise=False, cl
                                                                (False, 128, 2, 0.5, 6, 3e-3)])   # the last: a learning rate that drives ratios out of the clip range
 def test_ppo_update_matches_oracle(sharing, P, n_agents, clip, epochs, lr_):
     from codebase_b200.dqn.model import sharing_to_nets
-    from codebase_b200.lbf import TrajStore
-
     rng = np.random.default_rng(P + epochs)
     hp = lr.A2CHP(grad_clip=clip, lr=lr_, target_update_interval_or_tau=2)
-    m = _model(sharing, hp, P, n_agents, epochs, 0.2)
+    m = ac_model(hp, n_agents, D, P, T, sharing=sharing, cls="PPONetwork", num_epochs=epochs)
     nets = sharing_to_nets(sharing, n_agents)
     st = lr.A2CState(m.theta[: m.n_actor].cpu().clone(), m.theta[m.n_actor:].cpu().clone(), m.theta_tgt.cpu().clone(), nets, nets, D, A)
     for u, step in enumerate((0, 3, 4)):
-        s = _batch_arrays(rng, P, n_agents)
-        want = lr.ppo_update(st, _oracle_batch(s), hp, step, epochs, 0.2)
-        ts = TrajStore(P, n_agents, T, D, m.device)
-        for k in ("obs", "act", "rew", "done", "filled"):
-            getattr(ts, k).copy_(torch.as_tensor(s[k]))
-        met = m.metrics_dict(m.update_from_store(ts, P, step))
+        s = ac_batch(rng, P, n_agents, T, D)
+        want = lr.ppo_update(st, ac_oracle_batch(s), hp, step, epochs, 0.2)
+        met = m.metrics_dict(m.update_from_store(traj_store(s, m.device), P, step))
         _close([met["loss"], met["actor_loss"], met["value_loss"], met["entropy"]], [want["loss"], want["actor_loss"], want["value_loss"], want["entropy"]], rtol=2e-5, atol=2e-5)
         d = np.abs(m.theta.cpu().numpy() - np.concatenate([st.actor.numpy(), st.critic.numpy()]))
         assert np.quantile(d, 0.999) < 1e-5 * max(1.0, lr_ / 3e-4) and d.max() < 2 * hp.lr * epochs * (u + 1) + 1e-6, (np.quantile(d, 0.999), d.max())
@@ -191,22 +191,17 @@ def test_ppo_update_matches_oracle(sharing, P, n_agents, clip, epochs, lr_):
 @pytest.mark.parametrize("cls", ["A2CNetwork", "PPONetwork"])
 def test_standardise_returns_matches_oracle(cls):
     """cfg.standardise_returns=True on the device (marl_a2c_standardise_returns): metrics, running statistics and parameters against the oracle"""
-    from codebase_b200.lbf import TrajStore
-
     P, n_agents, epochs = 200, 2, 3
     rng = np.random.default_rng(21)
     hp = lr.A2CHP(target_update_interval_or_tau=2)
-    m = _model(False, hp, P, n_agents, epochs, 0.2, standardise=True, cls=cls)
+    m = ac_model(hp, n_agents, D, P, T, cls=cls, standardise=True, num_epochs=epochs)
     st = lr.A2CState(m.theta[: m.n_actor].cpu().clone(), m.theta[m.n_actor:].cpu().clone(), m.theta_tgt.cpu().clone(), [0, 1], [0, 1], D, A,
                      ret_ms=lr.RunningMeanStdRef((n_agents,)))
     for u, step in enumerate((0, 2, 5)):
-        s = _batch_arrays(rng, P, n_agents)
+        s = ac_batch(rng, P, n_agents, T, D)
         s["rew"] *= 3.0   # returns away from the unit scale the statistics start at
-        want = lr.ppo_update(st, _oracle_batch(s), hp, step, epochs, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, _oracle_batch(s), hp, step)
-        ts = TrajStore(P, n_agents, T, D, m.device)
-        for k in ("obs", "act", "rew", "done", "filled"):
-            getattr(ts, k).copy_(torch.as_tensor(s[k]))
-        met = m.metrics_dict(m.update_from_store(ts, P, step))
+        want = lr.ppo_update(st, ac_oracle_batch(s), hp, step, epochs, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, ac_oracle_batch(s), hp, step)
+        met = m.metrics_dict(m.update_from_store(traj_store(s, m.device), P, step))
         _close([met["loss"], met["actor_loss"], met["value_loss"], met["entropy"]], [want["loss"], want["actor_loss"], want["value_loss"], want["entropy"]], rtol=2e-5, atol=2e-5)
         mean, var, count = m.ret_ms()
         _close(mean.numpy(), st.ret_ms.mean.numpy()); _close(var.numpy(), st.ret_ms.var.numpy()); assert abs(count - st.ret_ms.count) < 1e-6
@@ -222,12 +217,10 @@ def test_standardise_returns_matches_oracle(cls):
 @pytest.mark.parametrize("cls,sharing", [("A2CNetwork", False), ("PPONetwork", True)])
 def test_centralised_critic_matches_oracle(cls, sharing):
     """MAA2C / MAPPO on the device: the critic passes read the joint observation rows (source mode 2; `values()`: mode 3)"""
-    from codebase_b200.lbf import TrajStore
-
     P, n_agents, epochs = 300, 2, 2
     rng = np.random.default_rng(31)
     hp = lr.A2CHP(target_update_interval_or_tau=2)
-    m = _model(sharing, hp, P, n_agents, epochs, 0.2, cls=cls, centralised=True)
+    m = ac_model(hp, n_agents, D, P, T, sharing=sharing, cls=cls, centralised=True, num_epochs=epochs)
     nets = [0, 0] if sharing else [0, 1]
     assert m.n_critic == len(set(nets)) * lr.net_size(n_agents * D, 1)
     st = lr.A2CState(m.theta[: m.n_actor].cpu().clone(), m.theta[m.n_actor:].cpu().clone(), m.theta_tgt.cpu().clone(), nets, nets, D, A, centralised=True)
@@ -236,12 +229,9 @@ def test_centralised_critic_matches_oracle(cls, sharing):
     want_v = torch.cat(lr.agents_forward(st.critic, nets, [joint] * n_agents, n_agents * D, 1), -1).numpy()
     _close(m.values(torch.tensor(obs, device="cuda")).cpu().numpy(), want_v)
     for u, step in enumerate((0, 2, 5)):
-        s = _batch_arrays(rng, P, n_agents)
-        want = lr.ppo_update(st, _oracle_batch(s), hp, step, epochs, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, _oracle_batch(s), hp, step)
-        ts = TrajStore(P, n_agents, T, D, m.device)
-        for k in ("obs", "act", "rew", "done", "filled"):
-            getattr(ts, k).copy_(torch.as_tensor(s[k]))
-        met = m.metrics_dict(m.update_from_store(ts, P, step))
+        s = ac_batch(rng, P, n_agents, T, D)
+        want = lr.ppo_update(st, ac_oracle_batch(s), hp, step, epochs, 0.2) if cls == "PPONetwork" else lr.a2c_update(st, ac_oracle_batch(s), hp, step)
+        met = m.metrics_dict(m.update_from_store(traj_store(s, m.device), P, step))
         _close([met["loss"], met["actor_loss"], met["value_loss"], met["entropy"]], [want["loss"], want["actor_loss"], want["value_loss"], want["entropy"]], rtol=2e-5, atol=2e-5)
         d = np.abs(m.theta.cpu().numpy() - np.concatenate([st.actor.numpy(), st.critic.numpy()]))
         assert np.quantile(d, 0.999) < 1e-5, (u, np.quantile(d, 0.999))

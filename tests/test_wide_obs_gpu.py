@@ -8,7 +8,7 @@ import torch
 
 from oracle import learner_ref as lr
 
-from tests.helpers import assert_grad_close, check_margin, redraw_on_near_tie
+from tests.helpers import ac_batch, ac_model, ac_oracle_batch, assert_grad_close, check_margin, redraw_on_near_tie, space, traj_store
 
 pytestmark = pytest.mark.gpu
 T, A = 25, 6
@@ -17,34 +17,6 @@ T, A = 25, 6
 def _close(a, b, rtol=1e-5, atol=1e-5):
     a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
     assert np.allclose(a, b, rtol=rtol, atol=atol), float(np.abs(a - b).max())
-
-
-def _space(shape=None, n=None):
-    return types.SimpleNamespace(shape=shape, n=n)
-
-
-def _random_store(rng, cap, n_agents, D, coop):
-    obs = rng.integers(-1, 15, size=(cap, n_agents, T + 1, D)).astype(np.float32)
-    act = rng.integers(0, A, size=(cap, n_agents, T)).astype(np.int32)
-    rew = (rng.random((cap, n_agents, T)) < 0.2).astype(np.float32) * rng.random((cap, n_agents, T)).astype(np.float32)
-    if coop:
-        rew[:] = rew[:, :1]
-    length = rng.integers(1, T + 1, size=cap)
-    done = np.zeros((cap, T + 1), np.uint8); filled = np.zeros((cap, T), np.uint8)
-    for e in range(cap):
-        filled[e, : length[e]] = 1
-        done[e, length[e]] = 1
-    return dict(obs=obs, act=act, rew=rew, done=done, filled=filled)
-
-
-def _to_store(s, device):
-    from codebase_b200.lbf import TrajStore
-
-    cap, n_agents, _, D = s["obs"].shape
-    ts = TrajStore(cap, n_agents, T, D, device)
-    for k in ("obs", "act", "rew", "done", "filled"):
-        getattr(ts, k).copy_(torch.as_tensor(s[k]))
-    return ts
 
 
 @pytest.mark.parametrize("mixer,n_agents,D,B", [(0, 4, 27, 96), (1, 4, 27, 300), (0, 2, 17, 64), (0, 3, 32, 40)])
@@ -56,19 +28,19 @@ def test_dqn_family_update_wide_obs(mixer, n_agents, D, B):
     hp = lr.DqnHP(mixer=mixer)
     cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, double_q=hp.double_q,
                                 target_update_interval_or_tau=hp.target_update_interval_or_tau, standardise_returns=False)
-    m = (M.VDNetwork if mixer else M.QNetwork)([_space(shape=(D,))] * n_agents, [_space(n=A)] * n_agents, cfg, [128, 128], False, False, True, "cuda",
+    m = (M.VDNetwork if mixer else M.QNetwork)([space(shape=(D,))] * n_agents, [space(n=A)] * n_agents, cfg, [128, 128], False, False, True, "cuda",
                                              max_batch=B, max_episode_length=T)
     st = lr.DqnState(m.theta.cpu().clone(), m.theta_tgt.cpu().clone(), m.agent_net, D, A)
     obs = rng.integers(-1, 15, size=(50, n_agents, D)).astype(np.float32)
     want_q = torch.stack(lr.agents_forward(st.theta, m.agent_net, [torch.tensor(obs[:, i]) for i in range(n_agents)], D, A), 1).numpy()
     _close(m.q_values(torch.tensor(obs, device="cuda")).cpu().numpy(), want_q)
-    store = _random_store(rng, 200, n_agents, D, bool(mixer))
+    store = ac_batch(rng, 200, n_agents, T, D, obs_high=15, coop=bool(mixer))
     idx = rng.integers(0, 200, size=B).astype(np.int32)
     batch = lr.batch_from_store(store, idx)
     check_margin(lr, st, batch, hp)   # near-tie in the double-Q argmax: re-drawn by the decorator
     st0 = lr.DqnState(st.theta.clone(), st.theta_tgt.clone(), st.agent_net, st.in_dim, st.out_dim)   # dqn_update steps st in place
     want = lr.dqn_update(st, batch, hp)
-    m.update_grads(_to_store(store, m.device), torch.tensor(idx, device="cuda"))
+    m.update_grads(traj_store(store, m.device), torch.tensor(idx, device="cuda"))
     gr = m.grad.cpu().numpy()
     scale = max(1.0, float(np.abs(want["grad"].numpy()).max()))
     assert_grad_close(lr, st0, batch, hp, gr[: m.n_params] / gr[m.n_params + 1], want["grad"].numpy())   # re-drawn when a ReLU unit on its kink explains the mismatch
@@ -78,23 +50,16 @@ def test_dqn_family_update_wide_obs(mixer, n_agents, D, B):
 
 
 def test_a2c_update_wide_obs():
-    from codebase_b200.ac.model import A2CNetwork
-
     rng = np.random.default_rng(5)
     n_agents, D, P = 4, 27, 128
     hp = lr.A2CHP()
-    cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, n_steps=hp.n_steps, entropy_coef=hp.entropy_coef,
-                                value_loss_coef=hp.value_loss_coef, target_update_interval_or_tau=hp.target_update_interval_or_tau, standardise_returns=False)
-    net = types.SimpleNamespace(layers=[128, 128], parameter_sharing=True, use_rnn=False, use_orthogonal_init=True, centralised=False)
-    m = A2CNetwork([_space(shape=(D,))] * n_agents, [_space(n=A)] * n_agents, cfg, net, net, "cuda", max_envs=P, max_episode_length=T)
+    m = ac_model(hp, n_agents, D, P, T, sharing=True)
     nets = [0] * n_agents
     st = lr.A2CState(m.theta[: m.n_actor].cpu().clone(), m.theta[m.n_actor:].cpu().clone(), m.theta_tgt.cpu().clone(), nets, nets, D, A)
-    s = _random_store(rng, P, n_agents, D, False)
-    t = {k: torch.as_tensor(v) for k, v in s.items()}
-    batch = dict(obss=t["obs"].permute(2, 0, 1, 3).reshape(T + 1, P, n_agents * D).float(), actions=t["act"].permute(2, 0, 1).long(),
-                 rewards=t["rew"].permute(2, 0, 1).float(), dones=t["done"].permute(1, 0).float(), filled=t["filled"].permute(1, 0).float())
+    s = ac_batch(rng, P, n_agents, T, D, obs_high=15)
+    batch = ac_oracle_batch(s)
     want = lr.a2c_update(st, batch, hp, 0)
-    met = m.metrics_dict(m.update_from_store(_to_store(s, m.device), P, 0))
+    met = m.metrics_dict(m.update_from_store(traj_store(s, m.device), P, 0))
     _close([met["loss"], met["actor_loss"], met["value_loss"], met["entropy"]], [want["loss"], want["actor_loss"], want["value_loss"], want["entropy"]])
     d = np.abs(m.theta.cpu().numpy() - np.concatenate([st.actor.numpy(), st.critic.numpy()]))
     assert np.quantile(d, 0.999) < 1e-5
