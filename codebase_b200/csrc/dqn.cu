@@ -6,6 +6,7 @@
 #include "learner.cuh"
 #include "retms.cuh"
 #include "qmix.cuh"
+#include "gru.cuh"
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -24,10 +25,13 @@ __global__ void replay_sample_kernel(uint64_t seed, uint64_t update_idx, int bat
 }
 
 // ---- VDN: agent-coupled TD error (marlbase/dqn/model.py:224-269) ------------------------------------------------
+// C columns of G agents each: column c sums the Q-values of agents [c G, c G + G) and takes agent c G's reward.  VDN: C = 1, G = N;
+// independent learners (the recurrent pass, whose backward has no TD head of its own): C = N, G = 1.
 struct VdnTdParams {
   const float* q; const float* tq;  // [N][B][T+1][A]
   TrajView traj; const int32_t* idx; int B, N, A; float gamma; int double_q;
-  float* td;         // [B][T] = 2 * delta * filled
+  int C, G;
+  float* td;         // [C][B][T] = 2 * delta * filled
   float* loss_part;  // [gridDim][4]
 };
 
@@ -35,11 +39,11 @@ __global__ void __launch_bounds__(256) vdn_td_kernel(VdnTdParams p) {
   __shared__ float red[512];
   const int T = p.traj.T, i = blockIdx.x * 256 + threadIdx.x;
   float loss = 0.f, fill = 0.f;
-  if (i < p.B * T) {
-    const int b = i / T, t = i - b * T;
+  if (i < p.C * p.B * T) {
+    const int c = i / (p.B * T), rem = i - c * p.B * T, b = rem / T, t = rem - b * T;
     const size_t ep = (size_t)p.idx[b];
     float chosen = 0.f, tsum = 0.f;
-    for (int a = 0; a < p.N; ++a) {
+    for (int a = c * p.G; a < (c + 1) * p.G; ++a) {
       const size_t row = ((size_t)a * p.B + b) * (T + 1) + t;
       const float* q0 = p.q + row * p.A; const float* q1 = q0 + p.A; const float* t1 = p.tq + (row + 1) * p.A;
       chosen += q0[p.traj.act[(ep * p.N + a) * T + t]];
@@ -54,9 +58,9 @@ __global__ void __launch_bounds__(256) vdn_td_kernel(VdnTdParams p) {
       }
     }
     const float filled = (float)p.traj.filled[ep * T + t];
-    const float y = p.traj.rew[(ep * p.N + 0) * T + t] + p.gamma * tsum * (1.f - (float)p.traj.done[ep * (T + 1) + t + 1]);
+    const float y = p.traj.rew[(ep * p.N + c * p.G) * T + t] + p.gamma * tsum * (1.f - (float)p.traj.done[ep * (T + 1) + t + 1]);
     const float delta = chosen - y;
-    loss = delta * delta * filled; fill = filled;
+    loss = delta * delta * filled; fill = c == 0 ? filled : 0.f;
     p.td[i] = 2.f * delta * filled;
   }
   red[threadIdx.x] = loss; red[256 + threadIdx.x] = fill;
@@ -165,6 +169,9 @@ struct marl_dqn {
   // QMIX (hp.mixer == 2): the mixing network's parameters / Adam state / gradient (+ 4 statistics), per-sample records, chunked partial sums, tile list
   QmixLayout ql = {}; float *mix = nullptr, *mix_tgt = nullptr, *mix_m = nullptr, *mix_v = nullptr, *mix_grad = nullptr, *mix_rec = nullptr, *mix_part = nullptr, *mix_img = nullptr, *mix_img_tgt = nullptr;
   QmixTile* mix_tiles = nullptr; int mix_n_tiles = 0; QmixMicro* mix_micro = nullptr; int mix_n_micro = 0; bool mix_wgrad_tiles = false;
+  // recurrent agent networks (marl_dqn_create_rnn): GRU parameter layout and the online pass's saved rows [N][B][T+1][kGruSaveRow]
+  bool rnn = false; GruLayout gl = {}; float* gru_save = nullptr;
+  int P() const { return rnn ? gl.P : ns.lay.P; }
 };
 static const int kTimingPairs = 1024;
 
@@ -172,7 +179,7 @@ static int dqn_alloc(float** p, size_t n_floats) { return dev_alloc_zero(p, n_fl
 
 extern "C" {
 
-int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device, marl_dqn** out) {
+static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device, bool rnn, marl_dqn** out) {
   MARL_REQUIRE(cfg && hp && out, "marl_dqn_create: NULL argument");
   *out = nullptr;
   MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "marl_dqn_create: n_agents out of range");
@@ -182,6 +189,7 @@ int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_
   MARL_REQUIRE(max_batch >= 1 && max_T >= 1, "marl_dqn_create: max_batch/max_T must be >= 1");
   MARL_REQUIRE(hp->mixer >= 0 && hp->mixer <= 2, "marl_dqn_create: mixer must be 0 (independent), 1 (VDN) or 2 (QMIX)");
   for (int a = 0; a < cfg->n_agents; ++a) MARL_REQUIRE(cfg->agent_net[a] >= 0 && cfg->agent_net[a] < cfg->n_nets, "marl_dqn_create: agent_net[%d] out of range", a);
+  MARL_REQUIRE(!rnn || (cfg->in_dim >= 1 && cfg->in_dim <= kMaxObsDim), "marl_dqn_create_rnn: obs dim %d not supported (1..%d)", cfg->in_dim, kMaxObsDim);
   if (int rc = check_device(device)) return rc;
   marl_dqn* h = new marl_dqn();
   h->ns.n_agents = cfg->n_agents; h->ns.n_nets = cfg->n_nets; h->ns.in = cfg->in_dim; h->ns.out = cfg->out_dim;
@@ -189,14 +197,15 @@ int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_
   h->ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim);
   h->hp = *hp; h->device = device; h->max_batch = max_batch; h->max_T = max_T;
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
-  h->n_params = (int64_t)cfg->n_nets * h->ns.lay.P;
-  h->scratch_pitch = (h->ns.lay.P + 3) & ~3;
+  h->rnn = rnn; h->gl = GruLayout::make(cfg->in_dim, cfg->out_dim);
+  h->n_params = (int64_t)cfg->n_nets * h->P();
+  h->scratch_pitch = (h->P() + 3) & ~3;
   const size_t rows = (size_t)cfg->n_agents * max_batch * (max_T + 1);
   int rc = 0;
   rc |= dqn_alloc(&h->theta, h->n_params); rc |= dqn_alloc(&h->theta_tgt, h->n_params);
   rc |= dqn_alloc(&h->m, h->n_params); rc |= dqn_alloc(&h->v, h->n_params); rc |= dqn_alloc(&h->grad, h->n_params + 4);
   rc |= dqn_alloc(&h->scratch, (size_t)h->n_sm * h->scratch_pitch);
-  rc |= dqn_alloc(&h->loss_part, 4 * ((size_t)h->n_sm + (size_t)max_batch * max_T / 256 + 2));
+  rc |= dqn_alloc(&h->loss_part, 4 * ((size_t)h->n_sm + (size_t)(rnn ? cfg->n_agents : 1) * max_batch * max_T / 256 + 2));
   rc |= dqn_alloc(&h->tq, rows * cfg->out_dim);
   rc |= dqn_alloc(&h->loss_dev, 8);
   rc |= dqn_alloc(&h->sumsq, (size_t)(h->n_params + 63) / 64 + 1);
@@ -204,14 +213,32 @@ int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_
   if (hp->mixer == 1) { rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim); rc |= dqn_alloc(&h->td, (size_t)max_batch * max_T); }
   if (hp->mixer == 2) { rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim); rc |= dqn_alloc(&h->td, (size_t)cfg->n_agents * max_batch * max_T); }
   rc |= dqn_alloc(reinterpret_cast<float**>(&h->idx), max_batch);
-  rc |= dqn_alloc(reinterpret_cast<float**>(&h->image), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
-  rc |= dqn_alloc(reinterpret_cast<float**>(&h->image_tgt), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
+  if (rnn) {   // the recurrent pass always hands the TD error to its backward: online Q-values of every row and one TD entry per (agent, b, t)
+    if (!h->q_all) rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim);
+    if (hp->mixer == 0) rc |= dqn_alloc(&h->td, (size_t)cfg->n_agents * max_batch * max_T);
+    rc |= dqn_alloc(&h->gru_save, rows * kGruSaveRow);
+  } else {
+    rc |= dqn_alloc(reinterpret_cast<float**>(&h->image), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
+    rc |= dqn_alloc(reinterpret_cast<float**>(&h->image_tgt), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
+  }
   if (rc) { marl_dqn_destroy(h); return MARL_ENOMEM; }
-  if (int rc2 = learner_kernels_init(cfg->in_dim)) { marl_dqn_destroy(h); return rc2; }
-  if (int rc2 = tc_forward_init()) { marl_dqn_destroy(h); return rc2; }
-  if (int rc2 = tc_train_init()) { marl_dqn_destroy(h); return rc2; }
+  if (rnn) {
+    if (int rc2 = gru_kernels_init()) { marl_dqn_destroy(h); return rc2; }
+  } else {
+    if (int rc2 = learner_kernels_init(cfg->in_dim)) { marl_dqn_destroy(h); return rc2; }
+    if (int rc2 = tc_forward_init()) { marl_dqn_destroy(h); return rc2; }
+    if (int rc2 = tc_train_init()) { marl_dqn_destroy(h); return rc2; }
+  }
   *out = h;
   return MARL_OK;
+}
+
+int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device, marl_dqn** out) {
+  return dqn_create(cfg, hp, max_batch, max_T, device, false, out);
+}
+
+int marl_dqn_create_rnn(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device, marl_dqn** out) {
+  return dqn_create(cfg, hp, max_batch, max_T, device, true, out);
 }
 
 int marl_dqn_destroy(marl_dqn* h) {
@@ -221,7 +248,7 @@ int marl_dqn_destroy(marl_dqn* h) {
   cudaFree(h->loss_part); cudaFree(h->tq); cudaFree(h->q_all); cudaFree(h->td); cudaFree(h->loss_dev); cudaFree(h->sumsq); cudaFree(h->idx); cudaFree(h->image); cudaFree(h->image_tgt); cudaFree(h->image_bwd); cudaFree(h->tc_h1); cudaFree(h->tc_h2); cudaFree(h->tc_dh1); cudaFree(h->tc_rec); cudaFree(h->tc_x); cudaFree(h->grid_barrier);
   for (int r = 0; r < kMaxRanks; ++r) if (h->peer_base[r] != nullptr && r != h->xchg.rank) cudaIpcCloseMemHandle(h->peer_base[r]);
   cudaFree(h->mix); cudaFree(h->mix_tgt); cudaFree(h->mix_m); cudaFree(h->mix_v); cudaFree(h->mix_grad); cudaFree(h->mix_rec); cudaFree(h->mix_part); cudaFree(h->mix_tiles); cudaFree(h->mix_micro); cudaFree(h->mix_img); cudaFree(h->mix_img_tgt);
-  cudaFree(h->xbuf); cudaFree(h->ret_ms); cudaFree(h->ret); cudaFree(h->chosen); cudaFree(h->ret_count); cudaFree(h->ret_part);
+  cudaFree(h->xbuf); cudaFree(h->ret_ms); cudaFree(h->ret); cudaFree(h->chosen); cudaFree(h->ret_count); cudaFree(h->ret_part); cudaFree(h->gru_save);
   for (auto& e : h->ev) cudaEventDestroy(e);
   delete h;
   return MARL_OK;
@@ -242,7 +269,7 @@ int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
     int rc = 0;
     rc |= dqn_alloc(&h->ret_ms, 2 * n); rc |= dqn_alloc(&h->ret, (size_t)C * h->max_batch * h->max_T); rc |= dqn_alloc(&h->chosen, (size_t)C * h->max_batch * h->max_T);
     if (!h->q_all) rc |= dqn_alloc(&h->q_all, rows * h->ns.out);
-    if (!h->td || h->hp.mixer == 0) { cudaFree(h->td); h->td = nullptr; rc |= dqn_alloc(&h->td, (size_t)C * h->max_batch * h->max_T); }
+    if (!h->td || (h->hp.mixer == 0 && !h->rnn)) { cudaFree(h->td); h->td = nullptr; rc |= dqn_alloc(&h->td, (size_t)C * h->max_batch * h->max_T); }
     if (rc) return MARL_ENOMEM;
     MARL_CUDA_TRY(cudaMalloc(&h->ret_count, sizeof(double))); MARL_CUDA_TRY(cudaMalloc(&h->ret_part, (size_t)kRetBlocks * n * 2 * sizeof(double)));
     MARL_CUDA_TRY(cudaMemcpy(h->ret_ms, init.data(), 2 * n * sizeof(float), cudaMemcpyHostToDevice));
@@ -372,6 +399,7 @@ int marl_dqn_sync_target(marl_dqn* h, void* stream) {
 
 int marl_dqn_forward(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_target, float* q_out, void* stream) {
   MARL_REQUIRE(h && obs && q_out && n_envs >= 1, "marl_dqn_forward: bad argument");
+  MARL_REQUIRE(!h->rnn, "marl_dqn_forward: the learner has recurrent agent networks: use marl_dqn_forward_rnn, which carries the hidden state");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   const RowPlan plan = make_plan(h->ns, n_envs, 1, h->n_sm, 32);
   RowSource src; memset(&src, 0, sizeof(src));
@@ -380,6 +408,25 @@ int marl_dqn_forward(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_
   const int rc = forward_any(h->ns, plan, src, use_target ? h->theta_tgt : h->theta, use_target ? h->image_tgt : h->image, q_out, (cudaStream_t)stream, current);
   if (rc == MARL_OK) current = tc_forward_enabled() != 0;
   return rc;
+}
+
+static GruFwdParams gru_fwd_params(const marl_dqn* h, const RowSource& src, int units, int steps, bool target) {
+  GruFwdParams fp; memset(&fp, 0, sizeof(fp));
+  fp.plan = make_plan(h->ns, units, steps, 1, 1); fp.src = src;
+  fp.theta = target ? h->theta_tgt : h->theta; fp.lay = h->gl;
+  return fp;
+}
+
+int marl_dqn_forward_rnn(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_target, const float* h_in, float* h_out, float* q_out, void* stream) {
+  MARL_REQUIRE(h && obs && q_out && n_envs >= 1, "marl_dqn_forward_rnn: bad argument");
+  MARL_REQUIRE(h->rnn, "marl_dqn_forward_rnn: the learner was not created with marl_dqn_create_rnn");
+  MARL_REQUIRE(h_in == nullptr || h_in != h_out, "marl_dqn_forward_rnn: h_in and h_out must not alias");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  RowSource src; memset(&src, 0, sizeof(src));
+  src.mode = 0; src.dense = obs; src.E = n_envs; src.N = h->ns.n_agents; src.D = h->ns.in;
+  GruFwdParams fp = gru_fwd_params(h, src, n_envs, 1, use_target != 0);
+  fp.h_in = h_in; fp.h_out = h_out; fp.q_out = q_out;
+  return launch_gru_forward(fp, (cudaStream_t)stream);
 }
 
 int marl_replay_sample(uint64_t seed, uint64_t update_idx, int32_t batch, int32_t n_valid, int32_t* idx_out, void* stream) {
@@ -399,17 +446,34 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   cudaStream_t st = (cudaStream_t)stream;
   const int T = traj->T;
   const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
-  const RowPlan plan = make_plan(h->ns, batch, T + 1, h->n_sm, min_units);
+  const RowPlan plan = h->rnn ? make_plan(h->ns, batch, 1, h->n_sm, kGruSeqs) : make_plan(h->ns, batch, T + 1, h->n_sm, min_units);
   RowSource src; memset(&src, 0, sizeof(src));
   src.mode = 1; src.traj = to_view(traj); src.idx = episode_idx; src.N = h->ns.n_agents; src.D = h->ns.in;
+  const bool rec = h->timing && h->ev_used < kTimingPairs;
   // target network on every gathered row (dqn/model.py:132-134); several ranks: the previous update launched it between its push and its finish
   if (h->tq_ahead) {
     h->tq_ahead = false;
+  } else if (h->rnn) {
+    GruFwdParams fp = gru_fwd_params(h, src, batch, T + 1, true);
+    fp.q_out = h->tq;
+    if (int rc = launch_gru_forward(fp, st)) return rc;
   } else {
     if (int rc = forward_any(h->ns, plan, src, h->theta_tgt, h->image_tgt, h->tq, st, h->tgt_image_current)) return rc;
     h->tgt_image_current = tc_forward_enabled() != 0;
   }
-  int n_loss_parts = plan.cta_begin[plan.n_nets];
+  // online Q-values of every row for the external TD heads; the recurrent pass also saves what its backward needs
+  auto online_forward = [&]() -> int {
+    if (h->rnn) {
+      if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
+      GruFwdParams fp = gru_fwd_params(h, src, batch, T + 1, false);
+      fp.q_out = h->q_all; fp.save = h->gru_save;
+      return launch_gru_forward(fp, st);
+    }
+    if (int rc = forward_any(h->ns, plan, src, h->theta, h->image, h->q_all, st, h->image_current)) return rc;
+    h->image_current = tc_forward_enabled() != 0;
+    return MARL_OK;
+  };
+  int n_loss_parts = h->rnn ? 0 : plan.cta_begin[plan.n_nets];
   const float* td_ext = nullptr;
   float* loss_part = h->loss_part;
   int td_agent_stride = 0;
@@ -417,8 +481,7 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
     // online Q-values of every row, returns + chosen Q, RunningMeanStd step, TD error (dqn/model.py:147-158 / 256-264)
     MARL_REQUIRE(h->hp.mixer == 0 || batch == h->n_stat, "marl_dqn_update: VDN's standardise_returns keeps one statistic per batch entry (the reference's reshape(-1, B)): "
                  "batch %d must stay at max_batch %d", batch, h->n_stat);
-    if (int rc = forward_any(h->ns, plan, src, h->theta, h->image, h->q_all, st, h->image_current)) return rc;
-    h->image_current = tc_forward_enabled() != 0;
+    if (int rc = online_forward()) return rc;
     const int C = h->hp.mixer == 1 ? 1 : h->ns.n_agents;
     StdRetParams sp; memset(&sp, 0, sizeof(sp));
     sp.q = h->q_all; sp.tq = h->tq; sp.traj = src.traj; sp.idx = episode_idx; sp.B = batch; sp.N = h->ns.n_agents; sp.A = h->ns.out; sp.vdn = h->hp.mixer == 1;
@@ -435,21 +498,23 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
     n_loss_parts += vb;
     td_ext = h->td;
     td_agent_stride = h->hp.mixer == 1 ? 0 : batch * T;
-  } else if (h->hp.mixer == 1) {  // VDN: online Q-values of all agents first, then the agent-summed TD error
-    if (int rc = forward_any(h->ns, plan, src, h->theta, h->image, h->q_all, st, h->image_current)) return rc;
-    h->image_current = tc_forward_enabled() != 0;
+  } else if (h->hp.mixer == 1 || (h->rnn && h->hp.mixer == 0)) {
+    // VDN: online Q-values of all agents first, then the agent-summed TD error; recurrent independent learners: one column per agent
+    if (int rc = online_forward()) return rc;
+    const bool vdn = h->hp.mixer == 1;
     VdnTdParams vp; vp.q = h->q_all; vp.tq = h->tq; vp.traj = src.traj; vp.idx = episode_idx; vp.B = batch; vp.N = h->ns.n_agents; vp.A = h->ns.out;
     vp.gamma = h->hp.gamma; vp.double_q = h->hp.double_q; vp.td = h->td;
-    const int vb = (batch * T + 255) / 256;
+    vp.C = vdn ? 1 : h->ns.n_agents; vp.G = vdn ? h->ns.n_agents : 1;
+    const int vb = (vp.C * batch * T + 255) / 256;
     vp.loss_part = h->loss_part + 4 * (size_t)n_loss_parts;  // the train kernel's parts read as zero in this mode
     vdn_td_kernel<<<vb, 256, 0, st>>>(vp);
     MARL_CUDA_TRY(cudaGetLastError());
     n_loss_parts += vb;
     td_ext = h->td;
+    td_agent_stride = vdn ? 0 : batch * T;
   } else if (h->hp.mixer == 2) {  // QMIX: the mixer turns the agents' Q-values into the TD error and hands dL/dq_a back per agent (qmix.cuh)
     MARL_REQUIRE(h->mix != nullptr, "marl_dqn_update: QMIX needs marl_dqn_qmix_init first");
-    if (int rc = forward_any(h->ns, plan, src, h->theta, h->image, h->q_all, st, h->image_current)) return rc;
-    h->image_current = tc_forward_enabled() != 0;
+    if (int rc = online_forward()) return rc;
     QmixParams qp; memset(&qp, 0, sizeof(qp));
     qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = episode_idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
     qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
@@ -474,9 +539,13 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   TrainParams tp; memset(&tp, 0, sizeof(tp));
   tp.plan = plan; tp.src = src; tp.theta = h->theta; tp.lay = h->ns.lay; tp.tq = h->tq; tp.td_ext = td_ext; tp.td_agent_stride = td_agent_stride;
   tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = loss_part;
-  const bool rec = h->timing && h->ev_used < kTimingPairs;
-  if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
-  if (tc_backward_enabled() && h->ns.in < kMaxObsDim) {
+  if (h->rnn) {   // BPTT from td_ext; the timed window opened before the online forward
+    GruBwdParams bp; memset(&bp, 0, sizeof(bp));
+    bp.plan = plan; bp.traj = src.traj; bp.idx = episode_idx; bp.B = batch; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
+    bp.td = td_ext; bp.td_agent_stride = td_agent_stride; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
+    if (int rc = launch_gru_backward(bp, st)) return rc;
+  } else if (tc_backward_enabled() && h->ns.in < kMaxObsDim) {
+    if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
     if (!h->tc_h1) {  // intermediates of the tensor-core pipeline, allocated on first use
       const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
       int rc = 0;
@@ -493,10 +562,11 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
     if (int rc = launch_tc_dqn_train(tp, tb, st, rec ? &h->ev[4 * h->ev_used + 1] : nullptr)) return rc;
     if (rec) h->ev_split = true;
   } else {
+    if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
     if (int rc = launch_train(tp, kHeadDqn, st)) return rc;
   }
   if (rec) { cudaEventRecord(h->ev[4 * h->ev_used + 3], st); h->ev_used += 1; }
-  ReduceParams rp; rp.scratch = h->scratch; rp.loss_part = h->loss_part; rp.n_nets = h->ns.n_nets; rp.P = h->ns.lay.P; rp.scratch_pitch = h->scratch_pitch;
+  ReduceParams rp; rp.scratch = h->scratch; rp.loss_part = h->loss_part; rp.n_nets = h->ns.n_nets; rp.P = h->P(); rp.scratch_pitch = h->scratch_pitch;
   memcpy(rp.cta_begin, plan.cta_begin, sizeof(rp.cta_begin));
   rp.n_loss_parts = n_loss_parts; rp.grad = h->grad; rp.stats = h->grad + h->n_params; rp.stats_accumulate = 0; rp.sumsq_part = h->sumsq;
   if (rp_out != nullptr) { *rp_out = rp; return MARL_OK; }
@@ -694,6 +764,7 @@ int marl_dqn_peer_attach(marl_dqn* h, int32_t rank, int32_t world, const void* h
   MARL_REQUIRE(world >= 2 && world <= kMaxRanks && rank >= 0 && rank < world, "marl_dqn_peer_attach: rank %d / world %d out of range (2..%d ranks)", rank, world, kMaxRanks);
   MARL_REQUIRE(h->xbuf != nullptr && h->xchg.world <= 1, "marl_dqn_peer_attach: call marl_dqn_peer_handle first, attach once");
   MARL_REQUIRE(h->hp.mixer != 2, "marl_dqn_peer_attach: the mixer's gradient is not part of the peer exchange: QMIX runs on one GPU");
+  MARL_REQUIRE(!h->rnn, "marl_dqn_peer_attach: recurrent agent networks run on one GPU");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   {  // the exchange lives inside the fused reduce + Adam kernel: refuse here, before any update mutates counters, when that kernel cannot
      // cover this parameter count with one co-resident wave (a later fallback to the two-kernel tail would dead-lock the peers' polls)

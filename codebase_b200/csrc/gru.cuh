@@ -1,0 +1,53 @@
+// gru.cuh -- recurrent (GRU) agent networks of the DQN family (algorithm.model.use_rnn=True): parameter layout, the
+// sequence forward and the BPTT backward.  Replaces marlbase/utils/models.py:51-116 (RNNNetwork with layers = [128, 128]:
+// first_layer Linear(D, 128) + ReLU, nn.GRU(128, 128, num_layers=1), final_layer Linear(128, A)).
+#pragma once
+#include "learner.cuh"
+
+namespace marl {
+
+constexpr int kGruSeqs = 16;                 // sequences per CTA tile (two halves of 8, one per 128-thread half of the block)
+constexpr int kGruThreads = 256;
+constexpr int kGruSaveRow = 6 * kHidden;     // floats the online pass saves per row: x1 | r | z | n | W_hn h + b_hn | h'
+
+// Flat parameters of one network in the reference's state_dict order.
+struct GruLayout {
+  int in, out;
+  int w1, b1, wih, whh, bih, bhh, w3, b3, P;   // float offsets, P = total
+  __host__ __device__ static GruLayout make(int in_, int out_) {
+    GruLayout l; l.in = in_; l.out = out_;
+    l.w1 = 0; l.b1 = l.w1 + kHidden * in_;
+    l.wih = l.b1 + kHidden; l.whh = l.wih + 3 * kHidden * kHidden;
+    l.bih = l.whh + 3 * kHidden * kHidden; l.bhh = l.bih + 3 * kHidden;
+    l.w3 = l.bhh + 3 * kHidden; l.b3 = l.w3 + out_ * kHidden; l.P = l.b3 + out_;
+    return l;
+  }
+};
+
+// One launch runs every sequence of every network for all of its steps.  plan: slot lists of the networks, units_per_agent = B (training:
+// one sequence per sampled episode and agent) or E (act step), unit_rows = steps per sequence (T + 1, or 1).  src: mode 1 gathers
+// through the replay indices, mode 0 reads dense obs [E][N][D].
+struct GruFwdParams {
+  RowPlan plan; RowSource src;
+  const float* theta; GruLayout lay;
+  const float* h_in;   // mode 0: [E][N][128] initial state (NULL: zeros); mode 1: always zeros (the reference's hiddens=None)
+  float* h_out;        // mode 0: [E][N][128] final state (NULL: not written)
+  float* q_out;        // mode 0: [E][N][A]; mode 1: [N][B][T+1][A]
+  float* save;         // mode 1, online pass: [N][B][T+1][kGruSaveRow] for the backward (NULL: not saved)
+};
+
+// BPTT from dL/dq of the taken actions.  CTA c of net k (plan.cta_begin) owns a contiguous run of that net's sequences and writes the
+// gradient sums of all eight tensors into scratch[c][0 .. P) in fixed order.
+struct GruBwdParams {
+  RowPlan plan; TrajView traj; const int32_t* idx; int B;
+  const float* theta; GruLayout lay;
+  const float* save;                    // the online pass's saved rows
+  const float* td; int td_agent_stride; // 2 * delta * filled at [agent * stride + b * T + t]
+  float* scratch; int scratch_pitch;
+};
+
+int gru_kernels_init();
+int launch_gru_forward(const GruFwdParams& p, cudaStream_t st);
+int launch_gru_backward(const GruBwdParams& p, cudaStream_t st);
+
+}  // namespace marl

@@ -75,14 +75,50 @@ def state_dict_to_flat(sd, prefix, n_nets):
     return torch.cat([p.float() for p in parts])
 
 
+def rnn_shapes(in_dim, out_dim):
+    """RNNNetwork with layers=[128, 128] (utils/models.py:51-116): (state_dict name, shape) in the reference's order."""
+    H3 = 3 * HIDDEN
+    return (("first_layer.weight", (HIDDEN, in_dim)), ("first_layer.bias", (HIDDEN,)), ("rnn.weight_ih_l0", (H3, HIDDEN)),
+            ("rnn.weight_hh_l0", (H3, HIDDEN)), ("rnn.bias_ih_l0", (H3,)), ("rnn.bias_hh_l0", (H3,)),
+            ("final_layer.weight", (out_dim, HIDDEN)), ("final_layer.bias", (out_dim,)))
+
+
+def init_flat_rnn_params(n_nets, in_dim, out_dim, use_orthogonal_init=True):
+    """RNNNetwork.__init__ (host side, once): first_layer and the GRU keep PyTorch's default initialisation; use_orthogonal_init applies to
+    final_layer only (orthogonal, gain sqrt 2, zero bias).  Modules are created in the reference's order, so the RNG stream matches."""
+    parts = []
+    for _ in range(n_nets):
+        first, gru, final = torch.nn.Linear(in_dim, HIDDEN), torch.nn.GRU(HIDDEN, HIDDEN, num_layers=1), torch.nn.Linear(HIDDEN, out_dim)
+        if use_orthogonal_init:
+            torch.nn.init.orthogonal_(final.weight.data, gain=math.sqrt(2))
+            torch.nn.init.constant_(final.bias.data, 0)
+        for t in (first.weight, first.bias, gru.weight_ih_l0, gru.weight_hh_l0, gru.bias_ih_l0, gru.bias_hh_l0, final.weight, final.bias):
+            parts.append(t.data.reshape(-1))
+    return torch.cat(parts).float()
+
+
+def flat_to_rnn_state_dict(flat, prefix, n_nets, in_dim, out_dim):
+    sd, o = OrderedDict(), 0
+    for k in range(n_nets):
+        for name, shape in rnn_shapes(in_dim, out_dim):
+            n = int(np.prod(shape))
+            sd[f"{prefix}.{k}.{name}"] = flat[o:o + n].view(*shape).clone()
+            o += n
+    return sd
+
+
+def rnn_state_dict_to_flat(sd, prefix, n_nets, in_dim, out_dim):
+    return torch.cat([sd[f"{prefix}.{k}.{name}"].reshape(-1).float() for k in range(n_nets) for name, _ in rnn_shapes(in_dim, out_dim)])
+
+
 class QNetwork:
     mixer = 0
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch=None, max_episode_length=None):
-        if use_rnn:
-            raise NotImplementedError("use_rnn=True (GRU) is out of scope of the GPU hot path (every shipped config has use_rnn: False)")
+        self.use_rnn = bool(use_rnn)
         if list(layers) != [HIDDEN, HIDDEN]:
-            raise NotImplementedError(f"layers={list(layers)}: the fused kernels implement the shipped [128, 128] MLP only")
+            raise NotImplementedError(f"layers={list(layers)}: the fused kernels implement the shipped [128, 128] network only "
+                                      f"({'one 128-wide GRU layer' if use_rnn else 'MLP'})")
         opt = getattr(cfg, "optimizer", "Adam")
         if (opt if isinstance(opt, str) else opt.__name__) != "Adam":
             raise NotImplementedError("only optimizer=Adam is implemented")
@@ -108,15 +144,17 @@ class QNetwork:
                        0.9, 0.999, 1e-8, self.mixer)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            nat.check(self._lib.marl_dqn_create(C.byref(mcfg), C.byref(hp), C.c_int32(self.max_batch), C.c_int32(self.max_T), C.c_int32(self.device.index),
-                                                C.byref(self._h)), "marl_dqn_create")
+            create = self._lib.marl_dqn_create_rnn if self.use_rnn else self._lib.marl_dqn_create
+            nat.check(create(C.byref(mcfg), C.byref(hp), C.c_int32(self.max_batch), C.c_int32(self.max_T), C.c_int32(self.device.index),
+                             C.byref(self._h)), "marl_dqn_create_rnn" if self.use_rnn else "marl_dqn_create")
         ptrs = [C.c_void_p() for _ in range(5)]
         n = C.c_int64()
         nat.check(self._lib.marl_dqn_param_ptrs(self._h, *[C.byref(p) for p in ptrs], C.byref(n)), "marl_dqn_param_ptrs")
         self.n_params = int(n.value)
         self.theta, self.theta_tgt, self.adam_m, self.adam_v = [nat.device_view(p.value, self.n_params, self.device) for p in ptrs[:4]]
         self.grad = nat.device_view(ptrs[4].value, self.n_params + 4, self.device)  # + (loss numerator, filled count, 2 spare)
-        self.theta.copy_(init_flat_params(self.n_nets, self.in_dim, self.n_actions, use_orthogonal_init))
+        init = init_flat_rnn_params if self.use_rnn else init_flat_params
+        self.theta.copy_(init(self.n_nets, self.in_dim, self.n_actions, use_orthogonal_init))
         self.params_changed()
         self.hard_update()
         self._metrics = torch.zeros(6, dtype=torch.float32, device=self.device)
@@ -134,15 +172,26 @@ class QNetwork:
 
     # ---- reference API ------------------------------------------------------------------------------------------
     def init_hiddens(self, batch_size):
-        return [None] * self.n_agents
+        """utils/models.py:98-103: zeros (num_layers=1, batch, 128) per agent for recurrent networks, None per agent otherwise."""
+        if not self.use_rnn:
+            return [None] * self.n_agents
+        return [torch.zeros(1, batch_size, HIDDEN, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
 
-    def q_values(self, obs: torch.Tensor, target: bool = False, out: torch.Tensor | None = None) -> torch.Tensor:
-        """Network pass of model.act (dqn/model.py:96-99) for E envs: obs f32[E,N,D] -> q f32[E,N,A]."""
+    def q_values(self, obs: torch.Tensor, target: bool = False, out: torch.Tensor | None = None, h: torch.Tensor | None = None,
+                 h_out: torch.Tensor | None = None):
+        """Network pass of model.act (dqn/model.py:96-99) for E envs: obs f32[E,N,D] -> q f32[E,N,A].
+        Recurrent networks take one step from h f32[E,N,128] (None: the zero state) and return (q, h_out); h_out must not be h."""
         E = obs.shape[0]
         if out is None:
             out = torch.empty(E, self.n_agents, self.n_actions, dtype=torch.float32, device=self.device)
-        nat.check(self._lib.marl_dqn_forward(self._h, nat.ptr(obs), C.c_int32(E), C.c_int32(int(target)), nat.ptr(out), nat.stream_ptr()), "marl_dqn_forward")
-        return out
+        if not self.use_rnn:
+            nat.check(self._lib.marl_dqn_forward(self._h, nat.ptr(obs), C.c_int32(E), C.c_int32(int(target)), nat.ptr(out), nat.stream_ptr()), "marl_dqn_forward")
+            return out
+        if h_out is None:
+            h_out = torch.empty(E, self.n_agents, HIDDEN, dtype=torch.float32, device=self.device)
+        nat.check(self._lib.marl_dqn_forward_rnn(self._h, nat.ptr(obs), C.c_int32(E), C.c_int32(int(target)), nat.ptr(h), nat.ptr(h_out), nat.ptr(out),
+                                                 nat.stream_ptr()), "marl_dqn_forward_rnn")
+        return out, h_out
 
     def act(self, inputs, hiddens, epsilon, action_masks=None):
         """dqn/model.py:94-116 for API parity (single env or a stack of envs).  The training / evaluation loops use the fused
@@ -151,7 +200,14 @@ class QNetwork:
             raise NotImplementedError("action masks only exist for smaclite in the reference (out of scope)")
         obs = torch.as_tensor(np.stack([np.asarray(i, np.float32) for i in inputs], 0), device=self.device)
         obs = obs.view(self.n_agents, -1, self.in_dim).transpose(0, 1).contiguous()
-        q = self.q_values(obs)
+        if self.use_rnn:   # hiddens: per agent (1, E, 128) or None (dqn/model.py:99 carries them through the critic)
+            h = None
+            if hiddens is not None and not all(x is None for x in hiddens):
+                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, HIDDEN) for x in hiddens], 1).float().contiguous()
+            q, h_out = self.q_values(obs, h=h)
+            hiddens = [h_out[:, i].unsqueeze(0).clone() for i in range(self.n_agents)]
+        else:
+            q = self.q_values(obs)
         # the reference's stream: ONE `random.random()` per call decides the joint exploration (dqn/model.py:105), the random joint
         # action comes from Python's `random` as well (seed it with random.seed, as the reference's users do)
         if epsilon > random.random():
@@ -204,6 +260,8 @@ class QNetwork:
     def attach_peers(self, group=None):
         """Several ranks, one process per GPU: exchange CUDA IPC handles through torch.distributed and let `update` / `update_n` sum
         the gradients of all ranks over NVLink peer memory inside the fused reduce + Adam kernel (no all-reduce call per update)."""
+        if self.use_rnn:
+            raise NotImplementedError("recurrent agent networks run on one GPU: the peer-memory gradient exchange covers the MLP learners only")
         import torch.distributed as dist
 
         world, rank = dist.get_world_size(group), dist.get_rank(group)
@@ -242,13 +300,18 @@ class QNetwork:
         nat.check(self._lib.marl_dqn_params_changed(self._h), "marl_dqn_params_changed")
 
     def state_dict(self):
-        sd = flat_to_state_dict(self.theta.detach().cpu(), f"critic.{self._kind}", self.n_nets, self.in_dim, self.n_actions)
-        sd.update(flat_to_state_dict(self.theta_tgt.detach().cpu(), f"target.{self._kind}", self.n_nets, self.in_dim, self.n_actions))
+        to_sd = flat_to_rnn_state_dict if self.use_rnn else flat_to_state_dict
+        sd = to_sd(self.theta.detach().cpu(), f"critic.{self._kind}", self.n_nets, self.in_dim, self.n_actions)
+        sd.update(to_sd(self.theta_tgt.detach().cpu(), f"target.{self._kind}", self.n_nets, self.in_dim, self.n_actions))
         return sd
 
     def load_state_dict(self, sd):
-        self.theta.copy_(state_dict_to_flat(sd, f"critic.{self._kind}", self.n_nets))
-        self.theta_tgt.copy_(state_dict_to_flat(sd, f"target.{self._kind}", self.n_nets))
+        if self.use_rnn:
+            for dst, prefix in ((self.theta, "critic"), (self.theta_tgt, "target")):
+                dst.copy_(rnn_state_dict_to_flat(sd, f"{prefix}.{self._kind}", self.n_nets, self.in_dim, self.n_actions))
+        else:
+            self.theta.copy_(state_dict_to_flat(sd, f"critic.{self._kind}", self.n_nets))
+            self.theta_tgt.copy_(state_dict_to_flat(sd, f"target.{self._kind}", self.n_nets))
         self.params_changed()
 
     def parameters(self):

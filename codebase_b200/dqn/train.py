@@ -70,12 +70,21 @@ class Collector:
         self.env, self.model, self.T = env.native, model, int(time_limit)
         self.proper, self.clear_stale = bool(use_proper_termination), bool(clear_stale)
         self.q = torch.empty(self.env.E, self.env.N, model.n_actions, dtype=torch.float32, device=self.env.device)
+        # recurrent networks: two [E][N][128] hidden-state buffers used in turn (step input, step output)
+        self.rnn = bool(getattr(model, "use_rnn", False))
+        if self.rnn:
+            self.h = [torch.zeros(self.env.E, self.env.N, 128, dtype=torch.float32, device=self.env.device) for _ in range(2)]
 
     def collect(self, rb: TrajStore | None, slot0: int, epsilon: float):
         env = self.env
         env.reset(traj=rb, slot0=slot0)
-        for _ in range(self.T):
-            self.model.q_values(env.obs, out=self.q)
+        if self.rnn:   # every env starts a new episode here: the reference's init_hiddens at each episode start (dqn/train.py:210)
+            self.h[0].zero_()
+        for t in range(self.T):
+            if self.rnn:
+                self.model.q_values(env.obs, out=self.q, h=self.h[t & 1], h_out=self.h[(t + 1) & 1])
+            else:
+                self.model.q_values(env.obs, out=self.q)
             env.rollout_step(self.q, policy=1, epsilon=epsilon, traj=rb, slot0=slot0, use_proper_termination=self.proper, clear_stale=self.clear_stale)
         return env.final_len, env.final_ret  # device tensors: every env finished exactly one episode
 

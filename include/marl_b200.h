@@ -242,6 +242,22 @@ int marl_dqn_timing(marl_dqn* q, int32_t enable, float* total_ms, int32_t* count
 int marl_dqn_timing_kernels(marl_dqn* q, float* ms3, int32_t* count);
 int marl_dqn_set_counters(marl_dqn* q, int64_t updates, int64_t last_target_update);
 
+/* Recurrent agent networks (algorithm.model.use_rnn=True; marlbase/utils/models.py:51-130, RNNNetwork with layers = [128, 128]):
+ * first_layer Linear(in, 128) + ReLU, nn.GRU(128, 128, num_layers=1) (gate order r, z, n), final_layer Linear(128, out), no activation
+ * between the GRU and final_layer.  marl_dqn_create_rnn returns the same handle type; marl_dqn_param_ptrs then exposes [n_nets][P] floats,
+ * per network in the reference's state_dict order: first_layer.weight [128][in], first_layer.bias [128], rnn.weight_ih_l0 [384][128],
+ * rnn.weight_hh_l0 [384][128], rnn.bias_ih_l0 [384], rnn.bias_hh_l0 [384], final_layer.weight [out][128], final_layer.bias [out].
+ * Training runs every sampled episode from a zero hidden state (dqn/model.py:127,133).  marl_dqn_update / _update_n / _update_grads +
+ * _update_apply, standardise_returns, qmix_init, sync_target, the counters and marl_dqn_timing work unchanged (the timed window covers the
+ * online sequence forward, the TD head and the backward; marl_dqn_timing_kernels reports count 0).  The "tensor_core_*" options do not apply
+ * to recurrent handles (FP32 FFMA throughout); marl_dqn_forward and marl_dqn_peer_attach refuse them; in_dim <= 32. */
+int marl_dqn_create_rnn(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device,
+                        marl_dqn** out);
+/* One step of model.act's network pass (dqn/model.py:96-99) for E envs: obs device float[E][N][in], h_in / h_out device float[E][N][128]
+ * (h_in == NULL: the zero state of init_hiddens; h_out == NULL: not written) -> q_out float[E][N][out].  h_in and h_out must not alias. */
+int marl_dqn_forward_rnn(marl_dqn* q, const float* obs, int32_t n_envs, int32_t use_target, const float* h_in, float* h_out,
+                         float* q_out, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------
  * Independent actor-critic learner (IA2C).  Replaces marlbase/ac/model.py A2CNetwork (22-246) with a
  * decentralised critic (ia2c.yaml:18), independent or shared per-agent networks.
