@@ -1,9 +1,11 @@
 """Independent actor-critic learner on the GPU path -- drop-in for marlbase/ac/model.py A2CNetwork (22-246).
 
 Same constructor signature / Hydra `_target_` role (configs/algorithm/ia2c.yaml:8-26) and the reference's
-`state_dict()` key names (`actor.independent.{i}.network.…`, `critic.…`, `target_critic.…`; shared: `.networks.{k}.`).
+`state_dict()` key names (`actor.independent.{i}.network.…`, `critic.…`, `target_critic.…`; shared: `.networks.{k}.`; recurrent parts:
+`actor.independent.{i}.first_layer.weight`, `….rnn.weight_ih_l0`, …).
 All arithmetic runs in libmarlb200.so (marl_a2c_*): actor forward, target-critic pass, n-step returns
 (utils/utils.py:38-63), fused forward / loss / backward of critic and actor, Adam, target sync.  No CPU fallback.
+`actor.use_rnn` / `critic.use_rnn` make that part the reference's RNNNetwork (one 128-wide GRU layer), independently of each other.
 """
 from __future__ import annotations
 
@@ -12,17 +14,18 @@ import ctypes as C
 import torch
 
 from .. import _native as nat
-from ..dqn.model import HIDDEN, _dim, flat_to_state_dict, init_flat_params, sharing_to_nets, state_dict_to_flat
+from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dict, init_flat_params, init_flat_rnn_params, rnn_state_dict_to_flat,
+                         sharing_to_nets, state_dict_to_flat)
 from ..lbf import TrajStore
 
 
 class A2CNetwork:
     def __init__(self, obs_space, action_space, cfg, actor, critic, device, max_envs=None, max_episode_length=None):
         for part, name in ((actor, "actor"), (critic, "critic")):
-            if part.use_rnn:
-                raise NotImplementedError(f"{name}.use_rnn=True (GRU) is out of scope of the GPU hot path")
             if list(part.layers) != [HIDDEN, HIDDEN]:
-                raise NotImplementedError(f"{name}.layers={list(part.layers)}: the fused kernels implement the shipped [128, 128] MLP only")
+                raise NotImplementedError(f"{name}.layers={list(part.layers)}: the fused kernels implement the shipped [128, 128] network only "
+                                          f"({'one 128-wide GRU layer' if part.use_rnn else 'MLP'})")
+        self.actor_rnn, self.critic_rnn = bool(actor.use_rnn), bool(critic.use_rnn)
         opt = getattr(cfg, "optimizer", "Adam")
         if (opt if isinstance(opt, str) else opt.__name__) != "Adam":
             raise NotImplementedError("only optimizer=Adam is implemented")
@@ -57,8 +60,13 @@ class A2CNetwork:
                        self.target_update_interval_or_tau, 0.9, 0.999, 1e-8)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
-            nat.check(self._lib.marl_a2c_create(C.byref(acfg), C.byref(ccfg), C.byref(hp), C.c_int32(self.max_envs), C.c_int32(self.max_T),
-                                                C.c_int32(self.device.index), C.byref(self._h)), "marl_a2c_create")
+            if self.actor_rnn or self.critic_rnn:
+                nat.check(self._lib.marl_a2c_create_rnn(C.byref(acfg), C.byref(ccfg), C.byref(hp), C.c_int32(int(self.actor_rnn)), C.c_int32(int(self.critic_rnn)),
+                                                        C.c_int32(self.max_envs), C.c_int32(self.max_T), C.c_int32(self.device.index), C.byref(self._h)),
+                          "marl_a2c_create_rnn")
+            else:
+                nat.check(self._lib.marl_a2c_create(C.byref(acfg), C.byref(ccfg), C.byref(hp), C.c_int32(self.max_envs), C.c_int32(self.max_T),
+                                                    C.c_int32(self.device.index), C.byref(self._h)), "marl_a2c_create")
         ptrs = [C.c_void_p() for _ in range(5)]
         na, nc = C.c_int64(), C.c_int64()
         nat.check(self._lib.marl_a2c_param_ptrs(self._h, *[C.byref(p) for p in ptrs], C.byref(na), C.byref(nc)), "marl_a2c_param_ptrs")
@@ -68,8 +76,11 @@ class A2CNetwork:
         self.theta_tgt = nat.device_view(ptrs[1].value, self.n_critic, self.device)
         self.adam_m, self.adam_v = nat.device_view(ptrs[2].value, n, self.device), nat.device_view(ptrs[3].value, n, self.device)
         self.grad = nat.device_view(ptrs[4].value, n + 4, self.device)
-        self.theta[: self.n_actor].copy_(init_flat_params(self.n_actor_nets, self.in_dim, self.n_actions, actor.use_orthogonal_init))
-        self.theta[self.n_actor:].copy_(init_flat_params(self.n_critic_nets, self.critic_in, 1, critic.use_orthogonal_init))
+        # each part by its own rule (RNNNetwork: orthogonal on final_layer only), actor first as the reference creates them
+        init_a = init_flat_rnn_params if self.actor_rnn else init_flat_params
+        init_c = init_flat_rnn_params if self.critic_rnn else init_flat_params
+        self.theta[: self.n_actor].copy_(init_a(self.n_actor_nets, self.in_dim, self.n_actions, actor.use_orthogonal_init))
+        self.theta[self.n_actor:].copy_(init_c(self.n_critic_nets, self.critic_in, 1, critic.use_orthogonal_init))
         self.soft_update(1.0)
         self._metrics = torch.zeros(6, dtype=torch.float32, device=self.device)
         self.standardise_returns = bool(getattr(cfg, "standardise_returns", False))   # ac/model.py:112-114
@@ -103,34 +114,63 @@ class A2CNetwork:
                 nat.device_view(ptrs[2].value, N * n_envs * T, self.device).view(N, n_envs, T))
 
     # ---- reference API ------------------------------------------------------------------------------------------------
+    def _hiddens(self, recurrent, batch_size):
+        """utils/models.py:98-103: zeros (num_layers=1, batch, 128) per agent for a recurrent part, None per agent otherwise."""
+        if not recurrent:
+            return [None] * self.n_agents
+        return [torch.zeros(1, batch_size, HIDDEN, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
+
     def init_actor_hiddens(self, batch_size):
-        return [None] * self.n_agents
+        return self._hiddens(self.actor_rnn, batch_size)
 
     def init_critic_hiddens(self, batch_size, target=False):
-        return [None] * self.n_agents
+        return self._hiddens(self.critic_rnn, batch_size)
 
-    def logits(self, obs: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
-        """Actor pass of act (ac/model.py:148-150): obs f32[E,N,D] -> logits f32[E,N,A]."""
+    def _forward_rnn(self, which, obs, out, h, h_out):
+        if h_out is None:
+            h_out = torch.empty(obs.shape[0], self.n_agents, HIDDEN, dtype=torch.float32, device=self.device)
+        nat.check(self._lib.marl_a2c_forward_rnn(self._h, C.c_int32(which), nat.ptr(obs), C.c_int32(obs.shape[0]), nat.ptr(h), nat.ptr(h_out), nat.ptr(out),
+                                                 nat.stream_ptr()), "marl_a2c_forward_rnn")
+        return out, h_out
+
+    def logits(self, obs: torch.Tensor, out: torch.Tensor | None = None, h: torch.Tensor | None = None, h_out: torch.Tensor | None = None):
+        """Actor pass of act (ac/model.py:148-150): obs f32[E,N,D] -> logits f32[E,N,A].
+        A recurrent actor takes one step from h f32[E,N,128] (None: the zero state) and returns (logits, h_out); h_out must not be h."""
         E = obs.shape[0]
         if out is None:
             out = torch.empty(E, self.n_agents, self.n_actions, dtype=torch.float32, device=self.device)
+        if self.actor_rnn:
+            return self._forward_rnn(0, obs, out, h, h_out)
         nat.check(self._lib.marl_a2c_forward_actor(self._h, nat.ptr(obs), C.c_int32(E), nat.ptr(out), nat.stream_ptr()), "marl_a2c_forward_actor")
         return out
 
-    def values(self, obs: torch.Tensor, target: bool = False) -> torch.Tensor:
-        """get_value (ac/model.py:155-163): obs f32[E,N,D] -> f32[E,N] (centralised critic: each agent's network reads all N x D values of its env)."""
+    def values(self, obs: torch.Tensor, target: bool = False, h: torch.Tensor | None = None, h_out: torch.Tensor | None = None):
+        """get_value (ac/model.py:155-163): obs f32[E,N,D] -> f32[E,N] (centralised critic: each agent's network reads all N x D values of its env).
+        A recurrent critic takes one step from h f32[E,N,128] (None: the zero state) and returns (values, h_out)."""
         E = obs.shape[0]
         out = torch.empty(E, self.n_agents, 1, dtype=torch.float32, device=self.device)
+        if self.critic_rnn:
+            v, h_out = self._forward_rnn(2 if target else 1, obs, out, h, h_out)
+            return v.squeeze(-1), h_out
         nat.check(self._lib.marl_a2c_forward_critic(self._h, nat.ptr(obs), C.c_int32(E), C.c_int32(int(target)), nat.ptr(out), nat.stream_ptr()), "marl_a2c_forward_critic")
         return out.squeeze(-1)
 
     def act(self, inputs, actor_hiddens, action_mask=None):
         """ac/model.py:147-153 for API parity: list of N tensors [P, obs] -> i64[N, P, 1].  The training loop uses the fused
-        marl_lbf_rollout_step(policy=2) which samples from the Philox stream inside the env kernel."""
+        marl_lbf_rollout_step(policy=2) which samples from the Philox stream inside the env kernel.  A recurrent actor carries actor_hiddens
+        (per agent (1, P, 128) or None) and returns the new ones."""
         if action_mask is not None:
             raise NotImplementedError("action masks only exist for smaclite in the reference (out of scope)")
         obs = torch.stack([torch.as_tensor(i, dtype=torch.float32, device=self.device) for i in inputs], 1).contiguous()
-        dist = torch.distributions.Categorical(logits=self.logits(obs))
+        if self.actor_rnn:
+            h = None
+            if actor_hiddens is not None and not all(x is None for x in actor_hiddens):
+                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, HIDDEN) for x in actor_hiddens], 1).float().contiguous()
+            logits, h_out = self.logits(obs, h=h)
+            actor_hiddens = [h_out[:, i].unsqueeze(0).clone() for i in range(self.n_agents)]
+        else:
+            logits = self.logits(obs)
+        dist = torch.distributions.Categorical(logits=logits)
         return dist.sample().T.unsqueeze(-1).contiguous(), actor_hiddens
 
     def update_from_store(self, batch: TrajStore, n_envs: int, step: int):
@@ -171,15 +211,22 @@ class A2CNetwork:
 
     def state_dict(self):
         th, tg = self.theta.detach().cpu(), self.theta_tgt.detach().cpu()
-        sd = flat_to_state_dict(th[: self.n_actor], f"actor.{self._akind}", self.n_actor_nets, self.in_dim, self.n_actions)
-        sd.update(flat_to_state_dict(th[self.n_actor:], f"critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1))
-        sd.update(flat_to_state_dict(tg, f"target_critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1))
+        to_a = flat_to_rnn_state_dict if self.actor_rnn else flat_to_state_dict
+        to_c = flat_to_rnn_state_dict if self.critic_rnn else flat_to_state_dict
+        sd = to_a(th[: self.n_actor], f"actor.{self._akind}", self.n_actor_nets, self.in_dim, self.n_actions)
+        sd.update(to_c(th[self.n_actor:], f"critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1))
+        sd.update(to_c(tg, f"target_critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1))
         return sd
 
     def load_state_dict(self, sd):
-        self.theta[: self.n_actor].copy_(state_dict_to_flat(sd, f"actor.{self._akind}", self.n_actor_nets))
-        self.theta[self.n_actor:].copy_(state_dict_to_flat(sd, f"critic.{self._ckind}", self.n_critic_nets))
-        self.theta_tgt.copy_(state_dict_to_flat(sd, f"target_critic.{self._ckind}", self.n_critic_nets))
+        def flat(prefix, recurrent, n_nets, in_dim, out_dim):
+            if recurrent:
+                return rnn_state_dict_to_flat(sd, prefix, n_nets, in_dim, out_dim)
+            return state_dict_to_flat(sd, prefix, n_nets)
+
+        self.theta[: self.n_actor].copy_(flat(f"actor.{self._akind}", self.actor_rnn, self.n_actor_nets, self.in_dim, self.n_actions))
+        self.theta[self.n_actor:].copy_(flat(f"critic.{self._ckind}", self.critic_rnn, self.n_critic_nets, self.critic_in, 1))
+        self.theta_tgt.copy_(flat(f"target_critic.{self._ckind}", self.critic_rnn, self.n_critic_nets, self.critic_in, 1))
 
     def parameters(self):
         return [self.theta]

@@ -30,6 +30,10 @@ class Collector:
         self.env, self.model, self.T, self.proper = envs.native, model, int(time_limit), bool(use_proper_termination)
         self.batch = TrajStore(self.env.E, self.env.N, self.T, self.env.D, self.env.device)
         self.logits = torch.empty(self.env.E, self.env.N, model.n_actions, dtype=torch.float32, device=self.env.device)
+        # recurrent actor: two [E][N][128] hidden-state buffers used in turn (step input, step output)
+        self.rnn = bool(getattr(model, "actor_rnn", False))
+        if self.rnn:
+            self.h = [torch.zeros(self.env.E, self.env.N, 128, dtype=torch.float32, device=self.env.device) for _ in range(2)]
 
     def collect(self):
         env, b = self.env, self.batch
@@ -37,8 +41,13 @@ class Collector:
         # early episode end must read as reward 0 / zero observation, not as the previous batch's longer episode in the same slot
         b.obs.zero_(); b.act.zero_(); b.rew.zero_(); b.filled.zero_(); b.done.zero_()
         env.reset(traj=b, slot0=0)
-        for _ in range(self.T):
-            self.model.logits(env.obs, out=self.logits)
+        if self.rnn:   # every env starts its episode here: init_actor_hiddens at the start of each collection (ac/train.py:69-77)
+            self.h[0].zero_()
+        for t in range(self.T):
+            if self.rnn:
+                self.model.logits(env.obs, out=self.logits, h=self.h[t & 1], h_out=self.h[(t + 1) & 1])
+            else:
+                self.model.logits(env.obs, out=self.logits)
             env.rollout_step(self.logits, policy=2, traj=b, slot0=0, use_proper_termination=self.proper)
         return env.final_len, env.final_ret
 

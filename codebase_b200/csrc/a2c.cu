@@ -4,7 +4,11 @@
 // update (189-246: target-critic pass, compute_nstep_returns utils/utils.py:38-63, evaluate_actions 165-182,
 // policy-gradient + entropy + value losses, Adam, target sync), for independent or shared per-agent networks with a
 // decentralised critic (critic.centralised: False, configs/algorithm/ia2c.yaml:18).
-#include "learner.cuh"
+//
+// Recurrent parts (marl_a2c_create_rnn; actor.use_rnn / critic.use_rnn, utils/models.py:51-116): every pass runs each env's episode from h = 0
+// (ac/model.py:189-246, 265-352 call the networks with hiddens=None) through gru_forward; a trained part then runs the sequence loss head and the
+// BPTT backward (gru_kernels.cu) into the same per-CTA partials and reduce + Adam tail as the MLP parts.
+#include "gru.cuh"
 #include "retms.cuh"
 #include <math.h>
 #include <vector>
@@ -105,6 +109,10 @@ struct marl_a2c {
   // standardise_returns: RunningMeanStd(shape=(n_agents,)) -- mean[N] | var[N] (float32), count (a Python float in the reference), partial sums
   int standardise = 0; float* ret_ms = nullptr; double* ret_count = nullptr; double* ret_part = nullptr;
   int centralised = 0; float* joint = nullptr;   // critic.centralised: joint observations of the batch [P][T+1][N * D]
+  // recurrent parts: GRU layouts, the sequence outputs of the part being trained and their gradient [N][P][T+1][out], the online pass's saved rows
+  // [N][P][T+1][kGruSaveRow] (one buffer: the critic pass ends before the actor pass starts)
+  int actor_rnn = 0, critic_rnn = 0; GruLayout agl = {}, cgl = {};
+  float *rnn_q = nullptr, *rnn_dq = nullptr, *gru_save = nullptr;
 };
 constexpr int kMaxPpoEpochs = 64;
 
@@ -116,11 +124,13 @@ int marl_a2c_destroy(marl_a2c* h) {
   cudaFree(h->theta); cudaFree(h->theta_tgt); cudaFree(h->m); cudaFree(h->v); cudaFree(h->grad); cudaFree(h->scratch); cudaFree(h->loss_part);
   cudaFree(h->vt); cudaFree(h->ret); cudaFree(h->adv); cudaFree(h->metrics); cudaFree(h->idx); cudaFree(h->image);
   cudaFree(h->logits_all); cudaFree(h->old_logp); cudaFree(h->epoch_metrics); cudaFree(h->ret_ms); cudaFree(h->ret_count); cudaFree(h->ret_part); cudaFree(h->joint);
+  cudaFree(h->rnn_q); cudaFree(h->rnn_dq); cudaFree(h->gru_save);
   delete h;
   return MARL_OK;
 }
 
-int marl_a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, int32_t max_envs, int32_t max_T, int32_t device, marl_a2c** out) {
+static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, bool actor_rnn, bool critic_rnn, int32_t max_envs, int32_t max_T,
+                      int32_t device, marl_a2c** out) {
   MARL_REQUIRE(hp && out, "marl_a2c_create: NULL argument");
   *out = nullptr;
   if (int rc = check_mlp_cfg(actor, "marl_a2c_create(actor)")) return rc;
@@ -136,26 +146,48 @@ int marl_a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const
   h->hp = *hp; h->device = device; h->max_envs = max_envs; h->max_T = max_T;
   h->centralised = (critic->in_dim != actor->in_dim || (actor->n_agents == 1 && false)) ? 1 : 0;
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
-  h->n_actor = (int64_t)actor->n_nets * h->actor.lay.P; h->n_critic = (int64_t)critic->n_nets * h->critic.lay.P; h->n_params = h->n_actor + h->n_critic;
-  const int pmax = h->actor.lay.P > h->critic.lay.P ? h->actor.lay.P : h->critic.lay.P;
+  h->actor_rnn = actor_rnn ? 1 : 0; h->critic_rnn = critic_rnn ? 1 : 0;
+  h->agl = GruLayout::make(actor->in_dim, actor->out_dim); h->cgl = GruLayout::make(critic->in_dim, critic->out_dim);
+  const int pa = actor_rnn ? h->agl.P : h->actor.lay.P, pc = critic_rnn ? h->cgl.P : h->critic.lay.P;
+  h->n_actor = (int64_t)actor->n_nets * pa; h->n_critic = (int64_t)critic->n_nets * pc; h->n_params = h->n_actor + h->n_critic;
+  const int pmax = pa > pc ? pa : pc;
   h->scratch_pitch = (pmax + 3) & ~3;
   const size_t rows = (size_t)actor->n_agents * max_envs * (max_T + 1);
+  const bool rnn = actor_rnn || critic_rnn;
+  // the loss statistics: one part per training CTA of an MLP part, one per head block of a recurrent part
+  const size_t loss_parts = (size_t)h->n_sm + (rnn ? (size_t)gru_head_blocks(actor->n_agents, max_envs, max_T) : 0);
   int rc = 0;
   rc |= dev_alloc_zero(&h->theta, h->n_params); rc |= dev_alloc_zero(&h->theta_tgt, h->n_critic);
   rc |= dev_alloc_zero(&h->m, h->n_params); rc |= dev_alloc_zero(&h->v, h->n_params); rc |= dev_alloc_zero(&h->grad, h->n_params + 4);
-  rc |= dev_alloc_zero(&h->scratch, (size_t)h->n_sm * h->scratch_pitch); rc |= dev_alloc_zero(&h->loss_part, 4 * (size_t)h->n_sm);
+  rc |= dev_alloc_zero(&h->scratch, (size_t)h->n_sm * h->scratch_pitch); rc |= dev_alloc_zero(&h->loss_part, 4 * loss_parts);
   rc |= dev_alloc_zero(&h->vt, rows); rc |= dev_alloc_zero(&h->ret, rows); rc |= dev_alloc_zero(&h->adv, rows); rc |= dev_alloc_zero(&h->metrics, 8);
   rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->idx), max_envs);
   rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->image), (size_t)(actor->n_nets > critic->n_nets ? actor->n_nets : critic->n_nets) * tc_image_bytes() / 4 + 4);
+  if (rnn) {
+    const int out_max = actor_rnn ? actor->out_dim : 1;
+    rc |= dev_alloc_zero(&h->rnn_q, rows * out_max); rc |= dev_alloc_zero(&h->rnn_dq, rows * out_max); rc |= dev_alloc_zero(&h->gru_save, rows * kGruSaveRow);
+  }
   if (rc) { marl_a2c_destroy(h); return MARL_ENOMEM; }
   iota_kernel<<<(max_envs + 255) / 256, 256>>>(h->idx, max_envs);
   if (h->centralised && dev_alloc_zero(&h->joint, (size_t)max_envs * (max_T + 1) * critic->in_dim)) { marl_a2c_destroy(h); return MARL_ENOMEM; }
   if (int rc2 = learner_kernels_init(actor->in_dim)) { marl_a2c_destroy(h); return rc2; }
   if (int rc2 = learner_kernels_init(critic->in_dim)) { marl_a2c_destroy(h); return rc2; }
   if (int rc2 = tc_forward_init()) { marl_a2c_destroy(h); return rc2; }
+  if (rnn) {
+    if (int rc2 = gru_kernels_init()) { marl_a2c_destroy(h); return rc2; }
+  }
   if (cudaDeviceSynchronize() != cudaSuccess) { set_error("marl_a2c_create: device error during setup"); marl_a2c_destroy(h); return MARL_ECUDA; }
   *out = h;
   return MARL_OK;
+}
+
+int marl_a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, int32_t max_envs, int32_t max_T, int32_t device, marl_a2c** out) {
+  return a2c_create(actor, critic, hp, false, false, max_envs, max_T, device, out);
+}
+
+int marl_a2c_create_rnn(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, int32_t actor_rnn, int32_t critic_rnn, int32_t max_envs,
+                        int32_t max_T, int32_t device, marl_a2c** out) {
+  return a2c_create(actor, critic, hp, actor_rnn != 0, critic_rnn != 0, max_envs, max_T, device, out);
 }
 
 /* theta = [actor nets | critic nets] (flat, reference state_dict order per net), theta_tgt = target critic. */
@@ -191,16 +223,45 @@ static int a2c_dense_forward(marl_a2c* h, const NetSet& ns, const float* theta, 
 /* actor forward of A2CNetwork.act (ac/model.py:148-150): obs float[E][N][in] -> logits float[E][N][n_actions] */
 int marl_a2c_forward_actor(marl_a2c* h, const float* obs, int32_t n_envs, float* logits_out, void* stream) {
   MARL_REQUIRE(h && obs && logits_out && n_envs >= 1, "marl_a2c_forward_actor: bad argument");
+  MARL_REQUIRE(!h->actor_rnn, "marl_a2c_forward_actor: the actor is recurrent: use marl_a2c_forward_rnn, which carries the hidden state");
   return a2c_dense_forward(h, h->actor, h->theta, obs, n_envs, logits_out, stream);
 }
 
 /* get_value (ac/model.py:155-163): values float[E][N][1] from the critic or the target critic */
 int marl_a2c_forward_critic(marl_a2c* h, const float* obs, int32_t n_envs, int32_t use_target, float* values_out, void* stream) {
   MARL_REQUIRE(h && obs && values_out && n_envs >= 1, "marl_a2c_forward_critic: bad argument");
+  MARL_REQUIRE(!h->critic_rnn, "marl_a2c_forward_critic: the critic is recurrent: use marl_a2c_forward_rnn, which carries the hidden state");
   return a2c_dense_forward(h, h->critic, use_target ? h->theta_tgt : h->theta + h->n_actor, obs, n_envs, values_out, stream);
 }
 
-struct A2cPass { RowSource src, csrc; RowPlan cplan, aplan; };   // csrc: the critic's rows (== src unless the critic is centralised)
+/* one step of a recurrent part (ac/model.py:147-153 act, 155-163 get_value) carrying the hidden state; which: 0 actor, 1 critic, 2 target critic */
+int marl_a2c_forward_rnn(marl_a2c* h, int32_t which, const float* obs, int32_t n_envs, const float* h_in, float* h_out, float* out, void* stream) {
+  MARL_REQUIRE(h && obs && out && n_envs >= 1 && which >= 0 && which <= 2, "marl_a2c_forward_rnn: bad argument");
+  const bool actor = which == 0;
+  MARL_REQUIRE(actor ? h->actor_rnn : h->critic_rnn, "marl_a2c_forward_rnn: the %s is not recurrent: use marl_a2c_forward_%s", actor ? "actor" : "critic",
+               actor ? "actor" : "critic");
+  MARL_REQUIRE(h_in == nullptr || h_in != h_out, "marl_a2c_forward_rnn: h_in and h_out must not alias");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  const NetSet& ns = actor ? h->actor : h->critic;
+  GruFwdParams fp; memset(&fp, 0, sizeof(fp));
+  fp.plan = make_plan(ns, n_envs, 1, 1, 1);
+  fp.src.mode = 0; fp.src.dense = obs; fp.src.E = n_envs; fp.src.N = ns.n_agents; fp.src.D = ns.in;
+  if (!actor && h->centralised) { fp.src.mode = 3; fp.src.joint = obs; }   // obs float[E][N][D] read as the joint rows float[E][N * D]
+  fp.theta = which == 0 ? h->theta : (which == 1 ? h->theta + h->n_actor : h->theta_tgt);
+  fp.lay = actor ? h->agl : h->cgl;
+  fp.h_in = h_in; fp.h_out = h_out; fp.q_out = out;
+  return launch_gru_forward(fp, (cudaStream_t)stream);
+}
+
+struct A2cPass { RowSource src, csrc; RowPlan cplan, aplan; int n_envs; };   // csrc: the critic's rows (== src unless the critic is centralised)
+
+// sequence forward of a recurrent part over every env's T + 1 steps from h = 0: outputs [N][P][T+1][out], saved rows for BPTT when `save`
+static int a2c_gru_forward(const NetSet& ns, const GruLayout& gl, const RowSource& src, const float* theta, int n_envs, float* q_out, float* save, cudaStream_t st) {
+  GruFwdParams fp; memset(&fp, 0, sizeof(fp));
+  fp.plan = make_plan(ns, n_envs, src.traj.T + 1, 1, 1); fp.src = src;
+  fp.theta = theta; fp.lay = gl; fp.q_out = q_out; fp.save = save;
+  return launch_gru_forward(fp, st);
+}
 
 // target-critic pass + n-step returns (ac/model.py:190-201): everything of an update that does not depend on the trainable parameters
 static int a2c_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, cudaStream_t st, A2cPass& ps) {
@@ -212,6 +273,7 @@ static int a2c_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs,
   const int T = batch->T, N = h->actor.n_agents;
   const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
   memset(&ps.src, 0, sizeof(ps.src));
+  ps.n_envs = n_envs;
   ps.src.mode = 1; ps.src.traj = to_view(batch); ps.src.idx = h->idx; ps.src.N = N; ps.src.D = h->actor.in;
   ps.cplan = make_plan(h->critic, n_envs, T + 1, h->n_sm, min_units);
   ps.aplan = make_plan(h->actor, n_envs, T + 1, h->n_sm, min_units);
@@ -224,7 +286,11 @@ static int a2c_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs,
     ps.csrc.mode = 2; ps.csrc.joint = h->joint; ps.csrc.D = h->critic.in;
   }
   // 1. target critic on all T+1 observations (ac/model.py:190-193)
-  if (int rc = forward_any(h->critic, ps.cplan, ps.csrc, h->theta_tgt, h->image, h->vt, st)) return rc;
+  if (h->critic_rnn) {
+    if (int rc = a2c_gru_forward(h->critic, h->cgl, ps.csrc, h->theta_tgt, n_envs, h->vt, nullptr, st)) return rc;
+  } else {
+    if (int rc = forward_any(h->critic, ps.cplan, ps.csrc, h->theta_tgt, h->image, h->vt, st)) return rc;
+  }
   // 2. n-step returns (ac/model.py:198-201)
   NStepParams np; np.vt = h->vt; np.traj = ps.src.traj; np.idx = h->idx; np.N = N; np.P = n_envs; np.n_steps = h->hp.n_steps; np.ret = h->ret;
   np.ret_ms = h->standardise ? h->ret_ms : nullptr;
@@ -264,23 +330,51 @@ int marl_a2c_ret_ms_ptrs(marl_a2c* h, float** ret_ms, double** count) {
 }
 
 // critic and actor training passes -> grad[] (un-normalised sums) + loss statistics; old_logp != NULL: PPO's clipped surrogate
+// A recurrent part's training pass: sequence forward from h = 0 saving what BPTT needs (outputs of row T are not used: the GRU is causal, so this
+// equals the reference's pass over the first T observations), the loss head on rows t < T, BPTT from the dense dL/dout -> per-CTA gradient
+// partials in scratch and per-block loss statistics in loss_part.  Sets the reduction's plan, P and loss-part count in rp.
+static int a2c_rnn_part(marl_a2c* h, const NetSet& ns, const GruLayout& gl, const RowSource& src, const TrainParams& tp, int head, int n_envs, cudaStream_t st,
+                        ReduceParams& rp) {
+  const int T = src.traj.T;
+  if (int rc = a2c_gru_forward(ns, gl, src, tp.theta, n_envs, h->rnn_q, h->gru_save, st)) return rc;
+  GruHeadParams hp; hp.tp = tp; hp.traj = src.traj; hp.idx = h->idx; hp.N = ns.n_agents; hp.P = n_envs; hp.A = ns.out;
+  hp.q = h->rnn_q; hp.dq = h->rnn_dq; hp.loss_part = h->loss_part;
+  if (int rc = launch_gru_ac_head(hp, head, st)) return rc;
+  GruBwdParams bp; memset(&bp, 0, sizeof(bp));
+  bp.plan = make_plan(ns, n_envs, 1, h->n_sm, kGruSeqs); bp.traj = src.traj; bp.idx = h->idx; bp.B = n_envs; bp.theta = tp.theta; bp.lay = gl;
+  bp.save = h->gru_save; bp.src = src; bp.dout = h->rnn_dq; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
+  if (int rc = launch_gru_backward(bp, st)) return rc;
+  memcpy(rp.cta_begin, bp.plan.cta_begin, sizeof(rp.cta_begin));
+  rp.P = gl.P; rp.n_loss_parts = gru_head_blocks(ns.n_agents, n_envs, T);
+  return MARL_OK;
+}
+
 static int a2c_gradients(marl_a2c* h, const A2cPass& ps, cudaStream_t st, const float* old_logp, float ppo_clip) {
   // 3. critic: forward, value loss, backward; leaves advantage = returns - V for the actor pass
   TrainParams tp; memset(&tp, 0, sizeof(tp));
   tp.plan = ps.cplan; tp.src = ps.csrc; tp.theta = h->theta + h->n_actor; tp.lay = h->critic.lay; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch;
   tp.loss_part = h->loss_part; tp.returns = h->ret; tp.adv_out = h->adv; tp.value_coef = h->hp.value_loss_coef;
-  if (int rc = launch_train(tp, kHeadA2cCritic, st)) return rc;
   ReduceParams rp; memset(&rp, 0, sizeof(rp));  // (sumsq_part stays NULL: two passes write different gradient slices)
-  rp.scratch = h->scratch; rp.loss_part = h->loss_part; rp.n_nets = h->critic.n_nets; rp.P = h->critic.lay.P; rp.scratch_pitch = h->scratch_pitch;
-  memcpy(rp.cta_begin, ps.cplan.cta_begin, sizeof(rp.cta_begin));
-  rp.n_loss_parts = ps.cplan.cta_begin[ps.cplan.n_nets]; rp.grad = h->grad + h->n_actor; rp.stats = h->grad + h->n_params; rp.stats_accumulate = 0;
+  rp.scratch = h->scratch; rp.loss_part = h->loss_part; rp.n_nets = h->critic.n_nets; rp.scratch_pitch = h->scratch_pitch;
+  if (h->critic_rnn) {
+    if (int rc = a2c_rnn_part(h, h->critic, h->cgl, ps.csrc, tp, kHeadA2cCritic, ps.n_envs, st, rp)) return rc;
+  } else {
+    if (int rc = launch_train(tp, kHeadA2cCritic, st)) return rc;
+    rp.P = h->critic.lay.P; memcpy(rp.cta_begin, ps.cplan.cta_begin, sizeof(rp.cta_begin)); rp.n_loss_parts = ps.cplan.cta_begin[ps.cplan.n_nets];
+  }
+  rp.grad = h->grad + h->n_actor; rp.stats = h->grad + h->n_params; rp.stats_accumulate = 0;
   if (int rc = launch_grad_reduce(rp, st)) return rc;
   // 4. actor: forward, log-softmax, policy-gradient (or clipped surrogate) + entropy loss, backward
   tp.plan = ps.aplan; tp.src = ps.src; tp.theta = h->theta; tp.lay = h->actor.lay; tp.adv = h->adv; tp.entropy_coef = h->hp.entropy_coef;
   tp.old_logp = old_logp; tp.ppo_clip = ppo_clip;
-  if (int rc = launch_train(tp, kHeadA2cActor, st)) return rc;
-  rp.n_nets = h->actor.n_nets; rp.P = h->actor.lay.P; memcpy(rp.cta_begin, ps.aplan.cta_begin, sizeof(rp.cta_begin));
-  rp.n_loss_parts = ps.aplan.cta_begin[ps.aplan.n_nets]; rp.grad = h->grad; rp.stats_accumulate = 1;
+  rp.n_nets = h->actor.n_nets;
+  if (h->actor_rnn) {
+    if (int rc = a2c_rnn_part(h, h->actor, h->agl, ps.src, tp, kHeadA2cActor, ps.n_envs, st, rp)) return rc;
+  } else {
+    if (int rc = launch_train(tp, kHeadA2cActor, st)) return rc;
+    rp.P = h->actor.lay.P; memcpy(rp.cta_begin, ps.aplan.cta_begin, sizeof(rp.cta_begin)); rp.n_loss_parts = ps.aplan.cta_begin[ps.aplan.n_nets];
+  }
+  rp.grad = h->grad; rp.stats_accumulate = 1;
   return launch_grad_reduce(rp, st);
 }
 
@@ -328,7 +422,11 @@ int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, in
     if (rc) return MARL_ENOMEM;
   }
   // log-probabilities of the taken actions under the collecting policy = the current actor (ac/model.py:281-292)
-  if (int rc = forward_any(h->actor, ps.aplan, ps.src, h->theta, h->image, h->logits_all, st)) return rc;
+  if (h->actor_rnn) {
+    if (int rc = a2c_gru_forward(h->actor, h->agl, ps.src, h->theta, n_envs, h->logits_all, nullptr, st)) return rc;
+  } else {
+    if (int rc = forward_any(h->actor, ps.aplan, ps.src, h->theta, h->image, h->logits_all, st)) return rc;
+  }
   OldLogpParams op; op.logits = h->logits_all; op.traj = ps.src.traj; op.idx = h->idx; op.N = h->actor.n_agents; op.P = n_envs; op.A = h->actor.out; op.out = h->old_logp;
   old_logp_kernel<<<(op.N * n_envs * batch->T + 255) / 256, 256, 0, st>>>(op);
   MARL_CUDA_TRY(cudaGetLastError());

@@ -542,7 +542,7 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   if (h->rnn) {   // BPTT from td_ext; the timed window opened before the online forward
     GruBwdParams bp; memset(&bp, 0, sizeof(bp));
     bp.plan = plan; bp.traj = src.traj; bp.idx = episode_idx; bp.B = batch; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
-    bp.td = td_ext; bp.td_agent_stride = td_agent_stride; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
+    bp.td = td_ext; bp.td_agent_stride = td_agent_stride; bp.src = src; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
     if (int rc = launch_gru_backward(bp, st)) return rc;
   } else if (tc_backward_enabled() && h->ns.in < kMaxObsDim) {
     if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);

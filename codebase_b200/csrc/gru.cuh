@@ -1,5 +1,5 @@
-// gru.cuh -- recurrent (GRU) agent networks of the DQN family (algorithm.model.use_rnn=True): parameter layout, the
-// sequence forward and the BPTT backward.  Replaces marlbase/utils/models.py:51-116 (RNNNetwork with layers = [128, 128]:
+// gru.cuh -- recurrent (GRU) agent networks of the DQN family (algorithm.model.use_rnn=True) and of the actor-critic learners
+// (actor.use_rnn / critic.use_rnn): parameter layout, the sequence forward, the actor-critic loss head and the BPTT backward.  Replaces marlbase/utils/models.py:51-116 (RNNNetwork with layers = [128, 128]:
 // first_layer Linear(D, 128) + ReLU, nn.GRU(128, 128, num_layers=1), final_layer Linear(128, A)).
 #pragma once
 #include "learner.cuh"
@@ -26,7 +26,7 @@ struct GruLayout {
 
 // One launch runs every sequence of every network for all of its steps.  plan: slot lists of the networks, units_per_agent = B (training:
 // one sequence per sampled episode and agent) or E (act step), unit_rows = steps per sequence (T + 1, or 1).  src: mode 1 gathers
-// through the replay indices, mode 0 reads dense obs [E][N][D].
+// through the replay indices, mode 0 reads dense obs [E][N][D], modes 2 / 3 the joint rows of a centralised critic (learner.cuh).
 struct GruFwdParams {
   RowPlan plan; RowSource src;
   const float* theta; GruLayout lay;
@@ -36,18 +36,33 @@ struct GruFwdParams {
   float* save;         // mode 1, online pass: [N][B][T+1][kGruSaveRow] for the backward (NULL: not saved)
 };
 
-// BPTT from dL/dq of the taken actions.  CTA c of net k (plan.cta_begin) owns a contiguous run of that net's sequences and writes the
-// gradient sums of all eight tensors into scratch[c][0 .. P) in fixed order.
+// BPTT from dL/dq.  CTA c of net k (plan.cta_begin) owns a contiguous run of that net's sequences and writes the gradient sums of all eight
+// tensors into scratch[c][0 .. P) in fixed order.
 struct GruBwdParams {
   RowPlan plan; TrajView traj; const int32_t* idx; int B;
   const float* theta; GruLayout lay;
   const float* save;                    // the online pass's saved rows
-  const float* td; int td_agent_stride; // 2 * delta * filled at [agent * stride + b * T + t]
+  const float* td; int td_agent_stride; // DQN: 2 * delta * filled of the taken action at [agent * stride + b * T + t]
+  const float* dout;                    // actor-critic: dense dL/dout [N][B][T+1][out] (rows t < T read); non-NULL replaces td
+  RowSource src;                        // the rows the online pass read: mode 1 (each agent's observations) or 2 (joint rows, centralised critic)
   float* scratch; int scratch_pitch;
 };
+
+// Loss head of a recurrent actor-critic part on the stored sequence outputs q [N][P][T+1][A]: one thread per (agent, env, t < T) runs
+// head_a2c_critic or head_a2c_actor (ac_heads.cuh), writes dL/dq into dq (same layout) and block b's loss statistics into loss_part[b][0 .. 4)
+// (fixed-order tree, no atomics).
+constexpr int kGruHeadThreads = 256;
+struct GruHeadParams {
+  TrainParams tp;   // the head's fields: returns, adv_out, value_coef (critic); adv, entropy_coef, old_logp, ppo_clip (actor)
+  TrajView traj; const int32_t* idx; int N, P, A;
+  const float* q; float* dq;
+  float* loss_part;
+};
+inline int gru_head_blocks(int N, int P, int T) { return (int)(((long long)N * P * T + kGruHeadThreads - 1) / kGruHeadThreads); }
 
 int gru_kernels_init();
 int launch_gru_forward(const GruFwdParams& p, cudaStream_t st);
 int launch_gru_backward(const GruBwdParams& p, cudaStream_t st);
+int launch_gru_ac_head(const GruHeadParams& p, int head, cudaStream_t st);
 
 }  // namespace marl

@@ -4,7 +4,10 @@
 // is needed and each pass is one launch.  Thread j of each 128-thread half owns hidden unit j of 8 sequences: its three gate rows of
 // W_ih / W_hh give r, z, n and h' of that unit without a cross-thread reduction.  The weights are read through L1 / L2 (W_ih + W_hh are
 // 384 KB per network, more than shared memory holds); every weight a thread loads is used for 8 sequences.
+//
+// The actor-critic learners add a loss-head kernel between the two: it reads the outputs the forward stored and hands the backward a dense dL/dout.
 #include "gru.cuh"
+#include "ac_heads.cuh"
 
 namespace marl {
 
@@ -168,8 +171,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         float v = 0.f;
         if (k < D && vt + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s, agent, unit);
-          const size_t ep = (size_t)p.idx[unit];
-          v = p.traj.obs[((ep * p.traj.N + agent) * (size_t)(T + 1) + t) * D + k];
+          v = row_ptr(p.src, agent, unit, t)[k];
         }
         S.x[s][k] = v;
       }
@@ -178,8 +180,12 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         float v = 0.f;
         if (a < A && vt + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s, agent, unit);
-          const size_t ep = (size_t)p.idx[unit];
-          if (p.traj.act[(ep * p.traj.N + agent) * T + t] == a) v = p.td[(size_t)agent * p.td_agent_stride + (size_t)unit * T + t];
+          if (p.dout != nullptr) {
+            v = p.dout[(((size_t)agent * B + unit) * (T + 1) + t) * A + a];
+          } else {
+            const size_t ep = (size_t)p.idx[unit];
+            if (p.traj.act[(ep * p.traj.N + agent) * T + t] == a) v = p.td[(size_t)agent * p.td_agent_stride + (size_t)unit * T + t];
+          }
         }
         S.dq[s][a] = v;
       }
@@ -265,6 +271,43 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
   }
 }
 
+template <int HEAD>
+__global__ void __launch_bounds__(kGruHeadThreads) gru_ac_head_kernel(GruHeadParams p) {
+  __shared__ float red[4][kGruHeadThreads];
+  const int T = p.traj.T, tid = threadIdx.x, i = blockIdx.x * kGruHeadThreads + tid;
+  float st[4] = {0.f, 0.f, 0.f, 0.f};
+  if (i < p.N * p.P * T) {
+    RowCtx c;
+    c.agent = i / (p.P * T);
+    const int rem = i - c.agent * p.P * T;
+    c.b = rem / T; c.tt = rem - c.b * T; c.T = T; c.A = p.A; c.B = p.P;
+    const size_t ep = (size_t)p.idx[c.b];
+    c.act = p.traj.act[(ep * p.traj.N + c.agent) * T + c.tt];
+    c.filled = (float)p.traj.filled[ep * T + c.tt];
+    c.rew = 0.f; c.done1 = 0.f;   // not read by the actor-critic heads
+    const size_t row = ((size_t)c.agent * p.P + c.b) * (T + 1) + c.tt;
+    float dq[kOutPad];
+#pragma unroll
+    for (int o = 0; o < kOutPad; ++o) dq[o] = 0.f;
+    if constexpr (HEAD == kHeadA2cCritic) head_a2c_critic(p.tp, c, p.q + row * p.A, dq, st);
+    else head_a2c_actor(p.tp, c, p.q + row * p.A, dq, st);
+#pragma unroll
+    for (int o = 0; o < kOutPad; ++o)
+      if (o < p.A) p.dq[row * p.A + o] = dq[o];
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) red[k][tid] = st[k];
+  __syncthreads();
+  for (int s = kGruHeadThreads / 2; s > 0; s >>= 1) {
+    if (tid < s) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) red[k][tid] += red[k][tid + s];
+    }
+    __syncthreads();
+  }
+  if (tid < 4) p.loss_part[4 * blockIdx.x + tid] = red[tid][0];
+}
+
 int gru_kernels_init() {
   static bool done = false;
   if (!done) {
@@ -287,6 +330,14 @@ int launch_gru_forward(const GruFwdParams& p, cudaStream_t st) {
 
 int launch_gru_backward(const GruBwdParams& p, cudaStream_t st) {
   gru_backward_kernel<<<p.plan.cta_begin[p.plan.n_nets], kGruThreads, sizeof(GruBwdSmem), st>>>(p);
+  MARL_CUDA_TRY(cudaGetLastError());
+  return MARL_OK;
+}
+
+int launch_gru_ac_head(const GruHeadParams& p, int head, cudaStream_t st) {
+  const int blocks = gru_head_blocks(p.N, p.P, p.traj.T);
+  if (head == kHeadA2cCritic) gru_ac_head_kernel<kHeadA2cCritic><<<blocks, kGruHeadThreads, 0, st>>>(p);
+  else gru_ac_head_kernel<kHeadA2cActor><<<blocks, kGruHeadThreads, 0, st>>>(p);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }

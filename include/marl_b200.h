@@ -308,6 +308,20 @@ int marl_a2c_ret_ms_ptrs(marl_a2c* a, float** ret_ms /* mean[N] | var[N] */, dou
  * surrogate; the target critic follows after the last epoch.  metrics_out: device float[6] as marl_a2c_update, averaged over the epochs. */
 int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, int64_t step, int32_t num_epochs, float ppo_clip,
                     float* metrics_out, void* stream);
+/* Recurrent actor and / or critic (actor.use_rnn / critic.use_rnn; marlbase/utils/models.py:51-116 RNNNetwork with layers = [128, 128], the
+ * network and per-network parameter order of marl_dqn_create_rnn).  actor_rnn / critic_rnn != 0 make that part a GRU network; the other part stays
+ * the MLP.  marl_a2c_param_ptrs then exposes [actor nets | critic nets], each part in its own layout.  Every update pass runs each env's episode
+ * from the zero state (ac/model.py:189-246,265-352: hiddens=None): the target critic over all T+1 observations, the critic and the actor over the
+ * first T.  marl_a2c_update, _update_grads + _update_apply, marl_ppo_update, standardise_returns, sync_target and scratch_ptrs work unchanged.
+ * The "tensor_core_*" options do not apply to recurrent parts (FP32 FFMA); marl_a2c_forward_actor / _forward_critic refuse a recurrent part. */
+int marl_a2c_create_rnn(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, int32_t actor_rnn, int32_t critic_rnn,
+                        int32_t max_envs, int32_t max_T, int32_t device, marl_a2c** out);
+/* One step of a recurrent part for E envs, carrying the hidden state (act, ac/model.py:147-153; get_value, 155-163).  which: 0 actor, 1 critic,
+ * 2 target critic.  obs device float[E][N][in] (a centralised critic reads each env's N x in values), h_in / h_out device float[E][N][128]
+ * (h_in == NULL: the zero state of init_*_hiddens; h_out == NULL: not written) -> out float[E][N][n_actions] (actor) or float[E][N][1].
+ * h_in and h_out must not alias; a part that is not recurrent is refused. */
+int marl_a2c_forward_rnn(marl_a2c* h, int32_t which, const float* obs, int32_t n_envs, const float* h_in, float* h_out, float* out,
+                         void* stream);
 
 #ifdef __cplusplus
 }
