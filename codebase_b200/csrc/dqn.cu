@@ -144,6 +144,7 @@ struct marl_dqn {
   int64_t n_params = 0;  // n_nets * P
   int scratch_pitch = 0;
   float *theta = nullptr, *theta_tgt = nullptr, *m = nullptr, *v = nullptr, *grad = nullptr;
+  size_t loss_part_n = 0;   // 4-float blocks of loss statistics that loss_part holds
   float *scratch = nullptr, *loss_part = nullptr, *tq = nullptr, *q_all = nullptr, *td = nullptr, *loss_dev = nullptr, *sumsq = nullptr;
   bool grads_are_local = false;  // set by update_grads, cleared when the caller may have all-reduced grad
   int32_t* idx = nullptr;
@@ -177,6 +178,15 @@ static const int kTimingPairs = 1024;
 
 static int dqn_alloc(float** p, size_t n_floats) { return dev_alloc_zero(p, n_floats); }
 
+// loss_part only ever grows: standardise_returns and the QMIX mixer each need room for their own statistics blocks, in either call order
+static int dqn_grow_loss_part(marl_dqn* h, size_t blocks) {
+  if (blocks <= h->loss_part_n) return 0;
+  cudaFree(h->loss_part); h->loss_part = nullptr; h->loss_part_n = 0;
+  if (dqn_alloc(&h->loss_part, 4 * blocks)) return 1;
+  h->loss_part_n = blocks;
+  return 0;
+}
+
 extern "C" {
 
 static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device, bool rnn, marl_dqn** out) {
@@ -205,7 +215,7 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
   rc |= dqn_alloc(&h->theta, h->n_params); rc |= dqn_alloc(&h->theta_tgt, h->n_params);
   rc |= dqn_alloc(&h->m, h->n_params); rc |= dqn_alloc(&h->v, h->n_params); rc |= dqn_alloc(&h->grad, h->n_params + 4);
   rc |= dqn_alloc(&h->scratch, (size_t)h->n_sm * h->scratch_pitch);
-  rc |= dqn_alloc(&h->loss_part, 4 * ((size_t)h->n_sm + (size_t)(rnn ? cfg->n_agents : 1) * max_batch * max_T / 256 + 2));
+  rc |= dqn_grow_loss_part(h, (size_t)h->n_sm + (size_t)(rnn ? cfg->n_agents : 1) * max_batch * max_T / 256 + 2);
   rc |= dqn_alloc(&h->tq, rows * cfg->out_dim);
   rc |= dqn_alloc(&h->loss_dev, 8);
   rc |= dqn_alloc(&h->sumsq, (size_t)(h->n_params + 63) / 64 + 1);
@@ -254,14 +264,13 @@ int marl_dqn_destroy(marl_dqn* h) {
   return MARL_OK;
 }
 
-/* cfg.standardise_returns (dqn/model.py:82-84, 221-222): RunningMeanStd over the TD targets, one column per agent (VDN: per batch entry, see the
- * kernels above); mean 0, var 1, count 1e-4 on first enable. */
+/* cfg.standardise_returns (dqn/model.py:82-84, 221-222, 357-358): RunningMeanStd over the TD targets, one column per agent (VDN and QMIX: per
+ * batch entry, see the kernels above and qmix.cuh); mean 0, var 1, count 1e-4 on first enable. */
 int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
   MARL_REQUIRE(h != nullptr, "marl_dqn_standardise_returns: NULL handle");
-  MARL_REQUIRE(h->hp.mixer != 2 || !enable, "marl_dqn_standardise_returns: not implemented for QMIX (qmix.yaml inherits standardise_returns: False)");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   if (enable && !h->ret_ms) {
-    const int n = h->hp.mixer == 1 ? h->max_batch : h->ns.n_agents, C = h->hp.mixer == 1 ? 1 : h->ns.n_agents;
+    const int n = h->hp.mixer != 0 ? h->max_batch : h->ns.n_agents, C = h->hp.mixer != 0 ? 1 : h->ns.n_agents;
     const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
     std::vector<float> init(2 * n, 0.f);
     for (int a = 0; a < n; ++a) init[n + a] = 1.f;
@@ -275,9 +284,8 @@ int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
     MARL_CUDA_TRY(cudaMemcpy(h->ret_ms, init.data(), 2 * n * sizeof(float), cudaMemcpyHostToDevice));
     MARL_CUDA_TRY(cudaMemcpy(h->ret_count, &c0, sizeof(double), cudaMemcpyHostToDevice));
     h->n_stat = n;
-    // the per-update loss statistics of this path come from one block per 256 (c, b, t) entries
-    cudaFree(h->loss_part); h->loss_part = nullptr;
-    if (dqn_alloc(&h->loss_part, 4 * ((size_t)h->n_sm + (size_t)C * h->max_batch * h->max_T / 256 + 2))) return MARL_ENOMEM;
+    // the per-update loss statistics of this path come from one block per 256 (c, b, t) entries (QMIX: per tile, sized by marl_dqn_qmix_init)
+    if (dqn_grow_loss_part(h, (size_t)h->n_sm + (size_t)C * h->max_batch * h->max_T / 256 + 2)) return MARL_ENOMEM;
   }
   h->standardise = enable ? 1 : 0;
   return MARL_OK;
@@ -290,18 +298,27 @@ int marl_dqn_ret_ms_ptrs(marl_dqn* h, float** ret_ms, double** count, int32_t* n
 
 /* QMixNetwork.__init__ (dqn/model.py:365-379): the mixing network over the concatenated observations (state_dim = N * in_dim).  Parameters are
  * initialised by the caller through marl_dqn_qmix_ptrs (nn.Linear defaults), then marl_dqn_sync_target copies them to the target mixer. */
+typedef void (*QmixMixFn)(QmixParams, const float*, const float*);
+static QmixMixFn qmix_mix_fn(int hl, int mode) {
+  static const QmixMixFn fns[2][3] = {{qmix_mix_kernel<1, 0>, qmix_mix_kernel<1, 1>, qmix_mix_kernel<1, 2>},
+                                      {qmix_mix_kernel<2, 0>, qmix_mix_kernel<2, 1>, qmix_mix_kernel<2, 2>}};
+  return fns[hl - 1][mode];
+}
+
 int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, int32_t hypernet_embed) {
   MARL_REQUIRE(h != nullptr && h->hp.mixer == 2, "marl_dqn_qmix_init: the learner was not created with mixer = 2");
   MARL_REQUIRE(h->mix == nullptr, "marl_dqn_qmix_init: already initialised");
-  MARL_REQUIRE(hypernet_layers == 2, "marl_dqn_qmix_init: hypernet_layers = %d: only the shipped two-layer hypernetworks (qmix.yaml) are implemented", hypernet_layers);
+  MARL_REQUIRE(hypernet_layers == 1 || hypernet_layers == 2, "marl_dqn_qmix_init: hypernet_layers = %d: the reference's QMixer has 1 or 2 hypernetwork layers", hypernet_layers);
   MARL_REQUIRE(embed_dim >= 4 && embed_dim <= kQmixEmbedMax && embed_dim % 4 == 0, "marl_dqn_qmix_init: embed_dim %d not supported (multiple of 4, <= %d)", embed_dim, kQmixEmbedMax);
-  MARL_REQUIRE(hypernet_embed >= 4 && hypernet_embed <= kQmixHypMax && hypernet_embed % 4 == 0, "marl_dqn_qmix_init: hypernet_embed %d not supported (multiple of 4, <= %d)", hypernet_embed, kQmixHypMax);
+  MARL_REQUIRE(hypernet_layers == 1 || (hypernet_embed >= 4 && hypernet_embed <= kQmixHypMax && hypernet_embed % 4 == 0),
+               "marl_dqn_qmix_init: hypernet_embed %d not supported (multiple of 4, <= %d)", hypernet_embed, kQmixHypMax);
   const int N = h->ns.n_agents, S = N * h->ns.in;
   MARL_REQUIRE(S <= kQmixStateMax && N <= kQmixAgentsMax, "marl_dqn_qmix_init: state_dim %d (<= %d) or n_agents %d (<= %d) too large", S, kQmixStateMax, N, kQmixAgentsMax);
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  h->ql = qmix_layout(N, S, embed_dim, hypernet_embed);
+  h->ql = qmix_layout(N, S, embed_dim, hypernet_embed, hypernet_layers);
   const size_t n = (size_t)h->ql.n, samples = (size_t)h->max_batch * h->max_T;
-  MARL_REQUIRE(qm_smem_bytes(h->ql) <= 227 * 1024, "marl_dqn_qmix_init: the mixer's %zu parameters + a 32-sample tile (%zu bytes) do not fit shared memory", n, qm_smem_bytes(h->ql));
+  MARL_REQUIRE(qm_smem_bytes(h->ql) <= 227 * 1024, "marl_dqn_qmix_init: the mixer's %zu resident parameters + a 32-sample tile (%zu bytes) do not fit shared memory",
+               n - (size_t)h->ql.res0, qm_smem_bytes(h->ql));
   std::vector<QmixTile> tiles(kQmixMaxTiles);
   const int nt = qmix_tiles(h->ql, tiles.data());
   MARL_REQUIRE(nt > 0, "marl_dqn_qmix_init: too many weight-gradient tiles");
@@ -310,8 +327,7 @@ int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, 
   rc |= dqn_alloc(&h->mix_rec, (size_t)h->ql.R * samples); rc |= dqn_alloc(&h->mix_part, (size_t)(2 * h->n_sm > kQmixChunks ? 2 * h->n_sm : kQmixChunks) * n);
   rc |= dqn_alloc(reinterpret_cast<float**>(&h->mix_tiles), (size_t)nt * sizeof(QmixTile) / 4);
   rc |= dqn_alloc(&h->mix_img, (n + 3) & ~(size_t)3); rc |= dqn_alloc(&h->mix_img_tgt, (n + 3) & ~(size_t)3);
-  cudaFree(h->loss_part); h->loss_part = nullptr;   // one block of statistics per tile of kQmTS samples
-  rc |= dqn_alloc(&h->loss_part, 4 * ((size_t)h->n_sm + samples / kQmTS + 2));
+  rc |= dqn_grow_loss_part(h, (size_t)h->n_sm + samples / kQmTS + 2);   // one block of statistics per tile of kQmTS samples
   if (rc) return MARL_ENOMEM;
   MARL_CUDA_TRY(cudaMemcpy(h->mix_tiles, tiles.data(), (size_t)nt * sizeof(QmixTile), cudaMemcpyHostToDevice));
   h->mix_n_tiles = nt;
@@ -321,8 +337,10 @@ int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, 
   if (dqn_alloc(reinterpret_cast<float**>(&h->mix_micro), (size_t)nm * sizeof(QmixMicro) / 4)) return MARL_ENOMEM;
   MARL_CUDA_TRY(cudaMemcpy(h->mix_micro, micro.data(), (size_t)nm * sizeof(QmixMicro), cudaMemcpyHostToDevice));
   h->mix_n_micro = nm;
-  static size_t mix_limits[64] = {}, wg_limits[64] = {};   // per device (one process normally drives one GPU)
-  size_t& mix_smem_limit = mix_limits[h->device & 63]; size_t& wg_smem_limit = wg_limits[h->device & 63];
+  // the attribute is per function, process-wide: only ever raise it (a second learner with a smaller mixer must not lower the first one's limit).
+  // Every instantiation of qmix_mix_kernel is a function of its own; standardise_returns may be switched on after this call, so all three modes.
+  static size_t mix_limits[64][2][3] = {}, wg_limits[64] = {};   // per device (one process normally drives one GPU)
+  size_t& wg_smem_limit = wg_limits[h->device & 63];
   const size_t wg_smem = (size_t)(h->ql.R + 2) * kQmP * sizeof(float);
   const char* ev = getenv("MARL_QMIX_WGRAD_TILES");
   h->mix_wgrad_tiles = (ev != nullptr && ev[0] == '1') || wg_smem > 110 * 1024;   // the single-read form needs all record fields of 32 samples in shared memory
@@ -330,18 +348,23 @@ int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, 
     MARL_CUDA_TRY(cudaFuncSetAttribute(qmix_wgrad2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem));
     wg_smem_limit = wg_smem;
   }
-  // the attribute is per function, process-wide: only ever raise it (a second learner with a smaller mixer must not lower the first one's limit)
-  if (qm_smem_bytes(h->ql) > mix_smem_limit) {
-    MARL_CUDA_TRY(cudaFuncSetAttribute(qmix_mix_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qm_smem_bytes(h->ql)));
-    mix_smem_limit = qm_smem_bytes(h->ql);
+  for (int mode = 0; mode < 3; ++mode) {
+    size_t& mix_smem_limit = mix_limits[h->device & 63][hypernet_layers - 1][mode];
+    if (qm_smem_bytes(h->ql) > mix_smem_limit) {
+      MARL_CUDA_TRY(cudaFuncSetAttribute(qmix_mix_fn(hypernet_layers, mode), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qm_smem_bytes(h->ql)));
+      mix_smem_limit = qm_smem_bytes(h->ql);
+    }
   }
   return MARL_OK;
 }
 /* Host-only self-check of the QMIX weight-gradient decompositions (no device needed): counts[0 .. n) = how many micro-tile entries of the single-read
  * kernel write parameter j, counts[n .. 2n) = the same for the 32 x 32 tile form; both must be 1 everywhere.  Returns n through n_params. */
-int marl_debug_qmix_coverage(int32_t n_agents, int32_t state_dim, int32_t embed_dim, int32_t hypernet_embed, int32_t* counts, int64_t cap, int64_t* n_params) {
-  MARL_REQUIRE(n_agents >= 1 && state_dim >= 1 && embed_dim >= 4 && hypernet_embed >= 4 && n_params != nullptr, "marl_debug_qmix_coverage: bad argument");
-  const QmixLayout L = qmix_layout(n_agents, state_dim, embed_dim, hypernet_embed);
+int marl_debug_qmix_coverage_layers(int32_t n_agents, int32_t state_dim, int32_t embed_dim, int32_t hypernet_layers, int32_t hypernet_embed, int32_t* counts,
+                                    int64_t cap, int64_t* n_params) {
+  MARL_REQUIRE(n_agents >= 1 && state_dim >= 1 && embed_dim >= 4 && n_params != nullptr, "marl_debug_qmix_coverage: bad argument");
+  MARL_REQUIRE(hypernet_layers == 1 || (hypernet_layers == 2 && hypernet_embed >= 4), "marl_debug_qmix_coverage: hypernet_layers = %d (1 or 2) / hypernet_embed = %d",
+               hypernet_layers, hypernet_embed);
+  const QmixLayout L = qmix_layout(n_agents, state_dim, embed_dim, hypernet_embed, hypernet_layers);
   *n_params = L.n;
   if (counts == nullptr) return MARL_OK;
   MARL_REQUIRE(cap >= 2 * (int64_t)L.n, "marl_debug_qmix_coverage: counts needs 2 x %d entries", L.n);
@@ -372,6 +395,10 @@ int marl_debug_qmix_coverage(int32_t n_agents, int32_t state_dim, int32_t embed_
       }
   }
   return MARL_OK;
+}
+
+int marl_debug_qmix_coverage(int32_t n_agents, int32_t state_dim, int32_t embed_dim, int32_t hypernet_embed, int32_t* counts, int64_t cap, int64_t* n_params) {
+  return marl_debug_qmix_coverage_layers(n_agents, state_dim, embed_dim, 2, hypernet_embed, counts, cap, n_params);
 }
 
 int marl_dqn_qmix_ptrs(marl_dqn* h, float** mix, float** mix_tgt, float** adam_m, float** adam_v, float** grad, int64_t* n_params) {
@@ -477,7 +504,40 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   const float* td_ext = nullptr;
   float* loss_part = h->loss_part;
   int td_agent_stride = 0;
-  if (h->standardise) {
+  if (h->hp.mixer == 2) {  // QMIX: the mixer turns the agents' Q-values into the TD error and hands dL/dq_a back per agent (qmix.cuh)
+    MARL_REQUIRE(h->mix != nullptr, "marl_dqn_update: QMIX needs marl_dqn_qmix_init first");
+    MARL_REQUIRE(!h->standardise || batch == h->n_stat, "marl_dqn_update: QMIX's standardise_returns keeps one statistic per batch entry (the reference's "
+                 "reshape(-1, B)): batch %d must stay at max_batch %d", batch, h->n_stat);
+    if (int rc = online_forward()) return rc;
+    QmixParams qp; memset(&qp, 0, sizeof(qp));
+    qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = episode_idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
+    qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
+    qp.loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
+    const int Sn = batch * T, qb = (Sn + kQmTS - 1) / kQmTS, n = h->ql.n, hl = h->ql.hl;
+    qmix_pack_kernel<<<dim3((n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
+    if (h->standardise) {   // target pass -> returns, RunningMeanStd step (one column per batch entry), online pass on the standardised returns
+      qp.ret_ms = h->ret_ms; qp.n_stat = h->n_stat; qp.ret = h->ret;
+      qmix_mix_fn(hl, 1)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+      RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T; rp.N = batch; rp.P = 1;
+      MARL_CUDA_TRY(ret_ms_step(rp, st));
+      qmix_mix_fn(hl, 2)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+    } else {
+      qmix_mix_fn(hl, 0)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+    }
+    const int want = h->mix_wgrad_tiles ? kQmixChunks : 2 * h->n_sm;
+    const int chunk_len = (((Sn + want - 1) / want) + 31) & ~31, chunks = (Sn + chunk_len - 1) / chunk_len;
+    if (h->mix_wgrad_tiles) {
+      qmix_wgrad_kernel<<<dim3(h->mix_n_tiles, chunks), 256, 0, st>>>(h->mix_rec, Sn, h->mix_tiles, chunk_len, h->mix_part, n);
+    } else {
+      for (int round = 0; round * kQmMicroPerRound < h->mix_n_micro; ++round)
+        qmix_wgrad2_kernel<<<chunks, 256, (size_t)(h->ql.R + 2) * kQmP * sizeof(float), st>>>(h->mix_rec, Sn, h->ql.R, h->mix_micro, h->mix_n_micro, round, chunk_len, h->mix_part, n);
+    }
+    qmix_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(h->mix_part, chunks, n, h->mix_grad, qp.loss_part, qb);
+    MARL_CUDA_TRY(cudaGetLastError());
+    n_loss_parts += qb;
+    td_ext = h->td;
+    td_agent_stride = batch * T;
+  } else if (h->standardise) {
     // online Q-values of every row, returns + chosen Q, RunningMeanStd step, TD error (dqn/model.py:147-158 / 256-264)
     MARL_REQUIRE(h->hp.mixer == 0 || batch == h->n_stat, "marl_dqn_update: VDN's standardise_returns keeps one statistic per batch entry (the reference's reshape(-1, B)): "
                  "batch %d must stay at max_batch %d", batch, h->n_stat);
@@ -512,29 +572,6 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
     n_loss_parts += vb;
     td_ext = h->td;
     td_agent_stride = vdn ? 0 : batch * T;
-  } else if (h->hp.mixer == 2) {  // QMIX: the mixer turns the agents' Q-values into the TD error and hands dL/dq_a back per agent (qmix.cuh)
-    MARL_REQUIRE(h->mix != nullptr, "marl_dqn_update: QMIX needs marl_dqn_qmix_init first");
-    if (int rc = online_forward()) return rc;
-    QmixParams qp; memset(&qp, 0, sizeof(qp));
-    qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = episode_idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
-    qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
-    qp.loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
-    const int Sn = batch * T, qb = (Sn + kQmTS - 1) / kQmTS, n = h->ql.n;
-    qmix_pack_kernel<<<dim3((n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
-    qmix_mix_kernel<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
-    const int want = h->mix_wgrad_tiles ? kQmixChunks : 2 * h->n_sm;
-    const int chunk_len = (((Sn + want - 1) / want) + 31) & ~31, chunks = (Sn + chunk_len - 1) / chunk_len;
-    if (h->mix_wgrad_tiles) {
-      qmix_wgrad_kernel<<<dim3(h->mix_n_tiles, chunks), 256, 0, st>>>(h->mix_rec, Sn, h->mix_tiles, chunk_len, h->mix_part, n);
-    } else {
-      for (int round = 0; round * kQmMicroPerRound < h->mix_n_micro; ++round)
-        qmix_wgrad2_kernel<<<chunks, 256, (size_t)(h->ql.R + 2) * kQmP * sizeof(float), st>>>(h->mix_rec, Sn, h->ql.R, h->mix_micro, h->mix_n_micro, round, chunk_len, h->mix_part, n);
-    }
-    qmix_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(h->mix_part, chunks, n, h->mix_grad, qp.loss_part, qb);
-    MARL_CUDA_TRY(cudaGetLastError());
-    n_loss_parts += qb;
-    td_ext = h->td;
-    td_agent_stride = batch * T;
   }
   TrainParams tp; memset(&tp, 0, sizeof(tp));
   tp.plan = plan; tp.src = src; tp.theta = h->theta; tp.lay = h->ns.lay; tp.tq = h->tq; tp.td_ext = td_ext; tp.td_agent_stride = td_agent_stride;

@@ -15,6 +15,9 @@
 //                      record read once, 4 x 8 register micro-tiles -> per-CTA partial sums (every parameter belongs to exactly one micro-tile).
 //                      (qmix_wgrad_kernel: the first, tile-per-CTA form, kept behind MARL_QMIX_WGRAD_TILES=1 as a cross-check.)
 //   qmix_reduce_kernel the chunks in fixed order -> gradient; the filled count next to it (Adam's 1 / filled.sum()).
+// One-layer hypernetworks (hypernet_layers = 1): W1 = Linear(S -> N*E), w_final = Linear(S -> E), five linear layers (QmixLayout.hl, qmix_linears);
+// W1 stays in global memory (read through L1 / L2), the rest of the image in shared memory.  standardise_returns splits qmix_mix_kernel into a
+// target pass (returns) and an online pass around ret_ms_step (MODE 1 / 2).
 // The mixer's parameters take the shared Adam step WITHOUT gradient clipping: the reference clips self.critic.parameters() only (dqn/model.py:169-170).
 #pragma once
 #include "learner.cuh"
@@ -24,23 +27,53 @@ namespace marl {
 constexpr int kQmixEmbedMax = 64, kQmixHypMax = 64, kQmixAgentsMax = 8, kQmixStateMax = 256, kQmixChunks = 32, kQmixMaxTiles = 512;
 
 struct QmixLayout {   // offsets (floats) into the mixer's flat parameter vector (reference state_dict order) and into a sample's record
-  int N, S, E, He, n;
+  int N, S, E, He, n, hl;   // hl: hypernetwork layers (1 or 2); He = 0 when hl == 1
   int w1a, b1a, w1b, b1b, wfa, bfa, wfb, bfb, wb, bb, wva, bva, wvb, bvb;
   int r_x, r_h1, r_h2, r_hv, r_dz1, r_draw1, r_dzf, r_drawf, r_dhb, r_dzv, r_dv, R;
+  int res0;   // first parameter of the image that qmix_mix_kernel keeps in shared memory (hl == 1: W1 stays in global memory)
 };
 
-inline QmixLayout qmix_layout(int N, int S, int E, int He) {
-  QmixLayout L; L.N = N; L.S = S; L.E = E; L.He = He;
+// hl == 2: hyper_w_1.{0,2}, hyper_w_final.{0,2}, hyper_b_1, V.{0,2}; record x | h1 | h2 | hv | dz1 | draw1 | dzf | drawf | dhb | dzv | dv.
+// hl == 1: hyper_w_1 = Linear(S -> N*E) at w1b, hyper_w_final = Linear(S -> E) at wfb, then hyper_b_1, V.{0,2} (w1a / b1a / wfa / bfa and the
+// record's h1, h2, dz1, dzf fields are unused, -1); record x | hv | draw1 | drawf | dhb | dzv | dv.
+inline QmixLayout qmix_layout(int N, int S, int E, int He, int hl = 2) {
+  QmixLayout L; L.N = N; L.S = S; L.E = E; L.He = hl == 2 ? He : 0; L.hl = hl;
   int o = 0;
-  L.w1a = o; o += He * S; L.b1a = o; o += He; L.w1b = o; o += N * E * He; L.b1b = o; o += N * E;
-  L.wfa = o; o += He * S; L.bfa = o; o += He; L.wfb = o; o += E * He; L.bfb = o; o += E;
+  if (hl == 2) {
+    L.w1a = o; o += He * S; L.b1a = o; o += He; L.w1b = o; o += N * E * He; L.b1b = o; o += N * E;
+    L.wfa = o; o += He * S; L.bfa = o; o += He; L.wfb = o; o += E * He; L.bfb = o; o += E;
+  } else {
+    L.w1a = L.b1a = L.wfa = L.bfa = -1;
+    L.w1b = o; o += N * E * S; L.b1b = o; o += N * E; L.wfb = o; o += E * S; L.bfb = o; o += E;
+  }
   L.wb = o; o += E * S; L.bb = o; o += E; L.wva = o; o += E * S; L.bva = o; o += E; L.wvb = o; o += E; L.bvb = o; o += 1;
   L.n = o;
+  L.res0 = hl == 2 ? 0 : N * E * S;
   int r = 0;
-  L.r_x = r; r += S; L.r_h1 = r; r += He; L.r_h2 = r; r += He; L.r_hv = r; r += E;
-  L.r_dz1 = r; r += He; L.r_draw1 = r; r += N * E; L.r_dzf = r; r += He; L.r_drawf = r; r += E; L.r_dhb = r; r += E; L.r_dzv = r; r += E; L.r_dv = r; r += 1;
+  if (hl == 2) {
+    L.r_x = r; r += S; L.r_h1 = r; r += He; L.r_h2 = r; r += He; L.r_hv = r; r += E;
+    L.r_dz1 = r; r += He; L.r_draw1 = r; r += N * E; L.r_dzf = r; r += He; L.r_drawf = r; r += E; L.r_dhb = r; r += E; L.r_dzv = r; r += E; L.r_dv = r; r += 1;
+  } else {
+    L.r_h1 = L.r_h2 = L.r_dz1 = L.r_dzf = -1;
+    L.r_x = r; r += S; L.r_hv = r; r += E; L.r_draw1 = r; r += N * E; L.r_drawf = r; r += E; L.r_dhb = r; r += E; L.r_dzv = r; r += E; L.r_dv = r; r += 1;
+  }
   L.R = r;
   return L;
+}
+
+// the mixer's linear layers (weight-gradient tables and the image pack): out / in width, record rows of the output gradient and of the input,
+// weight and bias offsets.  Seven layers with two-layer hypernetworks, five with one.
+struct QmixLin { int O, I, doff, ioff, woff, boff; };
+__host__ __device__ inline int qmix_linears(const QmixLayout& L, QmixLin* out) {
+  if (L.hl == 2) {
+    out[0] = {L.He, L.S, L.r_dz1, L.r_x, L.w1a, L.b1a}; out[1] = {L.N * L.E, L.He, L.r_draw1, L.r_h1, L.w1b, L.b1b};
+    out[2] = {L.He, L.S, L.r_dzf, L.r_x, L.wfa, L.bfa}; out[3] = {L.E, L.He, L.r_drawf, L.r_h2, L.wfb, L.bfb};
+    out[4] = {L.E, L.S, L.r_dhb, L.r_x, L.wb, L.bb}; out[5] = {L.E, L.S, L.r_dzv, L.r_x, L.wva, L.bva}; out[6] = {1, L.E, L.r_dv, L.r_hv, L.wvb, L.bvb};
+    return 7;
+  }
+  out[0] = {L.N * L.E, L.S, L.r_draw1, L.r_x, L.w1b, L.b1b}; out[1] = {L.E, L.S, L.r_drawf, L.r_x, L.wfb, L.bfb};
+  out[2] = {L.E, L.S, L.r_dhb, L.r_x, L.wb, L.bb}; out[3] = {L.E, L.S, L.r_dzv, L.r_x, L.wva, L.bva}; out[4] = {1, L.E, L.r_dv, L.r_hv, L.wvb, L.bvb};
+  return 5;
 }
 
 struct QmixTile { int o0, i0, O, I, doff, ioff, woff, boff; };   // a 32 x 32 tile of one linear layer's weight-gradient matrix ([O][I], bias = column I)
@@ -53,6 +86,9 @@ struct QmixParams {
   float* rec;         // [R][B*T]
   float* td;          // [N][B][T] = dL/dq_a (un-normalised: x 2 delta filled)
   float* loss_part;   // [gridDim][4]
+  // standardise_returns (two launches around ret_ms_step): the target pass writes ret[b][t], the online pass reads it back standardised
+  const float* ret_ms; int n_stat;   // mean[n_stat] | var[n_stat], one column per batch entry
+  float* ret;                        // [B][T]
 };
 
 // ---- qmix_mix_kernel: 32 samples per CTA (lane = sample), 8 warps share each layer's outputs -----------------------------------------------------
@@ -64,19 +100,23 @@ constexpr int kQmTS = 32, kQmP = 33, kQmWarps = 8;
 __global__ void __launch_bounds__(256) qmix_pack_kernel(QmixLayout L, const float* __restrict__ mix, const float* __restrict__ mix_tgt, float* img, float* img_tgt) {
   const float* src = blockIdx.y ? mix_tgt : mix;
   float* dst = blockIdx.y ? img_tgt : img;
-  const int woff[7] = {L.w1a, L.w1b, L.wfa, L.wfb, L.wb, L.wva, L.wvb}, O[7] = {L.He, L.N * L.E, L.He, L.E, L.E, L.E, 1}, I[7] = {L.S, L.He, L.S, L.He, L.S, L.S, L.E};
+  QmixLin lin[7];
+  const int nl = qmix_linears(L, lin);   // (in parameter order)
   for (int j = blockIdx.x * 256 + threadIdx.x; j < L.n; j += gridDim.x * 256) {
-    int k = 6;
-    while (k > 0 && j < woff[k]) --k;
-    const int r = j - woff[k];
-    if (r < O[k] * I[k]) { const int o = r / I[k], i = r - o * I[k]; dst[woff[k] + i * O[k] + o] = src[j]; }
+    int wo = lin[0].woff, O = lin[0].O, I = lin[0].I;   // the layer that holds j (constant indices: the table stays in registers)
+#pragma unroll
+    for (int k = 1; k < 7; ++k)
+      if (k < nl && j >= lin[k].woff) { wo = lin[k].woff; O = lin[k].O; I = lin[k].I; }
+    const int r = j - wo;
+    if (r < O * I) { const int o = r / I, i = r - o * I; dst[wo + i * O + o] = src[j]; }
     else dst[j] = src[j];   // bias
   }
 }
 
 struct QmSmem { float *W, *X, *H1, *H2, *HV, *PRE, *RAWF, *RAW1, *QA, *RED, *RED2; };
 __host__ __device__ inline int qm_act_rows(const QmixLayout& L) { return L.S + 2 * L.He + 3 * L.E + L.N * L.E + L.N + kQmWarps + L.N * kQmWarps; }
-__host__ __device__ inline size_t qm_smem_bytes(const QmixLayout& L) { return ((size_t)((L.n + 3) & ~3) + (size_t)qm_act_rows(L) * kQmP) * sizeof(float); }
+// the resident image (parameters res0 .. n) + the tile's activations (He = 0 with one-layer hypernetworks: no H1 / H2 rows)
+__host__ __device__ inline size_t qm_smem_bytes(const QmixLayout& L) { return ((size_t)((L.n - L.res0 + 3) & ~3) + (size_t)qm_act_rows(L) * kQmP) * sizeof(float); }
 
 // out[o][lane] = act(bias[o] + sum_i wT[i][o] in[i][lane]) for this warp's groups of 4 G consecutive outputs: one load of the input feeds 4 G FMAs,
 // a weight load (16 bytes, the same address in every lane) four.  G = 2 whenever the layer is wide enough to keep all eight warps busy.
@@ -159,6 +199,33 @@ __device__ __forceinline__ float qm_forward(const QmSmem& sm, const QmixLayout& 
   return y;
 }
 
+// One-layer hypernetworks: sm.W holds parameters res0 .. n (everything but W1's weights); W1 (transposed, [S][N*E]) is read from the global image
+// w1g through L1 / L2 -- the same warp-uniform 16-byte loads as from shared memory.  The four layers all read the state only: one barrier.
+__device__ __forceinline__ float qm_forward1(const QmSmem& sm, const QmixLayout& L, const float* __restrict__ w1g, int warp, int lane) {
+  const float* W = sm.W;
+  const int r0 = L.res0;
+  qm_layer(W + (L.wva - r0), W + (L.bva - r0), sm.X, sm.HV, L.S, L.E, true, warp, lane);
+  qm_layer(W + (L.wb - r0), W + (L.bb - r0), sm.X, sm.PRE, L.S, L.E, false, warp, lane);
+  qm_layer(W + (L.wfb - r0), W + (L.bfb - r0), sm.X, sm.RAWF, L.S, L.E, false, warp, lane);
+  qm_layer(w1g, W + (L.b1b - r0), sm.X, sm.RAW1, L.S, L.N * L.E, false, warp, lane);
+  __syncthreads();
+  float part = 0.f;
+  for (int e = warp; e < L.E; e += kQmWarps) {
+    float pe = sm.PRE[e * kQmP + lane];
+    for (int a = 0; a < L.N; ++a) pe = fmaf(sm.QA[a * kQmP + lane], fabsf(sm.RAW1[(a * L.E + e) * kQmP + lane]), pe);
+    sm.PRE[e * kQmP + lane] = pe;
+    const float hid = pe > 0.f ? pe : expm1f(pe);
+    part = fmaf(hid, fabsf(sm.RAWF[e * kQmP + lane]), part);
+    part = fmaf(W[L.wvb - r0 + e], sm.HV[e * kQmP + lane], part);
+  }
+  sm.RED[warp * kQmP + lane] = part;
+  __syncthreads();
+  float y = W[L.bvb - r0];
+#pragma unroll
+  for (int k = 0; k < kQmWarps; ++k) y += sm.RED[k * kQmP + lane];
+  return y;
+}
+
 // the tile's inputs: state = the agents' observations at step t + dt side by side; q_a = chosen Q (dt = 0) or the double-Q / max target pick (dt = 1).
 // lane = sample (b, t, episode slot `ep` of this thread's sample); the rows are shared out over the warps
 __device__ __forceinline__ void qm_load_inputs(const QmSmem& sm, const QmixParams& p, bool live, int b, int t, size_t ep, int dt, int warp, int lane) {
@@ -191,12 +258,18 @@ __device__ __forceinline__ void qm_load_inputs(const QmSmem& sm, const QmixParam
   }
 }
 
+// HL: hypernetwork layers (the image's shared-memory part and the forward / backward follow the layout's table).  MODE 0: target and online pass
+// in one launch.  standardise_returns needs the whole batch's returns before any TD error: MODE 1 runs the target pass only and writes
+// ret[b][t] = r + gamma (Q_tot' sqrt(var[b]) + mean[b]) (1 - done) for every sample; ret_ms_step standardises them; MODE 2 runs the online
+// pass against the standardised ret.
+template <int HL, int MODE>
 __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p, const float* __restrict__ img, const float* __restrict__ img_tgt) {
   extern __shared__ __align__(16) float qsm[];
   const QmixLayout& L = p.L;
   QmSmem sm;
   sm.W = qsm;
-  float* o = qsm + ((L.n + 3) & ~3);
+  const int n_res = HL == 2 ? L.n : L.n - L.res0;   // image floats resident in shared memory
+  float* o = qsm + ((n_res + 3) & ~3);
   sm.X = o; o += L.S * kQmP; sm.H1 = o; o += L.He * kQmP; sm.H2 = o; o += L.He * kQmP; sm.HV = o; o += L.E * kQmP; sm.PRE = o; o += L.E * kQmP;
   sm.RAWF = o; o += L.E * kQmP; sm.RAW1 = o; o += L.N * L.E * kQmP; sm.QA = o; o += L.N * kQmP; sm.RED = o; o += kQmWarps * kQmP; sm.RED2 = o;
   const int T = p.traj.T, Sn = p.B * T, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -204,69 +277,89 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
   const bool live = s < Sn;
   const int b = live ? s / T : 0, t = live ? s - b * T : 0;
   const size_t ep = (size_t)p.idx[b];
-  const int n4 = (L.n + 3) >> 2;
+  const int n4 = (n_res + 3) >> 2, r4 = HL == 2 ? 0 : L.res0 >> 2;
   // ---- target: Q_tot' of the picks at t + 1 on the state at t + 1 ----
-  for (int i = threadIdx.x; i < n4; i += kQmWarps * 32) reinterpret_cast<float4*>(sm.W)[i] = reinterpret_cast<const float4*>(img_tgt)[i];
-  qm_load_inputs(sm, p, live, b, t, ep, 1, warp, lane);
-  __syncthreads();
-  const float ytgt = qm_forward(sm, L, warp, lane);
-  __syncthreads();
-  // ---- online ----
-  for (int i = threadIdx.x; i < n4; i += kQmWarps * 32) reinterpret_cast<float4*>(sm.W)[i] = reinterpret_cast<const float4*>(img)[i];
-  qm_load_inputs(sm, p, live, b, t, ep, 0, warp, lane);
-  __syncthreads();
-  const float y = qm_forward(sm, L, warp, lane);
-  const float filled = live ? (float)p.traj.filled[ep * T + t] : 0.f;
-  const float ret = live ? p.traj.rew[(ep * L.N + 0) * T + t] + p.gamma * ytgt * (1.f - (float)p.traj.done[ep * (T + 1) + t + 1]) : 0.f;
-  const float delta = live ? y - ret : 0.f, dy = 2.f * delta * filled;
-  float* rc = p.rec + s;   // this sample's column of the field-major record
-  if (live) {
-    // the layers' inputs (x, h1, h2) -> record; rows are shared out over the warps
-    for (int i = warp; i < L.S; i += kQmWarps) rc[(size_t)(L.r_x + i) * Sn] = sm.X[i * kQmP + lane];
-    for (int j = warp; j < L.He; j += kQmWarps) { rc[(size_t)(L.r_h1 + j) * Sn] = sm.H1[j * kQmP + lane]; rc[(size_t)(L.r_h2 + j) * Sn] = sm.H2[j * kQmP + lane]; }
-    if (warp == 0) rc[(size_t)L.r_dv * Sn] = dy;
+  float ytgt = 0.f;
+  if constexpr (MODE != 2) {
+    for (int i = threadIdx.x; i < n4; i += kQmWarps * 32) reinterpret_cast<float4*>(sm.W)[i] = reinterpret_cast<const float4*>(img_tgt)[r4 + i];
+    qm_load_inputs(sm, p, live, b, t, ep, 1, warp, lane);
+    __syncthreads();
+    if constexpr (HL == 2) ytgt = qm_forward(sm, L, warp, lane);
+    else ytgt = qm_forward1(sm, L, img_tgt + L.w1b, warp, lane);
+    __syncthreads();
   }
-  // per embedding unit: V's hidden layer, w_final, the ELU; PRE <- dL/d(ELU argument), RAWF <- dL/d(w_final before abs), RAW1 <- dL/d(W1 before abs)
-  for (int e = warp; e < L.E; e += kQmWarps) {
-    const float pe = sm.PRE[e * kQmP + lane], hid = pe > 0.f ? pe : expm1f(pe), rf = sm.RAWF[e * kQmP + lane], hv = sm.HV[e * kQmP + lane];
-    const float dp = dy * fabsf(rf) * (pe > 0.f ? 1.f : hid + 1.f);
-    const float drf = dy * hid * qmix_sgn(rf);
+  if constexpr (MODE == 1) {   // the target mixer's output de-standardised with the statistics so far (dqn/model.py:415-418), no FMA contraction
+    if (live && warp == 0) {
+      const float tq = __fadd_rn(__fmul_rn(ytgt, sqrtf(p.ret_ms[p.n_stat + b])), p.ret_ms[b]);
+      const float rew = p.traj.rew[(ep * L.N + 0) * T + t];
+      p.ret[s] = __fadd_rn(rew, __fmul_rn(__fmul_rn(p.gamma, tq), 1.f - (float)p.traj.done[ep * (T + 1) + t + 1]));
+    }
+  } else {
+    // ---- online ----
+    for (int i = threadIdx.x; i < n4; i += kQmWarps * 32) reinterpret_cast<float4*>(sm.W)[i] = reinterpret_cast<const float4*>(img)[r4 + i];
+    qm_load_inputs(sm, p, live, b, t, ep, 0, warp, lane);
+    __syncthreads();
+    float y;
+    if constexpr (HL == 2) y = qm_forward(sm, L, warp, lane);
+    else y = qm_forward1(sm, L, img + L.w1b, warp, lane);
+    const float filled = live ? (float)p.traj.filled[ep * T + t] : 0.f;
+    float ret;
+    if constexpr (MODE == 2) ret = live ? p.ret[s] : 0.f;
+    else ret = live ? p.traj.rew[(ep * L.N + 0) * T + t] + p.gamma * ytgt * (1.f - (float)p.traj.done[ep * (T + 1) + t + 1]) : 0.f;
+    const float delta = live ? y - ret : 0.f, dy = 2.f * delta * filled;
+    float* rc = p.rec + s;   // this sample's column of the field-major record
     if (live) {
-      rc[(size_t)(L.r_hv + e) * Sn] = hv;
-      rc[(size_t)(L.r_dzv + e) * Sn] = hv > 0.f ? dy * sm.W[L.wvb + e] : 0.f;
-      rc[(size_t)(L.r_drawf + e) * Sn] = drf;
-      rc[(size_t)(L.r_dhb + e) * Sn] = dp;
+      // the layers' inputs (x, h1, h2) -> record; rows are shared out over the warps
+      for (int i = warp; i < L.S; i += kQmWarps) rc[(size_t)(L.r_x + i) * Sn] = sm.X[i * kQmP + lane];
+      if constexpr (HL == 2)
+        for (int j = warp; j < L.He; j += kQmWarps) { rc[(size_t)(L.r_h1 + j) * Sn] = sm.H1[j * kQmP + lane]; rc[(size_t)(L.r_h2 + j) * Sn] = sm.H2[j * kQmP + lane]; }
+      if (warp == 0) rc[(size_t)L.r_dv * Sn] = dy;
     }
-    sm.RAWF[e * kQmP + lane] = drf;
-    sm.PRE[e * kQmP + lane] = dp;     // (this thread's own entries: the next loop reads them back without a barrier)
-  }
-  for (int a = 0; a < L.N; ++a) {
-    const float qa = sm.QA[a * kQmP + lane];
-    float dq = 0.f;
+    const float* wvb = HL == 2 ? sm.W + L.wvb : sm.W + (L.wvb - L.res0);
+    // per embedding unit: V's hidden layer, w_final, the ELU; PRE <- dL/d(ELU argument), RAWF <- dL/d(w_final before abs), RAW1 <- dL/d(W1 before abs)
     for (int e = warp; e < L.E; e += kQmWarps) {
-      const float dp = sm.PRE[e * kQmP + lane], r1 = sm.RAW1[(a * L.E + e) * kQmP + lane];
-      dq = fmaf(dp, fabsf(r1), dq);
-      const float d1 = dp * qa * qmix_sgn(r1);
-      sm.RAW1[(a * L.E + e) * kQmP + lane] = d1;
-      if (live) rc[(size_t)(L.r_draw1 + a * L.E + e) * Sn] = d1;
+      const float pe = sm.PRE[e * kQmP + lane], hid = pe > 0.f ? pe : expm1f(pe), rf = sm.RAWF[e * kQmP + lane], hv = sm.HV[e * kQmP + lane];
+      const float dp = dy * fabsf(rf) * (pe > 0.f ? 1.f : hid + 1.f);
+      const float drf = dy * hid * qmix_sgn(rf);
+      if (live) {
+        rc[(size_t)(L.r_hv + e) * Sn] = hv;
+        rc[(size_t)(L.r_dzv + e) * Sn] = hv > 0.f ? dy * wvb[e] : 0.f;
+        rc[(size_t)(L.r_drawf + e) * Sn] = drf;
+        rc[(size_t)(L.r_dhb + e) * Sn] = dp;
+      }
+      if constexpr (HL == 2) sm.RAWF[e * kQmP + lane] = drf;
+      sm.PRE[e * kQmP + lane] = dp;     // (this thread's own entries: the next loop reads them back without a barrier)
     }
-    sm.RED2[(a * kQmWarps + warp) * kQmP + lane] = dq;
-  }
-  __syncthreads();
-  for (int a = warp; a < L.N; a += kQmWarps) {   // dL/dq_a -> the agents' training pass
-    float v = 0.f;
+    for (int a = 0; a < L.N; ++a) {
+      const float qa = sm.QA[a * kQmP + lane];
+      float dq = 0.f;
+      for (int e = warp; e < L.E; e += kQmWarps) {
+        const float dp = sm.PRE[e * kQmP + lane], r1 = sm.RAW1[(a * L.E + e) * kQmP + lane];
+        dq = fmaf(dp, fabsf(r1), dq);
+        const float d1 = dp * qa * qmix_sgn(r1);
+        if constexpr (HL == 2) sm.RAW1[(a * L.E + e) * kQmP + lane] = d1;
+        if (live) rc[(size_t)(L.r_draw1 + a * L.E + e) * Sn] = d1;
+      }
+      sm.RED2[(a * kQmWarps + warp) * kQmP + lane] = dq;
+    }
+    __syncthreads();
+    for (int a = warp; a < L.N; a += kQmWarps) {   // dL/dq_a -> the agents' training pass
+      float v = 0.f;
 #pragma unroll
-    for (int k = 0; k < kQmWarps; ++k) v += sm.RED2[(a * kQmWarps + k) * kQmP + lane];
-    if (live) p.td[((size_t)a * p.B + b) * T + t] = v;
-  }
-  qm_layer_t(sm.W + L.wfb, sm.RAWF, sm.H2, L.He, L.E, rc + (size_t)L.r_dzf * Sn, Sn, live, warp, lane);
-  qm_layer_t(sm.W + L.w1b, sm.RAW1, sm.H1, L.He, L.N * L.E, rc + (size_t)L.r_dz1 * Sn, Sn, live, warp, lane);
-  // loss statistics of the tile (warp 0 holds every sample once)
-  if (warp == 0) {
-    float loss = delta * delta * filled, fill = filled;
+      for (int k = 0; k < kQmWarps; ++k) v += sm.RED2[(a * kQmWarps + k) * kQmP + lane];
+      if (live) p.td[((size_t)a * p.B + b) * T + t] = v;
+    }
+    if constexpr (HL == 2) {   // the hypernetworks' hidden layers (one-layer hypernetworks stop at dRAW1 / dRAWF)
+      qm_layer_t(sm.W + L.wfb, sm.RAWF, sm.H2, L.He, L.E, rc + (size_t)L.r_dzf * Sn, Sn, live, warp, lane);
+      qm_layer_t(sm.W + L.w1b, sm.RAW1, sm.H1, L.He, L.N * L.E, rc + (size_t)L.r_dz1 * Sn, Sn, live, warp, lane);
+    }
+    // loss statistics of the tile (warp 0 holds every sample once)
+    if (warp == 0) {
+      float loss = delta * delta * filled, fill = filled;
 #pragma unroll
-    for (int off = 16; off > 0; off >>= 1) { loss += __shfl_xor_sync(0xFFFFFFFFu, loss, off); fill += __shfl_xor_sync(0xFFFFFFFFu, fill, off); }
-    if (lane == 0) { p.loss_part[4 * blockIdx.x] = loss; p.loss_part[4 * blockIdx.x + 1] = fill; p.loss_part[4 * blockIdx.x + 2] = 0.f; p.loss_part[4 * blockIdx.x + 3] = 0.f; }
+      for (int off = 16; off > 0; off >>= 1) { loss += __shfl_xor_sync(0xFFFFFFFFu, loss, off); fill += __shfl_xor_sync(0xFFFFFFFFu, fill, off); }
+      if (lane == 0) { p.loss_part[4 * blockIdx.x] = loss; p.loss_part[4 * blockIdx.x + 1] = fill; p.loss_part[4 * blockIdx.x + 2] = 0.f; p.loss_part[4 * blockIdx.x + 3] = 0.f; }
+    }
   }
 }
 
@@ -315,18 +408,17 @@ struct QmixMicro { int d_row, n_o, x_row, i0, I, woff, boff, o0; };
 constexpr int kQmMicroPerRound = 512;   // 2 per thread
 
 inline int qmix_micro_tiles(const QmixLayout& L, QmixMicro* out, int cap) {
-  struct Lay { int O, I, doff, ioff, woff, boff; };
-  const Lay lays[7] = {
-      {L.He, L.S, L.r_dz1, L.r_x, L.w1a, L.b1a}, {L.N * L.E, L.He, L.r_draw1, L.r_h1, L.w1b, L.b1b}, {L.He, L.S, L.r_dzf, L.r_x, L.wfa, L.bfa},
-      {L.E, L.He, L.r_drawf, L.r_h2, L.wfb, L.bfb}, {L.E, L.S, L.r_dhb, L.r_x, L.wb, L.bb}, {L.E, L.S, L.r_dzv, L.r_x, L.wva, L.bva},
-      {1, L.E, L.r_dv, L.r_hv, L.wvb, L.bvb}};
+  QmixLin lays[7];
+  const int nl = qmix_linears(L, lays);
   int n = 0;
-  for (const Lay& l : lays)
+  for (int k = 0; k < nl; ++k) {
+    const QmixLin& l = lays[k];
     for (int o0 = 0; o0 < l.O; o0 += 4)
       for (int i0 = 0; i0 <= l.I; i0 += 8) {
         if (n == cap) return -1;
         out[n++] = QmixMicro{l.doff + o0, l.O - o0 < 4 ? l.O - o0 : 4, l.ioff + i0, i0, l.I, l.woff, l.boff, o0};
       }
+  }
   return n;
 }
 
@@ -414,20 +506,19 @@ __global__ void __launch_bounds__(256) qmix_reduce_kernel(const float* __restric
   }
 }
 
-// tiles of the seven linear layers (host side)
+// tiles of the mixer's linear layers (host side)
 inline int qmix_tiles(const QmixLayout& L, QmixTile* out) {
-  struct Lay { int O, I, doff, ioff, woff, boff; };
-  const Lay lays[7] = {
-      {L.He, L.S, L.r_dz1, L.r_x, L.w1a, L.b1a}, {L.N * L.E, L.He, L.r_draw1, L.r_h1, L.w1b, L.b1b}, {L.He, L.S, L.r_dzf, L.r_x, L.wfa, L.bfa},
-      {L.E, L.He, L.r_drawf, L.r_h2, L.wfb, L.bfb}, {L.E, L.S, L.r_dhb, L.r_x, L.wb, L.bb}, {L.E, L.S, L.r_dzv, L.r_x, L.wva, L.bva},
-      {1, L.E, L.r_dv, L.r_hv, L.wvb, L.bvb}};
+  QmixLin lays[7];
+  const int nl = qmix_linears(L, lays);
   int n = 0;
-  for (const Lay& l : lays)
+  for (int k = 0; k < nl; ++k) {
+    const QmixLin& l = lays[k];
     for (int o0 = 0; o0 < l.O; o0 += 32)
       for (int i0 = 0; i0 <= l.I; i0 += 32) {   // column I is the bias
         if (n == kQmixMaxTiles) return -1;
         out[n++] = QmixTile{o0, i0, l.O, l.I, l.doff, l.ioff, l.woff, l.boff};
       }
+  }
   return n;
 }
 

@@ -164,7 +164,7 @@ class QNetwork:
             nat.check(self._lib.marl_dqn_standardise_returns(self._h, C.c_int32(1)), "marl_dqn_standardise_returns")
 
     def ret_ms(self):
-        """(mean, var, count) of the RunningMeanStd over the TD targets (standardise_returns): one entry per agent; VDN: per batch entry."""
+        """(mean, var, count) of the RunningMeanStd over the TD targets (standardise_returns): one entry per agent; VDN, QMIX: per batch entry."""
         pm, pc, n = C.c_void_p(), C.c_void_p(), C.c_int32()
         nat.check(self._lib.marl_dqn_ret_ms_ptrs(self._h, C.byref(pm), C.byref(pc), C.byref(n)), "marl_dqn_ret_ms_ptrs")
         ms = nat.device_view(pm.value, 2 * n.value, self.device).cpu()
@@ -338,32 +338,63 @@ class VDNetwork(QNetwork):
 
 
 MIXER_KEYS = ("hyper_w_1.0", "hyper_w_1.2", "hyper_w_final.0", "hyper_w_final.2", "hyper_b_1", "V.0", "V.2")
+MIXER_KEYS_1 = ("hyper_w_1", "hyper_w_final", "hyper_b_1", "V.0", "V.2")   # hypernet_layers == 1
 
 
-def mixer_shapes(n_agents, state_dim, embed_dim, hypernet_embed):
-    """(out, in) of the mixing network's seven Linear layers in the reference's state_dict order (dqn/model.py:283-311, hypernet_layers == 2)."""
+def mixer_keys(hypernet_layers=2):
+    return MIXER_KEYS if hypernet_layers == 2 else MIXER_KEYS_1
+
+
+def mixer_shapes(n_agents, state_dim, embed_dim, hypernet_embed, hypernet_layers=2):
+    """(out, in) of the mixing network's Linear layers in the reference's state_dict order (dqn/model.py:283-311): seven with two-layer
+    hypernetworks, five with one (hyper_w_1 = Linear(S, N*E), hyper_w_final = Linear(S, E); hypernet_embed unused)."""
     N, S, E, He = n_agents, state_dim, embed_dim, hypernet_embed
+    if hypernet_layers == 1:
+        return ((N * E, S), (E, S), (E, S), (E, S), (1, E))
     return ((He, S), (N * E, He), (He, S), (E, He), (E, S), (E, S), (1, E))
+
+
+def check_mixing(obs_space, mixing, standardise_returns):
+    """The mixer configurations the QMIX kernels implement (csrc/qmix.cuh): 1..8 agents, a state (the observations side by side) of 1..256
+    features, embed_dim and (two-layer hypernetworks) hypernet_embed multiples of 4 up to 64, hypernet_layers 1 or 2.  Anything else fails here,
+    in Python, before any native call; marl_dqn_qmix_init checks the same limits and whether the mixer fits shared memory."""
+    mixing = dict(mixing)
+    N, S = len(obs_space), sum(_dim(o) for o in obs_space)
+    E, hl, He = int(mixing["embed_dim"]), int(mixing["hypernet_layers"]), int(mixing["hypernet_embed"])
+    why = []
+    if not 1 <= N <= 8:
+        why.append("n_agents must be 1..8")
+    if not 1 <= S <= 256:
+        why.append("state_dim must be 1..256")
+    if not (4 <= E <= 64 and E % 4 == 0):
+        why.append("embed_dim must be a multiple of 4 up to 64")
+    if hl not in (1, 2):
+        why.append("hypernet_layers must be 1 or 2")
+    elif hl == 2 and not (4 <= He <= 64 and He % 4 == 0):
+        why.append("hypernet_embed must be a multiple of 4 up to 64")
+    if why:
+        raise NotImplementedError(f"QMIX with n_agents={N}, state_dim={S}, embed_dim={E}, hypernet_layers={hl}, hypernet_embed={He}, "
+                                  f"standardise_returns={standardise_returns} is not implemented by the mixing kernels: {'; '.join(why)}")
 
 
 class QMixNetwork(QNetwork):
     """marlbase/dqn/model.py:343-443: the agents' Q-values of the chosen (target: double-Q) actions go through a monotonic mixing network conditioned
     on the state (all observations concatenated); one Adam over critic + mixer, the gradient clip covers the critic only, target updates include
-    the mixer.  The mixer runs in qmix.cuh's kernels next to the tensor-core training pass of the agents' networks (csrc/dqn.cu, mixer == 2)."""
+    the mixer.  The mixer runs in qmix.cuh's kernels next to the tensor-core training pass of the agents' networks (csrc/dqn.cu, mixer == 2).
+    mixing.hypernet_layers 1 and 2 are the reference's two forms; standardise_returns keeps one statistic per batch entry, as the reference's
+    RunningMeanStd(shape=(1,)) does once it has seen a (T, B) batch, so every update must use batch_size == max_batch."""
 
     mixer = 2
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, mixing, device, max_batch=None, max_episode_length=None):
-        if bool(getattr(cfg, "standardise_returns", False)):
-            raise NotImplementedError("standardise_returns with QMIX is not implemented (qmix.yaml inherits standardise_returns: False)")
-        if int(dict(mixing)["hypernet_layers"]) != 2:
-            raise NotImplementedError(f"mixing.hypernet_layers={dict(mixing)['hypernet_layers']}: only the shipped two-layer hypernetworks (qmix.yaml) are implemented")
+        check_mixing(obs_space, mixing, bool(getattr(cfg, "standardise_returns", False)))
         super().__init__(obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch, max_episode_length)
         mixing = dict(mixing)
         self.embed_dim, self.hypernet_embed = int(mixing["embed_dim"]), int(mixing["hypernet_embed"])
+        self.hypernet_layers = int(mixing["hypernet_layers"])
         self.state_dim = self.n_agents * self.in_dim
         with torch.cuda.device(self.device):
-            nat.check(self._lib.marl_dqn_qmix_init(self._h, C.c_int32(self.embed_dim), C.c_int32(int(mixing["hypernet_layers"])), C.c_int32(self.hypernet_embed)), "marl_dqn_qmix_init")
+            nat.check(self._lib.marl_dqn_qmix_init(self._h, C.c_int32(self.embed_dim), C.c_int32(self.hypernet_layers), C.c_int32(self.hypernet_embed)), "marl_dqn_qmix_init")
         ptrs = [C.c_void_p() for _ in range(5)]
         n = C.c_int64()
         nat.check(self._lib.marl_dqn_qmix_ptrs(self._h, *[C.byref(p) for p in ptrs], C.byref(n)), "marl_dqn_qmix_ptrs")
@@ -372,15 +403,18 @@ class QMixNetwork(QNetwork):
         self.mix_grad = nat.device_view(ptrs[4].value, self.n_mix + 4, self.device)
         # QMixer's layers are plain nn.Linear (PyTorch's default initialisation), created in this order (dqn/model.py:283-311)
         parts = []
-        for (o, i) in mixer_shapes(self.n_agents, self.state_dim, self.embed_dim, self.hypernet_embed):
+        for (o, i) in self._mixer_shapes():
             lin = torch.nn.Linear(i, o)
             parts += [lin.weight.data.reshape(-1), lin.bias.data.reshape(-1)]
         self.mix.copy_(torch.cat(parts).float())
         self.hard_update()
 
+    def _mixer_shapes(self):
+        return mixer_shapes(self.n_agents, self.state_dim, self.embed_dim, self.hypernet_embed, self.hypernet_layers)
+
     def _mixer_sd(self, flat, prefix):
         sd, o = {}, 0
-        for k, (no, ni) in zip(MIXER_KEYS, mixer_shapes(self.n_agents, self.state_dim, self.embed_dim, self.hypernet_embed)):
+        for k, (no, ni) in zip(mixer_keys(self.hypernet_layers), self._mixer_shapes()):
             sd[f"{prefix}.{k}.weight"] = flat[o:o + no * ni].view(no, ni).clone(); o += no * ni
             sd[f"{prefix}.{k}.bias"] = flat[o:o + no].clone(); o += no
         return sd
@@ -394,7 +428,7 @@ class QMixNetwork(QNetwork):
     def load_state_dict(self, sd):
         super().load_state_dict(sd)
         for dst, prefix in ((self.mix, "mixer"), (self.mix_tgt, "target_mixer")):
-            dst.copy_(torch.cat([sd[f"{prefix}.{k}.{p}"].reshape(-1).float() for k in MIXER_KEYS for p in ("weight", "bias")]))
+            dst.copy_(torch.cat([sd[f"{prefix}.{k}.{p}"].reshape(-1).float() for k in mixer_keys(self.hypernet_layers) for p in ("weight", "bias")]))
 
     def parameters(self):
         return [self.theta, self.mix]

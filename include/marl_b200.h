@@ -184,12 +184,14 @@ int marl_dqn_destroy(marl_dqn* q);
  * loss numerator, filled count, 2 spare).  Initialise theta through these (orthogonal init is done by the caller). */
 /* cfg.standardise_returns of the DQN family (marlbase/dqn/model.py:82-84,147-158; VDN 221-222,256-264; utils/standardise_stream.py): a
  * RunningMeanStd over the TD targets of every update -- target Q-values are de-standardised with the statistics so far, the statistics absorb the
- * batch's returns, the returns are standardised before the loss.  One column per agent; VDN: one per batch entry (the reference's reshape). */
+ * batch's returns, the returns are standardised before the loss.  One column per agent; VDN and QMIX: one per batch entry (the reference's
+ * reshape), so their updates must use batch == max_batch. */
 int marl_dqn_standardise_returns(marl_dqn* q, int32_t enable);
 int marl_dqn_ret_ms_ptrs(marl_dqn* q, float** ret_ms /* mean[n] | var[n] */, double** count, int32_t* n_stat);
 /* QMixNetwork (marlbase/dqn/model.py:272-443, configs/algorithm/qmix.yaml): with hp.mixer == 2, call once after marl_dqn_create.  The mixing
- * network (hypernet_layers == 2) works on state = the agents' observations concatenated (state_dim = n_agents * in_dim); its parameters are one flat
- * vector in the reference's state_dict order: hyper_w_1.0, hyper_w_1.2, hyper_w_final.0, hyper_w_final.2, hyper_b_1, V.0, V.2 (weight, bias each).
+ * network works on state = the agents' observations concatenated (state_dim = n_agents * in_dim); its parameters are one flat vector in the
+ * reference's state_dict order (weight, bias each): hypernet_layers == 2: hyper_w_1.0, hyper_w_1.2, hyper_w_final.0, hyper_w_final.2, hyper_b_1,
+ * V.0, V.2; hypernet_layers == 1: hyper_w_1, hyper_w_final, hyper_b_1, V.0, V.2 (hypernet_embed is then ignored).  Other values are refused.
  * marl_dqn_qmix_ptrs exposes parameters / target / Adam state / gradient (+ 4 statistics); initialise `mix` through it (nn.Linear defaults are the
  * caller's job), then marl_dqn_sync_target.  marl_dqn_update* then train agents and mixer with the one Adam step of the reference (the gradient
  * clip covers the agents' networks only, dqn/model.py:169-170); target updates (hard / Polyak) include the mixer (433-443). */
@@ -199,6 +201,9 @@ int marl_dqn_qmix_init(marl_dqn* q, int32_t embed_dim, int32_t hypernet_layers, 
  * counts == NULL just returns n. */
 int marl_debug_qmix_coverage(int32_t n_agents, int32_t state_dim, int32_t embed_dim, int32_t hypernet_embed, int32_t* counts, int64_t cap,
                              int64_t* n_params);
+/* The same self-check for either hypernetwork form (hypernet_layers 1 or 2; anything else is refused).  marl_debug_qmix_coverage is this with 2. */
+int marl_debug_qmix_coverage_layers(int32_t n_agents, int32_t state_dim, int32_t embed_dim, int32_t hypernet_layers, int32_t hypernet_embed,
+                                    int32_t* counts, int64_t cap, int64_t* n_params);
 int marl_dqn_qmix_ptrs(marl_dqn* q, float** mix, float** mix_tgt, float** adam_m, float** adam_v, float** grad, int64_t* n_params);
 int marl_dqn_param_ptrs(marl_dqn* q, float** theta, float** theta_tgt, float** adam_m, float** adam_v, float** grad,
                         int64_t* n_params);
