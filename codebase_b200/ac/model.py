@@ -19,8 +19,30 @@ from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dic
 from ..lbf import TrajStore
 
 
+MAX_IN_DIM = 128   # widest actor / critic input of the actor-critic kernels (csrc/learner.cuh kMaxInDim)
+
+
+def check_input_widths(obs_space, critic):
+    """The input widths the actor-critic kernels take: an actor of 1..128 observation features and a critic of 1..128 inputs (a centralised
+    critic reads all agents' observations side by side: n_agents x obs).  Anything wider fails here, in Python, before any native call;
+    marl_a2c_create checks the same limit."""
+    dims = [_dim(o) for o in obs_space]
+    actor_in = max(dims)
+    critic_in = sum(dims) if bool(critic.centralised) and len(dims) > 1 else actor_in
+    why = []
+    if actor_in > MAX_IN_DIM:
+        why.append(f"the actor's observation is {actor_in} wide")
+    if critic_in > MAX_IN_DIM:
+        what = f"the centralised critic's joint observation is {len(dims)} x {actor_in} = {critic_in} wide" if critic_in != actor_in else \
+            f"the critic's observation is {critic_in} wide"
+        why.append(what)
+    if why:
+        raise NotImplementedError(f"{'; '.join(why)}: the actor-critic kernels take at most {MAX_IN_DIM} input features")
+
+
 class A2CNetwork:
     def __init__(self, obs_space, action_space, cfg, actor, critic, device, max_envs=None, max_episode_length=None):
+        check_input_widths(obs_space, critic)
         for part, name in ((actor, "actor"), (critic, "critic")):
             if list(part.layers) != [HIDDEN, HIDDEN]:
                 raise NotImplementedError(f"{name}.layers={list(part.layers)}: the fused kernels implement the shipped [128, 128] network only "
@@ -40,9 +62,6 @@ class A2CNetwork:
         # critic.centralised (MAA2C / MAPPO, ac/model.py:62-65): every agent's critic reads the concatenation of all agents' observations
         self.centralised = bool(critic.centralised) and self.n_agents > 1
         self.critic_in = self.n_agents * self.in_dim if self.centralised else self.in_dim
-        if self.critic_in > 32:
-            raise NotImplementedError(f"critic.centralised: the joint observation is {self.critic_in} wide; the learner kernels stage at most 32 input features "
-                                      "(2 agents on Foraging-8x8-2p-3f: 30)")
         self.gamma, self.entropy_coef, self.n_steps = float(cfg.gamma), float(cfg.entropy_coef), int(cfg.n_steps)
         self.grad_clip, self.value_loss_coef = cfg.grad_clip, float(cfg.value_loss_coef)
         self.target_update_interval_or_tau = float(cfg.target_update_interval_or_tau)

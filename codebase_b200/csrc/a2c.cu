@@ -133,8 +133,8 @@ static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, con
                       int32_t device, marl_a2c** out) {
   MARL_REQUIRE(hp && out, "marl_a2c_create: NULL argument");
   *out = nullptr;
-  if (int rc = check_mlp_cfg(actor, "marl_a2c_create(actor)")) return rc;
-  if (int rc = check_mlp_cfg(critic, "marl_a2c_create(critic)")) return rc;
+  if (int rc = check_mlp_cfg(actor, "marl_a2c_create(actor)", kMaxInDim)) return rc;
+  if (int rc = check_mlp_cfg(critic, "marl_a2c_create(critic)", kMaxInDim)) return rc;
   MARL_REQUIRE(actor->n_agents == critic->n_agents && (actor->in_dim == critic->in_dim || critic->in_dim == actor->n_agents * actor->in_dim),
                "marl_a2c_create: the critic's input width must be the actor's (%d) or, for a centralised critic, n_agents x it (%d)", actor->in_dim, actor->n_agents * actor->in_dim);
   MARL_REQUIRE(critic->out_dim == 1, "marl_a2c_create: the critic outputs one state value per agent");
@@ -170,8 +170,8 @@ static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, con
   if (rc) { marl_a2c_destroy(h); return MARL_ENOMEM; }
   iota_kernel<<<(max_envs + 255) / 256, 256>>>(h->idx, max_envs);
   if (h->centralised && dev_alloc_zero(&h->joint, (size_t)max_envs * (max_T + 1) * critic->in_dim)) { marl_a2c_destroy(h); return MARL_ENOMEM; }
-  if (int rc2 = learner_kernels_init(actor->in_dim)) { marl_a2c_destroy(h); return rc2; }
-  if (int rc2 = learner_kernels_init(critic->in_dim)) { marl_a2c_destroy(h); return rc2; }
+  if (int rc2 = learner_kernels_init(actor->in_dim, kMaxInDim)) { marl_a2c_destroy(h); return rc2; }
+  if (int rc2 = learner_kernels_init(critic->in_dim, kMaxInDim)) { marl_a2c_destroy(h); return rc2; }
   if (int rc2 = tc_forward_init()) { marl_a2c_destroy(h); return rc2; }
   if (rnn) {
     if (int rc2 = gru_kernels_init()) { marl_a2c_destroy(h); return rc2; }

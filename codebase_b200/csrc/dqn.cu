@@ -235,7 +235,7 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
   if (rnn) {
     if (int rc2 = gru_kernels_init()) { marl_dqn_destroy(h); return rc2; }
   } else {
-    if (int rc2 = learner_kernels_init(cfg->in_dim)) { marl_dqn_destroy(h); return rc2; }
+    if (int rc2 = learner_kernels_init(cfg->in_dim, kMaxObsDim)) { marl_dqn_destroy(h); return rc2; }
     if (int rc2 = tc_forward_init()) { marl_dqn_destroy(h); return rc2; }
     if (int rc2 = tc_train_init()) { marl_dqn_destroy(h); return rc2; }
   }

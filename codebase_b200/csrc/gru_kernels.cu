@@ -20,8 +20,10 @@ __device__ __forceinline__ void gru_seq(const RowPlan& p, int net, int v, int& a
   unit = v - slot * p.units_per_agent;
 }
 
+// KX: staged input columns per sequence (kMaxObsDim, or kMaxInDim for the wider inputs of the actor-critic learners)
+template <int KX>
 __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p) {
-  __shared__ float xs[kGruSeqs][kMaxObsDim];
+  __shared__ float xs[kGruSeqs][KX];
   __shared__ float x1[kGruSeqs][kHidden];
   __shared__ float hs[kGruSeqs][kHidden];
   const int net = blockIdx.y, j = threadIdx.x & (kHidden - 1), s0 = (threadIdx.x >> 7) * 8;
@@ -46,8 +48,8 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
   const float bir = th[p.lay.bih + j], biz = th[p.lay.bih + kHidden + j], bin = th[p.lay.bih + 2 * kHidden + j];
   const float bhr = th[p.lay.bhh + j], bhz = th[p.lay.bhh + kHidden + j], bhn = th[p.lay.bhh + 2 * kHidden + j];
   for (int t = 0; t < steps; ++t) {
-    for (int i = threadIdx.x; i < kGruSeqs * kMaxObsDim; i += kGruThreads) {
-      const int s = i / kMaxObsDim, k = i - s * kMaxObsDim;
+    for (int i = threadIdx.x; i < kGruSeqs * KX; i += kGruThreads) {
+      const int s = i / KX, k = i - s * KX;
       float v = 0.f;
       if (k < D && v0 + s < nseq) {
         int agent, unit; gru_seq(p.plan, net, v0 + s, agent, unit);
@@ -124,9 +126,10 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
   }
 }
 
+template <int KX>
 struct GruBwdSmem {
   float dq[kGruSeqs][kOutPad];
-  float x[kGruSeqs][kMaxObsDim];
+  float x[kGruSeqs][KX];
   float x1[kGruSeqs][kHidden];        // first-layer output of step t
   float hp[kGruSeqs][kHidden];        // h_{t-1}
   float hc[kGruSeqs][kHidden];        // h_t
@@ -135,9 +138,10 @@ struct GruBwdSmem {
   float dgh[kGruSeqs][3 * kHidden];   // dL / d(W_hh h + b_hh)
 };
 
+template <int KX>
 __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams p) {
   extern __shared__ float4 smem_raw[];
-  GruBwdSmem& S = *reinterpret_cast<GruBwdSmem*>(smem_raw);
+  GruBwdSmem<KX>& S = *reinterpret_cast<GruBwdSmem<KX>*>(smem_raw);
   const int j = threadIdx.x & (kHidden - 1), s0 = (threadIdx.x >> 7) * 8;
   int net, v_begin, v_end;
   cta_rows(p.plan, net, v_begin, v_end);   // unit_rows = 1: rows are sequences
@@ -166,8 +170,8 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         }
         S.x1[s][k] = a; S.hc[s][k] = b; S.hp[s][k] = c;
       }
-      for (int i = threadIdx.x; i < kGruSeqs * kMaxObsDim; i += kGruThreads) {
-        const int s = i / kMaxObsDim, k = i - s * kMaxObsDim;
+      for (int i = threadIdx.x; i < kGruSeqs * KX; i += kGruThreads) {
+        const int s = i / KX, k = i - s * KX;
         float v = 0.f;
         if (k < D && vt + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s, agent, unit);
@@ -311,7 +315,8 @@ __global__ void __launch_bounds__(kGruHeadThreads) gru_ac_head_kernel(GruHeadPar
 int gru_kernels_init() {
   static bool done = false;
   if (!done) {
-    MARL_CUDA_TRY(cudaFuncSetAttribute(gru_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GruBwdSmem)));
+    MARL_CUDA_TRY(cudaFuncSetAttribute(gru_backward_kernel<kMaxObsDim>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GruBwdSmem<kMaxObsDim>)));
+    MARL_CUDA_TRY(cudaFuncSetAttribute(gru_backward_kernel<kMaxInDim>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(GruBwdSmem<kMaxInDim>)));
     done = true;
   }
   return MARL_OK;
@@ -323,13 +328,17 @@ int launch_gru_forward(const GruFwdParams& p, cudaStream_t st) {
     const int n = (p.plan.slot_begin[k + 1] - p.plan.slot_begin[k]) * p.plan.units_per_agent;
     most = n > most ? n : most;
   }
-  gru_forward_kernel<<<dim3((most + kGruSeqs - 1) / kGruSeqs, p.plan.n_nets), kGruThreads, 0, st>>>(p);
+  const dim3 grid((most + kGruSeqs - 1) / kGruSeqs, p.plan.n_nets);
+  if (p.lay.in <= kMaxObsDim) gru_forward_kernel<kMaxObsDim><<<grid, kGruThreads, 0, st>>>(p);
+  else gru_forward_kernel<kMaxInDim><<<grid, kGruThreads, 0, st>>>(p);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }
 
 int launch_gru_backward(const GruBwdParams& p, cudaStream_t st) {
-  gru_backward_kernel<<<p.plan.cta_begin[p.plan.n_nets], kGruThreads, sizeof(GruBwdSmem), st>>>(p);
+  const int grid = p.plan.cta_begin[p.plan.n_nets];
+  if (p.lay.in <= kMaxObsDim) gru_backward_kernel<kMaxObsDim><<<grid, kGruThreads, sizeof(GruBwdSmem<kMaxObsDim>), st>>>(p);
+  else gru_backward_kernel<kMaxInDim><<<grid, kGruThreads, sizeof(GruBwdSmem<kMaxInDim>), st>>>(p);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }

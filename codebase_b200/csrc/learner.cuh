@@ -6,7 +6,8 @@
 
 namespace marl {
 
-constexpr int kMaxObsDim = 32;  // KP = 16 or 32 float input tiles
+constexpr int kMaxObsDim = 32;   // tensor-core paths and the DQN family: KP = 16 or 32 float input tiles
+constexpr int kMaxInDim = 128;   // FP32 MLP kernels (actor-critic learners: KP = 64 / 128 tiles above 32) and the GRU kernels
 
 struct TrajView {  // device view of marl_traj_view
   const float* obs; const int32_t* act; const float* rew; const uint8_t* done; const uint8_t* filled;
@@ -169,7 +170,7 @@ struct AdamParams {
 };
 
 // host-side launchers (defined next to the kernels in learner_kernels.cu); return MARL_* codes
-int learner_kernels_init(int in_dim);                       // opt in to > 48 KB dynamic shared memory
+int learner_kernels_init(int in_dim, int max_in);           // opt in to > 48 KB dynamic shared memory; max_in: kMaxObsDim or kMaxInDim
 int launch_mlp_forward(const FwdParams& p, cudaStream_t st);
 int launch_train(const TrainParams& p, int head, cudaStream_t st);
 int launch_grad_reduce(const ReduceParams& p, cudaStream_t st);
@@ -271,9 +272,10 @@ int launch_tc_dqn_train(const TrainParams& tp, const TcBuffers& buf, cudaStream_
 
 // Forward pass through whichever implementation is selected.  `image` is scratch for the packed weights (n_nets images);
 // it is rebuilt from `theta` on every call (3 us) so that it can never go stale against direct parameter writes.
+// The tensor-core forward's W1 image is kMaxObsDim wide: wider layers always run the FP32 kernel.
 inline int forward_any(const NetSet& ns, const RowPlan& plan, const RowSource& src, const float* theta, uint8_t* image, float* out, cudaStream_t st,
                        bool image_is_current = false) {
-  if (tc_forward_enabled() && image != nullptr) {
+  if (tc_forward_enabled() && image != nullptr && ns.in <= kMaxObsDim) {
     if (!image_is_current)
       if (int rc = launch_pack_weights(theta, ns.lay, ns.n_nets, image, st)) return rc;
     FwdParams fp; fp.plan = plan; fp.src = src; fp.theta = theta; fp.lay = ns.lay; fp.out = out;
@@ -282,12 +284,13 @@ inline int forward_any(const NetSet& ns, const RowPlan& plan, const RowSource& s
   return launch_forward(ns, plan, src, theta, out, st);
 }
 
-inline int check_mlp_cfg(const marl_mlp_cfg* cfg, const char* who) {
+// max_in: the widest input the caller's kernels take (kMaxObsDim or kMaxInDim)
+inline int check_mlp_cfg(const marl_mlp_cfg* cfg, const char* who, int max_in) {
   MARL_REQUIRE(cfg != nullptr, "%s: NULL network config", who);
   MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "%s: n_agents out of range", who);
   MARL_REQUIRE(cfg->n_nets >= 1 && cfg->n_nets <= cfg->n_agents, "%s: n_nets out of range", who);
   MARL_REQUIRE(cfg->hidden == kHidden, "%s: only layers=[128,128] is implemented on the GPU path (got hidden=%d)", who, cfg->hidden);
-  MARL_REQUIRE(cfg->in_dim >= 1 && cfg->in_dim <= kMaxObsDim, "%s: obs dim %d not supported (1..%d)", who, cfg->in_dim, kMaxObsDim);
+  MARL_REQUIRE(cfg->in_dim >= 1 && cfg->in_dim <= max_in, "%s: obs dim %d not supported (1..%d)", who, cfg->in_dim, max_in);
   MARL_REQUIRE(cfg->out_dim >= 1 && cfg->out_dim <= kOutPad, "%s: output width %d not supported (1..%d)", who, cfg->out_dim, kOutPad);
   for (int a = 0; a < cfg->n_agents; ++a) MARL_REQUIRE(cfg->agent_net[a] >= 0 && cfg->agent_net[a] < cfg->n_nets, "%s: agent_net[%d] out of range", who, a);
   return MARL_OK;

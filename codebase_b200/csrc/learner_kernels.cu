@@ -36,6 +36,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_forward_kernel(FwdParams p
     __syncthreads();
     setup_rows<false>(meta, p.plan, p.src, net, vr0, nrows);
     __syncthreads();
+    if constexpr (!w1_resident<KP>()) w.load_w1_async(p.theta + (size_t)net * p.lay.P, p.lay);   // into H1: the previous tile is done with it
     gather_tile_async<KP>(X, meta, p.src.D);
     cp_async_wait_all();
     __syncthreads();
@@ -273,6 +274,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1) train_kernel(TrainParams p) {
     __syncthreads();
     setup_rows<true>(meta, p.plan, p.src, net, vr0, nrows);
     __syncthreads();
+    // into H1: the previous tile's dW1 has consumed dH1 (barrier above)
+    if constexpr (!w1_resident<KP>()) w.load_w1_async(p.theta + (size_t)net * p.lay.P, p.lay);
     gather_tile_async<KP>(X, meta, p.src.D);
     cp_async_wait_all();
     __syncthreads();
@@ -660,24 +663,29 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
 }
 
 // ---- launchers ------------------------------------------------------------------------------------------------
+// KP = 64 / 128 tiles serve the actor-critic learners only: the DQN head is not instantiated at those widths
 template <int KP>
 static int init_kp() {
+  static_assert(train_smem_bytes<KP>() <= 232448, "the tile does not fit the 227 KB opt-in shared memory of sm_90");
   MARL_CUDA_TRY(cudaFuncSetAttribute(mlp_forward_kernel<KP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)forward_smem_bytes<KP>()));
-  MARL_CUDA_TRY(cudaFuncSetAttribute(train_kernel<KP, kHeadDqn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)train_smem_bytes<KP>()));
+  if constexpr (KP <= kMaxObsDim)
+    MARL_CUDA_TRY(cudaFuncSetAttribute(train_kernel<KP, kHeadDqn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)train_smem_bytes<KP>()));
   MARL_CUDA_TRY(cudaFuncSetAttribute(train_kernel<KP, kHeadA2cCritic>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)train_smem_bytes<KP>()));
   MARL_CUDA_TRY(cudaFuncSetAttribute(train_kernel<KP, kHeadA2cActor>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)train_smem_bytes<KP>()));
   return MARL_OK;
 }
 
-int learner_kernels_init(int in_dim) {
-  MARL_REQUIRE(in_dim >= 1 && in_dim <= kMaxObsDim, "learner kernels: observation width %d not supported (1..%d)", in_dim, kMaxObsDim);
-  return in_dim <= 16 ? init_kp<16>() : init_kp<32>();
+int learner_kernels_init(int in_dim, int max_in) {
+  MARL_REQUIRE(in_dim >= 1 && in_dim <= max_in, "learner kernels: observation width %d not supported (1..%d)", in_dim, max_in);
+  return in_dim <= 16 ? init_kp<16>() : in_dim <= 32 ? init_kp<32>() : in_dim <= 64 ? init_kp<64>() : init_kp<128>();
 }
 
 int launch_mlp_forward(const FwdParams& p, cudaStream_t st) {
   const int grid = p.plan.cta_begin[p.plan.n_nets];
   if (p.lay.in <= 16) mlp_forward_kernel<16><<<grid, kMlpThreads, forward_smem_bytes<16>(), st>>>(p);
-  else mlp_forward_kernel<32><<<grid, kMlpThreads, forward_smem_bytes<32>(), st>>>(p);
+  else if (p.lay.in <= 32) mlp_forward_kernel<32><<<grid, kMlpThreads, forward_smem_bytes<32>(), st>>>(p);
+  else if (p.lay.in <= 64) mlp_forward_kernel<64><<<grid, kMlpThreads, forward_smem_bytes<64>(), st>>>(p);
+  else mlp_forward_kernel<128><<<grid, kMlpThreads, forward_smem_bytes<128>(), st>>>(p);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }
@@ -686,16 +694,24 @@ template <int KP>
 static int launch_train_kp(const TrainParams& p, int head, cudaStream_t st) {
   const int grid = p.plan.cta_begin[p.plan.n_nets];
   const size_t sm = train_smem_bytes<KP>();
-  if (head == kHeadDqn) train_kernel<KP, kHeadDqn><<<grid, kMlpThreads, sm, st>>>(p);
-  else if (head == kHeadA2cCritic) train_kernel<KP, kHeadA2cCritic><<<grid, kMlpThreads, sm, st>>>(p);
+  if constexpr (KP <= kMaxObsDim) {
+    if (head == kHeadDqn) {
+      train_kernel<KP, kHeadDqn><<<grid, kMlpThreads, sm, st>>>(p);
+      MARL_CUDA_TRY(cudaGetLastError());
+      return MARL_OK;
+    }
+  }
+  if (head == kHeadA2cCritic) train_kernel<KP, kHeadA2cCritic><<<grid, kMlpThreads, sm, st>>>(p);
   else if (head == kHeadA2cActor) train_kernel<KP, kHeadA2cActor><<<grid, kMlpThreads, sm, st>>>(p);
-  else { set_error("launch_train: unknown head %d", head); return MARL_EINVAL; }
+  else { set_error("launch_train: head %d not available at input width %d", head, p.lay.in); return MARL_EINVAL; }
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }
 
 int launch_train(const TrainParams& p, int head, cudaStream_t st) {
-  return p.lay.in <= 16 ? launch_train_kp<16>(p, head, st) : launch_train_kp<32>(p, head, st);
+  if (p.lay.in <= 16) return launch_train_kp<16>(p, head, st);
+  if (p.lay.in <= 32) return launch_train_kp<32>(p, head, st);
+  return p.lay.in <= 64 ? launch_train_kp<64>(p, head, st) : launch_train_kp<128>(p, head, st);
 }
 
 int launch_grad_reduce(const ReduceParams& p, cudaStream_t st) {

@@ -187,22 +187,37 @@ struct NetLayout {
   }
 };
 
-// Shared-memory weight block of one network.
+// Is W1 resident in shared memory for the whole launch?  Input tiles of KP <= 32 floats: yes.  Wider ones (KP = 64, 128): a resident W1
+// (32 / 66 KB) does not fit beside the two 128 x 132 activation tiles, so W1 is staged per tile into the H1 region, which is free while
+// layer 1 accumulates in registers (at KP = 128 it fills that region exactly).  Layer 1 is W1's only reader (the backward stops at dW1).
+template <int KP>
+constexpr bool w1_resident() { return KP <= 32; }
+
+// Shared-memory weight block of one network.  Without a resident W1, `w1` points at the H1 tile, which the kernels place right after
+// the block (base + kFloats).
 template <int KP>
 struct WeightSmem {
-  static constexpr int kFloats = kHidden * pitch_of<KP>() + kHidden * kPitchH + kOutPad * kHidden + kHidden + kHidden + kOutPad;
+  static constexpr int kW1Floats = kHidden * pitch_of<KP>();
+  static constexpr int kFloats = (w1_resident<KP>() ? kW1Floats : 0) + kHidden * kPitchH + kOutPad * kHidden + kHidden + kHidden + kOutPad;
   float* w1; float* w2; float* w3; float* b1; float* b2; float* b3;
   __device__ explicit WeightSmem(float* base) {
-    w1 = base; w2 = w1 + kHidden * pitch_of<KP>(); w3 = w2 + kHidden * kPitchH; b1 = w3 + kOutPad * kHidden; b2 = b1 + kHidden; b3 = b2 + kHidden;
+    if constexpr (w1_resident<KP>()) { w1 = base; w2 = w1 + kW1Floats; }
+    else { w2 = base; w1 = base + kFloats; }
+    w3 = w2 + kHidden * kPitchH; b1 = w3 + kOutPad * kHidden; b2 = b1 + kHidden; b3 = b2 + kHidden;
   }
-  // cooperative asynchronous load from global params (native layouts) into the swizzled smem layouts; 4-byte
-  // cp.async because theta + net*P is only 4-byte aligned.  Caller: cp_async_wait_all() + __syncthreads() before use.
-  __device__ void load_async(const float* __restrict__ theta, const NetLayout& l) {
+  // W1 [128][in] -> the [128][KP] smem tile, zero-padded.  Caller: cp_async_wait_all() + __syncthreads() before use.
+  __device__ void load_w1_async(const float* __restrict__ theta, const NetLayout& l) {
     for (int i = threadIdx.x; i < kHidden * KP; i += kMlpThreads) {
       const int n = i / KP, k = i % KP;
       if (k < l.in) cp_async4(&at1<KP>(w1, n, k), theta + l.w1 + n * l.in + k);
       else at1<KP>(w1, n, k) = 0.f;
     }
+  }
+  // cooperative asynchronous load from global params (native layouts) into the swizzled smem layouts; 4-byte
+  // cp.async because theta + net*P is only 4-byte aligned.  Caller: cp_async_wait_all() + __syncthreads() before use.
+  // Without a resident W1 the caller stages it per tile (load_w1_async).
+  __device__ void load_async(const float* __restrict__ theta, const NetLayout& l) {
+    if constexpr (w1_resident<KP>()) load_w1_async(theta, l);
 #pragma unroll 8
     for (int i = threadIdx.x; i < kHidden * kHidden; i += kMlpThreads) cp_async4(&at1<kHidden>(w2, i / kHidden, i % kHidden), theta + l.w2 + i);
     for (int i = threadIdx.x; i < kOutPad * kHidden; i += kMlpThreads) {
@@ -220,6 +235,7 @@ __device__ __forceinline__ void mlp_forward_tile(const float* X, float* H1, floa
   float acc[8][8];
   zero_acc(acc);
   gemm_nt<KP>(X, w.w1, tc, acc);
+  if constexpr (!w1_resident<KP>()) __syncthreads();   // W1 lives in the H1 region: every warp is done with it before H1 is written
   store_relu_bias(H1, w.b1, tc, acc);
   __syncthreads();
   zero_acc(acc);

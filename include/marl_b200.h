@@ -160,7 +160,8 @@ typedef struct {
   int32_t n_agents, n_nets;
   int32_t agent_net[MARL_MAX_AGENTS]; /* network of each agent: identity = independent (parameter_sharing False),
                                          all 0 = full sharing, else the seps indices (utils/models.py:189-196) */
-  int32_t in_dim;                     /* flatdim(observation_space[i]) */
+  int32_t in_dim;                     /* flatdim(observation_space[i]) (or n_agents x it: centralised critic); 1..32 for marl_dqn_*,
+                                         1..128 for marl_a2c_* (actor and critic) */
   int32_t hidden;                     /* layers = [hidden, hidden]; 128 (idqn.yaml:8-10) */
   int32_t out_dim;                    /* n_actions (Q / logits) or 1 (state value) */
 } marl_mlp_cfg;
@@ -281,6 +282,7 @@ typedef struct {
 
 typedef struct marl_a2c marl_a2c;
 
+/* actor->in_dim and critic->in_dim: 1..128 (inputs wider than 32 always run the FP32 kernels, whatever "tensor_core_forward" says) */
 int marl_a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, int32_t max_envs,
                     int32_t max_T, int32_t device, marl_a2c** out);
 int marl_a2c_destroy(marl_a2c* a);
