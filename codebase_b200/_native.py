@@ -66,6 +66,11 @@ class A2cHP(C.Structure):
                 ("eps", C.c_float)]
 
 
+class Optimizer(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("beta1", C.c_double), ("beta2", C.c_double), ("alpha", C.c_double), ("eps", C.c_double),
+                ("weight_decay", C.c_double)]
+
+
 class _DevArray:
     """Zero-copy torch view of library-owned device memory through the CUDA array interface."""
 

@@ -14,6 +14,7 @@ import ctypes as C
 import torch
 
 from .. import _native as nat
+from .. import optimizers
 from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dict, init_flat_params, init_flat_rnn_params, rnn_state_dict_to_flat,
                          sharing_to_nets, state_dict_to_flat)
 from ..lbf import TrajStore
@@ -48,9 +49,7 @@ class A2CNetwork:
                 raise NotImplementedError(f"{name}.layers={list(part.layers)}: the fused kernels implement the shipped [128, 128] network only "
                                           f"({'one 128-wide GRU layer' if part.use_rnn else 'MLP'})")
         self.actor_rnn, self.critic_rnn = bool(actor.use_rnn), bool(critic.use_rnn)
-        opt = getattr(cfg, "optimizer", "Adam")
-        if (opt if isinstance(opt, str) else opt.__name__) != "Adam":
-            raise NotImplementedError("only optimizer=Adam is implemented")
+        self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
             raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
         self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
@@ -86,6 +85,7 @@ class A2CNetwork:
             else:
                 nat.check(self._lib.marl_a2c_create(C.byref(acfg), C.byref(ccfg), C.byref(hp), C.c_int32(self.max_envs), C.c_int32(self.max_T),
                                                     C.c_int32(self.device.index), C.byref(self._h)), "marl_a2c_create")
+        optimizers.apply(self._lib, "marl_a2c_set_optimizer", self._h, self.optimizer_name)
         ptrs = [C.c_void_p() for _ in range(5)]
         na, nc = C.c_int64(), C.c_int64()
         nat.check(self._lib.marl_a2c_param_ptrs(self._h, *[C.byref(p) for p in ptrs], C.byref(na), C.byref(nc)), "marl_a2c_param_ptrs")
@@ -113,6 +113,11 @@ class A2CNetwork:
         ms = nat.device_view(pm.value, 2 * self.n_agents, self.device).cpu()
         cnt = nat.device_view(pc.value, 1, self.device, "<f8").cpu()
         return ms[: self.n_agents], ms[self.n_agents:], float(cnt[0])
+
+    def optimizer_state(self):
+        """The optimiser state of actor + critic by torch's names (Adam / AdamW: exp_avg, exp_avg_sq; RMSprop: square_avg; Adagrad: sum; SGD:
+        none), flat device views in the layout of `theta`."""
+        return optimizers.state(self.optimizer_name, self.adam_m, self.adam_v)
 
     # ---- views into the flat parameter vector ------------------------------------------------------------------
     @property

@@ -105,6 +105,7 @@ struct marl_a2c {
   int32_t* idx = nullptr;
   uint8_t* image = nullptr;  // packed weight images for the tensor-core forward path
   int64_t opt_steps = 0;
+  marl_optimizer opt = {};   // the optimiser of actor + critic (marl_a2c_set_optimizer; Adam with hp's constants by default)
   float *logits_all = nullptr, *old_logp = nullptr, *epoch_metrics = nullptr;   // PPO (allocated on first use)
   // standardise_returns: RunningMeanStd(shape=(n_agents,)) -- mean[N] | var[N] (float32), count (a Python float in the reference), partial sums
   int standardise = 0; float* ret_ms = nullptr; double* ret_count = nullptr; double* ret_part = nullptr;
@@ -144,6 +145,7 @@ static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, con
   marl_a2c* h = new marl_a2c();
   h->actor = to_netset(actor); h->critic = to_netset(critic);
   h->hp = *hp; h->device = device; h->max_envs = max_envs; h->max_T = max_T;
+  h->opt.kind = MARL_OPT_ADAM; h->opt.beta1 = hp->beta1; h->opt.beta2 = hp->beta2; h->opt.eps = hp->eps;
   h->centralised = (critic->in_dim != actor->in_dim || (actor->n_agents == 1 && false)) ? 1 : 0;
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
   h->actor_rnn = actor_rnn ? 1 : 0; h->critic_rnn = critic_rnn ? 1 : 0;
@@ -393,15 +395,14 @@ static int a2c_apply(marl_a2c* h, int64_t step, float* metrics_out, void* stream
   AdamParams ap; memset(&ap, 0, sizeof(ap));
   ap.theta = h->theta; ap.theta_tgt = h->theta_tgt; ap.m = h->m; ap.v = h->v; ap.grad = h->grad; ap.n = (int)h->n_params;
   ap.tgt_begin = (int)h->n_actor; ap.tgt_n = (int)h->n_critic;
-  ap.lr = h->hp.lr; ap.beta1 = h->hp.beta1; ap.beta2 = h->hp.beta2; ap.eps = h->hp.eps; ap.grad_clip = h->hp.grad_clip;
-  ap.bc1 = (float)(1.0 - pow((double)h->hp.beta1, (double)h->opt_steps));
-  ap.bc2_sqrt = (float)sqrt(1.0 - pow((double)h->hp.beta2, (double)h->opt_steps));
+  ap.grad_clip = h->hp.grad_clip;
+  set_step_consts(ap, h->opt, h->hp.lr, h->opt_steps);
   const float tu = h->hp.target_update_interval_or_tau;  // ac/model.py:233-239: `step` counts environment steps
   ap.tau = tu;
   if (target_update && tu > 1.0f && fmod((double)step, (double)tu) == 0.0) ap.target_mode = 1;
   else if (target_update && tu < 1.0f) ap.target_mode = 2;
   ap.loss_out = metrics_out ? metrics_out : h->metrics;
-  return launch_adam(ap, (cudaStream_t)stream);
+  return launch_adam(ap, h->opt.kind, (cudaStream_t)stream);
 }
 
 int marl_a2c_update_apply(marl_a2c* h, int64_t step, float* metrics_out, void* stream) { return a2c_apply(h, step, metrics_out, stream, true); }
@@ -436,6 +437,18 @@ int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, in
   }
   mean_metrics_kernel<<<1, 32, 0, st>>>(h->epoch_metrics, num_epochs, metrics_out ? metrics_out : h->metrics);
   MARL_CUDA_TRY(cudaGetLastError());
+  return MARL_OK;
+}
+
+/* The optimiser of actor + critic: before the first step only; zeroes the optimiser state. */
+int marl_a2c_set_optimizer(marl_a2c* h, const marl_optimizer* opt) {
+  MARL_REQUIRE(h != nullptr, "marl_a2c_set_optimizer: NULL handle");
+  if (int rc = check_optimizer(opt, "marl_a2c_set_optimizer")) return rc;
+  MARL_REQUIRE(h->opt_steps == 0, "marl_a2c_set_optimizer: the learner has already taken an optimiser step; choose the optimiser right after creation");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  MARL_CUDA_TRY(cudaMemset(h->m, 0, h->n_params * sizeof(float)));
+  MARL_CUDA_TRY(cudaMemset(h->v, 0, h->n_params * sizeof(float)));
+  h->opt = *opt;
   return MARL_OK;
 }
 

@@ -161,6 +161,8 @@ struct marl_dqn {
   // online images: valid = a full pack happened and every later change of theta came from adam_kernel (which updates them in place)
   bool image_current = false, bwd_image_current = false;
   int64_t updates = 0, last_target_update = 0;
+  marl_optimizer opt = {};      // the optimiser (marl_dqn_set_optimizer; Adam with hp's constants by default)
+  bool opt_stepped = false;     // an optimiser step has been launched: the state in m / v belongs to `opt`
   RowPlan train_plan; int n_loss_parts = 0;
   // optional CUDA-event timing of the training kernel (bench.py's roofline leg)
   // measurement hook: 4 events per timed update (before the training pass, after each of its kernels; the FP32 path uses 0 and 3)
@@ -206,6 +208,7 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
   memcpy(h->ns.agent_net, cfg->agent_net, sizeof(int) * MARL_MAX_AGENTS);
   h->ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim);
   h->hp = *hp; h->device = device; h->max_batch = max_batch; h->max_T = max_T;
+  h->opt.kind = MARL_OPT_ADAM; h->opt.beta1 = hp->beta1; h->opt.beta2 = hp->beta2; h->opt.eps = hp->eps;
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
   h->rnn = rnn; h->gl = GruLayout::make(cfg->in_dim, cfg->out_dim);
   h->n_params = (int64_t)cfg->n_nets * h->P();
@@ -617,10 +620,10 @@ int marl_dqn_update_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t
 // Optimiser-step parameters of the next update (advances the update counters)
 static void dqn_adam_params(marl_dqn* h, float* loss_out, AdamParams& ap) {
   h->updates += 1;
+  h->opt_stepped = true;
   memset(&ap, 0, sizeof(ap)); ap.theta = h->theta; ap.theta_tgt = h->theta_tgt; ap.m = h->m; ap.v = h->v; ap.grad = h->grad; ap.n = (int)h->n_params;
-  ap.lr = h->hp.lr; ap.beta1 = h->hp.beta1; ap.beta2 = h->hp.beta2; ap.eps = h->hp.eps; ap.grad_clip = h->hp.grad_clip;
-  ap.bc1 = (float)(1.0 - pow((double)h->hp.beta1, (double)h->updates));
-  ap.bc2_sqrt = (float)sqrt(1.0 - pow((double)h->hp.beta2, (double)h->updates));
+  ap.grad_clip = h->hp.grad_clip;
+  set_step_consts(ap, h->opt, h->hp.lr, h->updates);
   // update_target (dqn/model.py:176-185)
   const float tu = h->hp.target_update_interval_or_tau;
   ap.target_mode = 0; ap.tau = tu; ap.tgt_begin = 0; ap.tgt_n = (int)h->n_params;
@@ -639,14 +642,14 @@ static void dqn_adam_params(marl_dqn* h, float* loss_out, AdamParams& ap) {
   }
 }
 
-// QMIX: the mixer's share of the single Adam step (same step count, learning rate and target update as the agents' networks; no clipping:
+// QMIX: the mixer's share of the single optimiser step (same optimiser, step count, learning rate and target update as the agents' networks; no clipping:
 // clip_grad_norm_ covers self.critic.parameters() only, dqn/model.py:169-170)
 static int qmix_adam(marl_dqn* h, const AdamParams& main, cudaStream_t st) {
   if (h->hp.mixer != 2) return MARL_OK;
   AdamParams ap = main;
   ap.theta = h->mix; ap.theta_tgt = h->mix_tgt; ap.m = h->mix_m; ap.v = h->mix_v; ap.grad = h->mix_grad; ap.n = h->ql.n; ap.tgt_begin = 0; ap.tgt_n = h->ql.n;
   ap.grad_clip = 0.f; ap.loss_out = nullptr; ap.sumsq_part = nullptr; ap.n_sumsq = 0; ap.image = nullptr; ap.bwd_image = nullptr; ap.img_nets = 0;
-  return launch_adam(ap, st);
+  return launch_adam(ap, h->opt.kind, st);
 }
 
 int marl_dqn_update_apply(marl_dqn* h, float* loss_out, void* stream) {
@@ -654,7 +657,7 @@ int marl_dqn_update_apply(marl_dqn* h, float* loss_out, void* stream) {
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   AdamParams ap;
   dqn_adam_params(h, loss_out, ap);
-  if (int rc = launch_adam(ap, (cudaStream_t)stream)) return rc;
+  if (int rc = launch_adam(ap, h->opt.kind, (cudaStream_t)stream)) return rc;
   return qmix_adam(h, ap, (cudaStream_t)stream);
 }
 
@@ -675,7 +678,7 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
   // step), then wait for the peers and finish: the wait hides under ~17 us of forward.  Not when this step rewrites theta_tgt.  Off by default: on two
   // GPUs the extra launch (prologue, second pass over the Adam state) cost more than the hidden wait saved (120.9 vs 116.8 us per update).
   if (h->xchg.world > 1 && tc_split_exchange_enabled()) {
-    if (launch_reduce_push(rp, ap, &h->xchg, sp, h->grid_barrier, &h->push_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
+    if (launch_reduce_push(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->push_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
       if (next != nullptr && ap.target_mode == 0 && !h->standardise && h->hp.mixer == 0) {
         const int T = traj->T;
         const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
@@ -686,18 +689,18 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
         h->tgt_image_current = tc_forward_enabled() != 0;
         h->tq_ahead = true;
       }
-      if (int rc = launch_adam_finish(rp, ap, &h->xchg, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream)) return rc;
+      if (int rc = launch_adam_finish(rp, ap, h->opt.kind, &h->xchg, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream)) return rc;
       if (fused_out) *fused_out = true;
       return MARL_OK;
     }
   }
-  if (launch_reduce_adam(rp, ap, &h->xchg, sp, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
+  if (launch_reduce_adam(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
     if (fused_out) *fused_out = true;
     return qmix_adam(h, ap, (cudaStream_t)stream);
   }
   MARL_REQUIRE(h->xchg.world <= 1, "marl_dqn_update: the peer-memory exchange needs the fused tail kernel (parameter count too large for one wave)");
   if (int rc = launch_grad_reduce(rp, (cudaStream_t)stream)) return rc;
-  if (int rc = launch_adam(ap, (cudaStream_t)stream)) return rc;
+  if (int rc = launch_adam(ap, h->opt.kind, (cudaStream_t)stream)) return rc;
   return qmix_adam(h, ap, (cudaStream_t)stream);
 }
 
@@ -806,7 +809,7 @@ int marl_dqn_peer_attach(marl_dqn* h, int32_t rank, int32_t world, const void* h
   {  // the exchange lives inside the fused reduce + Adam kernel: refuse here, before any update mutates counters, when that kernel cannot
      // cover this parameter count with one co-resident wave (a later fallback to the two-kernel tail would dead-lock the peers' polls)
     int pb = 0, ns = 0;
-    MARL_REQUIRE(reduce_adam_shape((int)h->n_params, h->n_sm, true, &pb, &ns) == MARL_OK,
+    MARL_REQUIRE(reduce_adam_shape((int)h->n_params, h->n_sm, true, h->opt.kind, &pb, &ns) == MARL_OK,
                  "marl_dqn_peer_attach: %lld parameters do not fit the fused reduce + Adam kernel on %d SMs; use the all-reduce between marl_dqn_update_grads and _apply",
                  (long long)h->n_params, h->n_sm);
   }
@@ -844,6 +847,27 @@ int marl_dqn_counters(marl_dqn* h, int64_t* updates, int64_t* last_target_update
   MARL_REQUIRE(h != nullptr, "marl_dqn_counters: NULL handle");
   if (updates) *updates = h->updates;
   if (last_target_update) *last_target_update = h->last_target_update;
+  return MARL_OK;
+}
+
+/* The optimiser of the agents' networks (and of the mixer): before the first step only; zeroes the optimiser state. */
+int marl_dqn_set_optimizer(marl_dqn* h, const marl_optimizer* opt) {
+  MARL_REQUIRE(h != nullptr, "marl_dqn_set_optimizer: NULL handle");
+  if (int rc = check_optimizer(opt, "marl_dqn_set_optimizer")) return rc;
+  MARL_REQUIRE(!h->opt_stepped, "marl_dqn_set_optimizer: the learner has already taken an optimiser step; choose the optimiser right after creation");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  if (h->xchg.world > 1) {   // the peer exchange lives in the fused tail: the new optimiser's instantiation must fit one wave as well
+    int pb = 0, ns = 0;
+    MARL_REQUIRE(reduce_adam_shape((int)h->n_params, h->n_sm, true, opt->kind, &pb, &ns) == MARL_OK,
+                 "marl_dqn_set_optimizer: %lld parameters do not fit the fused tail of optimizer kind %d on %d SMs", (long long)h->n_params, opt->kind, h->n_sm);
+  }
+  MARL_CUDA_TRY(cudaMemset(h->m, 0, h->n_params * sizeof(float)));
+  MARL_CUDA_TRY(cudaMemset(h->v, 0, h->n_params * sizeof(float)));
+  if (h->mix) {
+    MARL_CUDA_TRY(cudaMemset(h->mix_m, 0, (size_t)h->ql.n * sizeof(float)));
+    MARL_CUDA_TRY(cudaMemset(h->mix_v, 0, (size_t)h->ql.n * sizeof(float)));
+  }
+  h->opt = *opt;
   return MARL_OK;
 }
 

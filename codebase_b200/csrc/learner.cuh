@@ -155,16 +155,22 @@ struct ReduceParams {
   float* sumsq_part;     // [ceil(n_nets*P / 64)] per-block sum of squares of the reduced gradients (NULL: skip)
 };
 
+// The optimiser of a step (marl_optimizer.kind): a template parameter of the two step kernels, so each one compiles to its own code
+enum OptKind { kOptAdam = MARL_OPT_ADAM, kOptAdamW = MARL_OPT_ADAMW, kOptRmsprop = MARL_OPT_RMSPROP, kOptAdagrad = MARL_OPT_ADAGRAD, kOptSgd = MARL_OPT_SGD,
+               kNumOpt };
+
+// The optimiser state lives in m / v: Adam, AdamW exp_avg / exp_avg_sq; RMSprop square_avg in v; Adagrad sum in v; SGD none.
 struct AdamParams {
   float* theta; float* theta_tgt; float* m; float* v;
   const float* grad;   // [n] gradient sums followed by 4 statistics: (loss numerator, filled count, aux0, aux1)
   int n;               // trainable floats
   int tgt_begin, tgt_n;  // theta[tgt_begin .. tgt_begin+tgt_n) is mirrored by theta_tgt[0 .. tgt_n)
-  float lr, beta1, beta2, eps, bc1, bc2_sqrt, grad_clip;  // grad_clip <= 0: off
+  float lr, beta1, beta2, eps, bc1, bc2_sqrt, grad_clip;  // grad_clip <= 0: off; RMSprop: beta2 = alpha, beta1 = 1 - alpha (rounded from double)
   int target_mode;  // 0 none, 1 hard copy, 2 polyak
   float tau;
   float* loss_out;  // [6]: stats[0]/filled, grad norm, stats[2]/filled, stats[3]/filled, filled, 0
   const float* sumsq_part; int n_sumsq;  // optional per-block sums of squares of grad[0..n) (local gradients only: single GPU)
+  float decay;      // AdamW: theta *= decay (= 1 - lr * weight_decay) before the Adam step.  In the slot before `image`: no other field moves
   // optional packed tensor-core images of theta[0 .. img_nets * img_lay.P), kept current parameter by parameter (NULL: none)
   uint8_t* image; uint8_t* bwd_image; NetLayout img_lay; int img_nets; size_t image_bytes, bwd_image_bytes;
 };
@@ -187,14 +193,40 @@ struct XchgParams {
 };
 // replay indices for the next update, drawn by the fused tail kernel (idx == NULL: none); same stream as replay_sample_kernel
 struct SampleParams { uint64_t seed, update_idx; int batch, n_valid; int32_t* idx; };
-int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier, unsigned long long* epoch,
-                       int n_sm, cudaStream_t st);
-int launch_reduce_push(const ReduceParams& rp, const AdamParams& ap, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier, unsigned long long* push_epoch,
-                       int n_sm, cudaStream_t st);
-int launch_adam_finish(const ReduceParams& rp, const AdamParams& ap, XchgParams* xp, unsigned long long* barrier, unsigned long long* epoch, int n_sm, cudaStream_t st);
-int launch_adam(const AdamParams& p, cudaStream_t st);
-// can the fused tail cover n parameters with one co-resident wave on n_sm SMs?  (pb, ns: the block shape it would use)
-int reduce_adam_shape(int n, int n_sm, bool xchg, int* pb, int* ns);
+// opt: the OptKind of the step
+int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
+                       unsigned long long* epoch, int n_sm, cudaStream_t st);
+int launch_reduce_push(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
+                       unsigned long long* push_epoch, int n_sm, cudaStream_t st);
+int launch_adam_finish(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, unsigned long long* barrier, unsigned long long* epoch, int n_sm,
+                       cudaStream_t st);
+int launch_adam(const AdamParams& p, int opt, cudaStream_t st);
+// can the fused tail with optimiser `opt` cover n parameters with one co-resident wave on n_sm SMs?  (pb, ns: the block shape it would use)
+int reduce_adam_shape(int n, int n_sm, bool xchg, int opt, int* pb, int* ns);
+// the step constants of `o` for the next step (step = 1, 2, ...): lr, betas, eps, bias corrections, AdamW's decay.  The handle has checked o.
+// Adam / AdamW: the betas as float32 (the hp fields' values: a handle's Adam steps stay what they were before marl_optimizer existed).
+// RMSprop / AdamW: torch's Python-scalar arithmetic in double, rounded once to float32 as torch's CPU kernels round a scalar argument.
+inline void set_step_consts(AdamParams& ap, const marl_optimizer& o, float lr, int64_t step) {
+  ap.lr = lr; ap.eps = (float)o.eps; ap.bc1 = 1.f; ap.bc2_sqrt = 1.f; ap.decay = 1.f;
+  if (o.kind == MARL_OPT_ADAM || o.kind == MARL_OPT_ADAMW) {
+    const float b1 = (float)o.beta1, b2 = (float)o.beta2;
+    ap.beta1 = b1; ap.beta2 = b2;
+    ap.bc1 = (float)(1.0 - pow((double)b1, (double)step));
+    ap.bc2_sqrt = (float)sqrt(1.0 - pow((double)b2, (double)step));
+    if (o.kind == MARL_OPT_ADAMW) ap.decay = (float)(1.0 - (double)lr * o.weight_decay);   // param.mul_(1 - lr * weight_decay)
+  } else if (o.kind == MARL_OPT_RMSPROP) {
+    ap.beta2 = (float)o.alpha;                // square_avg.mul_(alpha)
+    ap.beta1 = (float)(1.0 - o.alpha);        // addcmul_(grad, grad, value=1 - alpha)
+  }
+}
+// marl_*_set_optimizer's argument check
+inline int check_optimizer(const marl_optimizer* o, const char* who) {
+  MARL_REQUIRE(o != nullptr, "%s: NULL optimizer", who);
+  MARL_REQUIRE(o->kind >= 0 && o->kind < kNumOpt, "%s: optimizer kind %d unknown (Adam 0, AdamW 1, RMSprop 2, Adagrad 3, SGD 4)", who, o->kind);
+  MARL_REQUIRE(o->eps >= 0.0 && o->weight_decay >= 0.0 && o->beta1 >= 0.0 && o->beta1 < 1.0 && o->beta2 >= 0.0 && o->beta2 < 1.0 && o->alpha >= 0.0 && o->alpha <= 1.0,
+               "%s: optimizer constants out of range", who);
+  return MARL_OK;
+}
 
 template <int KP>
 constexpr size_t forward_smem_bytes() { return sizeof(float) * (WeightSmem<KP>::kFloats + 2 * kTileRows * kPitchH + kTileRows * kOutPad + 48) + RowMeta::kBytes; }

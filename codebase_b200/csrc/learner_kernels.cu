@@ -8,7 +8,7 @@
 //                       forward, double-Q TD target, MSE, masked mean numerator, full backward; every CTA keeps its
 //                       network's weights resident in shared memory and walks its episodes tile by tile.
 //  grad_reduce_kernel   deterministic sum of the per-CTA gradient partials (+ loss / filled sums).
-//  adam_kernel          clip_grad_norm_ + Adam.step + update_target (marlbase/dqn/model.py:169-196).
+//  adam_kernel<OPT>     clip_grad_norm_ + optimiser step (Adam, AdamW, RMSprop, Adagrad or SGD) + update_target (marlbase/dqn/model.py:169-196).
 //
 // Persistent CTAs, one per SM (132 on H100) split across networks; FP32 FFMA register-tiled GEMMs (see mlp.cuh).
 #include "tc_common.cuh"
@@ -385,9 +385,40 @@ __global__ void __launch_bounds__(64 * kReduceSlices) grad_reduce_kernel(ReduceP
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// One optimiser step of one parameter (torch.optim's single-tensor implementations with the constants of AdamParams): g = the clipped
+// gradient, m / v = the state (the kernels store only the state an optimiser uses), returns the new parameter.  AdamW's decay, RMSprop,
+// Adagrad and SGD follow torch's CPU kernels: add_(alpha=) and addcmul_ are one fused multiply-add (addcmul_: (value * t1) * t2 + self), bit
+// for bit (tests/test_optimizers.py); addcdiv_ is written as (value * t1) / t2, then the sum, which equals torch's result on all but about 1 in
+// 10 000 elements (one ulp).  Every other product and sum is explicit (__f*_rn), so nothing else contracts into an FMA (`/` and sqrtf are IEEE
+// round-to-nearest in this build: no --use_fast_math).
+// The Adam step keeps the expressions this file has always had.
+template <int OPT> constexpr bool opt_uses_m() { return OPT == kOptAdam || OPT == kOptAdamW; }
+template <int OPT> constexpr bool opt_uses_v() { return OPT != kOptSgd; }
+
+template <int OPT>
+__device__ __forceinline__ float opt_step(const AdamParams& p, float g, float& m, float& v, float th) {
+  if constexpr (OPT == kOptAdam || OPT == kOptAdamW) {
+    if constexpr (OPT == kOptAdamW) th = __fmul_rn(th, p.decay);      // param.mul_(1 - lr * weight_decay)
+    m = m + (g - m) * (1.f - p.beta1);                       // exp_avg.lerp_(grad, 1 - beta1)
+    v = v * p.beta2 + g * g * (1.f - p.beta2);               // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
+    const float denom = sqrtf(v) / p.bc2_sqrt + p.eps;
+    return th - (p.lr / p.bc1) * (m / denom);
+  } else if constexpr (OPT == kOptRmsprop) {
+    v = __fmaf_rn(__fmul_rn(p.beta1, g), g, __fmul_rn(v, p.beta2));                  // square_avg.mul_(alpha).addcmul_(grad, grad, 1 - alpha)
+    return __fadd_rn(th, __fmul_rn(-p.lr, g) / __fadd_rn(sqrtf(v), p.eps));   // param.addcdiv_(grad, sqrt(s) + eps, value=-lr)
+  } else if constexpr (OPT == kOptAdagrad) {
+    v = __fmaf_rn(g, g, v);                                                           // state_sum.addcmul_(grad, grad, value=1)
+    return __fadd_rn(th, __fmul_rn(-p.lr, g) / __fadd_rn(sqrtf(v), p.eps));   // param.addcdiv_(grad, sqrt(sum) + eps, value=-lr)
+  } else {
+    return __fmaf_rn(-p.lr, g, th);                                                   // param.add_(grad, alpha=-lr)
+  }
+}
+
 // grad holds un-normalised sums followed by 4 statistics (loss numerator, filled count, aux, aux) -- possibly
 // all-reduced over ranks.
 // Every CTA recomputes the global norm in the same order (bit-identical clip coefficient on every CTA and rank).
+template <int OPT>
 __global__ void __launch_bounds__(256) adam_kernel(AdamParams p) {
   __shared__ float red[256];
   pdl_wait();
@@ -422,12 +453,11 @@ __global__ void __launch_bounds__(256) adam_kernel(AdamParams p) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i < p.n) {
     const float g = p.grad[i] * inv_fill * clip;
-    float m = p.m[i], v = p.v[i], th = p.theta[i];
-    m = m + (g - m) * (1.f - p.beta1);                       // exp_avg.lerp_(grad, 1 - beta1)
-    v = v * p.beta2 + g * g * (1.f - p.beta2);               // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-    const float denom = sqrtf(v) / p.bc2_sqrt + p.eps;
-    th = th - (p.lr / p.bc1) * (m / denom);
-    p.m[i] = m; p.v[i] = v; p.theta[i] = th;
+    float m = p.m[i], v = p.v[i];   // (loads an optimiser does not use are dead code)
+    const float th = opt_step<OPT>(p, g, m, v, p.theta[i]);
+    if constexpr (opt_uses_m<OPT>()) p.m[i] = m;
+    if constexpr (opt_uses_v<OPT>()) p.v[i] = v;
+    p.theta[i] = th;
     if (p.image != nullptr && i < p.img_nets * p.img_lay.P) {  // keep the packed tensor-core images of theta current
       const int net = i / p.img_lay.P;
       pack_param(p.img_lay, i - net * p.img_lay.P, th, p.image + (size_t)net * p.image_bytes, p.bwd_image ? p.bwd_image + (size_t)net * p.bwd_image_bytes : nullptr);
@@ -493,7 +523,7 @@ TSG_GETTER(tsg_adam, g_ts_adam)
 // launches so that the wait for the peers hides under other work (the next update's target forward runs between them): 2 = reduce + push; the LAST
 // block to finish its pushes publishes this rank's epoch flags (an arrival counter, nobody spins) and the next update's replay indices are drawn here;
 // 3 = poll the local flags, sum the ranks' copies, clip + Adam.
-template <int MODE>
+template <int MODE, int OPT>
 __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams rp, AdamParams ap, XchgParams xp, SampleParams sp, int pb, int ns,
                                                                     unsigned long long* barrier, unsigned long long target) {
   constexpr bool XCHG = MODE != 0;
@@ -524,7 +554,7 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
   }
   // this thread's optimiser state: the loads fly under the reductions and barriers below
   float m_i = 0.f, v_i = 0.f, th_i = 0.f;
-  if (MODE != 2 && q == 0 && i < ap.n) { m_i = ap.m[i]; v_i = ap.v[i]; th_i = ap.theta[i]; }
+  if (MODE != 2 && q == 0 && i < ap.n) { m_i = ap.m[i]; v_i = ap.v[i]; th_i = ap.theta[i]; }   // (loads an optimiser does not use are dead code)
   part[q][lane] = s;
   __syncthreads();
   TSG(g_ts_adam, 2);
@@ -631,11 +661,10 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
   if (q == 0 && i < ap.n) {
     const float gg = g * inv_fill * clip;
     float m = m_i, v = v_i, th = th_i;
-    m = m + (gg - m) * (1.f - ap.beta1);                       // exp_avg.lerp_(grad, 1 - beta1)
-    v = v * ap.beta2 + gg * gg * (1.f - ap.beta2);             // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-    const float denom = sqrtf(v) / ap.bc2_sqrt + ap.eps;
-    th = th - (ap.lr / ap.bc1) * (m / denom);
-    ap.m[i] = m; ap.v[i] = v; ap.theta[i] = th;
+    th = opt_step<OPT>(ap, gg, m, v, th);
+    if constexpr (opt_uses_m<OPT>()) ap.m[i] = m;
+    if constexpr (opt_uses_v<OPT>()) ap.v[i] = v;
+    ap.theta[i] = th;
     if (ap.image != nullptr && i < ap.img_nets * ap.img_lay.P) {
       const int net = i / ap.img_lay.P;
       pack_param(ap.img_lay, i - net * ap.img_lay.P, th, ap.image + (size_t)net * ap.image_bytes, ap.bwd_image ? ap.bwd_image + (size_t)net * ap.bwd_image_bytes : nullptr);
@@ -720,28 +749,53 @@ int launch_grad_reduce(const ReduceParams& p, cudaStream_t st) {
   return MARL_OK;
 }
 
+// Every instantiation of the two step kernels, by (mode, optimiser).  Mode 2 (push only) returns before the step: one instantiation serves
+// every optimiser.
+using TailFn = void (*)(ReduceParams, AdamParams, XchgParams, SampleParams, int, int, unsigned long long*, unsigned long long);
+template <int MODE>
+static TailFn tail_fn_mode(int opt) {
+  static const TailFn fns[kNumOpt] = {reduce_adam_kernel<MODE, kOptAdam>, reduce_adam_kernel<MODE, kOptAdamW>, reduce_adam_kernel<MODE, kOptRmsprop>,
+                                      reduce_adam_kernel<MODE, kOptAdagrad>, reduce_adam_kernel<MODE, kOptSgd>};
+  return fns[opt];
+}
+static TailFn tail_fn(int mode, int opt) {
+  switch (mode) {
+    case 0: return tail_fn_mode<0>(opt);
+    case 1: return tail_fn_mode<1>(opt);
+    case 2: return reduce_adam_kernel<2, kOptAdam>;
+    default: return tail_fn_mode<3>(opt);
+  }
+}
+using StepFn = void (*)(AdamParams);
+static StepFn step_fn(int opt) {
+  static const StepFn fns[kNumOpt] = {adam_kernel<kOptAdam>, adam_kernel<kOptAdamW>, adam_kernel<kOptRmsprop>, adam_kernel<kOptAdagrad>, adam_kernel<kOptSgd>};
+  return fns[opt];
+}
+
 // Fused tail; returns MARL_EINVAL without launching when no co-resident grid covers the parameters (the caller then uses the two
 // kernels).  The hand-made grid barrier needs every block resident at once, so the block shape follows from the device: capacity =
-// SMs x (blocks of 1024 threads per SM, from the occupancy API: 1 at this kernel's register count), pb = parameters per block =
-// ceil(n / capacity) rounded up to a warp multiple, ns = slices = 1024 / pb.
+// SMs x (blocks of 1024 threads per SM, from the occupancy API of the instantiation that will run: 1 at these kernels' register counts),
+// pb = parameters per block = ceil(n / capacity) rounded up to a warp multiple, ns = slices = 1024 / pb.
 // xp: NULL or world == 1 -> single GPU; else the exchange over peer memory (xp->epoch is advanced here).
-int reduce_adam_shape(int n, int n_sm, bool xchg, int* pb_out, int* ns_out) {
-  static int occ[2] = {0, 0};
-  if (occ[xchg] == 0) {
+int reduce_adam_shape(int n, int n_sm, bool xchg, int opt, int* pb_out, int* ns_out) {
+  MARL_REQUIRE(opt >= 0 && opt < kNumOpt, "reduce_adam_shape: optimizer kind %d unknown", opt);
+  static int occ[2][kNumOpt] = {};
+  int& oc = occ[xchg][opt];
+  if (oc == 0) {
     int o = 0;
     if (xchg) {   // the split form shares the block shape: the smaller occupancy of the three variants counts
       int o1 = 0, o2 = 0, o3 = 0;
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o1, reduce_adam_kernel<1>, kFusedThreads, 0));
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o2, reduce_adam_kernel<2>, kFusedThreads, 0));
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o3, reduce_adam_kernel<3>, kFusedThreads, 0));
+      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o1, tail_fn(1, opt), kFusedThreads, 0));
+      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o2, tail_fn(2, opt), kFusedThreads, 0));
+      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o3, tail_fn(3, opt), kFusedThreads, 0));
       o = o1 < o2 ? o1 : o2; o = o < o3 ? o : o3;
     } else {
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, reduce_adam_kernel<0>, kFusedThreads, 0));
+      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, tail_fn(0, opt), kFusedThreads, 0));
     }
-    occ[xchg] = o > 0 ? o : -1;
+    oc = o > 0 ? o : -1;
   }
-  if (occ[xchg] < 1) return MARL_EINVAL;
-  const int capacity = n_sm * occ[xchg];
+  if (oc < 1) return MARL_EINVAL;
+  const int capacity = n_sm * oc;
   const int pb = ((n + capacity - 1) / capacity + 31) / 32 * 32;
   if (pb < 128 || pb > kFusedMaxParams) return MARL_EINVAL;
   int ns = kFusedThreads / pb;
@@ -751,22 +805,22 @@ int reduce_adam_shape(int n, int n_sm, bool xchg, int* pb_out, int* ns_out) {
   return MARL_OK;
 }
 
-int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier, unsigned long long* epoch,
-                       int n_sm, cudaStream_t st) {
+int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
+                       unsigned long long* epoch, int n_sm, cudaStream_t st) {
   const bool xchg = xp != nullptr && xp->world > 1;
   const int n = rp.n_nets * rp.P;
   int pb = 0, ns = 0;
-  if (ap.n != n || reduce_adam_shape(n, n_sm, xchg, &pb, &ns) != MARL_OK) return MARL_EINVAL;
+  if (ap.n != n || reduce_adam_shape(n, n_sm, xchg, opt, &pb, &ns) != MARL_OK) return MARL_EINVAL;
   const int grid = (n + pb - 1) / pb;   // <= capacity by construction
   XchgParams x; memset(&x, 0, sizeof(x));
   if (xchg) {
     xp->epoch += 1;
     x = *xp;
     *epoch += 2ULL * (unsigned long long)grid;               // two arrival rounds
-    MARL_CUDA_TRY(launch_pdl(reduce_adam_kernel<1>, dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
+    MARL_CUDA_TRY(launch_pdl(tail_fn(1, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
   } else {
     *epoch += (unsigned long long)grid;
-    MARL_CUDA_TRY(launch_pdl(reduce_adam_kernel<0>, dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
+    MARL_CUDA_TRY(launch_pdl(tail_fn(0, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
   }
   return MARL_OK;
 }
@@ -774,30 +828,32 @@ int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, XchgParams*
 // The exchange split over two launches (several ranks): launch_reduce_push, then whatever should hide the wait for the peers, then launch_adam_finish.
 // barrier[0] counts the finishing kernel's grid-barrier arrivals, barrier[1] the pushing kernel's block arrivals (epoch / push_epoch: their values once
 // the respective launch has fully arrived).
-int launch_reduce_push(const ReduceParams& rp, const AdamParams& ap, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier, unsigned long long* push_epoch,
-                       int n_sm, cudaStream_t st) {
+int launch_reduce_push(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
+                       unsigned long long* push_epoch, int n_sm, cudaStream_t st) {
   const int n = rp.n_nets * rp.P;
   int pb = 0, ns = 0;
-  if (xp == nullptr || xp->world <= 1 || ap.n != n || reduce_adam_shape(n, n_sm, true, &pb, &ns) != MARL_OK) return MARL_EINVAL;
+  if (xp == nullptr || xp->world <= 1 || ap.n != n || reduce_adam_shape(n, n_sm, true, opt, &pb, &ns) != MARL_OK) return MARL_EINVAL;
   const int grid = (n + pb - 1) / pb;
   xp->epoch += 1;
   *push_epoch += (unsigned long long)grid;
-  MARL_CUDA_TRY(launch_pdl(reduce_adam_kernel<2>, dim3(grid), dim3(pb * ns), 0, st, rp, ap, *xp, sp, pb, ns, barrier, *push_epoch));
+  MARL_CUDA_TRY(launch_pdl(tail_fn(2, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, *xp, sp, pb, ns, barrier, *push_epoch));
   return MARL_OK;
 }
-int launch_adam_finish(const ReduceParams& rp, const AdamParams& ap, XchgParams* xp, unsigned long long* barrier, unsigned long long* epoch, int n_sm, cudaStream_t st) {
+int launch_adam_finish(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, unsigned long long* barrier, unsigned long long* epoch, int n_sm,
+                       cudaStream_t st) {
   const int n = rp.n_nets * rp.P;
   int pb = 0, ns = 0;
-  if (xp == nullptr || xp->world <= 1 || reduce_adam_shape(n, n_sm, true, &pb, &ns) != MARL_OK) return MARL_EINVAL;
+  if (xp == nullptr || xp->world <= 1 || reduce_adam_shape(n, n_sm, true, opt, &pb, &ns) != MARL_OK) return MARL_EINVAL;
   const int grid = (n + pb - 1) / pb;
   SampleParams none; memset(&none, 0, sizeof(none));
   *epoch += (unsigned long long)grid;                          // one arrival round
-  MARL_CUDA_TRY(launch_pdl(reduce_adam_kernel<3>, dim3(grid), dim3(pb * ns), 0, st, rp, ap, *xp, none, pb, ns, barrier, *epoch));
+  MARL_CUDA_TRY(launch_pdl(tail_fn(3, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, *xp, none, pb, ns, barrier, *epoch));
   return MARL_OK;
 }
 
-int launch_adam(const AdamParams& p, cudaStream_t st) {
-  MARL_CUDA_TRY(launch_pdl(adam_kernel, dim3((p.n + 255) / 256), dim3(256), 0, st, p));
+int launch_adam(const AdamParams& p, int opt, cudaStream_t st) {
+  MARL_REQUIRE(opt >= 0 && opt < kNumOpt, "launch_adam: optimizer kind %d unknown", opt);
+  MARL_CUDA_TRY(launch_pdl(step_fn(opt), dim3((p.n + 255) / 256), dim3(256), 0, st, p));
   return MARL_OK;
 }
 

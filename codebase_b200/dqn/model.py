@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 from .. import _native as nat
+from .. import optimizers
 from ..lbf import TrajStore
 
 HIDDEN = 128
@@ -119,9 +120,7 @@ class QNetwork:
         if list(layers) != [HIDDEN, HIDDEN]:
             raise NotImplementedError(f"layers={list(layers)}: the fused kernels implement the shipped [128, 128] network only "
                                       f"({'one 128-wide GRU layer' if use_rnn else 'MLP'})")
-        opt = getattr(cfg, "optimizer", "Adam")
-        if (opt if isinstance(opt, str) else opt.__name__) != "Adam":
-            raise NotImplementedError("only optimizer=Adam is implemented")
+        self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
             raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
         self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
@@ -147,6 +146,7 @@ class QNetwork:
             create = self._lib.marl_dqn_create_rnn if self.use_rnn else self._lib.marl_dqn_create
             nat.check(create(C.byref(mcfg), C.byref(hp), C.c_int32(self.max_batch), C.c_int32(self.max_T), C.c_int32(self.device.index),
                              C.byref(self._h)), "marl_dqn_create_rnn" if self.use_rnn else "marl_dqn_create")
+        optimizers.apply(self._lib, "marl_dqn_set_optimizer", self._h, self.optimizer_name)
         ptrs = [C.c_void_p() for _ in range(5)]
         n = C.c_int64()
         nat.check(self._lib.marl_dqn_param_ptrs(self._h, *[C.byref(p) for p in ptrs], C.byref(n)), "marl_dqn_param_ptrs")
@@ -169,6 +169,11 @@ class QNetwork:
         nat.check(self._lib.marl_dqn_ret_ms_ptrs(self._h, C.byref(pm), C.byref(pc), C.byref(n)), "marl_dqn_ret_ms_ptrs")
         ms = nat.device_view(pm.value, 2 * n.value, self.device).cpu()
         return ms[: n.value], ms[n.value:], float(nat.device_view(pc.value, 1, self.device, "<f8").cpu()[0])
+
+    def optimizer_state(self):
+        """The optimiser state by torch's names (Adam / AdamW: exp_avg, exp_avg_sq; RMSprop: square_avg; Adagrad: sum; SGD: none), flat [n_params]
+        device views in the layout of `theta`."""
+        return optimizers.state(self.optimizer_name, self.adam_m, self.adam_v)
 
     # ---- reference API ------------------------------------------------------------------------------------------
     def init_hiddens(self, batch_size):
@@ -408,6 +413,12 @@ class QMixNetwork(QNetwork):
             parts += [lin.weight.data.reshape(-1), lin.bias.data.reshape(-1)]
         self.mix.copy_(torch.cat(parts).float())
         self.hard_update()
+
+    def optimizer_state(self):
+        """QNetwork.optimizer_state() plus the mixer's state under "mixer.<name>" (one optimiser over critic + mixer, as the reference's)."""
+        st = super().optimizer_state()
+        st.update({f"mixer.{k}": t for k, t in optimizers.state(self.optimizer_name, self.mix_m, self.mix_v).items()})
+        return st
 
     def _mixer_shapes(self):
         return mixer_shapes(self.n_agents, self.state_dim, self.embed_dim, self.hypernet_embed, self.hypernet_layers)

@@ -178,6 +178,29 @@ typedef struct {
 
 typedef struct marl_dqn marl_dqn;
 
+/* The optimiser of a learner (algorithm.optimizer): the reference builds torch.optim.<name>(parameters, lr=cfg.lr) with torch's defaults for
+ * everything else (marlbase/dqn/model.py:66-71,368-371, ac/model.py:103-109).  Each step runs per parameter on the gradient after
+ * clip_grad_norm_ (g), with lr = hp.lr, as torch's single-tensor implementation does:
+ *   MARL_OPT_ADAM     exp_avg (adam_m), exp_avg_sq (adam_v): Adam with bias correction; beta1, beta2, eps
+ *   MARL_OPT_ADAMW    theta *= 1 - lr * weight_decay, then the Adam step
+ *   MARL_OPT_RMSPROP  square_avg (adam_v): s = alpha * s + (1 - alpha) * g^2; theta -= lr * g / (sqrt(s) + eps)
+ *   MARL_OPT_ADAGRAD  sum (adam_v): s += g^2; theta -= lr * g / (sqrt(s) + eps)   (lr_decay 0, initial accumulator 0)
+ *   MARL_OPT_SGD      theta -= lr * g   (no state; momentum 0)
+ * torch's defaults: Adam betas (0.9, 0.999), eps 1e-8; AdamW the same and weight_decay 0.01; RMSprop alpha 0.99, eps 1e-8; Adagrad eps 1e-10.
+ * Fields an optimiser does not use are ignored. */
+#define MARL_OPT_ADAM 0
+#define MARL_OPT_ADAMW 1
+#define MARL_OPT_RMSPROP 2
+#define MARL_OPT_ADAGRAD 3
+#define MARL_OPT_SGD 4
+typedef struct {   /* the constants as torch holds them (Python floats); the step rounds them where torch does */
+  int32_t kind;           /* MARL_OPT_* */
+  double  beta1, beta2;   /* Adam, AdamW */
+  double  alpha;          /* RMSprop */
+  double  eps;            /* Adam, AdamW, RMSprop, Adagrad */
+  double  weight_decay;   /* AdamW (decoupled) */
+} marl_optimizer;
+
 int marl_dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device,
                     marl_dqn** out);
 int marl_dqn_destroy(marl_dqn* q);
@@ -231,6 +254,9 @@ int marl_dqn_update(marl_dqn* q, const marl_traj_view* traj, const int32_t* epis
 int marl_dqn_update_n(marl_dqn* q, const marl_traj_view* traj, int32_t batch, int32_t n_valid, uint64_t seed,
                       uint64_t first_update_idx, int32_t n_updates, float* loss_out, void* stream);
 int marl_dqn_counters(marl_dqn* q, int64_t* updates, int64_t* last_target_update);
+/* Choose the optimiser (MLP and recurrent handles; QMIX: the mixer takes the same one, unclipped).  Without this call the handle runs Adam with
+ * hp.beta1 / beta2 / eps.  Zeroes adam_m / adam_v (and the mixer's); refused (MARL_EINVAL) once the handle has taken an optimiser step. */
+int marl_dqn_set_optimizer(marl_dqn* q, const marl_optimizer* opt);
 /* Multi-GPU (one process per GPU on one NVLink node; replaces the torch.distributed all-reduce a data-parallel port of
  * dqn/train.py would add between loss.backward() and optimiser.step()): marl_dqn_peer_handle allocates this rank's exchange buffer
  * and writes its 64-byte CUDA IPC handle; the caller gathers all ranks' handles (rank-ordered, 64 bytes each) and passes them to
@@ -305,6 +331,9 @@ int marl_a2c_update_grads(marl_a2c* a, const marl_traj_view* batch, int32_t n_en
 int marl_a2c_update_apply(marl_a2c* a, int64_t step, float* metrics_out, void* stream);
 int marl_a2c_update(marl_a2c* a, const marl_traj_view* batch, int32_t n_envs, int64_t step, float* metrics_out,
                     void* stream);
+/* Choose the optimiser of actor and critic (one optimiser over both, as the reference's; MLP and recurrent handles).  Without this call the handle
+ * runs Adam with hp.beta1 / beta2 / eps.  Zeroes adam_m / adam_v; refused (MARL_EINVAL) once the handle has taken an optimiser step. */
+int marl_a2c_set_optimizer(marl_a2c* a, const marl_optimizer* opt);
 /* cfg.standardise_returns of the actor-critic learners (marlbase/ac/model.py:112-114,195-204,272-281; utils/standardise_stream.py:6-43): a
  * RunningMeanStd(shape=(n_agents,)) over the n-step returns of every update -- the bootstrap values are de-standardised with the statistics so far,
  * the statistics absorb the batch's returns (all T x P of them, unmasked), the returns are standardised.  enable != 0 initialises them on first use. */
