@@ -35,6 +35,14 @@ class LbfState(C.Structure):
     ]
 
 
+class RwareCfg(C.Structure):
+    _fields_ = [
+        ("shelf_rows", C.c_int32), ("shelf_columns", C.c_int32), ("column_height", C.c_int32), ("n_agents", C.c_int32),
+        ("request_queue_size", C.c_int32), ("max_steps", C.c_int32), ("max_inactivity_steps", C.c_int32), ("sensor_range", C.c_int32),
+        ("time_limit", C.c_int32), ("cooperative_reward", C.c_int32), ("observe_id", C.c_int32), ("standardise_rewards", C.c_int32),
+    ]
+
+
 class TrajView(C.Structure):
     _fields_ = [
         ("obs", C.c_void_p), ("act", C.c_void_p), ("rew", C.c_void_p), ("done", C.c_void_p), ("filled", C.c_void_p),

@@ -33,6 +33,7 @@ constexpr uint32_t kTagReset = 0x52455345u;   // env spawns: ctr = (env_gid, epi
 constexpr uint32_t kTagAct = 0x41435430u;     // epsilon-greedy: ctr = (env_gid, episode, t, block)
 constexpr uint32_t kTagCat = 0x43415430u;     // categorical:    ctr = (env_gid, episode, t, block)
 constexpr uint32_t kTagSample = 0x53414d50u;  // replay sampling: ctr = (update_lo, update_hi, block, 0)
+constexpr uint32_t kTagRequest = 0x52455155u; // RWARE replacement requests: ctr = (env_gid, episode, step, goal)
 
 struct u32x4 { uint32_t x, y, z, w; };
 

@@ -1,0 +1,126 @@
+// env_common.cuh -- the parts of an env-step kernel that do not depend on the environment (sm_90a): the fused action selection
+// (epsilon-greedy, categorical), marlbase's StandardiseReward and CooperativeReward wrappers and the trajectory-store writes.
+// Included by lbf_env.cu and rware_env.cu.  Lanes of one env form a group of G consecutive lanes starting at `gbase`; `sub` is the agent.
+#pragma once
+#include "common.cuh"
+
+namespace marl {
+
+struct TrajDev {
+  float* obs; int32_t* act; float* rew; uint8_t* done; uint8_t* filled; int capacity, T; int enabled;
+};
+
+struct StepArgs {
+  int E; uint64_t seed; uint32_t gid0;
+  int policy;  // 0 explicit actions, 1 eps-greedy over values, 2 categorical over logits
+  const int32_t* actions; const float* values; float epsilon; int n_actions;
+  float* obs_out; float* rew_out; uint8_t* done_out; uint8_t* trunc_out; float* final_ret; int32_t* final_len;
+  int32_t* actions_out;
+  int autoreset, use_proper_termination, clear_stale, slot0;
+};
+
+// Sequential 32-bit draws of one (seed, env, episode) reset: draw i = word i % 4 of Philox block (env_gid, episode, i / 4, 0)
+struct DrawStream {
+  uint32_t k0, k1, gid, ep, n; u32x4 buf;
+  __device__ DrawStream(uint64_t seed, uint32_t gid_, uint32_t ep_)
+      : k0((uint32_t)seed), k1((uint32_t)(seed >> 32) ^ kTagReset), gid(gid_), ep(ep_), n(0), buf{0, 0, 0, 0} {}
+  __device__ uint32_t next() {
+    if ((n & 3u) == 0) buf = philox4x32_10(gid, ep, n >> 2, 0u, k0, k1);
+    return pick(buf, (n++) & 3u);
+  }
+  __device__ int randint(int lo, int hi) { return lo + (int)bounded(next(), (uint32_t)(hi - lo)); }
+};
+
+// dqn/model.py:105-115: one uniform per step decides the joint exploration
+__device__ __forceinline__ int select_eps_greedy(const StepArgs& a, uint32_t gid, uint32_t ep_cur, int step0, int e, int N, int sub) {
+  const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32) ^ kTagAct;
+  const u32x4 b0 = philox4x32_10(gid, ep_cur, (uint32_t)step0, 0u, k0, k1);
+  const float* q = a.values + ((size_t)e * N + sub) * a.n_actions;
+  int a_raw = 0;
+  if (a.epsilon > u01(b0.x)) {
+    const u32x4 bj = philox4x32_10(gid, ep_cur, (uint32_t)step0, 1u + (uint32_t)(sub >> 2), k0, k1);
+    a_raw = (int)bounded(pick(bj, sub & 3), (uint32_t)a.n_actions);
+  } else {
+    float best = q[0];
+    for (int k = 1; k < a.n_actions; ++k) { const float v = q[k]; if (v > best) { best = v; a_raw = k; } }
+  }
+  return a_raw;
+}
+
+// ac/model.py:150-152: Categorical(logits).sample() by inverse CDF on a Philox uniform
+__device__ __forceinline__ int select_categorical(const StepArgs& a, uint32_t gid, uint32_t ep_cur, int step0, int e, int N, int sub) {
+  const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32) ^ kTagCat;
+  const u32x4 bj = philox4x32_10(gid, ep_cur, (uint32_t)step0, (uint32_t)(sub >> 2), k0, k1);
+  const float u = u01(pick(bj, sub & 3));
+  const float* lg = a.values + ((size_t)e * N + sub) * a.n_actions;
+  float m = lg[0];
+  for (int k = 1; k < a.n_actions; ++k) m = fmaxf(m, lg[k]);
+  float tot = 0.f;
+  for (int k = 0; k < a.n_actions; ++k) tot += expf(lg[k] - m);
+  const float thresh = u * tot;
+  float cum = 0.f;
+  int a_raw = a.n_actions - 1;
+  for (int k = 0; k < a.n_actions; ++k) { cum += expf(lg[k] - m); if (thresh < cum) { a_raw = k; break; } }
+  return a_raw;
+}
+
+// StandardiseReward.reward (wrappers.py:119-141), the wrapper's numpy arithmetic: float32 state arrays, float64 where the python-float reward list
+// enters (q, r, the standardised reward), float32 for the variance.  RecordEpisodeStatistics sits inside it and keeps the raw reward.
+// st: the env's state wmean[N] | t[N] | sumw; n: its reward count.  Every lane of the warp calls it (it has a __syncwarp).
+__device__ __forceinline__ double standardise_reward(float* st, int32_t* n_ptr, int N, int sub, bool alive, double rew) {
+  double rew_w = rew;
+  float wmean = 0.f, tt = 0.f, sumw = 0.f; int n = 0;
+  if (alive) { wmean = st[sub]; tt = st[N + sub]; sumw = st[2 * N]; n = *n_ptr; }
+  __syncwarp();   // every agent lane has read sumw / n before lane 0 of the env writes them
+  if (alive) {
+    const double q = __dsub_rn(rew, (double)wmean);                                        // (no FMA contraction: numpy rounds every operation)
+    const float temp_sumw = __fadd_rn(sumw, 1.0f);
+    const double r = __ddiv_rn(q, (double)temp_sumw);
+    wmean = (float)__dadd_rn((double)wmean, r);
+    tt = (float)__dadd_rn((double)tt, __dmul_rn(__dmul_rn(q, r), (double)sumw));
+    n += 1;
+    st[sub] = wmean; st[N + sub] = tt;
+    if (sub == 0) { st[2 * N] = temp_sumw; *n_ptr = n; }
+    if (n > 1) {
+      const float var = __fdiv_rn(__fmul_rn(tt, (float)n), __fmul_rn(temp_sumw, (float)(n - 1)));
+      rew_w = __ddiv_rn(__dsub_rn(rew, (double)wmean), (double)__fadd_rn(__fsqrt_rn(var), 1e-6f));
+    }
+  }
+  return rew_w;
+}
+
+// CooperativeReward: python sum() over agents in index order
+__device__ __forceinline__ double cooperative_sum(double rew_w, int gbase, int N) {
+  double tot = 0.0;
+  for (int i = 0; i < N; ++i) {
+    const double ri = __shfl_sync(0xFFFFFFFFu, rew_w, gbase + i);
+    tot += ri;
+  }
+  return tot;
+}
+
+// trajectory scalars (rb.add, dqn/train.py:73-89; batch_* writes, ac/train.py:90-99) of env e.  Returns the slot whose observation row
+// step1 this step fills, -1 for none.
+__device__ __forceinline__ int traj_write_scalars(const TrajDev& traj, const StepArgs& a, int e, int N, int sub, bool active, int step0, int a_raw,
+                                                  float rew_f, bool done, bool finished) {
+  int slot = -1;
+  const int step1 = step0 + 1;
+  const int sl = (a.slot0 + e) % traj.capacity;
+  if (active && step0 < traj.T) {
+    slot = sl;
+    if (sub < N) {
+      traj.act[((size_t)sl * N + sub) * traj.T + step0] = a_raw;
+      traj.rew[((size_t)sl * N + sub) * traj.T + step0] = rew_f;
+    }
+    if (sub == 0) {
+      traj.done[(size_t)sl * (traj.T + 1) + step1] = (uint8_t)(a.use_proper_termination ? done : finished);
+      traj.filled[(size_t)sl * traj.T + step0] = 1;
+    }
+  } else if (!active && a.clear_stale && sub == 0 && step0 < traj.T) {
+    // steps after the episode ended: the reference leaves a reused slot's old tail in place (SURVEY H6)
+    for (int t = step0; t < traj.T; ++t) traj.filled[(size_t)sl * traj.T + t] = 0;
+  }
+  return slot;
+}
+
+}  // namespace marl

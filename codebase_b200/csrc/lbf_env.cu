@@ -15,7 +15,7 @@
 //   * collisions: __match_any_sync on (env, target cell); loading: __ballot_sync of the adjacent loading
 //     lanes + shuffle reduction of their levels, food cells resolved in ascending agent order;
 //   * observations are assembled in shared memory and written back as one contiguous coalesced run.
-#include "common.cuh"
+#include "env_common.cuh"
 #include <string.h>
 
 namespace marl {
@@ -35,36 +35,11 @@ struct LbfStateDev {
   int32_t* stdr_n;   // [E] number of rewards seen
 };
 
-struct TrajDev {
-  float* obs; int32_t* act; float* rew; uint8_t* done; uint8_t* filled; int capacity, T; int enabled;
-};
-
-struct StepArgs {
-  int E; uint64_t seed; uint32_t gid0;
-  int policy;  // 0 explicit actions, 1 eps-greedy over values, 2 categorical over logits
-  const int32_t* actions; const float* values; float epsilon; int n_actions;
-  float* obs_out; float* rew_out; uint8_t* done_out; uint8_t* trunc_out; float* final_ret; int32_t* final_len;
-  int32_t* actions_out;
-  int autoreset, use_proper_termination, clear_stale, slot0;
-};
-
 constexpr int kThreads = 128;
 constexpr int kMaxFood = 32;
 
 __device__ __forceinline__ int imin(int a, int b) { return a < b ? a : b; }
 __device__ __forceinline__ int imax(int a, int b) { return a > b ? a : b; }
-
-// ---- spawning (ForagingEnv.spawn_players / spawn_food) ----------------------------------------------------
-struct DrawStream {
-  uint32_t k0, k1, gid, ep, n; u32x4 buf;
-  __device__ DrawStream(uint64_t seed, uint32_t gid_, uint32_t ep_)
-      : k0((uint32_t)seed), k1((uint32_t)(seed >> 32) ^ kTagReset), gid(gid_), ep(ep_), n(0), buf{0, 0, 0, 0} {}
-  __device__ uint32_t next() {
-    if ((n & 3u) == 0) buf = philox4x32_10(gid, ep, n >> 2, 0u, k0, k1);
-    return pick(buf, (n++) & 3u);
-  }
-  __device__ int randint(int lo, int hi) { return lo + (int)bounded(next(), (uint32_t)(hi - lo)); }
-};
 
 // upstream _is_empty_location: no food on the cell and no player position equal to it.  Default: the players placed so far (positions were cleared);
 // upstream_reset: every player that has a position -- level byte > 0 -- including the not yet re-placed ones of the previous episode.
@@ -288,30 +263,10 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   if (alive) {
     if (a.policy == 0) {
       a_raw = a.actions[(size_t)e * c.N + sub];
-    } else if (a.policy == 1) {  // dqn/model.py:105-115: one uniform per step decides the joint exploration
-      const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32) ^ kTagAct;
-      const u32x4 b0 = philox4x32_10(gid, ep_cur, (uint32_t)step0, 0u, k0, k1);
-      const float* q = a.values + ((size_t)e * c.N + sub) * a.n_actions;
-      if (a.epsilon > u01(b0.x)) {
-        const u32x4 bj = philox4x32_10(gid, ep_cur, (uint32_t)step0, 1u + (uint32_t)(sub >> 2), k0, k1);
-        a_raw = (int)bounded(pick(bj, sub & 3), (uint32_t)a.n_actions);
-      } else {
-        float best = q[0];
-        for (int k = 1; k < a.n_actions; ++k) { const float v = q[k]; if (v > best) { best = v; a_raw = k; } }
-      }
-    } else {  // ac/model.py:150-152: Categorical(logits).sample() by inverse CDF on a Philox uniform
-      const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32) ^ kTagCat;
-      const u32x4 bj = philox4x32_10(gid, ep_cur, (uint32_t)step0, (uint32_t)(sub >> 2), k0, k1);
-      const float u = u01(pick(bj, sub & 3));
-      const float* lg = a.values + ((size_t)e * c.N + sub) * a.n_actions;
-      float m = lg[0];
-      for (int k = 1; k < a.n_actions; ++k) m = fmaxf(m, lg[k]);
-      float tot = 0.f;
-      for (int k = 0; k < a.n_actions; ++k) tot += expf(lg[k] - m);
-      const float thresh = u * tot;
-      float cum = 0.f;
-      a_raw = a.n_actions - 1;
-      for (int k = 0; k < a.n_actions; ++k) { cum += expf(lg[k] - m); if (thresh < cum) { a_raw = k; break; } }
+    } else if (a.policy == 1) {
+      a_raw = select_eps_greedy(a, gid, ep_cur, step0, e, c.N, sub);
+    } else {
+      a_raw = select_categorical(a, gid, ep_cur, step0, e, c.N, sub);
     }
   }
   if (a.actions_out && env_ok && sub < c.N) a.actions_out[(size_t)e * c.N + sub] = a_raw;
@@ -375,34 +330,9 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   const bool trunc = active && (c.time_limit > 0 && step1 >= c.time_limit);
   const bool finished = done || trunc;
 
-  // StandardiseReward.reward (wrappers.py:119-141), the wrapper's numpy arithmetic: float32 state arrays, float64 where the python-float reward list
-  // enters (q, r, the standardised reward), float32 for the variance.  RecordEpisodeStatistics sits inside it and keeps the raw reward.
   double rew_w = rew;
-  if (c.std_rew) {
-    float wmean = 0.f, tt = 0.f, sumw = 0.f; int n = 0;
-    float* st = s.stdr + (size_t)(env_ok ? e : 0) * (2 * c.N + 1);
-    if (alive) { wmean = st[sub]; tt = st[c.N + sub]; sumw = st[2 * c.N]; n = s.stdr_n[e]; }
-    __syncwarp();   // every agent lane has read sumw / n before lane 0 of the env writes them
-    if (alive) {
-      const double q = __dsub_rn(rew, (double)wmean);                                        // (no FMA contraction: numpy rounds every operation)
-      const float temp_sumw = __fadd_rn(sumw, 1.0f);
-      const double r = __ddiv_rn(q, (double)temp_sumw);
-      wmean = (float)__dadd_rn((double)wmean, r);
-      tt = (float)__dadd_rn((double)tt, __dmul_rn(__dmul_rn(q, r), (double)sumw));
-      n += 1;
-      st[sub] = wmean; st[c.N + sub] = tt;
-      if (sub == 0) { st[2 * c.N] = temp_sumw; s.stdr_n[e] = n; }
-      if (n > 1) {
-        const float var = __fdiv_rn(__fmul_rn(tt, (float)n), __fmul_rn(temp_sumw, (float)(n - 1)));
-        rew_w = __ddiv_rn(__dsub_rn(rew, (double)wmean), (double)__fadd_rn(__fsqrt_rn(var), 1e-6f));
-      }
-    }
-  }
-  double tot = 0.0;  // CooperativeReward: python sum() over agents in index order
-  for (int i = 0; i < c.N; ++i) {
-    const double ri = __shfl_sync(FULL, rew_w, gbase + i);
-    tot += ri;
-  }
+  if (c.std_rew) rew_w = standardise_reward(s.stdr + (size_t)(env_ok ? e : 0) * (2 * c.N + 1), s.stdr_n + (env_ok ? e : 0), c.N, sub, alive, rew);
+  const double tot = cooperative_sum(rew_w, gbase, c.N);
   const float rew_f = (float)(c.coop_reward ? tot : rew_w);
   float ep_ret = 0.f;
   if (alive) {
@@ -411,25 +341,8 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   }
   if (env_ok && sub < c.N) a.rew_out[(size_t)e * c.N + sub] = alive ? rew_f : 0.f;
 
-  // trajectory scalars (rb.add, dqn/train.py:73-89; batch_* writes, ac/train.py:90-99)
   int slot = -1;
-  if (traj.enabled && env_ok) {
-    const int sl = (a.slot0 + e) % traj.capacity;
-    if (active && step0 < traj.T) {
-      slot = sl;
-      if (sub < c.N) {
-        traj.act[((size_t)sl * c.N + sub) * traj.T + step0] = a_raw;
-        traj.rew[((size_t)sl * c.N + sub) * traj.T + step0] = rew_f;
-      }
-      if (sub == 0) {
-        traj.done[(size_t)sl * (traj.T + 1) + step1] = (uint8_t)(a.use_proper_termination ? done : finished);
-        traj.filled[(size_t)sl * traj.T + step0] = 1;
-      }
-    } else if (!active && a.clear_stale && sub == 0 && step0 < traj.T) {
-      // steps after the episode ended: the reference leaves a reused slot's old tail in place (SURVEY H6)
-      for (int t = step0; t < traj.T; ++t) traj.filled[(size_t)sl * traj.T + t] = 0;
-    }
-  }
+  if (traj.enabled && env_ok) slot = traj_write_scalars(traj, a, e, c.N, sub, active, step0, a_raw, rew_f, done, finished);
 
   // publish moved positions for the observation pass
   if (env_ok && sub < c.N) pl_s[le * G + sub] = (uint32_t)r | ((uint32_t)cc << 8) | ((uint32_t)lvl << 16);

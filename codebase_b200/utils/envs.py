@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from ..lbf import LbfConfig, NativeLbf, parse_env_id
+from ..rware import NativeRware, RwareConfig, is_rware_id, parse_rware_id
 from . import spaces
 
 SUPPORTED_WRAPPERS = {"CooperativeReward"}
@@ -30,15 +31,17 @@ class _Unwrapped:
 
 
 class B200VecEnv:
-    def __init__(self, cfg: LbfConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None):
+    def __init__(self, cfg: LbfConfig | RwareConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None):
         self.cfg, self.num_envs = cfg, int(parallel_envs)
-        self.native = NativeLbf(cfg, self.num_envs, seed, env_gid0, device)
+        rware = isinstance(cfg, RwareConfig)
+        self.native = (NativeRware if rware else NativeLbf)(cfg, self.num_envs, seed, env_gid0, device)
         self.n_agents = cfg.n_agents
         self.unwrapped = _Unwrapped(cfg.n_agents)
-        hi = float(max(cfg.rows, cfg.cols))
-        self.single_observation_space = spaces.Tuple([spaces.Box(-1.0, hi, (cfg.obs_dim,), np.float32)] * cfg.n_agents)
+        # LBF: coordinates and levels, -1 for absent entities; RWARE: coordinates, the rest 0 / 1
+        lo, hi = (0.0, float(max(cfg.rows, cfg.cols) - 1)) if rware else (-1.0, float(max(cfg.rows, cfg.cols)))
+        self.single_observation_space = spaces.Tuple([spaces.Box(lo, hi, (cfg.obs_dim,), np.float32)] * cfg.n_agents)
         self.single_action_space = spaces.Tuple([spaces.Discrete(cfg.n_actions)] * cfg.n_agents)
-        self.observation_space = spaces.Tuple([spaces.Box(-1.0, hi, (self.num_envs, cfg.obs_dim), np.float32)] * cfg.n_agents)
+        self.observation_space = spaces.Tuple([spaces.Box(lo, hi, (self.num_envs, cfg.obs_dim), np.float32)] * cfg.n_agents)
         self.action_space = spaces.Tuple([spaces.Discrete(cfg.n_actions)] * cfg.n_agents)
         self._t0 = perf_counter()
 
@@ -93,14 +96,15 @@ def episode_info(returns, length, seconds):
 def make_env(seed, enable_video=False, name=None, time_limit=None, clear_info=False, observe_id=False, standardise_rewards=False,
              wrappers=None, parallel_envs=None, env_gid0=0, device=None, **kwargs):
     """marlbase/utils/envs.py:115-119 with the same config keys.  `parallel_envs` absent -> 1 env (the reference's single-env
-    factory); the GPU overlays set it to thousands."""
+    factory); the GPU overlays set it to thousands.  `name`: a Level-Based Foraging id (codebase_b200.lbf) or a multi-robot warehouse id
+    (codebase_b200.rware); extra keys override the env's constructor arguments."""
     if enable_video:
         raise NotImplementedError("video recording is out of scope of the GPU hot path (algorithm.video_interval must stay False)")
     wrappers = list(wrappers or [])
     unknown = [w for w in wrappers if w not in SUPPORTED_WRAPPERS]
     if unknown:
         raise NotImplementedError(f"env.wrappers {unknown} are not implemented on the GPU path (supported: {sorted(SUPPORTED_WRAPPERS)})")
-    cfg = parse_env_id(name, time_limit or 0, **kwargs)
+    cfg = (parse_rware_id if is_rware_id(name) else parse_env_id)(name, time_limit or 0, **kwargs)
     cfg.cooperative_reward = int("CooperativeReward" in wrappers)
     cfg.observe_id, cfg.standardise_rewards = int(bool(observe_id)), int(bool(standardise_rewards))   # envs.py:97-101, inside the listed wrappers
     if seed is None:

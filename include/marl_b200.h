@@ -150,6 +150,51 @@ int marl_lbf_rollout_step(marl_lbf* env, const float* values, const marl_rollout
                           int32_t* actions_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
+ * Multi-robot warehouse (RWARE), E environments per handle, one transition of all of them per launch.
+ * Replaces `env.reset()` / `env.step(actions)` of the gym.make()'d third-party `rware` Warehouse (2.x, gymnasium; ids
+ * `rware-{tiny,small,medium,large}-{N}ag[-easy|-hard]-v2`) under the same wrapper stack as marl_lbf_*.  Semantics: DESIGN.md Appendix B.
+ * The entry points mirror the marl_lbf_* contracts; the trajectory view and the rollout arguments are the same structs.
+ * ---------------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t shelf_rows, shelf_columns;  /* grid = ((column_height + 1) * shelf_rows + 2) rows x (3 * shelf_columns + 1) columns */
+  int32_t column_height;              /* 8 for the registered ids */
+  int32_t n_agents;                   /* 1..31 */
+  int32_t request_queue_size;         /* requested shelves at any time; 1 .. shelves - 1 */
+  int32_t max_steps;                  /* env-internal horizon (terminates); 0 = none */
+  int32_t max_inactivity_steps;       /* terminates after this many steps without a delivery; 0 = None */
+  int32_t sensor_range;               /* 0..3; observation = 8 + 7 * (2r + 1)^2 floats */
+  int32_t time_limit;                 /* TimeLimit wrapper (truncates); 0 = absent */
+  int32_t cooperative_reward;         /* CooperativeReward wrapper */
+  int32_t observe_id;                 /* ObserveID wrapper: one-hot agent id in front of every observation */
+  int32_t standardise_rewards;        /* StandardiseReward wrapper, as marl_lbf_cfg.standardise_rewards */
+} marl_rware_cfg;
+
+typedef struct marl_rware marl_rware;
+
+int marl_rware_create(const marl_rware_cfg* cfg, int32_t n_envs, uint64_t seed, uint32_t env_gid0, int32_t device, marl_rware** out);
+int marl_rware_destroy(marl_rware* env);
+int marl_rware_obs_dim(const marl_rware_cfg* cfg);   /* 8 + 7 * (2 * sensor_range + 1)^2 (+ n_agents with observe_id) */
+/* Overwrite the transition state (device pointers): shelves uint8[E][rows*cols] (shelf id 1..255 at its current cell, 0 none; a carried shelf
+ * sits at its carrier's cell), agents uint8[E][N][4] = (x, y, direction, carried shelf id or 0), requested uint32[E][8] (bit k: shelf k is
+ * requested), step / inactive int32[E] (steps so far, steps since the last delivery).  Episode returns and lengths restart at 0. */
+int marl_rware_set_state(marl_rware* env, const uint8_t* shelves, const uint8_t* agents, const uint32_t* requested, const int32_t* step,
+                         const int32_t* inactive, void* stream);
+/* Copy the state out into caller-owned DEVICE buffers (any may be NULL), in the layout of marl_rware_set_state plus ep_return float[E][N],
+ * ep_len int32[E], episode_idx uint32[E], active uint8[E]. */
+int marl_rware_get_state(marl_rware* env, uint8_t* shelves, uint8_t* agents, uint32_t* requested, int32_t* step, int32_t* inactive,
+                         float* ep_return, int32_t* ep_len, uint32_t* episode_idx, uint8_t* active, void* stream);
+/* as marl_lbf_reset */
+int marl_rware_reset(marl_rware* env, const uint8_t* reset_mask, float* obs_out, const marl_traj_view* traj, int32_t slot0, void* stream);
+/* as marl_lbf_step; actions outside 0..4 act as NOOP */
+int marl_rware_step(marl_rware* env, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,
+                    float* final_ret_out, int32_t* final_len_out, int32_t autoreset, void* stream);
+/* as marl_lbf_rollout_step with args->policy = 2 (categorical on logits); policy 1 (epsilon-greedy) returns MARL_EINVAL: no DQN-family
+ * learner takes RWARE's observation width */
+int marl_rware_rollout_step(marl_rware* env, const float* values, const marl_rollout_args* args, const marl_traj_view* traj,
+                            float* obs_inout, float* rew_out, uint8_t* done_out, uint8_t* trunc_out, float* final_ret_out,
+                            int32_t* final_len_out, int32_t* actions_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------
  * Per-agent MLP sets and the DQN-family learner (IDQN, VDN).
  * Replaces marlbase/dqn/model.py QNetwork (14-196) / VDNetwork (199-269) and the network containers of
  * marlbase/utils/models.py:133-300.  Parameters are one flat float array [n_nets][P] in the reference's
