@@ -17,7 +17,7 @@ from .. import _native as nat
 from .. import optimizers
 from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dict, init_flat_params, init_flat_rnn_params, rnn_state_dict_to_flat,
                          sharing_to_nets, state_dict_to_flat)
-from ..lbf import TrajStore
+from ..native_env import TrajStore
 
 
 MAX_IN_DIM = 128   # widest actor / critic input of the actor-critic kernels (csrc/learner.cuh kMaxInDim)

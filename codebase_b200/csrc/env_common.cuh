@@ -1,7 +1,11 @@
 // env_common.cuh -- the parts of an env-step kernel that do not depend on the environment (sm_90a): the fused action selection
-// (epsilon-greedy, categorical), marlbase's StandardiseReward and CooperativeReward wrappers and the trajectory-store writes.
+// (epsilon-greedy, categorical), marlbase's StandardiseReward and CooperativeReward wrappers and the trajectory-store writes; and on the
+// host, the handle, buffer ownership, trajectory checks and step launch of the env C ABIs.
 // Included by lbf_env.cu and rware_env.cu.  Lanes of one env form a group of G consecutive lanes starting at `gbase`; `sub` is the agent.
 #pragma once
+#include <string.h>
+#include <initializer_list>
+#include <vector>
 #include "common.cuh"
 
 namespace marl {
@@ -121,6 +125,98 @@ __device__ __forceinline__ int traj_write_scalars(const TrajDev& traj, const Ste
     for (int t = step0; t < traj.T; ++t) traj.filled[(size_t)sl * traj.T + t] = 0;
   }
   return slot;
+}
+
+// ---- host side: the handle layer of the env C ABIs ----------------------------------------------------------------------------------------
+// A handle (marl_lbf, marl_rware) derives from EnvHandle and adds its config `cfg`, device config `dev` (with N and D) and state pointers `st`.
+struct EnvHandle {
+  int E, device;
+  uint64_t seed;
+  uint32_t gid0;
+  int envs_per_cta, threads;   // step kernel launch shape
+  size_t step_smem;
+  std::vector<void*> bufs;     // the device buffers the handle owns, released by env_destroy
+};
+
+struct DevBuf {
+  void** ptr; size_t bytes;
+  template <typename T> DevBuf(T** p, size_t n) : ptr(reinterpret_cast<void**>(p)), bytes(n) {}
+};
+
+// Zero-initialised device buffers, each recorded in h->bufs; stops at the first failure (the caller then destroys the handle).
+inline int alloc_buffers(EnvHandle* h, const char* who, std::initializer_list<DevBuf> list) {
+  for (const DevBuf& b : list) {
+    cudaError_t e = cudaMalloc(b.ptr, b.bytes);
+    if (e == cudaSuccess) { h->bufs.push_back(*b.ptr); e = cudaMemset(*b.ptr, 0, b.bytes); }
+    if (e != cudaSuccess) { set_error("%s: cudaMalloc(%zu) failed: %s", who, b.bytes, cudaGetErrorString(e)); return MARL_ENOMEM; }
+  }
+  return MARL_OK;
+}
+
+template <typename H>
+int env_destroy(H* h) {
+  if (!h) return MARL_OK;
+  cudaSetDevice(h->device);
+  for (void* p : h->bufs) cudaFree(p);
+  delete h;
+  return MARL_OK;
+}
+
+// The attribute is a per-function, process-wide setting: only ever raise it (a second env with a smaller tile must not lower the limit of the
+// first).  `limit` is the kernel's current limit, kept by the caller.
+template <typename K>
+int raise_smem_limit(K* kernel, size_t bytes, size_t& limit, const char* who) {
+  if (bytes <= limit) return MARL_OK;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e != cudaSuccess) { set_error("%s: %zu B of shared memory per CTA not available: %s", who, bytes, cudaGetErrorString(e)); return MARL_EINVAL; }
+  limit = bytes;
+  return MARL_OK;
+}
+
+inline TrajDev to_traj(const marl_traj_view* t) {
+  TrajDev d; memset(&d, 0, sizeof(d));
+  if (t) { d.obs = t->obs; d.act = t->act; d.rew = t->rew; d.done = t->done; d.filled = t->filled; d.capacity = t->capacity; d.T = t->T; d.enabled = 1; }
+  return d;
+}
+
+template <typename H>
+int check_traj(const H* env, const marl_traj_view* t) {
+  if (!t) return MARL_OK;
+  MARL_REQUIRE(t->obs && t->act && t->rew && t->done && t->filled, "traj view has NULL buffers");
+  MARL_REQUIRE(t->n_agents == env->dev.N && t->obs_dim == env->dev.D, "traj view shape (N=%d, obs=%d) does not match env (N=%d, obs=%d)", t->n_agents, t->obs_dim, env->dev.N, env->dev.D);
+  MARL_REQUIRE(t->capacity >= env->E && t->T >= 1, "traj capacity %d must hold one episode per env (%d)", t->capacity, env->E);
+  return MARL_OK;
+}
+
+// StepArgs of a step on explicit actions (policy 0)
+inline StepArgs step_args(const EnvHandle* h, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,
+                          float* final_ret_out, int32_t* final_len_out, int32_t autoreset) {
+  StepArgs a; memset(&a, 0, sizeof(a));
+  a.E = h->E; a.seed = h->seed; a.gid0 = h->gid0; a.policy = 0; a.actions = actions; a.obs_out = obs_out; a.rew_out = rew_out;
+  a.done_out = done_out; a.trunc_out = trunc_out; a.final_ret = final_ret_out; a.final_len = final_len_out; a.autoreset = autoreset;
+  return a;
+}
+
+// StepArgs of a rollout step, after the checks every env shares.  The caller has checked its pointers and the policy.
+template <typename H>
+int rollout_step_args(const H* h, const char* who, const float* values, const marl_rollout_args* ra, const marl_traj_view* traj, float* obs_inout,
+                      float* rew_out, uint8_t* done_out, uint8_t* trunc_out, float* final_ret_out, int32_t* final_len_out, int32_t* actions_out,
+                      StepArgs& a) {
+  MARL_REQUIRE(ra->n_actions >= 1 && ra->n_actions <= 64, "%s: n_actions out of range", who);
+  if (int rc = check_traj(h, traj)) return rc;
+  MARL_REQUIRE(!(traj && ra->autoreset), "%s: trajectory recording needs autoreset=0 (episode-synchronous collection)", who);
+  a = step_args(h, nullptr, obs_inout, rew_out, done_out, trunc_out, final_ret_out, final_len_out, ra->autoreset);
+  a.policy = ra->policy; a.values = values; a.epsilon = ra->epsilon; a.n_actions = ra->n_actions; a.actions_out = actions_out;
+  a.use_proper_termination = ra->use_proper_termination; a.clear_stale = ra->clear_stale; a.slot0 = ra->slot0;
+  return MARL_OK;
+}
+
+template <typename H, typename Dev, typename St>
+int launch_step(const H* h, void (*kernel)(Dev, St, StepArgs, TrajDev), const StepArgs& a, const marl_traj_view* traj, void* stream) {
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, h->threads, h->step_smem, (cudaStream_t)stream>>>(h->dev, h->st, a, to_traj(traj));
+  MARL_CUDA_TRY(cudaGetLastError());
+  return MARL_OK;
 }
 
 }  // namespace marl

@@ -16,7 +16,6 @@
 //     lanes + shuffle reduction of their levels, food cells resolved in ascending agent order;
 //   * observations are assembled in shared memory and written back as one contiguous coalesced run.
 #include "env_common.cuh"
-#include <string.h>
 
 namespace marl {
 
@@ -410,14 +409,10 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
 // =============================================================================================================
 using namespace marl;
 
-struct marl_lbf {
+struct marl_lbf : EnvHandle {
   marl_lbf_cfg cfg;
   LbfCfgDev dev;
   LbfStateDev st;
-  int E, device;
-  uint64_t seed;
-  uint32_t gid0;
-  size_t step_smem;
 };
 
 static int validate_cfg(const marl_lbf_cfg* c) {
@@ -441,22 +436,8 @@ static LbfCfgDev to_dev(const marl_lbf_cfg& c) {
   d.RC = c.rows * c.cols; d.pitch = (d.RC + 15) & ~15;
   int g = 1; while (g < c.n_agents) g <<= 1;
   d.obs_id = c.observe_id ? 1 : 0; d.std_rew = c.standardise_rewards ? 1 : 0; d.upstream_reset = c.upstream_reset ? 1 : 0;
-  d.G = g; d.D = 3 * c.max_num_food + 3 * c.n_agents + (d.obs_id ? c.n_agents : 0);
+  d.G = g; d.D = marl_lbf_obs_dim(&c);
   return d;
-}
-
-static TrajDev to_traj(const marl_traj_view* t) {
-  TrajDev d; memset(&d, 0, sizeof(d));
-  if (t) { d.obs = t->obs; d.act = t->act; d.rew = t->rew; d.done = t->done; d.filled = t->filled; d.capacity = t->capacity; d.T = t->T; d.enabled = 1; }
-  return d;
-}
-
-static int check_traj(const marl_lbf* env, const marl_traj_view* t) {
-  if (!t) return MARL_OK;
-  MARL_REQUIRE(t->obs && t->act && t->rew && t->done && t->filled, "traj view has NULL buffers");
-  MARL_REQUIRE(t->n_agents == env->dev.N && t->obs_dim == env->dev.D, "traj view shape (N=%d, obs=%d) does not match env (N=%d, obs=%d)", t->n_agents, t->obs_dim, env->dev.N, env->dev.D);
-  MARL_REQUIRE(t->capacity >= env->E && t->T >= 1, "traj capacity %d must hold one episode per env (%d)", t->capacity, env->E);
-  return MARL_OK;
 }
 
 extern "C" {
@@ -473,45 +454,21 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
   h->cfg = *cfg; h->dev = to_dev(*cfg); h->E = n_envs; h->device = device; h->seed = seed; h->gid0 = env_gid0;
   const LbfCfgDev& d = h->dev;
   const size_t E = (size_t)n_envs;
-  memset(&h->st, 0, sizeof(h->st));
-#define ALLOC0(ptr, bytes)                                                  \
-  do {                                                                      \
-    cudaError_t _e = cudaMalloc((void**)&(ptr), (bytes));                   \
-    if (_e == cudaSuccess) _e = cudaMemset((ptr), 0, (bytes));              \
-    if (_e != cudaSuccess) { set_error("marl_lbf_create: cudaMalloc(%zu) failed: %s", (size_t)(bytes), cudaGetErrorString(_e)); marl_lbf_destroy(h); return MARL_ENOMEM; } \
-  } while (0)
-  ALLOC0(h->st.field, E * d.pitch);
-  ALLOC0(h->st.players, E * d.N * 4);
-  ALLOC0(h->st.step, E * 4);
-  ALLOC0(h->st.food_spawned, E * 4);
-  ALLOC0(h->st.ep_return, E * d.N * 4);
-  ALLOC0(h->st.ep_len, E * 4);
-  ALLOC0(h->st.episode_idx, E * 4);
-  ALLOC0(h->st.active, E);
-  ALLOC0(h->st.stdr, E * (2 * d.N + 1) * 4);
-  ALLOC0(h->st.stdr_n, E * 4);
-#undef ALLOC0
   const int EPC = (kThreads / 32) * (32 / d.G);
+  h->envs_per_cta = EPC; h->threads = kThreads;
   h->step_smem = (size_t)EPC * (d.pitch + 4) + (size_t)EPC * d.G * 4 + (size_t)EPC * d.NF * 4 + (size_t)EPC * 16 + (size_t)EPC * d.N * d.D * 4;
-  // the attribute is a per-function, process-wide setting: only ever raise it (a second env with a smaller tile must not lower the limit of the first)
   static size_t step_smem_limit = 48 * 1024;
-  if (h->step_smem > step_smem_limit) {
-    cudaError_t e = cudaFuncSetAttribute(lbf_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->step_smem);
-    if (e == cudaSuccess) step_smem_limit = h->step_smem;
-    if (e != cudaSuccess) { set_error("marl_lbf_create: %zu B of shared memory per CTA not available: %s", h->step_smem, cudaGetErrorString(e)); marl_lbf_destroy(h); return MARL_EINVAL; }
-  }
+  int rc = alloc_buffers(h, "marl_lbf_create", {{&h->st.field, E * d.pitch}, {&h->st.players, E * d.N * 4}, {&h->st.step, E * 4},
+                                                {&h->st.food_spawned, E * 4}, {&h->st.ep_return, E * d.N * 4}, {&h->st.ep_len, E * 4},
+                                                {&h->st.episode_idx, E * 4}, {&h->st.active, E}, {&h->st.stdr, E * (2 * d.N + 1) * 4},
+                                                {&h->st.stdr_n, E * 4}});
+  if (rc == MARL_OK) rc = raise_smem_limit(lbf_step_kernel, h->step_smem, step_smem_limit, "marl_lbf_create");
+  if (rc != MARL_OK) { marl_lbf_destroy(h); return rc; }
   *out = h;
   return MARL_OK;
 }
 
-int marl_lbf_destroy(marl_lbf* h) {
-  if (!h) return MARL_OK;
-  cudaSetDevice(h->device);
-  cudaFree(h->st.field); cudaFree(h->st.players); cudaFree(h->st.step); cudaFree(h->st.food_spawned);
-  cudaFree(h->st.ep_return); cudaFree(h->st.ep_len); cudaFree(h->st.episode_idx); cudaFree(h->st.active); cudaFree(h->st.stdr); cudaFree(h->st.stdr_n);
-  delete h;
-  return MARL_OK;
-}
+int marl_lbf_destroy(marl_lbf* h) { return env_destroy(h); }
 
 int marl_lbf_state_ptrs(marl_lbf* h, marl_lbf_state* out) {
   MARL_REQUIRE(h && out, "marl_lbf_state_ptrs: NULL argument");
@@ -548,22 +505,11 @@ int marl_lbf_reset(marl_lbf* h, const uint8_t* reset_mask, float* obs_out, const
   return MARL_OK;
 }
 
-static int launch_step(marl_lbf* h, const StepArgs& a, const marl_traj_view* traj, void* stream) {
-  const int EPC = (kThreads / 32) * (32 / h->dev.G);
-  const int grid = (h->E + EPC - 1) / EPC;
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  lbf_step_kernel<<<grid, kThreads, h->step_smem, (cudaStream_t)stream>>>(h->dev, h->st, a, to_traj(traj));
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
-}
-
 int marl_lbf_step(marl_lbf* h, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,
                   float* final_ret_out, int32_t* final_len_out, int32_t autoreset, void* stream) {
   MARL_REQUIRE(h && actions && rew_out && done_out && trunc_out, "marl_lbf_step: NULL argument");
-  StepArgs a; memset(&a, 0, sizeof(a));
-  a.E = h->E; a.seed = h->seed; a.gid0 = h->gid0; a.policy = 0; a.actions = actions; a.obs_out = obs_out; a.rew_out = rew_out;
-  a.done_out = done_out; a.trunc_out = trunc_out; a.final_ret = final_ret_out; a.final_len = final_len_out; a.autoreset = autoreset;
-  return launch_step(h, a, nullptr, stream);
+  const StepArgs a = step_args(h, actions, obs_out, rew_out, done_out, trunc_out, final_ret_out, final_len_out, autoreset);
+  return launch_step(h, lbf_step_kernel, a, nullptr, stream);
 }
 
 int marl_lbf_rollout_step(marl_lbf* h, const float* values, const marl_rollout_args* ra, const marl_traj_view* traj, float* obs_inout,
@@ -571,14 +517,11 @@ int marl_lbf_rollout_step(marl_lbf* h, const float* values, const marl_rollout_a
                           int32_t* actions_out, void* stream) {
   MARL_REQUIRE(h && values && ra && rew_out && done_out && trunc_out, "marl_lbf_rollout_step: NULL argument");
   MARL_REQUIRE(ra->policy == 1 || ra->policy == 2, "marl_lbf_rollout_step: policy must be 1 (eps-greedy) or 2 (categorical)");
-  MARL_REQUIRE(ra->n_actions >= 1 && ra->n_actions <= 64, "marl_lbf_rollout_step: n_actions out of range");
-  if (int rc = check_traj(h, traj)) return rc;
-  MARL_REQUIRE(!(traj && ra->autoreset), "marl_lbf_rollout_step: trajectory recording needs autoreset=0 (episode-synchronous collection)");
-  StepArgs a; memset(&a, 0, sizeof(a));
-  a.E = h->E; a.seed = h->seed; a.gid0 = h->gid0; a.policy = ra->policy; a.values = values; a.epsilon = ra->epsilon; a.n_actions = ra->n_actions;
-  a.obs_out = obs_inout; a.rew_out = rew_out; a.done_out = done_out; a.trunc_out = trunc_out; a.final_ret = final_ret_out; a.final_len = final_len_out;
-  a.actions_out = actions_out; a.autoreset = ra->autoreset; a.use_proper_termination = ra->use_proper_termination; a.clear_stale = ra->clear_stale; a.slot0 = ra->slot0;
-  return launch_step(h, a, traj, stream);
+  StepArgs a;
+  if (int rc = rollout_step_args(h, "marl_lbf_rollout_step", values, ra, traj, obs_inout, rew_out, done_out, trunc_out, final_ret_out, final_len_out,
+                                 actions_out, a))
+    return rc;
+  return launch_step(h, lbf_step_kernel, a, traj, stream);
 }
 
 }  // extern "C"

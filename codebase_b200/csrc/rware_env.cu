@@ -15,7 +15,6 @@
 //     atomicMax); the winner of each merge is a max-reduction of (chain length, insertion rank) over the lanes with the same target;
 //   * observations are assembled in shared memory and written back as one contiguous run per env.
 #include "env_common.cuh"
-#include <string.h>
 
 namespace marl {
 
@@ -357,14 +356,10 @@ __global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwSt
 // =============================================================================================================
 using namespace marl;
 
-struct marl_rware {
+struct marl_rware : EnvHandle {
   marl_rware_cfg cfg;
   RwCfgDev dev;
   RwStateDev st;
-  int E, device;
-  uint64_t seed;
-  uint32_t gid0;
-  size_t step_smem;
 };
 
 static int rware_count_shelves(const marl_rware_cfg& c) {
@@ -402,20 +397,6 @@ static RwCfgDev rware_to_dev(const marl_rware_cfg& c) {
   return d;
 }
 
-static TrajDev rware_traj(const marl_traj_view* t) {
-  TrajDev d; memset(&d, 0, sizeof(d));
-  if (t) { d.obs = t->obs; d.act = t->act; d.rew = t->rew; d.done = t->done; d.filled = t->filled; d.capacity = t->capacity; d.T = t->T; d.enabled = 1; }
-  return d;
-}
-
-static int rware_check_traj(const marl_rware* env, const marl_traj_view* t) {
-  if (!t) return MARL_OK;
-  MARL_REQUIRE(t->obs && t->act && t->rew && t->done && t->filled, "traj view has NULL buffers");
-  MARL_REQUIRE(t->n_agents == env->dev.N && t->obs_dim == env->dev.D, "traj view shape (N=%d, obs=%d) does not match env (N=%d, obs=%d)", t->n_agents, t->obs_dim, env->dev.N, env->dev.D);
-  MARL_REQUIRE(t->capacity >= env->E && t->T >= 1, "traj capacity %d must hold one episode per env (%d)", t->capacity, env->E);
-  return MARL_OK;
-}
-
 extern "C" {
 
 int marl_rware_obs_dim(const marl_rware_cfg* cfg) {
@@ -434,44 +415,20 @@ int marl_rware_create(const marl_rware_cfg* cfg, int32_t n_envs, uint64_t seed, 
   h->cfg = *cfg; h->dev = rware_to_dev(*cfg); h->E = n_envs; h->device = device; h->seed = seed; h->gid0 = env_gid0;
   const RwCfgDev& d = h->dev;
   const size_t E = (size_t)n_envs;
-  memset(&h->st, 0, sizeof(h->st));
-#define ALLOC0(ptr, bytes)                                                  \
-  do {                                                                      \
-    cudaError_t _e = cudaMalloc((void**)&(ptr), (bytes));                   \
-    if (_e == cudaSuccess) _e = cudaMemset((ptr), 0, (bytes));              \
-    if (_e != cudaSuccess) { set_error("marl_rware_create: cudaMalloc(%zu) failed: %s", (size_t)(bytes), cudaGetErrorString(_e)); marl_rware_destroy(h); return MARL_ENOMEM; } \
-  } while (0)
-  ALLOC0(h->st.shelves, E * d.pitch);
-  ALLOC0(h->st.agents, E * d.N * 4);
-  ALLOC0(h->st.req, E * kReqWords * 4);
-  ALLOC0(h->st.step, E * 4);
-  ALLOC0(h->st.inactive, E * 4);
-  ALLOC0(h->st.ep_return, E * d.N * 4);
-  ALLOC0(h->st.ep_len, E * 4);
-  ALLOC0(h->st.episode_idx, E * 4);
-  ALLOC0(h->st.active, E);
-  ALLOC0(h->st.stdr, E * (2 * d.N + 1) * 4);
-  ALLOC0(h->st.stdr_n, E * 4);
-#undef ALLOC0
+  h->envs_per_cta = kRwEnvsPerCta; h->threads = kRwThreads;
   h->step_smem = kRwEnvsPerCta * rware_warp_smem(d.N, d.D, d.pitch);
-  static size_t step_smem_limit = 48 * 1024;   // per-function, process-wide: only ever raised
-  if (h->step_smem > step_smem_limit) {
-    cudaError_t e = cudaFuncSetAttribute(rware_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->step_smem);
-    if (e == cudaSuccess) step_smem_limit = h->step_smem;
-    if (e != cudaSuccess) { set_error("marl_rware_create: %zu B of shared memory per CTA not available: %s", h->step_smem, cudaGetErrorString(e)); marl_rware_destroy(h); return MARL_EINVAL; }
-  }
+  static size_t step_smem_limit = 48 * 1024;
+  int rc = alloc_buffers(h, "marl_rware_create", {{&h->st.shelves, E * d.pitch}, {&h->st.agents, E * d.N * 4}, {&h->st.req, E * kReqWords * 4},
+                                                  {&h->st.step, E * 4}, {&h->st.inactive, E * 4}, {&h->st.ep_return, E * d.N * 4},
+                                                  {&h->st.ep_len, E * 4}, {&h->st.episode_idx, E * 4}, {&h->st.active, E},
+                                                  {&h->st.stdr, E * (2 * d.N + 1) * 4}, {&h->st.stdr_n, E * 4}});
+  if (rc == MARL_OK) rc = raise_smem_limit(rware_step_kernel, h->step_smem, step_smem_limit, "marl_rware_create");
+  if (rc != MARL_OK) { marl_rware_destroy(h); return rc; }
   *out = h;
   return MARL_OK;
 }
 
-int marl_rware_destroy(marl_rware* h) {
-  if (!h) return MARL_OK;
-  cudaSetDevice(h->device);
-  cudaFree(h->st.shelves); cudaFree(h->st.agents); cudaFree(h->st.req); cudaFree(h->st.step); cudaFree(h->st.inactive); cudaFree(h->st.ep_return);
-  cudaFree(h->st.ep_len); cudaFree(h->st.episode_idx); cudaFree(h->st.active); cudaFree(h->st.stdr); cudaFree(h->st.stdr_n);
-  delete h;
-  return MARL_OK;
-}
+int marl_rware_destroy(marl_rware* h) { return env_destroy(h); }
 
 int marl_rware_set_state(marl_rware* h, const uint8_t* shelves, const uint8_t* agents, const uint32_t* requested, const int32_t* step,
                          const int32_t* inactive, void* stream) {
@@ -495,16 +452,9 @@ int marl_rware_get_state(marl_rware* h, uint8_t* shelves, uint8_t* agents, uint3
 
 int marl_rware_reset(marl_rware* h, const uint8_t* reset_mask, float* obs_out, const marl_traj_view* traj, int32_t slot0, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_rware_reset: NULL handle");
-  if (int rc = rware_check_traj(h, traj)) return rc;
+  if (int rc = check_traj(h, traj)) return rc;
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  rware_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, rware_traj(traj), slot0);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
-}
-
-static int rware_launch(marl_rware* h, const StepArgs& a, const marl_traj_view* traj, void* stream) {
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  rware_step_kernel<<<(h->E + kRwEnvsPerCta - 1) / kRwEnvsPerCta, kRwThreads, h->step_smem, (cudaStream_t)stream>>>(h->dev, h->st, a, rware_traj(traj));
+  rware_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, to_traj(traj), slot0);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }
@@ -512,10 +462,8 @@ static int rware_launch(marl_rware* h, const StepArgs& a, const marl_traj_view* 
 int marl_rware_step(marl_rware* h, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,
                     float* final_ret_out, int32_t* final_len_out, int32_t autoreset, void* stream) {
   MARL_REQUIRE(h && actions && rew_out && done_out && trunc_out, "marl_rware_step: NULL argument");
-  StepArgs a; memset(&a, 0, sizeof(a));
-  a.E = h->E; a.seed = h->seed; a.gid0 = h->gid0; a.policy = 0; a.actions = actions; a.obs_out = obs_out; a.rew_out = rew_out;
-  a.done_out = done_out; a.trunc_out = trunc_out; a.final_ret = final_ret_out; a.final_len = final_len_out; a.autoreset = autoreset;
-  return rware_launch(h, a, nullptr, stream);
+  const StepArgs a = step_args(h, actions, obs_out, rew_out, done_out, trunc_out, final_ret_out, final_len_out, autoreset);
+  return launch_step(h, rware_step_kernel, a, nullptr, stream);
 }
 
 int marl_rware_rollout_step(marl_rware* h, const float* values, const marl_rollout_args* ra, const marl_traj_view* traj, float* obs_inout,
@@ -525,14 +473,11 @@ int marl_rware_rollout_step(marl_rware* h, const float* values, const marl_rollo
   MARL_REQUIRE(ra->policy != 1, "marl_rware_rollout_step: policy 1 (epsilon-greedy) is not available on RWARE: no DQN-family learner takes its %d-feature "
                "observations (at most 32)", h->dev.D);
   MARL_REQUIRE(ra->policy == 2, "marl_rware_rollout_step: policy must be 2 (categorical)");
-  MARL_REQUIRE(ra->n_actions >= 1 && ra->n_actions <= 64, "marl_rware_rollout_step: n_actions out of range");
-  if (int rc = rware_check_traj(h, traj)) return rc;
-  MARL_REQUIRE(!(traj && ra->autoreset), "marl_rware_rollout_step: trajectory recording needs autoreset=0 (episode-synchronous collection)");
-  StepArgs a; memset(&a, 0, sizeof(a));
-  a.E = h->E; a.seed = h->seed; a.gid0 = h->gid0; a.policy = ra->policy; a.values = values; a.epsilon = ra->epsilon; a.n_actions = ra->n_actions;
-  a.obs_out = obs_inout; a.rew_out = rew_out; a.done_out = done_out; a.trunc_out = trunc_out; a.final_ret = final_ret_out; a.final_len = final_len_out;
-  a.actions_out = actions_out; a.autoreset = ra->autoreset; a.use_proper_termination = ra->use_proper_termination; a.clear_stale = ra->clear_stale; a.slot0 = ra->slot0;
-  return rware_launch(h, a, traj, stream);
+  StepArgs a;
+  if (int rc = rollout_step_args(h, "marl_rware_rollout_step", values, ra, traj, obs_inout, rew_out, done_out, trunc_out, final_ret_out, final_len_out,
+                                 actions_out, a))
+    return rc;
+  return launch_step(h, rware_step_kernel, a, traj, stream);
 }
 
 }  // extern "C"

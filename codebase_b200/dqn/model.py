@@ -18,7 +18,7 @@ import torch
 
 from .. import _native as nat
 from .. import optimizers
-from ..lbf import TrajStore
+from ..native_env import TrajStore
 
 HIDDEN = 128
 

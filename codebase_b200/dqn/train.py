@@ -24,7 +24,7 @@ from pathlib import Path
 import torch
 
 from ..config import Config, instantiate
-from ..lbf import TrajStore
+from ..native_env import TrajStore
 from ..utils.envs import episode_info
 
 

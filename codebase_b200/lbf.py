@@ -6,13 +6,13 @@ README.md:80-85): ``[lbforaging:]Foraging[-grid][-2s]-{s}x{s}-{p}p-{f}f[-coop][-
 """
 from __future__ import annotations
 
-import ctypes as C
 import re
 from dataclasses import dataclass, asdict
 
 import torch
 
 from . import _native as nat
+from .native_env import NativeEnv, TrajStore  # noqa: F401  (callers import TrajStore from here too)
 
 _ID = re.compile(r"^(?:lbforaging:)?Foraging(?P<grid>-grid)?(?P<po>-2s)?-(?P<s>\d+)x(?P<s2>\d+)-(?P<p>\d+)p-(?P<f>\d+)f(?P<coop>-coop)?(?P<pen>-pen)?-v(?P<v>\d+)$")
 
@@ -46,6 +46,11 @@ class LbfConfig:
     def n_actions(self) -> int:
         return 6
 
+    @property
+    def obs_bounds(self) -> tuple[float, float]:
+        """Observation-space bounds: coordinates and levels, -1 for absent entities."""
+        return -1.0, float(max(self.rows, self.cols))
+
     def to_native(self) -> nat.LbfCfg:
         return nat.LbfCfg(**asdict(self))
 
@@ -67,92 +72,14 @@ def parse_env_id(name: str, time_limit: int = 0, **overrides) -> LbfConfig:
     return cfg
 
 
-class TrajStore:
-    """Episode-major trajectory store on the device: replay ring (marlbase/dqn/train.py:19-124) or on-policy batch
-    (marlbase/ac/train.py:36-52)."""
+class NativeLbf(NativeEnv):
+    PREFIX = "lbf"
 
-    def __init__(self, capacity: int, n_agents: int, T: int, obs_dim: int, device):
-        self.capacity, self.N, self.T, self.D = capacity, n_agents, T, obs_dim
-        self.obs = torch.zeros(capacity, n_agents, T + 1, obs_dim, dtype=torch.float32, device=device)
-        self.act = torch.zeros(capacity, n_agents, T, dtype=torch.int32, device=device)
-        self.rew = torch.zeros(capacity, n_agents, T, dtype=torch.float32, device=device)
-        self.done = torch.zeros(capacity, T + 1, dtype=torch.uint8, device=device)
-        self.filled = torch.zeros(capacity, T, dtype=torch.uint8, device=device)
-        self.view = nat.TrajView(nat.ptr(self.obs), nat.ptr(self.act), nat.ptr(self.rew), nat.ptr(self.done), nat.ptr(self.filled),
-                                 capacity, n_agents, T, obs_dim)
-
-    def ref(self):
-        return C.byref(self.view)
-
-
-class NativeLbf:
-    def __init__(self, cfg: LbfConfig, n_envs: int, seed: int, env_gid0: int = 0, device: int | None = None):
-        if not torch.cuda.is_available():
-            raise nat.NativeError("codebase_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
-        self.cfg, self.E, self.seed, self.gid0 = cfg, int(n_envs), int(seed), int(env_gid0)
-        self.device_index = torch.cuda.current_device() if device is None else int(device)
-        self.device = torch.device("cuda", self.device_index)
-        self.N, self.D, self.A = cfg.n_agents, cfg.obs_dim, cfg.n_actions
-        self._ncfg = cfg.to_native()
-        self._h = C.c_void_p()
-        self._lib = nat.lib()
-        nat.check(self._lib.marl_lbf_create(C.byref(self._ncfg), C.c_int32(self.E), C.c_uint64(self.seed & (2**64 - 1)), C.c_uint32(self.gid0),
-                                            C.c_int32(self.device_index), C.byref(self._h)), "marl_lbf_create")
-        dev = self.device
-        self.obs = torch.zeros(self.E, self.N, self.D, dtype=torch.float32, device=dev)
-        self.rew = torch.zeros(self.E, self.N, dtype=torch.float32, device=dev)
-        self.done = torch.zeros(self.E, dtype=torch.uint8, device=dev)
-        self.trunc = torch.zeros(self.E, dtype=torch.uint8, device=dev)
-        self.final_ret = torch.zeros(self.E, self.N, dtype=torch.float32, device=dev)
-        self.final_len = torch.zeros(self.E, dtype=torch.int32, device=dev)
-        self.actions = torch.zeros(self.E, self.N, dtype=torch.int32, device=dev)
-
-    def close(self):
-        if self._h:
-            self._lib.marl_lbf_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def reset(self, mask: torch.Tensor | None = None, traj: TrajStore | None = None, slot0: int = 0) -> torch.Tensor:
-        nat.check(self._lib.marl_lbf_reset(self._h, nat.ptr(mask), nat.ptr(self.obs), traj.ref() if traj else None, C.c_int32(slot0), nat.stream_ptr()),
-                  "marl_lbf_reset")
-        return self.obs
-
-    def step(self, actions: torch.Tensor, autoreset: bool = False):
-        assert actions.dtype == torch.int32 and tuple(actions.shape) == (self.E, self.N)
-        nat.check(self._lib.marl_lbf_step(self._h, nat.ptr(actions), nat.ptr(self.obs), nat.ptr(self.rew), nat.ptr(self.done), nat.ptr(self.trunc),
-                                          nat.ptr(self.final_ret), nat.ptr(self.final_len), C.c_int32(int(autoreset)), nat.stream_ptr()), "marl_lbf_step")
-        return self.obs, self.rew, self.done, self.trunc
-
-    def rollout_step(self, values: torch.Tensor, policy: int, epsilon: float = 0.0, traj: TrajStore | None = None, slot0: int = 0,
-                     use_proper_termination: bool = False, autoreset: bool = False, clear_stale: bool = False):
-        """Fused action selection (1 = eps-greedy on Q-values, 2 = categorical on logits) + transition + trajectory write."""
-        assert values.dtype == torch.float32 and values.shape[0] == self.E and values.shape[1] == self.N
-        args = nat.RolloutArgs(policy, float(epsilon), int(values.shape[2]), int(use_proper_termination), int(autoreset), int(clear_stale), int(slot0))
-        nat.check(self._lib.marl_lbf_rollout_step(self._h, nat.ptr(values), C.byref(args), traj.ref() if traj else None, nat.ptr(self.obs), nat.ptr(self.rew),
-                                                  nat.ptr(self.done), nat.ptr(self.trunc), nat.ptr(self.final_ret), nat.ptr(self.final_len), nat.ptr(self.actions),
-                                                  nat.stream_ptr()), "marl_lbf_rollout_step")
-        return self.obs, self.rew, self.done, self.trunc
+    def _state_fields(self):
+        N = self.N
+        return (("field", torch.int8, (self.cfg.rows * self.cfg.cols,)), ("players", torch.int8, (N, 4)), ("step", torch.int32, ()),
+                ("food_spawned", torch.int32, ()), ("ep_return", torch.float32, (N,)), ("ep_len", torch.int32, ()),
+                ("episode_idx", torch.int32, ()), ("active", torch.uint8, ()))
 
     def set_state(self, field: torch.Tensor, players: torch.Tensor, step: torch.Tensor):
-        f = field.to(self.device, torch.int8).contiguous().view(self.E, -1)
-        p = players.to(self.device, torch.int8).contiguous().view(self.E, self.N, 4)
-        s = step.to(self.device, torch.int32).contiguous()
-        nat.check(self._lib.marl_lbf_set_state(self._h, nat.ptr(f), nat.ptr(p), nat.ptr(s), nat.stream_ptr()), "marl_lbf_set_state")
-        torch.cuda.current_stream().synchronize()  # f/p/s are temporaries
-
-    def get_state(self) -> dict:
-        dev, E, N = self.device, self.E, self.N
-        out = dict(field=torch.empty(E, self.cfg.rows * self.cfg.cols, dtype=torch.int8, device=dev),
-                   players=torch.empty(E, N, 4, dtype=torch.int8, device=dev), step=torch.empty(E, dtype=torch.int32, device=dev),
-                   food_spawned=torch.empty(E, dtype=torch.int32, device=dev), ep_return=torch.empty(E, N, dtype=torch.float32, device=dev),
-                   ep_len=torch.empty(E, dtype=torch.int32, device=dev), episode_idx=torch.empty(E, dtype=torch.int32, device=dev),
-                   active=torch.empty(E, dtype=torch.uint8, device=dev))
-        nat.check(self._lib.marl_lbf_get_state(self._h, *[nat.ptr(out[k]) for k in ("field", "players", "step", "food_spawned", "ep_return", "ep_len", "episode_idx", "active")],
-                                               nat.stream_ptr()), "marl_lbf_get_state")
-        return out
+        self._set_state(field, players, step)

@@ -7,13 +7,13 @@ so a correction is a one-line change.
 """
 from __future__ import annotations
 
-import ctypes as C
 import re
 from dataclasses import dataclass, asdict
 
 import torch
 
 from . import _native as nat
+from .native_env import NativeEnv
 
 _ID = re.compile(r"^(?:rware:)?rware-(?P<size>[a-z]+)-(?P<n>\d+)ag(?:-(?P<diff>easy|hard))?-v(?P<v>\d+)$")
 
@@ -58,6 +58,11 @@ class RwareConfig:
     def n_actions(self) -> int:
         return 5
 
+    @property
+    def obs_bounds(self) -> tuple[float, float]:
+        """Observation-space bounds: coordinates, the rest 0 / 1."""
+        return 0.0, float(max(self.rows, self.cols) - 1)
+
     def to_native(self) -> nat.RwareCfg:
         return nat.RwareCfg(**asdict(self))
 
@@ -95,80 +100,18 @@ def parse_rware_id(name: str, time_limit: int = 0, **overrides) -> RwareConfig:
     return cfg
 
 
-class NativeRware:
-    """E warehouses on one device, the same surface as codebase_b200.lbf.NativeLbf (reset, step, rollout_step, set_state, get_state)."""
+class NativeRware(NativeEnv):
+    """E warehouses on one device, the same surface as codebase_b200.lbf.NativeLbf."""
 
-    def __init__(self, cfg: RwareConfig, n_envs: int, seed: int, env_gid0: int = 0, device: int | None = None):
-        if not torch.cuda.is_available():
-            raise nat.NativeError("codebase_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
-        self.cfg, self.E, self.seed, self.gid0 = cfg, int(n_envs), int(seed), int(env_gid0)
-        self.device_index = torch.cuda.current_device() if device is None else int(device)
-        self.device = torch.device("cuda", self.device_index)
-        self.N, self.D, self.A = cfg.n_agents, cfg.obs_dim, cfg.n_actions
-        self._ncfg = cfg.to_native()
-        self._h = C.c_void_p()
-        self._lib = nat.lib()
-        nat.check(self._lib.marl_rware_create(C.byref(self._ncfg), C.c_int32(self.E), C.c_uint64(self.seed & (2**64 - 1)), C.c_uint32(self.gid0),
-                                              C.c_int32(self.device_index), C.byref(self._h)), "marl_rware_create")
-        dev = self.device
-        self.obs = torch.zeros(self.E, self.N, self.D, dtype=torch.float32, device=dev)
-        self.rew = torch.zeros(self.E, self.N, dtype=torch.float32, device=dev)
-        self.done = torch.zeros(self.E, dtype=torch.uint8, device=dev)
-        self.trunc = torch.zeros(self.E, dtype=torch.uint8, device=dev)
-        self.final_ret = torch.zeros(self.E, self.N, dtype=torch.float32, device=dev)
-        self.final_len = torch.zeros(self.E, dtype=torch.int32, device=dev)
-        self.actions = torch.zeros(self.E, self.N, dtype=torch.int32, device=dev)
+    PREFIX = "rware"
 
-    def close(self):
-        if self._h:
-            self._lib.marl_rware_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def reset(self, mask: torch.Tensor | None = None, traj=None, slot0: int = 0) -> torch.Tensor:
-        nat.check(self._lib.marl_rware_reset(self._h, nat.ptr(mask), nat.ptr(self.obs), traj.ref() if traj else None, C.c_int32(slot0), nat.stream_ptr()),
-                  "marl_rware_reset")
-        return self.obs
-
-    def step(self, actions: torch.Tensor, autoreset: bool = False):
-        assert actions.dtype == torch.int32 and tuple(actions.shape) == (self.E, self.N)
-        nat.check(self._lib.marl_rware_step(self._h, nat.ptr(actions), nat.ptr(self.obs), nat.ptr(self.rew), nat.ptr(self.done), nat.ptr(self.trunc),
-                                            nat.ptr(self.final_ret), nat.ptr(self.final_len), C.c_int32(int(autoreset)), nat.stream_ptr()), "marl_rware_step")
-        return self.obs, self.rew, self.done, self.trunc
-
-    def rollout_step(self, values: torch.Tensor, policy: int, epsilon: float = 0.0, traj=None, slot0: int = 0,
-                     use_proper_termination: bool = False, autoreset: bool = False, clear_stale: bool = False):
-        """Fused categorical sampling on logits (policy 2) + transition + trajectory write; policy 1 (epsilon-greedy) is refused."""
-        assert values.dtype == torch.float32 and values.shape[0] == self.E and values.shape[1] == self.N
-        args = nat.RolloutArgs(policy, float(epsilon), int(values.shape[2]), int(use_proper_termination), int(autoreset), int(clear_stale), int(slot0))
-        nat.check(self._lib.marl_rware_rollout_step(self._h, nat.ptr(values), C.byref(args), traj.ref() if traj else None, nat.ptr(self.obs), nat.ptr(self.rew),
-                                                    nat.ptr(self.done), nat.ptr(self.trunc), nat.ptr(self.final_ret), nat.ptr(self.final_len),
-                                                    nat.ptr(self.actions), nat.stream_ptr()), "marl_rware_rollout_step")
-        return self.obs, self.rew, self.done, self.trunc
+    def _state_fields(self):
+        N = self.N
+        return (("shelves", torch.uint8, (self.cfg.rows * self.cfg.cols,)), ("agents", torch.uint8, (N, 4)), ("requested", torch.int32, (8,)),
+                ("step", torch.int32, ()), ("inactive", torch.int32, ()), ("ep_return", torch.float32, (N,)), ("ep_len", torch.int32, ()),
+                ("episode_idx", torch.int32, ()), ("active", torch.uint8, ()))
 
     def set_state(self, shelves: torch.Tensor, agents: torch.Tensor, requested: torch.Tensor, step: torch.Tensor, inactive: torch.Tensor):
         """shelves uint8 [E][rows*cols] (shelf id at its current cell, 0 none), agents uint8 [E][N][4] = (x, y, dir, carried shelf id),
         requested uint32 [E][8] (bit k of the 256-bit mask: shelf k is requested), step / inactive int32 [E]."""
-        f = shelves.to(self.device, torch.uint8).contiguous().view(self.E, -1)
-        a = agents.to(self.device, torch.uint8).contiguous().view(self.E, self.N, 4)
-        q = requested.to(self.device, torch.int32).contiguous().view(self.E, 8)
-        s = step.to(self.device, torch.int32).contiguous()
-        i = inactive.to(self.device, torch.int32).contiguous()
-        nat.check(self._lib.marl_rware_set_state(self._h, nat.ptr(f), nat.ptr(a), nat.ptr(q), nat.ptr(s), nat.ptr(i), nat.stream_ptr()), "marl_rware_set_state")
-        torch.cuda.current_stream().synchronize()  # temporaries
-
-    def get_state(self) -> dict:
-        dev, E, N = self.device, self.E, self.N
-        out = dict(shelves=torch.empty(E, self.cfg.rows * self.cfg.cols, dtype=torch.uint8, device=dev),
-                   agents=torch.empty(E, N, 4, dtype=torch.uint8, device=dev), requested=torch.empty(E, 8, dtype=torch.int32, device=dev),
-                   step=torch.empty(E, dtype=torch.int32, device=dev), inactive=torch.empty(E, dtype=torch.int32, device=dev),
-                   ep_return=torch.empty(E, N, dtype=torch.float32, device=dev), ep_len=torch.empty(E, dtype=torch.int32, device=dev),
-                   episode_idx=torch.empty(E, dtype=torch.int32, device=dev), active=torch.empty(E, dtype=torch.uint8, device=dev))
-        keys = ("shelves", "agents", "requested", "step", "inactive", "ep_return", "ep_len", "episode_idx", "active")
-        nat.check(self._lib.marl_rware_get_state(self._h, *[nat.ptr(out[k]) for k in keys], nat.stream_ptr()), "marl_rware_get_state")
-        return out
+        self._set_state(shelves, agents, requested, step, inactive)

@@ -33,12 +33,10 @@ class _Unwrapped:
 class B200VecEnv:
     def __init__(self, cfg: LbfConfig | RwareConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None):
         self.cfg, self.num_envs = cfg, int(parallel_envs)
-        rware = isinstance(cfg, RwareConfig)
-        self.native = (NativeRware if rware else NativeLbf)(cfg, self.num_envs, seed, env_gid0, device)
+        self.native = (NativeRware if isinstance(cfg, RwareConfig) else NativeLbf)(cfg, self.num_envs, seed, env_gid0, device)
         self.n_agents = cfg.n_agents
         self.unwrapped = _Unwrapped(cfg.n_agents)
-        # LBF: coordinates and levels, -1 for absent entities; RWARE: coordinates, the rest 0 / 1
-        lo, hi = (0.0, float(max(cfg.rows, cfg.cols) - 1)) if rware else (-1.0, float(max(cfg.rows, cfg.cols)))
+        lo, hi = cfg.obs_bounds
         self.single_observation_space = spaces.Tuple([spaces.Box(lo, hi, (cfg.obs_dim,), np.float32)] * cfg.n_agents)
         self.single_action_space = spaces.Tuple([spaces.Discrete(cfg.n_actions)] * cfg.n_agents)
         self.observation_space = spaces.Tuple([spaces.Box(lo, hi, (self.num_envs, cfg.obs_dim), np.float32)] * cfg.n_agents)

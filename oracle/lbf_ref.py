@@ -272,33 +272,17 @@ class ForagingRef:
         self.current_step, self.food_spawned = int(step), int(food_spawned)
 
 
-class WrappedForaging:
-    """ForagingRef under marlbase's wrapper stack: TimeLimit(time_limit) -> RecordEpisodeStatistics -> [ObserveID] -> [StandardiseReward] ->
-    [CooperativeReward]  (marlbase/utils/envs.py:93-109).  The two optional wrappers transcribe the reference's numpy code literally
-    (wrappers.py:96-103 and 119-141): they are what pins the C restatement and the kernel for these two flags."""
+class StandardiseReward:
+    """marlbase's StandardiseReward wrapper (wrappers.py:111-141): per-agent running reward statistics."""
 
-    def __init__(self, cfg: LBFConfig, seed: int, env_gid: int = 0):
-        self.cfg, self.seed, self.gid = cfg, seed, env_gid
-        self.env = ForagingRef(cfg)
-        self.n_resets = 0
-        self.episode_reward = np.zeros(cfg.n_agents, np.float32)
-        self.episode_length = 0
+    def __init__(self, n_agents):
         # StandardiseReward.__init__ (wrappers.py:112-117)
-        self.stdr_wrp_sumw = np.zeros(cfg.n_agents, dtype=np.float32)
-        self.stdr_wrp_wmean = np.zeros(cfg.n_agents, dtype=np.float32)
-        self.stdr_wrp_t = np.zeros(cfg.n_agents, dtype=np.float32)
+        self.stdr_wrp_sumw = np.zeros(n_agents, dtype=np.float32)
+        self.stdr_wrp_wmean = np.zeros(n_agents, dtype=np.float32)
+        self.stdr_wrp_t = np.zeros(n_agents, dtype=np.float32)
         self.stdr_wrp_n = 0
 
-    def _observation(self):
-        observation = tuple(self.env.obs(i) for i in range(self.cfg.n_agents))
-        if self.cfg.observe_id:   # ObserveID.observation (wrappers.py:96-103)
-            n_agents = self.cfg.n_agents
-            observation = np.stack(observation)
-            observation = np.concatenate((np.eye(n_agents, dtype=observation.dtype), observation), axis=1)
-            observation = tuple(o.squeeze() for o in np.split(observation, n_agents))
-        return observation
-
-    def _standardise(self, reward):
+    def reward(self, reward):
         """StandardiseReward.reward (wrappers.py:119-141), verbatim arithmetic"""
         weight = 1.0
         q = reward - self.stdr_wrp_wmean
@@ -312,6 +296,29 @@ class WrappedForaging:
             return reward
         var = (self.stdr_wrp_t * self.stdr_wrp_n) / (self.stdr_wrp_sumw * (self.stdr_wrp_n - 1))
         return (reward - self.stdr_wrp_wmean) / (np.sqrt(var) + 1e-6)
+
+
+class WrappedForaging:
+    """ForagingRef under marlbase's wrapper stack: TimeLimit(time_limit) -> RecordEpisodeStatistics -> [ObserveID] -> [StandardiseReward] ->
+    [CooperativeReward]  (marlbase/utils/envs.py:93-109).  The two optional wrappers transcribe the reference's numpy code literally
+    (wrappers.py:96-103 and 119-141): they are what pins the C restatement and the kernel for these two flags."""
+
+    def __init__(self, cfg: LBFConfig, seed: int, env_gid: int = 0):
+        self.cfg, self.seed, self.gid = cfg, seed, env_gid
+        self.env = ForagingRef(cfg)
+        self.n_resets = 0
+        self.episode_reward = np.zeros(cfg.n_agents, np.float32)
+        self.episode_length = 0
+        self.stdr = StandardiseReward(cfg.n_agents)
+
+    def _observation(self):
+        observation = tuple(self.env.obs(i) for i in range(self.cfg.n_agents))
+        if self.cfg.observe_id:   # ObserveID.observation (wrappers.py:96-103)
+            n_agents = self.cfg.n_agents
+            observation = np.stack(observation)
+            observation = np.concatenate((np.eye(n_agents, dtype=observation.dtype), observation), axis=1)
+            observation = tuple(o.squeeze() for o in np.split(observation, n_agents))
+        return observation
 
     def reset(self):
         self.env.reset(self.seed, self.gid, self.n_resets)
@@ -333,7 +340,7 @@ class WrappedForaging:
                 info[f"agent{i}/episode_returns"] = r
             info["episode_length"] = self.episode_length
         if c.standardise_rewards:
-            reward = self._standardise(reward)
+            reward = self.stdr.reward(reward)
         if c.cooperative_reward:
             reward = c.n_agents * [sum(reward)]  # wrappers.py:106-108
         return self._observation(), reward, done, truncated, info

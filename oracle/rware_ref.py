@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .lbf_ref import DrawStream, philox4x32_10
+from .lbf_ref import DrawStream, StandardiseReward, philox4x32_10
 
 NOOP, FORWARD, LEFT, RIGHT, TOGGLE_LOAD = range(5)
 UP, DOWN, DIR_LEFT, DIR_RIGHT = range(4)
@@ -271,18 +271,12 @@ class WrappedWarehouse:
     [CooperativeReward] (marlbase/utils/envs.py:93-109), the optional wrappers' arithmetic as oracle/lbf_ref.WrappedForaging has it."""
 
     def __init__(self, cfg, seed, env_gid=0):
-        from .lbf_ref import WrappedForaging
-
         self.cfg, self.seed, self.gid = cfg, seed, env_gid
         self.env = Warehouse(cfg)
         self.n_resets = 0
         self.episode_reward = np.zeros(cfg.n_agents, np.float32)
         self.episode_length = 0
-        self._wrap = WrappedForaging.__new__(WrappedForaging)   # reuse its StandardiseReward transcription
-        self._wrap.stdr_wrp_sumw = np.zeros(cfg.n_agents, dtype=np.float32)
-        self._wrap.stdr_wrp_wmean = np.zeros(cfg.n_agents, dtype=np.float32)
-        self._wrap.stdr_wrp_t = np.zeros(cfg.n_agents, dtype=np.float32)
-        self._wrap.stdr_wrp_n = 0
+        self.stdr = StandardiseReward(cfg.n_agents)
 
     def observation(self):
         obs = np.stack([self.env.obs(i) for i in range(self.cfg.n_agents)])
@@ -309,7 +303,7 @@ class WrappedWarehouse:
             info["episode_returns"] = self.episode_reward.copy()
             info["episode_length"] = self.episode_length
         if c.standardise_rewards:
-            reward = self._wrap._standardise(reward)
+            reward = self.stdr.reward(reward)
         if c.cooperative_reward:
             reward = c.n_agents * [sum(reward)]
         return self.observation(), np.asarray(reward, np.float32), done, truncated, info
