@@ -5,7 +5,8 @@ Same constructor signature / Hydra `_target_` role (configs/algorithm/ia2c.yaml:
 `actor.independent.{i}.first_layer.weight`, `….rnn.weight_ih_l0`, …).
 All arithmetic runs in libmarlb200.so (marl_a2c_*): actor forward, target-critic pass, n-step returns
 (utils/utils.py:38-63), fused forward / loss / backward of critic and actor, Adam, target sync.  No CPU fallback.
-`actor.use_rnn` / `critic.use_rnn` make that part the reference's RNNNetwork (one 128-wide GRU layer), independently of each other.
+`actor.use_rnn` / `critic.use_rnn` make that part the reference's RNNNetwork (one GRU layer), independently of each other.  `actor.layers` and
+`critic.layers` are [H, H] with 1 <= H <= 128, each part its own H.
 """
 from __future__ import annotations
 
@@ -15,8 +16,8 @@ import torch
 
 from .. import _native as nat
 from .. import optimizers
-from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dict, init_flat_params, init_flat_rnn_params, rnn_state_dict_to_flat,
-                         sharing_to_nets, state_dict_to_flat)
+from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dict, hidden_width, init_flat_params, init_flat_rnn_params,
+                         rnn_state_dict_to_flat, sharing_to_nets, state_dict_to_flat)
 from ..native_env import TrajStore
 
 
@@ -44,10 +45,8 @@ def check_input_widths(obs_space, critic):
 class A2CNetwork:
     def __init__(self, obs_space, action_space, cfg, actor, critic, device, max_envs=None, max_episode_length=None):
         check_input_widths(obs_space, critic)
-        for part, name in ((actor, "actor"), (critic, "critic")):
-            if list(part.layers) != [HIDDEN, HIDDEN]:
-                raise NotImplementedError(f"{name}.layers={list(part.layers)}: the fused kernels implement the shipped [128, 128] network only "
-                                          f"({'one 128-wide GRU layer' if part.use_rnn else 'MLP'})")
+        self.actor_hidden = hidden_width(actor.layers, "actor.layers", bool(actor.use_rnn))
+        self.critic_hidden = hidden_width(critic.layers, "critic.layers", bool(critic.use_rnn))
         self.actor_rnn, self.critic_rnn = bool(actor.use_rnn), bool(critic.use_rnn)
         self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
@@ -72,8 +71,8 @@ class A2CNetwork:
         self.max_envs = int(max_envs or 1024)
         self.max_T = int(max_episode_length or 500)
         self._lib = nat.lib()
-        acfg = nat.MlpCfg(self.n_agents, self.n_actor_nets, (C.c_int32 * 32)(*self.actor_net), self.in_dim, HIDDEN, self.n_actions)
-        ccfg = nat.MlpCfg(self.n_agents, self.n_critic_nets, (C.c_int32 * 32)(*self.critic_net), self.critic_in, HIDDEN, 1)
+        acfg = nat.MlpCfg(self.n_agents, self.n_actor_nets, (C.c_int32 * 32)(*self.actor_net), self.in_dim, self.actor_hidden, self.n_actions)
+        ccfg = nat.MlpCfg(self.n_agents, self.n_critic_nets, (C.c_int32 * 32)(*self.critic_net), self.critic_in, self.critic_hidden, 1)
         hp = nat.A2cHP(float(cfg.lr), self.gamma, float(self.grad_clip or 0.0), self.n_steps, self.entropy_coef, self.value_loss_coef,
                        self.target_update_interval_or_tau, 0.9, 0.999, 1e-8)
         self._h = C.c_void_p()
@@ -98,8 +97,8 @@ class A2CNetwork:
         # each part by its own rule (RNNNetwork: orthogonal on final_layer only), actor first as the reference creates them
         init_a = init_flat_rnn_params if self.actor_rnn else init_flat_params
         init_c = init_flat_rnn_params if self.critic_rnn else init_flat_params
-        self.theta[: self.n_actor].copy_(init_a(self.n_actor_nets, self.in_dim, self.n_actions, actor.use_orthogonal_init))
-        self.theta[self.n_actor:].copy_(init_c(self.n_critic_nets, self.critic_in, 1, critic.use_orthogonal_init))
+        self.theta[: self.n_actor].copy_(init_a(self.n_actor_nets, self.in_dim, self.n_actions, actor.use_orthogonal_init, self.actor_hidden))
+        self.theta[self.n_actor:].copy_(init_c(self.n_critic_nets, self.critic_in, 1, critic.use_orthogonal_init, self.critic_hidden))
         self.soft_update(1.0)
         self._metrics = torch.zeros(6, dtype=torch.float32, device=self.device)
         self.standardise_returns = bool(getattr(cfg, "standardise_returns", False))   # ac/model.py:112-114
@@ -138,28 +137,29 @@ class A2CNetwork:
                 nat.device_view(ptrs[2].value, N * n_envs * T, self.device).view(N, n_envs, T))
 
     # ---- reference API ------------------------------------------------------------------------------------------------
-    def _hiddens(self, recurrent, batch_size):
-        """utils/models.py:98-103: zeros (num_layers=1, batch, 128) per agent for a recurrent part, None per agent otherwise."""
+    def _hiddens(self, recurrent, batch_size, width):
+        """utils/models.py:98-103: zeros (num_layers=1, batch, H) per agent for a recurrent part, None per agent otherwise."""
         if not recurrent:
             return [None] * self.n_agents
-        return [torch.zeros(1, batch_size, HIDDEN, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
+        return [torch.zeros(1, batch_size, width, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
 
     def init_actor_hiddens(self, batch_size):
-        return self._hiddens(self.actor_rnn, batch_size)
+        return self._hiddens(self.actor_rnn, batch_size, self.actor_hidden)
 
     def init_critic_hiddens(self, batch_size, target=False):
-        return self._hiddens(self.critic_rnn, batch_size)
+        return self._hiddens(self.critic_rnn, batch_size, self.critic_hidden)
 
     def _forward_rnn(self, which, obs, out, h, h_out):
         if h_out is None:
-            h_out = torch.empty(obs.shape[0], self.n_agents, HIDDEN, dtype=torch.float32, device=self.device)
+            width = self.actor_hidden if which == 0 else self.critic_hidden
+            h_out = torch.empty(obs.shape[0], self.n_agents, width, dtype=torch.float32, device=self.device)
         nat.check(self._lib.marl_a2c_forward_rnn(self._h, C.c_int32(which), nat.ptr(obs), C.c_int32(obs.shape[0]), nat.ptr(h), nat.ptr(h_out), nat.ptr(out),
                                                  nat.stream_ptr()), "marl_a2c_forward_rnn")
         return out, h_out
 
     def logits(self, obs: torch.Tensor, out: torch.Tensor | None = None, h: torch.Tensor | None = None, h_out: torch.Tensor | None = None):
         """Actor pass of act (ac/model.py:148-150): obs f32[E,N,D] -> logits f32[E,N,A].
-        A recurrent actor takes one step from h f32[E,N,128] (None: the zero state) and returns (logits, h_out); h_out must not be h."""
+        A recurrent actor takes one step from h f32[E,N,H] (None: the zero state) and returns (logits, h_out); h_out must not be h."""
         E = obs.shape[0]
         if out is None:
             out = torch.empty(E, self.n_agents, self.n_actions, dtype=torch.float32, device=self.device)
@@ -170,7 +170,7 @@ class A2CNetwork:
 
     def values(self, obs: torch.Tensor, target: bool = False, h: torch.Tensor | None = None, h_out: torch.Tensor | None = None):
         """get_value (ac/model.py:155-163): obs f32[E,N,D] -> f32[E,N] (centralised critic: each agent's network reads all N x D values of its env).
-        A recurrent critic takes one step from h f32[E,N,128] (None: the zero state) and returns (values, h_out)."""
+        A recurrent critic takes one step from h f32[E,N,H] (None: the zero state) and returns (values, h_out)."""
         E = obs.shape[0]
         out = torch.empty(E, self.n_agents, 1, dtype=torch.float32, device=self.device)
         if self.critic_rnn:
@@ -182,14 +182,14 @@ class A2CNetwork:
     def act(self, inputs, actor_hiddens, action_mask=None):
         """ac/model.py:147-153 for API parity: list of N tensors [P, obs] -> i64[N, P, 1].  The training loop uses the fused
         marl_lbf_rollout_step(policy=2) which samples from the Philox stream inside the env kernel.  A recurrent actor carries actor_hiddens
-        (per agent (1, P, 128) or None) and returns the new ones."""
+        (per agent (1, P, H) or None) and returns the new ones."""
         if action_mask is not None:
             raise NotImplementedError("action masks only exist for smaclite in the reference (out of scope)")
         obs = torch.stack([torch.as_tensor(i, dtype=torch.float32, device=self.device) for i in inputs], 1).contiguous()
         if self.actor_rnn:
             h = None
             if actor_hiddens is not None and not all(x is None for x in actor_hiddens):
-                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, HIDDEN) for x in actor_hiddens], 1).float().contiguous()
+                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, self.actor_hidden) for x in actor_hiddens], 1).float().contiguous()
             logits, h_out = self.logits(obs, h=h)
             actor_hiddens = [h_out[:, i].unsqueeze(0).clone() for i in range(self.n_agents)]
         else:
@@ -237,9 +237,9 @@ class A2CNetwork:
         th, tg = self.theta.detach().cpu(), self.theta_tgt.detach().cpu()
         to_a = flat_to_rnn_state_dict if self.actor_rnn else flat_to_state_dict
         to_c = flat_to_rnn_state_dict if self.critic_rnn else flat_to_state_dict
-        sd = to_a(th[: self.n_actor], f"actor.{self._akind}", self.n_actor_nets, self.in_dim, self.n_actions)
-        sd.update(to_c(th[self.n_actor:], f"critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1))
-        sd.update(to_c(tg, f"target_critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1))
+        sd = to_a(th[: self.n_actor], f"actor.{self._akind}", self.n_actor_nets, self.in_dim, self.n_actions, self.actor_hidden)
+        sd.update(to_c(th[self.n_actor:], f"critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1, self.critic_hidden))
+        sd.update(to_c(tg, f"target_critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1, self.critic_hidden))
         return sd
 
     def load_state_dict(self, sd):

@@ -30,10 +30,10 @@ class Collector:
         self.env, self.model, self.T, self.proper = envs.native, model, int(time_limit), bool(use_proper_termination)
         self.batch = TrajStore(self.env.E, self.env.N, self.T, self.env.D, self.env.device)
         self.logits = torch.empty(self.env.E, self.env.N, model.n_actions, dtype=torch.float32, device=self.env.device)
-        # recurrent actor: two [E][N][128] hidden-state buffers used in turn (step input, step output)
+        # recurrent actor: two [E][N][H] hidden-state buffers used in turn (step input, step output)
         self.rnn = bool(getattr(model, "actor_rnn", False))
         if self.rnn:
-            self.h = [torch.zeros(self.env.E, self.env.N, 128, dtype=torch.float32, device=self.env.device) for _ in range(2)]
+            self.h = [torch.zeros(self.env.E, self.env.N, model.actor_hidden, dtype=torch.float32, device=self.env.device) for _ in range(2)]
 
     def collect(self):
         env, b = self.env, self.batch

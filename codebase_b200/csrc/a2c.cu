@@ -149,7 +149,7 @@ static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, con
   h->centralised = (critic->in_dim != actor->in_dim || (actor->n_agents == 1 && false)) ? 1 : 0;
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
   h->actor_rnn = actor_rnn ? 1 : 0; h->critic_rnn = critic_rnn ? 1 : 0;
-  h->agl = GruLayout::make(actor->in_dim, actor->out_dim); h->cgl = GruLayout::make(critic->in_dim, critic->out_dim);
+  h->agl = GruLayout::make(actor->in_dim, actor->out_dim, actor->hidden); h->cgl = GruLayout::make(critic->in_dim, critic->out_dim, critic->hidden);
   const int pa = actor_rnn ? h->agl.P : h->actor.lay.P, pc = critic_rnn ? h->cgl.P : h->critic.lay.P;
   h->n_actor = (int64_t)actor->n_nets * pa; h->n_critic = (int64_t)critic->n_nets * pc; h->n_params = h->n_actor + h->n_critic;
   const int pmax = pa > pc ? pa : pc;
@@ -164,7 +164,8 @@ static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, con
   rc |= dev_alloc_zero(&h->scratch, (size_t)h->n_sm * h->scratch_pitch); rc |= dev_alloc_zero(&h->loss_part, 4 * loss_parts);
   rc |= dev_alloc_zero(&h->vt, rows); rc |= dev_alloc_zero(&h->ret, rows); rc |= dev_alloc_zero(&h->adv, rows); rc |= dev_alloc_zero(&h->metrics, 8);
   rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->idx), max_envs);
-  rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->image), (size_t)(actor->n_nets > critic->n_nets ? actor->n_nets : critic->n_nets) * tc_image_bytes() / 4 + 4);
+  if (actor->hidden == kHidden && critic->hidden == kHidden)   // the tensor-core images exist for 128-wide networks only (no image: the FP32 kernels)
+    rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->image), (size_t)(actor->n_nets > critic->n_nets ? actor->n_nets : critic->n_nets) * tc_image_bytes() / 4 + 4);
   if (rnn) {
     const int out_max = actor_rnn ? actor->out_dim : 1;
     rc |= dev_alloc_zero(&h->rnn_q, rows * out_max); rc |= dev_alloc_zero(&h->rnn_dq, rows * out_max); rc |= dev_alloc_zero(&h->gru_save, rows * kGruSaveRow);

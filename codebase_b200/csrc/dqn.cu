@@ -196,7 +196,7 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
   *out = nullptr;
   MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "marl_dqn_create: n_agents out of range");
   MARL_REQUIRE(cfg->n_nets >= 1 && cfg->n_nets <= cfg->n_agents, "marl_dqn_create: n_nets out of range");
-  MARL_REQUIRE(cfg->hidden == kHidden, "marl_dqn_create: only layers=[128,128] is implemented on the GPU path (got hidden=%d)", cfg->hidden);
+  MARL_REQUIRE(cfg->hidden >= 1 && cfg->hidden <= kHidden, "marl_dqn_create: hidden width %d not supported (layers = [H, H], 1 <= H <= %d)", cfg->hidden, kHidden);
   MARL_REQUIRE(cfg->out_dim >= 1 && cfg->out_dim <= kOutPad, "marl_dqn_create: n_actions %d not supported (1..%d)", cfg->out_dim, kOutPad);
   MARL_REQUIRE(max_batch >= 1 && max_T >= 1, "marl_dqn_create: max_batch/max_T must be >= 1");
   MARL_REQUIRE(hp->mixer >= 0 && hp->mixer <= 2, "marl_dqn_create: mixer must be 0 (independent), 1 (VDN) or 2 (QMIX)");
@@ -206,11 +206,11 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
   marl_dqn* h = new marl_dqn();
   h->ns.n_agents = cfg->n_agents; h->ns.n_nets = cfg->n_nets; h->ns.in = cfg->in_dim; h->ns.out = cfg->out_dim;
   memcpy(h->ns.agent_net, cfg->agent_net, sizeof(int) * MARL_MAX_AGENTS);
-  h->ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim);
+  h->ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim, cfg->hidden);
   h->hp = *hp; h->device = device; h->max_batch = max_batch; h->max_T = max_T;
   h->opt.kind = MARL_OPT_ADAM; h->opt.beta1 = hp->beta1; h->opt.beta2 = hp->beta2; h->opt.eps = hp->eps;
   cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
-  h->rnn = rnn; h->gl = GruLayout::make(cfg->in_dim, cfg->out_dim);
+  h->rnn = rnn; h->gl = GruLayout::make(cfg->in_dim, cfg->out_dim, cfg->hidden);
   h->n_params = (int64_t)cfg->n_nets * h->P();
   h->scratch_pitch = (h->P() + 3) & ~3;
   const size_t rows = (size_t)cfg->n_agents * max_batch * (max_T + 1);
@@ -230,7 +230,7 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
     if (!h->q_all) rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim);
     if (hp->mixer == 0) rc |= dqn_alloc(&h->td, (size_t)cfg->n_agents * max_batch * max_T);
     rc |= dqn_alloc(&h->gru_save, rows * kGruSaveRow);
-  } else {
+  } else if (cfg->hidden == kHidden) {   // the tensor-core images exist for 128-wide networks only: narrower ones run the FP32 kernels
     rc |= dqn_alloc(reinterpret_cast<float**>(&h->image), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
     rc |= dqn_alloc(reinterpret_cast<float**>(&h->image_tgt), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
   }
@@ -584,7 +584,7 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
     bp.plan = plan; bp.traj = src.traj; bp.idx = episode_idx; bp.B = batch; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
     bp.td = td_ext; bp.td_agent_stride = td_agent_stride; bp.src = src; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
     if (int rc = launch_gru_backward(bp, st)) return rc;
-  } else if (tc_backward_enabled() && h->ns.in < kMaxObsDim) {
+  } else if (tc_backward_enabled() && h->ns.in < kMaxObsDim && h->image != nullptr) {   // (no image: hidden width below 128)
     if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
     if (!h->tc_h1) {  // intermediates of the tensor-core pipeline, allocated on first use
       const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);

@@ -1,6 +1,8 @@
 // gru.cuh -- recurrent (GRU) agent networks of the DQN family (algorithm.model.use_rnn=True) and of the actor-critic learners
-// (actor.use_rnn / critic.use_rnn): parameter layout, the sequence forward, the actor-critic loss head and the BPTT backward.  Replaces marlbase/utils/models.py:51-116 (RNNNetwork with layers = [128, 128]:
-// first_layer Linear(D, 128) + ReLU, nn.GRU(128, 128, num_layers=1), final_layer Linear(128, A)).
+// (actor.use_rnn / critic.use_rnn): parameter layout, the sequence forward, the actor-critic loss head and the BPTT backward.  Replaces marlbase/utils/models.py:51-116 (RNNNetwork with layers = [H, H]:
+// first_layer Linear(D, H) + ReLU, nn.GRU(H, H, num_layers=1), final_layer Linear(H, A)), 1 <= H <= 128.  The kernels keep 128 units per sequence;
+// units >= H are padding that stays exactly 0 (zero input, r = z = 1/2, n = tanh(0) = 0, so h' = h / 2 = 0 from the zero state) and is never stored
+// in the parameters or the gradients.
 #pragma once
 #include "learner.cuh"
 
@@ -8,18 +10,19 @@ namespace marl {
 
 constexpr int kGruSeqs = 16;                 // sequences per CTA tile (two halves of 8, one per 128-thread half of the block)
 constexpr int kGruThreads = 256;
-constexpr int kGruSaveRow = 6 * kHidden;     // floats the online pass saves per row: x1 | r | z | n | W_hn h + b_hn | h'
+constexpr int kGruSaveRow = 6 * kHidden;     // floats the online pass saves per row: x1 | r | z | n | W_hn h + b_hn | h' (128 each; units >= H hold 0)
 
-// Flat parameters of one network in the reference's state_dict order.
+// Flat parameters of one network in the reference's state_dict order; H = the hidden width.  weight_ih_l0 / weight_hh_l0 are [3H][H] with the
+// gate blocks r, z, n at rows 0, H, 2H (torch's order).
 struct GruLayout {
-  int in, out;
+  int in, out, H;
   int w1, b1, wih, whh, bih, bhh, w3, b3, P;   // float offsets, P = total
-  __host__ __device__ static GruLayout make(int in_, int out_) {
-    GruLayout l; l.in = in_; l.out = out_;
-    l.w1 = 0; l.b1 = l.w1 + kHidden * in_;
-    l.wih = l.b1 + kHidden; l.whh = l.wih + 3 * kHidden * kHidden;
-    l.bih = l.whh + 3 * kHidden * kHidden; l.bhh = l.bih + 3 * kHidden;
-    l.w3 = l.bhh + 3 * kHidden; l.b3 = l.w3 + out_ * kHidden; l.P = l.b3 + out_;
+  __host__ __device__ static GruLayout make(int in_, int out_, int hid = kHidden) {
+    GruLayout l; l.in = in_; l.out = out_; l.H = hid;
+    l.w1 = 0; l.b1 = l.w1 + hid * in_;
+    l.wih = l.b1 + hid; l.whh = l.wih + 3 * hid * hid;
+    l.bih = l.whh + 3 * hid * hid; l.bhh = l.bih + 3 * hid;
+    l.w3 = l.bhh + 3 * hid; l.b3 = l.w3 + out_ * hid; l.P = l.b3 + out_;
     return l;
   }
 };
@@ -30,8 +33,8 @@ struct GruLayout {
 struct GruFwdParams {
   RowPlan plan; RowSource src;
   const float* theta; GruLayout lay;
-  const float* h_in;   // mode 0: [E][N][128] initial state (NULL: zeros); mode 1: always zeros (the reference's hiddens=None)
-  float* h_out;        // mode 0: [E][N][128] final state (NULL: not written)
+  const float* h_in;   // mode 0: [E][N][H] initial state (NULL: zeros); mode 1: always zeros (the reference's hiddens=None)
+  float* h_out;        // mode 0: [E][N][H] final state (NULL: not written)
   float* q_out;        // mode 0: [E][N][A]; mode 1: [N][B][T+1][A]
   float* save;         // mode 1, online pass: [N][B][T+1][kGruSaveRow] for the backward (NULL: not saved)
 };

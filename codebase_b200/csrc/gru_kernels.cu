@@ -3,7 +3,9 @@
 // A CTA owns kGruSeqs = 16 sequences of one network for all of their steps; sequences are independent, so no grid-wide synchronisation
 // is needed and each pass is one launch.  Thread j of each 128-thread half owns hidden unit j of 8 sequences: its three gate rows of
 // W_ih / W_hh give r, z, n and h' of that unit without a cross-thread reduction.  The weights are read through L1 / L2 (W_ih + W_hh are
-// 384 KB per network, more than shared memory holds); every weight a thread loads is used for 8 sequences.
+// 384 KB per network, more than shared memory holds); every weight a thread loads is used for 8 sequences.  A network of hidden width H < 128
+// keeps the 128 threads per half: threads j >= H read a valid row (H - 1) and write zeros, weights are read with row stride H, and the weight
+// gradients are written for units < H only, at their compact offsets (gru.cuh).
 //
 // The actor-critic learners add a loss-head kernel between the two: it reads the outputs the forward stored and hands the backward a dense dL/dout.
 #include "gru.cuh"
@@ -31,22 +33,24 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
   const int v0 = blockIdx.x * kGruSeqs;
   if (v0 >= nseq) return;   // uniform over the CTA
   const float* th = p.theta + (size_t)net * p.lay.P;
-  const int D = p.lay.in, A = p.lay.out, steps = p.plan.unit_rows, B = p.plan.units_per_agent;
+  const int D = p.lay.in, A = p.lay.out, steps = p.plan.unit_rows, B = p.plan.units_per_agent, H = p.lay.H;
+  const bool live = j < H;               // unit j exists (else padding: it stays 0)
+  const int jr = live ? j : H - 1;       // the weight row it reads
   for (int i = threadIdx.x; i < kGruSeqs * kHidden; i += kGruThreads) {
     const int s = i / kHidden, k = i - s * kHidden;
     float v = 0.f;
-    if (p.h_in != nullptr && v0 + s < nseq) {
+    if (p.h_in != nullptr && v0 + s < nseq && k < H) {
       int agent, unit; gru_seq(p.plan, net, v0 + s, agent, unit);
-      v = p.h_in[((size_t)unit * p.src.N + agent) * kHidden + k];
+      v = p.h_in[((size_t)unit * p.src.N + agent) * H + k];
     }
     hs[s][k] = v;
   }
-  const float* w1 = th + p.lay.w1 + j * D;
-  const float* wi = th + p.lay.wih + j * kHidden;
-  const float* wh = th + p.lay.whh + j * kHidden;
-  const float b1 = th[p.lay.b1 + j];
-  const float bir = th[p.lay.bih + j], biz = th[p.lay.bih + kHidden + j], bin = th[p.lay.bih + 2 * kHidden + j];
-  const float bhr = th[p.lay.bhh + j], bhz = th[p.lay.bhh + kHidden + j], bhn = th[p.lay.bhh + 2 * kHidden + j];
+  const float* w1 = th + p.lay.w1 + jr * D;
+  const float* wi = th + p.lay.wih + jr * H;
+  const float* wh = th + p.lay.whh + jr * H;
+  const float b1 = th[p.lay.b1 + jr];
+  const float bir = th[p.lay.bih + jr], biz = th[p.lay.bih + H + jr], bin = th[p.lay.bih + 2 * H + jr];
+  const float bhr = th[p.lay.bhh + jr], bhz = th[p.lay.bhh + H + jr], bhn = th[p.lay.bhh + 2 * H + jr];
   for (int t = 0; t < steps; ++t) {
     for (int i = threadIdx.x; i < kGruSeqs * KX; i += kGruThreads) {
       const int s = i / KX, k = i - s * KX;
@@ -68,16 +72,16 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
         for (int s = 0; s < 8; ++s) acc[s] = fmaf(w, xs[s0 + s][k], acc[s]);
       }
 #pragma unroll
-      for (int s = 0; s < 8; ++s) x1[s0 + s][j] = fmaxf(acc[s], 0.f);
+      for (int s = 0; s < 8; ++s) x1[s0 + s][j] = live ? fmaxf(acc[s], 0.f) : 0.f;
     }
     __syncthreads();
     float ar[8], az[8], ain[8], ahn[8];
 #pragma unroll
     for (int s = 0; s < 8; ++s) { ar[s] = 0.f; az[s] = 0.f; ain[s] = 0.f; ahn[s] = 0.f; }
 #pragma unroll 2
-    for (int k = 0; k < kHidden; ++k) {
-      const float wir = wi[k], wiz = wi[kHidden * kHidden + k], win = wi[2 * kHidden * kHidden + k];
-      const float whr = wh[k], whz = wh[kHidden * kHidden + k], whn = wh[2 * kHidden * kHidden + k];
+    for (int k = 0; k < H; ++k) {
+      const float wir = wi[k], wiz = wi[H * H + k], win = wi[2 * H * H + k];
+      const float whr = wh[k], whz = wh[H * H + k], whn = wh[2 * H * H + k];
 #pragma unroll
       for (int s = 0; s < 8; ++s) {
         const float xv = x1[s0 + s][k], hv = hs[s0 + s][k];
@@ -90,9 +94,10 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
     float hnew[8];
 #pragma unroll
     for (int s = 0; s < 8; ++s) {
-      const float r = gru_sigmoid(ar[s] + bir + bhr), z = gru_sigmoid(az[s] + biz + bhz);
-      const float ghn = ahn[s] + bhn, n = tanhf(ain[s] + bin + r * ghn);
+      float r = gru_sigmoid(ar[s] + bir + bhr), z = gru_sigmoid(az[s] + biz + bhz);
+      float ghn = ahn[s] + bhn, n = tanhf(ain[s] + bin + r * ghn);
       hnew[s] = (1.f - z) * n + z * hs[s0 + s][j];
+      if (!live) { r = 0.f; z = 0.f; ghn = 0.f; n = 0.f; hnew[s] = 0.f; }
       if (p.save != nullptr && v0 + s0 + s < nseq) {
         int agent, unit; gru_seq(p.plan, net, v0 + s0 + s, agent, unit);
         float* row = p.save + (((size_t)agent * B + unit) * steps + t) * kGruSaveRow;
@@ -106,9 +111,9 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
     if (threadIdx.x < kGruSeqs * kOutPad) {   // final_layer
       const int s = threadIdx.x / kOutPad, a = threadIdx.x - s * kOutPad;
       if (a < A && v0 + s < nseq) {
-        const float* w3 = th + p.lay.w3 + a * kHidden;
+        const float* w3 = th + p.lay.w3 + a * H;
         float q = th[p.lay.b3 + a];
-        for (int k = 0; k < kHidden; ++k) q = fmaf(w3[k], hs[s][k], q);
+        for (int k = 0; k < H; ++k) q = fmaf(w3[k], hs[s][k], q);
         int agent, unit; gru_seq(p.plan, net, v0 + s, agent, unit);
         const size_t o = src_dense_out(p.src.mode) ? ((size_t)unit * p.src.N + agent) : (((size_t)agent * B + unit) * steps + t);
         p.q_out[o * A + a] = q;
@@ -118,9 +123,9 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
   if (p.h_out != nullptr) {
     for (int i = threadIdx.x; i < kGruSeqs * kHidden; i += kGruThreads) {
       const int s = i / kHidden, k = i - s * kHidden;
-      if (v0 + s < nseq) {
+      if (v0 + s < nseq && k < H) {
         int agent, unit; gru_seq(p.plan, net, v0 + s, agent, unit);
-        p.h_out[((size_t)unit * p.src.N + agent) * kHidden + k] = hs[s][k];
+        p.h_out[((size_t)unit * p.src.N + agent) * H + k] = hs[s][k];
       }
     }
   }
@@ -146,13 +151,15 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
   int net, v_begin, v_end;
   cta_rows(p.plan, net, v_begin, v_end);   // unit_rows = 1: rows are sequences
   const float* th = p.theta + (size_t)net * p.lay.P;
-  const int D = p.lay.in, A = p.lay.out, T = p.traj.T, B = p.B;
+  const int D = p.lay.in, A = p.lay.out, T = p.traj.T, B = p.B, H = p.lay.H;
+  const bool live = j < H;               // unit j exists (else padding: every gradient through it is 0)
+  const int jr = live ? j : H - 1;       // the weight column it reads
   float* out = p.scratch + (size_t)blockIdx.x * p.scratch_pitch;
   for (int e = threadIdx.x; e < p.lay.P; e += kGruThreads) out[e] = 0.f;
   __syncthreads();
   const float* w3 = th + p.lay.w3;
-  const float* wi = th + p.lay.wih + j;
-  const float* wh = th + p.lay.whh + j;
+  const float* wi = th + p.lay.wih + jr;
+  const float* wh = th + p.lay.whh + jr;
   for (int vt = v_begin; vt < v_end; vt += kGruSeqs) {
     float dhc[8];   // dL/dh_t carried from step t + 1
 #pragma unroll
@@ -205,7 +212,8 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
           r = row[kHidden + j]; z = row[2 * kHidden + j]; n = row[3 * kHidden + j]; ghn = row[4 * kHidden + j];
         }
         float dh = dhc[s];
-        for (int a = 0; a < A; ++a) dh = fmaf(w3[a * kHidden + j], S.dq[s0 + s][a], dh);
+        for (int a = 0; a < A; ++a) dh = fmaf(w3[a * H + jr], S.dq[s0 + s][a], dh);
+        if (!live) dh = 0.f;
         const float dn = dh * (1.f - z), dz = dh * (S.hp[s0 + s][j] - n);
         dhd[s] = dh * z;
         const float dnp = dn * (1.f - n * n), drp = dnp * ghn * r * (1.f - r), dzp = dz * z * (1.f - z);
@@ -218,51 +226,62 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         float ah[8], ax[8];
 #pragma unroll
         for (int s = 0; s < 8; ++s) { ah[s] = dhd[s]; ax[s] = 0.f; }
+        for (int gate = 0; gate < 3; ++gate) {
+          const float* uhp = wh + gate * H * H;
+          const float* uip = wi + gate * H * H;
 #pragma unroll 2
-        for (int g = 0; g < 3 * kHidden; ++g) {
-          const float uh = wh[g * kHidden], ui = wi[g * kHidden];
+          for (int u = 0; u < H; ++u) {
+            const float uh = uhp[u * H], ui = uip[u * H];
+            const int g = gate * kHidden + u;
 #pragma unroll
-          for (int s = 0; s < 8; ++s) { ah[s] = fmaf(uh, S.dgh[s0 + s][g], ah[s]); ax[s] = fmaf(ui, S.dgi[s0 + s][g], ax[s]); }
+            for (int s = 0; s < 8; ++s) { ah[s] = fmaf(uh, S.dgh[s0 + s][g], ah[s]); ax[s] = fmaf(ui, S.dgi[s0 + s][g], ax[s]); }
+          }
         }
 #pragma unroll
-        for (int s = 0; s < 8; ++s) { dhc[s] = ah[s]; S.dx1[s0 + s][j] = S.x1[s0 + s][j] > 0.f ? ax[s] : 0.f; }
+        for (int s = 0; s < 8; ++s) { dhc[s] = live ? ah[s] : 0.f; S.dx1[s0 + s][j] = S.x1[s0 + s][j] > 0.f ? ax[s] : 0.f; }
       }
       __syncthreads();
       // (d) weight-gradient sums of this step over the tile's 16 sequences, added in fixed order
-      for (int e = threadIdx.x; e < kHidden * D; e += kGruThreads) {
+      for (int e = threadIdx.x; e < H * D; e += kGruThreads) {
         const int g = e / D, k = e - g * D;
         float acc = 0.f;
 #pragma unroll
         for (int s = 0; s < kGruSeqs; ++s) acc = fmaf(S.dx1[s][g], S.x[s][k], acc);
         out[p.lay.w1 + e] += acc;
       }
-      if (threadIdx.x < kHidden) {
+      if (threadIdx.x < H) {
         float acc = 0.f;
 #pragma unroll
         for (int s = 0; s < kGruSeqs; ++s) acc += S.dx1[s][threadIdx.x];
         out[p.lay.b1 + threadIdx.x] += acc;
       }
+      // (padded index e: gate row g = gate * 128 + u, column k; stored at (gate * H + u) * H + k when u, k < H)
       for (int e = threadIdx.x; e < 3 * kHidden * kHidden; e += kGruThreads) {
-        const int g = e >> 7, k = e & (kHidden - 1);
+        const int g = e >> 7, k = e & (kHidden - 1), u = g & (kHidden - 1);
+        if (u >= H || k >= H) continue;
         float ai = 0.f, ah = 0.f;
 #pragma unroll
         for (int s = 0; s < kGruSeqs; ++s) { ai = fmaf(S.dgi[s][g], S.x1[s][k], ai); ah = fmaf(S.dgh[s][g], S.hp[s][k], ah); }
-        out[p.lay.wih + e] += ai;
-        out[p.lay.whh + e] += ah;
+        const int o = ((g >> 7) * H + u) * H + k;
+        out[p.lay.wih + o] += ai;
+        out[p.lay.whh + o] += ah;
       }
       for (int g = threadIdx.x; g < 3 * kHidden; g += kGruThreads) {
+        const int u = g & (kHidden - 1);
+        if (u >= H) continue;
         float ai = 0.f, ah = 0.f;
 #pragma unroll
         for (int s = 0; s < kGruSeqs; ++s) { ai += S.dgi[s][g]; ah += S.dgh[s][g]; }
-        out[p.lay.bih + g] += ai;
-        out[p.lay.bhh + g] += ah;
+        out[p.lay.bih + (g >> 7) * H + u] += ai;
+        out[p.lay.bhh + (g >> 7) * H + u] += ah;
       }
       for (int e = threadIdx.x; e < A * kHidden; e += kGruThreads) {
         const int a = e >> 7, k = e & (kHidden - 1);
+        if (k >= H) continue;
         float acc = 0.f;
 #pragma unroll
         for (int s = 0; s < kGruSeqs; ++s) acc = fmaf(S.dq[s][a], S.hc[s][k], acc);
-        out[p.lay.w3 + e] += acc;
+        out[p.lay.w3 + a * H + k] += acc;
       }
       if (threadIdx.x < A) {
         float acc = 0.f;

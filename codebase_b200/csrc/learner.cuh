@@ -304,10 +304,11 @@ int launch_tc_dqn_train(const TrainParams& tp, const TcBuffers& buf, cudaStream_
 
 // Forward pass through whichever implementation is selected.  `image` is scratch for the packed weights (n_nets images);
 // it is rebuilt from `theta` on every call (3 us) so that it can never go stale against direct parameter writes.
-// The tensor-core forward's W1 image is kMaxObsDim wide: wider layers always run the FP32 kernel.
+// The tensor-core forward's W1 image is kMaxObsDim wide and its hidden layers 128 wide: wider inputs and narrower networks always run
+// the FP32 kernel (their handles allocate no image).
 inline int forward_any(const NetSet& ns, const RowPlan& plan, const RowSource& src, const float* theta, uint8_t* image, float* out, cudaStream_t st,
                        bool image_is_current = false) {
-  if (tc_forward_enabled() && image != nullptr && ns.in <= kMaxObsDim) {
+  if (tc_forward_enabled() && image != nullptr && ns.in <= kMaxObsDim && ns.lay.H == kHidden) {
     if (!image_is_current)
       if (int rc = launch_pack_weights(theta, ns.lay, ns.n_nets, image, st)) return rc;
     FwdParams fp; fp.plan = plan; fp.src = src; fp.theta = theta; fp.lay = ns.lay; fp.out = out;
@@ -321,7 +322,7 @@ inline int check_mlp_cfg(const marl_mlp_cfg* cfg, const char* who, int max_in) {
   MARL_REQUIRE(cfg != nullptr, "%s: NULL network config", who);
   MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "%s: n_agents out of range", who);
   MARL_REQUIRE(cfg->n_nets >= 1 && cfg->n_nets <= cfg->n_agents, "%s: n_nets out of range", who);
-  MARL_REQUIRE(cfg->hidden == kHidden, "%s: only layers=[128,128] is implemented on the GPU path (got hidden=%d)", who, cfg->hidden);
+  MARL_REQUIRE(cfg->hidden >= 1 && cfg->hidden <= kHidden, "%s: hidden width %d not supported (layers = [H, H], 1 <= H <= %d)", who, cfg->hidden, kHidden);
   MARL_REQUIRE(cfg->in_dim >= 1 && cfg->in_dim <= max_in, "%s: obs dim %d not supported (1..%d)", who, cfg->in_dim, max_in);
   MARL_REQUIRE(cfg->out_dim >= 1 && cfg->out_dim <= kOutPad, "%s: output width %d not supported (1..%d)", who, cfg->out_dim, kOutPad);
   for (int a = 0; a < cfg->n_agents; ++a) MARL_REQUIRE(cfg->agent_net[a] >= 0 && cfg->agent_net[a] < cfg->n_nets, "%s: agent_net[%d] out of range", who, a);
@@ -331,7 +332,7 @@ inline int check_mlp_cfg(const marl_mlp_cfg* cfg, const char* who, int max_in) {
 inline NetSet to_netset(const marl_mlp_cfg* cfg) {
   NetSet ns; ns.n_agents = cfg->n_agents; ns.n_nets = cfg->n_nets; ns.in = cfg->in_dim; ns.out = cfg->out_dim;
   memcpy(ns.agent_net, cfg->agent_net, sizeof(int) * MARL_MAX_AGENTS);
-  ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim);
+  ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim, cfg->hidden);
   return ns;
 }
 

@@ -65,7 +65,8 @@ __device__ __forceinline__ void rmw4(float* dst, float4 v, bool first) {
 }
 
 // Backward of one tile.  On entry: X, H1, H2 hold the forward activations, DQ[128][8] holds dLoss/dq (zero rows
-// beyond the valid ones).  gs = this CTA's gradient partial [P].  Uses DQ as scratch after it is consumed.
+// beyond the valid ones).  gs = this CTA's gradient partial [P] in the compact layout of `lay`: only entries of hidden
+// units < lay.H are written (the padded ones are exact zeros, mlp.cuh).  Uses DQ as scratch after it is consumed.
 template <int KP>
 __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2, float* DQ, const WeightSmem<KP>& w, const NetLayout& lay,
                                                   float* gs, bool first, const ThreadCoord& tc, const RowMeta* meta, int obs_dim, float* part) {
@@ -85,7 +86,7 @@ __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2
     }
 #pragma unroll
     for (int q = 0; q < 4; ++q)
-      if (o0 + q < lay.out) rmw(gs + lay.w3 + (o0 + q) * kHidden + j, g[0][q] + g[1][q], first);
+      if (o0 + q < lay.out && j < lay.H) rmw(gs + lay.w3 + (o0 + q) * lay.H + j, g[0][q] + g[1][q], first);
     // db3: one row per lane of the first four warps, shuffle-reduced, four partials combined after the barrier
     if (t < kTileRows) {
       const float4 d0 = *reinterpret_cast<const float4*>(DQ + t * kOutPad), d1 = *reinterpret_cast<const float4*>(DQ + t * kOutPad + 4);
@@ -129,7 +130,7 @@ __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2
   __syncthreads();  // dq fully consumed -> reuse DQ as the [8][128] reduction buffer
   *reinterpret_cast<float4*>(DQ + (t >> 5) * kHidden + (t & 31) * 4) = colsum;
   __syncthreads();
-  if (t < kHidden) {
+  if (t < lay.H) {
     float s = 0.f;
 #pragma unroll
     for (int wq = 0; wq < 8; ++wq) s += DQ[wq * kHidden + t];
@@ -140,11 +141,23 @@ __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2
     float acc[8][8];
     zero_acc(acc);
     gemm_tn<kHidden, kHidden>(H2, H1, kTileRows, tc, acc);
+    if (lay.H == kHidden) {
 #pragma unroll
-    for (int mi = 0; mi < 8; ++mi) {
-      float* row = gs + lay.w2 + tn_row(tc, mi) * kHidden;
-      rmw4(row + tn_col(tc, 0), make_float4(acc[mi][0], acc[mi][1], acc[mi][2], acc[mi][3]), first);
-      rmw4(row + tn_col(tc, 4), make_float4(acc[mi][4], acc[mi][5], acc[mi][6], acc[mi][7]), first);
+      for (int mi = 0; mi < 8; ++mi) {
+        float* row = gs + lay.w2 + tn_row(tc, mi) * kHidden;
+        rmw4(row + tn_col(tc, 0), make_float4(acc[mi][0], acc[mi][1], acc[mi][2], acc[mi][3]), first);
+        rmw4(row + tn_col(tc, 4), make_float4(acc[mi][4], acc[mi][5], acc[mi][6], acc[mi][7]), first);
+      }
+    } else {   // compact [H][H]: rows are not 16-byte aligned in general, so element by element
+#pragma unroll
+      for (int mi = 0; mi < 8; ++mi) {
+        const int m = tn_row(tc, mi);
+#pragma unroll
+        for (int nj = 0; nj < 8; ++nj) {
+          const int n = tn_col(tc, nj);
+          if (m < lay.H && n < lay.H) rmw(gs + lay.w2 + m * lay.H + n, acc[mi][nj], first);
+        }
+      }
     }
   }
   __syncthreads();  // H1 no longer needed as a GEMM operand; DQ reduction buffer consumed
@@ -178,7 +191,7 @@ __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2
   }
   __syncthreads();  // dh2 (H2 region) is dead from here on: bring the input tile back into it for dW1
   gather_tile_async<KP>(X, meta, obs_dim);
-  if (t < kHidden) rmw(gs + lay.b1 + t, DQ[t] + DQ[kHidden + t] + DQ[2 * kHidden + t] + DQ[3 * kHidden + t], first);
+  if (t < lay.H) rmw(gs + lay.b1 + t, DQ[t] + DQ[kHidden + t] + DQ[2 * kHidden + t] + DQ[3 * kHidden + t], first);
   cp_async_wait_all();
   __syncthreads();
   // ---- dW1[m][i] = sum_r dh1[r][m] * x[r][i] ---------------------------------------------------------------------
@@ -204,7 +217,8 @@ __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2
       const int i = i0 + 16 * ii;
       if (i < lay.in) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) rmw(gs + lay.w1 + (mg * 8 + q) * lay.in + i, acc[ii][q], first);
+        for (int q = 0; q < 8; ++q)
+          if (mg * 8 + q < lay.H) rmw(gs + lay.w1 + (mg * 8 + q) * lay.in + i, acc[ii][q], first);
       }
     }
   }

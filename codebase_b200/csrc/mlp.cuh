@@ -4,8 +4,11 @@
 // ReLU calls and their autograd backward: marlbase/utils/models.py:14-48 (FCNetwork), :133-173
 // (MultiAgentIndependentNetwork), :176-300 (MultiAgentSharedNetwork).
 //
-// Tile shape: R = 128 rows (one row = one observation of one agent) x H = 128 features, 256 threads, every
-// thread owns an 8x8 register block.  All activations and weights are row-major [row][K] in shared memory; 128-wide
+// Tile shape: R = 128 rows (one row = one observation of one agent) x 128 features, 256 threads, every
+// thread owns an 8x8 register block.  A network narrower than 128 (layers = [H, H], 1 <= H <= 128) is staged into the same
+// tiles zero-padded: a padded unit has zero weights and zero bias, so its activation is ReLU(0) = 0 and every gradient
+// reaching it is a product with a zero, exactly.  Parameters and gradients stay in the compact [H]-wide layout of NetLayout;
+// only the weight loads (zero fill) and the gradient epilogues (entries < H) know about H.  All activations and weights are row-major [row][K] in shared memory; 128-wide
 // tiles use a 132-float pitch, 16-wide tiles an XOR swizzle, so that every 128-bit shared load of the three GEMM forms
 // below is bank-conflict free:
 //   NT  C[r][n] = sum_k A[r][k] * B[n][k]     (forward layers: A = activations, B = nn.Linear weight [out][in])
@@ -176,13 +179,14 @@ __device__ __forceinline__ void gemm_nn(const float* __restrict__ A, const float
 }
 
 // ---- parameter layout of one network, reference state_dict order (network.0.weight, .0.bias, .2.weight, ...) ------
+// H: the hidden width (layers = [H, H], 1 <= H <= kHidden); P = H*in + H + H*H + H + out*H + out
 struct NetLayout {
-  int in, out;          // true dims
+  int in, out, H;       // true dims
   int w1, b1, w2, b2, w3, b3, P;  // float offsets, P = total
-  __host__ __device__ static NetLayout make(int in_, int out_) {
-    NetLayout l; l.in = in_; l.out = out_;
-    l.w1 = 0; l.b1 = l.w1 + kHidden * in_; l.w2 = l.b1 + kHidden; l.b2 = l.w2 + kHidden * kHidden;
-    l.w3 = l.b2 + kHidden; l.b3 = l.w3 + out_ * kHidden; l.P = l.b3 + out_;
+  __host__ __device__ static NetLayout make(int in_, int out_, int hid = kHidden) {
+    NetLayout l; l.in = in_; l.out = out_; l.H = hid;
+    l.w1 = 0; l.b1 = l.w1 + hid * in_; l.w2 = l.b1 + hid; l.b2 = l.w2 + hid * hid;
+    l.w3 = l.b2 + hid; l.b3 = l.w3 + out_ * hid; l.P = l.b3 + out_;
     return l;
   }
 };
@@ -205,26 +209,34 @@ struct WeightSmem {
     else { w2 = base; w1 = base + kFloats; }
     w3 = w2 + kHidden * kPitchH; b1 = w3 + kOutPad * kHidden; b2 = b1 + kHidden; b3 = b2 + kHidden;
   }
-  // W1 [128][in] -> the [128][KP] smem tile, zero-padded.  Caller: cp_async_wait_all() + __syncthreads() before use.
+  // W1 [H][in] -> the [128][KP] smem tile, zero-padded.  Caller: cp_async_wait_all() + __syncthreads() before use.
   __device__ void load_w1_async(const float* __restrict__ theta, const NetLayout& l) {
     for (int i = threadIdx.x; i < kHidden * KP; i += kMlpThreads) {
       const int n = i / KP, k = i % KP;
-      if (k < l.in) cp_async4(&at1<KP>(w1, n, k), theta + l.w1 + n * l.in + k);
+      if (n < l.H && k < l.in) cp_async4(&at1<KP>(w1, n, k), theta + l.w1 + n * l.in + k);
       else at1<KP>(w1, n, k) = 0.f;
     }
   }
-  // cooperative asynchronous load from global params (native layouts) into the swizzled smem layouts; 4-byte
-  // cp.async because theta + net*P is only 4-byte aligned.  Caller: cp_async_wait_all() + __syncthreads() before use.
-  // Without a resident W1 the caller stages it per tile (load_w1_async).
+  // cooperative asynchronous load from global params (native layouts, row stride H) into the swizzled smem layouts, rows and
+  // columns >= H zero-filled; 4-byte cp.async because theta + net*P is only 4-byte aligned.  Caller: cp_async_wait_all() +
+  // __syncthreads() before use.  Without a resident W1 the caller stages it per tile (load_w1_async).
   __device__ void load_async(const float* __restrict__ theta, const NetLayout& l) {
     if constexpr (w1_resident<KP>()) load_w1_async(theta, l);
 #pragma unroll 8
-    for (int i = threadIdx.x; i < kHidden * kHidden; i += kMlpThreads) cp_async4(&at1<kHidden>(w2, i / kHidden, i % kHidden), theta + l.w2 + i);
+    for (int i = threadIdx.x; i < kHidden * kHidden; i += kMlpThreads) {
+      const int n = i / kHidden, k = i % kHidden;
+      if (n < l.H && k < l.H) cp_async4(&at1<kHidden>(w2, n, k), theta + l.w2 + n * l.H + k);
+      else at1<kHidden>(w2, n, k) = 0.f;
+    }
     for (int i = threadIdx.x; i < kOutPad * kHidden; i += kMlpThreads) {
-      if (i / kHidden < l.out) cp_async4(w3 + i, theta + l.w3 + i);
+      const int o = i / kHidden, k = i % kHidden;
+      if (o < l.out && k < l.H) cp_async4(w3 + i, theta + l.w3 + o * l.H + k);
       else w3[i] = 0.f;
     }
-    for (int i = threadIdx.x; i < kHidden; i += kMlpThreads) { cp_async4(b1 + i, theta + l.b1 + i); cp_async4(b2 + i, theta + l.b2 + i); }
+    for (int i = threadIdx.x; i < kHidden; i += kMlpThreads) {
+      if (i < l.H) { cp_async4(b1 + i, theta + l.b1 + i); cp_async4(b2 + i, theta + l.b2 + i); }
+      else { b1[i] = 0.f; b2[i] = 0.f; }
+    }
     if (threadIdx.x < kOutPad) b3[threadIdx.x] = threadIdx.x < l.out ? theta[l.b3 + threadIdx.x] : 0.f;
   }
 };

@@ -9,6 +9,7 @@ owner of device buffers.  There is no CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import random
 import math
 from collections import OrderedDict
@@ -20,7 +21,19 @@ from .. import _native as nat
 from .. import optimizers
 from ..native_env import TrajStore
 
-HIDDEN = 128
+HIDDEN = 128       # the shipped network's width (layers = [128, 128]) and the widest the kernels take
+
+
+def hidden_width(layers, what="layers", use_rnn=False) -> int:
+    """The hidden width H of `layers` (algorithm.model.layers / actor.layers / critic.layers): the kernels implement two hidden layers of one width
+    (an MLP's two Linear layers, or an RNNNetwork's first_layer and GRU, which the reference requires to be equal), 1 <= H <= 128.  Anything else
+    fails here, in Python, before any native call; marl_dqn_create / marl_a2c_create check the same range."""
+    widths = list(layers)
+    ok = len(widths) == 2 and all(isinstance(w, numbers.Integral) and not isinstance(w, bool) for w in widths) and widths[0] == widths[1] and 1 <= widths[0] <= HIDDEN
+    if not ok:
+        raise NotImplementedError(f"{what}={widths}: the fused kernels implement two hidden layers of one width H, 1 <= H <= {HIDDEN} "
+                                  f"(layers = [H, H]; {'first_layer + one H-wide GRU layer' if use_rnn else 'MLP'})")
+    return int(widths[0])
 
 
 def _dim(space) -> int:
@@ -43,11 +56,11 @@ def sharing_to_nets(parameter_sharing, n_agents):
     return [order.index(i) for i in parameter_sharing]
 
 
-def init_flat_params(n_nets, in_dim, out_dim, use_orthogonal_init=True):
+def init_flat_params(n_nets, in_dim, out_dim, use_orthogonal_init=True, hidden=HIDDEN):
     """utils/models.py:8-11,35-44 (host side, once): nn.Linear default init, optionally orthogonal(gain sqrt 2) + zero bias."""
     parts = []
     for _ in range(n_nets):
-        for o, i in ((HIDDEN, in_dim), (HIDDEN, HIDDEN), (out_dim, HIDDEN)):
+        for o, i in ((hidden, in_dim), (hidden, hidden), (out_dim, hidden)):
             lin = torch.nn.Linear(i, o)
             if use_orthogonal_init:
                 torch.nn.init.orthogonal_(lin.weight.data, gain=math.sqrt(2))
@@ -56,10 +69,10 @@ def init_flat_params(n_nets, in_dim, out_dim, use_orthogonal_init=True):
     return torch.cat(parts).float()
 
 
-def flat_to_state_dict(flat, prefix, n_nets, in_dim, out_dim):
+def flat_to_state_dict(flat, prefix, n_nets, in_dim, out_dim, hidden=HIDDEN):
     sd, o = OrderedDict(), 0
     for k in range(n_nets):
-        for layer, shape in ((0, (HIDDEN, in_dim)), (2, (HIDDEN, HIDDEN)), (4, (out_dim, HIDDEN))):
+        for layer, shape in ((0, (hidden, in_dim)), (2, (hidden, hidden)), (4, (out_dim, hidden))):
             n = shape[0] * shape[1]
             sd[f"{prefix}.{k}.network.{layer}.weight"] = flat[o:o + n].view(*shape).clone()
             o += n
@@ -76,20 +89,20 @@ def state_dict_to_flat(sd, prefix, n_nets):
     return torch.cat([p.float() for p in parts])
 
 
-def rnn_shapes(in_dim, out_dim):
-    """RNNNetwork with layers=[128, 128] (utils/models.py:51-116): (state_dict name, shape) in the reference's order."""
-    H3 = 3 * HIDDEN
-    return (("first_layer.weight", (HIDDEN, in_dim)), ("first_layer.bias", (HIDDEN,)), ("rnn.weight_ih_l0", (H3, HIDDEN)),
-            ("rnn.weight_hh_l0", (H3, HIDDEN)), ("rnn.bias_ih_l0", (H3,)), ("rnn.bias_hh_l0", (H3,)),
-            ("final_layer.weight", (out_dim, HIDDEN)), ("final_layer.bias", (out_dim,)))
+def rnn_shapes(in_dim, out_dim, hidden=HIDDEN):
+    """RNNNetwork with layers=[H, H] (utils/models.py:51-116): (state_dict name, shape) in the reference's order."""
+    H, H3 = hidden, 3 * hidden
+    return (("first_layer.weight", (H, in_dim)), ("first_layer.bias", (H,)), ("rnn.weight_ih_l0", (H3, H)),
+            ("rnn.weight_hh_l0", (H3, H)), ("rnn.bias_ih_l0", (H3,)), ("rnn.bias_hh_l0", (H3,)),
+            ("final_layer.weight", (out_dim, H)), ("final_layer.bias", (out_dim,)))
 
 
-def init_flat_rnn_params(n_nets, in_dim, out_dim, use_orthogonal_init=True):
+def init_flat_rnn_params(n_nets, in_dim, out_dim, use_orthogonal_init=True, hidden=HIDDEN):
     """RNNNetwork.__init__ (host side, once): first_layer and the GRU keep PyTorch's default initialisation; use_orthogonal_init applies to
     final_layer only (orthogonal, gain sqrt 2, zero bias).  Modules are created in the reference's order, so the RNG stream matches."""
     parts = []
     for _ in range(n_nets):
-        first, gru, final = torch.nn.Linear(in_dim, HIDDEN), torch.nn.GRU(HIDDEN, HIDDEN, num_layers=1), torch.nn.Linear(HIDDEN, out_dim)
+        first, gru, final = torch.nn.Linear(in_dim, hidden), torch.nn.GRU(hidden, hidden, num_layers=1), torch.nn.Linear(hidden, out_dim)
         if use_orthogonal_init:
             torch.nn.init.orthogonal_(final.weight.data, gain=math.sqrt(2))
             torch.nn.init.constant_(final.bias.data, 0)
@@ -98,10 +111,10 @@ def init_flat_rnn_params(n_nets, in_dim, out_dim, use_orthogonal_init=True):
     return torch.cat(parts).float()
 
 
-def flat_to_rnn_state_dict(flat, prefix, n_nets, in_dim, out_dim):
+def flat_to_rnn_state_dict(flat, prefix, n_nets, in_dim, out_dim, hidden=HIDDEN):
     sd, o = OrderedDict(), 0
     for k in range(n_nets):
-        for name, shape in rnn_shapes(in_dim, out_dim):
+        for name, shape in rnn_shapes(in_dim, out_dim, hidden):
             n = int(np.prod(shape))
             sd[f"{prefix}.{k}.{name}"] = flat[o:o + n].view(*shape).clone()
             o += n
@@ -117,9 +130,7 @@ class QNetwork:
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch=None, max_episode_length=None):
         self.use_rnn = bool(use_rnn)
-        if list(layers) != [HIDDEN, HIDDEN]:
-            raise NotImplementedError(f"layers={list(layers)}: the fused kernels implement the shipped [128, 128] network only "
-                                      f"({'one 128-wide GRU layer' if use_rnn else 'MLP'})")
+        self.hidden = hidden_width(layers, "layers", self.use_rnn)
         self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
             raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
@@ -138,7 +149,7 @@ class QNetwork:
         self.max_batch = int(max_batch or getattr(cfg, "batch_size", 1024))
         self.max_T = int(max_episode_length or getattr(cfg, "max_episode_length", 0) or 500)
         self._lib = nat.lib()
-        mcfg = nat.MlpCfg(self.n_agents, self.n_nets, (C.c_int32 * 32)(*self.agent_net), self.in_dim, HIDDEN, self.n_actions)
+        mcfg = nat.MlpCfg(self.n_agents, self.n_nets, (C.c_int32 * 32)(*self.agent_net), self.in_dim, self.hidden, self.n_actions)
         hp = nat.DqnHP(float(cfg.lr), self.gamma, float(self.grad_clip or 0.0), int(self.double_q), self.target_update_interval_or_tau,
                        0.9, 0.999, 1e-8, self.mixer)
         self._h = C.c_void_p()
@@ -154,7 +165,7 @@ class QNetwork:
         self.theta, self.theta_tgt, self.adam_m, self.adam_v = [nat.device_view(p.value, self.n_params, self.device) for p in ptrs[:4]]
         self.grad = nat.device_view(ptrs[4].value, self.n_params + 4, self.device)  # + (loss numerator, filled count, 2 spare)
         init = init_flat_rnn_params if self.use_rnn else init_flat_params
-        self.theta.copy_(init(self.n_nets, self.in_dim, self.n_actions, use_orthogonal_init))
+        self.theta.copy_(init(self.n_nets, self.in_dim, self.n_actions, use_orthogonal_init, self.hidden))
         self.params_changed()
         self.hard_update()
         self._metrics = torch.zeros(6, dtype=torch.float32, device=self.device)
@@ -177,15 +188,15 @@ class QNetwork:
 
     # ---- reference API ------------------------------------------------------------------------------------------
     def init_hiddens(self, batch_size):
-        """utils/models.py:98-103: zeros (num_layers=1, batch, 128) per agent for recurrent networks, None per agent otherwise."""
+        """utils/models.py:98-103: zeros (num_layers=1, batch, H) per agent for recurrent networks, None per agent otherwise."""
         if not self.use_rnn:
             return [None] * self.n_agents
-        return [torch.zeros(1, batch_size, HIDDEN, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
+        return [torch.zeros(1, batch_size, self.hidden, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
 
     def q_values(self, obs: torch.Tensor, target: bool = False, out: torch.Tensor | None = None, h: torch.Tensor | None = None,
                  h_out: torch.Tensor | None = None):
         """Network pass of model.act (dqn/model.py:96-99) for E envs: obs f32[E,N,D] -> q f32[E,N,A].
-        Recurrent networks take one step from h f32[E,N,128] (None: the zero state) and return (q, h_out); h_out must not be h."""
+        Recurrent networks take one step from h f32[E,N,H] (None: the zero state) and return (q, h_out); h_out must not be h."""
         E = obs.shape[0]
         if out is None:
             out = torch.empty(E, self.n_agents, self.n_actions, dtype=torch.float32, device=self.device)
@@ -193,7 +204,7 @@ class QNetwork:
             nat.check(self._lib.marl_dqn_forward(self._h, nat.ptr(obs), C.c_int32(E), C.c_int32(int(target)), nat.ptr(out), nat.stream_ptr()), "marl_dqn_forward")
             return out
         if h_out is None:
-            h_out = torch.empty(E, self.n_agents, HIDDEN, dtype=torch.float32, device=self.device)
+            h_out = torch.empty(E, self.n_agents, self.hidden, dtype=torch.float32, device=self.device)
         nat.check(self._lib.marl_dqn_forward_rnn(self._h, nat.ptr(obs), C.c_int32(E), C.c_int32(int(target)), nat.ptr(h), nat.ptr(h_out), nat.ptr(out),
                                                  nat.stream_ptr()), "marl_dqn_forward_rnn")
         return out, h_out
@@ -205,10 +216,10 @@ class QNetwork:
             raise NotImplementedError("action masks only exist for smaclite in the reference (out of scope)")
         obs = torch.as_tensor(np.stack([np.asarray(i, np.float32) for i in inputs], 0), device=self.device)
         obs = obs.view(self.n_agents, -1, self.in_dim).transpose(0, 1).contiguous()
-        if self.use_rnn:   # hiddens: per agent (1, E, 128) or None (dqn/model.py:99 carries them through the critic)
+        if self.use_rnn:   # hiddens: per agent (1, E, H) or None (dqn/model.py:99 carries them through the critic)
             h = None
             if hiddens is not None and not all(x is None for x in hiddens):
-                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, HIDDEN) for x in hiddens], 1).float().contiguous()
+                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, self.hidden) for x in hiddens], 1).float().contiguous()
             q, h_out = self.q_values(obs, h=h)
             hiddens = [h_out[:, i].unsqueeze(0).clone() for i in range(self.n_agents)]
         else:
@@ -306,8 +317,8 @@ class QNetwork:
 
     def state_dict(self):
         to_sd = flat_to_rnn_state_dict if self.use_rnn else flat_to_state_dict
-        sd = to_sd(self.theta.detach().cpu(), f"critic.{self._kind}", self.n_nets, self.in_dim, self.n_actions)
-        sd.update(to_sd(self.theta_tgt.detach().cpu(), f"target.{self._kind}", self.n_nets, self.in_dim, self.n_actions))
+        sd = to_sd(self.theta.detach().cpu(), f"critic.{self._kind}", self.n_nets, self.in_dim, self.n_actions, self.hidden)
+        sd.update(to_sd(self.theta_tgt.detach().cpu(), f"target.{self._kind}", self.n_nets, self.in_dim, self.n_actions, self.hidden))
         return sd
 
     def load_state_dict(self, sd):

@@ -70,10 +70,10 @@ class Collector:
         self.env, self.model, self.T = env.native, model, int(time_limit)
         self.proper, self.clear_stale = bool(use_proper_termination), bool(clear_stale)
         self.q = torch.empty(self.env.E, self.env.N, model.n_actions, dtype=torch.float32, device=self.env.device)
-        # recurrent networks: two [E][N][128] hidden-state buffers used in turn (step input, step output)
+        # recurrent networks: two [E][N][H] hidden-state buffers used in turn (step input, step output)
         self.rnn = bool(getattr(model, "use_rnn", False))
         if self.rnn:
-            self.h = [torch.zeros(self.env.E, self.env.N, 128, dtype=torch.float32, device=self.env.device) for _ in range(2)]
+            self.h = [torch.zeros(self.env.E, self.env.N, model.hidden, dtype=torch.float32, device=self.env.device) for _ in range(2)]
 
     def collect(self, rb: TrajStore | None, slot0: int, epsilon: float):
         env = self.env

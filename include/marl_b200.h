@@ -207,7 +207,9 @@ typedef struct {
                                          all 0 = full sharing, else the seps indices (utils/models.py:189-196) */
   int32_t in_dim;                     /* flatdim(observation_space[i]) (or n_agents x it: centralised critic); 1..32 for marl_dqn_*,
                                          1..128 for marl_a2c_* (actor and critic) */
-  int32_t hidden;                     /* layers = [hidden, hidden]; 128 (idqn.yaml:8-10) */
+  int32_t hidden;                     /* layers = [hidden, hidden]: 1..128, default 128 (idqn.yaml:8-10).  Below 128 the parameters stay
+                                         compact (H = hidden in the layouts above and below) and the FP32 kernels run, whatever the
+                                         "tensor_core_*" options say */
   int32_t out_dim;                    /* n_actions (Q / logits) or 1 (state value) */
 } marl_mlp_cfg;
 
@@ -319,18 +321,18 @@ int marl_dqn_timing(marl_dqn* q, int32_t enable, float* total_ms, int32_t* count
 int marl_dqn_timing_kernels(marl_dqn* q, float* ms3, int32_t* count);
 int marl_dqn_set_counters(marl_dqn* q, int64_t updates, int64_t last_target_update);
 
-/* Recurrent agent networks (algorithm.model.use_rnn=True; marlbase/utils/models.py:51-130, RNNNetwork with layers = [128, 128]):
- * first_layer Linear(in, 128) + ReLU, nn.GRU(128, 128, num_layers=1) (gate order r, z, n), final_layer Linear(128, out), no activation
+/* Recurrent agent networks (algorithm.model.use_rnn=True; marlbase/utils/models.py:51-130, RNNNetwork with layers = [H, H], H = cfg.hidden):
+ * first_layer Linear(in, H) + ReLU, nn.GRU(H, H, num_layers=1) (gate order r, z, n), final_layer Linear(H, out), no activation
  * between the GRU and final_layer.  marl_dqn_create_rnn returns the same handle type; marl_dqn_param_ptrs then exposes [n_nets][P] floats,
- * per network in the reference's state_dict order: first_layer.weight [128][in], first_layer.bias [128], rnn.weight_ih_l0 [384][128],
- * rnn.weight_hh_l0 [384][128], rnn.bias_ih_l0 [384], rnn.bias_hh_l0 [384], final_layer.weight [out][128], final_layer.bias [out].
+ * per network in the reference's state_dict order: first_layer.weight [H][in], first_layer.bias [H], rnn.weight_ih_l0 [3H][H],
+ * rnn.weight_hh_l0 [3H][H], rnn.bias_ih_l0 [3H], rnn.bias_hh_l0 [3H], final_layer.weight [out][H], final_layer.bias [out].
  * Training runs every sampled episode from a zero hidden state (dqn/model.py:127,133).  marl_dqn_update / _update_n / _update_grads +
  * _update_apply, standardise_returns, qmix_init, sync_target, the counters and marl_dqn_timing work unchanged (the timed window covers the
  * online sequence forward, the TD head and the backward; marl_dqn_timing_kernels reports count 0).  The "tensor_core_*" options do not apply
  * to recurrent handles (FP32 FFMA throughout); marl_dqn_forward and marl_dqn_peer_attach refuse them; in_dim <= 32. */
 int marl_dqn_create_rnn(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device,
                         marl_dqn** out);
-/* One step of model.act's network pass (dqn/model.py:96-99) for E envs: obs device float[E][N][in], h_in / h_out device float[E][N][128]
+/* One step of model.act's network pass (dqn/model.py:96-99) for E envs: obs device float[E][N][in], h_in / h_out device float[E][N][H]
  * (h_in == NULL: the zero state of init_hiddens; h_out == NULL: not written) -> q_out float[E][N][out].  h_in and h_out must not alias. */
 int marl_dqn_forward_rnn(marl_dqn* q, const float* obs, int32_t n_envs, int32_t use_target, const float* h_in, float* h_out,
                          float* q_out, void* stream);
@@ -389,7 +391,7 @@ int marl_a2c_ret_ms_ptrs(marl_a2c* a, float** ret_ms /* mean[N] | var[N] */, dou
  * surrogate; the target critic follows after the last epoch.  metrics_out: device float[6] as marl_a2c_update, averaged over the epochs. */
 int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, int64_t step, int32_t num_epochs, float ppo_clip,
                     float* metrics_out, void* stream);
-/* Recurrent actor and / or critic (actor.use_rnn / critic.use_rnn; marlbase/utils/models.py:51-116 RNNNetwork with layers = [128, 128], the
+/* Recurrent actor and / or critic (actor.use_rnn / critic.use_rnn; marlbase/utils/models.py:51-116 RNNNetwork with layers = [H, H], the
  * network and per-network parameter order of marl_dqn_create_rnn).  actor_rnn / critic_rnn != 0 make that part a GRU network; the other part stays
  * the MLP.  marl_a2c_param_ptrs then exposes [actor nets | critic nets], each part in its own layout.  Every update pass runs each env's episode
  * from the zero state (ac/model.py:189-246,265-352: hiddens=None): the target critic over all T+1 observations, the critic and the actor over the
@@ -398,7 +400,8 @@ int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, in
 int marl_a2c_create_rnn(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, int32_t actor_rnn, int32_t critic_rnn,
                         int32_t max_envs, int32_t max_T, int32_t device, marl_a2c** out);
 /* One step of a recurrent part for E envs, carrying the hidden state (act, ac/model.py:147-153; get_value, 155-163).  which: 0 actor, 1 critic,
- * 2 target critic.  obs device float[E][N][in] (a centralised critic reads each env's N x in values), h_in / h_out device float[E][N][128]
+ * 2 target critic.  obs device float[E][N][in] (a centralised critic reads each env's N x in values), h_in / h_out device float[E][N][H]
+ * (H: that part's hidden width)
  * (h_in == NULL: the zero state of init_*_hiddens; h_out == NULL: not written) -> out float[E][N][n_actions] (actor) or float[E][N][1].
  * h_in and h_out must not alias; a part that is not recurrent is refused. */
 int marl_a2c_forward_rnn(marl_a2c* h, int32_t which, const float* obs, int32_t n_envs, const float* h_in, float* h_out, float* out,
