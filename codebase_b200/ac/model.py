@@ -16,8 +16,8 @@ import torch
 
 from .. import _native as nat
 from .. import optimizers
-from ..dqn.model import (HIDDEN, _dim, flat_to_rnn_state_dict, flat_to_state_dict, hidden_width, init_flat_params, init_flat_rnn_params,
-                         rnn_state_dict_to_flat, sharing_to_nets, state_dict_to_flat)
+from ..learner import NativeLearner, flat_to_state_dict, flatdim, hidden_width, init_flat_params, init_flat_rnn_params, mlp_shapes, rnn_shapes, \
+    sharing_to_nets, state_dict_to_flat
 from ..native_env import TrajStore
 
 
@@ -28,7 +28,7 @@ def check_input_widths(obs_space, critic):
     """The input widths the actor-critic kernels take: an actor of 1..128 observation features and a critic of 1..128 inputs (a centralised
     critic reads all agents' observations side by side: n_agents x obs).  Anything wider fails here, in Python, before any native call;
     marl_a2c_create checks the same limit."""
-    dims = [_dim(o) for o in obs_space]
+    dims = [flatdim(o) for o in obs_space]
     actor_in = max(dims)
     critic_in = sum(dims) if bool(critic.centralised) and len(dims) > 1 else actor_in
     why = []
@@ -42,24 +42,20 @@ def check_input_widths(obs_space, critic):
         raise NotImplementedError(f"{'; '.join(why)}: the actor-critic kernels take at most {MAX_IN_DIM} input features")
 
 
-class A2CNetwork:
+class A2CNetwork(NativeLearner):
+    _destroy = "marl_a2c_destroy"
+
     def __init__(self, obs_space, action_space, cfg, actor, critic, device, max_envs=None, max_episode_length=None):
         check_input_widths(obs_space, critic)
         self.actor_hidden = hidden_width(actor.layers, "actor.layers", bool(actor.use_rnn))
         self.critic_hidden = hidden_width(critic.layers, "critic.layers", bool(critic.use_rnn))
         self.actor_rnn, self.critic_rnn = bool(actor.use_rnn), bool(critic.use_rnn)
-        self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
-        if not torch.cuda.is_available() or not str(device).startswith("cuda"):
-            raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
-        self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
-        self.n_agents = len(obs_space)
-        obs_dims, act_dims = [_dim(o) for o in obs_space], [_dim(a) for a in action_space]
-        if len(set(obs_dims)) != 1 or len(set(act_dims)) != 1:
-            raise NotImplementedError("agents with different observation / action sizes are not implemented")
-        self.in_dim, self.n_actions = obs_dims[0], act_dims[0]
+        self._open(obs_space, action_space, cfg, device)
         # critic.centralised (MAA2C / MAPPO, ac/model.py:62-65): every agent's critic reads the concatenation of all agents' observations
         self.centralised = bool(critic.centralised) and self.n_agents > 1
         self.critic_in = self.n_agents * self.in_dim if self.centralised else self.in_dim
+        self._actor_shapes = (rnn_shapes if self.actor_rnn else mlp_shapes)(self.in_dim, self.n_actions, self.actor_hidden)
+        self._critic_shapes = (rnn_shapes if self.critic_rnn else mlp_shapes)(self.critic_in, 1, self.critic_hidden)
         self.gamma, self.entropy_coef, self.n_steps = float(cfg.gamma), float(cfg.entropy_coef), int(cfg.n_steps)
         self.grad_clip, self.value_loss_coef = cfg.grad_clip, float(cfg.value_loss_coef)
         self.target_update_interval_or_tau = float(cfg.target_update_interval_or_tau)
@@ -70,7 +66,6 @@ class A2CNetwork:
         self._ckind = "independent" if not critic.parameter_sharing else "networks"
         self.max_envs = int(max_envs or 1024)
         self.max_T = int(max_episode_length or 500)
-        self._lib = nat.lib()
         acfg = nat.MlpCfg(self.n_agents, self.n_actor_nets, (C.c_int32 * 32)(*self.actor_net), self.in_dim, self.actor_hidden, self.n_actions)
         ccfg = nat.MlpCfg(self.n_agents, self.n_critic_nets, (C.c_int32 * 32)(*self.critic_net), self.critic_in, self.critic_hidden, 1)
         hp = nat.A2cHP(float(cfg.lr), self.gamma, float(self.grad_clip or 0.0), self.n_steps, self.entropy_coef, self.value_loss_coef,
@@ -113,11 +108,6 @@ class A2CNetwork:
         cnt = nat.device_view(pc.value, 1, self.device, "<f8").cpu()
         return ms[: self.n_agents], ms[self.n_agents:], float(cnt[0])
 
-    def optimizer_state(self):
-        """The optimiser state of actor + critic by torch's names (Adam / AdamW: exp_avg, exp_avg_sq; RMSprop: square_avg; Adagrad: sum; SGD:
-        none), flat device views in the layout of `theta`."""
-        return optimizers.state(self.optimizer_name, self.adam_m, self.adam_v)
-
     # ---- views into the flat parameter vector ------------------------------------------------------------------
     @property
     def actor_params(self):
@@ -137,12 +127,6 @@ class A2CNetwork:
                 nat.device_view(ptrs[2].value, N * n_envs * T, self.device).view(N, n_envs, T))
 
     # ---- reference API ------------------------------------------------------------------------------------------------
-    def _hiddens(self, recurrent, batch_size, width):
-        """utils/models.py:98-103: zeros (num_layers=1, batch, H) per agent for a recurrent part, None per agent otherwise."""
-        if not recurrent:
-            return [None] * self.n_agents
-        return [torch.zeros(1, batch_size, width, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
-
     def init_actor_hiddens(self, batch_size):
         return self._hiddens(self.actor_rnn, batch_size, self.actor_hidden)
 
@@ -187,11 +171,8 @@ class A2CNetwork:
             raise NotImplementedError("action masks only exist for smaclite in the reference (out of scope)")
         obs = torch.stack([torch.as_tensor(i, dtype=torch.float32, device=self.device) for i in inputs], 1).contiguous()
         if self.actor_rnn:
-            h = None
-            if actor_hiddens is not None and not all(x is None for x in actor_hiddens):
-                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, self.actor_hidden) for x in actor_hiddens], 1).float().contiguous()
-            logits, h_out = self.logits(obs, h=h)
-            actor_hiddens = [h_out[:, i].unsqueeze(0).clone() for i in range(self.n_agents)]
+            logits, h_out = self.logits(obs, h=self._stack_hiddens(actor_hiddens, self.actor_hidden))
+            actor_hiddens = self._split_hiddens(h_out)
         else:
             logits = self.logits(obs)
         dist = torch.distributions.Categorical(logits=logits)
@@ -235,37 +216,15 @@ class A2CNetwork:
 
     def state_dict(self):
         th, tg = self.theta.detach().cpu(), self.theta_tgt.detach().cpu()
-        to_a = flat_to_rnn_state_dict if self.actor_rnn else flat_to_state_dict
-        to_c = flat_to_rnn_state_dict if self.critic_rnn else flat_to_state_dict
-        sd = to_a(th[: self.n_actor], f"actor.{self._akind}", self.n_actor_nets, self.in_dim, self.n_actions, self.actor_hidden)
-        sd.update(to_c(th[self.n_actor:], f"critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1, self.critic_hidden))
-        sd.update(to_c(tg, f"target_critic.{self._ckind}", self.n_critic_nets, self.critic_in, 1, self.critic_hidden))
+        sd = flat_to_state_dict(th[: self.n_actor], f"actor.{self._akind}", self.n_actor_nets, self._actor_shapes)
+        sd.update(flat_to_state_dict(th[self.n_actor:], f"critic.{self._ckind}", self.n_critic_nets, self._critic_shapes))
+        sd.update(flat_to_state_dict(tg, f"target_critic.{self._ckind}", self.n_critic_nets, self._critic_shapes))
         return sd
 
     def load_state_dict(self, sd):
-        def flat(prefix, recurrent, n_nets, in_dim, out_dim):
-            if recurrent:
-                return rnn_state_dict_to_flat(sd, prefix, n_nets, in_dim, out_dim)
-            return state_dict_to_flat(sd, prefix, n_nets)
-
-        self.theta[: self.n_actor].copy_(flat(f"actor.{self._akind}", self.actor_rnn, self.n_actor_nets, self.in_dim, self.n_actions))
-        self.theta[self.n_actor:].copy_(flat(f"critic.{self._ckind}", self.critic_rnn, self.n_critic_nets, self.critic_in, 1))
-        self.theta_tgt.copy_(flat(f"target_critic.{self._ckind}", self.critic_rnn, self.n_critic_nets, self.critic_in, 1))
-
-    def parameters(self):
-        return [self.theta]
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.marl_a2c_destroy(self._h)
-            self._h = None
-            self.theta = self.theta_tgt = self.adam_m = self.adam_v = self.grad = None  # views of freed library memory
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self.theta[: self.n_actor].copy_(state_dict_to_flat(sd, f"actor.{self._akind}", self.n_actor_nets, self._actor_shapes))
+        self.theta[self.n_actor:].copy_(state_dict_to_flat(sd, f"critic.{self._ckind}", self.n_critic_nets, self._critic_shapes))
+        self.theta_tgt.copy_(state_dict_to_flat(sd, f"target_critic.{self._ckind}", self.n_critic_nets, self._critic_shapes))
 
 
 class PPONetwork(A2CNetwork):

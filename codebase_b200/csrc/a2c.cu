@@ -11,7 +11,6 @@
 #include "gru.cuh"
 #include "retms.cuh"
 #include <math.h>
-#include <vector>
 
 namespace marl {
 
@@ -94,21 +93,14 @@ __global__ void iota_kernel(int32_t* x, int n) {
 
 using namespace marl;
 
-struct marl_a2c {
+struct marl_a2c : LearnerHandle {
   NetSet actor, critic;
   marl_a2c_hp hp;
-  int device = 0, n_sm = 148, max_envs = 0, max_T = 0;
-  int64_t n_actor = 0, n_critic = 0, n_params = 0;
-  int scratch_pitch = 0;
-  float *theta = nullptr, *theta_tgt = nullptr, *m = nullptr, *v = nullptr, *grad = nullptr;
-  float *scratch = nullptr, *loss_part = nullptr, *vt = nullptr, *ret = nullptr, *adv = nullptr, *metrics = nullptr;
-  int32_t* idx = nullptr;
-  uint8_t* image = nullptr;  // packed weight images for the tensor-core forward path
+  int max_envs = 0, max_T = 0;
+  int64_t n_actor = 0, n_critic = 0;
+  float *vt = nullptr, *ret = nullptr, *adv = nullptr, *metrics = nullptr;
   int64_t opt_steps = 0;
-  marl_optimizer opt = {};   // the optimiser of actor + critic (marl_a2c_set_optimizer; Adam with hp's constants by default)
   float *logits_all = nullptr, *old_logp = nullptr, *epoch_metrics = nullptr;   // PPO (allocated on first use)
-  // standardise_returns: RunningMeanStd(shape=(n_agents,)) -- mean[N] | var[N] (float32), count (a Python float in the reference), partial sums
-  int standardise = 0; float* ret_ms = nullptr; double* ret_count = nullptr; double* ret_part = nullptr;
   int centralised = 0; float* joint = nullptr;   // critic.centralised: joint observations of the batch [P][T+1][N * D]
   // recurrent parts: GRU layouts, the sequence outputs of the part being trained and their gradient [N][P][T+1][out], the online pass's saved rows
   // [N][P][T+1][kGruSaveRow] (one buffer: the critic pass ends before the actor pass starts)
@@ -119,16 +111,7 @@ constexpr int kMaxPpoEpochs = 64;
 
 extern "C" {
 
-int marl_a2c_destroy(marl_a2c* h) {
-  if (!h) return MARL_OK;
-  cudaSetDevice(h->device);
-  cudaFree(h->theta); cudaFree(h->theta_tgt); cudaFree(h->m); cudaFree(h->v); cudaFree(h->grad); cudaFree(h->scratch); cudaFree(h->loss_part);
-  cudaFree(h->vt); cudaFree(h->ret); cudaFree(h->adv); cudaFree(h->metrics); cudaFree(h->idx); cudaFree(h->image);
-  cudaFree(h->logits_all); cudaFree(h->old_logp); cudaFree(h->epoch_metrics); cudaFree(h->ret_ms); cudaFree(h->ret_count); cudaFree(h->ret_part); cudaFree(h->joint);
-  cudaFree(h->rnn_q); cudaFree(h->rnn_dq); cudaFree(h->gru_save);
-  delete h;
-  return MARL_OK;
-}
+int marl_a2c_destroy(marl_a2c* h) { return destroy_handle(h); }
 
 static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, const marl_a2c_hp* hp, bool actor_rnn, bool critic_rnn, int32_t max_envs, int32_t max_T,
                       int32_t device, marl_a2c** out) {
@@ -141,38 +124,36 @@ static int a2c_create(const marl_mlp_cfg* actor, const marl_mlp_cfg* critic, con
   MARL_REQUIRE(critic->out_dim == 1, "marl_a2c_create: the critic outputs one state value per agent");
   MARL_REQUIRE(max_envs >= 1 && max_T >= 1, "marl_a2c_create: max_envs/max_T must be >= 1");
   MARL_REQUIRE(hp->n_steps >= 1 && hp->n_steps <= kMaxNStep, "marl_a2c_create: n_steps %d out of range (1..%d)", hp->n_steps, kMaxNStep);
-  if (int rc = check_device(device)) return rc;
-  marl_a2c* h = new marl_a2c();
+  marl_a2c* h = nullptr;
+  if (int rc = open_learner(device, *hp, &h)) return rc;
   h->actor = to_netset(actor); h->critic = to_netset(critic);
-  h->hp = *hp; h->device = device; h->max_envs = max_envs; h->max_T = max_T;
-  h->opt.kind = MARL_OPT_ADAM; h->opt.beta1 = hp->beta1; h->opt.beta2 = hp->beta2; h->opt.eps = hp->eps;
-  h->centralised = (critic->in_dim != actor->in_dim || (actor->n_agents == 1 && false)) ? 1 : 0;
-  cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
+  h->max_envs = max_envs; h->max_T = max_T;
+  h->centralised = critic->in_dim != actor->in_dim ? 1 : 0;
   h->actor_rnn = actor_rnn ? 1 : 0; h->critic_rnn = critic_rnn ? 1 : 0;
   h->agl = GruLayout::make(actor->in_dim, actor->out_dim, actor->hidden); h->cgl = GruLayout::make(critic->in_dim, critic->out_dim, critic->hidden);
   const int pa = actor_rnn ? h->agl.P : h->actor.lay.P, pc = critic_rnn ? h->cgl.P : h->critic.lay.P;
   h->n_actor = (int64_t)actor->n_nets * pa; h->n_critic = (int64_t)critic->n_nets * pc; h->n_params = h->n_actor + h->n_critic;
   const int pmax = pa > pc ? pa : pc;
   h->scratch_pitch = (pmax + 3) & ~3;
-  const size_t rows = (size_t)actor->n_agents * max_envs * (max_T + 1);
+  const size_t rows = (size_t)actor->n_agents * max_envs * (max_T + 1), F = sizeof(float);
   const bool rnn = actor_rnn || critic_rnn;
   // the loss statistics: one part per training CTA of an MLP part, one per head block of a recurrent part
   const size_t loss_parts = (size_t)h->n_sm + (rnn ? (size_t)gru_head_blocks(actor->n_agents, max_envs, max_T) : 0);
-  int rc = 0;
-  rc |= dev_alloc_zero(&h->theta, h->n_params); rc |= dev_alloc_zero(&h->theta_tgt, h->n_critic);
-  rc |= dev_alloc_zero(&h->m, h->n_params); rc |= dev_alloc_zero(&h->v, h->n_params); rc |= dev_alloc_zero(&h->grad, h->n_params + 4);
-  rc |= dev_alloc_zero(&h->scratch, (size_t)h->n_sm * h->scratch_pitch); rc |= dev_alloc_zero(&h->loss_part, 4 * loss_parts);
-  rc |= dev_alloc_zero(&h->vt, rows); rc |= dev_alloc_zero(&h->ret, rows); rc |= dev_alloc_zero(&h->adv, rows); rc |= dev_alloc_zero(&h->metrics, 8);
-  rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->idx), max_envs);
-  if (actor->hidden == kHidden && critic->hidden == kHidden)   // the tensor-core images exist for 128-wide networks only (no image: the FP32 kernels)
-    rc |= dev_alloc_zero(reinterpret_cast<float**>(&h->image), (size_t)(actor->n_nets > critic->n_nets ? actor->n_nets : critic->n_nets) * tc_image_bytes() / 4 + 4);
-  if (rnn) {
+  const char* who = "marl_a2c_create";
+  int rc = alloc_buffers(h, who, {{&h->theta, h->n_params * F}, {&h->theta_tgt, h->n_critic * F}, {&h->m, h->n_params * F}, {&h->v, h->n_params * F},
+                                  {&h->grad, (h->n_params + 4) * F}, {&h->scratch, (size_t)h->n_sm * h->scratch_pitch * F}, {&h->loss_part, 4 * loss_parts * F},
+                                  {&h->vt, rows * F}, {&h->ret, rows * F}, {&h->adv, rows * F}, {&h->metrics, 8 * F}, {&h->idx, max_envs * F}});
+  if (!rc && actor->hidden == kHidden && critic->hidden == kHidden)   // the tensor-core images exist for 128-wide networks only (no image: the FP32 kernels)
+    rc = alloc_buffers(h, who, {{&h->image, ((size_t)(actor->n_nets > critic->n_nets ? actor->n_nets : critic->n_nets) * tc_image_bytes() / 4 + 4) * F}});
+  if (!rc && rnn) {
     const int out_max = actor_rnn ? actor->out_dim : 1;
-    rc |= dev_alloc_zero(&h->rnn_q, rows * out_max); rc |= dev_alloc_zero(&h->rnn_dq, rows * out_max); rc |= dev_alloc_zero(&h->gru_save, rows * kGruSaveRow);
+    rc = alloc_buffers(h, who, {{&h->rnn_q, rows * out_max * F}, {&h->rnn_dq, rows * out_max * F}, {&h->gru_save, rows * kGruSaveRow * F}});
   }
-  if (rc) { marl_a2c_destroy(h); return MARL_ENOMEM; }
+  if (rc) { marl_a2c_destroy(h); return rc; }
   iota_kernel<<<(max_envs + 255) / 256, 256>>>(h->idx, max_envs);
-  if (h->centralised && dev_alloc_zero(&h->joint, (size_t)max_envs * (max_T + 1) * critic->in_dim)) { marl_a2c_destroy(h); return MARL_ENOMEM; }
+  if (h->centralised) {
+    if (int rc2 = alloc_buffers(h, who, {{&h->joint, (size_t)max_envs * (max_T + 1) * critic->in_dim * F}})) { marl_a2c_destroy(h); return rc2; }
+  }
   if (int rc2 = learner_kernels_init(actor->in_dim, kMaxInDim)) { marl_a2c_destroy(h); return rc2; }
   if (int rc2 = learner_kernels_init(critic->in_dim, kMaxInDim)) { marl_a2c_destroy(h); return rc2; }
   if (int rc2 = tc_forward_init()) { marl_a2c_destroy(h); return rc2; }
@@ -217,9 +198,7 @@ int marl_a2c_sync_target(marl_a2c* h, void* stream) {  // soft_update(1.0), ac/m
 static int a2c_dense_forward(marl_a2c* h, const NetSet& ns, const float* theta, const float* obs, int n_envs, float* out, void* stream) {
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   const RowPlan plan = make_plan(ns, n_envs, 1, h->n_sm, 32);
-  RowSource src; memset(&src, 0, sizeof(src));
-  src.mode = 0; src.dense = obs; src.E = n_envs; src.N = ns.n_agents; src.D = ns.in;
-  if (ns.in != h->actor.in) { src.mode = 3; src.joint = obs; }   // centralised critic: obs float[E][N][D] read as the joint rows float[E][N * D]
+  const RowSource src = dense_rows(obs, n_envs, ns.n_agents, ns.in, ns.in != h->actor.in);   // (a centralised critic reads joint rows)
   return forward_any(ns, plan, src, theta, h->image, out, (cudaStream_t)stream);
 }
 
@@ -248,8 +227,7 @@ int marl_a2c_forward_rnn(marl_a2c* h, int32_t which, const float* obs, int32_t n
   const NetSet& ns = actor ? h->actor : h->critic;
   GruFwdParams fp; memset(&fp, 0, sizeof(fp));
   fp.plan = make_plan(ns, n_envs, 1, 1, 1);
-  fp.src.mode = 0; fp.src.dense = obs; fp.src.E = n_envs; fp.src.N = ns.n_agents; fp.src.D = ns.in;
-  if (!actor && h->centralised) { fp.src.mode = 3; fp.src.joint = obs; }   // obs float[E][N][D] read as the joint rows float[E][N * D]
+  fp.src = dense_rows(obs, n_envs, ns.n_agents, ns.in, !actor && h->centralised);
   fp.theta = which == 0 ? h->theta : (which == 1 ? h->theta + h->n_actor : h->theta_tgt);
   fp.lay = actor ? h->agl : h->cgl;
   fp.h_in = h_in; fp.h_out = h_out; fp.q_out = out;
@@ -274,12 +252,10 @@ static int a2c_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs,
   MARL_REQUIRE(batch->n_agents == h->actor.n_agents && batch->obs_dim == h->actor.in, "marl_a2c_update: batch shape mismatch");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   const int T = batch->T, N = h->actor.n_agents;
-  const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
-  memset(&ps.src, 0, sizeof(ps.src));
   ps.n_envs = n_envs;
-  ps.src.mode = 1; ps.src.traj = to_view(batch); ps.src.idx = h->idx; ps.src.N = N; ps.src.D = h->actor.in;
-  ps.cplan = make_plan(h->critic, n_envs, T + 1, h->n_sm, min_units);
-  ps.aplan = make_plan(h->actor, n_envs, T + 1, h->n_sm, min_units);
+  ps.src = episode_rows(batch, h->idx, N, h->actor.in);
+  ps.cplan = episode_plan(h->critic, n_envs, T, h->n_sm);
+  ps.aplan = episode_plan(h->actor, n_envs, T, h->n_sm);
   ps.csrc = ps.src;
   if (h->centralised) {   // get_value (ac/model.py:156-157): every agent's critic reads the concatenated observations
     JointParams jp; jp.traj = ps.src.traj; jp.idx = h->idx; jp.P = n_envs; jp.out = h->joint;
@@ -312,16 +288,8 @@ int marl_a2c_standardise_returns(marl_a2c* h, int32_t enable) {
   MARL_REQUIRE(h != nullptr, "marl_a2c_standardise_returns: NULL handle");
   MARL_REQUIRE(h->actor.n_agents <= 32, "marl_a2c_standardise_returns: at most 32 agents");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  if (enable && !h->ret_ms) {
-    const int N = h->actor.n_agents;
-    std::vector<float> init(2 * N, 0.f);
-    for (int a = 0; a < N; ++a) init[N + a] = 1.f;
-    const double c0 = 1e-4;
-    MARL_CUDA_TRY(cudaMalloc(&h->ret_ms, 2 * N * sizeof(float))); MARL_CUDA_TRY(cudaMalloc(&h->ret_count, sizeof(double)));
-    MARL_CUDA_TRY(cudaMalloc(&h->ret_part, (size_t)kRetBlocks * N * 2 * sizeof(double)));
-    MARL_CUDA_TRY(cudaMemcpy(h->ret_ms, init.data(), 2 * N * sizeof(float), cudaMemcpyHostToDevice));
-    MARL_CUDA_TRY(cudaMemcpy(h->ret_count, &c0, sizeof(double), cudaMemcpyHostToDevice));
-  }
+  if (enable)
+    if (int rc = enable_ret_stats(h, h->actor.n_agents, "marl_a2c_standardise_returns")) return rc;
   h->standardise = enable ? 1 : 0;
   return MARL_OK;
 }
@@ -393,6 +361,7 @@ static int a2c_apply(marl_a2c* h, int64_t step, float* metrics_out, void* stream
   MARL_REQUIRE(h != nullptr, "marl_a2c_update_apply: NULL handle");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   h->opt_steps += 1;
+  h->opt_stepped = true;
   AdamParams ap; memset(&ap, 0, sizeof(ap));
   ap.theta = h->theta; ap.theta_tgt = h->theta_tgt; ap.m = h->m; ap.v = h->v; ap.grad = h->grad; ap.n = (int)h->n_params;
   ap.tgt_begin = (int)h->n_actor; ap.tgt_n = (int)h->n_critic;
@@ -419,9 +388,9 @@ int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, in
   A2cPass ps;
   if (int rc = a2c_prepare(h, batch, n_envs, st, ps)) return rc;
   if (!h->logits_all) {
-    const size_t rows = (size_t)h->actor.n_agents * h->max_envs * (h->max_T + 1);
-    int rc = dev_alloc_zero(&h->logits_all, rows * h->actor.out) | dev_alloc_zero(&h->old_logp, rows) | dev_alloc_zero(&h->epoch_metrics, 6 * kMaxPpoEpochs);
-    if (rc) return MARL_ENOMEM;
+    const size_t rows = (size_t)h->actor.n_agents * h->max_envs * (h->max_T + 1), F = sizeof(float);
+    if (int rc = alloc_buffers(h, "marl_ppo_update", {{&h->logits_all, rows * h->actor.out * F}, {&h->old_logp, rows * F}, {&h->epoch_metrics, 6 * kMaxPpoEpochs * F}}))
+      return rc;
   }
   // log-probabilities of the taken actions under the collecting policy = the current actor (ac/model.py:281-292)
   if (h->actor_rnn) {
@@ -443,14 +412,8 @@ int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, in
 
 /* The optimiser of actor + critic: before the first step only; zeroes the optimiser state. */
 int marl_a2c_set_optimizer(marl_a2c* h, const marl_optimizer* opt) {
-  MARL_REQUIRE(h != nullptr, "marl_a2c_set_optimizer: NULL handle");
-  if (int rc = check_optimizer(opt, "marl_a2c_set_optimizer")) return rc;
-  MARL_REQUIRE(h->opt_steps == 0, "marl_a2c_set_optimizer: the learner has already taken an optimiser step; choose the optimiser right after creation");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  MARL_CUDA_TRY(cudaMemset(h->m, 0, h->n_params * sizeof(float)));
-  MARL_CUDA_TRY(cudaMemset(h->v, 0, h->n_params * sizeof(float)));
-  h->opt = *opt;
-  return MARL_OK;
+  if (int rc = check_set_optimizer(h, opt, "marl_a2c_set_optimizer")) return rc;
+  return reset_optimizer(h, *opt);
 }
 
 int marl_a2c_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, int64_t step, float* metrics_out, void* stream) {

@@ -4,6 +4,8 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <initializer_list>
+#include <vector>
 #include "../../include/marl_b200.h"
 
 namespace marl {
@@ -91,6 +93,47 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 #endif
+
+// ---- host side: device buffers owned by a handle -------------------------------------------------------------------------------------------
+// Env and learner handles derive from BufferOwner: every buffer they allocate is recorded in `bufs` and freed by destroy_handle.
+struct BufferOwner {
+  std::vector<void*> bufs;
+};
+
+struct DevBuf {
+  void** ptr; size_t bytes;
+  template <typename T> DevBuf(T** p, size_t n) : ptr(reinterpret_cast<void**>(p)), bytes(n) {}
+};
+
+// Zero-initialised device buffers, each recorded in h->bufs; stops at the first failure (the caller then destroys the handle).
+inline int alloc_buffers(BufferOwner* h, const char* who, std::initializer_list<DevBuf> list) {
+  for (const DevBuf& b : list) {
+    cudaError_t e = cudaMalloc(b.ptr, b.bytes);
+    if (e == cudaSuccess) { h->bufs.push_back(*b.ptr); e = cudaMemset(*b.ptr, 0, b.bytes); }
+    if (e != cudaSuccess) { set_error("%s: cudaMalloc(%zu) failed: %s", who, b.bytes, cudaGetErrorString(e)); return MARL_ENOMEM; }
+  }
+  return MARL_OK;
+}
+
+// Frees one owned buffer ahead of the handle (a buffer that is reallocated larger) and sets *p to NULL.
+template <typename T>
+void free_buffer(BufferOwner* h, T** p) {
+  if (*p == nullptr) return;
+  for (size_t i = 0; i < h->bufs.size(); ++i)
+    if (h->bufs[i] == (void*)*p) { h->bufs.erase(h->bufs.begin() + i); break; }
+  cudaFree(*p);
+  *p = nullptr;
+}
+
+// The destroy of an env or learner handle (H: a BufferOwner with a `device`): its buffers, then the handle.
+template <typename H>
+int destroy_handle(H* h) {
+  if (!h) return MARL_OK;
+  cudaSetDevice(h->device);
+  for (void* p : h->bufs) cudaFree(p);
+  delete h;
+  return MARL_OK;
+}
 
 int check_device(int device);
 int tc_forward_enabled();

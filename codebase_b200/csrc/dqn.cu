@@ -137,18 +137,13 @@ __global__ void __launch_bounds__(256) std_td_kernel(StdRetParams p) {
 
 using namespace marl;
 
-struct marl_dqn {
+struct marl_dqn : LearnerHandle {
   NetSet ns;
   marl_dqn_hp hp;
-  int device = 0, n_sm = 148, max_batch = 0, max_T = 0;
-  int64_t n_params = 0;  // n_nets * P
-  int scratch_pitch = 0;
-  float *theta = nullptr, *theta_tgt = nullptr, *m = nullptr, *v = nullptr, *grad = nullptr;
+  int max_batch = 0, max_T = 0;
   size_t loss_part_n = 0;   // 4-float blocks of loss statistics that loss_part holds
-  float *scratch = nullptr, *loss_part = nullptr, *tq = nullptr, *q_all = nullptr, *td = nullptr, *loss_dev = nullptr, *sumsq = nullptr;
+  float *tq = nullptr, *q_all = nullptr, *td = nullptr, *loss_dev = nullptr, *sumsq = nullptr;
   bool grads_are_local = false;  // set by update_grads, cleared when the caller may have all-reduced grad
-  int32_t* idx = nullptr;
-  uint8_t* image = nullptr;      // packed weight images for the tensor-core forward path (scratch, rebuilt per call)
   uint8_t* image_tgt = nullptr;  // image of theta_tgt, rebuilt only when the target network changed
   uint8_t* image_bwd = nullptr;  // MN-major image of W2 (online net) for the tensor-core backward
   float *tc_h1 = nullptr, *tc_h2 = nullptr, *tc_dh1 = nullptr, *tc_rec = nullptr, *tc_x = nullptr;
@@ -161,14 +156,12 @@ struct marl_dqn {
   // online images: valid = a full pack happened and every later change of theta came from adam_kernel (which updates them in place)
   bool image_current = false, bwd_image_current = false;
   int64_t updates = 0, last_target_update = 0;
-  marl_optimizer opt = {};      // the optimiser (marl_dqn_set_optimizer; Adam with hp's constants by default)
-  bool opt_stepped = false;     // an optimiser step has been launched: the state in m / v belongs to `opt`
   RowPlan train_plan; int n_loss_parts = 0;
   // optional CUDA-event timing of the training kernel (bench.py's roofline leg)
   // measurement hook: 4 events per timed update (before the training pass, after each of its kernels; the FP32 path uses 0 and 3)
   bool timing = false; std::vector<cudaEvent_t> ev; int ev_used = 0; bool ev_split = false;
-  // cfg.standardise_returns: RunningMeanStd over the TD targets (mean[n] | var[n], count, partial sums, returns / chosen-Q scratch)
-  int standardise = 0, n_stat = 0; float *ret_ms = nullptr, *ret = nullptr, *chosen = nullptr; double *ret_count = nullptr, *ret_part = nullptr;
+  // cfg.standardise_returns: returns / chosen-Q scratch next to the statistics
+  float *ret = nullptr, *chosen = nullptr;
   // QMIX (hp.mixer == 2): the mixing network's parameters / Adam state / gradient (+ 4 statistics), per-sample records, chunked partial sums, tile list
   QmixLayout ql = {}; float *mix = nullptr, *mix_tgt = nullptr, *mix_m = nullptr, *mix_v = nullptr, *mix_grad = nullptr, *mix_rec = nullptr, *mix_part = nullptr, *mix_img = nullptr, *mix_img_tgt = nullptr;
   QmixTile* mix_tiles = nullptr; int mix_n_tiles = 0; QmixMicro* mix_micro = nullptr; int mix_n_micro = 0; bool mix_wgrad_tiles = false;
@@ -178,15 +171,13 @@ struct marl_dqn {
 };
 static const int kTimingPairs = 1024;
 
-static int dqn_alloc(float** p, size_t n_floats) { return dev_alloc_zero(p, n_floats); }
-
 // loss_part only ever grows: standardise_returns and the QMIX mixer each need room for their own statistics blocks, in either call order
-static int dqn_grow_loss_part(marl_dqn* h, size_t blocks) {
-  if (blocks <= h->loss_part_n) return 0;
-  cudaFree(h->loss_part); h->loss_part = nullptr; h->loss_part_n = 0;
-  if (dqn_alloc(&h->loss_part, 4 * blocks)) return 1;
+static int dqn_grow_loss_part(marl_dqn* h, size_t blocks, const char* who) {
+  if (blocks <= h->loss_part_n) return MARL_OK;
+  free_buffer(h, &h->loss_part); h->loss_part_n = 0;
+  if (int rc = alloc_buffers(h, who, {{&h->loss_part, 4 * blocks * sizeof(float)}})) return rc;
   h->loss_part_n = blocks;
-  return 0;
+  return MARL_OK;
 }
 
 extern "C" {
@@ -194,47 +185,37 @@ extern "C" {
 static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device, bool rnn, marl_dqn** out) {
   MARL_REQUIRE(cfg && hp && out, "marl_dqn_create: NULL argument");
   *out = nullptr;
-  MARL_REQUIRE(cfg->n_agents >= 1 && cfg->n_agents <= MARL_MAX_AGENTS, "marl_dqn_create: n_agents out of range");
-  MARL_REQUIRE(cfg->n_nets >= 1 && cfg->n_nets <= cfg->n_agents, "marl_dqn_create: n_nets out of range");
-  MARL_REQUIRE(cfg->hidden >= 1 && cfg->hidden <= kHidden, "marl_dqn_create: hidden width %d not supported (layers = [H, H], 1 <= H <= %d)", cfg->hidden, kHidden);
-  MARL_REQUIRE(cfg->out_dim >= 1 && cfg->out_dim <= kOutPad, "marl_dqn_create: n_actions %d not supported (1..%d)", cfg->out_dim, kOutPad);
+  // the recurrent kernels take kMaxObsDim inputs; the MLP kernels' limit (learner_kernels_init) depends on the path that runs
+  const char* who = rnn ? "marl_dqn_create_rnn" : "marl_dqn_create";
+  if (int rc = check_mlp_cfg(cfg, who, rnn ? kMaxObsDim : kMaxInDim)) return rc;
   MARL_REQUIRE(max_batch >= 1 && max_T >= 1, "marl_dqn_create: max_batch/max_T must be >= 1");
   MARL_REQUIRE(hp->mixer >= 0 && hp->mixer <= 2, "marl_dqn_create: mixer must be 0 (independent), 1 (VDN) or 2 (QMIX)");
-  for (int a = 0; a < cfg->n_agents; ++a) MARL_REQUIRE(cfg->agent_net[a] >= 0 && cfg->agent_net[a] < cfg->n_nets, "marl_dqn_create: agent_net[%d] out of range", a);
-  MARL_REQUIRE(!rnn || (cfg->in_dim >= 1 && cfg->in_dim <= kMaxObsDim), "marl_dqn_create_rnn: obs dim %d not supported (1..%d)", cfg->in_dim, kMaxObsDim);
-  if (int rc = check_device(device)) return rc;
-  marl_dqn* h = new marl_dqn();
-  h->ns.n_agents = cfg->n_agents; h->ns.n_nets = cfg->n_nets; h->ns.in = cfg->in_dim; h->ns.out = cfg->out_dim;
-  memcpy(h->ns.agent_net, cfg->agent_net, sizeof(int) * MARL_MAX_AGENTS);
-  h->ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim, cfg->hidden);
-  h->hp = *hp; h->device = device; h->max_batch = max_batch; h->max_T = max_T;
-  h->opt.kind = MARL_OPT_ADAM; h->opt.beta1 = hp->beta1; h->opt.beta2 = hp->beta2; h->opt.eps = hp->eps;
-  cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
+  marl_dqn* h = nullptr;
+  if (int rc = open_learner(device, *hp, &h)) return rc;
+  h->ns = to_netset(cfg);
+  h->max_batch = max_batch; h->max_T = max_T;
   h->rnn = rnn; h->gl = GruLayout::make(cfg->in_dim, cfg->out_dim, cfg->hidden);
   h->n_params = (int64_t)cfg->n_nets * h->P();
   h->scratch_pitch = (h->P() + 3) & ~3;
-  const size_t rows = (size_t)cfg->n_agents * max_batch * (max_T + 1);
-  int rc = 0;
-  rc |= dqn_alloc(&h->theta, h->n_params); rc |= dqn_alloc(&h->theta_tgt, h->n_params);
-  rc |= dqn_alloc(&h->m, h->n_params); rc |= dqn_alloc(&h->v, h->n_params); rc |= dqn_alloc(&h->grad, h->n_params + 4);
-  rc |= dqn_alloc(&h->scratch, (size_t)h->n_sm * h->scratch_pitch);
-  rc |= dqn_grow_loss_part(h, (size_t)h->n_sm + (size_t)(rnn ? cfg->n_agents : 1) * max_batch * max_T / 256 + 2);
-  rc |= dqn_alloc(&h->tq, rows * cfg->out_dim);
-  rc |= dqn_alloc(&h->loss_dev, 8);
-  rc |= dqn_alloc(&h->sumsq, (size_t)(h->n_params + 63) / 64 + 1);
-  rc |= dqn_alloc(reinterpret_cast<float**>(&h->grid_barrier), 4);   // two zero-initialised 64-bit counters (grid barrier, push arrivals)
-  if (hp->mixer == 1) { rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim); rc |= dqn_alloc(&h->td, (size_t)max_batch * max_T); }
-  if (hp->mixer == 2) { rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim); rc |= dqn_alloc(&h->td, (size_t)cfg->n_agents * max_batch * max_T); }
-  rc |= dqn_alloc(reinterpret_cast<float**>(&h->idx), max_batch);
-  if (rnn) {   // the recurrent pass always hands the TD error to its backward: online Q-values of every row and one TD entry per (agent, b, t)
-    if (!h->q_all) rc |= dqn_alloc(&h->q_all, rows * cfg->out_dim);
-    if (hp->mixer == 0) rc |= dqn_alloc(&h->td, (size_t)cfg->n_agents * max_batch * max_T);
-    rc |= dqn_alloc(&h->gru_save, rows * kGruSaveRow);
-  } else if (cfg->hidden == kHidden) {   // the tensor-core images exist for 128-wide networks only: narrower ones run the FP32 kernels
-    rc |= dqn_alloc(reinterpret_cast<float**>(&h->image), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
-    rc |= dqn_alloc(reinterpret_cast<float**>(&h->image_tgt), (size_t)cfg->n_nets * tc_image_bytes() / 4 + 4);
+  const size_t rows = (size_t)cfg->n_agents * max_batch * (max_T + 1), F = sizeof(float);
+  int rc = alloc_buffers(h, who, {{&h->theta, h->n_params * F}, {&h->theta_tgt, h->n_params * F}, {&h->m, h->n_params * F}, {&h->v, h->n_params * F},
+                                  {&h->grad, (h->n_params + 4) * F}, {&h->scratch, (size_t)h->n_sm * h->scratch_pitch * F}});
+  if (!rc) rc = dqn_grow_loss_part(h, (size_t)h->n_sm + (size_t)(rnn ? cfg->n_agents : 1) * max_batch * max_T / 256 + 2, who);
+  if (!rc)
+    rc = alloc_buffers(h, who, {{&h->tq, rows * cfg->out_dim * F}, {&h->loss_dev, 8 * F}, {&h->sumsq, ((size_t)(h->n_params + 63) / 64 + 1) * F},
+                                {&h->grid_barrier, 4 * F}});   // two zero-initialised 64-bit counters (grid barrier, push arrivals)
+  // online Q-values of every row for the external TD heads (VDN, QMIX; the recurrent pass always hands the TD error to its backward) and the TD
+  // error: VDN one entry per (b, t), QMIX and the recurrent pass one per (agent, b, t)
+  if (!rc && (hp->mixer != 0 || rnn))
+    rc = alloc_buffers(h, who, {{&h->q_all, rows * cfg->out_dim * F}, {&h->td, (size_t)(hp->mixer == 1 ? 1 : cfg->n_agents) * max_batch * max_T * F}});
+  if (!rc) rc = alloc_buffers(h, who, {{&h->idx, max_batch * F}});
+  if (!rc && rnn) {
+    rc = alloc_buffers(h, who, {{&h->gru_save, rows * kGruSaveRow * F}});
+  } else if (!rc && cfg->hidden == kHidden) {   // the tensor-core images exist for 128-wide networks only: narrower ones run the FP32 kernels
+    const size_t image_bytes = ((size_t)cfg->n_nets * tc_image_bytes() / 4 + 4) * F;
+    rc = alloc_buffers(h, who, {{&h->image, image_bytes}, {&h->image_tgt, image_bytes}});
   }
-  if (rc) { marl_dqn_destroy(h); return MARL_ENOMEM; }
+  if (rc) { marl_dqn_destroy(h); return rc; }
   if (rnn) {
     if (int rc2 = gru_kernels_init()) { marl_dqn_destroy(h); return rc2; }
   } else {
@@ -257,14 +238,9 @@ int marl_dqn_create_rnn(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t 
 int marl_dqn_destroy(marl_dqn* h) {
   if (!h) return MARL_OK;
   cudaSetDevice(h->device);
-  cudaFree(h->theta); cudaFree(h->theta_tgt); cudaFree(h->m); cudaFree(h->v); cudaFree(h->grad); cudaFree(h->scratch);
-  cudaFree(h->loss_part); cudaFree(h->tq); cudaFree(h->q_all); cudaFree(h->td); cudaFree(h->loss_dev); cudaFree(h->sumsq); cudaFree(h->idx); cudaFree(h->image); cudaFree(h->image_tgt); cudaFree(h->image_bwd); cudaFree(h->tc_h1); cudaFree(h->tc_h2); cudaFree(h->tc_dh1); cudaFree(h->tc_rec); cudaFree(h->tc_x); cudaFree(h->grid_barrier);
   for (int r = 0; r < kMaxRanks; ++r) if (h->peer_base[r] != nullptr && r != h->xchg.rank) cudaIpcCloseMemHandle(h->peer_base[r]);
-  cudaFree(h->mix); cudaFree(h->mix_tgt); cudaFree(h->mix_m); cudaFree(h->mix_v); cudaFree(h->mix_grad); cudaFree(h->mix_rec); cudaFree(h->mix_part); cudaFree(h->mix_tiles); cudaFree(h->mix_micro); cudaFree(h->mix_img); cudaFree(h->mix_img_tgt);
-  cudaFree(h->xbuf); cudaFree(h->ret_ms); cudaFree(h->ret); cudaFree(h->chosen); cudaFree(h->ret_count); cudaFree(h->ret_part); cudaFree(h->gru_save);
   for (auto& e : h->ev) cudaEventDestroy(e);
-  delete h;
-  return MARL_OK;
+  return destroy_handle(h);
 }
 
 /* cfg.standardise_returns (dqn/model.py:82-84, 221-222, 357-358): RunningMeanStd over the TD targets, one column per agent (VDN and QMIX: per
@@ -273,22 +249,19 @@ int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
   MARL_REQUIRE(h != nullptr, "marl_dqn_standardise_returns: NULL handle");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   if (enable && !h->ret_ms) {
+    const char* who = "marl_dqn_standardise_returns";
     const int n = h->hp.mixer != 0 ? h->max_batch : h->ns.n_agents, C = h->hp.mixer != 0 ? 1 : h->ns.n_agents;
-    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
-    std::vector<float> init(2 * n, 0.f);
-    for (int a = 0; a < n; ++a) init[n + a] = 1.f;
-    const double c0 = 1e-4;
-    int rc = 0;
-    rc |= dqn_alloc(&h->ret_ms, 2 * n); rc |= dqn_alloc(&h->ret, (size_t)C * h->max_batch * h->max_T); rc |= dqn_alloc(&h->chosen, (size_t)C * h->max_batch * h->max_T);
-    if (!h->q_all) rc |= dqn_alloc(&h->q_all, rows * h->ns.out);
-    if (!h->td || (h->hp.mixer == 0 && !h->rnn)) { cudaFree(h->td); h->td = nullptr; rc |= dqn_alloc(&h->td, (size_t)C * h->max_batch * h->max_T); }
-    if (rc) return MARL_ENOMEM;
-    MARL_CUDA_TRY(cudaMalloc(&h->ret_count, sizeof(double))); MARL_CUDA_TRY(cudaMalloc(&h->ret_part, (size_t)kRetBlocks * n * 2 * sizeof(double)));
-    MARL_CUDA_TRY(cudaMemcpy(h->ret_ms, init.data(), 2 * n * sizeof(float), cudaMemcpyHostToDevice));
-    MARL_CUDA_TRY(cudaMemcpy(h->ret_count, &c0, sizeof(double), cudaMemcpyHostToDevice));
-    h->n_stat = n;
+    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), cbt = (size_t)C * h->max_batch * h->max_T, F = sizeof(float);
+    if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
+    if (!h->q_all)
+      if (int rc = alloc_buffers(h, who, {{&h->q_all, rows * h->ns.out * F}})) return rc;
+    if (!h->td || (h->hp.mixer == 0 && !h->rnn)) {
+      free_buffer(h, &h->td);
+      if (int rc = alloc_buffers(h, who, {{&h->td, cbt * F}})) return rc;
+    }
     // the per-update loss statistics of this path come from one block per 256 (c, b, t) entries (QMIX: per tile, sized by marl_dqn_qmix_init)
-    if (dqn_grow_loss_part(h, (size_t)h->n_sm + (size_t)C * h->max_batch * h->max_T / 256 + 2)) return MARL_ENOMEM;
+    if (int rc = dqn_grow_loss_part(h, (size_t)h->n_sm + cbt / 256 + 2, who)) return rc;
+    if (int rc = enable_ret_stats(h, n, who)) return rc;
   }
   h->standardise = enable ? 1 : 0;
   return MARL_OK;
@@ -325,19 +298,19 @@ int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, 
   std::vector<QmixTile> tiles(kQmixMaxTiles);
   const int nt = qmix_tiles(h->ql, tiles.data());
   MARL_REQUIRE(nt > 0, "marl_dqn_qmix_init: too many weight-gradient tiles");
-  int rc = 0;
-  rc |= dqn_alloc(&h->mix, n); rc |= dqn_alloc(&h->mix_tgt, n); rc |= dqn_alloc(&h->mix_m, n); rc |= dqn_alloc(&h->mix_v, n); rc |= dqn_alloc(&h->mix_grad, n + 4);
-  rc |= dqn_alloc(&h->mix_rec, (size_t)h->ql.R * samples); rc |= dqn_alloc(&h->mix_part, (size_t)(2 * h->n_sm > kQmixChunks ? 2 * h->n_sm : kQmixChunks) * n);
-  rc |= dqn_alloc(reinterpret_cast<float**>(&h->mix_tiles), (size_t)nt * sizeof(QmixTile) / 4);
-  rc |= dqn_alloc(&h->mix_img, (n + 3) & ~(size_t)3); rc |= dqn_alloc(&h->mix_img_tgt, (n + 3) & ~(size_t)3);
-  rc |= dqn_grow_loss_part(h, (size_t)h->n_sm + samples / kQmTS + 2);   // one block of statistics per tile of kQmTS samples
-  if (rc) return MARL_ENOMEM;
+  const char* who = "marl_dqn_qmix_init";
+  const size_t F = sizeof(float), n_img = (n + 3) & ~(size_t)3;
+  if (int rc = alloc_buffers(h, who, {{&h->mix, n * F}, {&h->mix_tgt, n * F}, {&h->mix_m, n * F}, {&h->mix_v, n * F}, {&h->mix_grad, (n + 4) * F},
+                                      {&h->mix_rec, (size_t)h->ql.R * samples * F}, {&h->mix_part, (size_t)(2 * h->n_sm > kQmixChunks ? 2 * h->n_sm : kQmixChunks) * n * F},
+                                      {&h->mix_tiles, (size_t)nt * sizeof(QmixTile)}, {&h->mix_img, n_img * F}, {&h->mix_img_tgt, n_img * F}}))
+    return rc;
+  if (int rc = dqn_grow_loss_part(h, (size_t)h->n_sm + samples / kQmTS + 2, who)) return rc;   // one block of statistics per tile of kQmTS samples
   MARL_CUDA_TRY(cudaMemcpy(h->mix_tiles, tiles.data(), (size_t)nt * sizeof(QmixTile), cudaMemcpyHostToDevice));
   h->mix_n_tiles = nt;
   std::vector<QmixMicro> micro(1 << 14);
   const int nm = qmix_micro_tiles(h->ql, micro.data(), (int)micro.size());
   MARL_REQUIRE(nm > 0, "marl_dqn_qmix_init: too many weight-gradient micro-tiles");
-  if (dqn_alloc(reinterpret_cast<float**>(&h->mix_micro), (size_t)nm * sizeof(QmixMicro) / 4)) return MARL_ENOMEM;
+  if (int rc = alloc_buffers(h, who, {{&h->mix_micro, (size_t)nm * sizeof(QmixMicro)}})) return rc;
   MARL_CUDA_TRY(cudaMemcpy(h->mix_micro, micro.data(), (size_t)nm * sizeof(QmixMicro), cudaMemcpyHostToDevice));
   h->mix_n_micro = nm;
   // the attribute is per function, process-wide: only ever raise it (a second learner with a smaller mixer must not lower the first one's limit).
@@ -432,8 +405,7 @@ int marl_dqn_forward(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_
   MARL_REQUIRE(!h->rnn, "marl_dqn_forward: the learner has recurrent agent networks: use marl_dqn_forward_rnn, which carries the hidden state");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   const RowPlan plan = make_plan(h->ns, n_envs, 1, h->n_sm, 32);
-  RowSource src; memset(&src, 0, sizeof(src));
-  src.mode = 0; src.dense = obs; src.E = n_envs; src.N = h->ns.n_agents; src.D = h->ns.in;
+  const RowSource src = dense_rows(obs, n_envs, h->ns.n_agents, h->ns.in);
   bool& current = use_target ? h->tgt_image_current : h->image_current;
   const int rc = forward_any(h->ns, plan, src, use_target ? h->theta_tgt : h->theta, use_target ? h->image_tgt : h->image, q_out, (cudaStream_t)stream, current);
   if (rc == MARL_OK) current = tc_forward_enabled() != 0;
@@ -452,9 +424,7 @@ int marl_dqn_forward_rnn(marl_dqn* h, const float* obs, int32_t n_envs, int32_t 
   MARL_REQUIRE(h->rnn, "marl_dqn_forward_rnn: the learner was not created with marl_dqn_create_rnn");
   MARL_REQUIRE(h_in == nullptr || h_in != h_out, "marl_dqn_forward_rnn: h_in and h_out must not alias");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  RowSource src; memset(&src, 0, sizeof(src));
-  src.mode = 0; src.dense = obs; src.E = n_envs; src.N = h->ns.n_agents; src.D = h->ns.in;
-  GruFwdParams fp = gru_fwd_params(h, src, n_envs, 1, use_target != 0);
+  GruFwdParams fp = gru_fwd_params(h, dense_rows(obs, n_envs, h->ns.n_agents, h->ns.in), n_envs, 1, use_target != 0);
   fp.h_in = h_in; fp.h_out = h_out; fp.q_out = q_out;
   return launch_gru_forward(fp, (cudaStream_t)stream);
 }
@@ -475,10 +445,8 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   const int T = traj->T;
-  const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
-  const RowPlan plan = h->rnn ? make_plan(h->ns, batch, 1, h->n_sm, kGruSeqs) : make_plan(h->ns, batch, T + 1, h->n_sm, min_units);
-  RowSource src; memset(&src, 0, sizeof(src));
-  src.mode = 1; src.traj = to_view(traj); src.idx = episode_idx; src.N = h->ns.n_agents; src.D = h->ns.in;
+  const RowPlan plan = h->rnn ? make_plan(h->ns, batch, 1, h->n_sm, kGruSeqs) : episode_plan(h->ns, batch, T, h->n_sm);
+  const RowSource src = episode_rows(traj, episode_idx, h->ns.n_agents, h->ns.in);
   const bool rec = h->timing && h->ev_used < kTimingPairs;
   // target network on every gathered row (dqn/model.py:132-134); several ranks: the previous update launched it between its push and its finish
   if (h->tq_ahead) {
@@ -587,12 +555,11 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   } else if (tc_backward_enabled() && h->ns.in < kMaxObsDim && h->image != nullptr) {   // (no image: hidden width below 128)
     if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
     if (!h->tc_h1) {  // intermediates of the tensor-core pipeline, allocated on first use
-      const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
-      int rc = 0;
-      rc |= dqn_alloc(&h->tc_h1, rows * kHidden); rc |= dqn_alloc(&h->tc_h2, rows * kHidden);
-      rc |= dqn_alloc(&h->tc_dh1, rows * kHidden); rc |= dqn_alloc(&h->tc_rec, rows * 32 /* kRowRec */); rc |= dqn_alloc(&h->tc_x, rows * kMaxObsDim);
-      rc |= dqn_alloc(reinterpret_cast<float**>(&h->image_bwd), (size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4);
-      if (rc) return MARL_ENOMEM;
+      const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), F = sizeof(float);
+      if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h1, rows * kHidden * F}, {&h->tc_h2, rows * kHidden * F}, {&h->tc_dh1, rows * kHidden * F},
+                                                        {&h->tc_rec, rows * 32 /* kRowRec */ * F}, {&h->tc_x, rows * kMaxObsDim * F},
+                                                        {&h->image_bwd, ((size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4) * F}}))
+        return rc;
     }
     if (!h->image_current || !h->bwd_image_current) {
       if (int rc = launch_pack_weights(h->theta, h->ns.lay, h->ns.n_nets, h->image, st, h->image_bwd)) return rc;
@@ -680,11 +647,8 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
   if (h->xchg.world > 1 && tc_split_exchange_enabled()) {
     if (launch_reduce_push(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->push_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
       if (next != nullptr && ap.target_mode == 0 && !h->standardise && h->hp.mixer == 0) {
-        const int T = traj->T;
-        const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
-        const RowPlan plan = make_plan(h->ns, batch, T + 1, h->n_sm, min_units);
-        RowSource src; memset(&src, 0, sizeof(src));
-        src.mode = 1; src.traj = to_view(traj); src.idx = next->idx; src.N = h->ns.n_agents; src.D = h->ns.in;
+        const RowPlan plan = episode_plan(h->ns, batch, traj->T, h->n_sm);
+        const RowSource src = episode_rows(traj, next->idx, h->ns.n_agents, h->ns.in);
         if (int rc = forward_any(h->ns, plan, src, h->theta_tgt, h->image_tgt, h->tq, (cudaStream_t)stream, h->tgt_image_current)) return rc;
         h->tgt_image_current = tc_forward_enabled() != 0;
         h->tq_ahead = true;
@@ -789,8 +753,7 @@ int marl_dqn_peer_handle(marl_dqn* h, void* handle_out) {
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   if (h->xbuf == nullptr) {   // sized for the largest world: [2 parities][kMaxRanks sources][slot] floats + kMaxRanks flags
     h->xchg.slot_floats = (int)((h->n_params + 4 + 63) / 64 * 64);
-    MARL_CUDA_TRY(cudaMalloc(&h->xbuf, xbuf_data_bytes(h) + 256));
-    MARL_CUDA_TRY(cudaMemset(h->xbuf, 0, xbuf_data_bytes(h) + 256));
+    if (int rc = alloc_buffers(h, "marl_dqn_peer_handle", {{&h->xbuf, xbuf_data_bytes(h) + 256}})) return rc;
   }
   cudaIpcMemHandle_t mh;
   MARL_CUDA_TRY(cudaIpcGetMemHandle(&mh, h->xbuf));
@@ -852,23 +815,17 @@ int marl_dqn_counters(marl_dqn* h, int64_t* updates, int64_t* last_target_update
 
 /* The optimiser of the agents' networks (and of the mixer): before the first step only; zeroes the optimiser state. */
 int marl_dqn_set_optimizer(marl_dqn* h, const marl_optimizer* opt) {
-  MARL_REQUIRE(h != nullptr, "marl_dqn_set_optimizer: NULL handle");
-  if (int rc = check_optimizer(opt, "marl_dqn_set_optimizer")) return rc;
-  MARL_REQUIRE(!h->opt_stepped, "marl_dqn_set_optimizer: the learner has already taken an optimiser step; choose the optimiser right after creation");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  if (int rc = check_set_optimizer(h, opt, "marl_dqn_set_optimizer")) return rc;
   if (h->xchg.world > 1) {   // the peer exchange lives in the fused tail: the new optimiser's instantiation must fit one wave as well
     int pb = 0, ns = 0;
     MARL_REQUIRE(reduce_adam_shape((int)h->n_params, h->n_sm, true, opt->kind, &pb, &ns) == MARL_OK,
                  "marl_dqn_set_optimizer: %lld parameters do not fit the fused tail of optimizer kind %d on %d SMs", (long long)h->n_params, opt->kind, h->n_sm);
   }
-  MARL_CUDA_TRY(cudaMemset(h->m, 0, h->n_params * sizeof(float)));
-  MARL_CUDA_TRY(cudaMemset(h->v, 0, h->n_params * sizeof(float)));
   if (h->mix) {
     MARL_CUDA_TRY(cudaMemset(h->mix_m, 0, (size_t)h->ql.n * sizeof(float)));
     MARL_CUDA_TRY(cudaMemset(h->mix_v, 0, (size_t)h->ql.n * sizeof(float)));
   }
-  h->opt = *opt;
-  return MARL_OK;
+  return reset_optimizer(h, *opt);
 }
 
 int marl_dqn_set_counters(marl_dqn* h, int64_t updates, int64_t last_target_update) {

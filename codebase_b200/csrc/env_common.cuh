@@ -1,11 +1,9 @@
 // env_common.cuh -- the parts of an env-step kernel that do not depend on the environment (sm_90a): the fused action selection
 // (epsilon-greedy, categorical), marlbase's StandardiseReward and CooperativeReward wrappers and the trajectory-store writes; and on the
-// host, the handle, buffer ownership, trajectory checks and step launch of the env C ABIs.
+// host, the handle, trajectory checks and step launch of the env C ABIs.
 // Included by lbf_env.cu and rware_env.cu.  Lanes of one env form a group of G consecutive lanes starting at `gbase`; `sub` is the agent.
 #pragma once
 #include <string.h>
-#include <initializer_list>
-#include <vector>
 #include "common.cuh"
 
 namespace marl {
@@ -129,38 +127,14 @@ __device__ __forceinline__ int traj_write_scalars(const TrajDev& traj, const Ste
 
 // ---- host side: the handle layer of the env C ABIs ----------------------------------------------------------------------------------------
 // A handle (marl_lbf, marl_rware) derives from EnvHandle and adds its config `cfg`, device config `dev` (with N and D) and state pointers `st`.
-struct EnvHandle {
+// Its device buffers come from alloc_buffers and are released by destroy_handle.
+struct EnvHandle : BufferOwner {
   int E, device;
   uint64_t seed;
   uint32_t gid0;
   int envs_per_cta, threads;   // step kernel launch shape
   size_t step_smem;
-  std::vector<void*> bufs;     // the device buffers the handle owns, released by env_destroy
 };
-
-struct DevBuf {
-  void** ptr; size_t bytes;
-  template <typename T> DevBuf(T** p, size_t n) : ptr(reinterpret_cast<void**>(p)), bytes(n) {}
-};
-
-// Zero-initialised device buffers, each recorded in h->bufs; stops at the first failure (the caller then destroys the handle).
-inline int alloc_buffers(EnvHandle* h, const char* who, std::initializer_list<DevBuf> list) {
-  for (const DevBuf& b : list) {
-    cudaError_t e = cudaMalloc(b.ptr, b.bytes);
-    if (e == cudaSuccess) { h->bufs.push_back(*b.ptr); e = cudaMemset(*b.ptr, 0, b.bytes); }
-    if (e != cudaSuccess) { set_error("%s: cudaMalloc(%zu) failed: %s", who, b.bytes, cudaGetErrorString(e)); return MARL_ENOMEM; }
-  }
-  return MARL_OK;
-}
-
-template <typename H>
-int env_destroy(H* h) {
-  if (!h) return MARL_OK;
-  cudaSetDevice(h->device);
-  for (void* p : h->bufs) cudaFree(p);
-  delete h;
-  return MARL_OK;
-}
 
 // The attribute is a per-function, process-wide setting: only ever raise it (a second env with a smaller tile must not lower the limit of the
 // first).  `limit` is the kernel's current limit, kept by the caller.

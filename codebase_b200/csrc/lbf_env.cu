@@ -468,7 +468,7 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
   return MARL_OK;
 }
 
-int marl_lbf_destroy(marl_lbf* h) { return env_destroy(h); }
+int marl_lbf_destroy(marl_lbf* h) { return destroy_handle(h); }
 
 int marl_lbf_state_ptrs(marl_lbf* h, marl_lbf_state* out) {
   MARL_REQUIRE(h && out, "marl_lbf_state_ptrs: NULL argument");

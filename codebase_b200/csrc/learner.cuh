@@ -265,18 +265,31 @@ inline RowPlan make_plan(const NetSet& ns, int units_per_agent, int unit_rows, i
   return p;
 }
 
+// A training pass over sampled episodes: one unit per episode (T + 1 rows), at least 64 rows per CTA
+inline RowPlan episode_plan(const NetSet& ns, int episodes, int T, int n_cta_max) {
+  const int min_units = (64 + T) / (T + 1) > 0 ? (64 + T) / (T + 1) : 1;
+  return make_plan(ns, episodes, T + 1, n_cta_max, min_units);
+}
+
 inline TrajView to_view(const marl_traj_view* t) {
   TrajView v; v.obs = t->obs; v.act = t->act; v.rew = t->rew; v.done = t->done; v.filled = t->filled;
   v.capacity = t->capacity; v.N = t->n_agents; v.T = t->T; v.D = t->obs_dim;
   return v;
 }
 
+// Dense rows obs float[E][N][D] (mode 0).  joint: a centralised critic's rows (mode 3), obs float[E][N][D_agent] read as float[E][D = N * D_agent].
+inline RowSource dense_rows(const float* obs, int E, int N, int D, bool joint = false) {
+  RowSource s; memset(&s, 0, sizeof(s));
+  s.mode = joint ? 3 : 0; s.dense = obs; s.E = E; s.N = N; s.D = D;
+  if (joint) s.joint = obs;
+  return s;
+}
 
-inline int dev_alloc_zero(float** p, size_t n_floats) {
-  cudaError_t e = cudaMalloc((void**)p, n_floats * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemset(*p, 0, n_floats * sizeof(float));
-  if (e != cudaSuccess) { set_error("cudaMalloc(%zu floats) failed: %s", n_floats, cudaGetErrorString(e)); return MARL_ENOMEM; }
-  return MARL_OK;
+// Rows of the episodes idx[] of a trajectory store (mode 1)
+inline RowSource episode_rows(const marl_traj_view* t, const int32_t* idx, int N, int D) {
+  RowSource s; memset(&s, 0, sizeof(s));
+  s.mode = 1; s.traj = to_view(t); s.idx = idx; s.N = N; s.D = D;
+  return s;
 }
 
 inline int launch_forward(const NetSet& ns, const RowPlan& plan, const RowSource& src, const float* theta, float* out, cudaStream_t st) {
@@ -334,6 +347,52 @@ inline NetSet to_netset(const marl_mlp_cfg* cfg) {
   memcpy(ns.agent_net, cfg->agent_net, sizeof(int) * MARL_MAX_AGENTS);
   ns.lay = NetLayout::make(cfg->in_dim, cfg->out_dim, cfg->hidden);
   return ns;
+}
+
+// ---- host side: the handle layer of the learner C ABIs ---------------------------------------------------------------------------------------
+// A learner handle (marl_dqn, marl_a2c) derives from LearnerHandle and adds its networks and hyper-parameters `hp`.  Every device buffer it
+// allocates comes from alloc_buffers and is released by destroy_handle.
+struct LearnerHandle : BufferOwner {
+  int device = 0, n_sm = 148;
+  int64_t n_params = 0;          // trainable floats of theta, m and v (grad: + 4 loss statistics)
+  int scratch_pitch = 0;         // floats per CTA of `scratch`: the largest network's P rounded up to 4
+  float *theta = nullptr, *theta_tgt = nullptr, *m = nullptr, *v = nullptr, *grad = nullptr, *scratch = nullptr, *loss_part = nullptr;
+  int32_t* idx = nullptr;
+  uint8_t* image = nullptr;      // packed weight images for the tensor-core forward path (NULL: hidden width below 128)
+  marl_optimizer opt = {};       // the optimiser (marl_*_set_optimizer; Adam with hp's constants by default)
+  bool opt_stepped = false;      // an optimiser step has been launched: the state in m / v belongs to `opt`
+  // standardise_returns: RunningMeanStd of n_stat columns -- mean[n_stat] | var[n_stat] (float32), count (a Python float in the reference),
+  // per-block partial sums (retms.cuh)
+  int standardise = 0, n_stat = 0; float* ret_ms = nullptr; double *ret_count = nullptr, *ret_part = nullptr;
+};
+
+// create's prologue: the device, its SM count and the default optimiser, Adam with hp's constants
+template <typename H, typename HP>
+int open_learner(int device, const HP& hp, H** out) {
+  if (int rc = check_device(device)) return rc;
+  H* h = new H();
+  h->hp = hp; h->device = device;
+  cudaDeviceProp prop; cudaGetDeviceProperties(&prop, device); h->n_sm = prop.multiProcessorCount;
+  h->opt.kind = MARL_OPT_ADAM; h->opt.beta1 = hp.beta1; h->opt.beta2 = hp.beta2; h->opt.eps = hp.eps;
+  *out = h;
+  return MARL_OK;
+}
+
+// marl_*_set_optimizer up to the learner's own checks: the handle, the argument, no step taken yet
+inline int check_set_optimizer(const LearnerHandle* h, const marl_optimizer* o, const char* who) {
+  MARL_REQUIRE(h != nullptr, "%s: NULL handle", who);
+  if (int rc = check_optimizer(o, who)) return rc;
+  MARL_REQUIRE(!h->opt_stepped, "%s: the learner has already taken an optimiser step; choose the optimiser right after creation", who);
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  return MARL_OK;
+}
+
+// ... and after them: zero the optimiser state and switch to `o`
+inline int reset_optimizer(LearnerHandle* h, const marl_optimizer& o) {
+  MARL_CUDA_TRY(cudaMemset(h->m, 0, h->n_params * sizeof(float)));
+  MARL_CUDA_TRY(cudaMemset(h->v, 0, h->n_params * sizeof(float)));
+  h->opt = o;
+  return MARL_OK;
 }
 
 }  // namespace marl

@@ -1,8 +1,8 @@
 // retms.cuh -- RunningMeanStd (marlbase/utils/standardise_stream.py:6-43) over a batch of returns, on the device: shared by the actor-critic
 // learners (a2c.cu: one column per agent) and the DQN family (dqn.cu: one column per agent, VDN: one column per batch entry -- the reference's
-// reshape(-1, arr.size(-1)) of its (E, B) returns).
+// reshape(-1, arr.size(-1)) of its (E, B) returns); and on the host, the handle's statistics buffers.
 #pragma once
-#include "common.cuh"
+#include "learner.cuh"
 
 namespace marl {
 
@@ -71,5 +71,19 @@ static inline cudaError_t ret_ms_step(const RetMsParams& rp, cudaStream_t st) {
   return cudaGetLastError();
 }
 
+// The handle's statistics of n columns, allocated on first enable: mean 0, var 1, count 1e-4 (RunningMeanStd.__init__).  The device is current.
+inline int enable_ret_stats(LearnerHandle* h, int n, const char* who) {
+  if (h->ret_ms) return MARL_OK;
+  if (int rc = alloc_buffers(h, who, {{&h->ret_ms, 2 * n * sizeof(float)}, {&h->ret_count, sizeof(double)},
+                                      {&h->ret_part, (size_t)kRetBlocks * n * 2 * sizeof(double)}}))
+    return rc;
+  std::vector<float> init(2 * n, 0.f);
+  for (int a = 0; a < n; ++a) init[n + a] = 1.f;
+  const double c0 = 1e-4;
+  MARL_CUDA_TRY(cudaMemcpy(h->ret_ms, init.data(), 2 * n * sizeof(float), cudaMemcpyHostToDevice));
+  MARL_CUDA_TRY(cudaMemcpy(h->ret_count, &c0, sizeof(double), cudaMemcpyHostToDevice));
+  h->n_stat = n;
+  return MARL_OK;
+}
 
 }  // namespace marl

@@ -428,7 +428,7 @@ int marl_rware_create(const marl_rware_cfg* cfg, int32_t n_envs, uint64_t seed, 
   return MARL_OK;
 }
 
-int marl_rware_destroy(marl_rware* h) { return env_destroy(h); }
+int marl_rware_destroy(marl_rware* h) { return destroy_handle(h); }
 
 int marl_rware_set_state(marl_rware* h, const uint8_t* shelves, const uint8_t* agents, const uint32_t* requested, const int32_t* step,
                          const int32_t* inactive, void* stream) {

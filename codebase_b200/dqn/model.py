@@ -9,137 +9,27 @@ owner of device buffers.  There is no CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
-import numbers
 import random
-import math
-from collections import OrderedDict
 
 import numpy as np
 import torch
 
 from .. import _native as nat
 from .. import optimizers
+from ..learner import NativeLearner, flat_to_state_dict, flatdim, hidden_width, init_flat_params, init_flat_rnn_params, mlp_shapes, rnn_shapes, \
+    sharing_to_nets, state_dict_to_flat
 from ..native_env import TrajStore
 
-HIDDEN = 128       # the shipped network's width (layers = [128, 128]) and the widest the kernels take
 
-
-def hidden_width(layers, what="layers", use_rnn=False) -> int:
-    """The hidden width H of `layers` (algorithm.model.layers / actor.layers / critic.layers): the kernels implement two hidden layers of one width
-    (an MLP's two Linear layers, or an RNNNetwork's first_layer and GRU, which the reference requires to be equal), 1 <= H <= 128.  Anything else
-    fails here, in Python, before any native call; marl_dqn_create / marl_a2c_create check the same range."""
-    widths = list(layers)
-    ok = len(widths) == 2 and all(isinstance(w, numbers.Integral) and not isinstance(w, bool) for w in widths) and widths[0] == widths[1] and 1 <= widths[0] <= HIDDEN
-    if not ok:
-        raise NotImplementedError(f"{what}={widths}: the fused kernels implement two hidden layers of one width H, 1 <= H <= {HIDDEN} "
-                                  f"(layers = [H, H]; {'first_layer + one H-wide GRU layer' if use_rnn else 'MLP'})")
-    return int(widths[0])
-
-
-def _dim(space) -> int:
-    """gymnasium.spaces.flatdim for the two space kinds the reference uses (dqn/model.py:32-33)."""
-    if getattr(space, "n", None) is not None:
-        return int(space.n)
-    return int(np.prod(space.shape))
-
-
-def sharing_to_nets(parameter_sharing, n_agents):
-    """utils/models.py:189-196: True -> one network, False -> one per agent, list -> seps indices (renumbered densely)."""
-    if parameter_sharing is True:
-        return [0] * n_agents
-    if parameter_sharing is False or parameter_sharing is None:
-        return list(range(n_agents))
-    order = []
-    for i in parameter_sharing:
-        if i not in order:
-            order.append(i)
-    return [order.index(i) for i in parameter_sharing]
-
-
-def init_flat_params(n_nets, in_dim, out_dim, use_orthogonal_init=True, hidden=HIDDEN):
-    """utils/models.py:8-11,35-44 (host side, once): nn.Linear default init, optionally orthogonal(gain sqrt 2) + zero bias."""
-    parts = []
-    for _ in range(n_nets):
-        for o, i in ((hidden, in_dim), (hidden, hidden), (out_dim, hidden)):
-            lin = torch.nn.Linear(i, o)
-            if use_orthogonal_init:
-                torch.nn.init.orthogonal_(lin.weight.data, gain=math.sqrt(2))
-                torch.nn.init.constant_(lin.bias.data, 0)
-            parts += [lin.weight.data.reshape(-1), lin.bias.data.reshape(-1)]
-    return torch.cat(parts).float()
-
-
-def flat_to_state_dict(flat, prefix, n_nets, in_dim, out_dim, hidden=HIDDEN):
-    sd, o = OrderedDict(), 0
-    for k in range(n_nets):
-        for layer, shape in ((0, (hidden, in_dim)), (2, (hidden, hidden)), (4, (out_dim, hidden))):
-            n = shape[0] * shape[1]
-            sd[f"{prefix}.{k}.network.{layer}.weight"] = flat[o:o + n].view(*shape).clone()
-            o += n
-            sd[f"{prefix}.{k}.network.{layer}.bias"] = flat[o:o + shape[0]].clone()
-            o += shape[0]
-    return sd
-
-
-def state_dict_to_flat(sd, prefix, n_nets):
-    parts = []
-    for k in range(n_nets):
-        for layer in (0, 2, 4):
-            parts += [sd[f"{prefix}.{k}.network.{layer}.weight"].reshape(-1), sd[f"{prefix}.{k}.network.{layer}.bias"].reshape(-1)]
-    return torch.cat([p.float() for p in parts])
-
-
-def rnn_shapes(in_dim, out_dim, hidden=HIDDEN):
-    """RNNNetwork with layers=[H, H] (utils/models.py:51-116): (state_dict name, shape) in the reference's order."""
-    H, H3 = hidden, 3 * hidden
-    return (("first_layer.weight", (H, in_dim)), ("first_layer.bias", (H,)), ("rnn.weight_ih_l0", (H3, H)),
-            ("rnn.weight_hh_l0", (H3, H)), ("rnn.bias_ih_l0", (H3,)), ("rnn.bias_hh_l0", (H3,)),
-            ("final_layer.weight", (out_dim, H)), ("final_layer.bias", (out_dim,)))
-
-
-def init_flat_rnn_params(n_nets, in_dim, out_dim, use_orthogonal_init=True, hidden=HIDDEN):
-    """RNNNetwork.__init__ (host side, once): first_layer and the GRU keep PyTorch's default initialisation; use_orthogonal_init applies to
-    final_layer only (orthogonal, gain sqrt 2, zero bias).  Modules are created in the reference's order, so the RNG stream matches."""
-    parts = []
-    for _ in range(n_nets):
-        first, gru, final = torch.nn.Linear(in_dim, hidden), torch.nn.GRU(hidden, hidden, num_layers=1), torch.nn.Linear(hidden, out_dim)
-        if use_orthogonal_init:
-            torch.nn.init.orthogonal_(final.weight.data, gain=math.sqrt(2))
-            torch.nn.init.constant_(final.bias.data, 0)
-        for t in (first.weight, first.bias, gru.weight_ih_l0, gru.weight_hh_l0, gru.bias_ih_l0, gru.bias_hh_l0, final.weight, final.bias):
-            parts.append(t.data.reshape(-1))
-    return torch.cat(parts).float()
-
-
-def flat_to_rnn_state_dict(flat, prefix, n_nets, in_dim, out_dim, hidden=HIDDEN):
-    sd, o = OrderedDict(), 0
-    for k in range(n_nets):
-        for name, shape in rnn_shapes(in_dim, out_dim, hidden):
-            n = int(np.prod(shape))
-            sd[f"{prefix}.{k}.{name}"] = flat[o:o + n].view(*shape).clone()
-            o += n
-    return sd
-
-
-def rnn_state_dict_to_flat(sd, prefix, n_nets, in_dim, out_dim):
-    return torch.cat([sd[f"{prefix}.{k}.{name}"].reshape(-1).float() for k in range(n_nets) for name, _ in rnn_shapes(in_dim, out_dim)])
-
-
-class QNetwork:
+class QNetwork(NativeLearner):
     mixer = 0
+    _destroy = "marl_dqn_destroy"
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch=None, max_episode_length=None):
         self.use_rnn = bool(use_rnn)
         self.hidden = hidden_width(layers, "layers", self.use_rnn)
-        self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
-        if not torch.cuda.is_available() or not str(device).startswith("cuda"):
-            raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
-        self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
-        self.n_agents = len(obs_space)
-        obs_dims, act_dims = [_dim(o) for o in obs_space], [_dim(a) for a in action_space]
-        if len(set(obs_dims)) != 1 or len(set(act_dims)) != 1:
-            raise NotImplementedError("agents with different observation / action sizes are not implemented")
-        self.in_dim, self.n_actions = obs_dims[0], act_dims[0]
+        self._open(obs_space, action_space, cfg, device)
+        self._shapes = (rnn_shapes if self.use_rnn else mlp_shapes)(self.in_dim, self.n_actions, self.hidden)
         self.action_space = action_space
         self.agent_net = sharing_to_nets(parameter_sharing, self.n_agents)
         self.n_nets = max(self.agent_net) + 1
@@ -148,7 +38,6 @@ class QNetwork:
         self.target_update_interval_or_tau = float(cfg.target_update_interval_or_tau)
         self.max_batch = int(max_batch or getattr(cfg, "batch_size", 1024))
         self.max_T = int(max_episode_length or getattr(cfg, "max_episode_length", 0) or 500)
-        self._lib = nat.lib()
         mcfg = nat.MlpCfg(self.n_agents, self.n_nets, (C.c_int32 * 32)(*self.agent_net), self.in_dim, self.hidden, self.n_actions)
         hp = nat.DqnHP(float(cfg.lr), self.gamma, float(self.grad_clip or 0.0), int(self.double_q), self.target_update_interval_or_tau,
                        0.9, 0.999, 1e-8, self.mixer)
@@ -181,17 +70,9 @@ class QNetwork:
         ms = nat.device_view(pm.value, 2 * n.value, self.device).cpu()
         return ms[: n.value], ms[n.value:], float(nat.device_view(pc.value, 1, self.device, "<f8").cpu()[0])
 
-    def optimizer_state(self):
-        """The optimiser state by torch's names (Adam / AdamW: exp_avg, exp_avg_sq; RMSprop: square_avg; Adagrad: sum; SGD: none), flat [n_params]
-        device views in the layout of `theta`."""
-        return optimizers.state(self.optimizer_name, self.adam_m, self.adam_v)
-
     # ---- reference API ------------------------------------------------------------------------------------------
     def init_hiddens(self, batch_size):
-        """utils/models.py:98-103: zeros (num_layers=1, batch, H) per agent for recurrent networks, None per agent otherwise."""
-        if not self.use_rnn:
-            return [None] * self.n_agents
-        return [torch.zeros(1, batch_size, self.hidden, dtype=torch.float32, device=self.device) for _ in range(self.n_agents)]
+        return self._hiddens(self.use_rnn, batch_size, self.hidden)
 
     def q_values(self, obs: torch.Tensor, target: bool = False, out: torch.Tensor | None = None, h: torch.Tensor | None = None,
                  h_out: torch.Tensor | None = None):
@@ -217,11 +98,8 @@ class QNetwork:
         obs = torch.as_tensor(np.stack([np.asarray(i, np.float32) for i in inputs], 0), device=self.device)
         obs = obs.view(self.n_agents, -1, self.in_dim).transpose(0, 1).contiguous()
         if self.use_rnn:   # hiddens: per agent (1, E, H) or None (dqn/model.py:99 carries them through the critic)
-            h = None
-            if hiddens is not None and not all(x is None for x in hiddens):
-                h = torch.stack([torch.as_tensor(x, device=self.device).reshape(-1, self.hidden) for x in hiddens], 1).float().contiguous()
-            q, h_out = self.q_values(obs, h=h)
-            hiddens = [h_out[:, i].unsqueeze(0).clone() for i in range(self.n_agents)]
+            q, h_out = self.q_values(obs, h=self._stack_hiddens(hiddens, self.hidden))
+            hiddens = self._split_hiddens(h_out)
         else:
             q = self.q_values(obs)
         # the reference's stream: ONE `random.random()` per call decides the joint exploration (dqn/model.py:105), the random joint
@@ -316,35 +194,14 @@ class QNetwork:
         nat.check(self._lib.marl_dqn_params_changed(self._h), "marl_dqn_params_changed")
 
     def state_dict(self):
-        to_sd = flat_to_rnn_state_dict if self.use_rnn else flat_to_state_dict
-        sd = to_sd(self.theta.detach().cpu(), f"critic.{self._kind}", self.n_nets, self.in_dim, self.n_actions, self.hidden)
-        sd.update(to_sd(self.theta_tgt.detach().cpu(), f"target.{self._kind}", self.n_nets, self.in_dim, self.n_actions, self.hidden))
+        sd = flat_to_state_dict(self.theta.detach().cpu(), f"critic.{self._kind}", self.n_nets, self._shapes)
+        sd.update(flat_to_state_dict(self.theta_tgt.detach().cpu(), f"target.{self._kind}", self.n_nets, self._shapes))
         return sd
 
     def load_state_dict(self, sd):
-        if self.use_rnn:
-            for dst, prefix in ((self.theta, "critic"), (self.theta_tgt, "target")):
-                dst.copy_(rnn_state_dict_to_flat(sd, f"{prefix}.{self._kind}", self.n_nets, self.in_dim, self.n_actions))
-        else:
-            self.theta.copy_(state_dict_to_flat(sd, f"critic.{self._kind}", self.n_nets))
-            self.theta_tgt.copy_(state_dict_to_flat(sd, f"target.{self._kind}", self.n_nets))
+        for dst, prefix in ((self.theta, "critic"), (self.theta_tgt, "target")):
+            dst.copy_(state_dict_to_flat(sd, f"{prefix}.{self._kind}", self.n_nets, self._shapes))
         self.params_changed()
-
-    def parameters(self):
-        return [self.theta]
-
-    def close(self):
-        if getattr(self, "_h", None):
-            self._lib.marl_dqn_destroy(self._h)
-            self._h = None
-            # the views below aliased library-owned device memory that no longer exists
-            self.theta = self.theta_tgt = self.adam_m = self.adam_v = self.grad = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class VDNetwork(QNetwork):
@@ -375,7 +232,7 @@ def check_mixing(obs_space, mixing, standardise_returns):
     features, embed_dim and (two-layer hypernetworks) hypernet_embed multiples of 4 up to 64, hypernet_layers 1 or 2.  Anything else fails here,
     in Python, before any native call; marl_dqn_qmix_init checks the same limits and whether the mixer fits shared memory."""
     mixing = dict(mixing)
-    N, S = len(obs_space), sum(_dim(o) for o in obs_space)
+    N, S = len(obs_space), sum(flatdim(o) for o in obs_space)
     E, hl, He = int(mixing["embed_dim"]), int(mixing["hypernet_layers"]), int(mixing["hypernet_embed"])
     why = []
     if not 1 <= N <= 8:

@@ -47,7 +47,7 @@ def test_update_matches_reference_golden(name):
 
 @pytest.mark.parametrize("sharing,P,n_agents,clip", [(False, 64, 2, 0.0), (True, 500, 2, 0.5), (False, 1024, 2, 0.0), ([0, 1, 0], 96, 3, 0.0)])
 def test_update_matches_oracle_on_random_batches(sharing, P, n_agents, clip):
-    from codebase_b200.dqn.model import sharing_to_nets
+    from codebase_b200.learner import sharing_to_nets
 
     rng = np.random.default_rng(P)
     hp = lr.A2CHP(grad_clip=clip)

@@ -151,18 +151,18 @@ def test_width_h_networks_at_128_are_the_oracles():
 # ---- the host-side check ----------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("layers", [[1, 1], [37, 37], [64, 64], [128, 128]])
 def test_host_check_accepts(layers):
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
-    assert M.hidden_width(layers) == layers[0]
-    assert M.hidden_width(layers, "actor.layers", use_rnn=True) == layers[0]
+    assert L.hidden_width(layers) == layers[0]
+    assert L.hidden_width(layers, "actor.layers", use_rnn=True) == layers[0]
 
 
 @pytest.mark.parametrize("layers", [[129, 129], [64, 32], [64], [64, 64, 64], [0, 0], []])
 def test_host_check_refuses(layers):
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
     with pytest.raises(NotImplementedError, match=re.escape(f"layers={layers}") + r".*1 <= H <= 128"):
-        M.hidden_width(layers)
+        L.hidden_width(layers)
 
 
 def _dqn_cfg():
@@ -202,31 +202,33 @@ def test_constructors_refuse_before_any_native_call(layers, monkeypatch):
 
 
 # ---- state_dict names and shapes --------------------------------------------------------------------------------------------------------------
-def test_state_dict_keys_and_shapes_match_the_reference_at_64():
+def test_layout_tables_match_the_reference_state_dict_at_64():
     """the reference's FCNetwork / RNNNetwork at layers [64, 64]: the names and shapes the flat layout converts to (recorded in the fixture)"""
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
     g = reference_outputs("hidden_width_reference")
-    mlp = M.flat_to_state_dict(torch.zeros(2 * hr.net_size(DQN_D, A, 64)), "critic.independent", 2, DQN_D, A, 64)
-    rnn = M.flat_to_rnn_state_dict(torch.zeros(2 * hr.net_size(DQN_D, A, 64, True)), "critic.independent", 2, DQN_D, A, 64)
+    mlp = L.flat_to_state_dict(torch.zeros(2 * hr.net_size(DQN_D, A, 64)), "critic.independent", 2, L.mlp_shapes(DQN_D, A, 64))
+    rnn = L.flat_to_state_dict(torch.zeros(2 * hr.net_size(DQN_D, A, 64, True)), "critic.independent", 2, L.rnn_shapes(DQN_D, A, 64))
     for sd, key in ((mlp, "idqn_64"), (rnn, "idqn_gru_64")):
         names = [str(x) for x in g[f"{key}_sd_names"]]
         shapes = [tuple(int(v) for v in s if v >= 0) for s in g[f"{key}_sd_shapes"]]
         mine = [(k, tuple(v.shape)) for k, v in sd.items() if k.startswith("critic.")]
         assert mine == list(zip(names, shapes))
     flat = torch.randn(2 * hr.net_size(DQN_D, A, 64, True))
-    assert torch.equal(M.rnn_state_dict_to_flat(M.flat_to_rnn_state_dict(flat, "c", 2, DQN_D, A, 64), "c", 2, DQN_D, A), flat)
+    shapes = L.rnn_shapes(DQN_D, A, 64)
+    assert torch.equal(L.state_dict_to_flat(L.flat_to_state_dict(flat, "c", 2, shapes), "c", 2, shapes), flat)
     flat = torch.randn(2 * hr.net_size(DQN_D, A, 37))
-    assert torch.equal(M.state_dict_to_flat(M.flat_to_state_dict(flat, "c", 2, DQN_D, A, 37), "c", 2), flat)
+    shapes = L.mlp_shapes(DQN_D, A, 37)
+    assert torch.equal(L.state_dict_to_flat(L.flat_to_state_dict(flat, "c", 2, shapes), "c", 2, shapes), flat)
 
 
 def test_host_initialisation_at_37():
     """init_flat_params / init_flat_rnn_params build the compact layout of width H (P = H*in + H + H*H + H + out*H + out)"""
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
-    assert M.init_flat_params(2, DQN_D, A, True, 37).numel() == 2 * hr.net_size(DQN_D, A, 37)
-    assert M.init_flat_rnn_params(1, DQN_D, A, True, 37).numel() == hr.net_size(DQN_D, A, 37, True)
-    w3 = hr.split_net(M.init_flat_params(1, DQN_D, A, True, 37), DQN_D, A, 37)[4]
+    assert L.init_flat_params(2, DQN_D, A, True, 37).numel() == 2 * hr.net_size(DQN_D, A, 37)
+    assert L.init_flat_rnn_params(1, DQN_D, A, True, 37).numel() == hr.net_size(DQN_D, A, 37, True)
+    w3 = hr.split_net(L.init_flat_params(1, DQN_D, A, True, 37), DQN_D, A, 37)[4]
     assert torch.allclose(w3 @ w3.T, 2.0 * torch.eye(A), atol=1e-5)
 
 

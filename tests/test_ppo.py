@@ -168,7 +168,7 @@ def test_oracle_ppo_kink_risk():
 @pytest.mark.parametrize("sharing,P,n_agents,clip,epochs,lr_", [(False, 64, 2, 0.0, 4, 3e-4), (True, 500, 2, 0.5, 4, 3e-4), ([0, 1, 0], 96, 3, 0.0, 2, 3e-4),
                                                                (False, 128, 2, 0.5, 6, 3e-3)])   # the last: a learning rate that drives ratios out of the clip range
 def test_ppo_update_matches_oracle(sharing, P, n_agents, clip, epochs, lr_):
-    from codebase_b200.dqn.model import sharing_to_nets
+    from codebase_b200.learner import sharing_to_nets
     rng = np.random.default_rng(P + epochs)
     hp = lr.A2CHP(grad_clip=clip, lr=lr_, target_update_interval_or_tau=2)
     m = ac_model(hp, n_agents, D, P, T, sharing=sharing, cls="PPONetwork", num_epochs=epochs)

@@ -196,42 +196,42 @@ def test_fixtures_stay_small():
 
 # ---- host-side layout, key names, initialisation -----------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("arnn,crnn", [(False, False), (True, False), (False, True), (True, True)])
-def test_parameter_layout_and_key_names(arnn, crnn):
+def test_layout_tables_and_key_names(arnn, crnn):
     """the flat [actor | critic] layout and the reference's state_dict names of each part, for the four combinations (shared actor, independent
     centralised critic)"""
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
     D_, CD = 15, 30
     na, nc = (gr.net_size(D_, A) if arnn else lr.net_size(D_, A)), 2 * (gr.net_size(CD, 1) if crnn else lr.net_size(CD, 1))
     assert gr.net_size(15, 6) == 101_894 and gr.net_size(30, 1) == 103_169
     flat = torch.randn(na + nc)
-    to_a = M.flat_to_rnn_state_dict if arnn else M.flat_to_state_dict
-    to_c = M.flat_to_rnn_state_dict if crnn else M.flat_to_state_dict
-    sd = {**to_a(flat[:na], "actor.networks", 1, D_, A), **to_c(flat[na:], "critic.independent", 2, CD, 1)}
+    shapes_a = (L.rnn_shapes if arnn else L.mlp_shapes)(D_, A)
+    shapes_c = (L.rnn_shapes if crnn else L.mlp_shapes)(CD, 1)
+    sd = {**L.flat_to_state_dict(flat[:na], "actor.networks", 1, shapes_a), **L.flat_to_state_dict(flat[na:], "critic.independent", 2, shapes_c)}
     first_a = "actor.networks.0.first_layer.weight" if arnn else "actor.networks.0.network.0.weight"
     first_c = "critic.independent.1.rnn.weight_hh_l0" if crnn else "critic.independent.1.network.2.weight"
     assert first_a in sd and first_c in sd and tuple(sd[first_c].shape) == ((384, 128) if crnn else (128, 128))
     if arnn:
         assert list(sd)[:8] == [f"actor.networks.0.{n}" for n in gr.NAMES]
-    back_a = M.rnn_state_dict_to_flat(sd, "actor.networks", 1, D_, A) if arnn else M.state_dict_to_flat(sd, "actor.networks", 1)
-    back_c = M.rnn_state_dict_to_flat(sd, "critic.independent", 2, CD, 1) if crnn else M.state_dict_to_flat(sd, "critic.independent", 2)
+    back_a = L.state_dict_to_flat(sd, "actor.networks", 1, shapes_a)
+    back_c = L.state_dict_to_flat(sd, "critic.independent", 2, shapes_c)
     assert torch.equal(torch.cat([back_a, back_c]), flat)
     assert gar.is_recurrent(flat[:na], [0, 0], D_, A) == arnn and gar.is_recurrent(flat[na:], [0, 1], CD, 1) == crnn
 
 
 def test_host_initialisation_rule():
     """a recurrent part: orthogonal (gain sqrt 2, zero bias) on final_layer only, PyTorch's defaults elsewhere; an MLP part: orthogonal on every layer"""
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
     torch.manual_seed(4)
-    parts = dict(zip(gr.NAMES, gr.split_net(M.init_flat_rnn_params(1, 30, 1, True), 30, 1)))
+    parts = dict(zip(gr.NAMES, gr.split_net(L.init_flat_rnn_params(1, 30, 1, True), 30, 1)))
     w3 = parts["final_layer.weight"]
     assert torch.allclose(w3 @ w3.T, 2.0 * torch.eye(1), atol=1e-5) and torch.all(parts["final_layer.bias"] == 0)
     bound = 1 / math.sqrt(128)
     for k in ("rnn.weight_ih_l0", "rnn.weight_hh_l0", "rnn.bias_ih_l0", "rnn.bias_hh_l0"):
         assert 0.9 * bound < float(parts[k].abs().max()) <= bound, k
     assert float(parts["first_layer.weight"].abs().max()) <= 1 / math.sqrt(30) and float(parts["first_layer.bias"].abs().max()) > 0
-    w1, b1 = lr.split_net(M.init_flat_params(1, 15, 6, True), 15, 6)[:2]
+    w1, b1 = lr.split_net(L.init_flat_params(1, 15, 6, True), 15, 6)[:2]
     assert torch.allclose(w1.T @ w1, 2.0 * torch.eye(15), atol=1e-4) and torch.all(b1 == 0)
 
 

@@ -151,29 +151,29 @@ def test_fixtures_stay_small():
         assert os.path.getsize(golden_path(name)) < 1 << 20, name
 
 
-def test_flat_state_dict_round_trip_uses_reference_keys():
-    from codebase_b200.dqn import model as M
+def test_rnn_layout_table_round_trip_uses_reference_keys():
+    from codebase_b200 import learner as L
 
     D_, A_ = 15, 6
     flat = torch.randn(2 * gr.net_size(D_, A_))
     assert gr.net_size(D_, A_) == 101_894
-    sd = M.flat_to_rnn_state_dict(flat, "critic.independent", 2, D_, A_)
+    sd = L.flat_to_state_dict(flat, "critic.independent", 2, L.rnn_shapes(D_, A_))
     assert list(sd)[:8] == [f"critic.independent.0.{n}" for n in gr.NAMES]
     shapes = {k.split(".", 3)[3]: tuple(v.shape) for k, v in sd.items() if k.startswith("critic.independent.1.")}
     assert shapes == {"first_layer.weight": (128, D_), "first_layer.bias": (128,), "rnn.weight_ih_l0": (384, 128), "rnn.weight_hh_l0": (384, 128),
                       "rnn.bias_ih_l0": (384,), "rnn.bias_hh_l0": (384,), "final_layer.weight": (A_, 128), "final_layer.bias": (A_,)}
-    assert torch.equal(M.rnn_state_dict_to_flat(sd, "critic.independent", 2, D_, A_), flat)
+    assert torch.equal(L.state_dict_to_flat(sd, "critic.independent", 2, L.rnn_shapes(D_, A_)), flat)
     assert torch.equal(gr.flat_from_state_dict(sd, "critic.independent", 2), flat)
 
 
 def test_host_initialisation_rule():
     """use_orthogonal_init touches final_layer only (orthogonal, gain sqrt 2, zero bias); first_layer keeps nn.Linear's default, the GRU
     PyTorch's uniform(+-1/sqrt(128))"""
-    from codebase_b200.dqn import model as M
+    from codebase_b200 import learner as L
 
     torch.manual_seed(3)
     D_, A_ = 15, 6
-    parts = dict(zip(gr.NAMES, gr.split_net(M.init_flat_rnn_params(1, D_, A_, True), D_, A_)))
+    parts = dict(zip(gr.NAMES, gr.split_net(L.init_flat_rnn_params(1, D_, A_, True), D_, A_)))
     w3 = parts["final_layer.weight"]
     assert torch.allclose(w3 @ w3.T, 2.0 * torch.eye(A_), atol=1e-5) and torch.all(parts["final_layer.bias"] == 0)
     bound = 1 / math.sqrt(128)
@@ -182,7 +182,7 @@ def test_host_initialisation_rule():
     w1 = parts["first_layer.weight"]
     assert float(w1.abs().max()) <= 1 / math.sqrt(D_) and not torch.allclose(w1 @ w1.T, 2.0 * torch.eye(128)[:128, :128], atol=1e-2)
     assert float(parts["first_layer.bias"].abs().max()) > 0
-    flat = M.init_flat_rnn_params(1, D_, A_, False)
+    flat = L.init_flat_rnn_params(1, D_, A_, False)
     assert float(gr.split_net(flat, D_, A_)[7].abs().max()) > 0   # no orthogonal init: final_layer keeps nn.Linear's default
 
 

@@ -42,7 +42,7 @@ def _hp(c):
 
 
 def _agent_net(c):
-    from codebase_b200.dqn.model import sharing_to_nets
+    from codebase_b200.learner import sharing_to_nets
 
     return sharing_to_nets(c.sharing, c.N)
 
