@@ -24,6 +24,7 @@ class LbfCfg(C.Structure):
         ("min_food_level", C.c_int32), ("max_food_level", C.c_int32), ("max_episode_steps", C.c_int32),
         ("time_limit", C.c_int32), ("force_coop", C.c_int32), ("normalize_reward", C.c_int32),
         ("cooperative_reward", C.c_int32), ("penalty", C.c_double), ("observe_id", C.c_int32), ("standardise_rewards", C.c_int32), ("upstream_reset", C.c_int32),
+        ("grid_observation", C.c_int32),
     ]
 
 

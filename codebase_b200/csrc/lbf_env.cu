@@ -36,6 +36,7 @@ struct LbfStateDev {
 
 constexpr int kThreads = 128;
 constexpr int kMaxFood = 32;
+constexpr int kMaxGridSight = 127;   // the largest field side: a wider window only adds padding (and keeps N*D*E-per-CTA in int range)
 
 __device__ __forceinline__ int imin(int a, int b) { return a < b ? a : b; }
 __device__ __forceinline__ int imax(int a, int b) { return a > b ? a : b; }
@@ -147,6 +148,35 @@ __device__ void build_obs(const LbfCfgDev& c, const uint32_t* foods, int nf, con
   for (; slot < c.N; ++slot) { po[3 * slot] = -1.f; po[3 * slot + 1] = -1.f; po[3 * slot + 2] = 0.f; }
 }
 
+// ---- grid observation (ForagingEnv._make_gym_obs with grid_observation=True; DESIGN.md Appendix A) --------
+// Feature d of the agent whose player word is `me`: layer d / W^2 and window cell (wr, wc) = divmod(d % W^2, W), W = 2*sight + 1, which is
+// field cell (row + wr - sight, col + wc - sight).  Layer 0: level of the player on the cell; 1: food level; 2 (access): 1 on a cell of the
+// field that holds neither.  Every layer is 0 off the field (upstream pads by `sight`).  f, amap: one env's field tile and agent map.
+__device__ __forceinline__ float grid_feature(const LbfCfgDev& c, const int8_t* f, const int8_t* amap, uint32_t me, int d) {
+  const int W = 2 * c.S + 1, W2 = W * W;
+  const int layer = d / W2, cell = d - layer * W2, wr = cell / W, wc = cell - wr * W;
+  const int r = (int)(me & 0xFF) + wr - c.S, cc = (int)((me >> 8) & 0xFF) + wc - c.S;
+  if (r < 0 || r >= c.R || cc < 0 || cc >= c.C) return 0.f;
+  const int lv = amap[r * c.C + cc], fo = f[r * c.C + cc];
+  return (float)(layer == 0 ? lv : layer == 1 ? fo : (lv == 0 && fo == 0));
+}
+
+// The CTA writes the grid observations of its envs (EPC per CTA, E in all), one thread per (env, agent, feature): every agent's D-run is
+// contiguous in obs_out [E][N][D] and in the trajectory store, so the stores stay coalesced for any D.  Tiles: field_s / amap_s [EPC][sp],
+// pl_s [EPC][G]; meta_s[l*4+1]: env l's trajectory slot (-1: no write), meta_s[l*4+2]: the observation row it fills.
+__device__ __forceinline__ void write_grid_obs(const LbfCfgDev& c, int E, const int8_t* field_s, const int8_t* amap_s, const uint32_t* pl_s,
+                                               const int* meta_s, float* obs_out, const TrajDev& traj) {
+  const int EPC = (kThreads / 32) * (32 / c.G), sp = c.pitch + 4, e0 = blockIdx.x * EPC, n_here = imin(EPC, E - e0);   // recomputed: nothing stays live
+  const int per_env = c.N * c.D;
+  for (int i = threadIdx.x; i < n_here * per_env; i += kThreads) {
+    const int l = i / per_env, rem = i - l * per_env, ag = rem / c.D, d = rem - ag * c.D;
+    const float v = grid_feature(c, field_s + (size_t)l * sp, amap_s + (size_t)l * sp, pl_s[l * c.G + ag], d);
+    if (obs_out) obs_out[(size_t)e0 * per_env + i] = v;
+    const int sl = meta_s[l * 4 + 1];
+    if (sl >= 0) traj.obs[(((size_t)sl * c.N + ag) * (traj.T + 1) + meta_s[l * 4 + 2]) * c.D + d] = v;
+  }
+}
+
 // upstream adjacent_food_location, `row > 1` / `col > 1` guards included
 __device__ __forceinline__ bool food_location(const LbfCfgDev& c, const int8_t* f, int r, int cc, int& fr, int& fc) {
   if (r > 1 && f[(r - 1) * c.C + cc] > 0) { fr = r - 1; fc = cc; return true; }
@@ -186,6 +216,38 @@ __global__ void lbf_reset_kernel(LbfCfgDev c, LbfStateDev s, int E, uint64_t see
   }
 }
 
+// ---- grid observations after a reset: lbf_reset_kernel resets the state, this kernel writes obs_out and (for the masked envs)
+// init_episode's row 0.  Same CTA shape and shared-memory layout as lbf_step_kernel<true>: field_s, pl_s, meta_s, amap_s.
+__global__ void __launch_bounds__(kThreads) lbf_grid_obs_kernel(LbfCfgDev c, LbfStateDev s, int E, const uint8_t* mask, float* obs_out,
+                                                               TrajDev traj, int slot0) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int EPC = (kThreads / 32) * (32 / c.G), sp = c.pitch + 4;
+  int8_t* field_s = reinterpret_cast<int8_t*>(smem_raw);
+  uint32_t* pl_s = reinterpret_cast<uint32_t*>(field_s + (size_t)EPC * sp);
+  int* meta_s = reinterpret_cast<int*>(pl_s + EPC * c.G);
+  int8_t* amap_s = reinterpret_cast<int8_t*>(meta_s + EPC * 4);
+  const int e0 = blockIdx.x * EPC, n_here = imin(EPC, E - e0);
+  for (int i = threadIdx.x; i < n_here * sp; i += kThreads) {
+    const int l = i / sp, p = i - l * sp;
+    field_s[i] = p < c.pitch ? s.field[(size_t)(e0 + l) * c.pitch + p] : (int8_t)0;
+    amap_s[i] = 0;
+  }
+  for (int l = threadIdx.x; l < n_here; l += kThreads) {
+    const bool doit = (mask == nullptr) || mask[e0 + l];
+    meta_s[l * 4 + 1] = (traj.enabled && doit) ? (slot0 + e0 + l) % traj.capacity : -1;
+    meta_s[l * 4 + 2] = 0;
+  }
+  __syncthreads();
+  for (int l = threadIdx.x; l < n_here; l += kThreads)
+    for (int ag = 0; ag < c.N; ++ag) {   // ascending agent order: on a shared cell the later player's level stays (see lbf_step_kernel)
+      const uint32_t w = s.players[((size_t)e0 + l) * c.N + ag];
+      pl_s[l * c.G + ag] = w;
+      amap_s[(size_t)l * sp + (int)(w & 0xFF) * c.C + (int)((w >> 8) & 0xFF)] = (int8_t)((w >> 16) & 0xFF);
+    }
+  __syncthreads();
+  write_grid_obs(c, E, field_s, amap_s, pl_s, meta_s, obs_out, traj);
+}
+
 __global__ void lbf_set_state_kernel(LbfCfgDev c, LbfStateDev s, int E, const int8_t* field, const uint32_t* players, const int32_t* step) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
@@ -214,6 +276,10 @@ __global__ void lbf_get_state_kernel(LbfCfgDev c, LbfStateDev s, int E, int8_t* 
 }
 
 // ---- the transition kernel ---------------------------------------------------------------------------------
+// kGrid = false: the vector observation, staged [EPC][N][D] in shared memory.  kGrid = true: the grid observation, which does not fit that
+// staging at grid widths (full sight on 8x8: 64 envs x 2 agents x 867 x 4 B = 444 KB); each env gets an int8 agent map beside its field tile
+// instead, and write_grid_obs produces the observation from the two.
+template <bool kGrid>
 __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStateDev s, StepArgs a, TrajDev traj) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int G = c.G, EPW = 32 / G, EPC = (kThreads / 32) * EPW;
@@ -222,9 +288,10 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   const int sp = c.pitch + 4, spw = sp >> 2, p16 = c.pitch >> 4;
   int8_t* field_s = reinterpret_cast<int8_t*>(smem_raw);                                   // [EPC][sp]
   uint32_t* pl_s = reinterpret_cast<uint32_t*>(field_s + (size_t)EPC * sp);                 // [EPC][G]
-  uint32_t* foods_s = pl_s + EPC * G;                                                       // [EPC][NF]
-  int* meta_s = reinterpret_cast<int*>(foods_s + EPC * c.NF);                               // [EPC][4]: nfood, traj slot (-1 = no write), t_next
-  float* obs_s = reinterpret_cast<float*>(meta_s + EPC * 4);                                // [EPC][N][D]
+  uint32_t* foods_s = pl_s + EPC * G;                                                       // [EPC][NF] (vector only)
+  int* meta_s = reinterpret_cast<int*>(foods_s + (kGrid ? 0 : EPC * c.NF));                 // [EPC][4]: nfood, traj slot (-1 = no write), t_next
+  float* obs_s = reinterpret_cast<float*>(meta_s + EPC * 4);                                // [EPC][N][D] (vector only)
+  int8_t* amap_s = reinterpret_cast<int8_t*>(meta_s + EPC * 4);                             // [EPC][sp] (grid only): player level per cell
 
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int le = warp * EPW + lane / G, sub = lane % G, gbase = (lane / G) * G;
@@ -241,6 +308,10 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
       const uint4 v = src[i];
       uint32_t* d = dst + l * spw + 4 * q;
       d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+    }
+    if constexpr (kGrid) {
+      uint32_t* am = reinterpret_cast<uint32_t*>(amap_s);
+      for (int i = threadIdx.x; i < n_here * spw; i += kThreads) am[i] = 0u;
     }
   }
   __syncthreads();
@@ -366,15 +437,24 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
     }
     a.done_out[e] = active ? (uint8_t)done : (uint8_t)1;
     a.trunc_out[e] = (uint8_t)trunc;
-    meta_s[le * 4 + 0] = list_foods(c, f, foods_s + le * c.NF, c.NF);
+    if constexpr (!kGrid) meta_s[le * 4 + 0] = list_foods(c, f, foods_s + le * c.NF, c.NF);
+    if constexpr (kGrid) {
+      // Two players can share a cell (one enters the cell of another whose own move collided), so the agent map is written in ascending
+      // agent order: the later player's level stays, as in upstream's assignment loop.
+      for (int i = 0; i < c.N; ++i) {
+        const uint32_t w = pl_s[le * G + i];
+        amap_s[(size_t)le * sp + (int)(w & 0xFF) * c.C + (int)((w >> 8) & 0xFF)] = (int8_t)((w >> 16) & 0xFF);
+      }
+    }
     meta_s[le * 4 + 1] = slot;
     meta_s[le * 4 + 2] = step1;
   }
   __syncwarp();
   if (env_ok && sub < c.N) {
     if (alive) s.ep_return[(size_t)e * c.N + sub] = (finished && a.autoreset) ? 0.f : ep_ret;
-    s.players[(size_t)e * c.N + sub] = pl_s[le * G + sub];
-    build_obs(c, foods_s + le * c.NF, meta_s[le * 4 + 0], pl_s + le * G, sub, obs_s + ((size_t)le * c.N + sub) * c.D);
+    const uint32_t w = pl_s[le * G + sub];
+    s.players[(size_t)e * c.N + sub] = w;
+    if constexpr (!kGrid) build_obs(c, foods_s + le * c.NF, meta_s[le * 4 + 0], pl_s + le * G, sub, obs_s + ((size_t)le * c.N + sub) * c.D);
   }
   __syncthreads();
 
@@ -387,6 +467,10 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
       const uint32_t* w = src + l * spw + 4 * q;
       dst[i] = make_uint4(w[0], w[1], w[2], w[3]);
     }
+  }
+  if constexpr (kGrid) {
+    write_grid_obs(c, a.E, field_s, amap_s, pl_s, meta_s, a.obs_out, traj);
+    return;
   }
   const int per_env = c.N * c.D;
   if (a.obs_out) {
@@ -424,7 +508,18 @@ static int validate_cfg(const marl_lbf_cfg* c) {
   MARL_REQUIRE(c->min_player_level >= 1 && c->max_player_level >= c->min_player_level && c->max_player_level <= 30, "marl_lbf: bad player levels");
   MARL_REQUIRE(c->sight >= 1, "marl_lbf: sight must be >= 1");
   MARL_REQUIRE(c->max_episode_steps >= 1, "marl_lbf: max_episode_steps must be >= 1");
+  if (c->grid_observation) {
+    MARL_REQUIRE(!c->observe_id, "marl_lbf: grid observations cannot be combined with observe_id (ObserveID assumes a flattened observation space)");
+    MARL_REQUIRE(c->sight <= kMaxGridSight, "marl_lbf: sight %d out of range for grid observations (1..%d)", c->sight, kMaxGridSight);
+  }
   return MARL_OK;
+}
+
+// Shared memory per CTA of lbf_step_kernel (both observation kinds) and lbf_grid_obs_kernel (grid)
+static size_t step_smem_bytes(const LbfCfgDev& d, bool grid) {
+  const size_t EPC = (size_t)(kThreads / 32) * (32 / d.G), sp = (size_t)d.pitch + 4;
+  if (grid) return EPC * (2 * sp + (size_t)d.G * 4 + 16);
+  return EPC * sp + EPC * d.G * 4 + EPC * d.NF * 4 + EPC * 16 + EPC * d.N * d.D * 4;
 }
 
 static LbfCfgDev to_dev(const marl_lbf_cfg& c) {
@@ -442,7 +537,14 @@ static LbfCfgDev to_dev(const marl_lbf_cfg& c) {
 
 extern "C" {
 
-int marl_lbf_obs_dim(const marl_lbf_cfg* cfg) { return cfg ? 3 * cfg->max_num_food + 3 * cfg->n_agents + (cfg->observe_id ? cfg->n_agents : 0) : MARL_EINVAL; }
+int marl_lbf_obs_dim(const marl_lbf_cfg* cfg) {
+  if (!cfg) return MARL_EINVAL;
+  if (cfg->grid_observation) {
+    if (cfg->sight < 1 || cfg->sight > kMaxGridSight) return MARL_EINVAL;
+    return 3 * (2 * cfg->sight + 1) * (2 * cfg->sight + 1);
+  }
+  return 3 * cfg->max_num_food + 3 * cfg->n_agents + (cfg->observe_id ? cfg->n_agents : 0);
+}
 
 int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint32_t env_gid0, int32_t device, marl_lbf** out) {
   MARL_REQUIRE(out != nullptr, "marl_lbf_create: out is NULL");
@@ -450,19 +552,31 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
   if (int rc = validate_cfg(cfg)) return rc;
   MARL_REQUIRE(n_envs >= 1, "marl_lbf_create: n_envs must be >= 1");
   if (int rc = check_device(device)) return rc;
+  const bool grid = cfg->grid_observation != 0;
+  if (grid) {   // every env of a CTA needs its field tile and its agent map: name the limit rather than fail in cudaFuncSetAttribute
+    const LbfCfgDev d = to_dev(*cfg);
+    const size_t need = step_smem_bytes(d, true);
+    int optin = 0;
+    MARL_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    MARL_REQUIRE(need <= (size_t)optin, "marl_lbf_create: grid observations of a %dx%d field with %d agents need %zu B of shared memory per CTA "
+                 "(%d envs x 2 tiles of %d B); the device allows %d B", cfg->rows, cfg->cols, cfg->n_agents, need,
+                 (kThreads / 32) * (32 / d.G), d.pitch + 4, optin);
+  }
   marl_lbf* h = new marl_lbf();
   h->cfg = *cfg; h->dev = to_dev(*cfg); h->E = n_envs; h->device = device; h->seed = seed; h->gid0 = env_gid0;
   const LbfCfgDev& d = h->dev;
   const size_t E = (size_t)n_envs;
   const int EPC = (kThreads / 32) * (32 / d.G);
   h->envs_per_cta = EPC; h->threads = kThreads;
-  h->step_smem = (size_t)EPC * (d.pitch + 4) + (size_t)EPC * d.G * 4 + (size_t)EPC * d.NF * 4 + (size_t)EPC * 16 + (size_t)EPC * d.N * d.D * 4;
-  static size_t step_smem_limit = 48 * 1024;
+  h->step_smem = step_smem_bytes(d, grid);
+  static size_t step_smem_limit = 48 * 1024, grid_step_smem_limit = 48 * 1024, grid_obs_smem_limit = 48 * 1024;
   int rc = alloc_buffers(h, "marl_lbf_create", {{&h->st.field, E * d.pitch}, {&h->st.players, E * d.N * 4}, {&h->st.step, E * 4},
                                                 {&h->st.food_spawned, E * 4}, {&h->st.ep_return, E * d.N * 4}, {&h->st.ep_len, E * 4},
                                                 {&h->st.episode_idx, E * 4}, {&h->st.active, E}, {&h->st.stdr, E * (2 * d.N + 1) * 4},
                                                 {&h->st.stdr_n, E * 4}});
-  if (rc == MARL_OK) rc = raise_smem_limit(lbf_step_kernel, h->step_smem, step_smem_limit, "marl_lbf_create");
+  if (rc == MARL_OK && !grid) rc = raise_smem_limit(lbf_step_kernel<false>, h->step_smem, step_smem_limit, "marl_lbf_create");
+  if (rc == MARL_OK && grid) rc = raise_smem_limit(lbf_step_kernel<true>, h->step_smem, grid_step_smem_limit, "marl_lbf_create");
+  if (rc == MARL_OK && grid) rc = raise_smem_limit(lbf_grid_obs_kernel, h->step_smem, grid_obs_smem_limit, "marl_lbf_create");
   if (rc != MARL_OK) { marl_lbf_destroy(h); return rc; }
   *out = h;
   return MARL_OK;
@@ -500,7 +614,13 @@ int marl_lbf_reset(marl_lbf* h, const uint8_t* reset_mask, float* obs_out, const
   MARL_REQUIRE(h != nullptr, "marl_lbf_reset: NULL handle");
   if (int rc = check_traj(h, traj)) return rc;
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, to_traj(traj), slot0);
+  if (!h->cfg.grid_observation) {
+    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, to_traj(traj), slot0);
+  } else {   // the state here, the grid observations and init_episode's row 0 from the CTA-wide element loop of lbf_grid_obs_kernel
+    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, nullptr, to_traj(nullptr), 0);
+    lbf_grid_obs_kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, kThreads, h->step_smem, (cudaStream_t)stream>>>(
+        h->dev, h->st, h->E, reset_mask, obs_out, to_traj(traj), slot0);
+  }
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }
@@ -509,7 +629,7 @@ int marl_lbf_step(marl_lbf* h, const int32_t* actions, float* obs_out, float* re
                   float* final_ret_out, int32_t* final_len_out, int32_t autoreset, void* stream) {
   MARL_REQUIRE(h && actions && rew_out && done_out && trunc_out, "marl_lbf_step: NULL argument");
   const StepArgs a = step_args(h, actions, obs_out, rew_out, done_out, trunc_out, final_ret_out, final_len_out, autoreset);
-  return launch_step(h, lbf_step_kernel, a, nullptr, stream);
+  return launch_step(h, h->cfg.grid_observation ? lbf_step_kernel<true> : lbf_step_kernel<false>, a, nullptr, stream);
 }
 
 int marl_lbf_rollout_step(marl_lbf* h, const float* values, const marl_rollout_args* ra, const marl_traj_view* traj, float* obs_inout,
@@ -521,7 +641,7 @@ int marl_lbf_rollout_step(marl_lbf* h, const float* values, const marl_rollout_a
   if (int rc = rollout_step_args(h, "marl_lbf_rollout_step", values, ra, traj, obs_inout, rew_out, done_out, trunc_out, final_ret_out, final_len_out,
                                  actions_out, a))
     return rc;
-  return launch_step(h, lbf_step_kernel, a, traj, stream);
+  return launch_step(h, h->cfg.grid_observation ? lbf_step_kernel<true> : lbf_step_kernel<false>, a, traj, stream);
 }
 
 }  // extern "C"

@@ -2,10 +2,12 @@
 
 All arrays are torch CUDA tensors; nothing here computes on the CPU.  Env ids follow the third-party
 ``lbforaging`` registration the reference passes to ``gym.make`` (marlbase/utils/envs.py:90-92,
-README.md:80-85): ``[lbforaging:]Foraging[-grid][-2s]-{s}x{s}-{p}p-{f}f[-coop][-pen]-v{1,2,3}``.
+README.md:80-85): ``[lbforaging:]Foraging[-grid][-{k}s]-{s}x{s}-{p}p-{f}f[-coop][-pen]-v{1,2,3}``.  Vector-observation ids take
+``-2s`` only; grid-observation ids (``-grid``) any sight 1 <= k <= s, and sight s without the tag (DESIGN.md Appendix A).
 """
 from __future__ import annotations
 
+import math
 import re
 from dataclasses import dataclass, asdict
 
@@ -14,7 +16,7 @@ import torch
 from . import _native as nat
 from .native_env import NativeEnv, TrajStore  # noqa: F401  (callers import TrajStore from here too)
 
-_ID = re.compile(r"^(?:lbforaging:)?Foraging(?P<grid>-grid)?(?P<po>-2s)?-(?P<s>\d+)x(?P<s2>\d+)-(?P<p>\d+)p-(?P<f>\d+)f(?P<coop>-coop)?(?P<pen>-pen)?-v(?P<v>\d+)$")
+_ID = re.compile(r"^(?:lbforaging:)?Foraging(?P<grid>-grid)?(?:-(?P<k>\d+)s)?-(?P<s>\d+)x(?P<s2>\d+)-(?P<p>\d+)p-(?P<f>\d+)f(?P<coop>-coop)?(?P<pen>-pen)?-v(?P<v>\d+)$")
 
 
 @dataclass
@@ -37,9 +39,12 @@ class LbfConfig:
     observe_id: int = 0            # env.observe_id: ObserveID wrapper (one-hot agent id in front of every observation)
     standardise_rewards: int = 0   # env.standardise_rewards: StandardiseReward wrapper (per-env running statistics)
     upstream_reset: int = 0        # 1: upstream's reset details (stale positions block cells, permutation draws consumed), see marl_lbf_cfg
+    grid_observation: int = 0      # 1: grid observation (Foraging-grid-* ids): agents | foods | access layers of the window, flattened
 
     @property
     def obs_dim(self) -> int:
+        if self.grid_observation:
+            return 3 * (2 * self.sight + 1) ** 2
         return 3 * self.max_num_food + 3 * self.n_agents + (self.n_agents if self.observe_id else 0)
 
     @property
@@ -48,7 +53,10 @@ class LbfConfig:
 
     @property
     def obs_bounds(self) -> tuple[float, float]:
-        """Observation-space bounds: coordinates and levels, -1 for absent entities."""
+        """Observation-space bounds: coordinates and levels, -1 for absent entities.  A grid observation is only served flattened, and
+        FlattenObservation's Box is unbounded."""
+        if self.grid_observation:
+            return -math.inf, math.inf
         return -1.0, float(max(self.rows, self.cols))
 
     def to_native(self) -> nat.LbfCfg:
@@ -59,12 +67,15 @@ def parse_env_id(name: str, time_limit: int = 0, **overrides) -> LbfConfig:
     m = _ID.match(name)
     if not m:
         raise ValueError(f"unsupported environment id {name!r}: the GPU path implements Level-Based Foraging ids only")
-    if m["grid"]:
-        raise ValueError("grid observations (Foraging-grid-*) are not implemented on the GPU path")
     s, s2, p, f, v = int(m["s"]), int(m["s2"]), int(m["p"]), int(m["f"]), int(m["v"])
-    cfg = LbfConfig(rows=s, cols=s2, n_agents=p, max_num_food=f, sight=2 if m["po"] else s,
+    grid, k = bool(m["grid"]), (int(m["k"]) if m["k"] is not None else None)
+    if k is not None and not grid and k != 2:
+        raise ValueError(f"unsupported environment id {name!r}: the GPU path implements Level-Based Foraging ids only")
+    if grid and k is not None and not 1 <= k <= s:
+        raise ValueError(f"environment id {name!r}: grid ids take a sight 1 <= k <= {s} (the field size), got -{k}s")
+    cfg = LbfConfig(rows=s, cols=s2, n_agents=p, max_num_food=f, sight=k if k is not None else s,
                     max_player_level=2 if v >= 3 else 3, force_coop=int(bool(m["coop"])),
-                    penalty=0.1 if m["pen"] else 0.0, time_limit=int(time_limit or 0))
+                    penalty=0.1 if m["pen"] else 0.0, time_limit=int(time_limit or 0), grid_observation=int(grid))
     for k, val in overrides.items():
         if not hasattr(cfg, k):
             raise TypeError(f"unknown LBF option {k!r}")

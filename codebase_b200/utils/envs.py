@@ -22,7 +22,7 @@ from ..lbf import LbfConfig, NativeLbf, parse_env_id
 from ..rware import NativeRware, RwareConfig, is_rware_id, parse_rware_id
 from . import spaces
 
-SUPPORTED_WRAPPERS = {"CooperativeReward"}
+SUPPORTED_WRAPPERS = {"CooperativeReward", "FlattenObservation"}
 
 
 class _Unwrapped:
@@ -31,12 +31,13 @@ class _Unwrapped:
 
 
 class B200VecEnv:
-    def __init__(self, cfg: LbfConfig | RwareConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None):
+    def __init__(self, cfg: LbfConfig | RwareConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None, flatten: bool = False):
+        """`flatten`: the FlattenObservation wrapper (marlbase/utils/wrappers.py:48-72), whose Box is unbounded."""
         self.cfg, self.num_envs = cfg, int(parallel_envs)
         self.native = (NativeRware if isinstance(cfg, RwareConfig) else NativeLbf)(cfg, self.num_envs, seed, env_gid0, device)
         self.n_agents = cfg.n_agents
         self.unwrapped = _Unwrapped(cfg.n_agents)
-        lo, hi = cfg.obs_bounds
+        lo, hi = (-np.inf, np.inf) if flatten else cfg.obs_bounds
         self.single_observation_space = spaces.Tuple([spaces.Box(lo, hi, (cfg.obs_dim,), np.float32)] * cfg.n_agents)
         self.single_action_space = spaces.Tuple([spaces.Discrete(cfg.n_actions)] * cfg.n_agents)
         self.observation_space = spaces.Tuple([spaces.Box(lo, hi, (self.num_envs, cfg.obs_dim), np.float32)] * cfg.n_agents)
@@ -103,8 +104,16 @@ def make_env(seed, enable_video=False, name=None, time_limit=None, clear_info=Fa
     if unknown:
         raise NotImplementedError(f"env.wrappers {unknown} are not implemented on the GPU path (supported: {sorted(SUPPORTED_WRAPPERS)})")
     cfg = (parse_rware_id if is_rware_id(name) else parse_env_id)(name, time_limit or 0, **kwargs)
+    flatten = "FlattenObservation" in wrappers
+    if getattr(cfg, "grid_observation", 0):
+        if observe_id:   # ObserveID wraps before env.wrappers (envs.py:98-99), so it meets the (3, W, W) Box and asserts (wrappers.py:79-82)
+            raise ValueError(f"env.observe_id=True cannot be used with the grid observations of {name!r}: "
+                             "the ObserveID wrapper assumes a flattened observation space, and it is applied before env.wrappers")
+        if not flatten:
+            raise ValueError(f"{name!r} has (3, W, W) grid observations, which the drivers cannot consume: "
+                             "add the FlattenObservation wrapper (env.wrappers=[FlattenObservation])")
     cfg.cooperative_reward = int("CooperativeReward" in wrappers)
     cfg.observe_id, cfg.standardise_rewards = int(bool(observe_id)), int(bool(standardise_rewards))   # envs.py:97-101, inside the listed wrappers
     if seed is None:
         seed = random.randint(0, 99999)  # envs.py:58-59
-    return B200VecEnv(cfg, int(parallel_envs or 1), int(seed), env_gid0, device)
+    return B200VecEnv(cfg, int(parallel_envs or 1), int(seed), env_gid0, device, flatten=flatten)

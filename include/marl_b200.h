@@ -68,6 +68,9 @@ typedef struct {
                                   yet still block their previous episode's cell (upstream never clears positions in reset()), (b) the two
                                   np_random.permutation() calls over the (identical) level bounds consume random draws (here: n - 1 Philox draws
                                   each, values unused).  0 (default): positions are cleared first and no draw is spent on the no-op permutations. */
+  int32_t grid_observation;    /* 1: upstream's grid observation (the `Foraging-grid-*` ids, DESIGN.md Appendix A): layers agents | foods | access of the
+                                  (2*sight+1)^2 window centred on the agent, field padded by `sight`, flattened in C order (FlattenObservation).
+                                  1 <= sight <= 127; not with observe_id (ObserveID assumes a flattened observation space). */
 } marl_lbf_cfg;
 
 typedef struct marl_lbf marl_lbf;
@@ -101,7 +104,7 @@ typedef struct {
 int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint32_t env_gid0, int32_t device,
                     marl_lbf** out);
 int marl_lbf_destroy(marl_lbf* env);
-int marl_lbf_obs_dim(const marl_lbf_cfg* cfg);             /* 3*max_num_food + 3*n_agents (+ n_agents with observe_id) */
+int marl_lbf_obs_dim(const marl_lbf_cfg* cfg);             /* 3*max_num_food + 3*n_agents (+ n_agents with observe_id); grid_observation: 3*(2*sight+1)^2 */
 int marl_lbf_state_ptrs(marl_lbf* env, marl_lbf_state* out);
 /* Overwrite the transition state (parity tests): host or device pointers are NOT mixed -- all device. */
 int marl_lbf_set_state(marl_lbf* env, const int8_t* field /*[E][rows*cols] dense*/, const int8_t* players,
