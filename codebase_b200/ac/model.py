@@ -190,6 +190,13 @@ class A2CNetwork(NativeLearner):
         nat.check(self._lib.marl_a2c_update_apply(self._h, C.c_int64(int(step)), nat.ptr(self._metrics), nat.stream_ptr()), "marl_a2c_update_apply")
         return self._metrics
 
+    def update_allreduce(self, batch: TrajStore, n_envs: int, step: int, all_reduce):
+        """update_from_store in the two-call form of data-parallel ranks: update_grads, `all_reduce([grad])` (an in-place sum over ranks of the
+        gradient sums, loss numerators and filled count), update_apply.  `step` is the global env-step count."""
+        self.update_grads(batch, n_envs)
+        all_reduce([self.grad])
+        return self.update_apply(step)
+
     def metrics_dict(self, m=None):
         """ac/model.py:241-246 from the device statistics (policy-gradient term, grad norm, entropy, value loss, ...)."""
         m = (self._metrics if m is None else m).tolist()
@@ -242,5 +249,34 @@ class PPONetwork(A2CNetwork):
                                             nat.ptr(self._metrics), nat.stream_ptr()), "marl_ppo_update")
         return self._metrics
 
-    def update_grads(self, batch, n_envs):
-        raise NotImplementedError("PPO's epochs each need their own optimiser step: the grads / apply split of the data-parallel A2C path does not apply")
+    # marl_ppo_update split per epoch: prepare once, then per epoch epoch_grads(e) -> (exchange) -> epoch_apply(e); with nothing in between the
+    # result is update_from_store's, bit for bit
+    def prepare(self, batch: TrajStore, n_envs: int):
+        """n-step returns and the collecting policy's log-probabilities of the batch (the batch must stay unchanged until the last epoch)."""
+        nat.check(self._lib.marl_ppo_prepare(self._h, batch.ref(), C.c_int32(n_envs), nat.stream_ptr()), "marl_ppo_prepare")
+
+    def epoch_grads(self, batch: TrajStore, n_envs: int, epoch: int):
+        """Epoch `epoch`'s gradient sums and statistics in `grad`; epoch 0 prepares the batch first."""
+        if epoch == 0:
+            self.prepare(batch, n_envs)
+        nat.check(self._lib.marl_ppo_epoch_grads(self._h, C.c_float(self.ppo_clip), nat.stream_ptr()), "marl_ppo_epoch_grads")
+
+    def epoch_apply(self, step: int, epoch: int):
+        """Epoch `epoch`'s optimiser step; the last epoch also updates the target critic and leaves the epochs' mean metrics."""
+        nat.check(self._lib.marl_ppo_epoch_apply(self._h, C.c_int64(int(step)), C.c_int32(epoch), C.c_int32(self.num_epochs), nat.ptr(self._metrics),
+                                                 nat.stream_ptr()), "marl_ppo_epoch_apply")
+        return self._metrics
+
+    def update_grads(self, batch: TrajStore, n_envs: int):
+        raise NotImplementedError("PPO takes one optimiser step per epoch: use epoch_grads(batch, n_envs, epoch) / epoch_apply(step, epoch), or update_allreduce")
+
+    def update_apply(self, step: int):
+        raise NotImplementedError("PPO takes one optimiser step per epoch: use epoch_grads(batch, n_envs, epoch) / epoch_apply(step, epoch), or update_allreduce")
+
+    def update_allreduce(self, batch: TrajStore, n_envs: int, step: int, all_reduce):
+        """update_from_store with one exchange of `grad` per epoch (each epoch is its own optimiser step)."""
+        for e in range(self.num_epochs):
+            self.epoch_grads(batch, n_envs, e)
+            all_reduce([self.grad])
+            self.epoch_apply(step, e)
+        return self._metrics

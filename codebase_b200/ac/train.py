@@ -18,6 +18,7 @@ from pathlib import Path
 
 import torch
 
+from .. import distributed
 from ..config import Config, instantiate
 from ..native_env import TrajStore
 from ..utils.envs import episode_info
@@ -52,36 +53,48 @@ class Collector:
         return env.final_len, env.final_ret
 
 
+def iteration_env_steps(t, P, dp) -> int:
+    """Env steps of one iteration on all ranks, as the reference counts them (ac/train.py:201): longest episode t of each rank's batch x P."""
+    return dp.sum_int(int(t) * int(P))
+
+
 def main(envs, eval_env, logger, time_limit, **cfg):
     cfg = Config(cfg)
     P = envs.num_envs
+    dp = distributed.current()
     from ..dqn.train import check_iteration_budget
 
-    check_iteration_budget(P, time_limit, cfg.total_steps, cfg.eval_interval)
+    check_iteration_budget(P * dp.world, time_limit, cfg.total_steps, cfg.eval_interval)
     model = instantiate(cfg.model, envs.single_observation_space, envs.single_action_space, cfg, max_envs=P, max_episode_length=time_limit)
+    dp.sync_learner(model)
     logger.watch(model)
     collector = Collector(envs, model, time_limit, cfg.use_proper_termination)
     step = updates = last_eval = last_save = 0
     while step < cfg.total_steps + 1:
         t0 = time.perf_counter()
         final_len, final_ret = collector.collect()
-        metrics = model.update_from_store(collector.batch, P, step)
+        if dp.active:   # `step` is global: the target critic's `step % interval == 0` sync fires on every rank at once
+            metrics = model.update_allreduce(collector.batch, P, step, dp.all_reduce_)
+        else:
+            metrics = model.update_from_store(collector.batch, P, step)
         t = int(final_len.max().item())
         if (step - last_eval) >= cfg.eval_interval:
             ln, ret = final_len.cpu().numpy(), final_ret.cpu().numpy()
             per_episode = (time.perf_counter() - t0) / P
-            infos = [episode_info(ret[i], ln[i], per_episode) for i in range(P)]
+            infos = []
+            for ln_r, ret_r, per_r in dp.gather_objects((ln, ret, per_episode)):   # the training episodes of every rank
+                infos += [episode_info(ret_r[i], ln_r[i], per_r) for i in range(len(ln_r))]
             infos.append(model.metrics_dict(metrics))
             infos.append({"updates": updates, "environment_steps": step})
             logger.log_metrics(infos)
             last_eval = step
-        if cfg.save_interval and (step - last_save) >= cfg.save_interval:
+        if cfg.save_interval and (step - last_save) >= cfg.save_interval and dp.is_main:
             Path("checkpoints").mkdir(exist_ok=True)
             torch.save(model.state_dict(), f"checkpoints/model_s{step}.pt")
             last_save = step
         if cfg.video_interval:
             raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the GPU hot path")
         updates += 1
-        step += t * P
+        step += iteration_env_steps(t, P, dp)
     envs.close()
     return dict(environment_steps=step, updates=updates)

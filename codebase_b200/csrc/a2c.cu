@@ -93,6 +93,8 @@ __global__ void iota_kernel(int32_t* x, int n) {
 
 using namespace marl;
 
+struct A2cPass { RowSource src, csrc; RowPlan cplan, aplan; int n_envs; };   // csrc: the critic's rows (== src unless the critic is centralised)
+
 struct marl_a2c : LearnerHandle {
   NetSet actor, critic;
   marl_a2c_hp hp;
@@ -101,6 +103,7 @@ struct marl_a2c : LearnerHandle {
   float *vt = nullptr, *ret = nullptr, *adv = nullptr, *metrics = nullptr;
   int64_t opt_steps = 0;
   float *logits_all = nullptr, *old_logp = nullptr, *epoch_metrics = nullptr;   // PPO (allocated on first use)
+  A2cPass ppo_pass = {}; bool ppo_prepared = false;   // PPO split into epochs: the batch's rows and plans from marl_ppo_prepare
   int centralised = 0; float* joint = nullptr;   // critic.centralised: joint observations of the batch [P][T+1][N * D]
   // recurrent parts: GRU layouts, the sequence outputs of the part being trained and their gradient [N][P][T+1][out], the online pass's saved rows
   // [N][P][T+1][kGruSaveRow] (one buffer: the critic pass ends before the actor pass starts)
@@ -233,8 +236,6 @@ int marl_a2c_forward_rnn(marl_a2c* h, int32_t which, const float* obs, int32_t n
   fp.h_in = h_in; fp.h_out = h_out; fp.q_out = out;
   return launch_gru_forward(fp, (cudaStream_t)stream);
 }
-
-struct A2cPass { RowSource src, csrc; RowPlan cplan, aplan; int n_envs; };   // csrc: the critic's rows (== src unless the critic is centralised)
 
 // sequence forward of a recurrent part over every env's T + 1 steps from h = 0: outputs [N][P][T+1][out], saved rows for BPTT when `save`
 static int a2c_gru_forward(const NetSet& ns, const GruLayout& gl, const RowSource& src, const float* theta, int n_envs, float* q_out, float* save, cudaStream_t st) {
@@ -380,12 +381,11 @@ int marl_a2c_update_apply(marl_a2c* h, int64_t step, float* metrics_out, void* s
 /* PPONetwork.update (ac/model.py:265-352) on the same handle: returns and the collecting policy's log-probabilities once, then `num_epochs`
  * optimisation steps on the same batch with the clipped surrogate (-min(r adv, clip(r, 1 -+ ppo_clip) adv) - entropy_coef H + value_loss_coef
  * value loss; clip_grad_norm_ over all parameters when hp.grad_clip > 0), the target critic synchronised after the last epoch.
- * metrics_out: device float[6] as marl_a2c_update, averaged over the epochs ([0] = the surrogate term). */
-int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, int64_t step, int32_t num_epochs, float ppo_clip, float* metrics_out, void* stream) {
-  MARL_REQUIRE(h != nullptr && num_epochs >= 1 && num_epochs <= kMaxPpoEpochs, "marl_ppo_update: num_epochs %d out of range (1..%d)", (int)num_epochs, kMaxPpoEpochs);
-  MARL_REQUIRE(ppo_clip > 0.f, "marl_ppo_update: ppo_clip must be positive");
-  cudaStream_t st = (cudaStream_t)stream;
-  A2cPass ps;
+ * metrics_out: device float[6] as marl_a2c_update, averaged over the epochs ([0] = the surrogate term).
+ * = marl_ppo_prepare, then num_epochs x (marl_ppo_epoch_grads + marl_ppo_epoch_apply) with nothing in between. */
+static int ppo_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, cudaStream_t st) {
+  h->ppo_prepared = false;
+  A2cPass& ps = h->ppo_pass;
   if (int rc = a2c_prepare(h, batch, n_envs, st, ps)) return rc;
   if (!h->logits_all) {
     const size_t rows = (size_t)h->actor.n_agents * h->max_envs * (h->max_T + 1), F = sizeof(float);
@@ -401,13 +401,49 @@ int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, in
   OldLogpParams op; op.logits = h->logits_all; op.traj = ps.src.traj; op.idx = h->idx; op.N = h->actor.n_agents; op.P = n_envs; op.A = h->actor.out; op.out = h->old_logp;
   old_logp_kernel<<<(op.N * n_envs * batch->T + 255) / 256, 256, 0, st>>>(op);
   MARL_CUDA_TRY(cudaGetLastError());
-  for (int e = 0; e < num_epochs; ++e) {
-    if (int rc = a2c_gradients(h, ps, st, h->old_logp, ppo_clip)) return rc;
-    if (int rc = a2c_apply(h, step, h->epoch_metrics + 6 * e, stream, e == num_epochs - 1)) return rc;
-  }
+  h->ppo_prepared = true;
+  return MARL_OK;
+}
+
+// one epoch's optimiser step; the last epoch (epoch == num_epochs - 1) also updates the target critic and writes the epochs' mean metrics
+static int ppo_epoch_apply(marl_a2c* h, int64_t step, int epoch, int num_epochs, float* metrics_out, cudaStream_t st) {
+  const bool last = epoch == num_epochs - 1;
+  if (int rc = a2c_apply(h, step, h->epoch_metrics + 6 * epoch, st, last)) return rc;
+  if (!last) return MARL_OK;
   mean_metrics_kernel<<<1, 32, 0, st>>>(h->epoch_metrics, num_epochs, metrics_out ? metrics_out : h->metrics);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
+}
+
+int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, int64_t step, int32_t num_epochs, float ppo_clip, float* metrics_out, void* stream) {
+  MARL_REQUIRE(h != nullptr && num_epochs >= 1 && num_epochs <= kMaxPpoEpochs, "marl_ppo_update: num_epochs %d out of range (1..%d)", (int)num_epochs, kMaxPpoEpochs);
+  MARL_REQUIRE(ppo_clip > 0.f, "marl_ppo_update: ppo_clip must be positive");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = ppo_prepare(h, batch, n_envs, st)) return rc;
+  for (int e = 0; e < num_epochs; ++e) {
+    if (int rc = a2c_gradients(h, h->ppo_pass, st, h->old_logp, ppo_clip)) return rc;
+    if (int rc = ppo_epoch_apply(h, step, e, num_epochs, metrics_out, st)) return rc;
+  }
+  return MARL_OK;
+}
+
+int marl_ppo_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, void* stream) {
+  MARL_REQUIRE(h != nullptr, "marl_ppo_prepare: NULL handle");
+  return ppo_prepare(h, batch, n_envs, (cudaStream_t)stream);
+}
+
+int marl_ppo_epoch_grads(marl_a2c* h, float ppo_clip, void* stream) {
+  MARL_REQUIRE(h != nullptr && h->ppo_prepared, "marl_ppo_epoch_grads: call marl_ppo_prepare first");
+  MARL_REQUIRE(ppo_clip > 0.f, "marl_ppo_epoch_grads: ppo_clip must be positive");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  return a2c_gradients(h, h->ppo_pass, (cudaStream_t)stream, h->old_logp, ppo_clip);
+}
+
+int marl_ppo_epoch_apply(marl_a2c* h, int64_t step, int32_t epoch, int32_t num_epochs, float* metrics_out, void* stream) {
+  MARL_REQUIRE(h != nullptr && h->ppo_prepared, "marl_ppo_epoch_apply: call marl_ppo_prepare first");
+  MARL_REQUIRE(num_epochs >= 1 && num_epochs <= kMaxPpoEpochs && epoch >= 0 && epoch < num_epochs,
+               "marl_ppo_epoch_apply: epoch %d / num_epochs %d out of range (1..%d epochs)", (int)epoch, (int)num_epochs, kMaxPpoEpochs);
+  return ppo_epoch_apply(h, step, epoch, num_epochs, metrics_out, (cudaStream_t)stream);
 }
 
 /* The optimiser of actor + critic: before the first step only; zeroes the optimiser state. */

@@ -646,7 +646,7 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
   // GPUs the extra launch (prologue, second pass over the Adam state) cost more than the hidden wait saved (120.9 vs 116.8 us per update).
   if (h->xchg.world > 1 && tc_split_exchange_enabled()) {
     if (launch_reduce_push(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->push_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
-      if (next != nullptr && ap.target_mode == 0 && !h->standardise && h->hp.mixer == 0) {
+      if (next != nullptr && ap.target_mode == 0 && !h->standardise && h->hp.mixer == 0 && !h->rnn) {
         const RowPlan plan = episode_plan(h->ns, batch, traj->T, h->n_sm);
         const RowSource src = episode_rows(traj, next->idx, h->ns.n_agents, h->ns.in);
         if (int rc = forward_any(h->ns, plan, src, h->theta_tgt, h->image_tgt, h->tq, (cudaStream_t)stream, h->tgt_image_current)) return rc;
@@ -655,7 +655,7 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
       }
       if (int rc = launch_adam_finish(rp, ap, h->opt.kind, &h->xchg, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream)) return rc;
       if (fused_out) *fused_out = true;
-      return MARL_OK;
+      return qmix_adam(h, ap, (cudaStream_t)stream);
     }
   }
   if (launch_reduce_adam(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
@@ -751,8 +751,11 @@ static size_t xbuf_data_bytes(const marl_dqn* h) { return (size_t)2 * kMaxRanks 
 int marl_dqn_peer_handle(marl_dqn* h, void* handle_out) {
   MARL_REQUIRE(h != nullptr && handle_out != nullptr, "marl_dqn_peer_handle: NULL argument");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
+  MARL_REQUIRE(h->hp.mixer != 2 || h->mix != nullptr, "marl_dqn_peer_handle: QMIX needs marl_dqn_qmix_init first (the mixer's gradient is part of the exchange)");
   if (h->xbuf == nullptr) {   // sized for the largest world: [2 parities][kMaxRanks sources][slot] floats + kMaxRanks flags
-    h->xchg.slot_floats = (int)((h->n_params + 4 + 63) / 64 * 64);
+    // slot = [agents' gradient sums | QMIX: the mixer's gradient sums | 4 statistics]
+    const int64_t n_extra = h->hp.mixer == 2 ? h->ql.n : 0;
+    h->xchg.slot_floats = (int)((h->n_params + n_extra + 4 + 63) / 64 * 64);
     if (int rc = alloc_buffers(h, "marl_dqn_peer_handle", {{&h->xbuf, xbuf_data_bytes(h) + 256}})) return rc;
   }
   cudaIpcMemHandle_t mh;
@@ -766,8 +769,6 @@ int marl_dqn_peer_attach(marl_dqn* h, int32_t rank, int32_t world, const void* h
   MARL_REQUIRE(h != nullptr && handles != nullptr, "marl_dqn_peer_attach: NULL argument");
   MARL_REQUIRE(world >= 2 && world <= kMaxRanks && rank >= 0 && rank < world, "marl_dqn_peer_attach: rank %d / world %d out of range (2..%d ranks)", rank, world, kMaxRanks);
   MARL_REQUIRE(h->xbuf != nullptr && h->xchg.world <= 1, "marl_dqn_peer_attach: call marl_dqn_peer_handle first, attach once");
-  MARL_REQUIRE(h->hp.mixer != 2, "marl_dqn_peer_attach: the mixer's gradient is not part of the peer exchange: QMIX runs on one GPU");
-  MARL_REQUIRE(!h->rnn, "marl_dqn_peer_attach: recurrent agent networks run on one GPU");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   {  // the exchange lives inside the fused reduce + Adam kernel: refuse here, before any update mutates counters, when that kernel cannot
      // cover this parameter count with one co-resident wave (a later fallback to the two-kernel tail would dead-lock the peers' polls)
@@ -790,6 +791,7 @@ int marl_dqn_peer_attach(marl_dqn* h, int32_t rank, int32_t world, const void* h
   h->xchg.own_flags = h->xchg.peer_flags[rank];
   h->xchg.timed_out = reinterpret_cast<int*>(static_cast<char*>(h->peer_base[rank]) + xbuf_data_bytes(h) + 128);   // behind the 8 flags, zeroed with the buffer
   h->xchg.rank = rank; h->xchg.world = world; h->xchg.epoch = 0;
+  if (h->hp.mixer == 2) { h->xchg.extra = h->mix_grad; h->xchg.n_extra = h->ql.n; }   // the mixer's step then reads the all-rank sum
   return MARL_OK;
 }
 

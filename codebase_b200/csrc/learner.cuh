@@ -190,6 +190,9 @@ struct XchgParams {
   unsigned long long* peer_flags[kMaxRanks];       // every rank's flag array (own included): flag[source rank]
   const unsigned long long* own_flags;             // = peer_flags[rank]
   int* timed_out;                                  // device flag (sticky): a peer's epoch flag did not arrive within the spin bound
+  // a second buffer summed in the same exchange (QMIX: the mixer's gradient sums, already reduced): slot = [n grads | n_extra | 4 statistics].
+  // extra[0 .. n_extra) is pushed, then overwritten with the all-rank sum, and extra[n_extra .. n_extra + 4) with the all-rank statistics
+  float* extra; int n_extra;
 };
 // replay indices for the next update, drawn by the fused tail kernel (idx == NULL: none); same stream as replay_sample_kernel
 struct SampleParams { uint64_t seed, update_idx; int batch, n_valid; int32_t* idx; };

@@ -582,6 +582,12 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
     else if (XCHG) { for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + i] = g; }   // local sums -> every rank (own included)
     else rp.grad[i] = g;
   }
+  if (XCHG && MODE != 3) {   // the second buffer's local sums -> every rank (grid-stride: any n_extra fits)
+    for (int k = blockIdx.x * (int)blockDim.x + t; k < xp.n_extra; k += (int)(gridDim.x * blockDim.x)) {
+      const float e = xp.extra[k];
+      for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + n + k] = e;
+    }
+  }
   // the four loss statistics: one warp each of block 0, fixed order
   if (MODE != 3 && blockIdx.x == 0 && t >= pb && t < pb + 128) {   // (the launcher guarantees ns >= 2 and pb >= 128)
     const int which = (t - pb) >> 5, l = t & 31;
@@ -591,7 +597,7 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
     for (int off = 16; off > 0; off >>= 1) x += __shfl_xor_sync(0xFFFFFFFFu, x, off);
     if (l == 0) {
       x += rp.stats_accumulate ? rp.stats[which] : 0.f;
-      if (XCHG) { for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + n + which] = x; } else rp.stats[which] = x;
+      if (XCHG) { for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + n + xp.n_extra + which] = x; } else rp.stats[which] = x;
     }
   }
   if (MODE == 2) {
@@ -635,9 +641,16 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
     }
     if (t < 4) {
       float x = 0.f;
-      for (int r = 0; r < xp.world; ++r) x += ld_relaxed_sys(mine + (size_t)r * xp.slot_floats + n + t);
+      for (int r = 0; r < xp.world; ++r) x += ld_relaxed_sys(mine + (size_t)r * xp.slot_floats + n + xp.n_extra + t);
       stats_sh[t] = x;
-      if (blockIdx.x == 0) rp.stats[t] = x;
+      if (blockIdx.x == 0) { rp.stats[t] = x; if (xp.n_extra > 0) xp.extra[xp.n_extra + t] = x; }
+    }
+    // the second buffer's all-rank sum, in rank order, in place: every block has pushed (read) its entries before the grid barrier above
+    // (MODE 1) or in the previous launch (MODE 3)
+    for (int k = blockIdx.x * (int)blockDim.x + t; k < xp.n_extra; k += (int)(gridDim.x * blockDim.x)) {
+      float e = 0.f;
+      for (int r = 0; r < xp.world; ++r) e += ld_relaxed_sys(mine + (size_t)r * xp.slot_floats + n + k);
+      xp.extra[k] = e;
     }
   }
   // block sum of squares: slice 0 holds the gradients (pb / 32 warps) -> shuffle tree per warp, then the partials in order

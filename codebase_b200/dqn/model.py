@@ -128,6 +128,21 @@ class QNetwork(NativeLearner):
                                               C.c_uint64(first_update_idx), C.c_int32(n_updates), nat.ptr(self._metrics), nat.stream_ptr()), "marl_dqn_update_n")
         return self._metrics
 
+    def exchanged_buffers(self):
+        """What data-parallel ranks sum between update_grads and update_apply: [gradient sums | loss numerator | filled count | 2 spare]."""
+        return [self.grad]
+
+    def update_n_allreduce(self, traj: TrajStore, batch_size: int, n_valid: int, seed: int, first_update_idx: int, n_updates: int, all_reduce):
+        """update_n's updates (same replay indices) in the two-call form: per update sample, update_grads, `all_reduce(exchanged_buffers())` (an
+        in-place sum over ranks), update_apply.  Every rank then divides by the global filled count and applies the same step."""
+        for u in range(n_updates):
+            nat.check(self._lib.marl_replay_sample(C.c_uint64(seed & (2**64 - 1)), C.c_uint64(first_update_idx + u), C.c_int32(batch_size), C.c_int32(n_valid),
+                                                   nat.ptr(self._idx), nat.stream_ptr()), "marl_replay_sample")
+            self.update_grads(traj, self._idx[:batch_size])
+            all_reduce(self.exchanged_buffers())
+            self.update_apply()
+        return self._metrics
+
     def update(self, batch):
         """Reference signature (dqn/model.py:165-174): `batch` is the reference's Batch namedtuple (obss (N,T+1,B,obs), actions
         (N,T,B), rewards (N,T,B), dones (T+1,B), filled (T,B)); converted to the device layout, then the native update."""
@@ -153,18 +168,33 @@ class QNetwork(NativeLearner):
 
     def attach_peers(self, group=None):
         """Several ranks, one process per GPU: exchange CUDA IPC handles through torch.distributed and let `update` / `update_n` sum
-        the gradients of all ranks over NVLink peer memory inside the fused reduce + Adam kernel (no all-reduce call per update)."""
-        if self.use_rnn:
-            raise NotImplementedError("recurrent agent networks run on one GPU: the peer-memory gradient exchange covers the MLP learners only")
+        the gradients of all ranks over NVLink peer memory inside the fused reduce + Adam kernel (no all-reduce call per update).
+        MLP and recurrent agent networks whose parameters fit one wave of the fused tail; QMIX's mixer gradient travels in the same exchange.
+        Every rank makes the same collective calls whatever fails where, and either every rank returns or every rank raises NativeError (a rank
+        that did attach keeps working with the two-call form: update_grads, an all-reduce, update_apply)."""
         import torch.distributed as dist
 
         world, rank = dist.get_world_size(group), dist.get_rank(group)
-        mine = (C.c_ubyte * 64)()
-        nat.check(self._lib.marl_dqn_peer_handle(self._h, mine), "marl_dqn_peer_handle")
+        mine, err = (C.c_ubyte * 64)(), None
+        try:
+            nat.check(self._lib.marl_dqn_peer_handle(self._h, mine), "marl_dqn_peer_handle")
+        except nat.NativeError as e:
+            err = str(e)
         handles = [None] * world
-        dist.all_gather_object(handles, bytes(mine), group=group)
-        blob = b"".join(handles)
-        nat.check(self._lib.marl_dqn_peer_attach(self._h, C.c_int32(rank), C.c_int32(world), blob), "marl_dqn_peer_attach")
+        dist.all_gather_object(handles, bytes(mine) if err is None else None, group=group)
+        if err is None:
+            if any(h is None for h in handles):
+                err = "a peer has no exchange buffer"
+            else:
+                try:
+                    nat.check(self._lib.marl_dqn_peer_attach(self._h, C.c_int32(rank), C.c_int32(world), b"".join(handles)), "marl_dqn_peer_attach")
+                except nat.NativeError as e:
+                    err = str(e)
+        errors = [None] * world
+        dist.all_gather_object(errors, err, group=group)   # agree on the outcome: one collective, reached by every rank
+        failed = [f"rank {r}: {e}" for r, e in enumerate(errors) if e is not None]
+        if failed:
+            raise nat.NativeError("peer-memory gradient exchange unavailable: " + "; ".join(failed))
         self.peers_attached = True
         dist.barrier(group)
 
@@ -312,8 +342,10 @@ class QMixNetwork(QNetwork):
     def parameters(self):
         return [self.theta, self.mix]
 
-    def attach_peers(self, group=None):
-        raise NotImplementedError("QMIX runs on one GPU: the mixer's gradient is not part of the peer-memory exchange")
+    def exchanged_buffers(self):
+        """The agents' buffer and the mixer's [gradient sums | loss numerator | filled count | 2 spare]: the mixer's step divides by its own
+        filled count, which the sum makes global."""
+        return [self.grad, self.mix_grad]
 
     def close(self):
         super().close()

@@ -18,11 +18,14 @@ seeded by run.py and cannot be reproduced -- SURVEY F6).
 """
 from __future__ import annotations
 
+import logging
 import time
 from pathlib import Path
 
 import torch
 
+from .. import _native as nat
+from .. import distributed
 from ..config import Config, instantiate
 from ..native_env import TrajStore
 from ..utils.envs import episode_info
@@ -95,11 +98,35 @@ def _episode_infos(final_len, final_ret, seconds):
     return [episode_info(ret[i], ln[i], per_episode) for i in range(len(ln))]
 
 
+def iteration_env_steps(final_len, dp) -> int:
+    """Env steps of one iteration on all ranks: the sum of every collected episode's length.  Then step, epsilon, training_start, the intervals
+    and the loop condition agree on every rank; this host collective also keeps a rank out of an in-kernel exchange while rank 0 evaluates or saves."""
+    return dp.sum_int(final_len.sum().item())
+
+
+def attach_peer_exchange(model, dp) -> bool:
+    """Several ranks, each on its own device: sum the gradients inside the fused reduce + Adam kernel over peer memory (IDQN / VDN / QMIX, MLP or
+    recurrent, whose parameters fit one wave of the fused tail).  All ranks or none: attach_peers agrees on the outcome on every rank, and a
+    refusal anywhere makes every rank use the all-reduce between the two calls.  Never with ranks that share a device: the exchange's bounded
+    spin assumes co-resident peers."""
+    if not (dp.active and dp.own_device):
+        return False
+    try:
+        model.attach_peers()
+    except nat.NativeError as e:  # e.g. no peer access between the devices, or too many parameters for one wave of the fused tail
+        logging.warning("%s: one all-reduce per update", e)
+        return False
+    return True
+
+
 def main(env, eval_env, logger, time_limit, **cfg):
     cfg = Config(cfg)
     E = env.num_envs
-    check_iteration_budget(E, time_limit, cfg.total_steps, cfg.eval_interval, cfg.eps_decay_over)
+    dp = distributed.current()
+    check_iteration_budget(E * dp.world, time_limit, cfg.total_steps, cfg.eval_interval, cfg.eps_decay_over)
     model = instantiate(cfg.model, env.single_observation_space, env.single_action_space, cfg, max_batch=cfg.batch_size, max_episode_length=time_limit)
+    dp.sync_learner(model)
+    peer = attach_peer_exchange(model, dp)
     logger.watch(model)
     capacity = int(cfg.buffer_size)
     if capacity < E:
@@ -109,17 +136,21 @@ def main(env, eval_env, logger, time_limit, **cfg):
     collector = Collector(env, model, time_limit, cfg.use_proper_termination, cfg.get("replay_clear_stale", False))
     evaluator = Collector(eval_env, model, time_limit) if eval_env is not None else None
     updates_per_iteration = int(cfg.get("updates_per_iteration") or E)
-    seed = int(cfg.get("seed_for_sampling", 0) or env.native.seed)
+    # replay sampling stream: one per rank
+    seed = int(cfg.get("seed_for_sampling", 0) or env.native.seed) + 7919 * dp.rank
 
     updates = step = pos = 0
     last_eval = last_save = 0
     metrics_dev = None
     while step < cfg.total_steps + 1:
         final_len, _ = collector.collect(rb, pos % capacity, eps_sched(step))
-        step += int(final_len.sum().item())
+        step += iteration_env_steps(final_len, dp)
         pos += E
         if step > cfg.training_start and pos >= cfg.batch_size:
-            metrics_dev = model.update_n(rb, int(cfg.batch_size), min(pos, capacity), seed, updates, updates_per_iteration)
+            if dp.active and not peer:
+                metrics_dev = model.update_n_allreduce(rb, int(cfg.batch_size), min(pos, capacity), seed, updates, updates_per_iteration, dp.all_reduce_)
+            else:
+                metrics_dev = model.update_n(rb, int(cfg.batch_size), min(pos, capacity), seed, updates, updates_per_iteration)
             updates += updates_per_iteration
         else:
             metrics_dev = None
@@ -138,7 +169,7 @@ def main(env, eval_env, logger, time_limit, **cfg):
         if cfg.video_interval:
             raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the GPU hot path")
 
-        if cfg.save_interval and (step - last_save) >= cfg.save_interval:
+        if cfg.save_interval and (step - last_save) >= cfg.save_interval and dp.is_main:
             Path("checkpoints").mkdir(exist_ok=True)
             torch.save(model.state_dict(), f"checkpoints/model_s{step}.pt")
             last_save = step

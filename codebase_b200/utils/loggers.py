@@ -79,6 +79,13 @@ class Logger:
         return None
 
 
+class NullLogger(Logger):
+    """The logger of data-parallel ranks other than 0: writes nothing (rank 0 logs the metrics of every rank)."""
+
+    def log_metrics(self, metrics):
+        pass
+
+
 class FileSystemLogger(Logger):
     def __init__(self, project_name, cfg):
         super().__init__(project_name, cfg)

@@ -311,7 +311,9 @@ int marl_dqn_set_optimizer(marl_dqn* q, const marl_optimizer* opt);
  * dqn/train.py would add between loss.backward() and optimiser.step()): marl_dqn_peer_handle allocates this rank's exchange buffer
  * and writes its 64-byte CUDA IPC handle; the caller gathers all ranks' handles (rank-ordered, 64 bytes each) and passes them to
  * marl_dqn_peer_attach.  Afterwards marl_dqn_update / marl_dqn_update_n sum the gradients of all ranks over peer memory inside the
- * fused reduce + Adam kernel (identical parameters on every rank, no NCCL call); every rank must issue the same update calls. */
+ * fused reduce + Adam kernel (identical parameters on every rank, no NCCL call); every rank must issue the same update calls.
+ * MLP and recurrent handles whose parameters fit one wave of the fused tail (attach refuses the others); QMIX (call marl_dqn_qmix_init before
+ * marl_dqn_peer_handle): the exchange slot is [agents' gradient sums | mixer's gradient sums | 4 statistics] and the mixer's step reads the all-rank sum. */
 int marl_dqn_peer_handle(marl_dqn* q, void* handle_out64);
 int marl_dqn_peer_attach(marl_dqn* q, int32_t rank, int32_t world, const void* handles);
 /* *timed_out = 1 when an update's in-kernel exchange gave up waiting for a peer (bounded spin, ~10 s): results since are invalid.
@@ -332,7 +334,7 @@ int marl_dqn_set_counters(marl_dqn* q, int64_t updates, int64_t last_target_upda
  * Training runs every sampled episode from a zero hidden state (dqn/model.py:127,133).  marl_dqn_update / _update_n / _update_grads +
  * _update_apply, standardise_returns, qmix_init, sync_target, the counters and marl_dqn_timing work unchanged (the timed window covers the
  * online sequence forward, the TD head and the backward; marl_dqn_timing_kernels reports count 0).  The "tensor_core_*" options do not apply
- * to recurrent handles (FP32 FFMA throughout); marl_dqn_forward and marl_dqn_peer_attach refuse them; in_dim <= 32. */
+ * to recurrent handles (FP32 FFMA throughout); marl_dqn_forward refuses them; in_dim <= 32. */
 int marl_dqn_create_rnn(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t max_batch, int32_t max_T, int32_t device,
                         marl_dqn** out);
 /* One step of model.act's network pass (dqn/model.py:96-99) for E envs: obs device float[E][N][in], h_in / h_out device float[E][N][H]
@@ -394,6 +396,16 @@ int marl_a2c_ret_ms_ptrs(marl_a2c* a, float** ret_ms /* mean[N] | var[N] */, dou
  * surrogate; the target critic follows after the last epoch.  metrics_out: device float[6] as marl_a2c_update, averaged over the epochs. */
 int marl_ppo_update(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, int64_t step, int32_t num_epochs, float ppo_clip,
                     float* metrics_out, void* stream);
+/* marl_ppo_update split where data-parallel ranks exchange grad[0 .. n_actor+n_critic+4) once per epoch.  marl_ppo_update is exactly
+ * marl_ppo_prepare followed by num_epochs x (marl_ppo_epoch_grads + marl_ppo_epoch_apply), so with nothing in between the results are the same bits.
+ *   _prepare:     target-critic pass, n-step returns and the collecting policy's log-probabilities of the batch (kept until the next prepare;
+ *                 the batch must not change before the last epoch)
+ *   _epoch_grads: one epoch's critic + actor passes with the clipped surrogate -> gradient sums + statistics in grad
+ *   _epoch_apply: / filled.sum(), optional clip, optimiser step (epoch = 0 .. num_epochs-1); the last epoch also updates the target critic for
+ *                 `step` and writes the epochs' mean metrics to metrics_out (device float[6] as marl_ppo_update) */
+int marl_ppo_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs, void* stream);
+int marl_ppo_epoch_grads(marl_a2c* h, float ppo_clip, void* stream);
+int marl_ppo_epoch_apply(marl_a2c* h, int64_t step, int32_t epoch, int32_t num_epochs, float* metrics_out, void* stream);
 /* Recurrent actor and / or critic (actor.use_rnn / critic.use_rnn; marlbase/utils/models.py:51-116 RNNNetwork with layers = [H, H], the
  * network and per-network parameter order of marl_dqn_create_rnn).  actor_rnn / critic_rnn != 0 make that part a GRU network; the other part stays
  * the MLP.  marl_a2c_param_ptrs then exposes [actor nets | critic nets], each part in its own layout.  Every update pass runs each env's episode
