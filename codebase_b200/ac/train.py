@@ -21,6 +21,7 @@ import torch
 from .. import distributed
 from ..config import Config, instantiate
 from ..native_env import TrajStore
+from ..utils import video
 from ..utils.envs import episode_info
 
 
@@ -58,10 +59,20 @@ def iteration_env_steps(t, P, dp) -> int:
     return dp.sum_int(int(t) * int(P))
 
 
+def record_episodes(env, model, n_timesteps, path):
+    """marlbase/ac/train.py:122-150 on a one-env B200VecEnv: `n_timesteps` frames of episodes sampled from the policy to the mp4 file `path`
+    (utils.video.record_policy); an episode ends on done or truncated."""
+    return video.record_policy(env, n_timesteps, path, model.logits, 2, 0.0, model.actor_hidden if model.actor_rnn else 0)
+
+
 def main(envs, eval_env, logger, time_limit, **cfg):
     cfg = Config(cfg)
     P = envs.num_envs
     dp = distributed.current()
+    video_env = None
+    if cfg.video_interval and eval_env is not None:   # rank 0 records
+        video.require_encoder()
+        video_env = video.recording_env(eval_env)
     from ..dqn.train import check_iteration_budget
 
     check_iteration_budget(P * dp.world, time_limit, cfg.total_steps, cfg.eval_interval)
@@ -69,7 +80,7 @@ def main(envs, eval_env, logger, time_limit, **cfg):
     dp.sync_learner(model)
     logger.watch(model)
     collector = Collector(envs, model, time_limit, cfg.use_proper_termination)
-    step = updates = last_eval = last_save = 0
+    step = updates = last_eval = last_save = last_video = 0
     while step < cfg.total_steps + 1:
         t0 = time.perf_counter()
         final_len, final_ret = collector.collect()
@@ -92,9 +103,12 @@ def main(envs, eval_env, logger, time_limit, **cfg):
             Path("checkpoints").mkdir(exist_ok=True)
             torch.save(model.state_dict(), f"checkpoints/model_s{step}.pt")
             last_save = step
-        if cfg.video_interval:
-            raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the GPU hot path")
+        if video_env is not None and (step - last_video) >= cfg.video_interval:
+            record_episodes(video_env, model, cfg.video_frames, f"./videos/step-{step}.mp4")
+            last_video = step
         updates += 1
         step += iteration_env_steps(t, P, dp)
     envs.close()
+    if video_env is not None:
+        video_env.close()
     return dict(environment_steps=step, updates=updates)

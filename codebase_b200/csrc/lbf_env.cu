@@ -16,6 +16,7 @@
 //     lanes + shuffle reduction of their levels, food cells resolved in ascending agent order;
 //   * observations are assembled in shared memory and written back as one contiguous coalesced run.
 #include "env_common.cuh"
+#include "render.cuh"
 
 namespace marl {
 
@@ -486,6 +487,46 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   }
 }
 
+// ---- frames (DESIGN.md §4.8): one CTA per (env, band of pixel rows) --------------------------------------------------
+// top: 1 + the index of the agent drawn last on each cell (0: none).  The cell's badge shows that agent's level, else the food's.
+__device__ __forceinline__ render::Rgb lbf_pixel(const LbfCfgDev& c, const int8_t* field, const int8_t* top, const uint32_t* pl, int x, int y) {
+  using namespace render;
+  constexpr int P = kLbfCell + 1, M = kLbfCell / 2;
+  if (x % P == 0 || y % P == 0) return kBlack;
+  const int col = x / P, row = y / P, lx = x - col * P - 1, ly = y - row * P - 1;
+  const int food = (uint8_t)field[row * c.C + col], who = top[row * c.C + col];
+  if (food == 0 && who == 0) return kWhite;
+  if (in_disc(lx, ly, kLbfBadgeC, kLbfBadgeC, kLbfBadgeR)) {
+    const int level = who ? (int)((pl[who - 1] >> 16) & 0xFF) : food;
+    const bool ink = in_number(lx, ly, level, kLbfBadgeC, kLbfBadgeC) || !in_disc(lx, ly, kLbfBadgeC, kLbfBadgeC, kLbfBadgeR - kLbfBadgeLine);
+    return ink ? kBlack : kWhite;
+  }
+  if (who && in_disc(lx, ly, M, M, kLbfAgentR)) return kLbfAgent;
+  if (food && in_disc(lx, ly, M, M, kLbfFoodR)) return kLbfFood;
+  return kWhite;
+}
+
+// One kernel for vector and grid ids: they share the state.  frames: [n][H][W][3], frame l of env env_first + l.
+__global__ void __launch_bounds__(render::kRenderThreads) lbf_render_kernel(LbfCfgDev c, LbfStateDev s, int env_first, uint8_t* frames, int H, int W) {
+  __shared__ __align__(16) uint8_t band_s[render::kBandBytes + 16];
+  __shared__ int8_t field_s[4096], top_s[4096];
+  __shared__ uint32_t pl_s[MARL_MAX_AGENTS];
+  const int l = blockIdx.x;
+  const size_t e = (size_t)env_first + l;
+  for (int i = threadIdx.x; i < c.RC; i += blockDim.x) { field_s[i] = s.field[e * c.pitch + i]; top_s[i] = 0; }
+  for (int i = threadIdx.x; i < c.N; i += blockDim.x) pl_s[i] = s.players[e * c.N + i];
+  __syncthreads();
+  if (threadIdx.x == 0)   // ascending agent order: on a shared cell the higher index is drawn last, as in the observation
+    for (int i = 0; i < c.N; ++i) {
+      const int r = (int)(pl_s[i] & 0xFF), cc = (int)((pl_s[i] >> 8) & 0xFF);
+      if (r < c.R && cc < c.C) top_s[r * c.C + cc] = (int8_t)(i + 1);
+    }
+  __syncthreads();
+  const int rows = render::band_rows(W), y0 = blockIdx.y * rows, y1 = imin(H, y0 + rows);
+  render::render_band(frames + (size_t)l * H * W * 3, W, y0, y1, band_s,
+                      [&](int x, int y) { return lbf_pixel(c, field_s, top_s, pl_s, x, y); });
+}
+
 }  // namespace marl
 
 // =============================================================================================================
@@ -642,6 +683,19 @@ int marl_lbf_rollout_step(marl_lbf* h, const float* values, const marl_rollout_a
                                  actions_out, a))
     return rc;
   return launch_step(h, h->cfg.grid_observation ? lbf_step_kernel<true> : lbf_step_kernel<false>, a, traj, stream);
+}
+
+int marl_lbf_frame_shape(const marl_lbf_cfg* cfg, int32_t* h, int32_t* w) {
+  MARL_REQUIRE(cfg && h && w, "marl_lbf_frame_shape: NULL argument");
+  if (int rc = validate_cfg(cfg)) return rc;
+  *h = render::frame_side(cfg->rows, render::kLbfCell); *w = render::frame_side(cfg->cols, render::kLbfCell);
+  return MARL_OK;
+}
+
+int marl_lbf_render(marl_lbf* h, int32_t env_first, int32_t n, uint8_t* frames, void* stream) {
+  MARL_REQUIRE(h != nullptr, "marl_lbf_render: NULL handle");
+  return render::launch_render(h, "marl_lbf_render", lbf_render_kernel, env_first, n, frames, render::frame_side(h->dev.R, render::kLbfCell),
+                               render::frame_side(h->dev.C, render::kLbfCell), stream);
 }
 
 }  // extern "C"

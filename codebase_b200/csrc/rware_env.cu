@@ -15,6 +15,7 @@
 //     atomicMax); the winner of each merge is a max-reduction of (chain length, insertion rank) over the lanes with the same target;
 //   * observations are assembled in shared memory and written back as one contiguous run per env.
 #include "env_common.cuh"
+#include "render.cuh"
 
 namespace marl {
 
@@ -349,6 +350,54 @@ __global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwSt
   }
 }
 
+// ---- frames (DESIGN.md §4.8): one CTA per (env, band of pixel rows) --------------------------------------------------------
+// Layers bottom to top: goal fill, shelf rectangle (its current cell, a carried one under its carrier), agent disc, direction line.
+// top: 1 + the index of the agent drawn on each cell (0: none; agents stand on distinct cells, a later index would be drawn last).
+__device__ __forceinline__ render::Rgb rware_pixel(const RwCfgDev& c, const uint8_t* sh, const int8_t* top, const uint32_t* ag, const uint32_t* req,
+                                                   int x, int y) {
+  using namespace render;
+  constexpr int P = kRwCell + 1, M = kRwCell / 2;
+  if (x % P == 0 || y % P == 0) return kBlack;
+  const int col = x / P, row = y / P, lx = x - col * P - 1, ly = y - row * P - 1, cell = row * c.C + col;
+  if (const int who = top[cell]) {
+    const uint32_t w = ag[who - 1];
+    const int d = (int)((w >> 16) & 0xFF);
+    if (d < 4) {
+      const int dx = d == 3 ? 1 : d == 2 ? -1 : 0, dy = d == 1 ? 1 : d == 0 ? -1 : 0;
+      if (on_line(lx, ly, M, M, M + dx * kRwAgentR, M + dy * kRwAgentR, kRwDirLine)) return kRwDir;
+    }
+    if (in_disc(lx, ly, M, M, kRwAgentR)) return (w >> 24) ? kRwAgentLoaded : kRwAgent;
+  }
+  const int sid = sh[cell];
+  if (sid && in_rect(lx, ly, kRwShelfPad, kRwShelfPad, kRwCell - kRwShelfPad, kRwCell - kRwShelfPad))
+    return requested(req, sid) ? kRwShelfRequested : kRwShelf;
+  if (cell == c.goal0 || cell == c.goal1) return kRwGoal;
+  return kWhite;
+}
+
+// frames: [n][H][W][3], frame l of env env_first + l
+__global__ void __launch_bounds__(render::kRenderThreads) rware_render_kernel(RwCfgDev c, RwStateDev s, int env_first, uint8_t* frames, int H, int W) {
+  __shared__ __align__(16) uint8_t band_s[render::kBandBytes + 16];
+  __shared__ uint8_t sh_s[4096];
+  __shared__ int8_t top_s[4096];
+  __shared__ uint32_t ag_s[32], req_s[kReqWords];
+  const int l = blockIdx.x;
+  const size_t e = (size_t)env_first + l;
+  for (int i = threadIdx.x; i < c.RC; i += blockDim.x) { sh_s[i] = s.shelves[e * c.pitch + i]; top_s[i] = 0; }
+  for (int i = threadIdx.x; i < c.N; i += blockDim.x) ag_s[i] = s.agents[e * c.N + i];
+  if (threadIdx.x < kReqWords) req_s[threadIdx.x] = s.req[e * kReqWords + threadIdx.x];
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int i = 0; i < c.N; ++i) {
+      const int x = (int)(ag_s[i] & 0xFF), y = (int)((ag_s[i] >> 8) & 0xFF);
+      if (x < c.C && y < c.R) top_s[y * c.C + x] = (int8_t)(i + 1);
+    }
+  __syncthreads();
+  const int rows = render::band_rows(W), y0 = blockIdx.y * rows, y1 = min(H, y0 + rows);
+  render::render_band(frames + (size_t)l * H * W * 3, W, y0, y1, band_s,
+                      [&](int x, int y) { return rware_pixel(c, sh_s, top_s, ag_s, req_s, x, y); });
+}
+
 }  // namespace marl
 
 // =============================================================================================================
@@ -478,6 +527,20 @@ int marl_rware_rollout_step(marl_rware* h, const float* values, const marl_rollo
                                  actions_out, a))
     return rc;
   return launch_step(h, rware_step_kernel, a, traj, stream);
+}
+
+int marl_rware_frame_shape(const marl_rware_cfg* cfg, int32_t* h, int32_t* w) {
+  MARL_REQUIRE(cfg && h && w, "marl_rware_frame_shape: NULL argument");
+  if (int rc = rware_validate(cfg)) return rc;
+  const RwCfgDev d = rware_to_dev(*cfg);
+  *h = render::frame_side(d.R, render::kRwCell); *w = render::frame_side(d.C, render::kRwCell);
+  return MARL_OK;
+}
+
+int marl_rware_render(marl_rware* h, int32_t env_first, int32_t n, uint8_t* frames, void* stream) {
+  MARL_REQUIRE(h != nullptr, "marl_rware_render: NULL handle");
+  return render::launch_render(h, "marl_rware_render", rware_render_kernel, env_first, n, frames, render::frame_side(h->dev.R, render::kRwCell),
+                               render::frame_side(h->dev.C, render::kRwCell), stream);
 }
 
 }  // extern "C"

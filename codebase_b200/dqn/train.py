@@ -28,6 +28,7 @@ from .. import _native as nat
 from .. import distributed
 from ..config import Config, instantiate
 from ..native_env import TrajStore
+from ..utils import video
 from ..utils.envs import episode_info
 
 
@@ -119,10 +120,21 @@ def attach_peer_exchange(model, dp) -> bool:
     return True
 
 
+def record_episodes(env, model, n_timesteps, path, epsilon):
+    """marlbase/dqn/train.py:239-261 on a one-env B200VecEnv: `n_timesteps` frames of epsilon-greedy episodes to the mp4 file `path`
+    (utils.video.record_policy).  An episode ends on done or truncated; the reference ignores truncation here and would step past its TimeLimit,
+    while the step kernel freezes a finished env."""
+    return video.record_policy(env, n_timesteps, path, model.q_values, 1, epsilon, model.hidden if model.use_rnn else 0)
+
+
 def main(env, eval_env, logger, time_limit, **cfg):
     cfg = Config(cfg)
     E = env.num_envs
     dp = distributed.current()
+    video_env = None
+    if cfg.video_interval and eval_env is not None:   # rank 0 records
+        video.require_encoder()
+        video_env = video.recording_env(eval_env)
     check_iteration_budget(E * dp.world, time_limit, cfg.total_steps, cfg.eval_interval, cfg.eps_decay_over)
     model = instantiate(cfg.model, env.single_observation_space, env.single_action_space, cfg, max_batch=cfg.batch_size, max_episode_length=time_limit)
     dp.sync_learner(model)
@@ -140,7 +152,7 @@ def main(env, eval_env, logger, time_limit, **cfg):
     seed = int(cfg.get("seed_for_sampling", 0) or env.native.seed) + 7919 * dp.rank
 
     updates = step = pos = 0
-    last_eval = last_save = 0
+    last_eval = last_save = last_video = 0
     metrics_dev = None
     while step < cfg.total_steps + 1:
         final_len, _ = collector.collect(rb, pos % capacity, eps_sched(step))
@@ -166,8 +178,10 @@ def main(env, eval_env, logger, time_limit, **cfg):
             logger.log_metrics(infos)
             last_eval = step
 
-        if cfg.video_interval:
-            raise NotImplementedError("algorithm.video_interval: video recording is out of scope of the GPU hot path")
+        # here, like evaluation: the other ranks wait in the next iteration's host collective, not in the in-kernel peer exchange
+        if video_env is not None and (step - last_video) >= cfg.video_interval:
+            record_episodes(video_env, model, cfg.video_frames, f"./videos/step-{step}.mp4", cfg.eps_evaluation)
+            last_video = step
 
         if cfg.save_interval and (step - last_save) >= cfg.save_interval and dp.is_main:
             Path("checkpoints").mkdir(exist_ok=True)
@@ -175,4 +189,6 @@ def main(env, eval_env, logger, time_limit, **cfg):
             last_save = step
 
     env.close()
+    if video_env is not None:
+        video_env.close()
     return dict(environment_steps=step, updates=updates)

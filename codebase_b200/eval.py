@@ -1,11 +1,12 @@
 """Evaluate a checkpoint of a finished (or running) run -- the role of marlbase/eval.py:16-64 with the same arguments:
 
-    python -m codebase_b200.eval path=outputs/<env>/<alg>/<hex> [load_step=N] [seed=S] [episodes=K]
+    python -m codebase_b200.eval path=outputs/<env>/<alg>/<hex> [load_step=N] [seed=S] [episodes=K] [video_frames=F]
 
 Like the reference it reads `<path>/config.yaml`, builds the run's env, picks `checkpoints/model_s<load_step>.pt` (the latest when load_step is
-not given), swaps `algorithm._target_`'s "train" for "eval" and calls it with (env, ckpt_path, **algorithm).  The reference's eval targets record
-a video of `video_frames` steps (dqn/eval.py, ac/eval.py); rendering is out of scope of the GPU path, so ours run `episodes` evaluation episodes on
-the device with the loaded parameters and write their returns to `<path>/eval_s<load_step>.json` instead."""
+not given), swaps `algorithm._target_`'s "train" for "eval" and calls it with (env, ckpt_path, **algorithm).  Ours run `episodes` evaluation
+episodes on the device with the loaded parameters and write their returns to `<path>/eval_s<load_step>.json`.  With `video_frames=F` they also
+record F frames of the policy to `<path>/eval.mp4`, as the reference's eval targets do (dqn/eval.py, ac/eval.py), on a one-env copy of the
+evaluation env (utils.video.recording_env)."""
 from __future__ import annotations
 
 import os
@@ -28,11 +29,12 @@ def latest_step(ckpt_dir: str) -> int:
 
 
 def parse_args(argv):
+    """The four keys always; `video_frames` only when it is given."""
     out = dict(path=None, load_step=None, seed=None, episodes=None)
     for a in argv:
         k, sep, v = a.partition("=")
-        if not sep or k not in out:
-            raise ValueError(f"unknown argument {a!r}: expected path=... [load_step=N] [seed=S] [episodes=K]")
+        if not sep or k not in (*out, "video_frames"):
+            raise ValueError(f"unknown argument {a!r}: expected path=... [load_step=N] [seed=S] [episodes=K] [video_frames=F]")
         out[k] = None if v in ("null", "None", "") else (v if k == "path" else int(v))
     return out
 
@@ -41,6 +43,12 @@ def main(argv=None):
     args = parse_args(list(sys.argv[1:] if argv is None else argv))
     path = args["path"]
     assert path and os.path.isdir(path), f"Path {path} is not a directory."
+    video_kw = {}
+    if args.get("video_frames"):
+        from .utils.video import require_encoder
+
+        require_encoder()
+        video_kw = dict(video_frames=int(args["video_frames"]), video_path=os.path.join(path, "eval.mp4"))
     config_path = os.path.join(path, "config.yaml")
     assert os.path.exists(config_path), f"Config file {config_path} does not exist."
     with open(config_path) as f:
@@ -58,7 +66,7 @@ def main(argv=None):
         np.random.seed(seed)
     algo = Config(run_config.algorithm.to_dict())
     algo["_target_"] = str(algo["_target_"]).replace("train", "eval")
-    result = call(algo, env, ckpt_path, time_limit=run_config.env.time_limit)
+    result = call(algo, env, ckpt_path, time_limit=run_config.env.time_limit, **video_kw)
     result.update(load_step=int(load_step), checkpoint=os.path.abspath(ckpt_path))
     import json
 

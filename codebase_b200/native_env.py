@@ -61,6 +61,19 @@ class NativeEnv:
         self.final_ret = torch.zeros(self.E, self.N, dtype=torch.float32, device=dev)
         self.final_len = torch.zeros(self.E, dtype=torch.int32, device=dev)
         self.actions = torch.zeros(self.E, self.N, dtype=torch.int32, device=dev)
+        self._c_render = getattr(lib, f"marl_{self.PREFIX}_render")
+        h, w = C.c_int32(), C.c_int32()
+        fs = getattr(lib, f"marl_{self.PREFIX}_frame_shape")
+        nat.check(fs(C.byref(self._ncfg), C.byref(h), C.byref(w)), fs.__name__)
+        self.frame_shape = (h.value, w.value, 3)
+
+    def render(self, env_first: int = 0, n: int = 1, out: torch.Tensor | None = None) -> torch.Tensor:
+        """RGB frames of envs [env_first, env_first + n), one launch: device uint8 [n, H, W, 3] (`out`, or a new tensor); H, W, 3 = frame_shape."""
+        if out is None:
+            out = torch.empty(int(n), *self.frame_shape, dtype=torch.uint8, device=self.device)
+        assert out.dtype == torch.uint8 and tuple(out.shape) == (int(n), *self.frame_shape), "render: out must be uint8 [n, H, W, 3]"
+        nat.check(self._c_render(self._h, C.c_int32(env_first), C.c_int32(n), nat.ptr(out), nat.stream_ptr()), self._c_render.__name__)
+        return out
 
     def close(self):
         if self._h:

@@ -78,6 +78,10 @@ class B200VecEnv:
             info["final_info"], info["_final_info"] = final, fin
         return self._obs_tuple(obs), rew.cpu().numpy(), done_h, trunc_h, info
 
+    def render(self):
+        """gymnasium's `rgb_array`: env 0's frame of the current state, uint8 (H, W, 3) on the host (drawn on the device, DESIGN.md §4.8)."""
+        return self.native.render(0, 1)[0].cpu().numpy()
+
     def close(self):
         self.native.close()
 
@@ -96,9 +100,8 @@ def make_env(seed, enable_video=False, name=None, time_limit=None, clear_info=Fa
              wrappers=None, parallel_envs=None, env_gid0=0, device=None, **kwargs):
     """marlbase/utils/envs.py:115-119 with the same config keys.  `parallel_envs` absent -> 1 env (the reference's single-env
     factory); the GPU overlays set it to thousands.  `name`: a Level-Based Foraging id (codebase_b200.lbf) or a multi-robot warehouse id
-    (codebase_b200.rware); extra keys override the env's constructor arguments."""
-    if enable_video:
-        raise NotImplementedError("video recording is out of scope of the GPU hot path (algorithm.video_interval must stay False)")
+    (codebase_b200.rware); extra keys override the env's constructor arguments.  `enable_video` is accepted and changes nothing: every native env
+    renders (B200VecEnv.render)."""
     wrappers = list(wrappers or [])
     unknown = [w for w in wrappers if w not in SUPPORTED_WRAPPERS]
     if unknown:

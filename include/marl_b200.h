@@ -152,6 +152,13 @@ int marl_lbf_rollout_step(marl_lbf* env, const float* values, const marl_rollout
                           uint8_t* trunc_out, float* final_ret_out, int32_t* final_len_out,
                           int32_t* actions_out, void* stream);
 
+/* Frames of the current state (video recording; geometry and palette: DESIGN.md §4.8).  A frame is uint8 RGB [h][w][3] with
+ * h = 1 + rows * 51 and w = 1 + cols * 51 (50-px cells, 1-px grid lines), as marl_lbf_frame_shape returns them.  marl_lbf_render writes the
+ * frames of envs [env_first, env_first + n) to the DEVICE buffer frames uint8[n][h][w][3], in one launch; an empty range or one outside
+ * [0, E) returns MARL_EINVAL. */
+int marl_lbf_frame_shape(const marl_lbf_cfg* cfg, int32_t* h, int32_t* w);
+int marl_lbf_render(marl_lbf* env, int32_t env_first, int32_t n, uint8_t* frames, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------
  * Multi-robot warehouse (RWARE), E environments per handle, one transition of all of them per launch.
  * Replaces `env.reset()` / `env.step(actions)` of the gym.make()'d third-party `rware` Warehouse (2.x, gymnasium; ids
@@ -196,6 +203,9 @@ int marl_rware_step(marl_rware* env, const int32_t* actions, float* obs_out, flo
 int marl_rware_rollout_step(marl_rware* env, const float* values, const marl_rollout_args* args, const marl_traj_view* traj,
                             float* obs_inout, float* rew_out, uint8_t* done_out, uint8_t* trunc_out, float* final_ret_out,
                             int32_t* final_len_out, int32_t* actions_out, void* stream);
+/* as marl_lbf_frame_shape / marl_lbf_render, with 30-px cells: h = 1 + rows * 31, w = 1 + cols * 31 */
+int marl_rware_frame_shape(const marl_rware_cfg* cfg, int32_t* h, int32_t* w);
+int marl_rware_render(marl_rware* env, int32_t env_first, int32_t n, uint8_t* frames, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * Per-agent MLP sets and the DQN-family learner (IDQN, VDN).
