@@ -58,8 +58,11 @@ class RolloutArgs(C.Structure):
     ]
 
 
+MAX_AGENTS = 32   # MARL_MAX_AGENTS (include/marl_b200.h): the length of marl_mlp_cfg.agent_net
+
+
 class MlpCfg(C.Structure):
-    _fields_ = [("n_agents", C.c_int32), ("n_nets", C.c_int32), ("agent_net", C.c_int32 * 32), ("in_dim", C.c_int32),
+    _fields_ = [("n_agents", C.c_int32), ("n_nets", C.c_int32), ("agent_net", C.c_int32 * MAX_AGENTS), ("in_dim", C.c_int32),
                 ("hidden", C.c_int32), ("out_dim", C.c_int32)]
 
 

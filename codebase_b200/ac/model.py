@@ -16,7 +16,7 @@ import torch
 
 from .. import _native as nat
 from .. import optimizers
-from ..learner import NativeLearner, flat_to_state_dict, flatdim, hidden_width, init_flat_params, init_flat_rnn_params, mlp_shapes, rnn_shapes, \
+from ..learner import MAX_AGENTS, NativeLearner, flat_to_state_dict, flatdim, hidden_width, init_flat_params, init_flat_rnn_params, mlp_shapes, rnn_shapes, \
     sharing_to_nets, state_dict_to_flat
 from ..native_env import TrajStore
 
@@ -66,8 +66,8 @@ class A2CNetwork(NativeLearner):
         self._ckind = "independent" if not critic.parameter_sharing else "networks"
         self.max_envs = int(max_envs or 1024)
         self.max_T = int(max_episode_length or 500)
-        acfg = nat.MlpCfg(self.n_agents, self.n_actor_nets, (C.c_int32 * 32)(*self.actor_net), self.in_dim, self.actor_hidden, self.n_actions)
-        ccfg = nat.MlpCfg(self.n_agents, self.n_critic_nets, (C.c_int32 * 32)(*self.critic_net), self.critic_in, self.critic_hidden, 1)
+        acfg = nat.MlpCfg(self.n_agents, self.n_actor_nets, (C.c_int32 * MAX_AGENTS)(*self.actor_net), self.in_dim, self.actor_hidden, self.n_actions)
+        ccfg = nat.MlpCfg(self.n_agents, self.n_critic_nets, (C.c_int32 * MAX_AGENTS)(*self.critic_net), self.critic_in, self.critic_hidden, 1)
         hp = nat.A2cHP(float(cfg.lr), self.gamma, float(self.grad_clip or 0.0), self.n_steps, self.entropy_coef, self.value_loss_coef,
                        self.target_update_interval_or_tau, 0.9, 0.999, 1e-8)
         self._h = C.c_void_p()

@@ -16,7 +16,7 @@ import torch
 
 from .. import _native as nat
 from .. import optimizers
-from ..learner import NativeLearner, flat_to_state_dict, flatdim, hidden_width, init_flat_params, init_flat_rnn_params, mlp_shapes, rnn_shapes, \
+from ..learner import MAX_AGENTS, NativeLearner, flat_to_state_dict, flatdim, hidden_width, init_flat_params, init_flat_rnn_params, mlp_shapes, rnn_shapes, \
     sharing_to_nets, state_dict_to_flat
 from ..native_env import TrajStore
 
@@ -38,7 +38,7 @@ class QNetwork(NativeLearner):
         self.target_update_interval_or_tau = float(cfg.target_update_interval_or_tau)
         self.max_batch = int(max_batch or getattr(cfg, "batch_size", 1024))
         self.max_T = int(max_episode_length or getattr(cfg, "max_episode_length", 0) or 500)
-        mcfg = nat.MlpCfg(self.n_agents, self.n_nets, (C.c_int32 * 32)(*self.agent_net), self.in_dim, self.hidden, self.n_actions)
+        mcfg = nat.MlpCfg(self.n_agents, self.n_nets, (C.c_int32 * MAX_AGENTS)(*self.agent_net), self.in_dim, self.hidden, self.n_actions)
         hp = nat.DqnHP(float(cfg.lr), self.gamma, float(self.grad_clip or 0.0), int(self.double_q), self.target_update_interval_or_tau,
                        0.9, 0.999, 1e-8, self.mixer)
         self._h = C.c_void_p()

@@ -14,6 +14,7 @@ from . import _native as nat
 from . import optimizers
 
 HIDDEN = 128       # the shipped network's width (layers = [128, 128]) and the widest the kernels take
+MAX_AGENTS = nat.MAX_AGENTS   # 32 = MARL_MAX_AGENTS: the most agents (and networks) a learner takes
 
 
 def hidden_width(layers, what="layers", use_rnn=False) -> int:
@@ -112,12 +113,15 @@ class NativeLearner:
     _destroy = None
 
     def _open(self, obs_space, action_space, cfg, device):
-        """The constructors' shared prologue: optimiser name, device (the GPU learners have no CPU fallback), agents and their space sizes."""
+        """The constructors' shared prologue: optimiser name, device (the GPU learners have no CPU fallback), agents and their space sizes.
+        More than MAX_AGENTS agents fail here, before any native call (marl_dqn_create / marl_a2c_create refuse them too)."""
+        self.n_agents = len(obs_space)
+        if self.n_agents > MAX_AGENTS:
+            raise NotImplementedError(f"{self.n_agents} agents: the learners take at most {MAX_AGENTS} agents (MARL_MAX_AGENTS)")
         self.optimizer_name = optimizers.optimizer_name(getattr(cfg, "optimizer", "Adam"))
         if not torch.cuda.is_available() or not str(device).startswith("cuda"):
             raise nat.NativeError("the GPU learners need algorithm.model.device=cuda (no CPU fallback)")
         self.device = torch.device(device if ":" in str(device) else f"cuda:{torch.cuda.current_device()}")
-        self.n_agents = len(obs_space)
         obs_dims, act_dims = [flatdim(o) for o in obs_space], [flatdim(a) for a in action_space]
         if len(set(obs_dims)) != 1 or len(set(act_dims)) != 1:
             raise NotImplementedError("agents with different observation / action sizes are not implemented")
