@@ -137,12 +137,18 @@ struct EnvHandle : BufferOwner {
 };
 
 // The attribute is a per-function, process-wide setting: only ever raise it (a second env with a smaller tile must not lower the limit of the
-// first).  `limit` is the kernel's current limit, kept by the caller.
+// first).  `limit` is the kernel's current limit, kept by the caller.  A refused size is reported through set_error only: nothing is left
+// in the runtime's last error for a later, unrelated cudaGetLastError (another launch's check, torch's) to report.  Defensive: no config
+// reaches the refusal today (marl_lbf_create checks its tile against the opt-in limit first, and RWARE's widest tile is about 207 KB).
 template <typename K>
 int raise_smem_limit(K* kernel, size_t bytes, size_t& limit, const char* who) {
   if (bytes <= limit) return MARL_OK;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  if (e != cudaSuccess) { set_error("%s: %zu B of shared memory per CTA not available: %s", who, bytes, cudaGetErrorString(e)); return MARL_EINVAL; }
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();
+    set_error("%s: %zu B of shared memory per CTA not available: %s", who, bytes, cudaGetErrorString(e));
+    return MARL_EINVAL;
+  }
   limit = bytes;
   return MARL_OK;
 }

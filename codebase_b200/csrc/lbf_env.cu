@@ -37,6 +37,7 @@ struct LbfStateDev {
 
 constexpr int kThreads = 128;
 constexpr int kMaxFood = 32;
+constexpr int kMaxVecObs = 3 * kMaxFood + 4 * MARL_MAX_AGENTS;   // the widest vector observation validate_cfg admits: foods, players, ObserveID's one-hot
 constexpr int kMaxGridSight = 127;   // the largest field side: a wider window only adds padding (and keeps N*D*E-per-CTA in int range)
 
 __device__ __forceinline__ int imin(int a, int b) { return a < b ? a : b; }
@@ -205,7 +206,7 @@ __global__ void lbf_reset_kernel(LbfCfgDev c, LbfStateDev s, int E, uint64_t see
   if (obs_out == nullptr && !(traj.enabled && doit)) return;
   uint32_t foods[kMaxFood];
   const int nf = list_foods(c, f, foods, kMaxFood);
-  float o[3 * (kMaxFood + MARL_MAX_AGENTS)];
+  float o[kMaxVecObs];
   for (int i = 0; i < c.N; ++i) {
     build_obs(c, foods, nf, pl, i, o);
     if (obs_out) for (int d = 0; d < c.D; ++d) obs_out[((size_t)e * c.N + i) * c.D + d] = o[d];
@@ -552,6 +553,8 @@ static int validate_cfg(const marl_lbf_cfg* c) {
   if (c->grid_observation) {
     MARL_REQUIRE(!c->observe_id, "marl_lbf: grid observations cannot be combined with observe_id (ObserveID assumes a flattened observation space)");
     MARL_REQUIRE(c->sight <= kMaxGridSight, "marl_lbf: sight %d out of range for grid observations (1..%d)", c->sight, kMaxGridSight);
+  } else {   // lbf_reset_kernel builds each observation in a float[kMaxVecObs]
+    MARL_REQUIRE(marl_lbf_obs_dim(c) <= kMaxVecObs, "marl_lbf: vector observation width %d out of range (1..%d)", marl_lbf_obs_dim(c), kMaxVecObs);
   }
   return MARL_OK;
 }
@@ -594,14 +597,19 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
   MARL_REQUIRE(n_envs >= 1, "marl_lbf_create: n_envs must be >= 1");
   if (int rc = check_device(device)) return rc;
   const bool grid = cfg->grid_observation != 0;
-  if (grid) {   // every env of a CTA needs its field tile and its agent map: name the limit rather than fail in cudaFuncSetAttribute
+  {   // every env of a CTA needs its tiles in shared memory: name the limit rather than fail in cudaFuncSetAttribute
     const LbfCfgDev d = to_dev(*cfg);
-    const size_t need = step_smem_bytes(d, true);
+    const size_t need = step_smem_bytes(d, grid);
+    const int epc = (kThreads / 32) * (32 / d.G);
     int optin = 0;
     MARL_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
-    MARL_REQUIRE(need <= (size_t)optin, "marl_lbf_create: grid observations of a %dx%d field with %d agents need %zu B of shared memory per CTA "
-                 "(%d envs x 2 tiles of %d B); the device allows %d B", cfg->rows, cfg->cols, cfg->n_agents, need,
-                 (kThreads / 32) * (32 / d.G), d.pitch + 4, optin);
+    if (grid)
+      MARL_REQUIRE(need <= (size_t)optin, "marl_lbf_create: grid observations of a %dx%d field with %d agents need %zu B of shared memory per CTA "
+                   "(%d envs x 2 tiles of %d B); the device allows %d B", cfg->rows, cfg->cols, cfg->n_agents, need, epc, d.pitch + 4, optin);
+    else
+      MARL_REQUIRE(need <= (size_t)optin, "marl_lbf_create: vector observations of a %dx%d field with %d agents need %zu B of shared memory per CTA "
+                   "(%d envs x a %d B field tile and %d observations of %d floats); the device allows %d B", cfg->rows, cfg->cols, cfg->n_agents,
+                   need, epc, d.pitch + 4, d.N, d.D, optin);
   }
   marl_lbf* h = new marl_lbf();
   h->cfg = *cfg; h->dev = to_dev(*cfg); h->E = n_envs; h->device = device; h->seed = seed; h->gid0 = env_gid0;

@@ -117,7 +117,8 @@ def test_fused_eps_greedy_rollout_and_replay_writes(cfgkw, proper):
     env = _native(cfgkw, E, seed, gid0)
     orc = lbf_c.OracleVecEnv(lbf_c.make_cfg(**cfgkw), E, seed, gid0)
     N, D, A = orc.N, orc.D, 6
-    cap, slot0 = E + 37, 30  # wraps around the ring
+    cap, slot0 = E + 37, 300
+    assert slot0 + E > cap  # the last envs' slots wrap to the front of the ring
     traj = TrajStore(cap, N, T, D, env.device)
     ref = dict(obs=np.zeros((cap, N, T + 1, D), np.float32), act=np.zeros((cap, N, T), np.int32), rew=np.zeros((cap, N, T), np.float32),
                done=np.zeros((cap, T + 1), np.uint8), filled=np.zeros((cap, T), np.uint8))
