@@ -39,7 +39,7 @@ __global__ void nstep_returns_kernel(NStepParams p) {
     float src;
     if (k == p.n_steps) {
       src = p.vt[((size_t)a * p.P + b) * (T + 1) + tt];
-      if (p.ret_ms) src = __fadd_rn(__fmul_rn(src, sqrtf(p.ret_ms[p.N + a])), p.ret_ms[a]);   // next_value * sqrt(var) + mean
+      if (p.ret_ms) src = unstandardise(src, p.ret_ms[a], p.ret_ms[p.N + a]);
     } else {
       src = p.traj.rew[(ep * p.N + a) * T + tt];
     }

@@ -4,6 +4,7 @@
 // update (zero_grad/backward/clip/Adam), update_target/hard_update/soft_update -- and ReplayBuffer.sample's index
 // draw + gather (marlbase/dqn/train.py:94-124).
 #include "learner.cuh"
+#include "dqn_heads.cuh"
 #include "retms.cuh"
 #include "qmix.cuh"
 #include "gru.cuh"
@@ -24,113 +25,65 @@ __global__ void replay_sample_kernel(uint64_t seed, uint64_t update_idx, int bat
   idx[i] = (int32_t)bounded(pick(b, i & 3), (uint32_t)n_valid);
 }
 
-// ---- VDN: agent-coupled TD error (marlbase/dqn/model.py:224-269) ------------------------------------------------
-// C columns of G agents each: column c sums the Q-values of agents [c G, c G + G) and takes agent c G's reward.  VDN: C = 1, G = N;
-// independent learners (the recurrent pass, whose backward has no TD head of its own): C = N, G = 1.
-struct VdnTdParams {
+// ---- TD error over C columns of G agents (marlbase/dqn/model.py:138-163, VDN 224-269) -----------------------------
+// Column c sums the Q-values and bootstrap values of agents [c G, c G + G) and takes agent c G's reward.  VDN: C = 1, G = N; independent learners
+// (the recurrent pass, whose backward has no TD head of its own; standardise_returns): C = N, G = 1.  One thread per (c, b, t).
+//   STAGE 0: td[c][b][t] = 2 delta filled and the loss statistics.
+//   STAGE 1 (standardise_returns, dqn/model.py:147-158, VDN 256-264: the TD target needs statistics of the whole batch's returns before any loss):
+//            ret = r + gamma (next * sqrt(var) + mean) (1 - done[t + 1]) and chosen = Q(o_t)[a_t], for every (b, t), filled or not, as the
+//            reference.  Columns of the statistics: one per agent (IDQN); the reference's VDN reshapes its (E, B) returns with reshape(-1, B), i.e.
+//            one column per batch entry -- stat_per_b selects that.  ret_ms_step (retms.cuh) then absorbs and standardises ret in place.
+//   STAGE 2: td from chosen and the standardised returns, and the loss statistics.
+struct ColTdParams {
   const float* q; const float* tq;  // [N][B][T+1][A]
   TrajView traj; const int32_t* idx; int B, N, A; float gamma; int double_q;
   int C, G;
+  const float* ret_ms; int n_stat, stat_per_b;   // STAGE 1: mean[n_stat] | var[n_stat]
+  float* ret; float* chosen;                     // STAGES 1, 2: [C][B][T]
   float* td;         // [C][B][T] = 2 * delta * filled
   float* loss_part;  // [gridDim][4]
 };
 
-__global__ void __launch_bounds__(256) vdn_td_kernel(VdnTdParams p) {
+// loss_part[block] = (sum of loss, sum of fill, 0, 0) over the block's 256 threads, in a fixed tree order
+__device__ __forceinline__ void block_loss_part(float loss, float fill, float* loss_part) {
   __shared__ float red[512];
+  red[threadIdx.x] = loss; red[256 + threadIdx.x] = fill;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) { red[threadIdx.x] += red[threadIdx.x + s]; red[256 + threadIdx.x] += red[256 + threadIdx.x + s]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) { loss_part[4 * blockIdx.x] = red[0]; loss_part[4 * blockIdx.x + 1] = red[256]; loss_part[4 * blockIdx.x + 2] = 0.f; loss_part[4 * blockIdx.x + 3] = 0.f; }
+}
+
+template <int STAGE>
+__global__ void __launch_bounds__(256) col_td_kernel(ColTdParams p) {
   const int T = p.traj.T, i = blockIdx.x * 256 + threadIdx.x;
   float loss = 0.f, fill = 0.f;
   if (i < p.C * p.B * T) {
     const int c = i / (p.B * T), rem = i - c * p.B * T, b = rem / T, t = rem - b * T;
     const size_t ep = (size_t)p.idx[b];
-    float chosen = 0.f, tsum = 0.f;
-    for (int a = c * p.G; a < (c + 1) * p.G; ++a) {
-      const size_t row = ((size_t)a * p.B + b) * (T + 1) + t;
-      const float* q0 = p.q + row * p.A; const float* q1 = q0 + p.A; const float* t1 = p.tq + (row + 1) * p.A;
-      chosen += q0[p.traj.act[(ep * p.N + a) * T + t]];
-      if (p.double_q) {
-        int best = 0; float bv = q1[0];
-        for (int o = 1; o < p.A; ++o) if (q1[o] > bv) { bv = q1[o]; best = o; }
-        tsum += t1[best];
+    if constexpr (STAGE == 2) {
+      p.td[i] = td_error(p.chosen[i], p.ret[i], (float)p.traj.filled[ep * T + t], c == 0, loss, fill);
+    } else {
+      float chosen = 0.f, next = 0.f;
+      for (int a = c * p.G; a < (c + 1) * p.G; ++a) {
+        const size_t row = ((size_t)a * p.B + b) * (T + 1) + t;
+        const float* q0 = p.q + row * p.A;
+        chosen += q0[p.traj.act[(ep * p.N + a) * T + t]];
+        next += next_value(q0 + p.A, p.tq + (row + 1) * p.A, p.A, p.double_q);
+      }
+      const float rew = p.traj.rew[(ep * p.N + c * p.G) * T + t], done1 = (float)p.traj.done[ep * (T + 1) + t + 1];
+      if constexpr (STAGE == 0) {
+        p.td[i] = td_error(chosen, td_target(rew, p.gamma, next, done1), (float)p.traj.filled[ep * T + t], c == 0, loss, fill);
       } else {
-        float m = t1[0];
-        for (int o = 1; o < p.A; ++o) m = fmaxf(m, t1[o]);
-        tsum += m;
+        const int col = p.stat_per_b ? b : c;
+        p.ret[i] = td_target_rn(rew, p.gamma, unstandardise(next, p.ret_ms[col], p.ret_ms[p.n_stat + col]), done1);
+        p.chosen[i] = chosen;
       }
     }
-    const float filled = (float)p.traj.filled[ep * T + t];
-    const float y = p.traj.rew[(ep * p.N + c * p.G) * T + t] + p.gamma * tsum * (1.f - (float)p.traj.done[ep * (T + 1) + t + 1]);
-    const float delta = chosen - y;
-    loss = delta * delta * filled; fill = c == 0 ? filled : 0.f;
-    p.td[i] = 2.f * delta * filled;
   }
-  red[threadIdx.x] = loss; red[256 + threadIdx.x] = fill;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) { red[threadIdx.x] += red[threadIdx.x + s]; red[256 + threadIdx.x] += red[256 + threadIdx.x + s]; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) { p.loss_part[4 * blockIdx.x] = red[0]; p.loss_part[4 * blockIdx.x + 1] = red[256]; p.loss_part[4 * blockIdx.x + 2] = 0.f; p.loss_part[4 * blockIdx.x + 3] = 0.f; }
-}
-
-// ---- cfg.standardise_returns (dqn/model.py:147-158, VDN 256-264): the TD target needs statistics of the whole batch's returns before any loss ----
-// 1. returns[c][b][t] = r + gamma * (target_qs * sqrt(var) + mean) * (1 - done[t + 1]) and chosen[c][b][t] = Q(o_t)[a_t] (VDN: both summed over the
-//    agents, c = 0); every (b, t), filled or not, as the reference.  Columns of the statistics: one per agent (IDQN); the reference's VDN reshapes
-//    its (E, B) returns with reshape(-1, B), i.e. one column per batch entry -- stat_per_b selects that.
-// 2. RunningMeanStd step (retms.cuh): statistics absorb the returns, returns are standardised in place.
-// 3. td[c][b][t] = 2 (chosen - returns) filled  +  the loss statistics.
-struct StdRetParams {
-  const float* q; const float* tq;  // [N][B][T+1][A]
-  TrajView traj; const int32_t* idx; int B, N, A, vdn; float gamma; int double_q;
-  const float* ret_ms; int n_stat, stat_per_b;   // mean[n_stat] | var[n_stat]
-  float* ret; float* chosen; float* td;          // [C][B][T], C = vdn ? 1 : N
-  float* loss_part;
-};
-__global__ void __launch_bounds__(256) std_returns_kernel(StdRetParams p) {
-  const int T = p.traj.T, C = p.vdn ? 1 : p.N, i = blockIdx.x * 256 + threadIdx.x;
-  if (i >= C * p.B * T) return;
-  const int c = i / (p.B * T), rem = i - c * p.B * T, b = rem / T, t = rem - b * T;
-  const size_t ep = (size_t)p.idx[b];
-  float chosen = 0.f, tsel = 0.f;
-  for (int a = (p.vdn ? 0 : c); a < (p.vdn ? p.N : c + 1); ++a) {
-    const size_t row = ((size_t)a * p.B + b) * (T + 1) + t;
-    const float* q0 = p.q + row * p.A; const float* q1 = q0 + p.A; const float* t1 = p.tq + (row + 1) * p.A;
-    chosen += q0[p.traj.act[(ep * p.N + a) * T + t]];
-    if (p.double_q) {
-      int best = 0; float bv = q1[0];
-      for (int o = 1; o < p.A; ++o) if (q1[o] > bv) { bv = q1[o]; best = o; }
-      tsel += t1[best];
-    } else {
-      float m = t1[0];
-      for (int o = 1; o < p.A; ++o) m = fmaxf(m, t1[o]);
-      tsel += m;
-    }
-  }
-  const int col = p.stat_per_b ? b : c;
-  tsel = __fadd_rn(__fmul_rn(tsel, sqrtf(p.ret_ms[p.n_stat + col])), p.ret_ms[col]);     // target_qs * sqrt(var) + mean
-  const float rew = p.traj.rew[(ep * p.N + (p.vdn ? 0 : c)) * T + t];
-  const float y = __fadd_rn(rew, __fmul_rn(__fmul_rn(p.gamma, tsel), 1.f - (float)p.traj.done[ep * (T + 1) + t + 1]));
-  // the statistics' columns must be contiguous: [col][...]
-  const size_t o = p.stat_per_b ? ((size_t)b * T + t) : (size_t)i;
-  p.ret[o] = y; p.chosen[o] = chosen;
-}
-__global__ void __launch_bounds__(256) std_td_kernel(StdRetParams p) {
-  __shared__ float red[512];
-  const int T = p.traj.T, C = p.vdn ? 1 : p.N, i = blockIdx.x * 256 + threadIdx.x;
-  float loss = 0.f, fill = 0.f;
-  if (i < C * p.B * T) {
-    const int c = i / (p.B * T), rem = i - c * p.B * T, b = rem / T, t = rem - b * T;
-    const float filled = (float)p.traj.filled[(size_t)p.idx[b] * T + t];
-    const float delta = p.chosen[i] - p.ret[i];
-    loss = delta * delta * filled; fill = c == 0 ? filled : 0.f;
-    p.td[i] = 2.f * delta * filled;
-  }
-  red[threadIdx.x] = loss; red[256 + threadIdx.x] = fill;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) { red[threadIdx.x] += red[threadIdx.x + s]; red[256 + threadIdx.x] += red[256 + threadIdx.x + s]; }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) { p.loss_part[4 * blockIdx.x] = red[0]; p.loss_part[4 * blockIdx.x + 1] = red[256]; p.loss_part[4 * blockIdx.x + 2] = 0.f; p.loss_part[4 * blockIdx.x + 3] = 0.f; }
+  if constexpr (STAGE != 1) block_loss_part(loss, fill, p.loss_part);
 }
 
 }  // namespace marl
@@ -400,23 +353,34 @@ int marl_dqn_sync_target(marl_dqn* h, void* stream) {
   return MARL_OK;
 }
 
-int marl_dqn_forward(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_target, float* q_out, void* stream) {
-  MARL_REQUIRE(h && obs && q_out && n_envs >= 1, "marl_dqn_forward: bad argument");
-  MARL_REQUIRE(!h->rnn, "marl_dqn_forward: the learner has recurrent agent networks: use marl_dqn_forward_rnn, which carries the hidden state");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  const RowPlan plan = make_plan(h->ns, n_envs, 1, h->n_sm, 32);
-  const RowSource src = dense_rows(obs, n_envs, h->ns.n_agents, h->ns.in);
-  bool& current = use_target ? h->tgt_image_current : h->image_current;
-  const int rc = forward_any(h->ns, plan, src, use_target ? h->theta_tgt : h->theta, use_target ? h->image_tgt : h->image, q_out, (cudaStream_t)stream, current);
-  if (rc == MARL_OK) current = tc_forward_enabled() != 0;
-  return rc;
-}
-
 static GruFwdParams gru_fwd_params(const marl_dqn* h, const RowSource& src, int units, int steps, bool target) {
   GruFwdParams fp; memset(&fp, 0, sizeof(fp));
   fp.plan = make_plan(h->ns, units, steps, 1, 1); fp.src = src;
   fp.theta = target ? h->theta_tgt : h->theta; fp.lay = h->gl;
   return fp;
+}
+
+// The online or target agent networks on the rows of src -> q_out: the GRU forward (training rows: whole episodes of the plan's units; save:
+// what the backward needs, NULL: nothing), else the tensor-core or the FP32 forward (forward_any), after which the packed image of the weights
+// it read is current exactly when the tensor-core forward is on.
+static int dqn_forward(marl_dqn* h, const RowPlan& plan, const RowSource& src, bool target, float* q_out, float* save, cudaStream_t st) {
+  if (h->rnn) {
+    GruFwdParams fp = gru_fwd_params(h, src, plan.units_per_agent, src.traj.T + 1, target);
+    fp.q_out = q_out; fp.save = save;
+    return launch_gru_forward(fp, st);
+  }
+  bool& current = target ? h->tgt_image_current : h->image_current;
+  if (int rc = forward_any(h->ns, plan, src, target ? h->theta_tgt : h->theta, target ? h->image_tgt : h->image, q_out, st, current)) return rc;
+  current = tc_forward_enabled() != 0;
+  return MARL_OK;
+}
+
+int marl_dqn_forward(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_target, float* q_out, void* stream) {
+  MARL_REQUIRE(h && obs && q_out && n_envs >= 1, "marl_dqn_forward: bad argument");
+  MARL_REQUIRE(!h->rnn, "marl_dqn_forward: the learner has recurrent agent networks: use marl_dqn_forward_rnn, which carries the hidden state");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  const RowPlan plan = make_plan(h->ns, n_envs, 1, h->n_sm, 32);
+  return dqn_forward(h, plan, dense_rows(obs, n_envs, h->ns.n_agents, h->ns.in), use_target != 0, q_out, nullptr, (cudaStream_t)stream);
 }
 
 int marl_dqn_forward_rnn(marl_dqn* h, const float* obs, int32_t n_envs, int32_t use_target, const float* h_in, float* h_out, float* q_out, void* stream) {
@@ -435,55 +399,20 @@ int marl_replay_sample(uint64_t seed, uint64_t update_idx, int32_t batch, int32_
   return MARL_OK;
 }
 
-// Gradient half of an update.  rp_out == NULL: the per-CTA partials are reduced into grad[] (grad_reduce_kernel); otherwise the
-// reduction is left to the caller (fused reduce + Adam tail) and its parameters are returned.
-static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* episode_idx, int32_t batch, void* stream, ReduceParams* rp_out) {
-  MARL_REQUIRE(h && traj && episode_idx, "marl_dqn_update_grads: NULL argument");
-  MARL_REQUIRE(batch >= 1 && batch <= h->max_batch, "marl_dqn_update_grads: batch %d exceeds max_batch %d", batch, h->max_batch);
-  MARL_REQUIRE(traj->T >= 1 && traj->T <= h->max_T, "marl_dqn_update_grads: T %d exceeds max_T %d", traj->T, h->max_T);
-  MARL_REQUIRE(traj->n_agents == h->ns.n_agents && traj->obs_dim == h->ns.in, "marl_dqn_update_grads: trajectory shape mismatch");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int T = traj->T;
-  const RowPlan plan = h->rnn ? make_plan(h->ns, batch, 1, h->n_sm, kGruSeqs) : episode_plan(h->ns, batch, T, h->n_sm);
-  const RowSource src = episode_rows(traj, episode_idx, h->ns.n_agents, h->ns.in);
-  const bool rec = h->timing && h->ev_used < kTimingPairs;
-  // target network on every gathered row (dqn/model.py:132-134); several ranks: the previous update launched it between its push and its finish
-  if (h->tq_ahead) {
-    h->tq_ahead = false;
-  } else if (h->rnn) {
-    GruFwdParams fp = gru_fwd_params(h, src, batch, T + 1, true);
-    fp.q_out = h->tq;
-    if (int rc = launch_gru_forward(fp, st)) return rc;
-  } else {
-    if (int rc = forward_any(h->ns, plan, src, h->theta_tgt, h->image_tgt, h->tq, st, h->tgt_image_current)) return rc;
-    h->tgt_image_current = tc_forward_enabled() != 0;
-  }
-  // online Q-values of every row for the external TD heads; the recurrent pass also saves what its backward needs
-  auto online_forward = [&]() -> int {
-    if (h->rnn) {
-      if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
-      GruFwdParams fp = gru_fwd_params(h, src, batch, T + 1, false);
-      fp.q_out = h->q_all; fp.save = h->gru_save;
-      return launch_gru_forward(fp, st);
-    }
-    if (int rc = forward_any(h->ns, plan, src, h->theta, h->image, h->q_all, st, h->image_current)) return rc;
-    h->image_current = tc_forward_enabled() != 0;
-    return MARL_OK;
-  };
-  int n_loss_parts = h->rnn ? 0 : plan.cta_begin[plan.n_nets];
-  const float* td_ext = nullptr;
-  float* loss_part = h->loss_part;
-  int td_agent_stride = 0;
+// The external TD head, for the cases the training pass's own head does not cover (QMIX, standardise_returns, VDN, the recurrent pass): the online
+// forward on every row, then dL/dQ of the taken actions into td, which becomes tp.td_ext (per agent at tp.td_agent_stride; VDN: per (b, t), stride 0),
+// and the head's loss statistics into loss_part blocks [n_loss_parts, ...), which n_loss_parts is advanced past.
+static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, int batch, TrainParams& tp, int& n_loss_parts, cudaStream_t st) {
+  if (h->hp.mixer == 0 && !h->rnn && !h->standardise) return MARL_OK;
+  if (int rc = dqn_forward(h, plan, src, false, h->q_all, h->gru_save, st)) return rc;
+  const int T = src.traj.T;
+  float* loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
+  tp.td_ext = h->td;
   if (h->hp.mixer == 2) {  // QMIX: the mixer turns the agents' Q-values into the TD error and hands dL/dq_a back per agent (qmix.cuh)
-    MARL_REQUIRE(h->mix != nullptr, "marl_dqn_update: QMIX needs marl_dqn_qmix_init first");
-    MARL_REQUIRE(!h->standardise || batch == h->n_stat, "marl_dqn_update: QMIX's standardise_returns keeps one statistic per batch entry (the reference's "
-                 "reshape(-1, B)): batch %d must stay at max_batch %d", batch, h->n_stat);
-    if (int rc = online_forward()) return rc;
     QmixParams qp; memset(&qp, 0, sizeof(qp));
-    qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = episode_idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
+    qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = src.idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
     qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
-    qp.loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
+    qp.loss_part = loss_part;
     const int Sn = batch * T, qb = (Sn + kQmTS - 1) / kQmTS, n = h->ql.n, hl = h->ql.hl;
     qmix_pack_kernel<<<dim3((n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
     if (h->standardise) {   // target pass -> returns, RunningMeanStd step (one column per batch entry), online pass on the standardised returns
@@ -506,73 +435,89 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
     qmix_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(h->mix_part, chunks, n, h->mix_grad, qp.loss_part, qb);
     MARL_CUDA_TRY(cudaGetLastError());
     n_loss_parts += qb;
-    td_ext = h->td;
-    td_agent_stride = batch * T;
-  } else if (h->standardise) {
-    // online Q-values of every row, returns + chosen Q, RunningMeanStd step, TD error (dqn/model.py:147-158 / 256-264)
-    MARL_REQUIRE(h->hp.mixer == 0 || batch == h->n_stat, "marl_dqn_update: VDN's standardise_returns keeps one statistic per batch entry (the reference's reshape(-1, B)): "
-                 "batch %d must stay at max_batch %d", batch, h->n_stat);
-    if (int rc = online_forward()) return rc;
-    const int C = h->hp.mixer == 1 ? 1 : h->ns.n_agents;
-    StdRetParams sp; memset(&sp, 0, sizeof(sp));
-    sp.q = h->q_all; sp.tq = h->tq; sp.traj = src.traj; sp.idx = episode_idx; sp.B = batch; sp.N = h->ns.n_agents; sp.A = h->ns.out; sp.vdn = h->hp.mixer == 1;
-    sp.gamma = h->hp.gamma; sp.double_q = h->hp.double_q; sp.ret_ms = h->ret_ms; sp.n_stat = h->n_stat; sp.stat_per_b = h->hp.mixer == 1;
-    sp.ret = h->ret; sp.chosen = h->chosen; sp.td = h->td;
-    const int vb = (C * batch * T + 255) / 256;
-    sp.loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
-    std_returns_kernel<<<vb, 256, 0, st>>>(sp);
+    tp.td_agent_stride = batch * T;
+    return MARL_OK;
+  }
+  // VDN: one column of all agents; independent learners: one column per agent
+  const bool vdn = h->hp.mixer == 1;
+  ColTdParams cp; memset(&cp, 0, sizeof(cp));
+  cp.q = h->q_all; cp.tq = h->tq; cp.traj = src.traj; cp.idx = src.idx; cp.B = batch; cp.N = h->ns.n_agents; cp.A = h->ns.out;
+  cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.C = vdn ? 1 : h->ns.n_agents; cp.G = vdn ? h->ns.n_agents : 1;
+  cp.td = h->td; cp.loss_part = loss_part;
+  const int blocks = (cp.C * batch * T + 255) / 256;
+  if (h->standardise) {   // returns + chosen Q, RunningMeanStd step, TD error on the standardised returns
+    cp.ret_ms = h->ret_ms; cp.n_stat = h->n_stat; cp.stat_per_b = vdn; cp.ret = h->ret; cp.chosen = h->chosen;
+    col_td_kernel<1><<<blocks, 256, 0, st>>>(cp);
     RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T;
-    if (h->hp.mixer == 1) { rp.N = batch; rp.P = 1; } else { rp.N = C; rp.P = batch; }
+    if (vdn) { rp.N = batch; rp.P = 1; } else { rp.N = cp.C; rp.P = batch; }
     MARL_CUDA_TRY(ret_ms_step(rp, st));
-    std_td_kernel<<<vb, 256, 0, st>>>(sp);
-    MARL_CUDA_TRY(cudaGetLastError());
-    n_loss_parts += vb;
-    td_ext = h->td;
-    td_agent_stride = h->hp.mixer == 1 ? 0 : batch * T;
-  } else if (h->hp.mixer == 1 || (h->rnn && h->hp.mixer == 0)) {
-    // VDN: online Q-values of all agents first, then the agent-summed TD error; recurrent independent learners: one column per agent
-    if (int rc = online_forward()) return rc;
-    const bool vdn = h->hp.mixer == 1;
-    VdnTdParams vp; vp.q = h->q_all; vp.tq = h->tq; vp.traj = src.traj; vp.idx = episode_idx; vp.B = batch; vp.N = h->ns.n_agents; vp.A = h->ns.out;
-    vp.gamma = h->hp.gamma; vp.double_q = h->hp.double_q; vp.td = h->td;
-    vp.C = vdn ? 1 : h->ns.n_agents; vp.G = vdn ? h->ns.n_agents : 1;
-    const int vb = (vp.C * batch * T + 255) / 256;
-    vp.loss_part = h->loss_part + 4 * (size_t)n_loss_parts;  // the train kernel's parts read as zero in this mode
-    vdn_td_kernel<<<vb, 256, 0, st>>>(vp);
-    MARL_CUDA_TRY(cudaGetLastError());
-    n_loss_parts += vb;
-    td_ext = h->td;
-    td_agent_stride = vdn ? 0 : batch * T;
-  }
-  TrainParams tp; memset(&tp, 0, sizeof(tp));
-  tp.plan = plan; tp.src = src; tp.theta = h->theta; tp.lay = h->ns.lay; tp.tq = h->tq; tp.td_ext = td_ext; tp.td_agent_stride = td_agent_stride;
-  tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = loss_part;
-  if (h->rnn) {   // BPTT from td_ext; the timed window opened before the online forward
-    GruBwdParams bp; memset(&bp, 0, sizeof(bp));
-    bp.plan = plan; bp.traj = src.traj; bp.idx = episode_idx; bp.B = batch; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
-    bp.td = td_ext; bp.td_agent_stride = td_agent_stride; bp.src = src; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
-    if (int rc = launch_gru_backward(bp, st)) return rc;
-  } else if (tc_backward_enabled() && h->ns.in < kMaxObsDim && h->image != nullptr) {   // (no image: hidden width below 128)
-    if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
-    if (!h->tc_h1) {  // intermediates of the tensor-core pipeline, allocated on first use
-      const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), F = sizeof(float);
-      if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h1, rows * kHidden * F}, {&h->tc_h2, rows * kHidden * F}, {&h->tc_dh1, rows * kHidden * F},
-                                                        {&h->tc_rec, rows * 32 /* kRowRec */ * F}, {&h->tc_x, rows * kMaxObsDim * F},
-                                                        {&h->image_bwd, ((size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4) * F}}))
-        return rc;
-    }
-    if (!h->image_current || !h->bwd_image_current) {
-      if (int rc = launch_pack_weights(h->theta, h->ns.lay, h->ns.n_nets, h->image, st, h->image_bwd)) return rc;
-      h->image_current = h->bwd_image_current = true;
-    }
-    TcBuffers tb; tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h1 = h->tc_h1; tb.h2 = h->tc_h2; tb.dh1 = h->tc_dh1; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
-    if (int rc = launch_tc_dqn_train(tp, tb, st, rec ? &h->ev[4 * h->ev_used + 1] : nullptr)) return rc;
-    if (rec) h->ev_split = true;
+    col_td_kernel<2><<<blocks, 256, 0, st>>>(cp);
   } else {
-    if (rec) cudaEventRecord(h->ev[4 * h->ev_used], st);
-    if (int rc = launch_train(tp, kHeadDqn, st)) return rc;
+    col_td_kernel<0><<<blocks, 256, 0, st>>>(cp);
   }
-  if (rec) { cudaEventRecord(h->ev[4 * h->ev_used + 3], st); h->ev_used += 1; }
+  MARL_CUDA_TRY(cudaGetLastError());
+  n_loss_parts += blocks;
+  tp.td_agent_stride = vdn ? 0 : batch * T;
+  return MARL_OK;
+}
+
+// The training pass from tp.td_ext, or from the agents' own TD head: GRU BPTT, the tensor-core pipeline (between: two timing events recorded
+// between its kernels, NULL: none; tc is set when it runs) or the fused FP32 kernel.
+static int dqn_train_pass(marl_dqn* h, const TrainParams& tp, cudaEvent_t* between, bool& tc, cudaStream_t st) {
+  tc = false;
+  if (h->rnn) {
+    GruBwdParams bp; memset(&bp, 0, sizeof(bp));
+    bp.plan = tp.plan; bp.traj = tp.src.traj; bp.idx = tp.src.idx; bp.B = tp.plan.units_per_agent; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
+    bp.td = tp.td_ext; bp.td_agent_stride = tp.td_agent_stride; bp.src = tp.src; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
+    return launch_gru_backward(bp, st);
+  }
+  if (!tc_backward_enabled() || h->ns.in >= kMaxObsDim || h->image == nullptr) return launch_train(tp, kHeadDqn, st);   // (no image: hidden width below 128)
+  if (!h->tc_h1) {  // intermediates of the tensor-core pipeline, allocated on first use
+    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), F = sizeof(float);
+    if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h1, rows * kHidden * F}, {&h->tc_h2, rows * kHidden * F}, {&h->tc_dh1, rows * kHidden * F},
+                                                      {&h->tc_rec, rows * 32 /* kRowRec */ * F}, {&h->tc_x, rows * kMaxObsDim * F},
+                                                      {&h->image_bwd, ((size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4) * F}}))
+      return rc;
+  }
+  if (!h->image_current || !h->bwd_image_current) {
+    if (int rc = launch_pack_weights(h->theta, h->ns.lay, h->ns.n_nets, h->image, st, h->image_bwd)) return rc;
+    h->image_current = h->bwd_image_current = true;
+  }
+  TcBuffers tb; tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h1 = h->tc_h1; tb.h2 = h->tc_h2; tb.dh1 = h->tc_dh1; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
+  tc = true;
+  return launch_tc_dqn_train(tp, tb, st, between);
+}
+
+// Gradient half of an update.  rp_out == NULL: the per-CTA partials are reduced into grad[] (grad_reduce_kernel); otherwise the
+// reduction is left to the caller (fused reduce + Adam tail) and its parameters are returned.
+static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* episode_idx, int32_t batch, void* stream, ReduceParams* rp_out) {
+  MARL_REQUIRE(h && traj && episode_idx, "marl_dqn_update_grads: NULL argument");
+  MARL_REQUIRE(batch >= 1 && batch <= h->max_batch, "marl_dqn_update_grads: batch %d exceeds max_batch %d", batch, h->max_batch);
+  MARL_REQUIRE(traj->T >= 1 && traj->T <= h->max_T, "marl_dqn_update_grads: T %d exceeds max_T %d", traj->T, h->max_T);
+  MARL_REQUIRE(traj->n_agents == h->ns.n_agents && traj->obs_dim == h->ns.in, "marl_dqn_update_grads: trajectory shape mismatch");
+  MARL_REQUIRE(h->hp.mixer != 2 || h->mix != nullptr, "marl_dqn_update: QMIX needs marl_dqn_qmix_init first");
+  MARL_REQUIRE(h->hp.mixer == 0 || !h->standardise || batch == h->n_stat, "marl_dqn_update: %s's standardise_returns keeps one statistic per batch entry (the "
+               "reference's reshape(-1, B)): batch %d must stay at max_batch %d", h->hp.mixer == 2 ? "QMIX" : "VDN", batch, h->n_stat);
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const RowPlan plan = h->rnn ? make_plan(h->ns, batch, 1, h->n_sm, kGruSeqs) : episode_plan(h->ns, batch, traj->T, h->n_sm);
+  const RowSource src = episode_rows(traj, episode_idx, h->ns.n_agents, h->ns.in);
+  // timing (bench.py's roofline leg): 4 events per timed update, around the training pass and between the tensor-core kernels; the recurrent
+  // path's window opens before its online forward
+  cudaEvent_t* ev = h->timing && h->ev_used < kTimingPairs ? &h->ev[4 * h->ev_used] : nullptr;
+  // target network on every gathered row (dqn/model.py:132-134); several ranks: the previous update launched it between its push and its finish
+  if (h->tq_ahead) h->tq_ahead = false;
+  else if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, st)) return rc;
+  TrainParams tp; memset(&tp, 0, sizeof(tp));
+  tp.plan = plan; tp.src = src; tp.theta = h->theta; tp.lay = h->ns.lay; tp.tq = h->tq;
+  tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = h->loss_part;
+  int n_loss_parts = h->rnn ? 0 : plan.cta_begin[plan.n_nets];
+  if (ev && h->rnn) cudaEventRecord(ev[0], st);
+  if (int rc = dqn_td_head(h, plan, src, batch, tp, n_loss_parts, st)) return rc;
+  if (ev && !h->rnn) cudaEventRecord(ev[0], st);
+  bool tc = false;
+  if (int rc = dqn_train_pass(h, tp, ev ? ev + 1 : nullptr, tc, st)) return rc;
+  if (ev) { cudaEventRecord(ev[3], st); h->ev_used += 1; h->ev_split |= tc; }
   ReduceParams rp; rp.scratch = h->scratch; rp.loss_part = h->loss_part; rp.n_nets = h->ns.n_nets; rp.P = h->P(); rp.scratch_pitch = h->scratch_pitch;
   memcpy(rp.cta_begin, plan.cta_begin, sizeof(rp.cta_begin));
   rp.n_loss_parts = n_loss_parts; rp.grad = h->grad; rp.stats = h->grad + h->n_params; rp.stats_accumulate = 0; rp.sumsq_part = h->sumsq;
@@ -649,8 +594,7 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
       if (next != nullptr && ap.target_mode == 0 && !h->standardise && h->hp.mixer == 0 && !h->rnn) {
         const RowPlan plan = episode_plan(h->ns, batch, traj->T, h->n_sm);
         const RowSource src = episode_rows(traj, next->idx, h->ns.n_agents, h->ns.in);
-        if (int rc = forward_any(h->ns, plan, src, h->theta_tgt, h->image_tgt, h->tq, (cudaStream_t)stream, h->tgt_image_current)) return rc;
-        h->tgt_image_current = tc_forward_enabled() != 0;
+        if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, (cudaStream_t)stream)) return rc;
         h->tq_ahead = true;
       }
       if (int rc = launch_adam_finish(rp, ap, h->opt.kind, &h->xchg, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream)) return rc;

@@ -13,6 +13,7 @@
 // Persistent CTAs, one per SM (132 on H100) split across networks; FP32 FFMA register-tiled GEMMs (see mlp.cuh).
 #include "tc_common.cuh"
 #include "ac_heads.cuh"
+#include "dqn_heads.cuh"
 
 namespace marl {
 
@@ -231,27 +232,12 @@ __device__ __forceinline__ void mlp_backward_tile(float* X, float* H1, float* H2
 
 __device__ __forceinline__ void head_dqn(const TrainParams& p, const RowCtx& c, const float* q, const float* qn, float (&dq)[kOutPad], float (&st)[4]) {
   const int act = c.act;
-  const float filled = c.filled;
   float g;
-  if (p.td_ext) {  // VDN: the agent-coupled TD error was computed by vdn_td_kernel
+  if (p.td_ext) {  // VDN, QMIX, standardise_returns: the TD error came from the column TD kernel or the mixer
     g = p.td_ext[(size_t)c.agent * p.td_agent_stride + (size_t)c.b * c.T + c.tt];
   } else {
-    const float rew = c.rew, done1 = c.done1;
     const float* tq = p.tq + (((size_t)c.agent * c.B + c.b) * (c.T + 1) + c.tt + 1) * c.A;
-    float tsel;
-    if (p.double_q) {  // dqn/model.py:138-143
-      int best = 0; float bv = qn[0];
-      for (int o = 1; o < c.A; ++o) if (qn[o] > bv) { bv = qn[o]; best = o; }
-      tsel = tq[best];
-    } else {
-      tsel = tq[0];
-      for (int o = 1; o < c.A; ++o) tsel = fmaxf(tsel, tq[o]);
-    }
-    const float y = rew + p.gamma * tsel * (1.f - done1);   // dqn/model.py:152
-    const float delta = q[act] - y;
-    st[0] += delta * delta * filled;                        // dqn/model.py:160-163
-    if (c.agent == 0) st[1] += filled;
-    g = 2.f * delta * filled;
+    g = td_error(q[act], td_target(c.rew, p.gamma, next_value(qn, tq, c.A, p.double_q), c.done1), c.filled, c.agent == 0, st[0], st[1]);
   }
 #pragma unroll
   for (int o = 0; o < kOutPad; ++o) dq[o] = (o == act) ? g : 0.f;

@@ -21,6 +21,8 @@
 // The mixer's parameters take the shared Adam step WITHOUT gradient clipping: the reference clips self.critic.parameters() only (dqn/model.py:169-170).
 #pragma once
 #include "learner.cuh"
+#include "dqn_heads.cuh"
+#include "retms.cuh"
 
 namespace marl {
 
@@ -240,19 +242,8 @@ __device__ __forceinline__ void qm_load_inputs(const QmSmem& sm, const QmixParam
     if (live) {
       const size_t row = ((size_t)a * p.B + b) * (T + 1) + t + dt;
       const float* q1 = p.q + row * p.A;
-      if (dt == 0) {
-        v = q1[p.traj.act[(ep * L.N + a) * T + t]];
-      } else {
-        const float* t1 = p.tq + row * p.A;
-        if (p.double_q) {
-          int best = 0; float bv = q1[0];
-          for (int o = 1; o < p.A; ++o) if (q1[o] > bv) { bv = q1[o]; best = o; }
-          v = t1[best];
-        } else {
-          v = t1[0];
-          for (int o = 1; o < p.A; ++o) v = fmaxf(v, t1[o]);
-        }
-      }
+      if (dt == 0) v = q1[p.traj.act[(ep * L.N + a) * T + t]];
+      else v = next_value(q1, p.tq + row * p.A, p.A, p.double_q);
     }
     sm.QA[a * kQmP + lane] = v;
   }
@@ -290,9 +281,8 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
   }
   if constexpr (MODE == 1) {   // the target mixer's output de-standardised with the statistics so far (dqn/model.py:415-418), no FMA contraction
     if (live && warp == 0) {
-      const float tq = __fadd_rn(__fmul_rn(ytgt, sqrtf(p.ret_ms[p.n_stat + b])), p.ret_ms[b]);
-      const float rew = p.traj.rew[(ep * L.N + 0) * T + t];
-      p.ret[s] = __fadd_rn(rew, __fmul_rn(__fmul_rn(p.gamma, tq), 1.f - (float)p.traj.done[ep * (T + 1) + t + 1]));
+      const float tq = unstandardise(ytgt, p.ret_ms[b], p.ret_ms[p.n_stat + b]);
+      p.ret[s] = td_target_rn(p.traj.rew[(ep * L.N + 0) * T + t], p.gamma, tq, (float)p.traj.done[ep * (T + 1) + t + 1]);
     }
   } else {
     // ---- online ----
@@ -305,7 +295,7 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
     const float filled = live ? (float)p.traj.filled[ep * T + t] : 0.f;
     float ret;
     if constexpr (MODE == 2) ret = live ? p.ret[s] : 0.f;
-    else ret = live ? p.traj.rew[(ep * L.N + 0) * T + t] + p.gamma * ytgt * (1.f - (float)p.traj.done[ep * (T + 1) + t + 1]) : 0.f;
+    else ret = live ? td_target(p.traj.rew[(ep * L.N + 0) * T + t], p.gamma, ytgt, (float)p.traj.done[ep * (T + 1) + t + 1]) : 0.f;
     const float delta = live ? y - ret : 0.f, dy = 2.f * delta * filled;
     float* rc = p.rec + s;   // this sample's column of the field-major record
     if (live) {

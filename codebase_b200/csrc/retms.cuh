@@ -52,6 +52,8 @@ static __global__ void ret_standardise_kernel(RetMsParams p) {
   const int a = i / n_per;
   p.ret[i] = __fdiv_rn(__fsub_rn(p.ret[i], p.ret_ms[a]), sqrtf(p.ret_ms[p.N + a]));
 }
+// a value in standardised units back in return units, x * sqrt(var) + mean, without FMA contraction as the reference's separate torch ops
+__device__ __forceinline__ float unstandardise(float x, float mean, float var) { return __fadd_rn(__fmul_rn(x, sqrtf(var)), mean); }
 // many short columns (VDN: one per batch entry, T values each): one thread per column, the other blocks' partials read as zero
 static __global__ void ret_moments_cols_kernel(RetMsParams p) {
   const int a = blockIdx.x * blockDim.x + threadIdx.x, n_per = p.P * p.T;

@@ -11,6 +11,7 @@
 //                        memory, accumulators in registers across all the CTA's rows; db3 on the CUDA cores
 // The partials feed the same grad_reduce_kernel / adam_kernel as the FP32 path.
 #include "tc_common.cuh"
+#include "dqn_heads.cuh"
 
 namespace marl {
 
@@ -151,20 +152,7 @@ __device__ __forceinline__ float td_grad(const TcTrainParams& p, size_t d, int a
   const float* q = p.rec + d * kRowRec;
   const float* qn = q + kRowRec;                 // the next row of the same episode
   const float* tq = p.tq + (d + 1) * A;          // target outputs share the [agent][unit][T + 1] row layout
-  float tsel;
-  if (p.double_q) {
-    int best = 0; float bv = qn[0];
-    for (int o = 1; o < A; ++o) if (qn[o] > bv) { bv = qn[o]; best = o; }
-    tsel = tq[best];
-  } else {
-    tsel = tq[0];
-    for (int o = 1; o < A; ++o) tsel = fmaxf(tsel, tq[o]);
-  }
-  const float y = rew + p.gamma * tsel * (1.f - done1);
-  const float delta = q[act] - y;
-  s0 += delta * delta * filled;
-  if (agent == 0) s1 += filled;
-  return 2.f * delta * filled;
+  return td_error(q[act], td_target(rew, p.gamma, next_value(qn, tq, A, p.double_q), done1), filled, agent == 0, s0, s1);
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) {
