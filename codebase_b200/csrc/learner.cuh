@@ -309,7 +309,7 @@ int launch_tc_forward(const FwdParams& p, const uint8_t* images, cudaStream_t st
 // ---- tensor-core training pipeline (tc_train.cu) ----------------------------------------------------------------------------
 struct TcBuffers {
   uint8_t* image; uint8_t* bwd_image;       // packed online-network images (forward K-major, backward K-major W2^T)
-  float *h1, *h2, *dh1;                     // [32][rows][4] (chunk-major) activations and hidden-layer gradient
+  float *h1, *h2;                           // [128][rows] (feature-major) activations
   float* rec;                               // [rows][16] row records (tc_train.cu)
   float* x;                                 // [rows][kMaxObsDim] gathered observation rows
   size_t rows;                              // allocated rows

@@ -248,10 +248,10 @@ struct TcTrainParams {
   RowPlan plan; RowSource src; NetLayout lay;
   const uint8_t* images;      // forward images [n_nets][kImageBytes]
   const uint8_t* bwd_images;  // backward images [n_nets][kBwdImageBytes]
-  // H1, H2, dH1: feature-major [128][rows] (the weight-gradient kernel stages 32 consecutive rows of one feature per warp instruction)
-  float* h1g; float* h2g; float* dh1g; size_t rows;
+  // H1, H2: feature-major [128][rows] (the weight-gradient kernel stages 32 consecutive rows of one feature per warp instruction)
+  float* h1g; float* h2g; size_t rows;
   float* rec;                 // [rows][kRowRec] row records
-  float* xg;                  // [rows][kMaxObsDim] gathered observation rows: the weight-gradient kernel reads them without chasing the episode index again
+  float* xg;                  // [rows][kMaxObsDim] gathered observation rows: the dH1 kernel reads them for dW1 without chasing the episode index again
   const float* tq; const float* td_ext; int td_agent_stride; float gamma; int double_q;
   float* scratch; int scratch_pitch; float* loss_part;
 };

@@ -6,9 +6,10 @@
 //                        feature-major), the gathered observation row, the row's outputs and the ReLU masks of H1 / H2 (row record)
 //   tc_dh1_kernel       TD head (needs the next row's outputs, hence after the forward) -> dLoss/dq[act] and the loss statistics;
 //                        dH1 = (dH2 x W2) * relu'(H1) with dH2[r][j] = g_r W3[act_r][j] relu'(H2[r][j]) built in registers (the TD loss touches
-//                        one output per row); B = K-major image of W2^T
-//   tc_dw_kernel        dW2 | db2, dW1 | db1, dW3: row-streaming TN GEMMs over 32-row chunks staged transposed (K = rows) into shared
-//                        memory, accumulators in registers across all the CTA's rows; db3 on the CUDA cores
+//                        one output per row); B = K-major image of W2^T; then dW1 | db1 = dH1^T x [X | 1] from dH1 staged transposed
+//                        (K = rows) into shared memory, so dH1 never leaves the SM
+//   tc_dw_kernel        dW2 | db2, dW3: row-streaming TN GEMMs over 32-row chunks staged transposed (K = rows) into shared memory,
+//                        accumulators in registers across all the CTA's rows; db3 on the CUDA cores
 // The partials feed the same grad_reduce_kernel / adam_kernel as the FP32 path.
 #include "tc_common.cuh"
 #include "dqn_heads.cuh"
@@ -22,6 +23,20 @@ __device__ __forceinline__ const float* train_row(const TcTrainParams& p, int ne
   const TrajView& tv = p.src.traj;
   ep = p.src.idx[unit];
   return tv.obs + (((size_t)ep * tv.N + agent) * (size_t)(tv.T + 1) + off) * p.src.D;
+}
+
+// The weight gradients contract over rows, so both operands of each are staged K-major (one 128-byte swizzled line of 32 rows per feature),
+// hi | lo, in 32-row chunks: chunk c of a CTA is rows [row_begin + 32 c, + 32), i.e. tile c / 4, warpgroup (c / 2) % 2, half c % 2.
+constexpr int kChunk = 32;
+constexpr int kLine = 128;                                              // one feature's 32 rows
+
+// byte offset of (line f, row r) in a K-major SWIZZLE_128B operand of 32 rows
+__device__ __forceinline__ int line_off(int f, int r) { return f * kLine + ((((r >> 2) ^ (f & 7)) & 7) << 4) + ((r & 3) << 2); }
+__device__ __forceinline__ void stage_hl(uint8_t* base, int lines, int f, int r, float x) {
+  float hi, lo;
+  tf32_split(x, hi, lo);
+  *reinterpret_cast<float*>(base + line_off(f, r)) = hi;
+  *reinterpret_cast<float*>(base + lines * kLine + line_off(f, r)) = lo;
 }
 
 // =====================================================================================================================
@@ -132,12 +147,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
 }
 
 // =====================================================================================================================
-// 2. TD head + dH1 = (dH2 x W2) * relu'(H1)
+// 2. TD head + dH1 = (dH2 x W2) * relu'(H1) + dW1 | db1 [j1][i | 1] += dH1^T x [X | 1]^T
 // =====================================================================================================================
-constexpr int kDh1W3 = kBwdImageBytes;                        // FP32 copy of W3 [8][128] behind the W2^T image
+// Two staging buffers, one chunk each: A = dH1 (128 lines), B = [X | 1] (32 lines, line D = ones, the lines behind it zero)
+constexpr int kDh1SA = kBwdImageBytes;                        // behind the W2^T image: [2][hi | lo][128 lines]
+constexpr int kDh1SB = kDh1SA + 2 * 2 * 128 * kLine;          // [2][hi | lo][32 lines]
+constexpr int kDh1W3 = kDh1SB + 2 * 2 * 32 * kLine;           // FP32 copy of W3 [8][128]
 constexpr int kDh1Bar = kDh1W3 + kOutPad * kHidden * 4;
 constexpr int kDh1Red = kDh1Bar + 64;                         // [2][kTcThreads] loss statistics
 constexpr int kDh1Smem = kDh1Red + 2 * kTcThreads * 4 + 1024;
+static_assert(kDh1SA % 1024 == 0 && kDh1SB % 1024 == 0 && kDh1Smem <= 227 * 1024,
+              "dH1 kernel: 1024-byte aligned operands within the shared memory of one SM");
 
 // dLoss/dq[act] of one row (0 at t == T) and its loss statistics (delta^2 filled, filled on agent 0)
 __device__ __forceinline__ float td_grad(const TcTrainParams& p, size_t d, int agent, int b, int tt, int ep, int& act, float& s0, float& s1) {
@@ -153,6 +173,49 @@ __device__ __forceinline__ float td_grad(const TcTrainParams& p, size_t d, int a
   const float* qn = q + kRowRec;                 // the next row of the same episode
   const float* tq = p.tq + (d + 1) * A;          // target outputs share the [agent][unit][T + 1] row layout
   return td_error(q[act], td_target(rew, p.gamma, next_value(qn, tq, A, p.double_q), done1), filled, agent == 0, s0, s1);
+}
+
+// One staging phase of the dW1 product: warpgroup `owner` stages its two chunks of a tile, c and c + 1 (its 64 rows of dH1 from the accumulator
+// fragments `h` masked by relu'(H1) `m1`, and of [X | 1] from `xv`), one per buffer; then both warpgroups issue the MMAs of those that hold rows
+// (warpgroup w: output rows j1 in [64 w, 64 w + 64); term order lo*hi, hi*lo, hi*hi per k-step).  Block-wide; the caller skips a phase with
+// no rows (c past the CTA's rows) on every thread.
+__device__ __forceinline__ void dw1_phase(int owner, int c, int row_begin, int row_end, int D, uint8_t* smem, uint32_t sb, const float (&h)[64],
+                                          uint64_t m1, const float (&xv)[2][kMaxObsDim / 4], float (&acc1)[16]) {
+  const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, g = (t & 31) >> 2, tq = t & 3;
+  const int half = wq >> 1, cr = 16 * (wq & 1) + g;   // this warp's rows are the warpgroup's chunk `half`, rows cr and cr + 8 of it
+  wg_wait<0>();
+  fence_regs(acc1);
+  __syncthreads();   // both warpgroups are done reading the buffers
+  if (wg == owner && row_begin + (c + half) * kChunk < row_end) {
+    uint8_t* sa = smem + kDh1SA + half * 2 * 128 * kLine;
+    uint8_t* sbx = smem + kDh1SB + half * 2 * 32 * kLine;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) stage_hl(sa, 128, frag_col(i, tq), cr + ((i & 2) ? 8 : 0), ((m1 >> i) & 1) ? h[i] : 0.f);
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int m = 0; m < kMaxObsDim / 4; ++m)
+        if (tq + 4 * m < D) stage_hl(sbx, 32, tq + 4 * m, cr + 8 * k, xv[k][m]);
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes, read by wgmma through the async proxy
+  __syncthreads();
+  wg_fence();
+  const uint32_t m_off = (uint32_t)(wg * kWgRows * kLine);
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    if (row_begin + (c + b) * kChunk >= row_end) continue;
+    const uint32_t a_base = sb + kDh1SA + b * 2 * 128 * kLine + m_off, b_base = sb + kDh1SB + b * 2 * 32 * kLine;
+#pragma unroll
+    for (int term = 0; term < 3; ++term) {
+      const uint32_t ah = term == 0 ? 1u : 0u, bh = term == 1 ? 1u : 0u;   // lo*hi, hi*lo, hi*hi
+#pragma unroll
+      for (int ks = 0; ks < kChunk / 8; ++ks) {
+        const uint32_t ko = (uint32_t)(ks * 32);
+        wgmma_ss_n32(acc1, sw128_desc(a_base + ah * 128 * kLine + ko), sw128_desc(b_base + bh * 32 * kLine + ko), 1u);
+      }
+    }
+  }
+  wg_commit();
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) {
@@ -180,9 +243,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
     tma_image_range(sb, p.bwd_images + (size_t)net * kBwdImageBytes, 0, kBwdImageBytes, bar);
     tma_bulk_g2s(sb + kDh1W3, p.images + (size_t)net * kImageBytes + kOffW3F, kOutPad * kHidden * 4, bar);
   }
+  const int D = p.src.D;
+  for (int i = t; i < 2 * 32 * kChunk; i += kTcThreads) {   // constant lines of both B buffers: the ones line (hi 1, lo 0) and the zero lines behind it
+    const int b = i / (32 * kChunk), f = (i / kChunk) % 32, r = i % kChunk;
+    if (f >= D) stage_hl(smem + kDh1SB + b * 2 * 32 * kLine, 32, f, r, f == D ? 1.f : 0.f);
+  }
+  float acc1[16];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) acc1[i] = 0.f;
+  // dH1 fragments, relu'(H1) and observation rows of the tile before: warpgroup 1 stages them after this tile's loads have been issued
+  float acc[64], xv[2][kMaxObsDim / 4];
+  uint64_t m1 = 0;
   float st0 = 0.f, st1 = 0.f;
   bool first = true;
-  for (int vr0 = row_begin + kWgRows * wg; vr0 < row_end; vr0 += kTileRows) {
+  // both warpgroups walk every tile (the staging barriers are block-wide); a warpgroup whose rows all lie past row_end skips its product
+  for (int t0 = row_begin; t0 < row_end; t0 += kTileRows) {
+    const int vr0 = t0 + kWgRows * wg, c0 = (t0 - row_begin) / kChunk;
     long long d[2];
     float gr[2];
     int act[2];
@@ -208,32 +284,57 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
         const float* rp = p.rec + (size_t)d[k] * kRowRec;
         mh1[k] = __float_as_uint(rp[kRecMask1 + tq]); mh2[k] = __float_as_uint(rp[kRecMask2 + tq]);
       }
+    // the previous tile's chunks 2 and 3 (warpgroup 1), behind this tile's gathers and mask loads: the MMAs on the buffers are long done by now
+    if (t0 > row_begin && row_begin + (c0 - 2) * kChunk < row_end) dw1_phase(1, c0 - 2, row_begin, row_end, D, smem, sb, acc, m1, xv, acc1);
     float v[64];
-    uint64_t m1 = 0;
+    m1 = 0;
 #pragma unroll
     for (int i = 0; i < 64; ++i) {
       const int k = (i >> 1) & 1, bit = ((i >> 2) << 1) | (i & 1);
       v[i] = ((mh2[k] >> bit) & 1u) ? gr[k] * w3f[act[k] * kHidden + frag_col(i, tq)] : 0.f;
       m1 |= (uint64_t)((mh1[k] >> bit) & 1u) << i;
     }
-    float acc[64];
-    {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    if (vr0 < row_end) {
       uint32_t hi[16][4], lo[16][4];
       frag_to_a(v, hi, lo);
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       // D[r][j1] = sum_{j2} dH2[r][j2] W2[j2][j1]: B = K-major image of W2^T (rows j1, K = j2)
       layer_rs<16>(acc, hi, lo, sb, sb + 4 * kPanelBytes, 16);
     }
+    // the observation rows of this thread's two rows, features tq + 4 m (a quad covers a row; 0 for rows without a source)
 #pragma unroll
-    for (int i = 0; i < 64; ++i) {
-      const int k = (i >> 1) & 1;
-      if (d[k] >= 0) p.dh1g[(size_t)frag_col(i, tq) * p.rows + (size_t)d[k]] = ((m1 >> i) & 1) ? acc[i] : 0.f;
-    }
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+      for (int m = 0; m < kMaxObsDim / 4; ++m) {
+        const int f = tq + 4 * m;
+        xv[k][m] = (d[k] >= 0 && f < D) ? p.xg[(size_t)d[k] * kMaxObsDim + f] : 0.f;
+      }
     const long long dr = tq == 0 ? d[0] : d[1];
     if (tq < 2 && dr >= 0) {
       float* rp = p.rec + (size_t)dr * kRowRec;
       rp[kRecG] = tq == 0 ? gr[0] : gr[1]; rp[kRecAct] = __int_as_float(tq == 0 ? act[0] : act[1]);
+    }
+    // ---- dW1 | db1 over the tile's four chunks in row order: warpgroup 0 stages chunks 0 and 1 now, warpgroup 1 chunks 2 and 3 at the top of
+    // the next tile (or after the last one)
+    dw1_phase(0, c0, row_begin, row_end, D, smem, sb, acc, m1, xv, acc1);
+  }
+  {
+    const int c_last = (row_end - 1 - row_begin) / kTileRows * (kTileRows / kChunk);
+    if (row_begin + (c_last + 2) * kChunk < row_end) dw1_phase(1, c_last + 2, row_begin, row_end, D, smem, sb, acc, m1, xv, acc1);
+  }
+  wg_wait<0>();
+  fence_regs(acc1);
+  TSG(g_ts_dh1, 30);
+  // ---- dW1 | db1 -> this CTA's gradient sums (the weight-gradient kernel writes the other parameters) ---------------------------------
+  {
+    const NetLayout& L = p.lay;
+    float* gs = p.scratch + (size_t)blockIdx.x * p.scratch_pitch;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int m = wg * kWgRows + 16 * wq + g + ((i & 2) ? 8 : 0), n = frag_col(i, tq);
+      if (n < D) gs[L.w1 + m * D + n] = acc1[i];
+      else if (n == D) gs[L.b1 + m] = acc1[i];
     }
   }
   // ---- per-CTA loss statistics, summed in a fixed order ----------------------------------------------------------------
@@ -250,27 +351,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
 // =====================================================================================================================
 // 3. weight gradients: row-streaming TN GEMMs over 32-row chunks, accumulators in registers
 // =====================================================================================================================
-// Every operand is staged K-major (one 128-byte swizzled line of 32 rows per feature), hi | lo:
 //   dW2 | db2 [j2][j1 | 1] += dH2^T x [H1 | 1]^T   (A: 128 lines, B: 136 lines, line 128 = ones)
-//   dW1 | db1 [j1][i | 1]  += dH1^T x [X | 1]^T    (B: 32 lines, line D = ones)
 //   dW3^T [j][a]           += H2^T x dq^T          (B: 8 lines, dq[r][a] = g_r at a = act_r)
-// Warpgroup w accumulates the M rows [64 w, 64 w + 64) of all three.
-constexpr int kChunk = 32;
-constexpr int kLine = 128;                                              // one feature's 32 rows
-constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA1 = kSB2 + 2 * 136 * kLine, kSB1 = kSA1 + 2 * 128 * kLine;
-constexpr int kSA3 = kSB1 + 2 * 32 * kLine, kSB3 = kSA3 + 2 * 128 * kLine, kSW3 = kSB3 + 2 * 8 * kLine;
+// Warpgroup w accumulates the M rows [64 w, 64 w + 64) of both.
+constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA3 = kSB2 + 2 * 136 * kLine, kSB3 = kSA3 + 2 * 128 * kLine, kSW3 = kSB3 + 2 * 8 * kLine;
 constexpr int kDwSmem = kSW3 + kOutPad * kHidden * 4 + 1024;
-static_assert(kSB2 % 1024 == 0 && kSA1 % 1024 == 0 && kSB1 % 1024 == 0 && kSA3 % 1024 == 0 && kSB3 % 1024 == 0 && kDwSmem <= 227 * 1024,
+static_assert(kSB2 % 1024 == 0 && kSA3 % 1024 == 0 && kSB3 % 1024 == 0 && kDwSmem <= 227 * 1024,
               "weight-gradient staging: 1024-byte aligned operands within the shared memory of one SM");
-
-// byte offset of (line f, row r) in a K-major SWIZZLE_128B operand of 32 rows
-__device__ __forceinline__ int line_off(int f, int r) { return f * kLine + ((((r >> 2) ^ (f & 7)) & 7) << 4) + ((r & 3) << 2); }
-__device__ __forceinline__ void stage_hl(uint8_t* base, int lines, int f, int r, float x) {
-  float hi, lo;
-  tf32_split(x, hi, lo);
-  *reinterpret_cast<float*>(base + line_off(f, r)) = hi;
-  *reinterpret_cast<float*>(base + lines * kLine + line_off(f, r)) = lo;
-}
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -287,15 +374,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     return;
   }
   TSG(g_ts_dw, 0);
-  const int D = p.src.D, A = p.lay.out;
-  // constant lines: the ones line (hi 1, lo 0) of [H1 | 1] and [X | 1] and the zero lines behind them; W3 copy
+  const int A = p.lay.out;
+  // constant lines: the ones line (hi 1, lo 0) of [H1 | 1] and the zero lines behind it; W3 copy
   for (int i = t; i < 8 * kChunk; i += kTcThreads) {
     const int f = 128 + i / kChunk, r = i % kChunk;
     stage_hl(smem + kSB2, 136, f, r, f == 128 ? 1.f : 0.f);
-  }
-  for (int i = t; i < 32 * kChunk; i += kTcThreads) {
-    const int f = i / kChunk, r = i % kChunk;
-    if (f >= D) stage_hl(smem + kSB1, 32, f, r, f == D ? 1.f : 0.f);
   }
   {
     const float4* w3src = reinterpret_cast<const float4*>(p.images + (size_t)net * kImageBytes + kOffW3F);
@@ -303,11 +386,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   }
   __syncthreads();
   const uint32_t sb = smem_u32(smem);
-  float acc2[68], acc1[16], acc3[4];
+  float acc2[68], acc3[4];
 #pragma unroll
   for (int i = 0; i < 68; ++i) acc2[i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < 16; ++i) acc1[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) acc3[i] = 0.f;
   float db3 = 0.f;   // warp a, lane 0: sum of dq[.][a]
@@ -315,7 +396,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   for (int c = 0; c < n_chunks; ++c) {
     // ---- this thread's row (lane) and features (warp + 8 i) of the chunk -> registers; their loads overlap the previous chunk's MMAs
     const int vr = row_begin + c * kChunk + lane;
-    float h1v[16], dh1v[16], h2v[16], xv[kMaxObsDim / 8], gr = 0.f;
+    float h1v[16], h2v[16], gr = 0.f;
     int act = 0;
     {
       long long d = -1;
@@ -329,16 +410,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
         const size_t o = (size_t)(warp + 8 * i) * p.rows + (size_t)d;
-        h1v[i] = d >= 0 ? p.h1g[o] : 0.f; dh1v[i] = d >= 0 ? p.dh1g[o] : 0.f; h2v[i] = d >= 0 ? p.h2g[o] : 0.f;
-      }
-#pragma unroll
-      for (int m = 0; m < kMaxObsDim / 8; ++m) {
-        const int f = warp + 8 * m;
-        xv[m] = (d >= 0 && f < D) ? p.xg[(size_t)d * kMaxObsDim + f] : 0.f;
+        h1v[i] = d >= 0 ? p.h1g[o] : 0.f; h2v[i] = d >= 0 ? p.h2g[o] : 0.f;
       }
     }
     wg_wait<0>();
-    fence_regs(acc2); fence_regs(acc1); fence_regs(acc3);
+    fence_regs(acc2); fence_regs(acc3);
     __syncthreads();   // both warpgroups are done reading the previous chunk
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
@@ -346,12 +422,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
       const float dh2 = h2v[i] > 0.f ? gr * w3f[act * kHidden + j] : 0.f;
       stage_hl(smem + kSA2, 128, j, lane, dh2);
       stage_hl(smem + kSB2, 136, j, lane, h1v[i]);
-      stage_hl(smem + kSA1, 128, j, lane, dh1v[i]);
       stage_hl(smem + kSA3, 128, j, lane, h2v[i]);
     }
-#pragma unroll
-    for (int m = 0; m < kMaxObsDim / 8; ++m)
-      if (warp + 8 * m < D) stage_hl(smem + kSB1, 32, warp + 8 * m, lane, xv[m]);
     {
       const float dq = act == warp ? gr : 0.f;   // warp = output a
       stage_hl(smem + kSB3, 8, warp, lane, dq);
@@ -371,14 +443,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
       for (int ks = 0; ks < kChunk / 8; ++ks) {
         const uint32_t ko = (uint32_t)(ks * 32);
         wgmma_ss_n136(acc2, sw128_desc(sb + kSA2 + ah * 128 * kLine + m_off + ko), sw128_desc(sb + kSB2 + bh * 136 * kLine + ko), 1u);
-        wgmma_ss_n32(acc1, sw128_desc(sb + kSA1 + ah * 128 * kLine + m_off + ko), sw128_desc(sb + kSB1 + bh * 32 * kLine + ko), 1u);
         wgmma_ss_n8(acc3, sw128_desc(sb + kSA3 + ah * 128 * kLine + m_off + ko), sw128_desc(sb + kSB3 + bh * 8 * kLine + ko), 1u);
       }
     }
     wg_commit();
   }
   wg_wait<0>();
-  fence_regs(acc2); fence_regs(acc1); fence_regs(acc3);
+  fence_regs(acc2); fence_regs(acc3);
   TSG(g_ts_dw, 30);
   // ---- accumulators -> this CTA's gradient sums ------------------------------------------------------------------------------------
   const NetLayout& L = p.lay;
@@ -387,12 +458,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     const int m = wg * kWgRows + 16 * wq + g + ((i & 2) ? 8 : 0), n = frag_col(i, tq);
     if (n < kHidden) gs[L.w2 + m * kHidden + n] = acc2[i];
     else if (n == kHidden) gs[L.b2 + m] = acc2[i];
-  }
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const int m = wg * kWgRows + 16 * wq + g + ((i & 2) ? 8 : 0), n = frag_col(i, tq);
-    if (n < D) gs[L.w1 + m * D + n] = acc1[i];
-    else if (n == D) gs[L.b1 + m] = acc1[i];
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -421,7 +486,7 @@ int launch_tc_dqn_train(const TrainParams& tp, const TcBuffers& buf, cudaStream_
   MARL_REQUIRE(tp.src.mode == 1, "tensor-core backward: rows must be gathered from the trajectory store (mode %d)", tp.src.mode);
   TcTrainParams p; memset(&p, 0, sizeof(p));
   p.plan = tp.plan; p.src = tp.src; p.lay = tp.lay; p.images = buf.image; p.bwd_images = buf.bwd_image;
-  p.h1g = buf.h1; p.h2g = buf.h2; p.dh1g = buf.dh1; p.rec = buf.rec; p.xg = buf.x; p.rows = buf.rows;
+  p.h1g = buf.h1; p.h2g = buf.h2; p.rec = buf.rec; p.xg = buf.x; p.rows = buf.rows;
   p.tq = tp.tq; p.td_ext = tp.td_ext; p.td_agent_stride = tp.td_agent_stride; p.gamma = tp.gamma; p.double_q = tp.double_q;
   p.scratch = tp.scratch; p.scratch_pitch = tp.scratch_pitch; p.loss_part = tp.loss_part;
   const int grid = tp.plan.cta_begin[tp.plan.n_nets];

@@ -205,7 +205,7 @@ class QNetwork(NativeLearner):
         return bool(v.value)
 
     def timing_kernels(self):
-        """After timing(False): (ms of online forward + TD head, ms of dH1, ms of weight gradients), launches -- tensor-core pass only."""
+        """After timing(False): (ms of online forward + TD head, ms of dH1 + dW1, ms of the other weight gradients), launches -- tensor-core pass only."""
         ms3, n = (C.c_float * 3)(), C.c_int32()
         nat.check(self._lib.marl_dqn_timing_kernels(self._h, ms3, C.byref(n)), "marl_dqn_timing_kernels")
         return [float(x) for x in ms3], int(n.value)

@@ -332,7 +332,7 @@ int marl_dqn_peer_status(marl_dqn* q, int32_t* timed_out);
 /* measurement hook (bench.py roofline leg): CUDA-event time of the training-kernel launches between enable=1 and enable=0 */
 int marl_dqn_timing(marl_dqn* q, int32_t enable, float* total_ms, int32_t* count);
 /* after marl_dqn_timing(q, 0, ..): the same window split over the three kernels of the tensor-core training pass, ms3[0..2] =
- * summed durations of (online forward + TD head, dH1, weight gradients); *count = 0 if the window ran the fused FP32 kernel */
+ * summed durations of (online forward + TD head, dH1 + dW1, the other weight gradients); *count = 0 if the window ran the fused FP32 kernel */
 int marl_dqn_timing_kernels(marl_dqn* q, float* ms3, int32_t* count);
 int marl_dqn_set_counters(marl_dqn* q, int64_t updates, int64_t last_target_update);
 
