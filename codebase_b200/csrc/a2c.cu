@@ -35,13 +35,13 @@ __global__ void nstep_returns_kernel(NStepParams p) {
   for (int k = 0; k <= p.n_steps; ++k) {
     const int tt = t + k;
     if (tt >= T) break;
-    const float d = (float)p.traj.done[ep * (T + 1) + tt];
+    const float d = (float)p.traj.done[p.traj.done_at(ep, tt)];
     float src;
     if (k == p.n_steps) {
-      src = p.vt[((size_t)a * p.P + b) * (T + 1) + tt];
+      src = p.vt[row_index(a, b, tt, p.P, T + 1)];
       if (p.ret_ms) src = unstandardise(src, p.ret_ms[a], p.ret_ms[p.N + a]);
     } else {
-      src = p.traj.rew[(ep * p.N + a) * T + tt];
+      src = p.traj.rew[p.traj.step_at(ep, a, tt)];
     }
     acc += (p.gpow[k] * src) * (1.f - d);
   }
@@ -55,8 +55,8 @@ __global__ void old_logp_kernel(OldLogpParams p) {
   const int T = p.traj.T, i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= p.N * p.P * T) return;
   const int a = i / (p.P * T), rem = i - a * p.P * T, b = rem / T, t = rem - b * T;
-  const float* q = p.logits + (((size_t)a * p.P + b) * (T + 1) + t) * p.A;
-  const int act = p.traj.act[((size_t)p.idx[b] * p.N + a) * T + t];
+  const float* q = p.logits + row_index(a, b, t, p.P, T + 1) * p.A;
+  const int act = p.traj.act[p.traj.step_at(p.idx[b], a, t)];
   float m = q[0];
   for (int o = 1; o < p.A; ++o) m = fmaxf(m, q[o]);
   float s = 0.f;
@@ -81,7 +81,7 @@ __global__ void joint_obs_kernel(JointParams p) {
   if (i >= (size_t)p.P * T1 * ND) return;
   const int c = (int)(i % ND), t = (int)((i / ND) % T1), b = (int)(i / ((size_t)ND * T1));
   const int j = c / p.traj.D, d = c - j * p.traj.D;
-  p.out[i] = p.traj.obs[(((size_t)p.idx[b] * p.traj.N + j) * T1 + t) * p.traj.D + d];
+  p.out[i] = p.traj.obs_row(p.idx[b], j, t)[d];
 }
 
 __global__ void iota_kernel(int32_t* x, int n) {
@@ -263,7 +263,7 @@ static int a2c_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs,
     const size_t n = (size_t)n_envs * (T + 1) * h->critic.in;
     joint_obs_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(jp);
     MARL_CUDA_TRY(cudaGetLastError());
-    ps.csrc.mode = 2; ps.csrc.joint = h->joint; ps.csrc.D = h->critic.in;
+    ps.csrc.mode = kRowsEpisodeJoint; ps.csrc.joint = h->joint; ps.csrc.D = h->critic.in;
   }
   // 1. target critic on all T+1 observations (ac/model.py:190-193)
   if (h->critic_rnn) {

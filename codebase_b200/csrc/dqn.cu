@@ -36,7 +36,7 @@ __global__ void replay_sample_kernel(uint64_t seed, uint64_t update_idx, int bat
 //   STAGE 2: td from chosen and the standardised returns, and the loss statistics.
 struct ColTdParams {
   const float* q; const float* tq;  // [N][B][T+1][A]
-  TrajView traj; const int32_t* idx; int B, N, A; float gamma; int double_q;
+  TrajView traj; const int32_t* idx; int B, A; float gamma; int double_q;
   int C, G;
   const float* ret_ms; int n_stat, stat_per_b;   // STAGE 1: mean[n_stat] | var[n_stat]
   float* ret; float* chosen;                     // STAGES 1, 2: [C][B][T]
@@ -64,18 +64,18 @@ __global__ void __launch_bounds__(256) col_td_kernel(ColTdParams p) {
     const int c = i / (p.B * T), rem = i - c * p.B * T, b = rem / T, t = rem - b * T;
     const size_t ep = (size_t)p.idx[b];
     if constexpr (STAGE == 2) {
-      p.td[i] = td_error(p.chosen[i], p.ret[i], (float)p.traj.filled[ep * T + t], c == 0, loss, fill);
+      p.td[i] = td_error(p.chosen[i], p.ret[i], (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill);
     } else {
       float chosen = 0.f, next = 0.f;
       for (int a = c * p.G; a < (c + 1) * p.G; ++a) {
-        const size_t row = ((size_t)a * p.B + b) * (T + 1) + t;
+        const size_t row = row_index(a, b, t, p.B, T + 1);
         const float* q0 = p.q + row * p.A;
-        chosen += q0[p.traj.act[(ep * p.N + a) * T + t]];
+        chosen += q0[p.traj.act[p.traj.step_at(ep, a, t)]];
         next += next_value(q0 + p.A, p.tq + (row + 1) * p.A, p.A, p.double_q);
       }
-      const float rew = p.traj.rew[(ep * p.N + c * p.G) * T + t], done1 = (float)p.traj.done[ep * (T + 1) + t + 1];
+      const float rew = p.traj.rew[p.traj.step_at(ep, c * p.G, t)], done1 = (float)p.traj.done[p.traj.done_at(ep, t + 1)];
       if constexpr (STAGE == 0) {
-        p.td[i] = td_error(chosen, td_target(rew, p.gamma, next, done1), (float)p.traj.filled[ep * T + t], c == 0, loss, fill);
+        p.td[i] = td_error(chosen, td_target(rew, p.gamma, next, done1), (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill);
       } else {
         const int col = p.stat_per_b ? b : c;
         p.ret[i] = td_target_rn(rew, p.gamma, unstandardise(next, p.ret_ms[col], p.ret_ms[p.n_stat + col]), done1);
@@ -441,7 +441,7 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
   // VDN: one column of all agents; independent learners: one column per agent
   const bool vdn = h->hp.mixer == 1;
   ColTdParams cp; memset(&cp, 0, sizeof(cp));
-  cp.q = h->q_all; cp.tq = h->tq; cp.traj = src.traj; cp.idx = src.idx; cp.B = batch; cp.N = h->ns.n_agents; cp.A = h->ns.out;
+  cp.q = h->q_all; cp.tq = h->tq; cp.traj = src.traj; cp.idx = src.idx; cp.B = batch; cp.A = h->ns.out;
   cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.C = vdn ? 1 : h->ns.n_agents; cp.G = vdn ? h->ns.n_agents : 1;
   cp.td = h->td; cp.loss_part = loss_part;
   const int blocks = (cp.C * batch * T + 255) / 256;

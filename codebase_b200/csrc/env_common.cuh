@@ -4,13 +4,9 @@
 // Included by lbf_env.cu and rware_env.cu.  Lanes of one env form a group of G consecutive lanes starting at `gbase`; `sub` is the agent.
 #pragma once
 #include <string.h>
-#include "common.cuh"
+#include "traj.cuh"
 
 namespace marl {
-
-struct TrajDev {
-  float* obs; int32_t* act; float* rew; uint8_t* done; uint8_t* filled; int capacity, T; int enabled;
-};
 
 struct StepArgs {
   int E; uint64_t seed; uint32_t gid0;
@@ -103,7 +99,7 @@ __device__ __forceinline__ double cooperative_sum(double rew_w, int gbase, int N
 
 // trajectory scalars (rb.add, dqn/train.py:73-89; batch_* writes, ac/train.py:90-99) of env e.  Returns the slot whose observation row
 // step1 this step fills, -1 for none.
-__device__ __forceinline__ int traj_write_scalars(const TrajDev& traj, const StepArgs& a, int e, int N, int sub, bool active, int step0, int a_raw,
+__device__ __forceinline__ int traj_write_scalars(const TrajView& traj, const StepArgs& a, int e, int N, int sub, bool active, int step0, int a_raw,
                                                   float rew_f, bool done, bool finished) {
   int slot = -1;
   const int step1 = step0 + 1;
@@ -111,16 +107,16 @@ __device__ __forceinline__ int traj_write_scalars(const TrajDev& traj, const Ste
   if (active && step0 < traj.T) {
     slot = sl;
     if (sub < N) {
-      traj.act[((size_t)sl * N + sub) * traj.T + step0] = a_raw;
-      traj.rew[((size_t)sl * N + sub) * traj.T + step0] = rew_f;
+      traj.act[traj.step_at(sl, sub, step0)] = a_raw;
+      traj.rew[traj.step_at(sl, sub, step0)] = rew_f;
     }
     if (sub == 0) {
-      traj.done[(size_t)sl * (traj.T + 1) + step1] = (uint8_t)(a.use_proper_termination ? done : finished);
-      traj.filled[(size_t)sl * traj.T + step0] = 1;
+      traj.done[traj.done_at(sl, step1)] = (uint8_t)(a.use_proper_termination ? done : finished);
+      traj.filled[traj.filled_at(sl, step0)] = 1;
     }
   } else if (!active && a.clear_stale && sub == 0 && step0 < traj.T) {
     // steps after the episode ended: the reference leaves a reused slot's old tail in place (SURVEY H6)
-    for (int t = step0; t < traj.T; ++t) traj.filled[(size_t)sl * traj.T + t] = 0;
+    for (int t = step0; t < traj.T; ++t) traj.filled[traj.filled_at(sl, t)] = 0;
   }
   return slot;
 }
@@ -151,12 +147,6 @@ int raise_smem_limit(K* kernel, size_t bytes, size_t& limit, const char* who) {
   }
   limit = bytes;
   return MARL_OK;
-}
-
-inline TrajDev to_traj(const marl_traj_view* t) {
-  TrajDev d; memset(&d, 0, sizeof(d));
-  if (t) { d.obs = t->obs; d.act = t->act; d.rew = t->rew; d.done = t->done; d.filled = t->filled; d.capacity = t->capacity; d.T = t->T; d.enabled = 1; }
-  return d;
 }
 
 template <typename H>
@@ -192,9 +182,9 @@ int rollout_step_args(const H* h, const char* who, const float* values, const ma
 }
 
 template <typename H, typename Dev, typename St>
-int launch_step(const H* h, void (*kernel)(Dev, St, StepArgs, TrajDev), const StepArgs& a, const marl_traj_view* traj, void* stream) {
+int launch_step(const H* h, void (*kernel)(Dev, St, StepArgs, TrajView), const StepArgs& a, const marl_traj_view* traj, void* stream) {
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, h->threads, h->step_smem, (cudaStream_t)stream>>>(h->dev, h->st, a, to_traj(traj));
+  kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, h->threads, h->step_smem, (cudaStream_t)stream>>>(h->dev, h->st, a, traj_view(traj));
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }

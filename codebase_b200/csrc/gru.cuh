@@ -28,15 +28,15 @@ struct GruLayout {
 };
 
 // One launch runs every sequence of every network for all of its steps.  plan: slot lists of the networks, units_per_agent = B (training:
-// one sequence per sampled episode and agent) or E (act step), unit_rows = steps per sequence (T + 1, or 1).  src: mode 1 gathers
-// through the replay indices, mode 0 reads dense obs [E][N][D], modes 2 / 3 the joint rows of a centralised critic (learner.cuh).
+// one sequence per sampled episode and agent) or E (act step), unit_rows = steps per sequence (T + 1, or 1).  src: kRowsEpisode
+// gathers through the replay indices, kRowsDense reads dense obs [E][N][D], the joint modes the rows of a centralised critic (learner.cuh).
 struct GruFwdParams {
   RowPlan plan; RowSource src;
   const float* theta; GruLayout lay;
-  const float* h_in;   // mode 0: [E][N][H] initial state (NULL: zeros); mode 1: always zeros (the reference's hiddens=None)
-  float* h_out;        // mode 0: [E][N][H] final state (NULL: not written)
-  float* q_out;        // mode 0: [E][N][A]; mode 1: [N][B][T+1][A]
-  float* save;         // mode 1, online pass: [N][B][T+1][kGruSaveRow] for the backward (NULL: not saved)
+  const float* h_in;   // dense rows: [E][N][H] initial state (NULL: zeros); episode rows: always zeros (the reference's hiddens=None)
+  float* h_out;        // dense rows: [E][N][H] final state (NULL: not written)
+  float* q_out;        // dense rows: [E][N][A]; episode rows: [N][B][T+1][A]
+  float* save;         // episode rows, online pass: [N][B][T+1][kGruSaveRow] for the backward (NULL: not saved)
 };
 
 // BPTT from dL/dq.  CTA c of net k (plan.cta_begin) owns a contiguous run of that net's sequences and writes the gradient sums of all eight
@@ -47,7 +47,7 @@ struct GruBwdParams {
   const float* save;                    // the online pass's saved rows
   const float* td; int td_agent_stride; // DQN: 2 * delta * filled of the taken action at [agent * stride + b * T + t]
   const float* dout;                    // actor-critic: dense dL/dout [N][B][T+1][out] (rows t < T read); non-NULL replaces td
-  RowSource src;                        // the rows the online pass read: mode 1 (each agent's observations) or 2 (joint rows, centralised critic)
+  RowSource src;                        // the rows the online pass read: kRowsEpisode (each agent's observations) or kRowsEpisodeJoint (centralised critic)
   float* scratch; int scratch_pitch;
 };
 

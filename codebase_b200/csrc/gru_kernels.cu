@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
       float v = 0.f;
       if (k < D && v0 + s < nseq) {
         int agent, unit; gru_seq(p.plan, net, v0 + s, agent, unit);
-        v = row_ptr(p.src, agent, unit, t)[k];
+        v = src_row(p.src, agent, unit, t)[k];
       }
       xs[s][k] = v;
     }
@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
       if (!live) { r = 0.f; z = 0.f; ghn = 0.f; n = 0.f; hnew[s] = 0.f; }
       if (p.save != nullptr && v0 + s0 + s < nseq) {
         int agent, unit; gru_seq(p.plan, net, v0 + s0 + s, agent, unit);
-        float* row = p.save + (((size_t)agent * B + unit) * steps + t) * kGruSaveRow;
+        float* row = p.save + row_index(agent, unit, t, B, steps) * kGruSaveRow;
         row[j] = x1[s0 + s][j]; row[kHidden + j] = r; row[2 * kHidden + j] = z; row[3 * kHidden + j] = n; row[4 * kHidden + j] = ghn; row[5 * kHidden + j] = hnew[s];
       }
     }
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_forward_kernel(GruFwdParams p
         float q = th[p.lay.b3 + a];
         for (int k = 0; k < H; ++k) q = fmaf(w3[k], hs[s][k], q);
         int agent, unit; gru_seq(p.plan, net, v0 + s, agent, unit);
-        const size_t o = src_dense_out(p.src.mode) ? ((size_t)unit * p.src.N + agent) : (((size_t)agent * B + unit) * steps + t);
+        const size_t o = out_row(p.src, agent, unit, t, B, steps);
         p.q_out[o * A + a] = q;
       }
     }
@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         float a = 0.f, b = 0.f, c = 0.f;
         if (vt + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s, agent, unit);
-          const float* row = p.save + (((size_t)agent * B + unit) * (T + 1) + t) * kGruSaveRow;
+          const float* row = p.save + row_index(agent, unit, t, B, T + 1) * kGruSaveRow;
           a = row[k]; b = row[5 * kHidden + k];
           if (t > 0) c = row[5 * kHidden + k - kGruSaveRow];
         }
@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         float v = 0.f;
         if (k < D && vt + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s, agent, unit);
-          v = row_ptr(p.src, agent, unit, t)[k];
+          v = src_row(p.src, agent, unit, t)[k];
         }
         S.x[s][k] = v;
       }
@@ -192,10 +192,9 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         if (a < A && vt + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s, agent, unit);
           if (p.dout != nullptr) {
-            v = p.dout[(((size_t)agent * B + unit) * (T + 1) + t) * A + a];
+            v = p.dout[row_index(agent, unit, t, B, T + 1) * A + a];
           } else {
-            const size_t ep = (size_t)p.idx[unit];
-            if (p.traj.act[(ep * p.traj.N + agent) * T + t] == a) v = p.td[(size_t)agent * p.td_agent_stride + (size_t)unit * T + t];
+            if (p.traj.act[p.traj.step_at(p.idx[unit], agent, t)] == a) v = p.td[(size_t)agent * p.td_agent_stride + (size_t)unit * T + t];
           }
         }
         S.dq[s][a] = v;
@@ -208,7 +207,7 @@ __global__ void __launch_bounds__(kGruThreads) gru_backward_kernel(GruBwdParams 
         float r = 0.f, z = 0.f, n = 0.f, ghn = 0.f;
         if (vt + s0 + s < v_end) {
           int agent, unit; gru_seq(p.plan, net, vt + s0 + s, agent, unit);
-          const float* row = p.save + (((size_t)agent * B + unit) * (T + 1) + t) * kGruSaveRow;
+          const float* row = p.save + row_index(agent, unit, t, B, T + 1) * kGruSaveRow;
           r = row[kHidden + j]; z = row[2 * kHidden + j]; n = row[3 * kHidden + j]; ghn = row[4 * kHidden + j];
         }
         float dh = dhc[s];
@@ -305,10 +304,10 @@ __global__ void __launch_bounds__(kGruHeadThreads) gru_ac_head_kernel(GruHeadPar
     const int rem = i - c.agent * p.P * T;
     c.b = rem / T; c.tt = rem - c.b * T; c.T = T; c.A = p.A; c.B = p.P;
     const size_t ep = (size_t)p.idx[c.b];
-    c.act = p.traj.act[(ep * p.traj.N + c.agent) * T + c.tt];
-    c.filled = (float)p.traj.filled[ep * T + c.tt];
+    c.act = p.traj.act[p.traj.step_at(ep, c.agent, c.tt)];
+    c.filled = (float)p.traj.filled[p.traj.filled_at(ep, c.tt)];
     c.rew = 0.f; c.done1 = 0.f;   // not read by the actor-critic heads
-    const size_t row = ((size_t)c.agent * p.P + c.b) * (T + 1) + c.tt;
+    const size_t row = row_index(c.agent, c.b, c.tt, p.P, T + 1);
     float dq[kOutPad];
 #pragma unroll
     for (int o = 0; o < kOutPad; ++o) dq[o] = 0.f;

@@ -167,7 +167,7 @@ __device__ __forceinline__ float grid_feature(const LbfCfgDev& c, const int8_t* 
 // contiguous in obs_out [E][N][D] and in the trajectory store, so the stores stay coalesced for any D.  Tiles: field_s / amap_s [EPC][sp],
 // pl_s [EPC][G]; meta_s[l*4+1]: env l's trajectory slot (-1: no write), meta_s[l*4+2]: the observation row it fills.
 __device__ __forceinline__ void write_grid_obs(const LbfCfgDev& c, int E, const int8_t* field_s, const int8_t* amap_s, const uint32_t* pl_s,
-                                               const int* meta_s, float* obs_out, const TrajDev& traj) {
+                                               const int* meta_s, float* obs_out, const TrajView& traj) {
   const int EPC = (kThreads / 32) * (32 / c.G), sp = c.pitch + 4, e0 = blockIdx.x * EPC, n_here = imin(EPC, E - e0);   // recomputed: nothing stays live
   const int per_env = c.N * c.D;
   for (int i = threadIdx.x; i < n_here * per_env; i += kThreads) {
@@ -175,7 +175,7 @@ __device__ __forceinline__ void write_grid_obs(const LbfCfgDev& c, int E, const 
     const float v = grid_feature(c, field_s + (size_t)l * sp, amap_s + (size_t)l * sp, pl_s[l * c.G + ag], d);
     if (obs_out) obs_out[(size_t)e0 * per_env + i] = v;
     const int sl = meta_s[l * 4 + 1];
-    if (sl >= 0) traj.obs[(((size_t)sl * c.N + ag) * (traj.T + 1) + meta_s[l * 4 + 2]) * c.D + d] = v;
+    if (sl >= 0) traj.obs_row(sl, ag, meta_s[l * 4 + 2])[d] = v;
   }
 }
 
@@ -190,7 +190,7 @@ __device__ __forceinline__ bool food_location(const LbfCfgDev& c, const int8_t* 
 
 // ---- reset kernel: one thread per env (rare: once per episode) ---------------------------------------------
 __global__ void lbf_reset_kernel(LbfCfgDev c, LbfStateDev s, int E, uint64_t seed, uint32_t gid0, const uint8_t* mask,
-                                 float* obs_out, TrajDev traj, int slot0) {
+                                 float* obs_out, TrajView traj, int slot0) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
   int8_t* f = s.field + (size_t)e * c.pitch;
@@ -203,16 +203,15 @@ __global__ void lbf_reset_kernel(LbfCfgDev c, LbfStateDev s, int E, uint64_t see
     s.step[e] = 0; s.ep_len[e] = 0; s.active[e] = 1;
     for (int i = 0; i < c.N; ++i) s.ep_return[(size_t)e * c.N + i] = 0.f;
   }
-  if (obs_out == nullptr && !(traj.enabled && doit)) return;
+  if (obs_out == nullptr && !(traj.obs && doit)) return;
   uint32_t foods[kMaxFood];
   const int nf = list_foods(c, f, foods, kMaxFood);
   float o[kMaxVecObs];
   for (int i = 0; i < c.N; ++i) {
     build_obs(c, foods, nf, pl, i, o);
     if (obs_out) for (int d = 0; d < c.D; ++d) obs_out[((size_t)e * c.N + i) * c.D + d] = o[d];
-    if (traj.enabled && doit) {  // ReplayBuffer.init_episode (dqn/train.py:65-71)
-      const size_t slot = (size_t)((slot0 + e) % traj.capacity);
-      float* dst = traj.obs + ((slot * c.N + i) * (size_t)(traj.T + 1)) * c.D;
+    if (traj.obs && doit) {  // ReplayBuffer.init_episode (dqn/train.py:65-71)
+      float* dst = traj.obs_row((slot0 + e) % traj.capacity, i, 0);
       for (int d = 0; d < c.D; ++d) dst[d] = o[d];
     }
   }
@@ -221,7 +220,7 @@ __global__ void lbf_reset_kernel(LbfCfgDev c, LbfStateDev s, int E, uint64_t see
 // ---- grid observations after a reset: lbf_reset_kernel resets the state, this kernel writes obs_out and (for the masked envs)
 // init_episode's row 0.  Same CTA shape and shared-memory layout as lbf_step_kernel<true>: field_s, pl_s, meta_s, amap_s.
 __global__ void __launch_bounds__(kThreads) lbf_grid_obs_kernel(LbfCfgDev c, LbfStateDev s, int E, const uint8_t* mask, float* obs_out,
-                                                               TrajDev traj, int slot0) {
+                                                               TrajView traj, int slot0) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int EPC = (kThreads / 32) * (32 / c.G), sp = c.pitch + 4;
   int8_t* field_s = reinterpret_cast<int8_t*>(smem_raw);
@@ -236,7 +235,7 @@ __global__ void __launch_bounds__(kThreads) lbf_grid_obs_kernel(LbfCfgDev c, Lbf
   }
   for (int l = threadIdx.x; l < n_here; l += kThreads) {
     const bool doit = (mask == nullptr) || mask[e0 + l];
-    meta_s[l * 4 + 1] = (traj.enabled && doit) ? (slot0 + e0 + l) % traj.capacity : -1;
+    meta_s[l * 4 + 1] = (traj.obs && doit) ? (slot0 + e0 + l) % traj.capacity : -1;
     meta_s[l * 4 + 2] = 0;
   }
   __syncthreads();
@@ -282,7 +281,7 @@ __global__ void lbf_get_state_kernel(LbfCfgDev c, LbfStateDev s, int E, int8_t* 
 // staging at grid widths (full sight on 8x8: 64 envs x 2 agents x 867 x 4 B = 444 KB); each env gets an int8 agent map beside its field tile
 // instead, and write_grid_obs produces the observation from the two.
 template <bool kGrid>
-__global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStateDev s, StepArgs a, TrajDev traj) {
+__global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStateDev s, StepArgs a, TrajView traj) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int G = c.G, EPW = 32 / G, EPC = (kThreads / 32) * EPW;
   // Shared-memory pitch of an env's grid = pitch + 4 bytes, i.e. an ODD number of words: the lanes of a warp work on different envs at the same cell
@@ -414,7 +413,7 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   if (env_ok && sub < c.N) a.rew_out[(size_t)e * c.N + sub] = alive ? rew_f : 0.f;
 
   int slot = -1;
-  if (traj.enabled && env_ok) slot = traj_write_scalars(traj, a, e, c.N, sub, active, step0, a_raw, rew_f, done, finished);
+  if (traj.obs && env_ok) slot = traj_write_scalars(traj, a, e, c.N, sub, active, step0, a_raw, rew_f, done, finished);
 
   // publish moved positions for the observation pass
   if (env_ok && sub < c.N) pl_s[le * G + sub] = (uint32_t)r | ((uint32_t)cc << 8) | ((uint32_t)lvl << 16);
@@ -479,11 +478,11 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
     float* dst = a.obs_out + (size_t)e0 * per_env;
     for (int i = threadIdx.x; i < n_here * per_env; i += kThreads) dst[i] = obs_s[i];
   }
-  if (traj.enabled) {
+  if (traj.obs) {
     for (int i = threadIdx.x; i < n_here * per_env; i += kThreads) {
       const int l = i / per_env, rem = i % per_env, ag = rem / c.D, d = rem % c.D;
       const int sl = meta_s[l * 4 + 1];
-      if (sl >= 0) traj.obs[(((size_t)sl * c.N + ag) * (traj.T + 1) + meta_s[l * 4 + 2]) * c.D + d] = obs_s[i];
+      if (sl >= 0) traj.obs_row(sl, ag, meta_s[l * 4 + 2])[d] = obs_s[i];
     }
   }
 }
@@ -664,11 +663,11 @@ int marl_lbf_reset(marl_lbf* h, const uint8_t* reset_mask, float* obs_out, const
   if (int rc = check_traj(h, traj)) return rc;
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   if (!h->cfg.grid_observation) {
-    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, to_traj(traj), slot0);
+    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, traj_view(traj), slot0);
   } else {   // the state here, the grid observations and init_episode's row 0 from the CTA-wide element loop of lbf_grid_obs_kernel
-    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, nullptr, to_traj(nullptr), 0);
+    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, nullptr, traj_view(nullptr), 0);
     lbf_grid_obs_kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, kThreads, h->step_smem, (cudaStream_t)stream>>>(
-        h->dev, h->st, h->E, reset_mask, obs_out, to_traj(traj), slot0);
+        h->dev, h->st, h->E, reset_mask, obs_out, traj_view(traj), slot0);
   }
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;

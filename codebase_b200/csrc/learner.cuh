@@ -2,17 +2,13 @@
 // forward+loss-head+backward training pass, deterministic gradient reduction, clip + Adam + target update.
 #pragma once
 #include "mlp.cuh"
+#include "traj.cuh"
 #include <string.h>
 
 namespace marl {
 
 constexpr int kMaxObsDim = 32;   // tensor-core paths and the DQN family: KP = 16 or 32 float input tiles
 constexpr int kMaxInDim = 128;   // FP32 MLP kernels (actor-critic learners: KP = 64 / 128 tiles above 32) and the GRU kernels
-
-struct TrajView {  // device view of marl_traj_view
-  const float* obs; const int32_t* act; const float* rew; const uint8_t* done; const uint8_t* filled;
-  int capacity, N, T, D;
-};
 
 // Which rows a launch covers and how CTAs split them.  A "unit" is an indivisible run of rows that must stay inside
 // one CTA: one sampled episode (T+1 rows) for training passes, one row for plain inference.
@@ -25,17 +21,27 @@ struct RowPlan {
   int units_per_agent;                  // B (episodes) or E (envs)
 };
 
+// Where a launch's observation rows come from.  The JOINT modes are observation rows shared by all agents (centralised critic,
+// ac/model.py:62-65,156-157: every agent's critic sees the concatenation of all agents' observations; D = their total width).
+enum RowMode {
+  kRowsDense = 0,         // dense obs float[E][N][D]: one row per (unit = env, agent); outputs [E][N]
+  kRowsEpisode = 1,       // the trajectory store's episodes idx[unit]; outputs and loss scalars per row (row_index)
+  kRowsEpisodeJoint = 2,  // joint rows float[units][T+1][D], outputs like kRowsEpisode, loss scalars from the trajectory store
+  kRowsDenseJoint = 3     // joint rows float[E][D]: the dense obs array read as [E][N * D_agent]; outputs like kRowsDense
+};
 struct RowSource {
-  // 0: dense obs float[E][N][D];  1: gather from the trajectory store through episode indices;
-  // 2 / 3: JOINT observation rows float[units][unit_rows][D] shared by all agents (centralised critic, ac/model.py:62-65,156-157: every agent's critic
-  //        sees the concatenation of all agents' observations; D = their total width): 2 = outputs laid out like mode 1 ([agent][unit][row], loss
-  //        scalars from the trajectory store), 3 = like mode 0 ([unit][agent]; `joint` is then simply the dense obs array read as [E][N * D_agent])
-  int mode;
+  int mode;   // RowMode
   const float* dense; int E, N, D;
   TrajView traj; const int32_t* idx;  // idx[B] ring slots (device)
   const float* joint;
 };
-__host__ __device__ __forceinline__ bool src_dense_out(int mode) { return mode == 0 || mode == 3; }
+__host__ __device__ __forceinline__ bool src_dense_out(int mode) { return mode == kRowsDense || mode == kRowsDenseJoint; }
+
+// The learner's per-row buffers (target outputs, Q-values, values, logits, GRU saved rows, tensor-core activations and records) are laid out
+// [agent][units_per_agent][unit_rows]: the index of row `off` of unit `unit` of `agent`
+__host__ __device__ __forceinline__ size_t row_index(int agent, int unit, int off, int units_per_agent, int unit_rows) {
+  return ((size_t)agent * units_per_agent + unit) * unit_rows + off;
+}
 
 __device__ __forceinline__ void cta_rows(const RowPlan& p, int& net, int& row_begin, int& row_end) {
   net = 0;
@@ -55,11 +61,17 @@ __device__ __forceinline__ void decode_row(const RowPlan& p, int net, int vr, in
   off = rem - unit * p.unit_rows;
 }
 
-__device__ __forceinline__ const float* row_ptr(const RowSource& s, int agent, int unit, int off) {
-  if (s.mode == 0) return s.dense + ((size_t)unit * s.N + agent) * s.D;
-  if (s.mode >= 2) return s.joint + ((size_t)unit * (s.mode == 2 ? s.traj.T + 1 : 1) + off) * s.D;   // (unit_rows: T + 1 when training, 1 for plain inference)
-  const size_t ep = (size_t)s.idx[unit];
-  return s.traj.obs + ((ep * s.traj.N + agent) * (size_t)(s.traj.T + 1) + off) * s.traj.D;
+// Observation row of (agent, unit, row off of the unit).  Independent of the plan: an episode's rows are its T + 1 steps, a dense unit has one
+// row (off == 0).
+__device__ __forceinline__ const float* src_row(const RowSource& s, int agent, int unit, int off) {
+  if (s.mode == kRowsDense) return s.dense + ((size_t)unit * s.N + agent) * s.D;
+  if (s.mode != kRowsEpisode) return s.joint + ((size_t)unit * (s.mode == kRowsEpisodeJoint ? s.traj.T + 1 : 1) + off) * s.D;
+  return s.traj.obs_row(s.idx[unit], agent, off);
+}
+
+// Where the outputs of a row go: [unit][N] for the dense sources, the per-row layout (row_index) otherwise
+__device__ __forceinline__ size_t out_row(const RowSource& s, int agent, int unit, int off, int units_per_agent, int unit_rows) {
+  return src_dense_out(s.mode) ? (size_t)unit * s.N + agent : row_index(agent, unit, off, units_per_agent, unit_rows);
 }
 
 // Per-tile row metadata staged in shared memory by the first 128 threads (one row each): the source pointer of the
@@ -81,19 +93,13 @@ __device__ __forceinline__ void setup_rows(RowMeta* m, const RowPlan& p, const R
   if (r < nrows) {
     int agent, unit, off;
     decode_row(p, net, vr0 + r, agent, unit, off);
-    if (s.mode == 0) {
-      src = s.dense + ((size_t)unit * s.N + agent) * s.D;
-    } else if (s.mode == 3) {
-      src = s.joint + ((size_t)unit * p.unit_rows + off) * s.D;
-    } else {
+    src = src_row(s, agent, unit, off);
+    const TrajView& tv = s.traj;
+    if (kWithScalars && !src_dense_out(s.mode) && off < tv.T) {
       const size_t ep = (size_t)s.idx[unit];
-      const TrajView& tv = s.traj;
-      src = s.mode == 2 ? s.joint + ((size_t)unit * p.unit_rows + off) * s.D : tv.obs + ((ep * tv.N + agent) * (size_t)(tv.T + 1) + off) * tv.D;
-      if (kWithScalars && off < tv.T) {
-        act = tv.act[(ep * tv.N + agent) * tv.T + off];
-        rew = tv.rew[(ep * tv.N + agent) * tv.T + off];
-        flags = (int)tv.filled[ep * tv.T + off] | ((int)tv.done[ep * (tv.T + 1) + off + 1] << 1);
-      }
+      act = tv.act[tv.step_at(ep, agent, off)];
+      rew = tv.rew[tv.step_at(ep, agent, off)];
+      flags = (int)tv.filled[tv.filled_at(ep, off)] | ((int)tv.done[tv.done_at(ep, off + 1)] << 1);
     }
   }
   m->src[r] = src; m->act[r] = act; m->rew[r] = rew; m->flags[r] = flags;
@@ -116,7 +122,7 @@ struct FwdParams {
   RowPlan plan; RowSource src;
   const float* theta;   // [n_nets][P]
   NetLayout lay;
-  float* out;           // mode 0: [E][N][out]; mode 1: [N][B][T+1][out]
+  float* out;           // dense sources: [E][N][out]; the others: [N][B][T+1][out] (out_row)
 };
 
 // Loss heads of the fused training kernel (what happens between the forward and the backward of a tile).
@@ -274,24 +280,18 @@ inline RowPlan episode_plan(const NetSet& ns, int episodes, int T, int n_cta_max
   return make_plan(ns, episodes, T + 1, n_cta_max, min_units);
 }
 
-inline TrajView to_view(const marl_traj_view* t) {
-  TrajView v; v.obs = t->obs; v.act = t->act; v.rew = t->rew; v.done = t->done; v.filled = t->filled;
-  v.capacity = t->capacity; v.N = t->n_agents; v.T = t->T; v.D = t->obs_dim;
-  return v;
-}
-
-// Dense rows obs float[E][N][D] (mode 0).  joint: a centralised critic's rows (mode 3), obs float[E][N][D_agent] read as float[E][D = N * D_agent].
+// Dense rows obs float[E][N][D].  joint: a centralised critic's rows, obs float[E][N][D_agent] read as float[E][D = N * D_agent].
 inline RowSource dense_rows(const float* obs, int E, int N, int D, bool joint = false) {
   RowSource s; memset(&s, 0, sizeof(s));
-  s.mode = joint ? 3 : 0; s.dense = obs; s.E = E; s.N = N; s.D = D;
+  s.mode = joint ? kRowsDenseJoint : kRowsDense; s.dense = obs; s.E = E; s.N = N; s.D = D;
   if (joint) s.joint = obs;
   return s;
 }
 
-// Rows of the episodes idx[] of a trajectory store (mode 1)
+// Rows of the episodes idx[] of a trajectory store
 inline RowSource episode_rows(const marl_traj_view* t, const int32_t* idx, int N, int D) {
   RowSource s; memset(&s, 0, sizeof(s));
-  s.mode = 1; s.traj = to_view(t); s.idx = idx; s.N = N; s.D = D;
+  s.mode = kRowsEpisode; s.traj = traj_view(t); s.idx = idx; s.N = N; s.D = D;
   return s;
 }
 
@@ -310,7 +310,7 @@ int launch_tc_forward(const FwdParams& p, const uint8_t* images, cudaStream_t st
 struct TcBuffers {
   uint8_t* image; uint8_t* bwd_image;       // packed online-network images (forward K-major, backward K-major W2^T)
   float *h1, *h2;                           // [128][rows] (feature-major) activations
-  float* rec;                               // [rows][16] row records (tc_train.cu)
+  float* rec;                               // [rows][kRowRec] row records (tc_train.cu)
   float* x;                                 // [rows][kMaxObsDim] gathered observation rows
   size_t rows;                              // allocated rows
 };

@@ -47,9 +47,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_forward_kernel(FwdParams p
       const int r = i / p.lay.out, o = i - r * p.lay.out;
       int agent, unit, off;
       decode_row(p.plan, net, vr0 + r, agent, unit, off);
-      const size_t dst = src_dense_out(p.src.mode) ? ((size_t)unit * p.src.N + agent)
-                                         : (((size_t)agent * p.plan.units_per_agent + unit) * p.plan.unit_rows + off);
-      p.out[dst * p.lay.out + o] = Q[r * kOutPad + o];
+      p.out[out_row(p.src, agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows) * p.lay.out + o] = Q[r * kOutPad + o];
     }
   }
 }
@@ -236,7 +234,7 @@ __device__ __forceinline__ void head_dqn(const TrainParams& p, const RowCtx& c, 
   if (p.td_ext) {  // VDN, QMIX, standardise_returns: the TD error came from the column TD kernel or the mixer
     g = p.td_ext[(size_t)c.agent * p.td_agent_stride + (size_t)c.b * c.T + c.tt];
   } else {
-    const float* tq = p.tq + (((size_t)c.agent * c.B + c.b) * (c.T + 1) + c.tt + 1) * c.A;
+    const float* tq = p.tq + (row_index(c.agent, c.b, c.tt, c.B, c.T + 1) + 1) * c.A;   // the next row's target outputs
     g = td_error(q[act], td_target(c.rew, p.gamma, next_value(qn, tq, c.A, p.double_q), c.done1), c.filled, c.agent == 0, st[0], st[1]);
   }
 #pragma unroll

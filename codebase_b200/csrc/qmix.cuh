@@ -234,15 +234,15 @@ __device__ __forceinline__ void qm_load_inputs(const QmSmem& sm, const QmixParam
   const QmixLayout& L = p.L;
   const int T = p.traj.T;
   for (int a = 0; a < L.N; ++a) {
-    const float* ob = p.traj.obs + ((ep * L.N + a) * (T + 1) + t + dt) * p.D;
+    const float* ob = p.traj.obs_row(ep, a, t + dt);
     for (int d = warp; d < p.D; d += kQmWarps) sm.X[(a * p.D + d) * kQmP + lane] = live ? ob[d] : 0.f;
   }
   for (int a = warp; a < L.N; a += kQmWarps) {
     float v = 0.f;
     if (live) {
-      const size_t row = ((size_t)a * p.B + b) * (T + 1) + t + dt;
+      const size_t row = row_index(a, b, t + dt, p.B, T + 1);
       const float* q1 = p.q + row * p.A;
-      if (dt == 0) v = q1[p.traj.act[(ep * L.N + a) * T + t]];
+      if (dt == 0) v = q1[p.traj.act[p.traj.step_at(ep, a, t)]];
       else v = next_value(q1, p.tq + row * p.A, p.A, p.double_q);
     }
     sm.QA[a * kQmP + lane] = v;
@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
   if constexpr (MODE == 1) {   // the target mixer's output de-standardised with the statistics so far (dqn/model.py:415-418), no FMA contraction
     if (live && warp == 0) {
       const float tq = unstandardise(ytgt, p.ret_ms[b], p.ret_ms[p.n_stat + b]);
-      p.ret[s] = td_target_rn(p.traj.rew[(ep * L.N + 0) * T + t], p.gamma, tq, (float)p.traj.done[ep * (T + 1) + t + 1]);
+      p.ret[s] = td_target_rn(p.traj.rew[p.traj.step_at(ep, 0, t)], p.gamma, tq, (float)p.traj.done[p.traj.done_at(ep, t + 1)]);
     }
   } else {
     // ---- online ----
@@ -292,10 +292,10 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
     float y;
     if constexpr (HL == 2) y = qm_forward(sm, L, warp, lane);
     else y = qm_forward1(sm, L, img + L.w1b, warp, lane);
-    const float filled = live ? (float)p.traj.filled[ep * T + t] : 0.f;
+    const float filled = live ? (float)p.traj.filled[p.traj.filled_at(ep, t)] : 0.f;
     float ret;
     if constexpr (MODE == 2) ret = live ? p.ret[s] : 0.f;
-    else ret = live ? td_target(p.traj.rew[(ep * L.N + 0) * T + t], p.gamma, ytgt, (float)p.traj.done[ep * (T + 1) + t + 1]) : 0.f;
+    else ret = live ? td_target(p.traj.rew[p.traj.step_at(ep, 0, t)], p.gamma, ytgt, (float)p.traj.done[p.traj.done_at(ep, t + 1)]) : 0.f;
     const float delta = live ? y - ret : 0.f, dy = 2.f * delta * filled;
     float* rc = p.rec + s;   // this sample's column of the field-major record
     if (live) {

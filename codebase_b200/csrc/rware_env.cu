@@ -98,7 +98,7 @@ __device__ void build_obs(const RwCfgDev& c, const uint8_t* sh, const uint32_t* 
 }
 
 // ---- reset / state kernels: one thread per env (rare) ------------------------------------------------------------
-__global__ void rware_reset_kernel(RwCfgDev c, RwStateDev s, int E, uint64_t seed, uint32_t gid0, const uint8_t* mask, float* obs_out, TrajDev traj,
+__global__ void rware_reset_kernel(RwCfgDev c, RwStateDev s, int E, uint64_t seed, uint32_t gid0, const uint8_t* mask, float* obs_out, TrajView traj,
                                    int slot0) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
@@ -115,7 +115,7 @@ __global__ void rware_reset_kernel(RwCfgDev c, RwStateDev s, int E, uint64_t see
   }
   for (int i = 0; i < c.N; ++i) {
     if (obs_out) build_obs(c, sh, ag, req, i, obs_out + ((size_t)e * c.N + i) * c.D);
-    if (traj.enabled && doit) build_obs(c, sh, ag, req, i, traj.obs + (((size_t)((slot0 + e) % traj.capacity) * c.N + i) * (traj.T + 1)) * c.D);
+    if (traj.obs && doit) build_obs(c, sh, ag, req, i, traj.obs_row((slot0 + e) % traj.capacity, i, 0));
   }
 }
 
@@ -153,7 +153,7 @@ __host__ __device__ inline size_t rware_warp_smem(int N, int D, int pitch) {
 }
 
 // ---- the transition kernel ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwStateDev s, StepArgs a, TrajDev traj) {
+__global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwStateDev s, StepArgs a, TrajView traj) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr uint32_t FULL = 0xFFFFFFFFu;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwSt
     if (finished && a.final_ret) a.final_ret[(size_t)e * c.N + lane] = ep_ret;
   }
   if (agent) a.rew_out[(size_t)e * c.N + lane] = alive ? rew_f : 0.f;
-  const int slot = traj.enabled ? traj_write_scalars(traj, a, e, c.N, lane, active, step0, a_raw, rew_f, done, finished) : -1;
+  const int slot = traj.obs ? traj_write_scalars(traj, a, e, c.N, lane, active, step0, a_raw, rew_f, done, finished) : -1;
 
   if (lane == 0) {
     if (active) {
@@ -343,9 +343,11 @@ __global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwSt
     for (int i = lane; i < per_env; i += 32) dst[i] = obs_s[i];
   }
   if (slot >= 0) {   // warp-uniform
+    // the config's N and D, which check_traj requires the view's to equal: this kernel holds them already, and the view's own make ptxas spill
+    TrajView tv = traj; tv.N = c.N; tv.D = c.D;
     for (int i = lane; i < per_env; i += 32) {
       const int ag = i / c.D, dd = i - ag * c.D;
-      traj.obs[(((size_t)slot * c.N + ag) * (traj.T + 1) + step1) * c.D + dd] = obs_s[i];
+      tv.obs_row(slot, ag, step1)[dd] = obs_s[i];
     }
   }
 }
@@ -503,7 +505,7 @@ int marl_rware_reset(marl_rware* h, const uint8_t* reset_mask, float* obs_out, c
   MARL_REQUIRE(h != nullptr, "marl_rware_reset: NULL handle");
   if (int rc = check_traj(h, traj)) return rc;
   MARL_CUDA_TRY(cudaSetDevice(h->device));
-  rware_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, to_traj(traj), slot0);
+  rware_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, traj_view(traj), slot0);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }

@@ -196,6 +196,15 @@ __device__ __forceinline__ void layer_rs(float (&d)[64], uint32_t (&ahi)[KSTEPS]
 // Thread (warp w of the warpgroup, lane): rows 16 w + lane / 4 (element bit 1 clear) and + 8 (set); element i holds column 8 (i / 4) + 2 (lane % 4)
 // + (i & 1).  Element pairs (4 ks, 4 ks + 2) / (4 ks + 1, 4 ks + 3) are exactly the A fragment of K step ks in the permuted K order (kperm).
 __device__ __forceinline__ int frag_col(int i, int quad_lane) { return 8 * (i >> 2) + 2 * quad_lane + (i & 1); }
+// this thread's A fragment of layer 1: observation columns 8 ks + 2 t and + 1 of its two rows (zero beyond D or past the last row)
+__device__ __forceinline__ void load_x_frag(const float* s0, const float* s1, int D, int quad_lane, float (&x)[kMaxObsDim / 8][4]) {
+#pragma unroll
+  for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {
+    const int c = 8 * ks + 2 * quad_lane;
+    x[ks][0] = (s0 && c < D) ? s0[c] : 0.f; x[ks][1] = (s1 && c < D) ? s1[c] : 0.f;
+    x[ks][2] = (s0 && c + 1 < D) ? s0[c + 1] : 0.f; x[ks][3] = (s1 && c + 1 < D) ? s1[c + 1] : 0.f;
+  }
+}
 // values of a 64 x 128 fragment -> A operand registers (hi / lo) of the next product
 __device__ __forceinline__ void frag_to_a(const float (&v)[64], uint32_t (&hi)[16][4], uint32_t (&lo)[16][4]) {
 #pragma unroll

@@ -35,29 +35,14 @@ __global__ void pack_weights_kernel(const float* __restrict__ theta, NetLayout l
   if (i < lay.P) pack_param(lay, i, th[i], img, bwd);
 }
 
-// observation row of a virtual row and where its outputs go (modes of RowSource)
+// observation row of a virtual row and where its outputs go
 __device__ __forceinline__ const float* fwd_src_row(const FwdParams& p, int net, int vr, size_t& dst) {
   int agent, unit, off;
   decode_row(p.plan, net, vr, agent, unit, off);
-  dst = src_dense_out(p.src.mode) ? ((size_t)unit * p.src.N + agent) : (((size_t)agent * p.plan.units_per_agent + unit) * p.plan.unit_rows + off);
-  const int D = p.src.D;
-  if (p.src.mode == 0) return p.src.dense + ((size_t)unit * p.src.N + agent) * D;
-  if (p.src.mode == 1) {
-    const TrajView& tv = p.src.traj;
-    return tv.obs + (((size_t)p.src.idx[unit] * tv.N + agent) * (size_t)(tv.T + 1) + off) * D;
-  }
-  return p.src.joint + ((size_t)unit * p.plan.unit_rows + off) * D;   // joint rows (centralised critic)
+  dst = out_row(p.src, agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows);
+  return src_row(p.src, agent, unit, off);
 }
 
-// this thread's A fragment of layer 1: observation columns 8 ks + 2 t and + 1 of its two rows (zero beyond D or past the last row)
-__device__ __forceinline__ void load_x_frag(const float* s0, const float* s1, int D, int quad_lane, float (&x)[kMaxObsDim / 8][4]) {
-#pragma unroll
-  for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {
-    const int c = 8 * ks + 2 * quad_lane;
-    x[ks][0] = (s0 && c < D) ? s0[c] : 0.f; x[ks][1] = (s1 && c < D) ? s1[c] : 0.f;
-    x[ks][2] = (s0 && c + 1 < D) ? s0[c + 1] : 0.f; x[ks][3] = (s1 && c + 1 < D) ? s1[c + 1] : 0.f;
-  }
-}
 // A fragment order: (row 0, K t) = column 2t, (row 1, K t), (row 0, K t + 4) = column 2t + 1, (row 1, K t + 4)
 __device__ __forceinline__ void x_to_a(const float (&x)[kMaxObsDim / 8][4], uint32_t (&hi)[kMaxObsDim / 8][4], uint32_t (&lo)[kMaxObsDim / 8][4]) {
 #pragma unroll

@@ -16,13 +16,12 @@
 
 namespace marl {
 
-// observation row of a virtual row of the training batch and the row's index in the [agent][unit][T + 1] layout of every per-row buffer
+// observation row of a virtual row of the training batch (episode rows only: launch_tc_dqn_train) and the row's index in every per-row buffer
 __device__ __forceinline__ const float* train_row(const TcTrainParams& p, int net, int vr, size_t& d, int& agent, int& unit, int& off, int& ep) {
   decode_row(p.plan, net, vr, agent, unit, off);
-  d = ((size_t)agent * p.plan.units_per_agent + unit) * p.plan.unit_rows + off;
-  const TrajView& tv = p.src.traj;
+  d = row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows);
   ep = p.src.idx[unit];
-  return tv.obs + (((size_t)ep * tv.N + agent) * (size_t)(tv.T + 1) + off) * p.src.D;
+  return p.src.traj.obs_row(ep, agent, off);
 }
 
 // The weight gradients contract over rows, so both operands of each are staged K-major (one 128-byte swizzled line of 32 rows per feature),
@@ -48,15 +47,6 @@ TSG_DEFINE(g_ts_dh1)
 TSG_GETTER(tsg_dh1, g_ts_dh1)
 TSG_DEFINE(g_ts_dw)
 TSG_GETTER(tsg_dw, g_ts_dw)
-
-__device__ __forceinline__ void load_x_frag_t(const float* s0, const float* s1, int D, int quad_lane, float (&x)[kMaxObsDim / 8][4]) {
-#pragma unroll
-  for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {
-    const int c = 8 * ks + 2 * quad_lane;
-    x[ks][0] = (s0 && c < D) ? s0[c] : 0.f; x[ks][1] = (s1 && c < D) ? s1[c] : 0.f;
-    x[ks][2] = (s0 && c + 1 < D) ? s0[c + 1] : 0.f; x[ks][3] = (s1 && c + 1 < D) ? s1[c + 1] : 0.f;
-  }
-}
 
 // store a 64 x 128 fragment feature-major (dst[j * rows + row]) and its ReLU mask words (rec field `mask`); rows of a missing source (d < 0)
 // are skipped
@@ -104,7 +94,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
     {
       float x[kMaxObsDim / 8][4];
       uint32_t xhi[kMaxObsDim / 8][4], xlo[kMaxObsDim / 8][4];
-      load_x_frag_t(s0, s1, D, tq, x);
+      load_x_frag(s0, s1, D, tq, x);
 #pragma unroll
       for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {   // the gathered row for the weight-gradient kernel
         const int c = 8 * ks + 2 * tq;
@@ -165,10 +155,10 @@ __device__ __forceinline__ float td_grad(const TcTrainParams& p, size_t d, int a
   const int T = tv.T, A = p.lay.out;
   act = 0;
   if (tt >= T) return 0.f;
-  act = tv.act[((size_t)ep * tv.N + agent) * T + tt];
+  act = tv.act[tv.step_at(ep, agent, tt)];
   if (p.td_ext) return p.td_ext[(size_t)agent * p.td_agent_stride + (size_t)b * T + tt];
-  const float rew = tv.rew[((size_t)ep * tv.N + agent) * T + tt];
-  const float filled = (float)tv.filled[(size_t)ep * T + tt], done1 = (float)tv.done[(size_t)ep * (T + 1) + tt + 1];
+  const float rew = tv.rew[tv.step_at(ep, agent, tt)];
+  const float filled = (float)tv.filled[tv.filled_at(ep, tt)], done1 = (float)tv.done[tv.done_at(ep, tt + 1)];
   const float* q = p.rec + d * kRowRec;
   const float* qn = q + kRowRec;                 // the next row of the same episode
   const float* tq = p.tq + (d + 1) * A;          // target outputs share the [agent][unit][T + 1] row layout
@@ -403,7 +393,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
       if (vr < row_end) {
         int agent, unit, off;
         decode_row(p.plan, net, vr, agent, unit, off);
-        d = ((long long)agent * p.plan.units_per_agent + unit) * p.plan.unit_rows + off;
+        d = (long long)row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows);
         const float* rp = p.rec + (size_t)d * kRowRec;
         gr = rp[kRecG]; act = __float_as_int(rp[kRecAct]);
       }
