@@ -44,6 +44,14 @@ class RwareCfg(C.Structure):
     ]
 
 
+class MatrixCfg(C.Structure):
+    _fields_ = [
+        ("n_agents", C.c_int32), ("n_actions", C.c_int32), ("payoff", C.POINTER(C.c_double)), ("ep_length", C.c_int32),
+        ("last_action_state", C.c_int32), ("time_limit", C.c_int32), ("cooperative_reward", C.c_int32), ("observe_id", C.c_int32),
+        ("standardise_rewards", C.c_int32),
+    ]
+
+
 class TrajView(C.Structure):
     _fields_ = [
         ("obs", C.c_void_p), ("act", C.c_void_p), ("rew", C.c_void_p), ("done", C.c_void_p), ("filled", C.c_void_p),

@@ -1,5 +1,6 @@
 // render.cuh -- the frame rasteriser the env render kernels share (sm_90a): palette and geometry, filled disc / rectangle / line primitives,
-// a 3x5 bitmap digit font, and the band loop that writes a frame's pixel rows.  Included by lbf_env.cu and rware_env.cu.  Semantics: DESIGN.md
+// a 3x5 bitmap digit font, and the band loop that writes a frame's pixel rows.  Included by the env kernels (lbf_env.cu, rware_env.cu,
+// matrix_env.cu).  Semantics: DESIGN.md
 // §4.8; oracle: tests/render_ref.py.
 //
 // Integer arithmetic only, so that a numpy restatement reproduces every frame bit for bit.  A frame of a rows x cols board with g-pixel cells is
@@ -33,6 +34,10 @@ __device__ constexpr Rgb kRwGoal{60, 60, 60};                 // (recalled)
 __device__ constexpr Rgb kRwShelf{72, 61, 139}, kRwShelfRequested{0, 128, 128};   // (recalled)
 __device__ constexpr Rgb kRwAgent{255, 140, 0}, kRwAgentLoaded{255, 0, 0};        // (recalled)
 __device__ constexpr Rgb kRwDir{0, 0, 0};                     // (recalled)
+
+// ---- matrix games (our own: upstream has no rgb_array renderer): one row per player, one column per action ----
+constexpr int kMxCell = 40;                        // px per cell
+__device__ constexpr Rgb kMxChosen{46, 104, 190};  // fills the cell of each player's previous action
 
 // ---- digits: 3x5 glyphs, bit 14 - (3*row + col) set for an inked pixel, drawn kFontScale px per glyph pixel, kDigitGap px apart ----
 constexpr int kFontScale = 2, kDigitGap = 2;

@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from ..lbf import LbfConfig, NativeLbf, parse_env_id
+from ..matrix import MatrixConfig, NativeMatrix, is_matrix_id, parse_matrix_id
 from ..rware import NativeRware, RwareConfig, is_rware_id, parse_rware_id
 from . import spaces
 
@@ -31,10 +32,12 @@ class _Unwrapped:
 
 
 class B200VecEnv:
-    def __init__(self, cfg: LbfConfig | RwareConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None, flatten: bool = False):
+    def __init__(self, cfg: LbfConfig | RwareConfig | MatrixConfig, parallel_envs: int, seed: int, env_gid0: int = 0, device=None,
+                 flatten: bool = False):
         """`flatten`: the FlattenObservation wrapper (marlbase/utils/wrappers.py:48-72), whose Box is unbounded."""
         self.cfg, self.num_envs = cfg, int(parallel_envs)
-        self.native = (NativeRware if isinstance(cfg, RwareConfig) else NativeLbf)(cfg, self.num_envs, seed, env_gid0, device)
+        handle = NativeRware if isinstance(cfg, RwareConfig) else NativeMatrix if isinstance(cfg, MatrixConfig) else NativeLbf
+        self.native = handle(cfg, self.num_envs, seed, env_gid0, device)
         self.n_agents = cfg.n_agents
         self.unwrapped = _Unwrapped(cfg.n_agents)
         lo, hi = (-np.inf, np.inf) if flatten else cfg.obs_bounds
@@ -99,14 +102,15 @@ def episode_info(returns, length, seconds):
 def make_env(seed, enable_video=False, name=None, time_limit=None, clear_info=False, observe_id=False, standardise_rewards=False,
              wrappers=None, parallel_envs=None, env_gid0=0, device=None, **kwargs):
     """marlbase/utils/envs.py:115-119 with the same config keys.  `parallel_envs` absent -> 1 env (the reference's single-env
-    factory); the GPU overlays set it to thousands.  `name`: a Level-Based Foraging id (codebase_b200.lbf) or a multi-robot warehouse id
-    (codebase_b200.rware); extra keys override the env's constructor arguments.  `enable_video` is accepted and changes nothing: every native env
+    factory); the GPU overlays set it to thousands.  `name`: a Level-Based Foraging id (codebase_b200.lbf), a multi-robot warehouse id
+    (codebase_b200.rware) or a matrix game id (codebase_b200.matrix); extra keys override the env's constructor arguments.  `enable_video` is accepted and changes nothing: every native env
     renders (B200VecEnv.render)."""
     wrappers = list(wrappers or [])
     unknown = [w for w in wrappers if w not in SUPPORTED_WRAPPERS]
     if unknown:
         raise NotImplementedError(f"env.wrappers {unknown} are not implemented on the GPU path (supported: {sorted(SUPPORTED_WRAPPERS)})")
-    cfg = (parse_rware_id if is_rware_id(name) else parse_env_id)(name, time_limit or 0, **kwargs)
+    parse = parse_rware_id if is_rware_id(name) else parse_matrix_id if is_matrix_id(name) else parse_env_id
+    cfg = parse(name, time_limit or 0, **kwargs)
     flatten = "FlattenObservation" in wrappers
     if getattr(cfg, "grid_observation", 0):
         if observe_id:   # ObserveID wraps before env.wrappers (envs.py:98-99), so it meets the (3, W, W) Box and asserts (wrappers.py:79-82)

@@ -208,6 +208,50 @@ int marl_rware_frame_shape(const marl_rware_cfg* cfg, int32_t* h, int32_t* w);
 int marl_rware_render(marl_rware* env, int32_t env_first, int32_t n, uint8_t* frames, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
+ * Repeated matrix games (the `matrixgames` package: climbing, penalty-k), E environments per handle, one transition of all of them per launch.
+ * Replaces `env.reset()` / `env.step(actions)` of the gym.make()'d `matrixgames` MatrixGame under the same wrapper stack as marl_lbf_*.
+ * Semantics: DESIGN.md Appendix C.  Every player has the same action count A; the reward of a step is payoff[a_0, ..., a_{N-1}] for every
+ * player.  The entry points mirror the marl_rware_* contracts; the trajectory view and the rollout arguments are the same structs.
+ * ---------------------------------------------------------------------------------------------------- */
+typedef struct {
+  int32_t n_agents;                   /* players N = payoff.ndim, 1..32 */
+  int32_t n_actions;                  /* actions A of every player, 1..8, with A^N <= 65536 */
+  const double* payoff;               /* HOST pointer to the A^N payoffs in C order (entry sum_i a_i * A^(N-1-i)); create copies them */
+  int32_t ep_length;                  /* terminates when the step count reaches it; >= 1 (25 for the registered ids) */
+  int32_t last_action_state;          /* 1: observation = one-hot of every player's previous action (N * A), all zero after a reset;
+                                         0 (`-nostate` ids): one constant feature, 0 */
+  int32_t time_limit;                 /* TimeLimit wrapper (truncates); 0 = absent */
+  int32_t cooperative_reward;         /* CooperativeReward wrapper */
+  int32_t observe_id;                 /* ObserveID wrapper: one-hot agent id in front of every observation */
+  int32_t standardise_rewards;        /* StandardiseReward wrapper, as marl_lbf_cfg.standardise_rewards */
+} marl_matrix_cfg;
+
+typedef struct marl_matrix marl_matrix;
+
+int marl_matrix_create(const marl_matrix_cfg* cfg, int32_t n_envs, uint64_t seed, uint32_t env_gid0, int32_t device, marl_matrix** out);
+int marl_matrix_destroy(marl_matrix* env);
+int marl_matrix_obs_dim(const marl_matrix_cfg* cfg);   /* N * A with last_action_state, else 1 (+ n_agents with observe_id) */
+/* Overwrite the transition state (device pointers): last_action int8[E][N] (each player's previous action, -1: none, as after a reset),
+ * step int32[E] (steps so far).  Episode returns and lengths restart at 0. */
+int marl_matrix_set_state(marl_matrix* env, const int8_t* last_action, const int32_t* step, void* stream);
+/* Copy the state out into caller-owned DEVICE buffers (any may be NULL), in the layout of marl_matrix_set_state plus ep_return float[E][N],
+ * ep_len int32[E], episode_idx uint32[E], active uint8[E]. */
+int marl_matrix_get_state(marl_matrix* env, int8_t* last_action, int32_t* step, float* ep_return, int32_t* ep_len, uint32_t* episode_idx,
+                          uint8_t* active, void* stream);
+/* as marl_lbf_reset; a reset draws nothing */
+int marl_matrix_reset(marl_matrix* env, const uint8_t* reset_mask, float* obs_out, const marl_traj_view* traj, int32_t slot0, void* stream);
+/* as marl_lbf_step; an action outside 0..A-1 is played as action 0 */
+int marl_matrix_step(marl_matrix* env, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,
+                     float* final_ret_out, int32_t* final_len_out, int32_t autoreset, void* stream);
+/* as marl_lbf_rollout_step (policy 1 or 2); args->n_actions must equal A */
+int marl_matrix_rollout_step(marl_matrix* env, const float* values, const marl_rollout_args* args, const marl_traj_view* traj,
+                             float* obs_inout, float* rew_out, uint8_t* done_out, uint8_t* trunc_out, float* final_ret_out,
+                             int32_t* final_len_out, int32_t* actions_out, void* stream);
+/* as marl_lbf_frame_shape / marl_lbf_render: an N x A board of 40-px cells, h = 1 + N * 41, w = 1 + A * 41 */
+int marl_matrix_frame_shape(const marl_matrix_cfg* cfg, int32_t* h, int32_t* w);
+int marl_matrix_render(marl_matrix* env, int32_t env_first, int32_t n, uint8_t* frames, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------
  * Per-agent MLP sets and the DQN-family learner (IDQN, VDN).
  * Replaces marlbase/dqn/model.py QNetwork (14-196) / VDNetwork (199-269) and the network containers of
  * marlbase/utils/models.py:133-300.  Parameters are one flat float array [n_nets][P] in the reference's
