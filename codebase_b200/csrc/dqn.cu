@@ -99,7 +99,7 @@ struct marl_dqn : LearnerHandle {
   bool grads_are_local = false;  // set by update_grads, cleared when the caller may have all-reduced grad
   uint8_t* image_tgt = nullptr;  // image of theta_tgt, rebuilt only when the target network changed
   uint8_t* image_bwd = nullptr;  // MN-major image of W2 (online net) for the tensor-core backward
-  float *tc_h1 = nullptr, *tc_h2 = nullptr, *tc_rec = nullptr, *tc_x = nullptr;
+  float *tc_h2 = nullptr, *tc_rec = nullptr, *tc_x = nullptr;
   bool tgt_image_current = false;
   unsigned long long* grid_barrier = nullptr; unsigned long long grid_epoch = 0;   // arrival counter of the fused reduce + Adam kernel
   unsigned long long push_epoch = 0;   // arrival counter of the push kernel (split exchange)
@@ -472,10 +472,10 @@ static int dqn_train_pass(marl_dqn* h, const TrainParams& tp, cudaEvent_t* betwe
     return launch_gru_backward(bp, st);
   }
   if (!tc_backward_enabled() || h->ns.in >= kMaxObsDim || h->image == nullptr) return launch_train(tp, kHeadDqn, st);   // (no image: hidden width below 128)
-  if (!h->tc_h1) {  // intermediates of the tensor-core pipeline, allocated on first use
+  if (!h->tc_h2) {  // intermediates of the tensor-core pipeline, allocated on first use (observation rows at pitch 8 ceil(in / 8))
     const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), F = sizeof(float);
-    if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h1, rows * kHidden * F}, {&h->tc_h2, rows * kHidden * F},
-                                                      {&h->tc_rec, rows * 32 /* kRowRec */ * F}, {&h->tc_x, rows * kMaxObsDim * F},
+    if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h2, rows * kHidden * F},
+                                                      {&h->tc_rec, rows * 32 /* kRowRec */ * F}, {&h->tc_x, rows * ((h->ns.in + 7) / 8 * 8) * F},
                                                       {&h->image_bwd, ((size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4) * F}}))
       return rc;
   }
@@ -483,7 +483,7 @@ static int dqn_train_pass(marl_dqn* h, const TrainParams& tp, cudaEvent_t* betwe
     if (int rc = launch_pack_weights(h->theta, h->ns.lay, h->ns.n_nets, h->image, st, h->image_bwd)) return rc;
     h->image_current = h->bwd_image_current = true;
   }
-  TcBuffers tb; tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h1 = h->tc_h1; tb.h2 = h->tc_h2; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
+  TcBuffers tb; tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h2 = h->tc_h2; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
   tc = true;
   return launch_tc_dqn_train(tp, tb, st, between);
 }

@@ -309,9 +309,9 @@ int launch_tc_forward(const FwdParams& p, const uint8_t* images, cudaStream_t st
 // ---- tensor-core training pipeline (tc_train.cu) ----------------------------------------------------------------------------
 struct TcBuffers {
   uint8_t* image; uint8_t* bwd_image;       // packed online-network images (forward K-major, backward K-major W2^T)
-  float *h1, *h2;                           // [128][rows] (feature-major) activations
+  float* h2;                                // [128][rows] (feature-major) H2 activations
   float* rec;                               // [rows][kRowRec] row records (tc_train.cu)
-  float* x;                                 // [rows][kMaxObsDim] gathered observation rows
+  float* x;                                 // [rows][8 ceil(in / 8)] gathered observation rows
   size_t rows;                              // allocated rows
 };
 int tc_train_init();

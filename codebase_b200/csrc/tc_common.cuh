@@ -205,6 +205,34 @@ __device__ __forceinline__ void load_x_frag(const float* s0, const float* s1, in
     x[ks][2] = (s0 && c + 1 < D) ? s0[c + 1] : 0.f; x[ks][3] = (s1 && c + 1 < D) ? s1[c + 1] : 0.f;
   }
 }
+// A fragment order: (row 0, K t) = column 2t, (row 1, K t), (row 0, K t + 4) = column 2t + 1, (row 1, K t + 4)
+__device__ __forceinline__ void x_to_a(const float (&x)[kMaxObsDim / 8][4], uint32_t (&hi)[kMaxObsDim / 8][4], uint32_t (&lo)[kMaxObsDim / 8][4]) {
+#pragma unroll
+  for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {
+    tf32_split_u(x[ks][0], hi[ks][0], lo[ks][0]); tf32_split_u(x[ks][1], hi[ks][1], lo[ks][1]);
+    tf32_split_u(x[ks][2], hi[ks][2], lo[ks][2]); tf32_split_u(x[ks][3], hi[ks][3], lo[ks][3]);
+  }
+}
+// bias + ReLU of a layer-1 accumulator fragment
+__device__ __forceinline__ void bias_relu(float (&h)[64], const float* b, int quad_lane) {
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const float2 bb = *reinterpret_cast<const float2*>(b + frag_col(i, quad_lane));
+    h[i] = fmaxf(h[i] + bb.x, 0.f); h[i + 1] = fmaxf(h[i + 1] + bb.y, 0.f);
+  }
+}
+// Layer 1 of a warpgroup's 64-row tile, H1 = relu(X W1^T + b1), in accumulator-fragment layout: x = this thread's A fragment (load_x_frag),
+// w1 = shared-memory address of the W1 hi panel of a forward image (the lo panel follows it, as in the image), b1 = its bias (shared memory),
+// k1steps = ceil(D / 8).  Every kernel that needs H1 computes it here: the same wgmma sequence on the same operands gives the same bits, so the
+// weight-gradient kernel rebuilds exactly the H1 the training forward used.
+__device__ __forceinline__ void layer1_tile(float (&h)[64], const float (&x)[kMaxObsDim / 8][4], uint32_t w1, const float* b1, int k1steps, int quad_lane) {
+  uint32_t xhi[kMaxObsDim / 8][4], xlo[kMaxObsDim / 8][4];
+  x_to_a(x, xhi, xlo);
+#pragma unroll
+  for (int i = 0; i < 64; ++i) h[i] = 0.f;
+  layer_rs<kMaxObsDim / 8>(h, xhi, xlo, w1, w1 + (kOffW1Lo - kOffW1Hi), k1steps);
+  bias_relu(h, b1, quad_lane);
+}
 // values of a 64 x 128 fragment -> A operand registers (hi / lo) of the next product
 __device__ __forceinline__ void frag_to_a(const float (&v)[64], uint32_t (&hi)[16][4], uint32_t (&lo)[16][4]) {
 #pragma unroll
@@ -257,10 +285,13 @@ struct TcTrainParams {
   RowPlan plan; RowSource src; NetLayout lay;
   const uint8_t* images;      // forward images [n_nets][kImageBytes]
   const uint8_t* bwd_images;  // backward images [n_nets][kBwdImageBytes]
-  // H1, H2: feature-major [128][rows] (the weight-gradient kernel stages 32 consecutive rows of one feature per warp instruction)
-  float* h1g; float* h2g; size_t rows;
+  // H2: feature-major [128][rows] (the weight-gradient kernel stages 32 consecutive rows of one feature per warp instruction); H1 is not stored:
+  // the weight-gradient kernel rebuilds it from xg (layer1_tile)
+  float* h2g; size_t rows;
   float* rec;                 // [rows][kRowRec] row records
-  float* xg;                  // [rows][kMaxObsDim] gathered observation rows: the dH1 kernel reads them for dW1 without chasing the episode index again
+  // [rows][x_pitch] gathered observation rows, x_pitch = 8 ceil(D / 8) (zero beyond D): the dH1 kernel reads them for dW1 and the
+  // weight-gradient kernel for H1, without chasing the episode index again
+  float* xg; int x_pitch;
   const float* tq; const float* td_ext; int td_agent_stride; float gamma; int double_q;
   float* scratch; int scratch_pitch; float* loss_part;
 };

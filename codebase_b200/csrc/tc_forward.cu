@@ -43,23 +43,6 @@ __device__ __forceinline__ const float* fwd_src_row(const FwdParams& p, int net,
   return src_row(p.src, agent, unit, off);
 }
 
-// A fragment order: (row 0, K t) = column 2t, (row 1, K t), (row 0, K t + 4) = column 2t + 1, (row 1, K t + 4)
-__device__ __forceinline__ void x_to_a(const float (&x)[kMaxObsDim / 8][4], uint32_t (&hi)[kMaxObsDim / 8][4], uint32_t (&lo)[kMaxObsDim / 8][4]) {
-#pragma unroll
-  for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {
-    tf32_split_u(x[ks][0], hi[ks][0], lo[ks][0]); tf32_split_u(x[ks][1], hi[ks][1], lo[ks][1]);
-    tf32_split_u(x[ks][2], hi[ks][2], lo[ks][2]); tf32_split_u(x[ks][3], hi[ks][3], lo[ks][3]);
-  }
-}
-// bias + ReLU of a layer-1 accumulator fragment
-__device__ __forceinline__ void bias_relu(float (&h)[64], const float* b, int quad_lane) {
-#pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    const float2 bb = *reinterpret_cast<const float2*>(b + frag_col(i, quad_lane));
-    h[i] = fmaxf(h[i] + bb.x, 0.f); h[i + 1] = fmaxf(h[i + 1] + bb.y, 0.f);
-  }
-}
-
 TSG_DEFINE(g_ts_forward)
 TSG_GETTER(tsg_forward, g_ts_forward)
 // Two warpgroups, each running its own 64-row tiles through layer 1 -> layer 2 -> head with nothing shared but the weight image, so that the
@@ -93,15 +76,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel(FwdParams p, 
     float acc[64];
     {
       float x[kMaxObsDim / 8][4];
-      uint32_t xhi[kMaxObsDim / 8][4], xlo[kMaxObsDim / 8][4];
       load_x_frag(s0, s1, D, tq, x);
-      x_to_a(x, xhi, xlo);
       if (first) mbar_wait(bar, 0);
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      layer_rs<kMaxObsDim / 8>(acc, xhi, xlo, sb + kOffW1Hi, sb + kOffW1Lo, k1steps);
+      layer1_tile(acc, x, sb + kOffW1Hi, b1, k1steps, tq);
     }
-    bias_relu(acc, b1, tq);
     {
       uint32_t hi[16][4], lo[16][4];
       frag_to_a(acc, hi, lo);

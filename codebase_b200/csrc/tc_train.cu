@@ -2,14 +2,15 @@
 //
 // Same arithmetic as train_kernel<KP, kHeadDqn> (QNetwork._compute_loss + backward, marlbase/dqn/model.py:118-168), split where a
 // weight gradient needs the rows of many tiles as its K dimension (tf32 wgmma reads both shared-memory operands K-major only):
-//   tc_dqn_fwd_kernel   online forward (A operand in registers, weights = K-major image), head on the CUDA cores; stores H1, H2 (FP32,
+//   tc_dqn_fwd_kernel   online forward (A operand in registers, weights = K-major image), head on the CUDA cores; stores H2 (FP32,
 //                        feature-major), the gathered observation row, the row's outputs and the ReLU masks of H1 / H2 (row record)
 //   tc_dh1_kernel       TD head (needs the next row's outputs, hence after the forward) -> dLoss/dq[act] and the loss statistics;
 //                        dH1 = (dH2 x W2) * relu'(H1) with dH2[r][j] = g_r W3[act_r][j] relu'(H2[r][j]) built in registers (the TD loss touches
 //                        one output per row); B = K-major image of W2^T; then dW1 | db1 = dH1^T x [X | 1] from dH1 staged transposed
 //                        (K = rows) into shared memory, so dH1 never leaves the SM
 //   tc_dw_kernel        dW2 | db2, dW3: row-streaming TN GEMMs over 32-row chunks staged transposed (K = rows) into shared memory,
-//                        accumulators in registers across all the CTA's rows; db3 on the CUDA cores
+//                        accumulators in registers across all the CTA's rows; db3 on the CUDA cores.  H1 is rebuilt from the gathered
+//                        observation rows with the forward's own layer-1 sequence (layer1_tile) instead of round-tripping through HBM
 // The partials feed the same grad_reduce_kernel / adam_kernel as the FP32 path.
 #include "tc_common.cuh"
 #include "dqn_heads.cuh"
@@ -48,18 +49,21 @@ TSG_GETTER(tsg_dh1, g_ts_dh1)
 TSG_DEFINE(g_ts_dw)
 TSG_GETTER(tsg_dw, g_ts_dw)
 
-// store a 64 x 128 fragment feature-major (dst[j * rows + row]) and its ReLU mask words (rec field `mask`); rows of a missing source (d < 0)
-// are skipped
+// the ReLU mask words of a 64 x 128 fragment (rec field `mask`); rows of a missing source (d < 0) are skipped
+__device__ __forceinline__ void store_frag_masks(const float (&v)[64], long long d0, long long d1, int quad_lane, float* rec, int mask) {
+  uint32_t m0, m1;
+  frag_masks(v, m0, m1);
+  if (d0 >= 0) rec[(size_t)d0 * kRowRec + mask + quad_lane] = __uint_as_float(m0);
+  if (d1 >= 0) rec[(size_t)d1 * kRowRec + mask + quad_lane] = __uint_as_float(m1);
+}
+// store a 64 x 128 fragment feature-major (dst[j * rows + row]) and its ReLU mask words
 __device__ __forceinline__ void store_frag_fm(float* dst, size_t rows, const float (&v)[64], long long d0, long long d1, int quad_lane, float* rec, int mask) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) {
     const long long d = (i & 2) ? d1 : d0;
     if (d >= 0) dst[(size_t)frag_col(i, quad_lane) * rows + (size_t)d] = v[i];
   }
-  uint32_t m0, m1;
-  frag_masks(v, m0, m1);
-  if (d0 >= 0) rec[(size_t)d0 * kRowRec + mask + quad_lane] = __uint_as_float(m0);
-  if (d1 >= 0) rec[(size_t)d1 * kRowRec + mask + quad_lane] = __uint_as_float(m1);
+  store_frag_masks(v, d0, d1, quad_lane, rec, mask);
 }
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams p) {
@@ -93,29 +97,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
     float acc[64];
     {
       float x[kMaxObsDim / 8][4];
-      uint32_t xhi[kMaxObsDim / 8][4], xlo[kMaxObsDim / 8][4];
       load_x_frag(s0, s1, D, tq, x);
 #pragma unroll
-      for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {   // the gathered row for the weight-gradient kernel
+      for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {   // the gathered row for the dH1 and weight-gradient kernels
         const int c = 8 * ks + 2 * tq;
         if (ks < k1steps) {
-          if (d0 >= 0) *reinterpret_cast<float2*>(p.xg + (size_t)d0 * kMaxObsDim + c) = make_float2(x[ks][0], x[ks][2]);
-          if (d1 >= 0) *reinterpret_cast<float2*>(p.xg + (size_t)d1 * kMaxObsDim + c) = make_float2(x[ks][1], x[ks][3]);
+          if (d0 >= 0) *reinterpret_cast<float2*>(p.xg + (size_t)d0 * p.x_pitch + c) = make_float2(x[ks][0], x[ks][2]);
+          if (d1 >= 0) *reinterpret_cast<float2*>(p.xg + (size_t)d1 * p.x_pitch + c) = make_float2(x[ks][1], x[ks][3]);
         }
-        tf32_split_u(x[ks][0], xhi[ks][0], xlo[ks][0]); tf32_split_u(x[ks][1], xhi[ks][1], xlo[ks][1]);
-        tf32_split_u(x[ks][2], xhi[ks][2], xlo[ks][2]); tf32_split_u(x[ks][3], xhi[ks][3], xlo[ks][3]);
       }
       if (first) mbar_wait(bar, 0);
-#pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-      layer_rs<kMaxObsDim / 8>(acc, xhi, xlo, sb + kOffW1Hi, sb + kOffW1Lo, k1steps);
+      layer1_tile(acc, x, sb + kOffW1Hi, b1, k1steps, tq);
     }
-#pragma unroll
-    for (int i = 0; i < 64; i += 2) {
-      const float2 bb = *reinterpret_cast<const float2*>(b1 + frag_col(i, tq));
-      acc[i] = fmaxf(acc[i] + bb.x, 0.f); acc[i + 1] = fmaxf(acc[i + 1] + bb.y, 0.f);
-    }
-    store_frag_fm(p.h1g, p.rows, acc, d0, d1, tq, p.rec, kRecMask1);
+    store_frag_masks(acc, d0, d1, tq, p.rec, kRecMask1);   // H1 itself is rebuilt by the weight-gradient kernel
     {
       uint32_t hi[16][4], lo[16][4];
       frag_to_a(acc, hi, lo);
@@ -298,7 +292,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
 #pragma unroll
       for (int m = 0; m < kMaxObsDim / 4; ++m) {
         const int f = tq + 4 * m;
-        xv[k][m] = (d[k] >= 0 && f < D) ? p.xg[(size_t)d[k] * kMaxObsDim + f] : 0.f;
+        xv[k][m] = (d[k] >= 0 && f < D) ? p.xg[(size_t)d[k] * p.x_pitch + f] : 0.f;
       }
     const long long dr = tq == 0 ? d[0] : d[1];
     if (tq < 2 && dr >= 0) {
@@ -343,16 +337,30 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
 // =====================================================================================================================
 //   dW2 | db2 [j2][j1 | 1] += dH2^T x [H1 | 1]^T   (A: 128 lines, B: 136 lines, line 128 = ones)
 //   dW3^T [j][a]           += H2^T x dq^T          (B: 8 lines, dq[r][a] = g_r at a = act_r)
-// Warpgroup w accumulates the M rows [64 w, 64 w + 64) of both.
-constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA3 = kSB2 + 2 * 136 * kLine, kSB3 = kSA3 + 2 * 128 * kLine, kSW3 = kSB3 + 2 * 8 * kLine;
-constexpr int kDwSmem = kSW3 + kOutPad * kHidden * 4 + 1024;
-static_assert(kSB2 % 1024 == 0 && kSA3 % 1024 == 0 && kSB3 % 1024 == 0 && kDwSmem <= 227 * 1024,
+// Warpgroup w accumulates the M rows [64 w, 64 w + 64) of both.  A2, A3 and B3 are staged per chunk by all eight warps, lane = row; H1 is rebuilt
+// per 64 rows (two chunks) by the warpgroup that ran those rows in the forward (layer1_tile on the W1 panels of the forward image) and staged
+// from its accumulator fragments into two B2 buffers, one per chunk.
+constexpr int kB2Bytes = 2 * 136 * kLine;                                  // one chunk of [H1 | 1], hi | lo
+constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA3 = kSB2 + 2 * kB2Bytes, kSB3 = kSA3 + 2 * 128 * kLine, kSW3 = kSB3 + 2 * 8 * kLine;
+constexpr int kSW1 = kSW3 + kOutPad * kHidden * 4;                         // W1 hi | lo panels of the forward image
+constexpr int kSB1 = kSW1 + (kOffW2Hi - kOffW1Hi), kSBar = kSB1 + kHidden * 4;
+constexpr int kDwSmem = kSBar + 64 + 1024;
+static_assert(kSB2 % 1024 == 0 && kB2Bytes % 1024 == 0 && kSA3 % 1024 == 0 && kSB3 % 1024 == 0 && kSW1 % 1024 == 0 && kDwSmem <= 227 * 1024,
               "weight-gradient staging: 1024-byte aligned operands within the shared memory of one SM");
+
+// gathered observation row of a virtual row (stored by the forward)
+__device__ __forceinline__ const float* xg_row(const TcTrainParams& p, int net, int vr) {
+  int agent, unit, off;
+  decode_row(p.plan, net, vr, agent, unit, off);
+  return p.xg + row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows) * (size_t)p.x_pitch;
+}
 
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
   const float* w3f = reinterpret_cast<const float*>(smem + kSW3);
+  const float* b1 = reinterpret_cast<const float*>(smem + kSB1);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kSBar);
   const int t = threadIdx.x, warp = t >> 5, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31, g = lane >> 2, tq = lane & 3;
   int net, row_begin, row_end;
   cta_rows(p.plan, net, row_begin, row_end);
@@ -364,29 +372,38 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     return;
   }
   TSG(g_ts_dw, 0);
-  const int A = p.lay.out;
-  // constant lines: the ones line (hi 1, lo 0) of [H1 | 1] and the zero lines behind it; W3 copy
-  for (int i = t; i < 8 * kChunk; i += kTcThreads) {
-    const int f = 128 + i / kChunk, r = i % kChunk;
-    stage_hl(smem + kSB2, 136, f, r, f == 128 ? 1.f : 0.f);
+  const uint32_t sb = smem_u32(smem);
+  if (t == 0) {  // W1 hi | lo + b1 of the forward image: TMA bulk copies onto one mbarrier
+    mbar_init(bar, 1); fence_mbar_init();
+    const uint8_t* img = p.images + (size_t)net * kImageBytes;
+    mbar_expect_tx(bar, (uint32_t)((kOffW2Hi - kOffW1Hi) + kHidden * 4));
+    tma_image_range(sb + kSW1 - kOffW1Hi, img, kOffW1Hi, kOffW2Hi, bar);
+    tma_bulk_g2s(sb + kSB1, img + kOffB1, kHidden * 4, bar);
+  }
+  const int A = p.lay.out, D = p.src.D, k1steps = (D + 7) >> 3;
+  // constant lines of both B2 buffers: the ones line (hi 1, lo 0) of [H1 | 1] and the zero lines behind it; W3 copy
+  for (int i = t; i < 2 * 8 * kChunk; i += kTcThreads) {
+    const int b = i / (8 * kChunk), f = 128 + (i / kChunk) % 8, r = i % kChunk;
+    stage_hl(smem + kSB2 + b * kB2Bytes, 136, f, r, f == 128 ? 1.f : 0.f);
   }
   {
     const float4* w3src = reinterpret_cast<const float4*>(p.images + (size_t)net * kImageBytes + kOffW3F);
     for (int i = t; i < kOutPad * kHidden / 4; i += kTcThreads) reinterpret_cast<float4*>(smem + kSW3)[i] = w3src[i];
   }
   __syncthreads();
-  const uint32_t sb = smem_u32(smem);
   float acc2[68], acc3[4];
 #pragma unroll
   for (int i = 0; i < 68; ++i) acc2[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) acc3[i] = 0.f;
   float db3 = 0.f;   // warp a, lane 0: sum of dq[.][a]
+  bool first = true;
   const int n_chunks = (row_end - row_begin + kChunk - 1) / kChunk;
-  for (int c = 0; c < n_chunks; ++c) {
+  int c = 0;
+  do {   // n_chunks >= 1: with a zero-trip path (a for loop) ptxas serialises every wgmma of the kernel (C7515)
     // ---- this thread's row (lane) and features (warp + 8 i) of the chunk -> registers; their loads overlap the previous chunk's MMAs
     const int vr = row_begin + c * kChunk + lane;
-    float h1v[16], h2v[16], gr = 0.f;
+    float h2v[16], gr = 0.f;
     int act = 0;
     {
       long long d = -1;
@@ -398,20 +415,26 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
         gr = rp[kRecG]; act = __float_as_int(rp[kRecAct]);
       }
 #pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const size_t o = (size_t)(warp + 8 * i) * p.rows + (size_t)d;
-        h1v[i] = d >= 0 ? p.h1g[o] : 0.f; h2v[i] = d >= 0 ? p.h2g[o] : 0.f;
-      }
+      for (int i = 0; i < 16; ++i) h2v[i] = d >= 0 ? p.h2g[(size_t)(warp + 8 * i) * p.rows + (size_t)d] : 0.f;
     }
+    // ---- H1 of chunks c and c + 1 (even c): the 64 rows of warpgroup (c / 2) % 2 of tile c / 4, as the forward computed them
+    const bool rebuild = (c & 1) == 0 && wg == ((c >> 1) & 1);
+    const int r0 = row_begin + c * kChunk + 16 * wq + g, r1 = r0 + 8;
+    float x[kMaxObsDim / 8][4], h1[64];
+    if (rebuild) load_x_frag(r0 < row_end ? xg_row(p, net, r0) : nullptr, r1 < row_end ? xg_row(p, net, r1) : nullptr, D, tq, x);
     wg_wait<0>();
     fence_regs(acc2); fence_regs(acc3);
+    // layer 1 behind the wait (its own wgmma.wait_group would wait for this warpgroup's chunk MMAs anyway); the x loads are already in flight
+    if (rebuild) {
+      if (first) { mbar_wait(bar, 0); first = false; }
+      layer1_tile(h1, x, sb + kSW1, b1, k1steps, tq);
+    }
     __syncthreads();   // both warpgroups are done reading the previous chunk
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int j = warp + 8 * i;
       const float dh2 = h2v[i] > 0.f ? gr * w3f[act * kHidden + j] : 0.f;
       stage_hl(smem + kSA2, 128, j, lane, dh2);
-      stage_hl(smem + kSB2, 136, j, lane, h1v[i]);
       stage_hl(smem + kSA3, 128, j, lane, h2v[i]);
     }
     {
@@ -422,22 +445,28 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
       db3 += s;
     }
+    if (rebuild) {   // this warp's rows are chunk c + (wq >> 1), rows 16 (wq & 1) + g and + 8 of it (0 past the CTA's rows)
+      uint8_t* b2 = smem + kSB2 + (wq >> 1) * kB2Bytes;
+      const int cr = 16 * (wq & 1) + g;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) stage_hl(b2, 136, frag_col(i, tq), cr + ((i & 2) ? 8 : 0), (((i & 2) ? r1 : r0) < row_end) ? h1[i] : 0.f);
+    }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes, read by wgmma through the async proxy
     __syncthreads();
     wg_fence();
-    const uint32_t m_off = (uint32_t)(wg * kWgRows * kLine);
+    const uint32_t m_off = (uint32_t)(wg * kWgRows * kLine), b2_off = (uint32_t)(kSB2 + (c & 1) * kB2Bytes);
 #pragma unroll
     for (int term = 0; term < 3; ++term) {
       const uint32_t ah = term == 0 ? 1u : 0u, bh = term == 1 ? 1u : 0u;   // lo*hi, hi*lo, hi*hi
 #pragma unroll
       for (int ks = 0; ks < kChunk / 8; ++ks) {
         const uint32_t ko = (uint32_t)(ks * 32);
-        wgmma_ss_n136(acc2, sw128_desc(sb + kSA2 + ah * 128 * kLine + m_off + ko), sw128_desc(sb + kSB2 + bh * 136 * kLine + ko), 1u);
+        wgmma_ss_n136(acc2, sw128_desc(sb + kSA2 + ah * 128 * kLine + m_off + ko), sw128_desc(sb + b2_off + bh * 136 * kLine + ko), 1u);
         wgmma_ss_n8(acc3, sw128_desc(sb + kSA3 + ah * 128 * kLine + m_off + ko), sw128_desc(sb + kSB3 + bh * 8 * kLine + ko), 1u);
       }
     }
     wg_commit();
-  }
+  } while (++c < n_chunks);
   wg_wait<0>();
   fence_regs(acc2); fence_regs(acc3);
   TSG(g_ts_dw, 30);
@@ -476,7 +505,7 @@ int launch_tc_dqn_train(const TrainParams& tp, const TcBuffers& buf, cudaStream_
   MARL_REQUIRE(tp.src.mode == 1, "tensor-core backward: rows must be gathered from the trajectory store (mode %d)", tp.src.mode);
   TcTrainParams p; memset(&p, 0, sizeof(p));
   p.plan = tp.plan; p.src = tp.src; p.lay = tp.lay; p.images = buf.image; p.bwd_images = buf.bwd_image;
-  p.h1g = buf.h1; p.h2g = buf.h2; p.rec = buf.rec; p.xg = buf.x; p.rows = buf.rows;
+  p.h2g = buf.h2; p.rec = buf.rec; p.xg = buf.x; p.x_pitch = 8 * ((tp.src.D + 7) / 8); p.rows = buf.rows;
   p.tq = tp.tq; p.td_ext = tp.td_ext; p.td_agent_stride = tp.td_agent_stride; p.gamma = tp.gamma; p.double_q = tp.double_q;
   p.scratch = tp.scratch; p.scratch_pitch = tp.scratch_pitch; p.loss_part = tp.loss_part;
   const int grid = tp.plan.cta_begin[tp.plan.n_nets];
