@@ -28,14 +28,6 @@ class LbfCfg(C.Structure):
     ]
 
 
-class LbfState(C.Structure):
-    _fields_ = [
-        ("field", C.c_void_p), ("players", C.c_void_p), ("step", C.c_void_p), ("food_spawned", C.c_void_p),
-        ("ep_return", C.c_void_p), ("ep_len", C.c_void_p), ("episode_idx", C.c_void_p), ("active", C.c_void_p),
-        ("field_pitch", C.c_int32), ("n_envs", C.c_int32),
-    ]
-
-
 class RwareCfg(C.Structure):
     _fields_ = [
         ("shelf_rows", C.c_int32), ("shelf_columns", C.c_int32), ("column_height", C.c_int32), ("n_agents", C.c_int32),

@@ -1,12 +1,23 @@
-// env_common.cuh -- the parts of an env-step kernel that do not depend on the environment (sm_90a): the fused action selection
-// (epsilon-greedy, categorical), marlbase's StandardiseReward and CooperativeReward wrappers and the trajectory-store writes; and on the
-// host, the handle, trajectory checks and step launch of the env C ABIs.
-// Included by lbf_env.cu and rware_env.cu.  Lanes of one env form a group of G consecutive lanes starting at `gbase`; `sub` is the agent.
+// env_common.cuh -- the parts of an env-step kernel that do not depend on the environment (sm_90a): the episode record with its reset,
+// step and autoreset rules (TimeLimit, RecordEpisodeStatistics), the fused action selection (epsilon-greedy, categorical), marlbase's
+// StandardiseReward and CooperativeReward wrappers and the trajectory-store writes; and on the host, the handle, trajectory checks and the
+// launches of the env C ABIs.
+// Included by lbf_env.cu, rware_env.cu and matrix_env.cu.  Lanes of one env form a group of G consecutive lanes starting at `gbase`; `sub` is
+// the agent.
 #pragma once
 #include <string.h>
 #include "traj.cuh"
 
 namespace marl {
+
+// The episode record of every env kind, one array per field: step[E] (TimeLimit's elapsed steps), ep_return[E][N] and ep_len[E]
+// (RecordEpisodeStatistics), episode_idx[E] (resets performed so far: the running episode is episode_idx - 1, the key of its Philox streams),
+// active[E] (0 once an episode ended without autoreset), and the StandardiseReward state, which survives resets.
+struct EpisodeStateDev {
+  int32_t* step; float* ep_return; int32_t* ep_len; uint32_t* episode_idx; uint8_t* active;
+  float* stdr;       // per env: wmean[N] | t[N] | sumw (float32 like the wrapper's numpy arrays)
+  int32_t* stdr_n;   // [E] number of rewards seen
+};
 
 struct StepArgs {
   int E; uint64_t seed; uint32_t gid0;
@@ -97,6 +108,93 @@ __device__ __forceinline__ double cooperative_sum(double rew_w, int gbase, int N
   return tot;
 }
 
+// ---- the episode record: every env kernel changes it through these -----------------------------------------------------------------------
+// Reset of env e (one thread per env): returns the index of the new episode, the key of the env's reset draws, and starts the record on it.
+__device__ __forceinline__ uint32_t begin_episode(const EpisodeStateDev& s, int e, int N) {
+  const uint32_t ep = s.episode_idx[e];
+  s.episode_idx[e] = ep + 1;
+  s.step[e] = 0; s.ep_len[e] = 0; s.active[e] = 1;
+  for (int i = 0; i < N; ++i) s.ep_return[(size_t)e * N + i] = 0.f;
+  return ep;
+}
+
+// set_state of env e: an episode continued from an injected state at `step`, keyed as the first episode when no reset has happened yet
+__device__ __forceinline__ void restart_episode(const EpisodeStateDev& s, int e, int N, int32_t step) {
+  s.step[e] = step; s.ep_len[e] = 0; s.active[e] = 1;
+  for (int i = 0; i < N; ++i) s.ep_return[(size_t)e * N + i] = 0.f;
+  if (s.episode_idx[e] == 0) s.episode_idx[e] = 1;
+}
+
+// get_state of env e: the record's fields into the outputs that are not NULL
+__device__ __forceinline__ void copy_episode(const EpisodeStateDev& s, int e, int N, int32_t* step, float* ep_return, int32_t* ep_len,
+                                             uint32_t* episode_idx, uint8_t* active) {
+  if (step) step[e] = s.step[e];
+  if (ep_return) for (int i = 0; i < N; ++i) ep_return[(size_t)e * N + i] = s.ep_return[(size_t)e * N + i];
+  if (ep_len) ep_len[e] = s.ep_len[e];
+  if (episode_idx) episode_idx[e] = s.episode_idx[e];
+  if (active) active[e] = s.active[e];
+}
+
+// The running episode of env e: the key of its action and transition draws
+__device__ __forceinline__ uint32_t episode_key(const EpisodeStateDev& s, int e) { return s.episode_idx[e] - 1u; }
+
+// TimeLimit (envs.py:95-96): an active episode is truncated once it has run `time_limit` steps (0: no limit)
+__device__ __forceinline__ bool truncated(bool active, int time_limit, int step1) { return active && (time_limit > 0 && step1 >= time_limit); }
+
+// RecordEpisodeStatistics of agent `sub` of env e (alive: the env is active and the lane is an agent), in two calls so that a kernel stores
+// the return where its registers allow (right after the accumulation, lbf_step_kernel<true> spills 16 B more).  add_return: the float32
+// accumulation of the raw reward (wrappers.py:33), and final_ret when the episode ended.  store_return: the running return, which an
+// autoreset restarts at 0.
+__device__ __forceinline__ float add_return(const EpisodeStateDev& s, const StepArgs& a, int e, int N, int sub, bool alive, bool finished, double rew) {
+  if (!alive) return 0.f;
+  const float ep_ret = s.ep_return[(size_t)e * N + sub] + (float)rew;
+  if (finished && a.final_ret) a.final_ret[(size_t)e * N + sub] = ep_ret;
+  return ep_ret;
+}
+
+__device__ __forceinline__ void store_return(const EpisodeStateDev& s, const StepArgs& a, int e, int N, int sub, bool alive, bool finished,
+                                             float ep_ret) {
+  if (alive) s.ep_return[(size_t)e * N + sub] = (finished && a.autoreset) ? 0.f : ep_ret;
+}
+
+// The reward wrappers over RecordEpisodeStatistics: StandardiseReward (std_rew), then CooperativeReward (coop: every agent gets the sum over
+// the env), then rew_out (0 for the agents of a frozen env).  Returns the reward as written.  Every lane of the warp calls it (see
+// standardise_reward and cooperative_sum); env_ok: the lane's env exists.
+__device__ __forceinline__ float wrap_reward(const EpisodeStateDev& s, const StepArgs& a, int e, bool env_ok, int N, int sub, int gbase, bool alive,
+                                             int std_rew, int coop, double rew) {
+  double rew_w = rew;
+  if (std_rew) rew_w = standardise_reward(s.stdr + (size_t)(env_ok ? e : 0) * (2 * N + 1), s.stdr_n + (env_ok ? e : 0), N, sub, alive, rew);
+  const double tot = cooperative_sum(rew_w, gbase, N);
+  const float rew_f = (float)(coop ? tot : rew_w);
+  if (env_ok && sub < N) a.rew_out[(size_t)e * N + sub] = alive ? rew_f : 0.f;
+  return rew_f;
+}
+
+// End of the step of env e, on one lane of the env: step and ep_len, final_len when the episode ended, then either the autoreset --
+// new_episode(ep) resets the env's own state for episode ep -- or a frozen env; then done_out (1 for a frozen env) and trunc_out.
+template <typename NewEpisode>
+__device__ __forceinline__ void end_step(const EpisodeStateDev& s, const StepArgs& a, int e, bool active, int step1, bool done, bool trunc,
+                                         const NewEpisode& new_episode) {
+  if (active) {
+    s.step[e] = step1;
+    const int len1 = s.ep_len[e] + 1;
+    s.ep_len[e] = len1;
+    if (done || trunc) {
+      if (a.final_len) a.final_len[e] = len1;
+      if (a.autoreset) {
+        const uint32_t ep = s.episode_idx[e];
+        new_episode(ep);
+        s.episode_idx[e] = ep + 1;
+        s.step[e] = 0; s.ep_len[e] = 0;
+      } else {
+        s.active[e] = 0;
+      }
+    }
+  }
+  a.done_out[e] = active ? (uint8_t)done : (uint8_t)1;
+  a.trunc_out[e] = (uint8_t)trunc;
+}
+
 // trajectory scalars (rb.add, dqn/train.py:73-89; batch_* writes, ac/train.py:90-99) of env e.  Returns the slot whose observation row
 // step1 this step fills, -1 for none.
 __device__ __forceinline__ int traj_write_scalars(const TrajView& traj, const StepArgs& a, int e, int N, int sub, bool active, int step0, int a_raw,
@@ -122,8 +220,8 @@ __device__ __forceinline__ int traj_write_scalars(const TrajView& traj, const St
 }
 
 // ---- host side: the handle layer of the env C ABIs ----------------------------------------------------------------------------------------
-// A handle (marl_lbf, marl_rware) derives from EnvHandle and adds its config `cfg`, device config `dev` (with N and D) and state pointers `st`.
-// Its device buffers come from alloc_buffers and are released by destroy_handle.
+// A handle (marl_lbf, marl_rware, marl_matrix) derives from EnvHandle and adds its config `cfg`, device config `dev` (with N and D) and state
+// pointers `st`, whose episode record is `st.ep`.  Its device buffers come from alloc_buffers and are released by destroy_handle.
 struct EnvHandle : BufferOwner {
   int E, device;
   uint64_t seed;
@@ -131,6 +229,12 @@ struct EnvHandle : BufferOwner {
   int envs_per_cta, threads;   // step kernel launch shape
   size_t step_smem;
 };
+
+// The zero-filled episode record of E envs of N agents
+inline int alloc_episode_state(BufferOwner* h, const char* who, EpisodeStateDev& s, size_t E, int N) {
+  return alloc_buffers(h, who, {{&s.step, E * 4}, {&s.ep_return, E * N * 4}, {&s.ep_len, E * 4}, {&s.episode_idx, E * 4}, {&s.active, E},
+                                {&s.stdr, E * (2 * N + 1) * 4}, {&s.stdr_n, E * 4}});
+}
 
 // The attribute is a per-function, process-wide setting: only ever raise it (a second env with a smaller tile must not lower the limit of the
 // first).  `limit` is the kernel's current limit, kept by the caller.  A refused size is reported through set_error only: nothing is left
@@ -185,6 +289,15 @@ template <typename H, typename Dev, typename St>
 int launch_step(const H* h, void (*kernel)(Dev, St, StepArgs, TrajView), const StepArgs& a, const marl_traj_view* traj, void* stream) {
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, h->threads, h->step_smem, (cudaStream_t)stream>>>(h->dev, h->st, a, traj_view(traj));
+  MARL_CUDA_TRY(cudaGetLastError());
+  return MARL_OK;
+}
+
+// The reset, set_state and get_state kernels: one thread per env, kernel(h->dev, h->st, h->E, args...)
+template <typename H, typename... KArgs, typename... Args>
+int launch_per_env(const H* h, void (*kernel)(KArgs...), void* stream, Args... args) {
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, args...);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }

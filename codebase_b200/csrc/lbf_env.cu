@@ -29,10 +29,8 @@ struct LbfCfgDev {
 };
 
 struct LbfStateDev {
-  int8_t* field; uint32_t* players; int32_t* step; int32_t* food_spawned; float* ep_return; int32_t* ep_len;
-  uint32_t* episode_idx; uint8_t* active;
-  float* stdr;       // StandardiseReward state per env: wmean[N] | t[N] | sumw (float32 like the wrapper's numpy arrays); survives resets
-  int32_t* stdr_n;   // [E] number of rewards seen
+  int8_t* field; uint32_t* players; int32_t* food_spawned;
+  EpisodeStateDev ep;
 };
 
 constexpr int kThreads = 128;
@@ -196,13 +194,7 @@ __global__ void lbf_reset_kernel(LbfCfgDev c, LbfStateDev s, int E, uint64_t see
   int8_t* f = s.field + (size_t)e * c.pitch;
   uint32_t* pl = s.players + (size_t)e * c.N;
   const bool doit = (mask == nullptr) || mask[e];
-  if (doit) {
-    const uint32_t ep = s.episode_idx[e];
-    s.food_spawned[e] = reset_env(c, seed, gid0 + (uint32_t)e, ep, f, pl);
-    s.episode_idx[e] = ep + 1;
-    s.step[e] = 0; s.ep_len[e] = 0; s.active[e] = 1;
-    for (int i = 0; i < c.N; ++i) s.ep_return[(size_t)e * c.N + i] = 0.f;
-  }
+  if (doit) s.food_spawned[e] = reset_env(c, seed, gid0 + (uint32_t)e, begin_episode(s.ep, e, c.N), f, pl);
   if (obs_out == nullptr && !(traj.obs && doit)) return;
   uint32_t foods[kMaxFood];
   const int nf = list_foods(c, f, foods, kMaxFood);
@@ -255,9 +247,9 @@ __global__ void lbf_set_state_kernel(LbfCfgDev c, LbfStateDev s, int E, const in
   int8_t* f = s.field + (size_t)e * c.pitch;
   int sum = 0;
   for (int p = 0; p < c.pitch; ++p) { const int8_t v = p < c.RC ? field[(size_t)e * c.RC + p] : (int8_t)0; f[p] = v; sum += v; }
-  for (int i = 0; i < c.N; ++i) { s.players[(size_t)e * c.N + i] = players[(size_t)e * c.N + i] & 0x00FFFFFFu; s.ep_return[(size_t)e * c.N + i] = 0.f; }
-  s.step[e] = step[e]; s.food_spawned[e] = sum; s.ep_len[e] = 0; s.active[e] = 1;
-  if (s.episode_idx[e] == 0) s.episode_idx[e] = 1;
+  for (int i = 0; i < c.N; ++i) s.players[(size_t)e * c.N + i] = players[(size_t)e * c.N + i] & 0x00FFFFFFu;
+  s.food_spawned[e] = sum;
+  restart_episode(s.ep, e, c.N, step[e]);
 }
 
 __global__ void lbf_get_state_kernel(LbfCfgDev c, LbfStateDev s, int E, int8_t* field, uint32_t* players, int32_t* step, int32_t* food_spawned,
@@ -265,15 +257,9 @@ __global__ void lbf_get_state_kernel(LbfCfgDev c, LbfStateDev s, int E, int8_t* 
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
   if (field) for (int p = 0; p < c.RC; ++p) field[(size_t)e * c.RC + p] = s.field[(size_t)e * c.pitch + p];
-  for (int i = 0; i < c.N; ++i) {
-    if (players) players[(size_t)e * c.N + i] = s.players[(size_t)e * c.N + i];
-    if (ep_return) ep_return[(size_t)e * c.N + i] = s.ep_return[(size_t)e * c.N + i];
-  }
-  if (step) step[e] = s.step[e];
+  if (players) for (int i = 0; i < c.N; ++i) players[(size_t)e * c.N + i] = s.players[(size_t)e * c.N + i];
   if (food_spawned) food_spawned[e] = s.food_spawned[e];
-  if (ep_len) ep_len[e] = s.ep_len[e];
-  if (episode_idx) episode_idx[e] = s.episode_idx[e];
-  if (active) active[e] = s.active[e];
+  copy_episode(s.ep, e, c.N, step, ep_return, ep_len, episode_idx, active);
 }
 
 // ---- the transition kernel ---------------------------------------------------------------------------------
@@ -319,11 +305,11 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
 
   const bool env_ok = e < a.E;
   int8_t* f = field_s + (size_t)le * sp;
-  const int step0 = env_ok ? s.step[e] : 0;
-  const bool active = env_ok && s.active[e];
+  const int step0 = env_ok ? s.ep.step[e] : 0;
+  const bool active = env_ok && s.ep.active[e];
   const bool alive = active && sub < c.N;
   const uint32_t gid = a.gid0 + (uint32_t)e;
-  const uint32_t ep_cur = env_ok ? s.episode_idx[e] - 1u : 0u;
+  const uint32_t ep_cur = env_ok ? episode_key(s.ep, e) : 0u;
   const int spawned = env_ok ? s.food_spawned[e] : 1;
   uint32_t me = (env_ok && sub < c.N) ? s.players[(size_t)e * c.N + sub] : 0u;
   int r = (int)(me & 0xFF), cc = (int)((me >> 8) & 0xFF);
@@ -398,19 +384,11 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   for (int off = 1; off < G; off <<= 1) nz |= __shfl_xor_sync(FULL, nz, off);
   const int step1 = step0 + 1;
   const bool done = active && ((nz == 0) || (c.max_steps <= step1));
-  const bool trunc = active && (c.time_limit > 0 && step1 >= c.time_limit);
+  const bool trunc = truncated(active, c.time_limit, step1);
   const bool finished = done || trunc;
 
-  double rew_w = rew;
-  if (c.std_rew) rew_w = standardise_reward(s.stdr + (size_t)(env_ok ? e : 0) * (2 * c.N + 1), s.stdr_n + (env_ok ? e : 0), c.N, sub, alive, rew);
-  const double tot = cooperative_sum(rew_w, gbase, c.N);
-  const float rew_f = (float)(c.coop_reward ? tot : rew_w);
-  float ep_ret = 0.f;
-  if (alive) {
-    ep_ret = s.ep_return[(size_t)e * c.N + sub] + (float)rew;  // float32 accumulation, raw reward (wrappers.py:33)
-    if (finished && a.final_ret) a.final_ret[(size_t)e * c.N + sub] = ep_ret;
-  }
-  if (env_ok && sub < c.N) a.rew_out[(size_t)e * c.N + sub] = alive ? rew_f : 0.f;
+  const float rew_f = wrap_reward(s.ep, a, e, env_ok, c.N, sub, gbase, alive, c.std_rew, c.coop_reward, rew);
+  const float ep_ret = add_return(s.ep, a, e, c.N, sub, alive, finished, rew);
 
   int slot = -1;
   if (traj.obs && env_ok) slot = traj_write_scalars(traj, a, e, c.N, sub, active, step0, a_raw, rew_f, done, finished);
@@ -420,24 +398,7 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   __syncwarp();
 
   if (env_ok && sub == 0) {
-    if (active) {
-      s.step[e] = step1;
-      const int len1 = s.ep_len[e] + 1;
-      s.ep_len[e] = len1;
-      if (finished) {
-        if (a.final_len) a.final_len[e] = len1;
-        if (a.autoreset) {
-          const uint32_t ep = s.episode_idx[e];
-          s.food_spawned[e] = reset_env(c, a.seed, gid, ep, f, pl_s + le * G);
-          s.episode_idx[e] = ep + 1;
-          s.step[e] = 0; s.ep_len[e] = 0;
-        } else {
-          s.active[e] = 0;
-        }
-      }
-    }
-    a.done_out[e] = active ? (uint8_t)done : (uint8_t)1;
-    a.trunc_out[e] = (uint8_t)trunc;
+    end_step(s.ep, a, e, active, step1, done, trunc, [&](uint32_t ep) { s.food_spawned[e] = reset_env(c, a.seed, gid, ep, f, pl_s + le * G); });
     if constexpr (!kGrid) meta_s[le * 4 + 0] = list_foods(c, f, foods_s + le * c.NF, c.NF);
     if constexpr (kGrid) {
       // Two players can share a cell (one enters the cell of another whose own move collided), so the agent map is written in ascending
@@ -452,7 +413,7 @@ __global__ void __launch_bounds__(kThreads) lbf_step_kernel(LbfCfgDev c, LbfStat
   }
   __syncwarp();
   if (env_ok && sub < c.N) {
-    if (alive) s.ep_return[(size_t)e * c.N + sub] = (finished && a.autoreset) ? 0.f : ep_ret;
+    store_return(s.ep, a, e, c.N, sub, alive, finished, ep_ret);
     const uint32_t w = pl_s[le * G + sub];
     s.players[(size_t)e * c.N + sub] = w;
     if constexpr (!kGrid) build_obs(c, foods_s + le * c.NF, meta_s[le * 4 + 0], pl_s + le * G, sub, obs_s + ((size_t)le * c.N + sub) * c.D);
@@ -618,10 +579,8 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
   h->envs_per_cta = EPC; h->threads = kThreads;
   h->step_smem = step_smem_bytes(d, grid);
   static size_t step_smem_limit = 48 * 1024, grid_step_smem_limit = 48 * 1024, grid_obs_smem_limit = 48 * 1024;
-  int rc = alloc_buffers(h, "marl_lbf_create", {{&h->st.field, E * d.pitch}, {&h->st.players, E * d.N * 4}, {&h->st.step, E * 4},
-                                                {&h->st.food_spawned, E * 4}, {&h->st.ep_return, E * d.N * 4}, {&h->st.ep_len, E * 4},
-                                                {&h->st.episode_idx, E * 4}, {&h->st.active, E}, {&h->st.stdr, E * (2 * d.N + 1) * 4},
-                                                {&h->st.stdr_n, E * 4}});
+  int rc = alloc_buffers(h, "marl_lbf_create", {{&h->st.field, E * d.pitch}, {&h->st.players, E * d.N * 4}, {&h->st.food_spawned, E * 4}});
+  if (rc == MARL_OK) rc = alloc_episode_state(h, "marl_lbf_create", h->st.ep, E, d.N);
   if (rc == MARL_OK && !grid) rc = raise_smem_limit(lbf_step_kernel<false>, h->step_smem, step_smem_limit, "marl_lbf_create");
   if (rc == MARL_OK && grid) rc = raise_smem_limit(lbf_step_kernel<true>, h->step_smem, grid_step_smem_limit, "marl_lbf_create");
   if (rc == MARL_OK && grid) rc = raise_smem_limit(lbf_grid_obs_kernel, h->step_smem, grid_obs_smem_limit, "marl_lbf_create");
@@ -632,43 +591,26 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
 
 int marl_lbf_destroy(marl_lbf* h) { return destroy_handle(h); }
 
-int marl_lbf_state_ptrs(marl_lbf* h, marl_lbf_state* out) {
-  MARL_REQUIRE(h && out, "marl_lbf_state_ptrs: NULL argument");
-  out->field = h->st.field; out->players = reinterpret_cast<int8_t*>(h->st.players); out->step = h->st.step;
-  out->food_spawned = h->st.food_spawned; out->ep_return = h->st.ep_return; out->ep_len = h->st.ep_len;
-  out->episode_idx = h->st.episode_idx; out->active = h->st.active; out->field_pitch = h->dev.pitch; out->n_envs = h->E;
-  return MARL_OK;
-}
-
 int marl_lbf_set_state(marl_lbf* h, const int8_t* field, const int8_t* players, const int32_t* step, void* stream) {
   MARL_REQUIRE(h && field && players && step, "marl_lbf_set_state: NULL argument");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  lbf_set_state_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, field, reinterpret_cast<const uint32_t*>(players), step);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, lbf_set_state_kernel, stream, field, reinterpret_cast<const uint32_t*>(players), step);
 }
 
 int marl_lbf_get_state(marl_lbf* h, int8_t* field, int8_t* players, int32_t* step, int32_t* food_spawned, float* ep_return, int32_t* ep_len,
                        uint32_t* episode_idx, uint8_t* active, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_lbf_get_state: NULL handle");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  lbf_get_state_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, field, reinterpret_cast<uint32_t*>(players), step, food_spawned,
-                                                                             ep_return, ep_len, episode_idx, active);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, lbf_get_state_kernel, stream, field, reinterpret_cast<uint32_t*>(players), step, food_spawned, ep_return, ep_len,
+                        episode_idx, active);
 }
 
 int marl_lbf_reset(marl_lbf* h, const uint8_t* reset_mask, float* obs_out, const marl_traj_view* traj, int32_t slot0, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_lbf_reset: NULL handle");
   if (int rc = check_traj(h, traj)) return rc;
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  if (!h->cfg.grid_observation) {
-    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, traj_view(traj), slot0);
-  } else {   // the state here, the grid observations and init_episode's row 0 from the CTA-wide element loop of lbf_grid_obs_kernel
-    lbf_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, nullptr, traj_view(nullptr), 0);
-    lbf_grid_obs_kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, kThreads, h->step_smem, (cudaStream_t)stream>>>(
-        h->dev, h->st, h->E, reset_mask, obs_out, traj_view(traj), slot0);
-  }
+  if (!h->cfg.grid_observation) return launch_per_env(h, lbf_reset_kernel, stream, h->seed, h->gid0, reset_mask, obs_out, traj_view(traj), slot0);
+  // the state here, the grid observations and init_episode's row 0 from the CTA-wide element loop of lbf_grid_obs_kernel
+  if (int rc = launch_per_env(h, lbf_reset_kernel, stream, h->seed, h->gid0, reset_mask, nullptr, traj_view(nullptr), 0)) return rc;
+  lbf_grid_obs_kernel<<<(h->E + h->envs_per_cta - 1) / h->envs_per_cta, kThreads, h->step_smem, (cudaStream_t)stream>>>(
+      h->dev, h->st, h->E, reset_mask, obs_out, traj_view(traj), slot0);
   MARL_CUDA_TRY(cudaGetLastError());
   return MARL_OK;
 }

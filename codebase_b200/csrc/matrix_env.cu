@@ -22,8 +22,8 @@ struct MxCfgDev {
 };
 
 struct MxStateDev {
-  int8_t* last_act; int32_t* step; float* ep_return; int32_t* ep_len; uint32_t* episode_idx; uint8_t* active;
-  float* stdr; int32_t* stdr_n;   // StandardiseReward state per env: wmean[N] | t[N] | sumw, and the reward count
+  int8_t* last_act;
+  EpisodeStateDev ep;
 };
 
 constexpr int kMxThreads = 128;
@@ -46,12 +46,9 @@ __global__ void matrix_reset_kernel(MxCfgDev c, MxStateDev s, int E, const uint8
   if (e >= E) return;
   const bool doit = (mask == nullptr) || mask[e];
   int last[MARL_MAX_AGENTS];
-  if (doit) {   // MatrixGame.reset draws nothing
-    s.episode_idx[e] += 1;
-    s.step[e] = 0; s.ep_len[e] = 0; s.active[e] = 1;
-  }
+  if (doit) (void)begin_episode(s.ep, e, c.N);   // MatrixGame.reset draws nothing
   for (int i = 0; i < c.N; ++i) {
-    if (doit) { s.last_act[(size_t)e * c.N + i] = -1; s.ep_return[(size_t)e * c.N + i] = 0.f; }
+    if (doit) s.last_act[(size_t)e * c.N + i] = -1;
     last[i] = s.last_act[(size_t)e * c.N + i];
   }
   for (int i = 0; i < c.N; ++i)
@@ -65,23 +62,16 @@ __global__ void matrix_reset_kernel(MxCfgDev c, MxStateDev s, int E, const uint8
 __global__ void matrix_set_state_kernel(MxCfgDev c, MxStateDev s, int E, const int8_t* last_act, const int32_t* step) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
-  for (int i = 0; i < c.N; ++i) { s.last_act[(size_t)e * c.N + i] = last_act[(size_t)e * c.N + i]; s.ep_return[(size_t)e * c.N + i] = 0.f; }
-  s.step[e] = step[e]; s.ep_len[e] = 0; s.active[e] = 1;
-  if (s.episode_idx[e] == 0) s.episode_idx[e] = 1;
+  for (int i = 0; i < c.N; ++i) s.last_act[(size_t)e * c.N + i] = last_act[(size_t)e * c.N + i];
+  restart_episode(s.ep, e, c.N, step[e]);
 }
 
 __global__ void matrix_get_state_kernel(MxCfgDev c, MxStateDev s, int E, int8_t* last_act, int32_t* step, float* ep_return, int32_t* ep_len,
                                         uint32_t* episode_idx, uint8_t* active) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
-  for (int i = 0; i < c.N; ++i) {
-    if (last_act) last_act[(size_t)e * c.N + i] = s.last_act[(size_t)e * c.N + i];
-    if (ep_return) ep_return[(size_t)e * c.N + i] = s.ep_return[(size_t)e * c.N + i];
-  }
-  if (step) step[e] = s.step[e];
-  if (ep_len) ep_len[e] = s.ep_len[e];
-  if (episode_idx) episode_idx[e] = s.episode_idx[e];
-  if (active) active[e] = s.active[e];
+  if (last_act) for (int i = 0; i < c.N; ++i) last_act[(size_t)e * c.N + i] = s.last_act[(size_t)e * c.N + i];
+  copy_episode(s.ep, e, c.N, step, ep_return, ep_len, episode_idx, active);
 }
 
 // ---- the transition kernel ---------------------------------------------------------------------------------------
@@ -99,11 +89,11 @@ __global__ void __launch_bounds__(kMxThreads) matrix_step_kernel(MxCfgDev c, MxS
 
   const bool env_ok = e < a.E;
   const bool agent = env_ok && sub < c.N;
-  const int step0 = env_ok ? s.step[e] : 0;
-  const bool active = env_ok && s.active[e];
+  const int step0 = env_ok ? s.ep.step[e] : 0;
+  const bool active = env_ok && s.ep.active[e];
   const bool alive = active && sub < c.N;
   const uint32_t gid = a.gid0 + (uint32_t)e;
-  const uint32_t ep_cur = env_ok ? s.episode_idx[e] - 1u : 0u;
+  const uint32_t ep_cur = env_ok ? episode_key(s.ep, e) : 0u;
   const int last0 = agent ? (int)s.last_act[(size_t)e * c.N + sub] : -1;
 
   // ---- action selection -------------------------------------------------------------------------------
@@ -127,44 +117,20 @@ __global__ void __launch_bounds__(kMxThreads) matrix_step_kernel(MxCfgDev c, MxS
   // keeps its own.  (Nothing here depends on the wrapped reward: it is done before the wrappers, which leaves less live across them.) ------
   const int step1 = step0 + 1;
   const bool done = active && step1 >= c.ep_length;
-  const bool trunc = active && (c.time_limit > 0 && step1 >= c.time_limit);
+  const bool trunc = truncated(active, c.time_limit, step1);
   const bool finished = done || trunc;
-  const bool reset_now = finished && a.autoreset;
-  const int last1 = !alive ? last0 : (reset_now ? -1 : act);
-  if (alive) {
-    const float ep_ret = s.ep_return[(size_t)e * c.N + sub] + (float)rew;   // float32 accumulation of the raw reward (wrappers.py:33)
-    if (finished && a.final_ret) a.final_ret[(size_t)e * c.N + sub] = ep_ret;
-    s.ep_return[(size_t)e * c.N + sub] = reset_now ? 0.f : ep_ret;
-    s.last_act[(size_t)e * c.N + sub] = (int8_t)last1;
-  }
+  const int last1 = !alive ? last0 : ((finished && a.autoreset) ? -1 : act);
+  store_return(s.ep, a, e, c.N, sub, alive, finished, add_return(s.ep, a, e, c.N, sub, alive, finished, rew));
+  if (alive) s.last_act[(size_t)e * c.N + sub] = (int8_t)last1;
   act_s[threadIdx.x] = last1;
   flag_s[threadIdx.x] = (int)active | (int)done << 1 | (int)finished << 2;
   if (env_ok && sub == 0) {   // every lane of the group read step / ep_len / episode_idx before the shuffles above
-    if (active) {
-      s.step[e] = step1;
-      const int len1 = s.ep_len[e] + 1;
-      s.ep_len[e] = len1;
-      if (finished) {
-        if (a.final_len) a.final_len[e] = len1;
-        if (a.autoreset) {
-          s.episode_idx[e] = ep_cur + 2u;
-          s.step[e] = 0; s.ep_len[e] = 0;
-        } else {
-          s.active[e] = 0;
-        }
-      }
-    }
-    a.done_out[e] = active ? (uint8_t)done : (uint8_t)1;
-    a.trunc_out[e] = (uint8_t)trunc;
+    end_step(s.ep, a, e, active, step1, done, trunc, [](uint32_t) {});   // the new episode's previous actions are the lanes' last1
     row_s[le] = step1;
   }
 
   // ---- reward wrappers, trajectory scalars ------------------------------------------------------------------------------------------
-  double rew_w = rew;
-  if (c.std_rew) rew_w = standardise_reward(s.stdr + (size_t)(env_ok ? e : 0) * (2 * c.N + 1), s.stdr_n + (env_ok ? e : 0), c.N, sub, alive, rew);
-  const double tot = cooperative_sum(rew_w, gbase, c.N);
-  const float rew_f = (float)(c.coop_reward ? tot : rew_w);
-  if (agent) a.rew_out[(size_t)e * c.N + sub] = alive ? rew_f : 0.f;
+  const float rew_f = wrap_reward(s.ep, a, e, env_ok, c.N, sub, gbase, alive, c.std_rew, c.coop_reward, rew);
   const int fl = flag_s[threadIdx.x];
   const int slot = (traj.obs && env_ok) ? traj_write_scalars(traj, a, e, c.N, sub, fl & 1, step0, a_raw, rew_f, (fl >> 1) & 1, (fl >> 2) & 1) : -1;
   if (env_ok && sub == 0) slot_s[le] = slot;
@@ -260,9 +226,8 @@ int marl_matrix_create(const marl_matrix_cfg* cfg, int32_t n_envs, uint64_t seed
   d.G = g;
   const size_t E = (size_t)n_envs, n_entries = (size_t)matrix_entries(d.N, d.A);
   h->envs_per_cta = (kMxThreads / 32) * (32 / g); h->threads = kMxThreads; h->step_smem = 0;
-  int rc = alloc_buffers(h, "marl_matrix_create", {{&h->payoff, n_entries * sizeof(double)}, {&h->st.last_act, E * d.N}, {&h->st.step, E * 4},
-                                                   {&h->st.ep_return, E * d.N * 4}, {&h->st.ep_len, E * 4}, {&h->st.episode_idx, E * 4},
-                                                   {&h->st.active, E}, {&h->st.stdr, E * (2 * d.N + 1) * 4}, {&h->st.stdr_n, E * 4}});
+  int rc = alloc_buffers(h, "marl_matrix_create", {{&h->payoff, n_entries * sizeof(double)}, {&h->st.last_act, E * d.N}});
+  if (rc == MARL_OK) rc = alloc_episode_state(h, "marl_matrix_create", h->st.ep, E, d.N);
   if (rc == MARL_OK) {
     cudaError_t err = cudaMemcpy(h->payoff, cfg->payoff, n_entries * sizeof(double), cudaMemcpyHostToDevice);
     if (err == cudaSuccess) err = cudaMemset(h->st.last_act, 0xFF, E * d.N);   // -1: no previous action, as after a reset
@@ -278,29 +243,19 @@ int marl_matrix_destroy(marl_matrix* h) { return destroy_handle(h); }
 
 int marl_matrix_set_state(marl_matrix* h, const int8_t* last_action, const int32_t* step, void* stream) {
   MARL_REQUIRE(h && last_action && step, "marl_matrix_set_state: NULL argument");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  matrix_set_state_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, last_action, step);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, matrix_set_state_kernel, stream, last_action, step);
 }
 
 int marl_matrix_get_state(marl_matrix* h, int8_t* last_action, int32_t* step, float* ep_return, int32_t* ep_len, uint32_t* episode_idx,
                           uint8_t* active, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_matrix_get_state: NULL handle");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  matrix_get_state_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, last_action, step, ep_return, ep_len,
-                                                                                episode_idx, active);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, matrix_get_state_kernel, stream, last_action, step, ep_return, ep_len, episode_idx, active);
 }
 
 int marl_matrix_reset(marl_matrix* h, const uint8_t* reset_mask, float* obs_out, const marl_traj_view* traj, int32_t slot0, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_matrix_reset: NULL handle");
   if (int rc = check_traj(h, traj)) return rc;
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  matrix_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, reset_mask, obs_out, traj_view(traj), slot0);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, matrix_reset_kernel, stream, reset_mask, obs_out, traj_view(traj), slot0);
 }
 
 int marl_matrix_step(marl_matrix* h, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,

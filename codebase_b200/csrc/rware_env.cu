@@ -25,9 +25,8 @@ struct RwCfgDev {
 };
 
 struct RwStateDev {
-  uint8_t* shelves; uint32_t* agents; uint32_t* req; int32_t* step; int32_t* inactive; float* ep_return; int32_t* ep_len;
-  uint32_t* episode_idx; uint8_t* active;
-  float* stdr; int32_t* stdr_n;   // StandardiseReward state per env: wmean[N] | t[N] | sumw, and the reward count
+  uint8_t* shelves; uint32_t* agents; uint32_t* req; int32_t* inactive;
+  EpisodeStateDev ep;
 };
 
 constexpr int kRwThreads = 128, kRwEnvsPerCta = kRwThreads / 32, kReqWords = 8, kSink = 31;
@@ -107,11 +106,8 @@ __global__ void rware_reset_kernel(RwCfgDev c, RwStateDev s, int E, uint64_t see
   uint32_t* req = s.req + (size_t)e * kReqWords;
   const bool doit = (mask == nullptr) || mask[e];
   if (doit) {
-    const uint32_t ep = s.episode_idx[e];
-    reset_env(c, seed, gid0 + (uint32_t)e, ep, sh, ag, req);
-    s.episode_idx[e] = ep + 1;
-    s.step[e] = 0; s.inactive[e] = 0; s.ep_len[e] = 0; s.active[e] = 1;
-    for (int i = 0; i < c.N; ++i) s.ep_return[(size_t)e * c.N + i] = 0.f;
+    reset_env(c, seed, gid0 + (uint32_t)e, begin_episode(s.ep, e, c.N), sh, ag, req);
+    s.inactive[e] = 0;
   }
   for (int i = 0; i < c.N; ++i) {
     if (obs_out) build_obs(c, sh, ag, req, i, obs_out + ((size_t)e * c.N + i) * c.D);
@@ -124,10 +120,10 @@ __global__ void rware_set_state_kernel(RwCfgDev c, RwStateDev s, int E, const ui
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
   for (int p = 0; p < c.pitch; ++p) s.shelves[(size_t)e * c.pitch + p] = p < c.RC ? shelves[(size_t)e * c.RC + p] : (uint8_t)0;
-  for (int i = 0; i < c.N; ++i) { s.agents[(size_t)e * c.N + i] = agents[(size_t)e * c.N + i]; s.ep_return[(size_t)e * c.N + i] = 0.f; }
+  for (int i = 0; i < c.N; ++i) s.agents[(size_t)e * c.N + i] = agents[(size_t)e * c.N + i];
   for (int w = 0; w < kReqWords; ++w) s.req[(size_t)e * kReqWords + w] = req[(size_t)e * kReqWords + w];
-  s.step[e] = step[e]; s.inactive[e] = inactive[e]; s.ep_len[e] = 0; s.active[e] = 1;
-  if (s.episode_idx[e] == 0) s.episode_idx[e] = 1;
+  s.inactive[e] = inactive[e];
+  restart_episode(s.ep, e, c.N, step[e]);
 }
 
 __global__ void rware_get_state_kernel(RwCfgDev c, RwStateDev s, int E, uint8_t* shelves, uint32_t* agents, uint32_t* req, int32_t* step,
@@ -135,16 +131,10 @@ __global__ void rware_get_state_kernel(RwCfgDev c, RwStateDev s, int E, uint8_t*
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= E) return;
   if (shelves) for (int p = 0; p < c.RC; ++p) shelves[(size_t)e * c.RC + p] = s.shelves[(size_t)e * c.pitch + p];
-  for (int i = 0; i < c.N; ++i) {
-    if (agents) agents[(size_t)e * c.N + i] = s.agents[(size_t)e * c.N + i];
-    if (ep_return) ep_return[(size_t)e * c.N + i] = s.ep_return[(size_t)e * c.N + i];
-  }
+  if (agents) for (int i = 0; i < c.N; ++i) agents[(size_t)e * c.N + i] = s.agents[(size_t)e * c.N + i];
   if (req) for (int w = 0; w < kReqWords; ++w) req[(size_t)e * kReqWords + w] = s.req[(size_t)e * kReqWords + w];
-  if (step) step[e] = s.step[e];
   if (inactive) inactive[e] = s.inactive[e];
-  if (ep_len) ep_len[e] = s.ep_len[e];
-  if (episode_idx) episode_idx[e] = s.episode_idx[e];
-  if (active) active[e] = s.active[e];
+  copy_episode(s.ep, e, c.N, step, ep_return, ep_len, episode_idx, active);
 }
 
 // Shared memory per warp (= per env): observations [N][D] floats | shelf grid [pitch] | agents [32] | requested [8] | chain lengths [32] | meta [4]
@@ -177,11 +167,11 @@ __global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwSt
   const bool agent = lane < c.N;
   const uint32_t me = agent ? s.agents[(size_t)e * c.N + lane] : 0u;
   int x = (int)(me & 0xFF), y = (int)((me >> 8) & 0xFF), d = (int)((me >> 16) & 0xFF), sh = (int)(me >> 24);
-  const int step0 = s.step[e];
-  const bool active = s.active[e] != 0;   // warp-uniform
+  const int step0 = s.ep.step[e];
+  const bool active = s.ep.active[e] != 0;   // warp-uniform
   const bool alive = active && agent;
   const uint32_t gid = a.gid0 + (uint32_t)e;
-  const uint32_t ep_cur = s.episode_idx[e] - 1u;
+  const uint32_t ep_cur = episode_key(s.ep, e);
   __syncwarp();
 
   // ---- action selection --------------------------------------------------------------------------------------
@@ -288,43 +278,22 @@ __global__ void __launch_bounds__(kRwThreads) rware_step_kernel(RwCfgDev c, RwSt
 
   // ---- termination + wrappers --------------------------------------------------------------------------------------
   const bool done = active && ((c.max_inact > 0 && inact1 >= c.max_inact) || (c.max_steps > 0 && step1 >= c.max_steps));
-  const bool trunc = active && (c.time_limit > 0 && step1 >= c.time_limit);
+  const bool trunc = truncated(active, c.time_limit, step1);
   const bool finished = done || trunc;
-  double rew_w = rew;
-  if (c.std_rew) rew_w = standardise_reward(s.stdr + (size_t)e * (2 * c.N + 1), s.stdr_n + e, c.N, lane, alive, rew);
-  const double tot = cooperative_sum(rew_w, 0, c.N);
-  const float rew_f = (float)(c.coop_reward ? tot : rew_w);
-  float ep_ret = 0.f;
-  if (alive) {
-    ep_ret = s.ep_return[(size_t)e * c.N + lane] + (float)rew;   // float32 accumulation of the raw reward (wrappers.py:33)
-    if (finished && a.final_ret) a.final_ret[(size_t)e * c.N + lane] = ep_ret;
-  }
-  if (agent) a.rew_out[(size_t)e * c.N + lane] = alive ? rew_f : 0.f;
+  const float rew_f = wrap_reward(s.ep, a, e, true, c.N, lane, 0, alive, c.std_rew, c.coop_reward, rew);
+  const float ep_ret = add_return(s.ep, a, e, c.N, lane, alive, finished, rew);
   const int slot = traj.obs ? traj_write_scalars(traj, a, e, c.N, lane, active, step0, a_raw, rew_f, done, finished) : -1;
 
   if (lane == 0) {
-    if (active) {
-      s.step[e] = step1; s.inactive[e] = inact1;
-      const int len1 = s.ep_len[e] + 1;
-      s.ep_len[e] = len1;
-      if (finished) {
-        if (a.final_len) a.final_len[e] = len1;
-        if (a.autoreset) {
-          const uint32_t ep = s.episode_idx[e];
-          reset_env(c, a.seed, gid, ep, sh_s, ag_s, req_s);
-          s.episode_idx[e] = ep + 1;
-          s.step[e] = 0; s.inactive[e] = 0; s.ep_len[e] = 0;
-        } else {
-          s.active[e] = 0;
-        }
-      }
-    }
-    a.done_out[e] = active ? (uint8_t)done : (uint8_t)1;
-    a.trunc_out[e] = (uint8_t)trunc;
+    if (active) s.inactive[e] = inact1;
+    end_step(s.ep, a, e, active, step1, done, trunc, [&](uint32_t ep) {
+      reset_env(c, a.seed, gid, ep, sh_s, ag_s, req_s);
+      s.inactive[e] = 0;
+    });
   }
   __syncwarp();
   if (agent) {
-    if (alive) s.ep_return[(size_t)e * c.N + lane] = (finished && a.autoreset) ? 0.f : ep_ret;
+    store_return(s.ep, a, e, c.N, lane, alive, finished, ep_ret);
     s.agents[(size_t)e * c.N + lane] = ag_s[lane];
     build_obs(c, sh_s, ag_s, req_s, lane, obs_s + (size_t)lane * c.D);
   }
@@ -470,9 +439,8 @@ int marl_rware_create(const marl_rware_cfg* cfg, int32_t n_envs, uint64_t seed, 
   h->step_smem = kRwEnvsPerCta * rware_warp_smem(d.N, d.D, d.pitch);
   static size_t step_smem_limit = 48 * 1024;
   int rc = alloc_buffers(h, "marl_rware_create", {{&h->st.shelves, E * d.pitch}, {&h->st.agents, E * d.N * 4}, {&h->st.req, E * kReqWords * 4},
-                                                  {&h->st.step, E * 4}, {&h->st.inactive, E * 4}, {&h->st.ep_return, E * d.N * 4},
-                                                  {&h->st.ep_len, E * 4}, {&h->st.episode_idx, E * 4}, {&h->st.active, E},
-                                                  {&h->st.stdr, E * (2 * d.N + 1) * 4}, {&h->st.stdr_n, E * 4}});
+                                                  {&h->st.inactive, E * 4}});
+  if (rc == MARL_OK) rc = alloc_episode_state(h, "marl_rware_create", h->st.ep, E, d.N);
   if (rc == MARL_OK) rc = raise_smem_limit(rware_step_kernel, h->step_smem, step_smem_limit, "marl_rware_create");
   if (rc != MARL_OK) { marl_rware_destroy(h); return rc; }
   *out = h;
@@ -484,30 +452,20 @@ int marl_rware_destroy(marl_rware* h) { return destroy_handle(h); }
 int marl_rware_set_state(marl_rware* h, const uint8_t* shelves, const uint8_t* agents, const uint32_t* requested, const int32_t* step,
                          const int32_t* inactive, void* stream) {
   MARL_REQUIRE(h && shelves && agents && requested && step && inactive, "marl_rware_set_state: NULL argument");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  rware_set_state_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, shelves, reinterpret_cast<const uint32_t*>(agents),
-                                                                               requested, step, inactive);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, rware_set_state_kernel, stream, shelves, reinterpret_cast<const uint32_t*>(agents), requested, step, inactive);
 }
 
 int marl_rware_get_state(marl_rware* h, uint8_t* shelves, uint8_t* agents, uint32_t* requested, int32_t* step, int32_t* inactive, float* ep_return,
                          int32_t* ep_len, uint32_t* episode_idx, uint8_t* active, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_rware_get_state: NULL handle");
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  rware_get_state_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, shelves, reinterpret_cast<uint32_t*>(agents), requested,
-                                                                               step, inactive, ep_return, ep_len, episode_idx, active);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, rware_get_state_kernel, stream, shelves, reinterpret_cast<uint32_t*>(agents), requested, step, inactive, ep_return, ep_len,
+                        episode_idx, active);
 }
 
 int marl_rware_reset(marl_rware* h, const uint8_t* reset_mask, float* obs_out, const marl_traj_view* traj, int32_t slot0, void* stream) {
   MARL_REQUIRE(h != nullptr, "marl_rware_reset: NULL handle");
   if (int rc = check_traj(h, traj)) return rc;
-  MARL_CUDA_TRY(cudaSetDevice(h->device));
-  rware_reset_kernel<<<(h->E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(h->dev, h->st, h->E, h->seed, h->gid0, reset_mask, obs_out, traj_view(traj), slot0);
-  MARL_CUDA_TRY(cudaGetLastError());
-  return MARL_OK;
+  return launch_per_env(h, rware_reset_kernel, stream, h->seed, h->gid0, reset_mask, obs_out, traj_view(traj), slot0);
 }
 
 int marl_rware_step(marl_rware* h, const int32_t* actions, float* obs_out, float* rew_out, uint8_t* done_out, uint8_t* trunc_out,

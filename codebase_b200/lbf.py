@@ -86,11 +86,9 @@ def parse_env_id(name: str, time_limit: int = 0, **overrides) -> LbfConfig:
 class NativeLbf(NativeEnv):
     PREFIX = "lbf"
 
-    def _state_fields(self):
-        N = self.N
-        return (("field", torch.int8, (self.cfg.rows * self.cfg.cols,)), ("players", torch.int8, (N, 4)), ("step", torch.int32, ()),
-                ("food_spawned", torch.int32, ()), ("ep_return", torch.float32, (N,)), ("ep_len", torch.int32, ()),
-                ("episode_idx", torch.int32, ()), ("active", torch.uint8, ()))
+    def _env_fields(self):
+        return (("field", torch.int8, (self.cfg.rows * self.cfg.cols,)), ("players", torch.int8, (self.N, 4)), ("step", torch.int32, ()),
+                ("food_spawned", torch.int32, ()))
 
     def set_state(self, field: torch.Tensor, players: torch.Tensor, step: torch.Tensor):
         self._set_state(field, players, step)

@@ -126,10 +126,8 @@ class NativeMatrix(NativeEnv):
 
     PREFIX = "matrix"
 
-    def _state_fields(self):
-        N = self.N
-        return (("last_action", torch.int8, (N,)), ("step", torch.int32, ()), ("ep_return", torch.float32, (N,)), ("ep_len", torch.int32, ()),
-                ("episode_idx", torch.int32, ()), ("active", torch.uint8, ()))
+    def _env_fields(self):
+        return (("last_action", torch.int8, (self.N,)), ("step", torch.int32, ()))
 
     def set_state(self, last_action: torch.Tensor, step: torch.Tensor):
         """last_action int8 [E][N] (each player's previous action, -1: none), step int32 [E]."""

@@ -33,8 +33,9 @@ class TrajStore:
 class NativeEnv:
     """E envs of one kind on one device, driven through the C entry points marl_<PREFIX>_*.
 
-    A subclass sets PREFIX and implements `_state_fields`: the state as (name, dtype, per-env shape), in the argument order of
-    marl_<PREFIX>_get_state.  Its `set_state` passes the leading fields that marl_<PREFIX>_set_state takes to `_set_state`."""
+    A subclass sets PREFIX and implements `_env_fields`: its own part of the state as (name, dtype, per-env shape), in the argument order of
+    marl_<PREFIX>_get_state, which continues with the episode record of every env kind.  Its `set_state` passes the leading fields that
+    marl_<PREFIX>_set_state takes to `_set_state`."""
 
     PREFIX = ""
 
@@ -107,8 +108,12 @@ class NativeEnv:
                                      nat.stream_ptr()), self._c_rollout_step.__name__)
         return self.obs, self.rew, self.done, self.trunc
 
-    def _state_fields(self) -> tuple:
+    def _env_fields(self) -> tuple:
         raise NotImplementedError
+
+    def _state_fields(self) -> tuple:
+        return self._env_fields() + (("ep_return", torch.float32, (self.N,)), ("ep_len", torch.int32, ()), ("episode_idx", torch.int32, ()),
+                                     ("active", torch.uint8, ()))
 
     def _set_state(self, *values: torch.Tensor):
         tmp = [v.to(self.device, dtype).contiguous().view(self.E, *shape) for v, (_, dtype, shape) in zip(values, self._state_fields())]

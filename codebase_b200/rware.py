@@ -105,11 +105,9 @@ class NativeRware(NativeEnv):
 
     PREFIX = "rware"
 
-    def _state_fields(self):
-        N = self.N
-        return (("shelves", torch.uint8, (self.cfg.rows * self.cfg.cols,)), ("agents", torch.uint8, (N, 4)), ("requested", torch.int32, (8,)),
-                ("step", torch.int32, ()), ("inactive", torch.int32, ()), ("ep_return", torch.float32, (N,)), ("ep_len", torch.int32, ()),
-                ("episode_idx", torch.int32, ()), ("active", torch.uint8, ()))
+    def _env_fields(self):
+        return (("shelves", torch.uint8, (self.cfg.rows * self.cfg.cols,)), ("agents", torch.uint8, (self.N, 4)), ("requested", torch.int32, (8,)),
+                ("step", torch.int32, ()), ("inactive", torch.int32, ()))
 
     def set_state(self, shelves: torch.Tensor, agents: torch.Tensor, requested: torch.Tensor, step: torch.Tensor, inactive: torch.Tensor):
         """shelves uint8 [E][rows*cols] (shelf id at its current cell, 0 none), agents uint8 [E][N][4] = (x, y, dir, carried shelf id),

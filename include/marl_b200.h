@@ -75,20 +75,6 @@ typedef struct {
 
 typedef struct marl_lbf marl_lbf;
 
-/* Device-resident state, exposed for parity tests and checkpointing (all device pointers). */
-typedef struct {
-  int8_t*   field;        /* [E][field_pitch], row-major rows*cols cells then zero padding            */
-  int8_t*   players;      /* [E][N][4] = (row, col, level, 0)                                        */
-  int32_t*  step;         /* [E] current_step == TimeLimit's elapsed steps                           */
-  int32_t*  food_spawned; /* [E] sum of food levels at reset (reward normaliser)                      */
-  float*    ep_return;    /* [E][N] float32 running episode return (wrappers.py:33)                  */
-  int32_t*  ep_len;       /* [E]                                                                     */
-  uint32_t* episode_idx;  /* [E] resets performed so far                                             */
-  uint8_t*  active;       /* [E] 0 after the episode ended when autoreset is off                     */
-  int32_t   field_pitch;  /* bytes per env in `field` (rows*cols rounded up to 16)                    */
-  int32_t   n_envs;
-} marl_lbf_state;
-
 /* Trajectory store: the device layout of BOTH the episode replay ring (marlbase/dqn/train.py:19-124,
  * capacity = buffer_size episodes) and the on-policy batch (marlbase/ac/train.py:36-52, capacity =
  * parallel_envs).  Episode-major so that one sampled episode of one agent is one contiguous run. */
@@ -105,7 +91,6 @@ int marl_lbf_create(const marl_lbf_cfg* cfg, int32_t n_envs, uint64_t seed, uint
                     marl_lbf** out);
 int marl_lbf_destroy(marl_lbf* env);
 int marl_lbf_obs_dim(const marl_lbf_cfg* cfg);             /* 3*max_num_food + 3*n_agents (+ n_agents with observe_id); grid_observation: 3*(2*sight+1)^2 */
-int marl_lbf_state_ptrs(marl_lbf* env, marl_lbf_state* out);
 /* Overwrite the transition state (parity tests): host or device pointers are NOT mixed -- all device. */
 int marl_lbf_set_state(marl_lbf* env, const int8_t* field /*[E][rows*cols] dense*/, const int8_t* players,
                        const int32_t* step, void* stream);
