@@ -15,6 +15,11 @@ NVCC_FLAGS = GENCODE + [
 ]
 
 
+def nvcc_path() -> str:
+    """the nvcc to run: $NVCC at the time of the call, else the CUDA toolkit's"""
+    return os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+
+
 def sources():
     return sorted(glob.glob(os.path.join(HERE, "*.cu")))
 
@@ -32,7 +37,7 @@ def build(force: bool = False, verbose: bool = False, out: str | None = None, de
     target = out or SO
     if out is None and not force and not needs_build():
         return SO
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    nvcc = nvcc_path()
     extra = (defines if defines is not None else os.environ.get("MARL_NVCC_DEFINES", "").split())
     srcs = sources()
     if os.environ.get("MARL_PARALLEL_BUILD", "1") == "1":   # one nvcc per translation unit, in parallel, then link

@@ -180,8 +180,9 @@ def dqn_loss(theta, theta_tgt, agent_net, in_dim, out_dim, batch, hp: DqnHP, ret
 def double_q_margin(st: DqnState, batch, hp: DqnHP):
     """Smallest gap between the best and the second-best ONLINE Q-value over every (agent, filled step t, episode) whose row t + 1 feeds the
     double-Q argmax (VDN: the same, per agent).  The argmax is discontinuous: when this margin is below the forward passes' ~1e-6 agreement, two
-    correct implementations may pick different target actions and their gradients then differ by ~1 / filled-steps -- not a defect."""
-    if not hp.double_q:
+    correct implementations may pick different target actions and their gradients then differ by ~1 / filled-steps -- not a defect.  With one
+    action there is nothing to pick between: the margin is infinite."""
+    if not hp.double_q or st.out_dim < 2:
         return float("inf")
     with torch.no_grad():
         q = torch.stack(agents_forward(st.theta, st.agent_net, list(batch["obss"]), st.in_dim, st.out_dim))[:, 1:]     # (N, T, B, A)

@@ -1,0 +1,137 @@
+"""The training pass's row split (csrc/learner.cuh: make_plan, episode_plan, cta_rows) restated in Python, and the branch class of a CTA.
+
+Which branches of the DQN tensor-core training pass run (csrc/tc_train.cu) depends on how many rows a CTA gets:
+  - tc_dh1_kernel walks 128-row tiles; warpgroup 1 stages its two 32-row chunks of a tile at the top of the next tile, or after the loop when the
+    last tile holds more than 64 rows; a chunk with no rows skips its MMAs;
+  - tc_dw_kernel streams 32-row chunks in a do-while loop (one trip for a CTA of at most 32 rows), rebuilds H1 every second chunk into one of two
+    buffers and zero-stages the rows past row_end of a partial chunk;
+  - the fused FP32 train_kernel walks its tiles from the top down (its partial tile is the one at row_begin) and carries the next row's outputs
+    across tile boundaries.
+A CTA's class is (tiles: 1, 2 or 3+; 32-row chunks of its last tile that hold rows: 1-4; whether the last chunk is full), 24 classes in all.  Two
+more cases concern a whole network: fewer than 64 rows in total, and a single CTA for the network.  find_batch picks a batch that reaches a class
+on a given SM count, so that a device with another SM count still tests every class.
+
+A CTA ends on an episode boundary, so its last rows are the final rows of its last episode, and row T of an episode has no TD error.  A tail
+made of row T alone carries no gradient and tests nothing.  A CTA therefore counts for its class only when its last chunk is full or holds at
+least TAIL_MIN rows, and the tests give the last episode of every CTA (last_episodes) its full length T: the tail -- the last chunk, and the rows warpgroup 1
+stages after the loop -- then holds rows t < T that carry TD errors (tail_td_rows)."""
+from __future__ import annotations
+
+import functools
+
+TILE, CHUNK = 128, 32
+TAIL_MIN = 8                   # rows of a partial last chunk for its CTA to count (TAIL_MIN - 1 of them carry TD errors)
+CLASSES = tuple(f"t{t}{'+' if t == 3 else ''}-c{c}-{'full' if full else 'part'}" for t in (1, 2, 3) for c in (1, 2, 3, 4) for full in (True, False))
+SMALL_NET = "net-rows<64"      # a network whose rows are fewer than the 64 a CTA is meant to get
+ONE_CTA = "one-cta-net"        # a network trained by a single CTA
+ALL_CLASSES = CLASSES + (SMALL_NET, ONE_CTA)
+
+
+def nets_of(N, sharing):
+    """agent -> network (codebase_b200.learner.sharing_to_nets): False one net per agent, True one shared net, a tuple of group labels"""
+    if sharing is True:
+        return [0] * N
+    if sharing is False or sharing is None:
+        return list(range(N))
+    order = list(dict.fromkeys(sharing))
+    return [order.index(i) for i in sharing]
+
+
+def make_plan(agent_net, units_per_agent, unit_rows, n_cta_max, min_units):
+    """make_plan: (cta_begin, slot_begin, slot_agent); CTAs [cta_begin[k], cta_begin[k + 1]) work on net k"""
+    n_nets, N = max(agent_net) + 1, len(agent_net)
+    slot_agent, slot_begin = [], []
+    for k in range(n_nets):
+        slot_begin.append(len(slot_agent))
+        slot_agent += [a for a in range(N) if agent_net[a] == k]
+    slot_begin.append(len(slot_agent))
+    total = N * units_per_agent
+    cta_begin, c = [], 0
+    for k in range(n_nets):
+        units = (slot_begin[k + 1] - slot_begin[k]) * units_per_agent
+        want = n_cta_max * units // (total if total > 0 else 1)
+        want = max(1, min(want, (units + min_units - 1) // min_units))
+        cta_begin.append(c)
+        c += want
+    cta_begin.append(c)
+    return dict(cta_begin=cta_begin, slot_begin=slot_begin, slot_agent=slot_agent, unit_rows=unit_rows, units_per_agent=units_per_agent)
+
+
+def episode_plan(agent_net, episodes, T, n_cta_max):
+    """a training pass over sampled episodes: one unit per episode (T + 1 rows), at least 64 rows per CTA"""
+    return make_plan(agent_net, episodes, T + 1, n_cta_max, max(1, (64 + T) // (T + 1)))
+
+
+def cta_rows(p, cta):
+    """cta_rows: (net, row_begin, row_end) of CTA `cta`"""
+    cb, sb = p["cta_begin"], p["slot_begin"]
+    net = 0
+    while net + 1 < len(cb) - 1 and cta >= cb[net + 1]:
+        net += 1
+    ncta, c = cb[net + 1] - cb[net], cta - cb[net]
+    units = (sb[net + 1] - sb[net]) * p["units_per_agent"]
+    return net, units * c // ncta * p["unit_rows"], units * (c + 1) // ncta * p["unit_rows"]
+
+
+def all_cta_rows(p):
+    return [cta_rows(p, c) for c in range(p["cta_begin"][-1])]
+
+
+def classes(rows):
+    """the branch class of a CTA of `rows` > 0 rows"""
+    tiles = (rows + TILE - 1) // TILE
+    last = rows - TILE * (tiles - 1)
+    return f"t{min(tiles, 3)}{'+' if tiles >= 3 else ''}-c{(last + CHUNK - 1) // CHUNK}-{'full' if last % CHUNK == 0 else 'part'}"
+
+
+def tail_counts(rows):
+    """a CTA of `rows` rows counts for its class: its last chunk is full or holds at least TAIL_MIN rows"""
+    return rows % CHUNK == 0 or rows % CHUNK >= TAIL_MIN
+
+
+@functools.lru_cache(maxsize=None)
+def plan_classes(agent_net, B, T, n_sm):
+    """every class a training pass of B episodes of T steps reaches on n_sm SMs (agent_net: a tuple), the small-net cases included"""
+    p = episode_plan(list(agent_net), B, T, n_sm)
+    out = set()
+    for net, r0, r1 in all_cta_rows(p):
+        if r1 > r0 and tail_counts(r1 - r0):
+            out.add(classes(r1 - r0))
+    for k in range(len(p["cta_begin"]) - 1):
+        if (p["slot_begin"][k + 1] - p["slot_begin"][k]) * B * (T + 1) < 64:
+            out.add(SMALL_NET)
+        if p["cta_begin"][k + 1] - p["cta_begin"][k] == 1:
+            out.add(ONE_CTA)
+    return frozenset(out)
+
+
+def find_batch(N, sharing, T_choices, n_sm, cls, max_rows=20_000):
+    """the smallest (B, T) -- fewest rows N B (T + 1), then smallest T -- with T in T_choices whose plan on n_sm SMs holds class `cls`; None when
+    none does within max_rows rows"""
+    nets = tuple(nets_of(N, sharing))
+    cands = sorted((N * B * (T + 1), T, B) for T in T_choices for B in range(1, max_rows // (N * (T + 1)) + 1))
+    for _, T, B in cands:
+        if cls in plan_classes(nets, B, T, n_sm):
+            return B, T
+    return None
+
+
+def last_episodes(agent_net, B, T, n_sm):
+    """the episodes (batch indices b) that end a CTA: units are agent-major, unit u of a net is episode u % B of its (u // B)-th agent"""
+    p = episode_plan(list(agent_net), B, T, n_sm)
+    return sorted({(r1 // (T + 1) - 1) % B for _, r0, r1 in all_cta_rows(p) if r1 > r0})
+
+
+def tail_td_rows(agent_net, B, T, n_sm, cls):
+    """for every CTA of class `cls`: (rows of its last chunk, rows of warpgroup 1's after-loop phase -- chunks 2 and 3 of the last tile -- with a TD
+    error, t < T, in the CTA's last episode); the after-loop count is None where the last tile holds 64 rows or fewer (no such phase)"""
+    p = episode_plan(list(agent_net), B, T, n_sm)
+    out = []
+    for _, r0, r1 in all_cta_rows(p):
+        if r1 <= r0 or not tail_counts(r1 - r0) or classes(r1 - r0) != cls:
+            continue
+        last_ep = r1 - (T + 1)
+        td = lambda lo: sum(1 for vr in range(max(lo, last_ep), r1) if vr % (T + 1) < T)   # noqa: E731
+        last_tile = r0 + (r1 - 1 - r0) // TILE * TILE
+        out.append((td(r0 + (r1 - 1 - r0) // CHUNK * CHUNK), td(last_tile + 2 * CHUNK) if r1 - last_tile > 2 * CHUNK else None))
+    return out

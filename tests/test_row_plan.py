@@ -1,0 +1,169 @@
+"""No GPU: tests/row_plan.py against the library's own planner, the class search on both H100 SM counts, and the edges of
+tests/test_tc_train_edges_gpu.py's shape tables.
+
+The planner check compiles a host-only driver that includes csrc/learner.cuh (nvcc with the library's flags, no device code runs) and prints
+episode_plan's cta_begin and every CTA's [row_begin, row_end).  cta_rows itself is device code: the driver restates its split in C++ integer
+arithmetic."""
+import subprocess
+
+import numpy as np
+import pytest
+
+from codebase_b200.csrc import build as native_build
+from tests import row_plan as rp
+from tests import test_tc_train_edges_gpu as g
+
+DRIVER = r"""
+#include "learner.cuh"
+#include <stdio.h>
+using namespace marl;
+// stdin: lines "N B T n_sm agent_net[0..N)"; stdout per line: "n_cta cta_begin[0..n_nets] | net row_begin row_end ..." (one triple per CTA)
+int main() {
+  int N, B, T, n_sm;
+  while (scanf("%d %d %d %d", &N, &B, &T, &n_sm) == 4) {
+    NetSet ns; ns.n_agents = N; ns.n_nets = 0;
+    for (int a = 0; a < N; ++a) { scanf("%d", &ns.agent_net[a]); if (ns.agent_net[a] + 1 > ns.n_nets) ns.n_nets = ns.agent_net[a] + 1; }
+    const RowPlan p = episode_plan(ns, B, T, n_sm);
+    const int n_cta = p.cta_begin[p.n_nets];
+    printf("%d", n_cta);
+    for (int k = 0; k <= p.n_nets; ++k) printf(" %d", p.cta_begin[k]);
+    printf(" |");
+    for (int c = 0; c < n_cta; ++c) {   // cta_rows with blockIdx.x = c
+      int net = 0;
+      while (net + 1 < p.n_nets && c >= p.cta_begin[net + 1]) ++net;
+      const int ncta = p.cta_begin[net + 1] - p.cta_begin[net], k = c - p.cta_begin[net];
+      const long long units = (long long)(p.slot_begin[net + 1] - p.slot_begin[net]) * p.units_per_agent;
+      printf(" %d %d %d", net, (int)(units * k / ncta) * p.unit_rows, (int)(units * (k + 1) / ncta) * p.unit_rows);
+    }
+    printf("\n");
+  }
+  return 0;
+}
+"""
+
+
+@pytest.fixture(scope="module")
+def driver(tmp_path_factory):
+    d = tmp_path_factory.mktemp("plan_driver")
+    src, exe = d / "plan_driver.cu", d / "plan_driver"
+    src.write_text(DRIVER)
+    flags = [f for f in native_build.NVCC_FLAGS if f != "-shared"]
+    subprocess.check_call([native_build.nvcc_path()] + flags + ["-I", native_build.HERE, str(src), "-o", str(exe)])
+    return str(exe)
+
+
+def _configs():
+    """seeded configs: N 1-32; independent, shared and uneven sharing groups; B 1-2048; T 1-200; 114, 132 and 144 SMs"""
+    rng = np.random.default_rng(0x9A7)
+    out = []
+    for i in range(300):
+        N = int(rng.integers(1, 33))
+        kind = i % 3
+        nets = list(range(N)) if kind == 0 else [0] * N if kind == 1 else rp.nets_of(N, tuple(int(x) for x in rng.integers(0, max(1, N // 3) + 1, N)))
+        B = int(rng.choice([rng.integers(1, 17), rng.integers(1, 257), rng.integers(1, 2049)]))
+        T = int(rng.choice([rng.integers(1, 11), rng.integers(1, 201)]))
+        out.append((N, B, T, int(rng.choice([114, 132, 144])), nets))
+    return out
+
+
+def test_mirror_matches_the_library_planner(driver):
+    cfgs = _configs()
+    stdin = "".join(f"{N} {B} {T} {n_sm} {' '.join(map(str, nets))}\n" for N, B, T, n_sm, nets in cfgs)
+    lines = subprocess.run([driver], input=stdin, capture_output=True, text=True, check=True).stdout.splitlines()
+    assert len(lines) == len(cfgs)
+    seen = set()
+    for (N, B, T, n_sm, nets), line in zip(cfgs, lines):
+        head, rows = line.split("|")
+        head, rows = [int(x) for x in head.split()], [int(x) for x in rows.split()]
+        p = rp.episode_plan(nets, B, T, n_sm)
+        assert head[0] == p["cta_begin"][-1] and head[1:] == p["cta_begin"], (N, B, T, n_sm, nets)
+        want = [x for r in rp.all_cta_rows(p) for x in r]
+        assert rows == want, (N, B, T, n_sm, nets)
+        seen |= rp.plan_classes(tuple(nets), B, T, n_sm)
+    assert len(seen) >= 12, sorted(seen)   # the random configs are not the coverage: find_batch is
+
+
+def test_classes_of_rows():
+    assert rp.classes(1) == rp.classes(31) == "t1-c1-part" and rp.classes(32) == "t1-c1-full" and rp.classes(96) == "t1-c3-full"
+    assert rp.classes(128) == "t1-c4-full" and rp.classes(129) == "t2-c1-part" and rp.classes(159) == "t2-c1-part" and rp.classes(160) == "t2-c1-full"
+    assert rp.classes(257) == "t3+-c1-part" and rp.classes(383) == "t3+-c4-part" and rp.classes(384 + 96) == "t3+-c3-full"
+    assert len(set(rp.CLASSES)) == 24 and {rp.classes(r) for r in range(1, 1025)} == set(rp.CLASSES)
+
+
+@pytest.mark.parametrize("n_sm", [114, 132])
+def test_every_class_is_found_within_the_row_budget(n_sm):
+    """an H100 PCIe (114 SMs) and SXM (132 SMs) split the same batch differently: each case of the class sweep finds its class on both"""
+    for cls, c in g.CLASS_CASES.items():
+        found = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, cls, g.MAX_ROWS)
+        assert found is not None, (n_sm, cls, c)
+        B, T = found
+        assert cls in rp.plan_classes(tuple(rp.nets_of(c.N, c.sharing)), B, T, n_sm) and c.N * B * (T + 1) <= g.MAX_ROWS
+    assert set(g.CLASS_CASES) == set(rp.ALL_CLASSES)
+
+
+@pytest.mark.parametrize("n_sm", [114, 132])
+def test_the_tail_rows_of_every_case_carry_td_errors(n_sm):
+    """With the last episode of every CTA at full length, every CTA of a case's class has TD rows (t < T) in its last chunk, and in the rows of
+    warpgroup 1's after-loop phase exactly where the last tile holds more than 64 rows (chunks 3 and 4): a fault in either tail moves the gradient"""
+    for name, c in {**g.CLASS_CASES, **g.WIDTH_CASES}.items():
+        cls = c.cls or name
+        if cls not in rp.CLASSES:
+            continue
+        B, T = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, cls, g.MAX_ROWS)
+        tails = rp.tail_td_rows(rp.nets_of(c.N, c.sharing), B, T, n_sm, cls)
+        assert tails, (n_sm, name)
+        for last_chunk, after_loop in tails:
+            assert last_chunk >= rp.TAIL_MIN - 1, (n_sm, name, B, T, last_chunk)
+            assert (after_loop is not None) == (cls.split("-")[1] in ("c3", "c4")), (n_sm, name)
+            assert after_loop is None or after_loop >= rp.TAIL_MIN - 1, (n_sm, name, B, T, after_loop)
+    # two multi-tile classes hold several episodes per CTA: tile boundaries inside an episode, CTAs of one net split by cta_rows' rounding
+    for cls in ("t2-c2-part", "t2-c3-part"):
+        c = g.CLASS_CASES[cls]
+        B, T = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, cls, g.MAX_ROWS)
+        p = rp.episode_plan(rp.nets_of(c.N, c.sharing), B, T, n_sm)
+        assert min(r1 - r0 for _, r0, r1 in rp.all_cta_rows(p)) >= 2 * (T + 1) and (T + 1) % rp.TILE != 0, (cls, B, T)
+
+
+def test_tail_rows_of_a_small_plan():
+    """tail_td_rows and last_episodes on a plan worked by hand: one net, 3 episodes of T = 63 (64 rows) in one CTA of 192 rows (t2-c2-full);
+    the last episode is b = 2, its rows 128..191; the last chunk is rows 160..191, of which t < 63 are 160..190"""
+    assert rp.episode_plan([0], 3, 63, 1)["cta_begin"] == [0, 1]
+    assert rp.last_episodes([0], 3, 63, 1) == [2]
+    assert rp.tail_td_rows([0], 3, 63, 1, "t2-c2-full") == [(31, None)]
+    # 2 agents sharing the net, B = 2, T = 99: 4 units of 100 rows on 2 CTAs -> 200 rows each (t2-c3-part, after-loop rows 192..199)
+    assert rp.last_episodes([0, 0], 2, 99, 2) == [1]
+    assert rp.tail_td_rows([0, 0], 2, 99, 2, "t2-c3-part") == [(7, 7), (7, 7)]
+
+
+def test_cases_sit_on_the_edges_they_claim():
+    C, W = g.CLASS_CASES, g.WIDTH_CASES
+    # the TD-head sources: the in-kernel head, td_ext with stride 0 (VDN), per agent (standardise_returns), the QMIX mixer
+    kinds = [(c.kind, c.standardise) for c in C.values()]
+    assert ("idqn", False) in kinds and ("vdn", False) in kinds and ("idqn", True) in kinds and 2 <= kinds.count(("qmix", False)) <= 3
+    # independent, shared and uneven-group networks
+    assert any(c.sharing is False and c.N > 1 for c in C.values()) and any(c.sharing is True and c.N > 1 for c in C.values())
+    assert any(isinstance(c.sharing, tuple) and len(set(c.sharing)) > 1 for c in C.values())
+    # double-Q only where a CTA holds few rows (near-ties grow with the rows) -- the single-action cases have no argmax to tie
+    for cls, c in {**C, **W}.items():
+        if c.double_q and c.A > 1:
+            for n_sm in (114, 132):
+                B, T = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, c.cls or cls, g.MAX_ROWS)
+                assert B * T <= 160, (cls, n_sm, B, T)
+    # the width sweep: the k1steps edges of layer1_tile (D = 8 k - 1, 8 k, 8 k + 1) and the widest input with a bias column
+    assert sorted(c.D for c in W.values()) == [1, 2, 7, 8, 9, 16, 17, 24, 25, 31]
+    for c in W.values():
+        k1 = (c.D + 7) // 8
+        assert c.D in (1, 2, 31) or c.D % 8 in (0, 1, 7), c
+        assert (8 * k1 == c.D) == (c.D in (8, 16, 24))   # the gathered-row pitch equals D: the ones line of [X | 1] opens a new 8-line group
+        assert c.D < g.MAX_OBS_TC
+    # every action count 1, 2, 3, 5 and 8 at least twice (A = 1: no argmax, db3[0] only; 2 and 5: partial head columns; 8: kOutPad)
+    counts = {a: sum(c.A == a for c in W.values()) for a in (1, 2, 3, 5, 8)}
+    assert all(v >= 2 for v in counts.values()) and sum(counts.values()) == len(W), counts
+    # each width case runs a multi-tile CTA whose last chunk is partial
+    for c in W.values():
+        assert c.cls.startswith(("t2", "t3")) and c.cls.endswith("part"), c
+    # the forward: E = 1 and a ragged multi-tile split of E rows per network
+    assert g.FWD_E[0] == 1 and g.FWD_E[1] % 32 != 0
+    # handle reuse: a smaller batch and a shorter T than the handle was created for
+    for name, (big, small) in g.REUSE_SHAPES.items():
+        assert small[0] < big[0] and small[1] < big[1], name
