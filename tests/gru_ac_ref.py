@@ -7,7 +7,8 @@ Restated from (path:line in the reference project's marlbase/):
 
 learner_ref's A2C / PPO update, loss and ReLU-kink functions run unchanged with an agents_forward that picks the network kind of each call from the
 flat vector's length: n_nets x P differs between the GRU and the MLP of the same widths.  So the actor and the critic are switched independently,
-and the recurrent learners share every line of loss arithmetic with the feed-forward ones.
+and the recurrent learners share every line of loss arithmetic with the feed-forward ones.  At a hidden width below 128 the networks are
+tests/hidden_width_ref.py's, the width read from the vector's length as well.
 """
 from __future__ import annotations
 
@@ -17,22 +18,30 @@ import torch
 
 from oracle import gru_ref as gr
 from oracle import learner_ref as lr
+from tests import hidden_width_ref as hr
 
 
 def is_recurrent(flat, agent_net, in_dim, out_dim):
     n_nets = max(agent_net) + 1
     if flat.numel() == n_nets * gr.net_size(in_dim, out_dim):
         return True
-    assert flat.numel() == n_nets * lr.net_size(in_dim, out_dim), (flat.numel(), n_nets, in_dim, out_dim)
-    return False
+    if flat.numel() == n_nets * lr.net_size(in_dim, out_dim):
+        return False
+    # another hidden width (layers: [H, H], H < 128): the kind whose width fits the vector's length, which must be unambiguous
+    rec, ff = hr.width_of(flat, agent_net, in_dim, out_dim, True), hr.width_of(flat, agent_net, in_dim, out_dim, False)
+    assert (rec is None) != (ff is None), (flat.numel(), n_nets, in_dim, out_dim, rec, ff)
+    return rec is not None
 
 
 def agents_forward(flat, agent_net, xs, in_dim, out_dim):
-    """learner_ref.agents_forward for either network kind: xs per agent (L, P, D); a GRU runs each sequence from the zero state"""
-    if is_recurrent(flat, agent_net, in_dim, out_dim):
+    """learner_ref.agents_forward for either network kind at any width: xs per agent (L, P, D); a GRU runs each sequence from the zero state"""
+    rec = is_recurrent(flat, agent_net, in_dim, out_dim)
+    if rec and flat.numel() == (max(agent_net) + 1) * gr.net_size(in_dim, out_dim):
         return gr.agents_forward(flat, agent_net, xs, in_dim, out_dim)
-    P = lr.net_size(in_dim, out_dim)
-    return [lr.mlp(flat[k * P:(k + 1) * P], x, in_dim, out_dim) for k, x in zip(agent_net, xs)]
+    if not rec and flat.numel() == (max(agent_net) + 1) * lr.net_size(in_dim, out_dim):
+        P = lr.net_size(in_dim, out_dim)
+        return [lr.mlp(flat[k * P:(k + 1) * P], x, in_dim, out_dim) for k, x in zip(agent_net, xs)]
+    return hr.agents_forward(flat, agent_net, xs, in_dim, out_dim, rec)
 
 
 @contextlib.contextmanager
@@ -49,6 +58,22 @@ def mixed():
 def init_part(recurrent, n_nets, in_dim, out_dim):
     """one part's initial parameters by its own rule (global RNG): RNNNetwork's (orthogonal on final_layer only) or FCNetwork's"""
     return gr.init_flat(n_nets, in_dim, out_dim) if recurrent else lr.init_flat(n_nets, in_dim, out_dim)
+
+
+def dqn_update(st: lr.DqnState, batch, hp: lr.DqnHP):
+    """gru_ref's DQN functions for recurrent agents of any width"""
+    with mixed():
+        return lr.dqn_update(st, batch, hp)
+
+
+def dqn_kink_risk(st: lr.DqnState, batch, hp: lr.DqnHP):
+    with mixed():
+        return lr.dqn_kink_risk(st, batch, hp)
+
+
+def double_q_margin(st: lr.DqnState, batch, hp: lr.DqnHP):
+    with mixed():
+        return lr.double_q_margin(st, batch, hp)
 
 
 def a2c_update(st: lr.A2CState, batch, hp: lr.A2CHP, step: int):
@@ -72,8 +97,10 @@ def ppo_kink_risk(st: lr.A2CState, batch, hp: lr.A2CHP, res, ppo_clip, epoch=-1)
 
 
 def act_steps(flat, agent_net, obs, in_dim, out_dim, h0=None):
-    """act / get_value over consecutive steps of a recurrent part: obs (S, E, N, in_dim) -> outputs (S, E, N, out), h (S, E, N, 128)"""
-    return gr.act_steps(flat, agent_net, obs, in_dim, out_dim, h0)
+    """act / get_value over consecutive steps of a recurrent part: obs (S, E, N, in_dim) -> outputs (S, E, N, out), h (S, E, N, H)"""
+    if flat.numel() == (max(agent_net) + 1) * gr.net_size(in_dim, out_dim):
+        return gr.act_steps(flat, agent_net, obs, in_dim, out_dim, h0)
+    return hr.act_steps(flat, agent_net, obs, in_dim, out_dim, h0)
 
 
 def joint(obs):

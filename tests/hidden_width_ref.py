@@ -103,13 +103,23 @@ def init_gru(n_nets, in_dim, out_dim, H, orthogonal=True):
 # ---- forward passes -----------------------------------------------------------------------------------------------------------------------------
 def mlp(flat_net, x, in_dim, out_dim, H):
     w1, b1, w2, b2, w3, b3 = split_net(flat_net, in_dim, out_dim, H)
-    return F.linear(F.relu(F.linear(F.relu(F.linear(x, w1, b1)), w2, b2)), w3, b3)
+    z1 = F.linear(x, w1, b1); h1 = F.relu(z1)
+    z2 = F.linear(h1, w2, b2); h2 = F.relu(z2)
+    if lr._TAPS is not None and flat_net.requires_grad:   # learner_ref.kink_risk reads every ReLU of the differentiated passes
+        h1.retain_grad(); h2.retain_grad()
+        lr._TAPS.append((z1, h1, x)); lr._TAPS.append((z2, h2, h1))
+    return F.linear(h2, w3, b3)
 
 
 def gru_net(flat_net, x, in_dim, out_dim, H, h0=None):
     """x (L, B, in_dim) -> q (L, B, out_dim), h (L, B, H): every step's hidden state; h0 (B, H) or None = zeros."""
     w1, b1, wih, whh, bih, bhh, w3, b3 = split_net(flat_net, in_dim, out_dim, H, True)
-    gi = F.linear(F.relu(F.linear(x, w1, b1)), wih, bih)
+    z1 = F.linear(x, w1, b1)
+    x1 = F.relu(z1)
+    if lr._TAPS is not None and flat_net.requires_grad:   # the first layer's ReLU is the net's only kink (oracle/gru_ref.py)
+        x1.retain_grad()
+        lr._TAPS.append((z1, x1, x))
+    gi = F.linear(x1, wih, bih)
     h = torch.zeros(x.shape[1], H, dtype=x.dtype) if h0 is None else h0
     hs = []
     for t in range(x.shape[0]):

@@ -1,4 +1,5 @@
-"""The training pass's row split (csrc/learner.cuh: make_plan, episode_plan, cta_rows) restated in Python, and the branch class of a CTA.
+"""The training pass's row split (csrc/learner.cuh: make_plan, episode_plan, cta_rows) restated in Python, and the branch class of a CTA; the
+recurrent kernels' sequence split (gru_plan, seq_class, find_units) further down.
 
 Which branches of the DQN tensor-core training pass run (csrc/tc_train.cu) depends on how many rows a CTA gets:
   - tc_dh1_kernel walks 128-row tiles; warpgroup 1 stages its two 32-row chunks of a tile at the top of the next tile, or after the loop when the
@@ -120,6 +121,98 @@ def last_episodes(agent_net, B, T, n_sm):
     """the episodes (batch indices b) that end a CTA: units are agent-major, unit u of a net is episode u % B of its (u // B)-th agent"""
     p = episode_plan(list(agent_net), B, T, n_sm)
     return sorted({(r1 // (T + 1) - 1) % B for _, r0, r1 in all_cta_rows(p) if r1 > r0})
+
+
+# ---- the recurrent (GRU) split ------------------------------------------------------------------------------------------------------------------
+# gru_backward_kernel (csrc/gru_kernels.cu) gets make_plan(ns, B, 1, n_sm, kGruSeqs): one unit per sequence (agent, b), a contiguous run
+# [v_begin, v_end) of one net's sequences per CTA.  It walks the run in 16-sequence tiles, each split into two 8-sequence halves (one per 128-thread
+# half of the block), resets the carried dL/dh per tile and adds each tile's sums into the CTA's scratch row.  A CTA's class is its tiles (1, 2,
+# 3+) and its last tile: lower (1-7 sequences: the second half is all padding), half (8), upper (9-15), full (16).  Three more cases: a net of
+# fewer than 16 sequences, a net trained by one CTA, and a tile of a multi-tile CTA that holds sequences of two agents (gru_seq crosses a slot).
+# gru_forward_kernel tiles every net's sequences from 0 and launches ceil(max / 16) CTAs per net: its shapes are each net's nseq % 16 and whether
+# a smaller net leaves CTAs idle.
+SEQS = 16                      # kGruSeqs
+SEQ_CLASSES = tuple(f"t{t}{'+' if t == 3 else ''}-{last}" for t in (1, 2, 3) for last in ("lower", "half", "upper", "full"))
+GRU_SMALL_NET = "gru-small-net"
+GRU_ONE_CTA = "gru-one-cta"
+GRU_STRADDLE = "gru-straddle"
+GRU_CLASSES = SEQ_CLASSES + (GRU_SMALL_NET, GRU_ONE_CTA, GRU_STRADDLE)
+FWD_REMAINDERS = ("lower", "half", "upper", "full")
+
+
+def _last_tile(n):
+    last = n - SEQS * ((n - 1) // SEQS)
+    return "lower" if last < 8 else "half" if last == 8 else "upper" if last < SEQS else "full"
+
+
+def gru_plan(agent_net, B, n_sm):
+    """the backward's plan: make_plan(ns, B, 1, n_sm, kGruSeqs); rows of cta_rows are sequences"""
+    return make_plan(list(agent_net), B, 1, n_sm, SEQS)
+
+
+def seq_class(n):
+    """the class of a CTA of n > 0 sequences"""
+    tiles = (n + SEQS - 1) // SEQS
+    return f"t{min(tiles, 3)}{'+' if tiles >= 3 else ''}-{_last_tile(n)}"
+
+
+def seq_of(p, net, v):
+    """sequence v of net -> (agent, b), as gru_seq"""
+    slot = v // p["units_per_agent"]
+    return p["slot_agent"][p["slot_begin"][net] + slot], v - slot * p["units_per_agent"]
+
+
+def tiles_of(v0, v1):
+    """the tiles [vt, vt_end) of a CTA's run [v0, v1)"""
+    return [(vt, min(vt + SEQS, v1)) for vt in range(v0, v1, SEQS)]
+
+
+def straddles(B, v0, v1):
+    """a tile of the multi-tile run [v0, v1) holds sequences of two agents (B sequences per agent)"""
+    return v1 - v0 > SEQS and any((vt // B + 1) * B < ve for vt, ve in tiles_of(v0, v1))
+
+
+@functools.lru_cache(maxsize=None)
+def gru_classes(agent_net, B, n_sm):
+    """every class the backward of B sequences per agent reaches on n_sm SMs (agent_net: a tuple)"""
+    p = gru_plan(agent_net, B, n_sm)
+    out = set()
+    for _, v0, v1 in all_cta_rows(p):
+        if v1 > v0:
+            out.add(seq_class(v1 - v0))
+            if straddles(B, v0, v1):
+                out.add(GRU_STRADDLE)
+    for k in range(len(p["cta_begin"]) - 1):
+        if (p["slot_begin"][k + 1] - p["slot_begin"][k]) * B < SEQS:
+            out.add(GRU_SMALL_NET)
+        if p["cta_begin"][k + 1] - p["cta_begin"][k] == 1:
+            out.add(GRU_ONE_CTA)
+    return frozenset(out)
+
+
+def find_units(N, sharing, n_sm, cls, max_seqs=7_000):
+    """the smallest B (sequences per agent) whose backward plan on n_sm SMs holds class `cls`, with N B <= max_seqs; None when none does"""
+    nets = tuple(nets_of(N, sharing))
+    for B in range(1, max_seqs // N + 1):
+        if cls in gru_classes(nets, B, n_sm):
+            return B
+    return None
+
+
+def cta_edge_sequences(p):
+    """(agent, b) of the first and the last sequence of every CTA and of every tile of the plan"""
+    out = set()
+    for net, v0, v1 in all_cta_rows(p):
+        for vt, ve in tiles_of(v0, v1):
+            out |= {seq_of(p, net, vt), seq_of(p, net, ve - 1)}
+    return sorted(out)
+
+
+def forward_shapes(agent_net, B):
+    """the forward's launch: (each net's nseq % 16 class, whether some CTAs of the ceil(max / 16) x n_nets grid are idle)"""
+    nseq = [agent_net.count(k) * B for k in range(max(agent_net) + 1)]
+    tiles = [(n + SEQS - 1) // SEQS for n in nseq]
+    return {_last_tile(n) for n in nseq}, min(tiles) < max(tiles)
 
 
 def tail_td_rows(agent_net, B, T, n_sm, cls):

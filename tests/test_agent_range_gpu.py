@@ -60,7 +60,10 @@ class Case:
     A: int = 6
     sharing: object = False       # the actor's (DQN: the agents') parameter sharing: False, True or a tuple of group labels
     critic_sharing: object = False
-    rnn: bool = False             # GRU agents (DQN) / GRU actor and critic (actor-critic)
+    rnn: bool = False             # GRU agents (DQN) / GRU actor (actor-critic)
+    critic_rnn: object = None     # GRU critic (None: as rnn)
+    H: int = 128                  # hidden width of the agents (DQN) / the actor
+    critic_H: int = 128
     B: int = 16                   # DQN: episodes per batch; actor-critic: environments (n_envs)
     T: int = 8
     double_q: bool = False
@@ -76,6 +79,10 @@ class Case:
     def joint(self):
         """the critic's input width (a centralised critic reads all N observations side by side)"""
         return self.N * self.D if self.kind in CENTRAL and self.N > 1 else self.D
+
+    @property
+    def crnn(self):
+        return self.rnn if self.critic_rnn is None else self.critic_rnn
 
     @property
     def tc_backward(self):
@@ -180,7 +187,7 @@ def _dqn_model(c):
     cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, double_q=c.double_q, target_update_interval_or_tau=c.tu,
                                 standardise_returns=c.standardise)
     cls = M.VDNetwork if c.kind == "vdn" else M.QNetwork
-    return cls([space(shape=(c.D,))] * c.N, [space(n=c.A)] * c.N, cfg, [128, 128], _sharing(c.sharing), c.rnn, True, "cuda", max_batch=c.B, max_episode_length=c.T)
+    return cls([space(shape=(c.D,))] * c.N, [space(n=c.A)] * c.N, cfg, [c.H, c.H], _sharing(c.sharing), c.rnn, True, "cuda", max_batch=c.B, max_episode_length=c.T)
 
 
 def _dqn_perturb(m):
@@ -208,8 +215,8 @@ def _dqn_store(c, seed, cap=None):
 
 
 def _dqn_ref(c):
-    """the oracle module of the case's agents: MLP (learner_ref) or GRU (gru_ref)"""
-    return gr if c.rnn else lr
+    """the oracle module of the case's agents: MLP (learner_ref) or GRU (gru_ref; tests/gru_ac_ref.py at a width below 128)"""
+    return (gr if c.H == gr.H else gar) if c.rnn else lr
 
 
 def _dqn_margin(c, st, b, hp):
@@ -259,7 +266,7 @@ def _check_dqn(c, m, st, st0, b64, want, met, hp, what, u=0, per_block=True):
 # ---- the actor-critic learners: the per-update checks of tests/test_rnn_ac_gpu.py (MLP or GRU parts) ---------------------------------------------
 def _rcase(c):
     """the case in tests/test_rnn_ac_gpu.py's terms, for its per-update checks"""
-    return rac.Case(ppo=c.kind in PPO, arnn=c.rnn, crnn=c.rnn, N=c.N, D=c.D, A=c.A, sharing=c.sharing, centralised=c.kind in CENTRAL, P=c.B, T=c.T,
+    return rac.Case(ppo=c.kind in PPO, arnn=c.rnn, crnn=c.crnn, N=c.N, D=c.D, A=c.A, sharing=c.sharing, centralised=c.kind in CENTRAL, P=c.B, T=c.T,
                     tu=c.tu, grad_clip=0.5, epochs=c.epochs, standardise=c.standardise)
 
 
@@ -270,8 +277,8 @@ def _ac_model(c, epochs=None):
     cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, n_steps=hp.n_steps, entropy_coef=hp.entropy_coef,
                                 value_loss_coef=hp.value_loss_coef, target_update_interval_or_tau=hp.target_update_interval_or_tau,
                                 standardise_returns=c.standardise, num_epochs=epochs or c.epochs, ppo_clip=0.2)
-    anet = types.SimpleNamespace(layers=[128, 128], parameter_sharing=_sharing(c.sharing), use_rnn=c.rnn, use_orthogonal_init=True, centralised=False)
-    cnet = types.SimpleNamespace(layers=[128, 128], parameter_sharing=_sharing(c.critic_sharing), use_rnn=c.rnn, use_orthogonal_init=True,
+    anet = types.SimpleNamespace(layers=[c.H, c.H], parameter_sharing=_sharing(c.sharing), use_rnn=c.rnn, use_orthogonal_init=True, centralised=False)
+    cnet = types.SimpleNamespace(layers=[c.critic_H, c.critic_H], parameter_sharing=_sharing(c.critic_sharing), use_rnn=c.crnn, use_orthogonal_init=True,
                                  centralised=c.kind in CENTRAL)
     cls = M.PPONetwork if c.kind in PPO else M.A2CNetwork
     return cls([space(shape=(c.D,))] * c.N, [space(n=c.A)] * c.N, cfg, anet, cnet, "cuda", max_envs=c.B, max_episode_length=c.T)
@@ -285,7 +292,7 @@ def _ac_oracle(c, m):
 
 def _ac_batch(c, seed):
     s = ac_batch(np.random.default_rng(seed), c.B, c.N, c.T, c.D, A=c.A)
-    if c.rnn:
+    if c.rnn or c.crnn:
         s["obs"] = (s["obs"] / 6.0).astype(np.float32)
     return s
 

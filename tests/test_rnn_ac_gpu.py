@@ -77,16 +77,14 @@ def _batch(c, rng):
 
 
 def _blocks(m, c):
-    """(name, slice) of every tensor of every actor and critic network in the flat [actor | critic] vector, GRU or MLP"""
+    """(name, slice) of every tensor of every actor and critic network in the flat [actor | critic] vector, GRU or MLP, at the model's widths"""
     out, o = [], 0
-    for part, rnn, n_nets, ind, outd in (("actor", c.arnn, m.n_actor_nets, c.D, c.A), ("critic", c.crnn, m.n_critic_nets, m.critic_in, 1)):
-        H = lr.H
-        if rnn:
-            names, sizes = GRU_NAMES, (H * ind, H, 3 * H * H, 3 * H * H, 3 * H, 3 * H, outd * H, outd)
-        else:
-            names, sizes = ("W1", "b1", "W2", "b2", "W3", "b3"), (H * ind, H, H * H, H, outd * H, outd)
+    for part, rnn, n_nets, shapes in (("actor", c.arnn, m.n_actor_nets, m._actor_shapes), ("critic", c.crnn, m.n_critic_nets, m._critic_shapes)):
+        names = GRU_NAMES if rnn else ("W1", "b1", "W2", "b2", "W3", "b3")
+        assert len(names) == len(shapes), (part, shapes)
         for k in range(n_nets):
-            for name, size in zip(names, sizes):
+            for name, (_, shape) in zip(names, shapes):
+                size = int(np.prod(shape))
                 out.append((f"{part}{k}.{name}", slice(o, o + size)))
                 o += size
     assert o == m.n_actor + m.n_critic

@@ -1,9 +1,9 @@
 """No GPU: tests/row_plan.py against the library's own planner, the class search on both H100 SM counts, and the edges of
-tests/test_tc_train_edges_gpu.py's shape tables.
+tests/test_tc_train_edges_gpu.py's and tests/test_gru_edges_gpu.py's shape tables.
 
-The planner check compiles a host-only driver that includes csrc/learner.cuh (nvcc with the library's flags, no device code runs) and prints
-episode_plan's cta_begin and every CTA's [row_begin, row_end).  cta_rows itself is device code: the driver restates its split in C++ integer
-arithmetic."""
+The planner check compiles a host-only driver that includes csrc/gru.cuh and csrc/learner.cuh (nvcc with the library's flags, no device code
+runs) and prints episode_plan's and the GRU backward's make_plan(ns, B, 1, n_sm, kGruSeqs) cta_begin and every CTA's [row_begin, row_end).
+cta_rows itself is device code: the driver restates its split in C++ integer arithmetic."""
 import subprocess
 
 import numpy as np
@@ -11,30 +11,40 @@ import pytest
 
 from codebase_b200.csrc import build as native_build
 from tests import row_plan as rp
+from tests import test_gru_edges_gpu as ge
 from tests import test_tc_train_edges_gpu as g
 
 DRIVER = r"""
-#include "learner.cuh"
+#include "gru.cuh"
 #include <stdio.h>
 using namespace marl;
-// stdin: lines "N B T n_sm agent_net[0..N)"; stdout per line: "n_cta cta_begin[0..n_nets] | net row_begin row_end ..." (one triple per CTA)
+// stdin: lines "N B T n_sm agent_net[0..N)"; stdout per line, for episode_plan(ns, B, T, n_sm) and then for the GRU backward's
+// make_plan(ns, B, 1, n_sm, kGruSeqs): "n_cta cta_begin[0..n_nets] | net row_begin row_end ..." (one triple per CTA), the two joined by " || "
+static void print_plan(const RowPlan& p) {
+  const int n_cta = p.cta_begin[p.n_nets];
+  printf("%d", n_cta);
+  for (int k = 0; k <= p.n_nets; ++k) printf(" %d", p.cta_begin[k]);
+  printf(" |");
+  for (int c = 0; c < n_cta; ++c) {   // cta_rows with blockIdx.x = c
+    int net = 0;
+    while (net + 1 < p.n_nets && c >= p.cta_begin[net + 1]) ++net;
+    const int ncta = p.cta_begin[net + 1] - p.cta_begin[net], k = c - p.cta_begin[net];
+    const long long units = (long long)(p.slot_begin[net + 1] - p.slot_begin[net]) * p.units_per_agent;
+    printf(" %d %d %d", net, (int)(units * k / ncta) * p.unit_rows, (int)(units * (k + 1) / ncta) * p.unit_rows);
+  }
+}
 int main() {
   int N, B, T, n_sm;
   while (scanf("%d %d %d %d", &N, &B, &T, &n_sm) == 4) {
     NetSet ns; ns.n_agents = N; ns.n_nets = 0;
     for (int a = 0; a < N; ++a) { scanf("%d", &ns.agent_net[a]); if (ns.agent_net[a] + 1 > ns.n_nets) ns.n_nets = ns.agent_net[a] + 1; }
-    const RowPlan p = episode_plan(ns, B, T, n_sm);
-    const int n_cta = p.cta_begin[p.n_nets];
-    printf("%d", n_cta);
-    for (int k = 0; k <= p.n_nets; ++k) printf(" %d", p.cta_begin[k]);
-    printf(" |");
-    for (int c = 0; c < n_cta; ++c) {   // cta_rows with blockIdx.x = c
-      int net = 0;
-      while (net + 1 < p.n_nets && c >= p.cta_begin[net + 1]) ++net;
-      const int ncta = p.cta_begin[net + 1] - p.cta_begin[net], k = c - p.cta_begin[net];
-      const long long units = (long long)(p.slot_begin[net + 1] - p.slot_begin[net]) * p.units_per_agent;
-      printf(" %d %d %d", net, (int)(units * k / ncta) * p.unit_rows, (int)(units * (k + 1) / ncta) * p.unit_rows);
-    }
+    print_plan(episode_plan(ns, B, T, n_sm));
+    printf(" || ");
+    const RowPlan q = make_plan(ns, B, 1, n_sm, kGruSeqs);
+    print_plan(q);
+    printf(" || %d", q.n_nets);
+    for (int k = 0; k <= q.n_nets; ++k) printf(" %d", q.slot_begin[k]);
+    for (int a = 0; a < N; ++a) printf(" %d", q.slot_agent[a]);
     printf("\n");
   }
   return 0;
@@ -71,16 +81,22 @@ def test_mirror_matches_the_library_planner(driver):
     stdin = "".join(f"{N} {B} {T} {n_sm} {' '.join(map(str, nets))}\n" for N, B, T, n_sm, nets in cfgs)
     lines = subprocess.run([driver], input=stdin, capture_output=True, text=True, check=True).stdout.splitlines()
     assert len(lines) == len(cfgs)
-    seen = set()
+    seen, seen_gru = set(), set()
     for (N, B, T, n_sm, nets), line in zip(cfgs, lines):
-        head, rows = line.split("|")
-        head, rows = [int(x) for x in head.split()], [int(x) for x in rows.split()]
-        p = rp.episode_plan(nets, B, T, n_sm)
-        assert head[0] == p["cta_begin"][-1] and head[1:] == p["cta_begin"], (N, B, T, n_sm, nets)
-        want = [x for r in rp.all_cta_rows(p) for x in r]
-        assert rows == want, (N, B, T, n_sm, nets)
+        episodes, seqs, slots = line.split(" || ")
+        for p, part in ((rp.episode_plan(nets, B, T, n_sm), episodes), (rp.gru_plan(nets, B, n_sm), seqs)):
+            head, rows = part.split("|")
+            head, rows = [int(x) for x in head.split()], [int(x) for x in rows.split()]
+            assert head[0] == p["cta_begin"][-1] and head[1:] == p["cta_begin"], (N, B, T, n_sm, nets)
+            want = [x for r in rp.all_cta_rows(p) for x in r]
+            assert rows == want, (N, B, T, n_sm, nets)
+        slots = [int(x) for x in slots.split()]
+        n_nets = slots[0]
+        assert slots[1:n_nets + 2] == p["slot_begin"] and slots[n_nets + 2:] == p["slot_agent"], (N, nets)   # what seq_of reads
         seen |= rp.plan_classes(tuple(nets), B, T, n_sm)
-    assert len(seen) >= 12, sorted(seen)   # the random configs are not the coverage: find_batch is
+        seen_gru |= rp.gru_classes(tuple(nets), B, n_sm)
+    assert len(seen) >= 12, sorted(seen)   # the random configs are not the coverage: find_batch / find_units are
+    assert len(seen_gru) >= 6, sorted(seen_gru)
 
 
 def test_classes_of_rows():
@@ -167,3 +183,74 @@ def test_cases_sit_on_the_edges_they_claim():
     # handle reuse: a smaller batch and a shorter T than the handle was created for
     for name, (big, small) in g.REUSE_SHAPES.items():
         assert small[0] < big[0] and small[1] < big[1], name
+
+
+# ---- the GRU split (tests/test_gru_edges_gpu.py) -------------------------------------------------------------------------------------------------
+def test_seq_classes():
+    assert [rp.seq_class(n) for n in (1, 7, 8, 9, 15, 16)] == ["t1-lower", "t1-lower", "t1-half", "t1-upper", "t1-upper", "t1-full"]
+    assert [rp.seq_class(n) for n in (17, 24, 25, 32, 33, 48, 49, 1000)] == ["t2-lower", "t2-half", "t2-upper", "t2-full", "t3+-lower", "t3+-full",
+                                                                             "t3+-lower", "t3+-half"]
+    assert len(set(rp.SEQ_CLASSES)) == 12 and {rp.seq_class(n) for n in range(1, 200)} == set(rp.SEQ_CLASSES)
+
+
+def test_edge_sequences_of_a_small_plan():
+    """2 agents sharing a net, B = 21, 2 SMs: 42 sequences on 2 CTAs of 21 (t2-lower); CTA 0 holds agent 0's 0..20 (tiles 0..15, 16..20), CTA 1
+    agent 1's, no tile straddles.  3 agents, B = 17, 2 SMs: 51 sequences on CTAs of 25 and 26; CTA 0's second tile 16..24 is agent 0's b = 16
+    and agent 1's 0..7, CTA 1 (25..50) holds agent 1's 8..16 and agent 2's 0..16, its first tile 25..40 straddles too"""
+    p = rp.gru_plan([0, 0], 21, 2)
+    assert rp.all_cta_rows(p) == [(0, 0, 21), (0, 21, 42)] and rp.seq_class(21) == "t2-lower"
+    assert rp.cta_edge_sequences(p) == [(0, 0), (0, 15), (0, 16), (0, 20), (1, 0), (1, 15), (1, 16), (1, 20)]
+    assert not rp.straddles(21, 0, 21) and not rp.straddles(21, 21, 42)
+    q = rp.gru_plan([0, 0, 0], 17, 2)
+    assert rp.all_cta_rows(q) == [(0, 0, 25), (0, 25, 51)] and rp.straddles(17, 0, 25) and rp.straddles(17, 25, 51)
+    assert rp.cta_edge_sequences(q) == [(0, 0), (0, 15), (0, 16), (1, 7), (1, 8), (2, 6), (2, 7), (2, 16)]
+    assert rp.GRU_STRADDLE in rp.gru_classes((0, 0, 0), 17, 2) and rp.GRU_STRADDLE not in rp.gru_classes((0, 0), 21, 2)
+    assert rp.forward_shapes([0, 1, 0, 0], 5) == ({"upper", "lower"}, False) and rp.forward_shapes([0, 1, 0, 0], 6) == ({"lower"}, True)   # 18 and 6 sequences: 2 tiles and 1
+
+
+@pytest.mark.parametrize("n_sm", [114, 132])
+def test_every_gru_case_finds_its_class(n_sm):
+    """each case of tests/test_gru_edges_gpu.py finds its class on an H100 PCIe (114 SMs) and SXM (132 SMs) within the sequence budget; the class
+    sweep covers all 15; its edge episodes are the first and last of every CTA and tile; the training forwards cover every nseq % 16 class and a
+    launch with idle CTAs"""
+    covered, fwd, idle = set(), set(), False
+    for name, c in ge.all_train_cases():
+        B = ge.units(c, n_sm)
+        nets = rp.nets_of(c.N, c.sharing)
+        assert c.cls in rp.gru_classes(tuple(nets), B, n_sm) and c.N * B <= ge.MAX_SEQS, (n_sm, name, B)
+        if name in ge.CLASS_CASES:
+            covered |= rp.gru_classes(tuple(nets), B, n_sm)
+        p = rp.gru_plan(nets, B, n_sm)
+        edges = rp.cta_edge_sequences(p)
+        for net, v0, v1 in rp.all_cta_rows(p):
+            assert rp.seq_of(p, net, v0) in edges and rp.seq_of(p, net, v1 - 1) in edges
+        r, i = rp.forward_shapes(nets, B)
+        fwd |= r; idle |= i
+    assert covered == set(rp.GRU_CLASSES) and set(ge.CLASS_CASES) == set(rp.GRU_CLASSES), sorted(set(rp.GRU_CLASSES) - covered)
+    assert fwd == set(rp.FWD_REMAINDERS) and idle, (fwd, idle)
+
+
+def test_gru_cases_sit_on_the_edges_they_claim():
+    C = ge.CLASS_CASES
+    kinds = {c.kind for c in C.values()}
+    assert kinds == {"idqn", "vdn", "qmix", "ia2c", "ippo", "maa2c", "mappo"}, kinds
+    assert any(c.sharing is False and c.N > 1 for c in C.values()) and any(c.sharing is True for c in C.values())
+    assert any(c.sharing == ge.SEPS for c in C.values()) and any(c.sharing == ge.GROUPS4 for c in C.values())
+    # one recurrent actor with an MLP critic, one MLP actor with a recurrent centralised critic
+    assert any(c.arnn and not c.crnn for c in C.values()) and any(not c.arnn and c.crnn and c.kind in ge.CENTRAL for c in C.values())
+    for cls, c in C.items():   # short episodes at the multi-tile classes keep the oracle cheap
+        assert not cls.startswith(("t2", "t3")) or 2 <= c.T <= 8, cls
+    W = ge.WIDTH_CASES
+    assert {1, 2, 37, 100, 127} <= {c.H for c in W.values()} | {c.critic_H for c in W.values() if not c.dqn}
+    assert all(c.dqn or c.H != c.critic_H for c in W.values())
+    assert {c.D for c in W.values() if c.dqn} == {1, 31, 32} and {33, 64, 128} <= {c.D for c in W.values() if not c.dqn}
+    assert any(c.kind in ge.CENTRAL and c.N * c.D == 128 for c in W.values())
+    assert {c.A for c in W.values()} == {1, 2, 3, 5, 8} and all(c.dqn for c in W.values() if c.A == 1)
+    assert all(c.cls in ("t2-upper", "t3+-lower") for c in W.values())
+    L = ge.LENGTH_CASES
+    assert {c.T for c in L.values()} == {1, 2, 100} and {c.kind for c in L.values() if c.T == 100} == {"idqn", "vdn", "ippo"}
+    assert all(c.cls.startswith("t1") for c in L.values() if c.T == 100)
+    assert ge.ACT_E == (1, 17, 9001) and {c.H for c in ge.ACT_CASES.values()} == {37, 128}
+    assert all(c.cls.startswith(("t2", "t3")) for c in ge.REUSE_CASES.values())
+    rows = [c.N * P * c.T for c, P in ge.HEAD_CASES.values()]
+    assert any(r % 256 == 0 for r in rows) and any(r % 256 == 1 and r > 256 for r in rows) and any(r < 256 for r in rows)
