@@ -4,13 +4,15 @@ Same constructor signature / Hydra `_target_` role (configs/algorithm/ia2c.yaml:
 `state_dict()` key names (`actor.independent.{i}.network.…`, `critic.…`, `target_critic.…`; shared: `.networks.{k}.`; recurrent parts:
 `actor.independent.{i}.first_layer.weight`, `….rnn.weight_ih_l0`, …).
 All arithmetic runs in libmarlb200.so (marl_a2c_*): actor forward, target-critic pass, n-step returns
-(utils/utils.py:38-63), fused forward / loss / backward of critic and actor, Adam, target sync.  No CPU fallback.
+(utils/utils.py:38-63) or, with `gae_lambda` set, λ-returns, fused forward / loss / backward of critic and actor, Adam, target sync.  No CPU fallback.
 `actor.use_rnn` / `critic.use_rnn` make that part the reference's RNNNetwork (one GRU layer), independently of each other.  `actor.layers` and
 `critic.layers` are [H, H] with 1 <= H <= 128, each part its own H.
 """
 from __future__ import annotations
 
 import ctypes as C
+import numbers
+import types
 
 import torch
 
@@ -42,10 +44,25 @@ def check_input_widths(obs_space, critic):
         raise NotImplementedError(f"{'; '.join(why)}: the actor-critic kernels take at most {MAX_IN_DIM} input features")
 
 
+def gae_lambda(cfg):
+    """cfg.gae_lambda: None (absent or null: the reference's n-step returns) or the λ in [0, 1] of the λ-returns that replace them.  Anything else
+    raises ValueError here, before any native call."""
+    lam = getattr(cfg, "gae_lambda", None)
+    if lam is None:
+        return None
+    if isinstance(lam, bool) or not isinstance(lam, numbers.Real):
+        raise ValueError(f"algorithm.gae_lambda must be null or a number in [0, 1], not {lam!r}")
+    lam = float(lam)
+    if not 0.0 <= lam <= 1.0:
+        raise ValueError(f"algorithm.gae_lambda must be in [0, 1], not {lam}")
+    return lam
+
+
 class A2CNetwork(NativeLearner):
     _destroy = "marl_a2c_destroy"
 
     def __init__(self, obs_space, action_space, cfg, actor, critic, device, max_envs=None, max_episode_length=None):
+        self.gae_lambda = gae_lambda(cfg)
         check_input_widths(obs_space, critic)
         self.actor_hidden = hidden_width(actor.layers, "actor.layers", bool(actor.use_rnn))
         self.critic_hidden = hidden_width(critic.layers, "critic.layers", bool(critic.use_rnn))
@@ -99,6 +116,14 @@ class A2CNetwork(NativeLearner):
         self.standardise_returns = bool(getattr(cfg, "standardise_returns", False))   # ac/model.py:112-114
         if self.standardise_returns:
             nat.check(self._lib.marl_a2c_standardise_returns(self._h, C.c_int32(1)), "marl_a2c_standardise_returns")
+        if self.gae_lambda is not None:
+            self.set_gae_lambda(self.gae_lambda)
+
+    def set_gae_lambda(self, lam):
+        """λ-returns of `lam` in [0, 1] in place of the n-step returns from the next update on (DESIGN.md §4.4c); None: the n-step returns again"""
+        lam = gae_lambda(types.SimpleNamespace(gae_lambda=lam))
+        nat.check(self._lib.marl_a2c_set_gae_lambda(self._h, C.c_int32(lam is not None), C.c_float(0.0 if lam is None else lam)), "marl_a2c_set_gae_lambda")
+        self.gae_lambda = lam
 
     def ret_ms(self):
         """(mean[N], var[N], count) of the RunningMeanStd over the returns (standardise_returns), as CPU values."""

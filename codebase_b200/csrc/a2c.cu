@@ -48,6 +48,68 @@ __global__ void nstep_returns_kernel(NStepParams p) {
   p.ret[i] = acc;
 }
 
+// λ-returns (algorithm.gae_lambda): the mixture (1 - λ) Σ_{n>=1} λ^(n-1) G_t^(n) of the n-step returns above, by the backward recursion
+//   R_t = a_t + b R_{t+1},  a_t = m_t r_t + γ(1 - λ) m_{t+1} V_{t+1},  b = γλ,  m_t = 1 - d_t,  R_T = 0 and m_T V_T taken as 0.
+// One warp per (agent, env) sequence, right to left over windows of 32 x kLamChunk steps: the warp stages a_t coalesced into shared memory, each
+// lane folds its kLamChunk-step chunk into the affine map R_in -> c + g R_in, a fixed-order suffix scan over the lanes composes the maps, each
+// lane replays its chunk from the return after it, and the warp writes the returns coalesced.  The window's first return carries into the next.
+constexpr int kLamChunk = 8, kLamWindow = 32 * kLamChunk, kLamWarps = 8;
+
+struct LambdaParams {
+  const float* vt;     // [N][P][T+1] target-critic values
+  TrajView traj; const int32_t* idx; int N, P;
+  float coef_v, coef_r;   // float32(γ(1 - λ)), float32(γλ)
+  float* ret;          // [N][P][T]
+  const float* ret_ms; // [mean[N] | var[N]] of the running return statistics, or NULL
+};
+
+__device__ __forceinline__ int lam_slot(int s) { return (s / kLamChunk) * (kLamChunk + 1) + s % kLamChunk; }   // lane chunks padded: no bank conflicts
+
+__global__ void lambda_returns_kernel(LambdaParams p) {
+  __shared__ float buf[kLamWarps][32 * (kLamChunk + 1)];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, seq = blockIdx.x * kLamWarps + w;
+  if (seq >= p.N * p.P) return;
+  const int T = p.traj.T, a = seq / p.P, b = seq - a * p.P;
+  const size_t ep = (size_t)p.idx[b];
+  const float* vt = p.vt + row_index(a, b, 0, p.P, T + 1);
+  const float* rew = p.traj.rew + p.traj.step_at(ep, a, 0);
+  const uint8_t* done = p.traj.done + p.traj.done_at(ep, 0);
+  float* ret = p.ret + row_index(a, b, 0, p.P, T);
+  const float mean = p.ret_ms ? p.ret_ms[a] : 0.f, var = p.ret_ms ? p.ret_ms[p.N + a] : 1.f;
+  float* s = buf[w];
+  float carry = 0.f;   // R at the step after the window
+  for (int w0 = ((T - 1) / kLamWindow) * kLamWindow; w0 >= 0; w0 -= kLamWindow) {
+    const int len = min(kLamWindow, T - w0);
+    for (int j = lane; j < len; j += 32) {
+      const int t = w0 + j;
+      float av = 0.f;
+      if (t + 1 < T) {
+        float v = vt[t + 1];
+        if (p.ret_ms) v = unstandardise(v, mean, var);
+        av = (p.coef_v * v) * (1.f - (float)done[t + 1]);
+      }
+      s[lam_slot(j)] = rew[t] * (1.f - (float)done[t]) + av;
+    }
+    __syncwarp();
+    const int lo = lane * kLamChunk, hi = min(lo + kLamChunk, len);
+    float c = 0.f, g = 1.f;   // this lane's chunk: R_lo = c + g R_hi
+    for (int j = hi - 1; j >= lo; --j) { c = s[lam_slot(j)] + p.coef_r * c; g *= p.coef_r; }
+    // suffix scan: lane l ends with the composition of the maps of lanes l .. 31
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const float c2 = __shfl_down_sync(0xffffffffu, c, off), g2 = __shfl_down_sync(0xffffffffu, g, off);
+      if (lane + off < 32) { c = c + g * c2; g *= g2; }
+    }
+    float r = __shfl_down_sync(0xffffffffu, c + g * carry, 1);   // R at the step after this lane's chunk
+    if (lane == 31) r = carry;
+    for (int j = hi - 1; j >= lo; --j) { r = s[lam_slot(j)] + p.coef_r * r; s[lam_slot(j)] = r; }
+    carry = __shfl_sync(0xffffffffu, r, 0);   // R_{w0}, as written
+    __syncwarp();
+    for (int j = lane; j < len; j += 32) ret[w0 + j] = s[lam_slot(j)];
+    __syncwarp();
+  }
+}
+
 // log-probabilities of the taken actions under the collecting policy (ac/model.py:281-292), from the actor outputs of every gathered row:
 // old_logp[a][b][t] = log_softmax(logits[a][b][t][:])[act[a][b][t]] -- the formulas of head_a2c_actor (learner_kernels.cu)
 struct OldLogpParams { const float* logits; TrajView traj; const int32_t* idx; int N, P, A; float* out; };
@@ -109,6 +171,7 @@ struct marl_a2c : LearnerHandle {
   // [N][P][T+1][kGruSaveRow] (one buffer: the critic pass ends before the actor pass starts)
   int actor_rnn = 0, critic_rnn = 0; GruLayout agl = {}, cgl = {};
   float *rnn_q = nullptr, *rnn_dq = nullptr, *gru_save = nullptr;
+  int gae = 0; float gae_lambda = 0.f;   // algorithm.gae_lambda: λ-returns (lambda_returns_kernel) in place of the n-step returns
 };
 constexpr int kMaxPpoEpochs = 64;
 
@@ -271,11 +334,18 @@ static int a2c_prepare(marl_a2c* h, const marl_traj_view* batch, int32_t n_envs,
   } else {
     if (int rc = forward_any(h->critic, ps.cplan, ps.csrc, h->theta_tgt, h->image, h->vt, st)) return rc;
   }
-  // 2. n-step returns (ac/model.py:198-201)
-  NStepParams np; np.vt = h->vt; np.traj = ps.src.traj; np.idx = h->idx; np.N = N; np.P = n_envs; np.n_steps = h->hp.n_steps; np.ret = h->ret;
-  np.ret_ms = h->standardise ? h->ret_ms : nullptr;
-  for (int k = 0; k <= h->hp.n_steps; ++k) np.gpow[k] = (float)pow((double)h->hp.gamma, (double)k);
-  nstep_returns_kernel<<<(N * n_envs * T + 255) / 256, 256, 0, st>>>(np);
+  // 2. n-step returns (ac/model.py:198-201), or the λ-returns of algorithm.gae_lambda
+  if (h->gae) {
+    LambdaParams lp; lp.vt = h->vt; lp.traj = ps.src.traj; lp.idx = h->idx; lp.N = N; lp.P = n_envs; lp.ret = h->ret;
+    lp.ret_ms = h->standardise ? h->ret_ms : nullptr;
+    lp.coef_v = (float)((double)h->hp.gamma * (1.0 - (double)h->gae_lambda)); lp.coef_r = (float)((double)h->hp.gamma * (double)h->gae_lambda);
+    lambda_returns_kernel<<<(N * n_envs + kLamWarps - 1) / kLamWarps, 32 * kLamWarps, 0, st>>>(lp);
+  } else {
+    NStepParams np; np.vt = h->vt; np.traj = ps.src.traj; np.idx = h->idx; np.N = N; np.P = n_envs; np.n_steps = h->hp.n_steps; np.ret = h->ret;
+    np.ret_ms = h->standardise ? h->ret_ms : nullptr;
+    for (int k = 0; k <= h->hp.n_steps; ++k) np.gpow[k] = (float)pow((double)h->hp.gamma, (double)k);
+    nstep_returns_kernel<<<(N * n_envs * T + 255) / 256, 256, 0, st>>>(np);
+  }
   MARL_CUDA_TRY(cudaGetLastError());
   if (h->standardise) {  // ac/model.py:202-204
     RetMsParams rp; rp.ret = h->ret; rp.N = N; rp.P = n_envs; rp.T = T; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count;
@@ -292,6 +362,15 @@ int marl_a2c_standardise_returns(marl_a2c* h, int32_t enable) {
   if (enable)
     if (int rc = enable_ret_stats(h, h->actor.n_agents, "marl_a2c_standardise_returns")) return rc;
   h->standardise = enable ? 1 : 0;
+  return MARL_OK;
+}
+/* algorithm.gae_lambda: enable != 0 replaces the n-step returns of every later update (A2C and PPO) by the λ-returns of `lambda` in [0, 1];
+ * enable == 0 restores them.  n_steps is not read while λ-returns are on. */
+int marl_a2c_set_gae_lambda(marl_a2c* h, int32_t enable, float lambda) {
+  MARL_REQUIRE(h != nullptr, "marl_a2c_set_gae_lambda: NULL handle");
+  MARL_REQUIRE(!enable || (lambda >= 0.f && lambda <= 1.f), "marl_a2c_set_gae_lambda: lambda %g is outside [0, 1]", (double)lambda);
+  h->gae = enable ? 1 : 0;
+  h->gae_lambda = enable ? lambda : 0.f;
   return MARL_OK;
 }
 /* the running statistics as device pointers: ret_ms float[2 n_agents] = mean | var, count double[1] (NULL before the first enable) */

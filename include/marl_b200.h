@@ -430,6 +430,11 @@ int marl_a2c_set_optimizer(marl_a2c* a, const marl_optimizer* opt);
  * the statistics absorb the batch's returns (all T x P of them, unmasked), the returns are standardised.  enable != 0 initialises them on first use. */
 int marl_a2c_standardise_returns(marl_a2c* a, int32_t enable);
 int marl_a2c_ret_ms_ptrs(marl_a2c* a, float** ret_ms /* mean[N] | var[N] */, double** count);
+/* algorithm.gae_lambda (IA2C, IPPO, MAA2C, MAPPO): enable != 0 makes every later update (marl_a2c_update*, marl_ppo_update / _prepare) use the
+ * λ-returns R_t = (1 - λ) Σ_{n>=1} λ^(n-1) G_t^(n) over the n-step returns G^(n) of compute_nstep_returns (the same masks, the same target-critic
+ * values, de-standardised under standardise_returns) in place of the n_steps-step return; hp.n_steps is not read meanwhile.  λ = 0 is the one-step
+ * return, λ = 1 the return to the end of the stored episode.  enable == 0 restores the n-step returns.  A λ outside [0, 1] is refused (MARL_EINVAL). */
+int marl_a2c_set_gae_lambda(marl_a2c* a, int32_t enable, float lambda);
 /* PPONetwork.update (marlbase/ac/model.py:265-352; configs/algorithm/ippo.yaml: num_epochs 4, ppo_clip 0.2, grad_clip 0.5) on an A2C handle:
  * n-step returns and the collecting policy's log-probabilities once, then num_epochs optimisation steps on the same batch with the clipped
  * surrogate; the target critic follows after the last epoch.  metrics_out: device float[6] as marl_a2c_update, averaged over the epochs. */
