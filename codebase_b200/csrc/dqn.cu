@@ -399,12 +399,16 @@ int marl_replay_sample(uint64_t seed, uint64_t update_idx, int32_t batch, int32_
   return MARL_OK;
 }
 
+static bool dqn_external_head(const marl_dqn* h) { return h->hp.mixer != 0 || h->rnn || h->standardise; }
+
 // The external TD head, for the cases the training pass's own head does not cover (QMIX, standardise_returns, VDN, the recurrent pass): the online
-// forward on every row, then dL/dQ of the taken actions into td, which becomes tp.td_ext (per agent at tp.td_agent_stride; VDN: per (b, t), stride 0),
-// and the head's loss statistics into loss_part blocks [n_loss_parts, ...), which n_loss_parts is advanced past.
-static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, int batch, TrainParams& tp, int& n_loss_parts, cudaStream_t st) {
-  if (h->hp.mixer == 0 && !h->rnn && !h->standardise) return MARL_OK;
-  if (int rc = dqn_forward(h, plan, src, false, h->q_all, h->gru_save, st)) return rc;
+// forward on every row (forward = false: the fused training forward has already written q_all), then dL/dQ of the taken actions into td, which
+// becomes tp.td_ext (per agent at tp.td_agent_stride; VDN: per (b, t), stride 0), and the head's loss statistics into loss_part blocks
+// [n_loss_parts, ...), which n_loss_parts is advanced past.
+static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, int batch, TrainParams& tp, int& n_loss_parts, bool forward, cudaStream_t st) {
+  if (!dqn_external_head(h)) return MARL_OK;
+  if (forward)
+    if (int rc = dqn_forward(h, plan, src, false, h->q_all, h->gru_save, st)) return rc;
   const int T = src.traj.T;
   float* loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
   tp.td_ext = h->td;
@@ -461,17 +465,11 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
   return MARL_OK;
 }
 
-// The training pass from tp.td_ext, or from the agents' own TD head: GRU BPTT, the tensor-core pipeline (between: two timing events recorded
-// between its kernels, NULL: none; tc is set when it runs) or the fused FP32 kernel.
-static int dqn_train_pass(marl_dqn* h, const TrainParams& tp, cudaEvent_t* between, bool& tc, cudaStream_t st) {
-  tc = false;
-  if (h->rnn) {
-    GruBwdParams bp; memset(&bp, 0, sizeof(bp));
-    bp.plan = tp.plan; bp.traj = tp.src.traj; bp.idx = tp.src.idx; bp.B = tp.plan.units_per_agent; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
-    bp.td = tp.td_ext; bp.td_agent_stride = tp.td_agent_stride; bp.src = tp.src; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
-    return launch_gru_backward(bp, st);
-  }
-  if (!tc_backward_enabled() || h->ns.in >= kMaxObsDim || h->image == nullptr) return launch_train(tp, kHeadDqn, st);   // (no image: hidden width below 128)
+// Does the tensor-core training pipeline run (else GRU BPTT or the fused FP32 kernel)?  (No image: hidden width below 128.)
+static bool dqn_tc_train(const marl_dqn* h) { return !h->rnn && tc_backward_enabled() && h->ns.in < kMaxObsDim && h->image != nullptr; }
+
+// The tensor-core pipeline's buffers (allocated on first use) and current online images
+static int dqn_tc_prepare(marl_dqn* h, TcBuffers& tb, cudaStream_t st) {
   if (!h->tc_h2) {  // intermediates of the tensor-core pipeline, allocated on first use (observation rows at pitch 8 ceil(in / 8))
     const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), F = sizeof(float);
     if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h2, rows * kHidden * F},
@@ -483,9 +481,47 @@ static int dqn_train_pass(marl_dqn* h, const TrainParams& tp, cudaEvent_t* betwe
     if (int rc = launch_pack_weights(h->theta, h->ns.lay, h->ns.n_nets, h->image, st, h->image_bwd)) return rc;
     h->image_current = h->bwd_image_current = true;
   }
-  TcBuffers tb; tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h2 = h->tc_h2; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
+  tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h2 = h->tc_h2; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
+  return MARL_OK;
+}
+
+// The training pass from tp.td_ext, or from the agents' own TD head: GRU BPTT, the tensor-core pipeline (between: two timing events recorded
+// between its kernels, NULL: none; tc is set when it runs) or the fused FP32 kernel.
+static int dqn_train_pass(marl_dqn* h, const TrainParams& tp, cudaEvent_t* between, bool& tc, cudaStream_t st) {
+  tc = false;
+  if (h->rnn) {
+    GruBwdParams bp; memset(&bp, 0, sizeof(bp));
+    bp.plan = tp.plan; bp.traj = tp.src.traj; bp.idx = tp.src.idx; bp.B = tp.plan.units_per_agent; bp.theta = h->theta; bp.lay = h->gl; bp.save = h->gru_save;
+    bp.td = tp.td_ext; bp.td_agent_stride = tp.td_agent_stride; bp.src = tp.src; bp.scratch = h->scratch; bp.scratch_pitch = h->scratch_pitch;
+    return launch_gru_backward(bp, st);
+  }
+  if (!dqn_tc_train(h)) return launch_train(tp, kHeadDqn, st);
+  TcBuffers tb;
+  if (int rc = dqn_tc_prepare(h, tb, st)) return rc;
   tc = true;
-  return launch_tc_dqn_train(tp, tb, st, between);
+  if (int rc = launch_tc_dqn_forward(tp, tb, nullptr, nullptr, nullptr, st)) return rc;
+  if (between) MARL_CUDA_TRY(cudaEventRecord(between[0], st));
+  return launch_tc_dqn_backward(tp, tb, st, between ? between[1] : nullptr);
+}
+
+// The tensor-core training pass with the target network in its forward kernel: pack the stale images, then one forward kernel for both networks
+// (q_all too when an external TD head runs), the external head, the two backward kernels.  ev (NULL: none): 4 timing events, before the forward,
+// after it, after the dH1 kernel (the external head runs between the last two) and at the end.
+static int dqn_fused_pass(marl_dqn* h, const RowPlan& plan, const RowSource& src, int batch, TrainParams& tp, int& n_loss_parts, cudaEvent_t* ev,
+                          cudaStream_t st) {
+  TcBuffers tb;
+  if (int rc = dqn_tc_prepare(h, tb, st)) return rc;
+  if (!h->tgt_image_current) {
+    if (int rc = launch_pack_weights(h->theta_tgt, h->ns.lay, h->ns.n_nets, h->image_tgt, st)) return rc;
+    h->tgt_image_current = true;
+  }
+  if (ev) MARL_CUDA_TRY(cudaEventRecord(ev[0], st));
+  if (int rc = launch_tc_dqn_forward(tp, tb, h->image_tgt, h->tq, dqn_external_head(h) ? h->q_all : nullptr, st)) return rc;
+  if (ev) MARL_CUDA_TRY(cudaEventRecord(ev[1], st));
+  if (int rc = dqn_td_head(h, plan, src, batch, tp, n_loss_parts, false, st)) return rc;
+  if (int rc = launch_tc_dqn_backward(tp, tb, st, ev ? ev[2] : nullptr)) return rc;
+  if (ev) { MARL_CUDA_TRY(cudaEventRecord(ev[3], st)); h->ev_used += 1; h->ev_split = true; }
+  return MARL_OK;
 }
 
 // Gradient half of an update.  rp_out == NULL: the per-CTA partials are reduced into grad[] (grad_reduce_kernel); otherwise the
@@ -505,19 +541,25 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   // timing (bench.py's roofline leg): 4 events per timed update, around the training pass and between the tensor-core kernels; the recurrent
   // path's window opens before its online forward
   cudaEvent_t* ev = h->timing && h->ev_used < kTimingPairs ? &h->ev[4 * h->ev_used] : nullptr;
-  // target network on every gathered row (dqn/model.py:132-134); several ranks: the previous update launched it between its push and its finish
-  if (h->tq_ahead) h->tq_ahead = false;
-  else if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, st)) return rc;
   TrainParams tp; memset(&tp, 0, sizeof(tp));
   tp.plan = plan; tp.src = src; tp.theta = h->theta; tp.lay = h->ns.lay; tp.tq = h->tq;
   tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = h->loss_part;
   int n_loss_parts = h->rnn ? 0 : plan.cta_begin[plan.n_nets];
-  if (ev && h->rnn) cudaEventRecord(ev[0], st);
-  if (int rc = dqn_td_head(h, plan, src, batch, tp, n_loss_parts, st)) return rc;
-  if (ev && !h->rnn) cudaEventRecord(ev[0], st);
-  bool tc = false;
-  if (int rc = dqn_train_pass(h, tp, ev ? ev + 1 : nullptr, tc, st)) return rc;
-  if (ev) { cudaEventRecord(ev[3], st); h->ev_used += 1; h->ev_split |= tc; }
+  // The target network on every gathered row (dqn/model.py:132-134) runs inside the tensor-core training forward when that pipeline runs with the
+  // tensor-core forward on (an FP32 target forward gives other bits).  Otherwise it is a forward of its own; several ranks with the split exchange:
+  // the previous update launched it between its push and its finish.
+  if (!h->tq_ahead && dqn_tc_train(h) && tc_forward_enabled()) {
+    if (int rc = dqn_fused_pass(h, plan, src, batch, tp, n_loss_parts, ev, st)) return rc;
+  } else {
+    if (h->tq_ahead) h->tq_ahead = false;
+    else if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, st)) return rc;
+    if (ev && h->rnn) cudaEventRecord(ev[0], st);
+    if (int rc = dqn_td_head(h, plan, src, batch, tp, n_loss_parts, true, st)) return rc;
+    if (ev && !h->rnn) cudaEventRecord(ev[0], st);
+    bool tc = false;
+    if (int rc = dqn_train_pass(h, tp, ev ? ev + 1 : nullptr, tc, st)) return rc;
+    if (ev) { cudaEventRecord(ev[3], st); h->ev_used += 1; h->ev_split |= tc; }
+  }
   ReduceParams rp; rp.scratch = h->scratch; rp.loss_part = h->loss_part; rp.n_nets = h->ns.n_nets; rp.P = h->P(); rp.scratch_pitch = h->scratch_pitch;
   memcpy(rp.cta_begin, plan.cta_begin, sizeof(rp.cta_begin));
   rp.n_loss_parts = n_loss_parts; rp.grad = h->grad; rp.stats = h->grad + h->n_params; rp.stats_accumulate = 0; rp.sumsq_part = h->sumsq;
@@ -665,8 +707,10 @@ int marl_dqn_params_changed(marl_dqn* h) {
 }
 
 /* Per-kernel split of the launches timed by the last marl_dqn_timing(1) .. marl_dqn_timing(0) window: summed CUDA-event durations of
- * the three kernels of the tensor-core training pass (online forward + TD head, dH1, weight gradients).  *count = 0 when the window
- * ran the single fused FP32 kernel instead. */
+ * the three kernels of the tensor-core training pass (training forward, dH1 + TD head, weight gradients).  With the tensor-core forward on
+ * (and no split exchange), slot 0 is the forward of both the online and the target network, and for VDN, QMIX and standardise_returns slot 1
+ * includes the external TD head that runs between the forward and the dH1 kernel.  *count = 0 when the window ran the single fused FP32
+ * kernel instead. */
 int marl_dqn_timing_kernels(marl_dqn* h, float* ms3, int32_t* count) {
   MARL_REQUIRE(h != nullptr && ms3 != nullptr, "marl_dqn_timing_kernels: NULL argument");
   MARL_REQUIRE(!h->timing, "marl_dqn_timing_kernels: call marl_dqn_timing(q, 0, ...) first");

@@ -315,7 +315,11 @@ struct TcBuffers {
   size_t rows;                              // allocated rows
 };
 int tc_train_init();
-int launch_tc_dqn_train(const TrainParams& tp, const TcBuffers& buf, cudaStream_t st, cudaEvent_t* between = nullptr);  // between[2]: recorded after kernels 1 and 2
+// the training forward (tc_dqn_fwd_kernel): the online network, and with tgt_images the target network on the same rows into tq_out; q_out (optional):
+// the online outputs for an external TD head
+int launch_tc_dqn_forward(const TrainParams& tp, const TcBuffers& buf, const uint8_t* tgt_images, float* tq_out, float* q_out, cudaStream_t st);
+// the backward kernels (tc_dh1_kernel, tc_dw_kernel) behind it; after_dh1 (optional) is recorded between them
+int launch_tc_dqn_backward(const TrainParams& tp, const TcBuffers& buf, cudaStream_t st, cudaEvent_t after_dh1 = nullptr);
 // tc_forward_enabled(): process-wide switch (marl_set_option("tensor_core_forward", 0|1)), declared in common.cuh
 
 // Forward pass through whichever implementation is selected.  `image` is scratch for the packed weights (n_nets images);

@@ -2,6 +2,7 @@
 // matrix descriptors, mbarrier + TMA bulk copies, and the packed weight-image layout.
 #pragma once
 #include "learner.cuh"
+#include <type_traits>
 
 namespace marl {
 
@@ -97,6 +98,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// named CTA barrier `id` over `count` threads: sync waits for all of them, arrive counts the calling warp and goes on
+__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 // cp.async.bulk: one thread moves a contiguous, 16-byte aligned block global -> shared; completion is counted in bytes on an mbarrier
 // (expect_tx by the issuing thread).  The packed weight images are byte-for-byte shared-memory images, so an image is a few instructions
 // instead of a loop of per-thread copies, and the writes arrive through the async proxy, the one wgmma reads its operands through.
@@ -205,14 +209,6 @@ __device__ __forceinline__ void load_x_frag(const float* s0, const float* s1, in
     x[ks][2] = (s0 && c + 1 < D) ? s0[c + 1] : 0.f; x[ks][3] = (s1 && c + 1 < D) ? s1[c + 1] : 0.f;
   }
 }
-// A fragment order: (row 0, K t) = column 2t, (row 1, K t), (row 0, K t + 4) = column 2t + 1, (row 1, K t + 4)
-__device__ __forceinline__ void x_to_a(const float (&x)[kMaxObsDim / 8][4], uint32_t (&hi)[kMaxObsDim / 8][4], uint32_t (&lo)[kMaxObsDim / 8][4]) {
-#pragma unroll
-  for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {
-    tf32_split_u(x[ks][0], hi[ks][0], lo[ks][0]); tf32_split_u(x[ks][1], hi[ks][1], lo[ks][1]);
-    tf32_split_u(x[ks][2], hi[ks][2], lo[ks][2]); tf32_split_u(x[ks][3], hi[ks][3], lo[ks][3]);
-  }
-}
 // bias + ReLU of a layer-1 accumulator fragment
 __device__ __forceinline__ void bias_relu(float (&h)[64], const float* b, int quad_lane) {
 #pragma unroll
@@ -223,14 +219,20 @@ __device__ __forceinline__ void bias_relu(float (&h)[64], const float* b, int qu
 }
 // Layer 1 of a warpgroup's 64-row tile, H1 = relu(X W1^T + b1), in accumulator-fragment layout: x = this thread's A fragment (load_x_frag),
 // w1 = shared-memory address of the W1 hi panel of a forward image (the lo panel follows it, as in the image), b1 = its bias (shared memory),
-// k1steps = ceil(D / 8).  Every kernel that needs H1 computes it here: the same wgmma sequence on the same operands gives the same bits, so the
-// weight-gradient kernel rebuilds exactly the H1 the training forward used.
-__device__ __forceinline__ void layer1_tile(float (&h)[64], const float (&x)[kMaxObsDim / 8][4], uint32_t w1, const float* b1, int k1steps, int quad_lane) {
-  uint32_t xhi[kMaxObsDim / 8][4], xlo[kMaxObsDim / 8][4];
-  x_to_a(x, xhi, xlo);
+// K1 = ceil(D / 8) k-steps, a compile-time count so that ptxas issues the layer's wgmmas as one chain (a run-time bound makes it wait after each).
+// Every kernel that needs H1 computes it here: the same wgmma sequence on the same operands gives the same bits, so the weight-gradient kernel
+// rebuilds exactly the H1 the training forward used.
+template <int K1>
+__device__ __forceinline__ void layer1_tile(float (&h)[64], const float (&x)[kMaxObsDim / 8][4], uint32_t w1, const float* b1, int quad_lane) {
+  uint32_t xhi[K1][4], xlo[K1][4];   // A fragment order: (row 0, K t) = column 2t, (row 1, K t), (row 0, K t + 4) = column 2t + 1, (row 1, K t + 4)
+#pragma unroll
+  for (int ks = 0; ks < K1; ++ks) {
+    tf32_split_u(x[ks][0], xhi[ks][0], xlo[ks][0]); tf32_split_u(x[ks][1], xhi[ks][1], xlo[ks][1]);
+    tf32_split_u(x[ks][2], xhi[ks][2], xlo[ks][2]); tf32_split_u(x[ks][3], xhi[ks][3], xlo[ks][3]);
+  }
 #pragma unroll
   for (int i = 0; i < 64; ++i) h[i] = 0.f;
-  layer_rs<kMaxObsDim / 8>(h, xhi, xlo, w1, w1 + (kOffW1Lo - kOffW1Hi), k1steps);
+  layer_rs<K1>(h, xhi, xlo, w1, w1 + (kOffW1Lo - kOffW1Hi), K1);
   bias_relu(h, b1, quad_lane);
 }
 // values of a 64 x 128 fragment -> A operand registers (hi / lo) of the next product
@@ -266,6 +268,18 @@ __device__ __forceinline__ void head_quad(float (&h)[64], const float* b2, const
   }
 }
 
+// Launch an instantiation of a kernel template over K1 = ceil(D / 8) (layer1_tile), D <= kMaxObsDim: F(std::integral_constant<int, K1>)
+template <typename F>
+inline int with_k1(int D, F&& f) {
+  switch ((D + 7) >> 3) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 3: return f(std::integral_constant<int, 3>());
+    default: return f(std::integral_constant<int, 4>());
+  }
+}
+static_assert(kMaxObsDim == 32, "with_k1 instantiates k-step counts 1 to 4");
+
 // ---- the tensor-core training pass (tc_train.cu) ---------------------------------------------------------------------
 // Row records [rows][kRowRec] floats: [0, 8) online outputs, [16, 20) / [20, 24) ReLU masks of H1 / H2 (training forward); [8] dLoss/dq[act],
 // [9] act (int bits) (dH1 kernel).  Mask word q holds the columns of the fragment threads with lane % 4 == q: bit 2n + b = column 8n + 2q + b.
@@ -294,6 +308,9 @@ struct TcTrainParams {
   float* xg; int x_pitch;
   const float* tq; const float* td_ext; int td_agent_stride; float gamma; int double_q;
   float* scratch; int scratch_pitch; float* loss_part;
+  // training forward only: the target network's images (NULL: the forward runs the online network alone) and where its outputs go (tq's
+  // [rows][out] layout); q_out (NULL: none) receives the online outputs in the same layout, for an external TD head
+  const uint8_t* tgt_images; float* tq_out; float* q_out;
 };
 
 }  // namespace marl

@@ -47,6 +47,7 @@ TSG_DEFINE(g_ts_forward)
 TSG_GETTER(tsg_forward, g_ts_forward)
 // Two warpgroups, each running its own 64-row tiles through layer 1 -> layer 2 -> head with nothing shared but the weight image, so that the
 // CUDA-core epilogue of one overlaps the MMAs of the other.
+template <int K1>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel(FwdParams p, const uint8_t* __restrict__ images) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);  // swizzle atoms need 1024-byte alignment
@@ -66,7 +67,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel(FwdParams p, 
   const float* b2 = reinterpret_cast<const float*>(smem + kOffB2);
   const float* b3 = reinterpret_cast<const float*>(smem + kOffB3);
   const float* w3f = reinterpret_cast<const float*>(smem + kOffW3F);
-  const int D = p.src.D, out = p.lay.out, k1steps = (D + 7) >> 3;
+  const int D = p.src.D, out = p.lay.out;
   bool first = true;
   for (int vr0 = row_begin + kWgRows * wg; vr0 < row_end; vr0 += kTileRows) {
     const int r0 = vr0 + 16 * wq + g, r1 = r0 + 8;
@@ -78,7 +79,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel(FwdParams p, 
       float x[kMaxObsDim / 8][4];
       load_x_frag(s0, s1, D, tq, x);
       if (first) mbar_wait(bar, 0);
-      layer1_tile(acc, x, sb + kOffW1Hi, b1, k1steps, tq);
+      layer1_tile<K1>(acc, x, sb + kOffW1Hi, b1, tq);
     }
     {
       uint32_t hi[16][4], lo[16][4];
@@ -104,7 +105,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_forward_kernel(FwdParams p, 
 constexpr int kFwdSmem = kImageBytes + 64 + 1024;   // + mbarriers, + slack for the 1024-byte alignment
 
 int tc_forward_init() {
-  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
+  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_forward_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
+  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_forward_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
+  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_forward_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
+  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_forward_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdSmem));
   return MARL_OK;
 }
 
@@ -116,8 +120,10 @@ int launch_pack_weights(const float* theta, const NetLayout& lay, int n_nets, ui
 }
 
 int launch_tc_forward(const FwdParams& p, const uint8_t* images, cudaStream_t st) {
-  MARL_CUDA_TRY(launch_pdl(tc_forward_kernel, dim3(p.plan.cta_begin[p.plan.n_nets]), dim3(kTcThreads), kFwdSmem, st, p, images));
-  return MARL_OK;
+  return with_k1(p.src.D, [&](auto k1) {
+    MARL_CUDA_TRY(launch_pdl(tc_forward_kernel<decltype(k1)::value>, dim3(p.plan.cta_begin[p.plan.n_nets]), dim3(kTcThreads), kFwdSmem, st, p, images));
+    return MARL_OK;
+  });
 }
 
 }  // namespace marl

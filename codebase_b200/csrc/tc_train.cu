@@ -3,7 +3,8 @@
 // Same arithmetic as train_kernel<KP, kHeadDqn> (QNetwork._compute_loss + backward, marlbase/dqn/model.py:118-168), split where a
 // weight gradient needs the rows of many tiles as its K dimension (tf32 wgmma reads both shared-memory operands K-major only):
 //   tc_dqn_fwd_kernel   online forward (A operand in registers, weights = K-major image), head on the CUDA cores; stores H2 (FP32,
-//                        feature-major), the gathered observation row, the row's outputs and the ReLU masks of H1 / H2 (row record)
+//                        feature-major), the gathered observation row, the row's outputs and the ReLU masks of H1 / H2 (row record);
+//                        then, on the same rows, the target network's forward (the TD target's bootstrap values)
 //   tc_dh1_kernel       TD head (needs the next row's outputs, hence after the forward) -> dLoss/dq[act] and the loss statistics;
 //                        dH1 = (dH2 x W2) * relu'(H1) with dH2[r][j] = g_r W3[act_r][j] relu'(H2[r][j]) built in registers (the TD loss touches
 //                        one output per row); B = K-major image of W2^T; then dW1 | db1 = dH1^T x [X | 1] from dH1 staged transposed
@@ -17,7 +18,7 @@
 
 namespace marl {
 
-// observation row of a virtual row of the training batch (episode rows only: launch_tc_dqn_train) and the row's index in every per-row buffer
+// observation row of a virtual row of the training batch (episode rows only: launch_tc_dqn_forward) and the row's index in every per-row buffer
 __device__ __forceinline__ const float* train_row(const TcTrainParams& p, int net, int vr, size_t& d, int& agent, int& unit, int& off, int& ep) {
   decode_row(p.plan, net, vr, agent, unit, off);
   d = row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows);
@@ -66,26 +67,67 @@ __device__ __forceinline__ void store_frag_fm(float* dst, size_t rows, const flo
   store_frag_masks(v, d0, d1, quad_lane, rec, mask);
 }
 
+// Shared memory of the training forward: the online image at 0, then the target network's W1 hi | lo (1024-byte aligned, as the swizzled panels
+// need) and its b1 | b2 | b3 | FP32 W3, then the mbarriers.  The target's W2 has no room of its own: it is loaded over the online W2 once every
+// phase-A layer 2 has run.
+constexpr int kTgtW1 = (kImageBytes + 1023) / 1024 * 1024;
+constexpr int kTgtB1 = kTgtW1 + (kOffW2Hi - kOffW1Hi);
+constexpr int kFwdBar = kTgtB1 + (kImageBytes - kOffB1);
+constexpr int kFwdTrainSmem = kFwdBar + 4 * 8 + 1024;
+static_assert(kOffW1Hi == 0 && kTgtW1 % 1024 == 0 && kFwdBar % 16 == 0 && kFwdTrainSmem <= 227 * 1024,
+              "training forward: 1024-byte aligned target W1 panels, online image and target operands within the shared memory of one SM");
+
+// Phase A runs the online network on the CTA's rows (warpgroup w: its 64-row tiles k = w, w + 2, ...) and stores what the backward needs.
+// Phase B (p.tgt_images != NULL) runs the target network on the same rows and writes p.tq_out.  Each thread of phase B re-reads the observation
+// values it stored in xg in phase A (same rows, same fragment mapping) instead of gathering them from the trajectory store again.  Tile split of
+// phase B: every warpgroup takes its own phase-A tiles again, except that with an odd tile count the last tile moves from warpgroup 0 (which had
+// one tile more in phase A) to the end of warpgroup 1's list, so both run the same number of tiles over the two phases.  Warpgroup 1 reads that
+// tile's rows after the target W2 wait, which thread 0 releases only after warpgroup 0 has passed the named barrier behind its stores.
+// Barriers: [0] online W1 + biases + FP32 W3, [1] online W2, [2] target W1 + biases + FP32 W3 (both at kernel start), [3] target W2 (issued
+// by thread 0 once both warpgroups are past their last phase-A layer 2: named barrier 1).
+template <int K1>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kImageBytes);   // [0] W1 + biases + FP32 W3, [1] W2
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kFwdBar);
   const int t = threadIdx.x, wg = t >> 7, wq = (t >> 5) & 3, lane = t & 31, g = lane >> 2, tq = lane & 3;
   int net, row_begin, row_end;
   cta_rows(p.plan, net, row_begin, row_end);
   if (row_begin >= row_end) { pdl_wait(); return; }
   TSG(g_ts_fwd, 0);
-  if (t == 0) { mbar_init(bar, 1); mbar_init(bar + 1, 1); fence_mbar_init(); }
+  const bool tgt = p.tgt_images != nullptr;
+  if (t == 0) { for (int i = 0; i < 4; ++i) mbar_init(bar + i, 1); fence_mbar_init(); }
   __syncthreads();
   pdl_wait();   // nothing above touches global memory
   pdl_launch_dependents();
   const uint32_t sb = smem_u32(smem);
-  if (t == 0) tma_forward_image(sb, p.images + (size_t)net * kImageBytes, bar);
+  if (t == 0) {
+    tma_forward_image(sb, p.images + (size_t)net * kImageBytes, bar);
+    if (tgt) {
+      const uint8_t* timg = p.tgt_images + (size_t)net * kImageBytes;
+      mbar_expect_tx(bar + 2, (uint32_t)((kOffW2Hi - kOffW1Hi) + (kImageBytes - kOffB1)));
+      tma_image_range(sb + kTgtW1, timg, kOffW1Hi, kOffW2Hi, bar + 2);
+      tma_image_range(sb + kTgtB1 - kOffB1, timg, kOffB1, kImageBytes, bar + 2);
+    }
+  }
   const float* b1 = reinterpret_cast<const float*>(smem + kOffB1);
   const float* b2 = reinterpret_cast<const float*>(smem + kOffB2);
   const float* b3 = reinterpret_cast<const float*>(smem + kOffB3);
   const float* w3f = reinterpret_cast<const float*>(smem + kOffW3F);
-  const int D = p.src.D, A = p.lay.out, k1steps = (D + 7) >> 3;
+  const int D = p.src.D, A = p.lay.out;
+  // both warpgroups are done with the online W2: warpgroup 0 (the last to finish phase A: it has as many tiles as warpgroup 1 or one more)
+  // waits for warpgroup 1's arrival, then thread 0 loads the target's W2 over it
+  auto online_w2_done = [&]() {
+    if (wg == 0) {
+      named_bar_sync(1, kTcThreads);
+      if (t == 0) {
+        mbar_expect_tx(bar + 3, (uint32_t)(kOffB1 - kOffW2Hi));
+        tma_image_range(sb, p.tgt_images + (size_t)net * kImageBytes, kOffW2Hi, kOffB1, bar + 3);
+      }
+    } else {
+      named_bar_arrive(1, kTcThreads);
+    }
+  };
   bool first = true;
   for (int vr0 = row_begin + kWgRows * wg; vr0 < row_end; vr0 += kTileRows) {
     const int r0 = vr0 + 16 * wq + g, r1 = r0 + 8;
@@ -99,15 +141,15 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
       float x[kMaxObsDim / 8][4];
       load_x_frag(s0, s1, D, tq, x);
 #pragma unroll
-      for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {   // the gathered row for the dH1 and weight-gradient kernels
+      for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {   // the gathered row for the dH1 and weight-gradient kernels (and phase B)
         const int c = 8 * ks + 2 * tq;
-        if (ks < k1steps) {
+        if (ks < K1) {
           if (d0 >= 0) *reinterpret_cast<float2*>(p.xg + (size_t)d0 * p.x_pitch + c) = make_float2(x[ks][0], x[ks][2]);
           if (d1 >= 0) *reinterpret_cast<float2*>(p.xg + (size_t)d1 * p.x_pitch + c) = make_float2(x[ks][1], x[ks][3]);
         }
       }
       if (first) mbar_wait(bar, 0);
-      layer1_tile(acc, x, sb + kOffW1Hi, b1, k1steps, tq);
+      layer1_tile<K1>(acc, x, sb + kOffW1Hi, b1, tq);
     }
     store_frag_masks(acc, d0, d1, tq, p.rec, kRecMask1);   // H1 itself is rebuilt by the weight-gradient kernel
     {
@@ -118,13 +160,74 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       layer_rs<16>(acc, hi, lo, sb + kOffW2Hi, sb + kOffW2Lo, 16);
     }
+    if (tgt && vr0 + kTileRows >= row_end) online_w2_done();   // this warpgroup's last phase-A tile
     float q0[kOutPad], q1[kOutPad];
     head_quad(acc, b2, w3f, A, tq, q0, q1);   // acc = H2 from here
     store_frag_fm(p.h2g, p.rows, acc, d0, d1, tq, p.rec, kRecMask2);
-    if (tq < 2 && (tq == 0 ? d0 : d1) >= 0) {
-      float* o = p.rec + (size_t)(tq == 0 ? d0 : d1) * kRowRec;
+    const long long d = tq == 0 ? d0 : d1;
+    if (tq < 2 && d >= 0) {
+      float* o = p.rec + (size_t)d * kRowRec;
 #pragma unroll
-      for (int a = 0; a < kOutPad; ++a) o[a] = a < A ? (tq == 0 ? q0[a] : q1[a]) + b3[a] : 0.f;
+      for (int a = 0; a < kOutPad; ++a) {
+        const float v = a < A ? (tq == 0 ? q0[a] : q1[a]) + b3[a] : 0.f;
+        o[a] = v;
+        if (p.q_out != nullptr && a < A) p.q_out[(size_t)d * A + a] = v;
+      }
+    }
+  }
+  if (!tgt) { TSG(g_ts_fwd, 31); return; }
+  if (row_begin + kWgRows * wg >= row_end) online_w2_done();   // no phase-A tile (warpgroup 1 of a CTA of at most 64 rows)
+  TSG(g_ts_fwd, 16);
+  // ---- phase B: the target network on the same rows -> tq_out
+  const float* tb1 = reinterpret_cast<const float*>(smem + kTgtB1);
+  const float* tb2 = reinterpret_cast<const float*>(smem + kTgtB1 + (kOffB2 - kOffB1));
+  const float* tb3 = reinterpret_cast<const float*>(smem + kTgtB1 + (kOffB3 - kOffB1));
+  const float* tw3f = reinterpret_cast<const float*>(smem + kTgtB1 + (kOffW3F - kOffB1));
+  const int n_tiles = (row_end - row_begin + kWgRows - 1) / kWgRows, n_mine = wg == 0 ? n_tiles / 2 : (n_tiles + 1) / 2;
+  first = true;
+  for (int i = 0; i < n_mine; ++i) {
+    const bool moved = wg + 2 * i >= n_tiles;   // warpgroup 1's extra tile (odd n_tiles): the last one, stored by warpgroup 0
+    const int vr0 = row_begin + kWgRows * (moved ? n_tiles - 1 : wg + 2 * i);
+    if (moved && first) mbar_wait(bar + 3, 0);   // its only tile (n_tiles == 1): read warpgroup 0's stores only after the barrier as well
+    const int r0 = vr0 + 16 * wq + g, r1 = r0 + 8;
+    long long d0 = -1, d1 = -1;
+    {
+      int agent, unit, off;
+      if (r0 < row_end) { decode_row(p.plan, net, r0, agent, unit, off); d0 = (long long)row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows); }
+      if (r1 < row_end) { decode_row(p.plan, net, r1, agent, unit, off); d1 = (long long)row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows); }
+    }
+    float acc[64];
+    {
+      float x[kMaxObsDim / 8][4];
+#pragma unroll
+      for (int ks = 0; ks < kMaxObsDim / 8; ++ks) {   // what phase A stored: zero beyond D, and for rows past the CTA's end
+        const int c = 8 * ks + 2 * tq;
+        float2 v0 = make_float2(0.f, 0.f), v1 = make_float2(0.f, 0.f);
+        if (ks < K1) {
+          if (d0 >= 0) v0 = *reinterpret_cast<const float2*>(p.xg + (size_t)d0 * p.x_pitch + c);
+          if (d1 >= 0) v1 = *reinterpret_cast<const float2*>(p.xg + (size_t)d1 * p.x_pitch + c);
+        }
+        x[ks][0] = v0.x; x[ks][1] = v1.x; x[ks][2] = v0.y; x[ks][3] = v1.y;
+      }
+      if (first) mbar_wait(bar + 2, 0);
+      layer1_tile<K1>(acc, x, sb + kTgtW1, tb1, tq);
+    }
+    {
+      uint32_t hi[16][4], lo[16][4];
+      frag_to_a(acc, hi, lo);
+      if (first) { mbar_wait(bar + 3, 0); first = false; }
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      layer_rs<16>(acc, hi, lo, sb + kOffW2Hi, sb + kOffW2Lo, 16);
+    }
+    float q0[kOutPad], q1[kOutPad];
+    head_quad(acc, tb2, tw3f, A, tq, q0, q1);
+    const long long d = tq == 0 ? d0 : d1;
+    if (tq < 2 && d >= 0) {
+      float* o = p.tq_out + (size_t)d * A;
+#pragma unroll
+      for (int a = 0; a < kOutPad; ++a)
+        if (a < A) o[a] = (tq == 0 ? q0[a] : q1[a]) + tb3[a];
     }
   }
   TSG(g_ts_fwd, 31);
@@ -355,6 +458,7 @@ __device__ __forceinline__ const float* xg_row(const TcTrainParams& p, int net, 
   return p.xg + row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows) * (size_t)p.x_pitch;
 }
 
+template <int K1>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
@@ -380,7 +484,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     tma_image_range(sb + kSW1 - kOffW1Hi, img, kOffW1Hi, kOffW2Hi, bar);
     tma_bulk_g2s(sb + kSB1, img + kOffB1, kHidden * 4, bar);
   }
-  const int A = p.lay.out, D = p.src.D, k1steps = (D + 7) >> 3;
+  const int A = p.lay.out, D = p.src.D;
   // constant lines of both B2 buffers: the ones line (hi 1, lo 0) of [H1 | 1] and the zero lines behind it; W3 copy
   for (int i = t; i < 2 * 8 * kChunk; i += kTcThreads) {
     const int b = i / (8 * kChunk), f = 128 + (i / kChunk) % 8, r = i % kChunk;
@@ -427,7 +531,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     // layer 1 behind the wait (its own wgmma.wait_group would wait for this warpgroup's chunk MMAs anyway); the x loads are already in flight
     if (rebuild) {
       if (first) { mbar_wait(bar, 0); first = false; }
-      layer1_tile(h1, x, sb + kSW1, b1, k1steps, tq);
+      layer1_tile<K1>(h1, x, sb + kSW1, b1, tq);
     }
     __syncthreads();   // both warpgroups are done reading the previous chunk
 #pragma unroll
@@ -490,31 +594,50 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
 // =====================================================================================================================
 // launchers
 // =====================================================================================================================
-constexpr int kFwdTrainSmem = kImageBytes + 64 + 1024;
 
 int tc_train_init() {
-  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_dqn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdTrainSmem));
   MARL_CUDA_TRY(cudaFuncSetAttribute(tc_dh1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDh1Smem));
-  MARL_CUDA_TRY(cudaFuncSetAttribute(tc_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kDwSmem));
+  for (int D = 1; D <= kMaxObsDim; D += 8)
+    if (int rc = with_k1(D, [](auto k1) {
+          MARL_CUDA_TRY(cudaFuncSetAttribute(tc_dqn_fwd_kernel<decltype(k1)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFwdTrainSmem));
+          MARL_CUDA_TRY(cudaFuncSetAttribute(tc_dw_kernel<decltype(k1)::value>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDwSmem));
+          return MARL_OK;
+        }))
+      return rc;
   return MARL_OK;
 }
 
-// all three kernels walk the same episode-aligned row split, so the per-CTA partials line up with ReduceParams::cta_begin
-int launch_tc_dqn_train(const TrainParams& tp, const TcBuffers& buf, cudaStream_t st, cudaEvent_t* between) {
-  MARL_REQUIRE(tp.lay.in < kMaxObsDim, "tensor-core backward: observation width %d needs a spare column for the bias trick (max %d)", tp.lay.in, kMaxObsDim - 1);
-  MARL_REQUIRE(tp.src.mode == 1, "tensor-core backward: rows must be gathered from the trajectory store (mode %d)", tp.src.mode);
+static TcTrainParams tc_params(const TrainParams& tp, const TcBuffers& buf) {
   TcTrainParams p; memset(&p, 0, sizeof(p));
   p.plan = tp.plan; p.src = tp.src; p.lay = tp.lay; p.images = buf.image; p.bwd_images = buf.bwd_image;
   p.h2g = buf.h2; p.rec = buf.rec; p.xg = buf.x; p.x_pitch = 8 * ((tp.src.D + 7) / 8); p.rows = buf.rows;
   p.tq = tp.tq; p.td_ext = tp.td_ext; p.td_agent_stride = tp.td_agent_stride; p.gamma = tp.gamma; p.double_q = tp.double_q;
   p.scratch = tp.scratch; p.scratch_pitch = tp.scratch_pitch; p.loss_part = tp.loss_part;
+  return p;
+}
+
+// all three kernels walk the same episode-aligned row split, so the per-CTA partials line up with ReduceParams::cta_begin
+int launch_tc_dqn_forward(const TrainParams& tp, const TcBuffers& buf, const uint8_t* tgt_images, float* tq_out, float* q_out, cudaStream_t st) {
+  MARL_REQUIRE(tp.lay.in < kMaxObsDim, "tensor-core backward: observation width %d needs a spare column for the bias trick (max %d)", tp.lay.in, kMaxObsDim - 1);
+  MARL_REQUIRE(tp.src.mode == 1, "tensor-core backward: rows must be gathered from the trajectory store (mode %d)", tp.src.mode);
+  MARL_REQUIRE(tgt_images == nullptr || tq_out != nullptr, "tensor-core training forward: target images without an output buffer");
+  TcTrainParams p = tc_params(tp, buf);
+  p.tgt_images = tgt_images; p.tq_out = tq_out; p.q_out = q_out;
+  return with_k1(tp.src.D, [&](auto k1) {
+    MARL_CUDA_TRY(launch_pdl(tc_dqn_fwd_kernel<decltype(k1)::value>, dim3(tp.plan.cta_begin[tp.plan.n_nets]), dim3(kTcThreads), kFwdTrainSmem, st, p));
+    return MARL_OK;
+  });
+}
+
+int launch_tc_dqn_backward(const TrainParams& tp, const TcBuffers& buf, cudaStream_t st, cudaEvent_t after_dh1) {
+  const TcTrainParams p = tc_params(tp, buf);
   const int grid = tp.plan.cta_begin[tp.plan.n_nets];
-  MARL_CUDA_TRY(launch_pdl(tc_dqn_fwd_kernel, dim3(grid), dim3(kTcThreads), kFwdTrainSmem, st, p));
-  if (between) MARL_CUDA_TRY(cudaEventRecord(between[0], st));
   MARL_CUDA_TRY(launch_pdl(tc_dh1_kernel, dim3(grid), dim3(kTcThreads), kDh1Smem, st, p));
-  if (between) MARL_CUDA_TRY(cudaEventRecord(between[1], st));
-  MARL_CUDA_TRY(launch_pdl(tc_dw_kernel, dim3(grid), dim3(kTcThreads), kDwSmem, st, p));
-  return MARL_OK;
+  if (after_dh1) MARL_CUDA_TRY(cudaEventRecord(after_dh1, st));
+  return with_k1(tp.src.D, [&](auto k1) {
+    MARL_CUDA_TRY(launch_pdl(tc_dw_kernel<decltype(k1)::value>, dim3(grid), dim3(kTcThreads), kDwSmem, st, p));
+    return MARL_OK;
+  });
 }
 
 }  // namespace marl
