@@ -1,5 +1,6 @@
 """The training pass's row split (csrc/learner.cuh: make_plan, episode_plan, cta_rows) restated in Python, and the branch class of a CTA; the
-recurrent kernels' sequence split (gru_plan, seq_class, find_units) further down.
+forward kernels' dense split (dense_plan, dense_classes, find_envs) after it; the recurrent kernels' sequence split (gru_plan, seq_class,
+find_units) further down.
 
 Which branches of the DQN tensor-core training pass run (csrc/tc_train.cu) depends on how many rows a CTA gets:
   - tc_dh1_kernel walks 128-row tiles; warpgroup 1 stages its two 32-row chunks of a tile at the top of the next tile, or after the loop when the
@@ -15,7 +16,19 @@ on a given SM count, so that a device with another SM count still tests every cl
 A CTA ends on an episode boundary, so its last rows are the final rows of its last episode, and row T of an episode has no TD error.  A tail
 made of row T alone carries no gradient and tests nothing.  A CTA therefore counts for its class only when its last chunk is full or holds at
 least TAIL_MIN rows, and the tests give the last episode of every CTA (last_episodes) its full length T: the tail -- the last chunk, and the rows warpgroup 1
-stages after the loop -- then holds rows t < T that carry TD errors (tail_td_rows)."""
+stages after the loop -- then holds rows t < T that carry TD errors (tail_td_rows).
+
+The actor-critic training pass (learner_kernels.cu: train_kernel<KP, kHeadA2cCritic> and <KP, kHeadA2cActor>, launched by a2c.cu's a2c_gradients
+over episode_plan of the critic's and of the actor's networks) walks the same 128-row tiles from the top down, and row T of an episode carries
+no loss there either (the heads run for t < T only): the same classes, find_batch, last_episodes and tail_td_rows apply to each of its passes.
+
+The forward kernels serve the act step (model.act, get_value) over make_plan(ns, E, 1, n_sm, 32) (dense_plan: one row per environment and
+agent, at most one CTA per 32 rows of a net), and the target-critic / PPO old-log-prob passes over episode_plan.  Each CTA walks its rows from
+row_begin:
+  - mlp_forward_kernel (FP32) in 128-row tiles, the last one partial unless the CTA's rows are a multiple of 128;
+  - tc_forward_kernel (wgmma) with two warpgroups on alternating 64-row tiles: in the last 128 rows, c1 and c2 leave warpgroup 1 idle (c2-full
+    is exactly 64 rows for warpgroup 0), c3 and c4 give it a partial or full tile.
+So the 24 CLASSES name the forward's branches too; a forward has no loss rows, so every CTA counts (dense_classes)."""
 from __future__ import annotations
 
 import functools
@@ -123,6 +136,31 @@ def last_episodes(agent_net, B, T, n_sm):
     return sorted({(r1 // (T + 1) - 1) % B for _, r0, r1 in all_cta_rows(p) if r1 > r0})
 
 
+# ---- the forward kernels' dense split -----------------------------------------------------------------------------------------------------------
+def dense_plan(agent_net, E, n_sm):
+    """the act step's plan (a2c_dense_forward, the DQN act forward): make_plan(ns, E, 1, n_sm, 32); unit = environment, one row each"""
+    return make_plan(list(agent_net), E, 1, n_sm, 32)
+
+
+@functools.lru_cache(maxsize=None)
+def dense_classes(agent_net, E, n_sm):
+    """every class a forward over E environments reaches on n_sm SMs (agent_net: a tuple).  cta_rows splits a net's `units` rows over `ncta`
+    CTAs by floor division, so each CTA gets units // ncta rows or one more: two sizes per net instead of a walk over every CTA."""
+    p = dense_plan(agent_net, E, n_sm)
+    cb, sb = p["cta_begin"], p["slot_begin"]
+    out = set()
+    for k in range(len(cb) - 1):
+        q, rem = divmod((sb[k + 1] - sb[k]) * E, cb[k + 1] - cb[k])
+        out |= {classes(r) for r in ({q, q + 1} if rem else {q}) if r > 0}
+    return frozenset(out)
+
+
+def find_envs(N, sharing, n_sm, cls, max_envs):
+    """the smallest E <= max_envs whose dense plan on n_sm SMs holds class `cls`; None when none does"""
+    nets = tuple(nets_of(N, sharing))
+    return next((E for E in range(1, max_envs + 1) if cls in dense_classes(nets, E, n_sm)), None)
+
+
 # ---- the recurrent (GRU) split ------------------------------------------------------------------------------------------------------------------
 # gru_backward_kernel (csrc/gru_kernels.cu) gets make_plan(ns, B, 1, n_sm, kGruSeqs): one unit per sequence (agent, b), a contiguous run
 # [v_begin, v_end) of one net's sequences per CTA.  It walks the run in 16-sequence tiles, each split into two 8-sequence halves (one per 128-thread
@@ -216,8 +254,9 @@ def forward_shapes(agent_net, B):
 
 
 def tail_td_rows(agent_net, B, T, n_sm, cls):
-    """for every CTA of class `cls`: (rows of its last chunk, rows of warpgroup 1's after-loop phase -- chunks 2 and 3 of the last tile -- with a TD
-    error, t < T, in the CTA's last episode); the after-loop count is None where the last tile holds 64 rows or fewer (no such phase)"""
+    """for every CTA of class `cls`: (rows of its last chunk, rows of warpgroup 1's after-loop phase -- chunks 2 and 3 of the last tile -- that
+    carry a loss, t < T, in the CTA's last episode: a TD error in the DQN pass, a value or policy loss in the actor-critic passes); the after-loop
+    count is None where the last tile holds 64 rows or fewer (no such phase)"""
     p = episode_plan(list(agent_net), B, T, n_sm)
     out = []
     for _, r0, r1 in all_cta_rows(p):

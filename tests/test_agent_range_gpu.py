@@ -313,12 +313,18 @@ def _critic_bias_floors(m, st0, b64, hp, returns):
 def _ac_step(c, m, st, s, hp, step, tr, what, per_block):
     """one update of the device and the oracle, then every per-update check of test_rnn_ac_gpu.py; per_block: the gradient per block too (PPO:
     the first epoch's, from a second handle stopped after one epoch).  Returns the worst block."""
-    rc = _rcase(c)
     b64 = _f64(ac_oracle_batch(s))
     st0 = copy.deepcopy(st)
+    want = rac._oracle_update(_rcase(c), st, b64, hp, step)
+    return _ac_check(c, m, st, st0, b64, want, traj_store(s, m.device), hp, step, tr, what, per_block)
+
+
+def _ac_check(c, m, st, st0, b64, want, ts, hp, step, tr, what, per_block, floors=None):
+    """_ac_step's device update and checks against an oracle update already taken (st0: the oracle's state before it, st: after, want: its
+    result), so that several handles can be held to one oracle update; ts: the store, whose first c.B environments are the batch b64; floors:
+    more blocks' scales for _assert_blocks"""
+    rc = _rcase(c)
     th0, tgt0 = m.theta.detach().clone(), m.theta_tgt.detach().clone()
-    want = rac._oracle_update(rc, st, b64, hp, step)
-    ts = traj_store(s, m.device)
     met = m.update_from_store(ts, c.B, step).cpu().numpy()
     worst = None
     if per_block:
@@ -335,7 +341,7 @@ def _ac_step(c, m, st, s, hp, step, tr, what, per_block):
             got, ref = m.grad.cpu().numpy()[:n] / fill, want["grad"]
             kink = lambda: gar.a2c_kink_risk(st0, b64, hp)   # noqa: E731
         worst = _assert_blocks(m, got, np.concatenate([ref["actor"].numpy(), ref["critic"].numpy()]), what, kink,
-                               floors=_critic_bias_floors(m, st0, b64, hp, want["returns"]))
+                               floors={**_critic_bias_floors(m, st0, b64, hp, want["returns"]), **(floors or {})})
     rac._check_update(m, rc, hp, st, st0, b64, want, met, step, tgt0.cpu().numpy(), tr, what)
     return worst
 

@@ -1,8 +1,9 @@
 """No GPU: tests/row_plan.py against the library's own planner, the class search on both H100 SM counts, and the edges of
-tests/test_tc_train_edges_gpu.py's and tests/test_gru_edges_gpu.py's shape tables.
+tests/test_tc_train_edges_gpu.py's, tests/test_ac_train_edges_gpu.py's and tests/test_gru_edges_gpu.py's shape tables.
 
 The planner check compiles a host-only driver that includes csrc/gru.cuh and csrc/learner.cuh (nvcc with the library's flags, no device code
-runs) and prints episode_plan's and the GRU backward's make_plan(ns, B, 1, n_sm, kGruSeqs) cta_begin and every CTA's [row_begin, row_end).
+runs) and prints episode_plan's, the GRU backward's make_plan(ns, B, 1, n_sm, kGruSeqs) and the act step's make_plan(ns, E, 1, n_sm, 32)
+cta_begin and every CTA's [row_begin, row_end).
 cta_rows itself is device code: the driver restates its split in C++ integer arithmetic."""
 import subprocess
 
@@ -11,6 +12,7 @@ import pytest
 
 from codebase_b200.csrc import build as native_build
 from tests import row_plan as rp
+from tests import test_ac_train_edges_gpu as ae
 from tests import test_gru_edges_gpu as ge
 from tests import test_tc_train_edges_gpu as g
 
@@ -19,7 +21,8 @@ DRIVER = r"""
 #include <stdio.h>
 using namespace marl;
 // stdin: lines "N B T n_sm agent_net[0..N)"; stdout per line, for episode_plan(ns, B, T, n_sm) and then for the GRU backward's
-// make_plan(ns, B, 1, n_sm, kGruSeqs): "n_cta cta_begin[0..n_nets] | net row_begin row_end ..." (one triple per CTA), the two joined by " || "
+// make_plan(ns, B, 1, n_sm, kGruSeqs): "n_cta cta_begin[0..n_nets] | net row_begin row_end ..." (one triple per CTA), the two joined by " || ";
+// then the GRU plan's slots, and the act step's dense plan make_plan(ns, E = B, 1, n_sm, 32) in the same form
 static void print_plan(const RowPlan& p) {
   const int n_cta = p.cta_begin[p.n_nets];
   printf("%d", n_cta);
@@ -45,6 +48,8 @@ int main() {
     printf(" || %d", q.n_nets);
     for (int k = 0; k <= q.n_nets; ++k) printf(" %d", q.slot_begin[k]);
     for (int a = 0; a < N; ++a) printf(" %d", q.slot_agent[a]);
+    printf(" || ");
+    print_plan(make_plan(ns, B, 1, n_sm, 32));
     printf("\n");
   }
   return 0;
@@ -83,8 +88,8 @@ def test_mirror_matches_the_library_planner(driver):
     assert len(lines) == len(cfgs)
     seen, seen_gru = set(), set()
     for (N, B, T, n_sm, nets), line in zip(cfgs, lines):
-        episodes, seqs, slots = line.split(" || ")
-        for p, part in ((rp.episode_plan(nets, B, T, n_sm), episodes), (rp.gru_plan(nets, B, n_sm), seqs)):
+        episodes, seqs, slots, dense = line.split(" || ")
+        for p, part in ((rp.episode_plan(nets, B, T, n_sm), episodes), (rp.gru_plan(nets, B, n_sm), seqs), (rp.dense_plan(nets, B, n_sm), dense)):
             head, rows = part.split("|")
             head, rows = [int(x) for x in head.split()], [int(x) for x in rows.split()]
             assert head[0] == p["cta_begin"][-1] and head[1:] == p["cta_begin"], (N, B, T, n_sm, nets)
@@ -92,9 +97,13 @@ def test_mirror_matches_the_library_planner(driver):
             assert rows == want, (N, B, T, n_sm, nets)
         slots = [int(x) for x in slots.split()]
         n_nets = slots[0]
-        assert slots[1:n_nets + 2] == p["slot_begin"] and slots[n_nets + 2:] == p["slot_agent"], (N, nets)   # what seq_of reads
+        q = rp.gru_plan(nets, B, n_sm)
+        assert slots[1:n_nets + 2] == q["slot_begin"] and slots[n_nets + 2:] == q["slot_agent"], (N, nets)   # what seq_of reads
         seen |= rp.plan_classes(tuple(nets), B, T, n_sm)
         seen_gru |= rp.gru_classes(tuple(nets), B, n_sm)
+        # dense_classes reads two CTA sizes per net instead of walking every CTA
+        d = rp.dense_plan(nets, B, n_sm)
+        assert rp.dense_classes(tuple(nets), B, n_sm) == {rp.classes(r1 - r0) for _, r0, r1 in rp.all_cta_rows(d) if r1 > r0}, (N, B, n_sm, nets)
     assert len(seen) >= 12, sorted(seen)   # the random configs are not the coverage: find_batch / find_units are
     assert len(seen_gru) >= 6, sorted(seen_gru)
 
@@ -254,3 +263,104 @@ def test_gru_cases_sit_on_the_edges_they_claim():
     assert all(c.cls.startswith(("t2", "t3")) for c in ge.REUSE_CASES.values())
     rows = [c.N * P * c.T for c, P in ge.HEAD_CASES.values()]
     assert any(r % 256 == 0 for r in rows) and any(r % 256 == 1 and r > 256 for r in rows) and any(r < 256 for r in rows)
+
+
+# ---- the actor-critic training pass and the forward kernels (tests/test_ac_train_edges_gpu.py) -----------------------------------------------------
+def _kp(width):
+    """the input tile of the FP32 kernels at an input width (learner_kernels_init / launch_train)"""
+    return 16 if width <= 16 else 32 if width <= 32 else 64 if width <= 64 else 128
+
+
+@pytest.mark.parametrize("n_sm", [114, 132])
+def test_every_ac_case_finds_its_class_in_both_passes(n_sm):
+    """On an H100 PCIe (114 SMs) and SXM (132 SMs), each training case finds its class within the row budget, in the actor pass and, over the
+    critic's own networks, in the critic pass; with the edge episodes at full length, every CTA of that class has rows with a loss (t < T) in its
+    last chunk in both passes: at least TAIL_MIN - 1 in its last episode, or all T of them where T is shorter.  Over the class sweep, the actor
+    passes and the critic passes each cover all 26 classes."""
+    actor, critic = set(), set()
+    for name, c in ae.all_train_cases():
+        found = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, c.cls, ae.MAX_ROWS)
+        assert found is not None, (n_sm, name)
+        P, T = found
+        assert c.N * P * (T + 1) <= ae.MAX_ROWS
+        for part, sharing in (("actor", c.sharing), ("critic", c.csharing)):
+            nets = rp.nets_of(c.N, sharing)
+            assert c.cls in rp.plan_classes(tuple(nets), P, T, n_sm), (n_sm, name, part, P, T)
+            assert set(rp.last_episodes(nets, P, T, n_sm)) <= set(ae.edge_episodes(c, P, T, n_sm))
+            if c.cls in rp.CLASSES:
+                tails = rp.tail_td_rows(nets, P, T, n_sm, c.cls)
+                assert tails and all(last >= min(rp.TAIL_MIN - 1, T) for last, _ in tails), (n_sm, name, part, P, T, tails)
+        if name in ae.CLASS_CASES:
+            actor |= rp.plan_classes(tuple(rp.nets_of(c.N, c.sharing)), P, T, n_sm)
+            critic |= rp.plan_classes(tuple(rp.nets_of(c.N, c.csharing)), P, T, n_sm)
+    assert set(ae.CLASS_CASES) == set(rp.ALL_CLASSES)
+    assert actor == critic == set(rp.ALL_CLASSES), (sorted(set(rp.ALL_CLASSES) - actor), sorted(set(rp.ALL_CLASSES) - critic))
+
+
+@pytest.mark.parametrize("n_sm", [114, 132])
+def test_every_forward_case_finds_its_class(n_sm):
+    """find_envs reaches each of the 24 classes for one agent, two independent agents and three in groups (0, 1, 0) within the environment
+    budget, and returns the smallest such E; so do the FP32-only and joint-row cases"""
+    for cls in rp.CLASSES:
+        for N, sharing in ae.FWD_N:
+            E = rp.find_envs(N, sharing, n_sm, cls, ae.FWD_MAX_ROWS // N)
+            nets = tuple(rp.nets_of(N, sharing))
+            assert E is not None and cls in rp.dense_classes(nets, E, n_sm), (n_sm, cls, N)
+            assert E == 1 or cls not in rp.dense_classes(nets, E - 1, n_sm), (n_sm, cls, N, E)
+    for name, (c, cls) in ae.FWD_EXTRA.items():
+        E = rp.find_envs(c.N, c.sharing, n_sm, cls, ae.FWD_MAX_ROWS // c.N)
+        assert E is not None and cls in rp.dense_classes(tuple(rp.nets_of(c.N, c.sharing)), E, n_sm), (n_sm, name)
+
+
+def test_dense_plan_of_a_small_launch():
+    """one agent, 2 SMs: E = 100 environments on 2 CTAs of 50 rows (t1-c2-part); E = 32 stays on one CTA, E = 40 takes two of 20 (at most
+    ceil(E / 32) CTAs); the first CTA of 33 rows is at E = 65 (32 + 33).  Two agents in one group, 132 SMs, E = 4225: 8450 rows on 132 CTAs of 64
+    or 65 (t1-c2-full and t1-c3-part)"""
+    assert rp.all_cta_rows(rp.dense_plan([0], 100, 2)) == [(0, 0, 50), (0, 50, 100)] and rp.dense_classes((0,), 100, 2) == {"t1-c2-part"}
+    assert rp.all_cta_rows(rp.dense_plan([0], 32, 2)) == [(0, 0, 32)] and rp.all_cta_rows(rp.dense_plan([0], 40, 2)) == [(0, 0, 20), (0, 20, 40)]
+    assert rp.dense_classes((0, 0), 4225, 132) == {"t1-c2-full", "t1-c3-part"}
+    assert rp.find_envs(1, False, 2, "t1-c2-part", 1000) == 65 and rp.find_envs(1, False, 2, "t3+-c1-part", 100) is None
+
+
+def test_ac_cases_sit_on_the_edges_they_claim():
+    C, W, L = ae.CLASS_CASES, ae.WIDTH_CASES, ae.LENGTH_CASES
+    assert {c.kind for c in C.values()} == {"ia2c", "ippo", "maa2c", "mappo"}
+    # independent, shared, uneven-group and SEPS actors; a few critics shared differently from their actor, so that cplan != aplan
+    assert any(c.sharing is False and c.N > 1 for c in C.values()) and any(c.sharing is True and c.N > 1 for c in C.values())
+    assert any(c.sharing == ae.SEPS for c in C.values()) and any(c.sharing in (ae.GROUPS3, ae.GROUPS4) for c in C.values())
+    differ = [(k, c) for k, c in C.items() if c.csharing != c.sharing]
+    assert len(differ) >= 3
+    for n_sm in (114, 132):
+        for cls, c in differ:
+            P, T = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, cls, ae.MAX_ROWS)
+            a, k = rp.episode_plan(rp.nets_of(c.N, c.sharing), P, T, n_sm), rp.episode_plan(rp.nets_of(c.N, c.csharing), P, T, n_sm)
+            assert a["cta_begin"] != k["cta_begin"], (n_sm, cls)
+    # KP 16, 32, 64 and 128 for the actor and for the critic; every actor KP at a t2 and at a t3+ class with a partial last tile
+    assert {_kp(c.D) for c in C.values()} == {_kp(c.joint) for c in C.values()} == {16, 32, 64, 128}
+    for kp in (16, 32, 64, 128):
+        for t in ("t2", "t3+"):
+            assert any(_kp(c.D) == kp and cls.startswith(t + "-") and cls.endswith("part") for cls, c in C.items()), (kp, t)
+    assert any(c.standardise for c in C.values())
+    # the tensor-core target and old-log-prob passes: cases of both kinds, PPO at 2, 3 and 4 epochs
+    assert any(c.tc_forward and c.kind not in ae.PPO for c in C.values()) and any(c.tc_forward and c.joint > ae.MAX_OBS_TC for c in C.values())
+    assert {c.epochs for c in C.values() if c.kind in ae.PPO and c.tc_forward} == {2, 3, 4}
+    # the width sweep: every KP edge, hidden widths below 128 with actor and critic apart, every action count, joint inputs on both sides of 32 and 64
+    assert {1, 16, 17, 32, 33, 64, 65, 127, 128} <= {c.D for c in W.values()}
+    assert {1, 2, 37, 100, 127} <= {c.H for c in W.values()} | {c.critic_H for c in W.values()} and all(c.H != c.critic_H for c in W.values())
+    assert {c.A for c in W.values()} == {1, 2, 3, 5, 8}
+    assert {32, 33, 64, 65, 128} <= {c.joint for c in W.values() if c.kind in ae.CENTRAL}
+    for c in list(W.values()) + list(L.values()):
+        assert c.cls.startswith(("t2", "t3")), c
+    assert all(c.cls.endswith("part") for c in W.values())
+    # lengths: T = 1 and 2, and one environment whose single episode walks three tiles
+    for n_sm in (114, 132):
+        Ts = {}
+        for name, c in L.items():
+            P, T = rp.find_batch(c.N, c.sharing, c.T_choices, n_sm, c.cls, ae.MAX_ROWS)
+            Ts.setdefault(T, []).append(P)
+        assert set(Ts) == {1, 2, 383} and Ts[383] == [1] * len(Ts[383]), Ts
+    # handle reuse at a t2 and a t3+ class
+    assert {c.cls[:2] for c in ae.REUSE_CASES.values()} == {"t2", "t3"}
+    # the forward's extra cases: an input of 100, a hidden width of 37, joint rows at 16 (tensor cores), 33 and 128
+    X = {name: c for name, (c, _) in ae.FWD_EXTRA.items()}
+    assert {c.joint for c in X.values() if c.kind in ae.CENTRAL} == {16, 33, 128} and any(c.D == 100 for c in X.values()) and any(c.H == 37 for c in X.values())
