@@ -443,13 +443,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
 // Warpgroup w accumulates the M rows [64 w, 64 w + 64) of both.  A2, A3 and B3 are staged per chunk by all eight warps, lane = row; H1 is rebuilt
 // per 64 rows (two chunks) by the warpgroup that ran those rows in the forward (layer1_tile on the W1 panels of the forward image) and staged
 // from its accumulator fragments into two B2 buffers, one per chunk.
+// The FP32 copy of W3 has rows of kW3Pitch = 129 floats: the 32 lanes of a staging warp read W3[act][j] at one j and their rows' actions, and with
+// a pitch of 128 every action would sit in the same bank (up to A-way conflicts on 16 loads per thread and chunk); with 129 they are distinct.
 constexpr int kB2Bytes = 2 * 136 * kLine;                                  // one chunk of [H1 | 1], hi | lo
-constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA3 = kSB2 + 2 * kB2Bytes, kSB3 = kSA3 + 2 * 128 * kLine, kSW3 = kSB3 + 2 * 8 * kLine;
-constexpr int kSW1 = kSW3 + kOutPad * kHidden * 4;                         // W1 hi | lo panels of the forward image
-constexpr int kSB1 = kSW1 + (kOffW2Hi - kOffW1Hi), kSBar = kSB1 + kHidden * 4;
+constexpr int kW3Pitch = kHidden + 1;
+constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA3 = kSB2 + 2 * kB2Bytes, kSB3 = kSA3 + 2 * 128 * kLine, kSW1 = kSB3 + 2 * 8 * kLine;
+constexpr int kSW3 = kSW1 + (kOffW2Hi - kOffW1Hi);                         // behind the W1 hi | lo panels of the forward image
+constexpr int kSB1 = kSW3 + (kOutPad * kW3Pitch * 4 + 15) / 16 * 16, kSBar = kSB1 + kHidden * 4;
 constexpr int kDwSmem = kSBar + 64 + 1024;
-static_assert(kSB2 % 1024 == 0 && kB2Bytes % 1024 == 0 && kSA3 % 1024 == 0 && kSB3 % 1024 == 0 && kSW1 % 1024 == 0 && kDwSmem <= 227 * 1024,
-              "weight-gradient staging: 1024-byte aligned operands within the shared memory of one SM");
+static_assert(kSB2 % 1024 == 0 && kB2Bytes % 1024 == 0 && kSA3 % 1024 == 0 && kSB3 % 1024 == 0 && kSW1 % 1024 == 0 && kSB1 % 16 == 0 &&
+              kDwSmem <= 227 * 1024, "weight-gradient staging: 1024-byte aligned operands within the shared memory of one SM");
 
 // gathered observation row of a virtual row (stored by the forward)
 __device__ __forceinline__ const float* xg_row(const TcTrainParams& p, int net, int vr) {
@@ -491,10 +494,11 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     stage_hl(smem + kSB2 + b * kB2Bytes, 136, f, r, f == 128 ? 1.f : 0.f);
   }
   {
-    const float4* w3src = reinterpret_cast<const float4*>(p.images + (size_t)net * kImageBytes + kOffW3F);
-    for (int i = t; i < kOutPad * kHidden / 4; i += kTcThreads) reinterpret_cast<float4*>(smem + kSW3)[i] = w3src[i];
+    const float* w3src = reinterpret_cast<const float*>(p.images + (size_t)net * kImageBytes + kOffW3F);
+    for (int i = t; i < kOutPad * kHidden; i += kTcThreads) reinterpret_cast<float*>(smem + kSW3)[(i / kHidden) * kW3Pitch + i % kHidden] = w3src[i];
   }
   __syncthreads();
+  TSG(g_ts_dw, 1);
   float acc2[68], acc3[4];
 #pragma unroll
   for (int i = 0; i < 68; ++i) acc2[i] = 0.f;
@@ -505,6 +509,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   const int n_chunks = (row_end - row_begin + kChunk - 1) / kChunk;
   int c = 0;
   do {   // n_chunks >= 1: with a zero-trip path (a for loop) ptxas serialises every wgmma of the kernel (C7515)
+    TSG(g_ts_dw, 2 + c);   // chunk c: slots 2-29 (chunks past 27 land on 30 / 31, which the epilogue writes again)
     // ---- this thread's row (lane) and features (warp + 8 i) of the chunk -> registers; their loads overlap the previous chunk's MMAs
     const int vr = row_begin + c * kChunk + lane;
     float h2v[16], gr = 0.f;
@@ -537,7 +542,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int j = warp + 8 * i;
-      const float dh2 = h2v[i] > 0.f ? gr * w3f[act * kHidden + j] : 0.f;
+      const float dh2 = h2v[i] > 0.f ? gr * w3f[act * kW3Pitch + j] : 0.f;
       stage_hl(smem + kSA2, 128, j, lane, dh2);
       stage_hl(smem + kSA3, 128, j, lane, h2v[i]);
     }
@@ -577,10 +582,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   // ---- accumulators -> this CTA's gradient sums ------------------------------------------------------------------------------------
   const NetLayout& L = p.lay;
 #pragma unroll
-  for (int i = 0; i < 68; ++i) {
+  for (int i = 0; i < 64; i += 2) {   // columns n, n + 1 of W2 in one 8-byte store (L.w2 and n are even, the CTA pitch a multiple of 4 floats)
     const int m = wg * kWgRows + 16 * wq + g + ((i & 2) ? 8 : 0), n = frag_col(i, tq);
-    if (n < kHidden) gs[L.w2 + m * kHidden + n] = acc2[i];
-    else if (n == kHidden) gs[L.b2 + m] = acc2[i];
+    *reinterpret_cast<float2*>(gs + L.w2 + m * kHidden + n) = make_float2(acc2[i], acc2[i + 1]);
+  }
+#pragma unroll
+  for (int i = 64; i < 68; ++i) {
+    const int m = wg * kWgRows + 16 * wq + g + ((i & 2) ? 8 : 0), n = frag_col(i, tq);
+    if (n == kHidden) gs[L.b2 + m] = acc2[i];
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
