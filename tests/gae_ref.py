@@ -7,7 +7,8 @@ The reference has no λ-return; the project defines it (DESIGN.md §4.4c) as the
 
 with m_t = 1 - dones[t] masking reward t and value t, and no term at an index >= T.  For n >= T - t every G_t^(n) is the return to the end of the
 stored episode, so the infinite sum is (1 - λ) Σ_{n=1}^{T-1} λ^(n-1) G^(n) + λ^(T-1) G^(T).  `lambda_returns` evaluates exactly that, every
-G^(n) from its definition, in float64: it shares no arithmetic with the kernel's backward recursion.
+G^(n) from its definition, in float64, streamed over n (O(T x sequences) memory, O(T² x sequences) time): it shares no arithmetic with the
+kernel's backward recursion.
 
 `lambda_returns_in(lam)` runs oracle.learner_ref's A2C / PPO updates with these returns in place of the n-step returns (their other arithmetic
 unchanged: the de-standardised target values, the running statistics, the losses); it composes with tests/gru_ac_ref.mixed().
@@ -22,9 +23,10 @@ import torch
 from oracle import learner_ref as lr
 
 
-def nstep_all(rewards, done, next_values, gamma):
-    """G^(n) for n = 1 .. T, float64: rewards (T, ...), done and next_values (>= T, ...) -> (T, T, ...) with [n - 1] = G^(n).
-    G_t^(n) = Σ_{k<n, t+k<T} γ^k m_{t+k} r_{t+k} + [t+n < T] γ^n m_{t+n} V_{t+n}: compute_nstep_returns term by term, vectorised over t."""
+def nstep_each(rewards, done, next_values, gamma):
+    """G^(n) for n = 1 .. T in turn, float64: rewards (T, ...), done and next_values (>= T, ...) -> yields (n, G^(n)) with G^(n) of shape (T, ...).
+    G_t^(n) = Σ_{k<n, t+k<T} γ^k m_{t+k} r_{t+k} + [t+n < T] γ^n m_{t+n} V_{t+n}: compute_nstep_returns term by term, vectorised over t.  Only the
+    reward sum is kept from one n to the next, so memory is O(T x sequences)."""
     r = np.asarray(rewards, np.float64)
     T = r.shape[0]
     m = 1.0 - np.asarray(done, np.float64)[:T]
@@ -36,21 +38,23 @@ def nstep_all(rewards, done, next_values, gamma):
             out[: T - k] = x[k:]
         return out
 
-    out = np.empty((T,) + r.shape, np.float64)
     rewards_part = np.zeros_like(r)
     for n in range(1, T + 1):
         rewards_part = rewards_part + gamma ** (n - 1) * shifted(mr, n - 1)
-        out[n - 1] = rewards_part + gamma ** n * shifted(mv, n)
-    return out
+        yield n, rewards_part + gamma ** n * shifted(mv, n)
+
+
+def nstep_all(rewards, done, next_values, gamma):
+    """every G^(n) of nstep_each at once: (T, T, ...) with [n - 1] = G^(n) (small T only)"""
+    return np.stack([G for _, G in nstep_each(rewards, done, next_values, gamma)])
 
 
 def lambda_returns(rewards, done, next_values, lam, gamma):
-    """(1 - λ) Σ_{n=1}^{T-1} λ^(n-1) G^(n) + λ^(T-1) G^(T), float64 (T, ...)"""
-    G = nstep_all(rewards, done, next_values, gamma)
-    T = G.shape[0]
-    out = lam ** (T - 1) * G[T - 1]
-    for n in range(1, T):
-        out = out + (1.0 - lam) * lam ** (n - 1) * G[n - 1]
+    """(1 - λ) Σ_{n=1}^{T-1} λ^(n-1) G^(n) + λ^(T-1) G^(T), float64 (T, ...), accumulated over n without keeping the G^(n)"""
+    T = np.asarray(rewards).shape[0]
+    out = 0.0
+    for n, G in nstep_each(rewards, done, next_values, gamma):
+        out = out + (lam ** (T - 1) if n == T else (1.0 - lam) * lam ** (n - 1)) * G
     return out
 
 

@@ -1,7 +1,8 @@
 """GPU: λ-returns (algorithm.gae_lambda, lambda_returns_kernel in csrc/a2c.cu) of IA2C, IPPO, MAA2C and MAPPO.
 
-- The returns against the float64 mixture of n-step returns (tests/gae_ref.py) at λ in {0, 0.3, 0.95, 1}, γ in {0.9, 0.99}, T from 1 to 500
-  (every window and lane boundary of the kernel's split near 32), one and four agents, with and without standardise_returns.
+- The returns against the float64 mixture of n-step returns (tests/gae_ref.py) at λ in {0, 0.3, 0.95, 1}, γ in {0.9, 0.99}, T in {1, 31, 32,
+  33, 64, 65, 500}, one and four agents, with and without standardise_returns, within 1e-5 of the batch's largest |R|.  These T are not the
+  kernel's boundaries (lanes of 8 steps, windows of 256): tests/test_returns_edges_gpu.py sweeps those, row by row.
 - Determinism, λ = 0 against the n_steps = 1 path, and the n-step path launching only nstep_returns_kernel while λ is unset.
 - Full updates against the oracle with the λ-returns (MLP and GRU parts, shared, independent and SePS networks, the centralised critic, PPO chains
   of 4 epochs), and the reference's own A2CNetwork / PPONetwork at n_steps = 1 and T as λ = 0 and λ = 1.
