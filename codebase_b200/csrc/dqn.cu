@@ -34,12 +34,15 @@ __global__ void replay_sample_kernel(uint64_t seed, uint64_t update_idx, int bat
 //            reference.  Columns of the statistics: one per agent (IDQN); the reference's VDN reshapes its (E, B) returns with reshape(-1, B), i.e.
 //            one column per batch entry -- stat_per_b selects that.  ret_ms_step (retms.cuh) then absorbs and standardises ret in place.
 //   STAGE 2: td from chosen and the standardised returns, and the loss statistics.
+//   STAGE 3 (algorithm.td_lambda): the bootstrap value boot[c][b][t] = v_{t+1} (unstandardised with the statistics so far when ret_ms is set; no
+//            reward or done applied) and chosen, for every (b, t); td_lambda_kernel then turns them into the λ-returns in ret, which STAGE 2 reads.
 struct ColTdParams {
   const float* q; const float* tq;  // [N][B][T+1][A]
   TrajView traj; const int32_t* idx; int B, A; float gamma; int double_q;
   int C, G;
-  const float* ret_ms; int n_stat, stat_per_b;   // STAGE 1: mean[n_stat] | var[n_stat]
-  float* ret; float* chosen;                     // STAGES 1, 2: [C][B][T]
+  const float* ret_ms; int n_stat, stat_per_b;   // STAGE 1 (STAGE 3: or NULL): mean[n_stat] | var[n_stat]
+  float* ret; float* chosen;                     // STAGES 1, 2, 3: [C][B][T]
+  float* boot;       // STAGE 3: [C][B][T]
   float* td;         // [C][B][T] = 2 * delta * filled
   float* loss_part;  // [gridDim][4]
 };
@@ -76,14 +79,82 @@ __global__ void __launch_bounds__(256) col_td_kernel(ColTdParams p) {
       const float rew = p.traj.rew[p.traj.step_at(ep, c * p.G, t)], done1 = (float)p.traj.done[p.traj.done_at(ep, t + 1)];
       if constexpr (STAGE == 0) {
         p.td[i] = td_error(chosen, td_target(rew, p.gamma, next, done1), (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill);
-      } else {
+      } else if constexpr (STAGE == 1) {
         const int col = p.stat_per_b ? b : c;
         p.ret[i] = td_target_rn(rew, p.gamma, unstandardise(next, p.ret_ms[col], p.ret_ms[p.n_stat + col]), done1);
+        p.chosen[i] = chosen;
+      } else {
+        const int col = p.stat_per_b ? b : c;
+        p.boot[i] = p.ret_ms ? unstandardise(next, p.ret_ms[col], p.ret_ms[p.n_stat + col]) : next;
         p.chosen[i] = chosen;
       }
     }
   }
-  if constexpr (STAGE != 1) block_loss_part(loss, fill, p.loss_part);
+  if constexpr (STAGE == 0 || STAGE == 2) block_loss_part(loss, fill, p.loss_part);
+}
+
+// TD(λ) targets (algorithm.td_lambda) of C columns over the sampled episodes, from the bootstrap values boot[c][b][t] = v_{t+1}:
+//   G_t = b_t + a_t G_{t+1},  a_t = γλ (1 - d_{t+1}) f_{t+1},  b_t = r_t + γ (1 - d_{t+1}) (1 - λ f_{t+1}) v_{t+1},  f_T := 0,
+// for every t in [0, T), filled or not; r_t is agent c G's reward.  The chain stops at the first unfilled row after t: a stale tail never reaches a
+// filled row's target.  One warp per (column, episode) sequence, right to left over windows of 32 x kTdlChunk steps: the warp stages (a_t, b_t)
+// coalesced in shared memory, each lane folds its chunk into the affine map G_in -> c + g G_in, a fixed-order suffix scan over the lanes composes the
+// maps, each lane replays its chunk from the return after it, and the warp writes the returns coalesced.  The window's first return carries into the next.
+constexpr int kTdlChunk = 8, kTdlWindow = 32 * kTdlChunk, kTdlWarps = 8;
+
+struct TdLambdaParams {
+  const float* boot;   // [C][B][T]
+  TrajView traj; const int32_t* idx; int C, G, B;
+  float gamma, lambda, gl;   // gl = float32(γλ)
+  float* ret;          // [C][B][T]
+};
+
+__device__ __forceinline__ int tdl_slot(int s) { return (s / kTdlChunk) * (kTdlChunk + 1) + s % kTdlChunk; }   // lane chunks padded: no bank conflicts
+
+__global__ void __launch_bounds__(32 * kTdlWarps) td_lambda_kernel(TdLambdaParams p) {
+  __shared__ float sa[kTdlWarps][32 * (kTdlChunk + 1)], sb[kTdlWarps][32 * (kTdlChunk + 1)];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, seq = blockIdx.x * kTdlWarps + w;
+  if (seq >= p.C * p.B) return;
+  const int T = p.traj.T, c = seq / p.B, b = seq - c * p.B;
+  const size_t ep = (size_t)p.idx[b];
+  const float* boot = p.boot + (size_t)seq * T;
+  const float* rew = p.traj.rew + p.traj.step_at(ep, c * p.G, 0);
+  const uint8_t* done = p.traj.done + p.traj.done_at(ep, 0);
+  const uint8_t* filled = p.traj.filled + p.traj.filled_at(ep, 0);
+  float* ret = p.ret + (size_t)seq * T;
+  float* a_s = sa[w];
+  float* b_s = sb[w];
+  float carry = 0.f;   // G at the step after the window
+  for (int w0 = ((T - 1) / kTdlWindow) * kTdlWindow; w0 >= 0; w0 -= kTdlWindow) {
+    const int len = min(kTdlWindow, T - w0);
+    for (int j = lane; j < len; j += 32) {
+      const int t = w0 + j;
+      const float live1 = 1.f - (float)done[t + 1], f1 = t + 1 < T ? (float)filled[t + 1] : 0.f;
+      a_s[tdl_slot(j)] = p.gl * live1 * f1;
+      b_s[tdl_slot(j)] = rew[t] + (p.gamma * live1) * ((1.f - p.lambda * f1) * boot[t]);
+    }
+    __syncwarp();
+    const int lo = lane * kTdlChunk, hi = min(lo + kTdlChunk, len);
+    float cc = 0.f, g = 1.f;   // this lane's chunk: G_lo = cc + g G_hi
+    for (int j = hi - 1; j >= lo; --j) { cc = b_s[tdl_slot(j)] + a_s[tdl_slot(j)] * cc; g *= a_s[tdl_slot(j)]; }
+    // suffix scan: lane l ends with the composition of the maps of lanes l .. 31
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const float c2 = __shfl_down_sync(0xffffffffu, cc, off), g2 = __shfl_down_sync(0xffffffffu, g, off);
+      if (lane + off < 32) { cc = cc + g * c2; g *= g2; }
+    }
+    float r = __shfl_down_sync(0xffffffffu, cc + g * carry, 1);   // G at the step after this lane's chunk
+    if (lane == 31) r = carry;
+    for (int j = hi - 1; j >= lo; --j) { r = b_s[tdl_slot(j)] + a_s[tdl_slot(j)] * r; b_s[tdl_slot(j)] = r; }
+    carry = __shfl_sync(0xffffffffu, r, 0);   // G_{w0}, as written
+    __syncwarp();
+    for (int j = lane; j < len; j += 32) ret[w0 + j] = b_s[tdl_slot(j)];
+    __syncwarp();
+  }
+}
+
+static cudaError_t launch_td_lambda(const TdLambdaParams& p, cudaStream_t st) {
+  td_lambda_kernel<<<(p.C * p.B + kTdlWarps - 1) / kTdlWarps, 32 * kTdlWarps, 0, st>>>(p);
+  return cudaGetLastError();
 }
 
 }  // namespace marl
@@ -113,8 +184,10 @@ struct marl_dqn : LearnerHandle {
   // optional CUDA-event timing of the training kernel (bench.py's roofline leg)
   // measurement hook: 4 events per timed update (before the training pass, after each of its kernels; the FP32 path uses 0 and 3)
   bool timing = false; std::vector<cudaEvent_t> ev; int ev_used = 0; bool ev_split = false;
-  // cfg.standardise_returns: returns / chosen-Q scratch next to the statistics
+  // cfg.standardise_returns, algorithm.td_lambda: returns / chosen-Q scratch next to the statistics
   float *ret = nullptr, *chosen = nullptr;
+  // algorithm.td_lambda (marl_dqn_set_td_lambda): λ-returns in place of the one-step target; boot: the bootstrap values v_{t+1} per (column, b, t)
+  bool td_lambda_on = false; float td_lambda = 0.f; float* boot = nullptr;
   // QMIX (hp.mixer == 2): the mixing network's parameters / Adam state / gradient (+ 4 statistics), per-sample records, chunked partial sums, tile list
   QmixLayout ql = {}; float *mix = nullptr, *mix_tgt = nullptr, *mix_m = nullptr, *mix_v = nullptr, *mix_grad = nullptr, *mix_rec = nullptr, *mix_part = nullptr, *mix_img = nullptr, *mix_img_tgt = nullptr;
   QmixTile* mix_tiles = nullptr; int mix_n_tiles = 0; QmixMicro* mix_micro = nullptr; int mix_n_micro = 0; bool mix_wgrad_tiles = false;
@@ -205,7 +278,8 @@ int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
     const char* who = "marl_dqn_standardise_returns";
     const int n = h->hp.mixer != 0 ? h->max_batch : h->ns.n_agents, C = h->hp.mixer != 0 ? 1 : h->ns.n_agents;
     const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), cbt = (size_t)C * h->max_batch * h->max_T, F = sizeof(float);
-    if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
+    if (!h->ret)   // (marl_dqn_set_td_lambda may have allocated them)
+      if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
     if (!h->q_all)
       if (int rc = alloc_buffers(h, who, {{&h->q_all, rows * h->ns.out * F}})) return rc;
     if (!h->td || (h->hp.mixer == 0 && !h->rnn)) {
@@ -219,6 +293,32 @@ int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
   h->standardise = enable ? 1 : 0;
   return MARL_OK;
 }
+/* algorithm.td_lambda: enable != 0 replaces the one-step TD target of every later update (marl_dqn_update*, update_n, the fused tail) by the λ-return
+ * of `lambda` in [0, 1] over the sampled episode (DESIGN.md §4.4d); enable == 0 restores the one-step target.  The first enable allocates the
+ * bootstrap values, returns, chosen Q-values, TD error, the online Q-values of every row and the loss statistics' room -- the external TD head's
+ * buffers, which IDQN then takes on every path. */
+int marl_dqn_set_td_lambda(marl_dqn* h, int32_t enable, float lambda) {
+  MARL_REQUIRE(!enable || (lambda >= 0.f && lambda <= 1.f), "marl_dqn_set_td_lambda: lambda %g is outside [0, 1]", (double)lambda);
+  MARL_REQUIRE(h != nullptr, "marl_dqn_set_td_lambda: NULL handle");
+  MARL_CUDA_TRY(cudaSetDevice(h->device));
+  if (enable && !h->boot) {
+    const char* who = "marl_dqn_set_td_lambda";
+    const int C = h->hp.mixer != 0 ? 1 : h->ns.n_agents;
+    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), cbt = (size_t)C * h->max_batch * h->max_T, F = sizeof(float);
+    if (!h->ret)
+      if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
+    if (!h->q_all)
+      if (int rc = alloc_buffers(h, who, {{&h->q_all, rows * h->ns.out * F}})) return rc;
+    if (!h->td)   // IDQN's MLP path has none yet; every other learner's was sized at create
+      if (int rc = alloc_buffers(h, who, {{&h->td, cbt * F}})) return rc;
+    if (int rc = dqn_grow_loss_part(h, (size_t)h->n_sm + cbt / 256 + 2, who)) return rc;
+    if (int rc = alloc_buffers(h, who, {{&h->boot, cbt * F}})) return rc;
+  }
+  h->td_lambda_on = enable != 0;
+  h->td_lambda = enable ? lambda : 0.f;
+  return MARL_OK;
+}
+
 int marl_dqn_ret_ms_ptrs(marl_dqn* h, float** ret_ms, double** count, int32_t* n_stat) {
   MARL_REQUIRE(h != nullptr, "marl_dqn_ret_ms_ptrs: NULL handle");
   if (ret_ms) *ret_ms = h->ret_ms; if (count) *count = h->ret_count; if (n_stat) *n_stat = h->n_stat;
@@ -229,8 +329,8 @@ int marl_dqn_ret_ms_ptrs(marl_dqn* h, float** ret_ms, double** count, int32_t* n
  * initialised by the caller through marl_dqn_qmix_ptrs (nn.Linear defaults), then marl_dqn_sync_target copies them to the target mixer. */
 typedef void (*QmixMixFn)(QmixParams, const float*, const float*);
 static QmixMixFn qmix_mix_fn(int hl, int mode) {
-  static const QmixMixFn fns[2][3] = {{qmix_mix_kernel<1, 0>, qmix_mix_kernel<1, 1>, qmix_mix_kernel<1, 2>},
-                                      {qmix_mix_kernel<2, 0>, qmix_mix_kernel<2, 1>, qmix_mix_kernel<2, 2>}};
+  static const QmixMixFn fns[2][4] = {{qmix_mix_kernel<1, 0>, qmix_mix_kernel<1, 1>, qmix_mix_kernel<1, 2>, qmix_mix_kernel<1, 3>},
+                                      {qmix_mix_kernel<2, 0>, qmix_mix_kernel<2, 1>, qmix_mix_kernel<2, 2>, qmix_mix_kernel<2, 3>}};
   return fns[hl - 1][mode];
 }
 
@@ -267,8 +367,9 @@ int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, 
   MARL_CUDA_TRY(cudaMemcpy(h->mix_micro, micro.data(), (size_t)nm * sizeof(QmixMicro), cudaMemcpyHostToDevice));
   h->mix_n_micro = nm;
   // the attribute is per function, process-wide: only ever raise it (a second learner with a smaller mixer must not lower the first one's limit).
-  // Every instantiation of qmix_mix_kernel is a function of its own; standardise_returns may be switched on after this call, so all three modes.
-  static size_t mix_limits[64][2][3] = {}, wg_limits[64] = {};   // per device (one process normally drives one GPU)
+  // Every instantiation of qmix_mix_kernel is a function of its own; standardise_returns and td_lambda may be switched on after this call, so all
+  // four modes.
+  static size_t mix_limits[64][2][4] = {}, wg_limits[64] = {};   // per device (one process normally drives one GPU)
   size_t& wg_smem_limit = wg_limits[h->device & 63];
   const size_t wg_smem = (size_t)(h->ql.R + 2) * kQmP * sizeof(float);
   const char* ev = getenv("MARL_QMIX_WGRAD_TILES");
@@ -277,7 +378,7 @@ int marl_dqn_qmix_init(marl_dqn* h, int32_t embed_dim, int32_t hypernet_layers, 
     MARL_CUDA_TRY(cudaFuncSetAttribute(qmix_wgrad2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg_smem));
     wg_smem_limit = wg_smem;
   }
-  for (int mode = 0; mode < 3; ++mode) {
+  for (int mode = 0; mode < 4; ++mode) {
     size_t& mix_smem_limit = mix_limits[h->device & 63][hypernet_layers - 1][mode];
     if (qm_smem_bytes(h->ql) > mix_smem_limit) {
       MARL_CUDA_TRY(cudaFuncSetAttribute(qmix_mix_fn(hypernet_layers, mode), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qm_smem_bytes(h->ql)));
@@ -399,7 +500,15 @@ int marl_replay_sample(uint64_t seed, uint64_t update_idx, int32_t batch, int32_
   return MARL_OK;
 }
 
-static bool dqn_external_head(const marl_dqn* h) { return h->hp.mixer != 0 || h->rnn || h->standardise; }
+static bool dqn_external_head(const marl_dqn* h) { return h->hp.mixer != 0 || h->rnn || h->standardise || h->td_lambda_on; }
+
+// algorithm.td_lambda: the λ-returns of C columns (reward of agent c G) from h->boot into h->ret
+static int dqn_td_lambda(const marl_dqn* h, const RowSource& src, int C, int G, int batch, cudaStream_t st) {
+  TdLambdaParams lp; lp.boot = h->boot; lp.traj = src.traj; lp.idx = src.idx; lp.C = C; lp.G = G; lp.B = batch; lp.ret = h->ret;
+  lp.gamma = h->hp.gamma; lp.lambda = h->td_lambda; lp.gl = (float)((double)h->hp.gamma * (double)h->td_lambda);
+  MARL_CUDA_TRY(launch_td_lambda(lp, st));
+  return MARL_OK;
+}
 
 // The external TD head, for the cases the training pass's own head does not cover (QMIX, standardise_returns, VDN, the recurrent pass): the online
 // forward on every row (forward = false: the fused training forward has already written q_all), then dL/dQ of the taken actions into td, which
@@ -419,7 +528,17 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
     qp.loss_part = loss_part;
     const int Sn = batch * T, qb = (Sn + kQmTS - 1) / kQmTS, n = h->ql.n, hl = h->ql.hl;
     qmix_pack_kernel<<<dim3((n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
-    if (h->standardise) {   // target pass -> returns, RunningMeanStd step (one column per batch entry), online pass on the standardised returns
+    if (h->td_lambda_on) {   // target pass -> bootstrap values, λ-return scan (one column, agent 0's reward), [RunningMeanStd step], online pass
+      qp.ret = h->ret; qp.boot = h->boot;
+      if (h->standardise) { qp.ret_ms = h->ret_ms; qp.n_stat = h->n_stat; }
+      qmix_mix_fn(hl, 3)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+      if (int rc = dqn_td_lambda(h, src, 1, h->ns.n_agents, batch, st)) return rc;
+      if (h->standardise) {
+        RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T; rp.N = batch; rp.P = 1;
+        MARL_CUDA_TRY(ret_ms_step(rp, st));
+      }
+      qmix_mix_fn(hl, 2)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+    } else if (h->standardise) {   // target pass -> returns, RunningMeanStd step (one column per batch entry), online pass on the standardised returns
       qp.ret_ms = h->ret_ms; qp.n_stat = h->n_stat; qp.ret = h->ret;
       qmix_mix_fn(hl, 1)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
       RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T; rp.N = batch; rp.P = 1;
@@ -449,7 +568,18 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
   cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.C = vdn ? 1 : h->ns.n_agents; cp.G = vdn ? h->ns.n_agents : 1;
   cp.td = h->td; cp.loss_part = loss_part;
   const int blocks = (cp.C * batch * T + 255) / 256;
-  if (h->standardise) {   // returns + chosen Q, RunningMeanStd step, TD error on the standardised returns
+  if (h->td_lambda_on) {   // bootstrap values + chosen Q, λ-return scan, [RunningMeanStd step], TD error on the (standardised) returns
+    cp.ret = h->ret; cp.chosen = h->chosen; cp.boot = h->boot; cp.stat_per_b = vdn;
+    if (h->standardise) { cp.ret_ms = h->ret_ms; cp.n_stat = h->n_stat; }
+    col_td_kernel<3><<<blocks, 256, 0, st>>>(cp);
+    if (int rc = dqn_td_lambda(h, src, cp.C, cp.G, batch, st)) return rc;
+    if (h->standardise) {
+      RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T;
+      if (vdn) { rp.N = batch; rp.P = 1; } else { rp.N = cp.C; rp.P = batch; }
+      MARL_CUDA_TRY(ret_ms_step(rp, st));
+    }
+    col_td_kernel<2><<<blocks, 256, 0, st>>>(cp);
+  } else if (h->standardise) {   // returns + chosen Q, RunningMeanStd step, TD error on the standardised returns
     cp.ret_ms = h->ret_ms; cp.n_stat = h->n_stat; cp.stat_per_b = vdn; cp.ret = h->ret; cp.chosen = h->chosen;
     col_td_kernel<1><<<blocks, 256, 0, st>>>(cp);
     RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T;
@@ -633,7 +763,7 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
   // GPUs the extra launch (prologue, second pass over the Adam state) cost more than the hidden wait saved (120.9 vs 116.8 us per update).
   if (h->xchg.world > 1 && tc_split_exchange_enabled()) {
     if (launch_reduce_push(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->push_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
-      if (next != nullptr && ap.target_mode == 0 && !h->standardise && h->hp.mixer == 0 && !h->rnn) {
+      if (next != nullptr && ap.target_mode == 0 && !dqn_external_head(h)) {
         const RowPlan plan = episode_plan(h->ns, batch, traj->T, h->n_sm);
         const RowSource src = episode_rows(traj, next->idx, h->ns.n_agents, h->ns.in);
         if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, (cudaStream_t)stream)) return rc;

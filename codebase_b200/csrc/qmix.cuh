@@ -17,7 +17,8 @@
 //   qmix_reduce_kernel the chunks in fixed order -> gradient; the filled count next to it (Adam's 1 / filled.sum()).
 // One-layer hypernetworks (hypernet_layers = 1): W1 = Linear(S -> N*E), w_final = Linear(S -> E), five linear layers (QmixLayout.hl, qmix_linears);
 // W1 stays in global memory (read through L1 / L2), the rest of the image in shared memory.  standardise_returns splits qmix_mix_kernel into a
-// target pass (returns) and an online pass around ret_ms_step (MODE 1 / 2).
+// target pass (returns) and an online pass around ret_ms_step (MODE 1 / 2); algorithm.td_lambda runs a target pass that writes the bootstrap values
+// (MODE 3), the λ-return scan, then the online pass (MODE 2).
 // The mixer's parameters take the shared Adam step WITHOUT gradient clipping: the reference clips self.critic.parameters() only (dqn/model.py:169-170).
 #pragma once
 #include "learner.cuh"
@@ -89,8 +90,9 @@ struct QmixParams {
   float* td;          // [N][B][T] = dL/dq_a (un-normalised: x 2 delta filled)
   float* loss_part;   // [gridDim][4]
   // standardise_returns (two launches around ret_ms_step): the target pass writes ret[b][t], the online pass reads it back standardised
-  const float* ret_ms; int n_stat;   // mean[n_stat] | var[n_stat], one column per batch entry
+  const float* ret_ms; int n_stat;   // mean[n_stat] | var[n_stat], one column per batch entry (MODE 3: NULL without standardise_returns)
   float* ret;                        // [B][T]
+  float* boot;                       // MODE 3 (algorithm.td_lambda): [B][T] the target mixer's Q_tot at t + 1
 };
 
 // ---- qmix_mix_kernel: 32 samples per CTA (lane = sample), 8 warps share each layer's outputs -----------------------------------------------------
@@ -252,7 +254,8 @@ __device__ __forceinline__ void qm_load_inputs(const QmSmem& sm, const QmixParam
 // HL: hypernetwork layers (the image's shared-memory part and the forward / backward follow the layout's table).  MODE 0: target and online pass
 // in one launch.  standardise_returns needs the whole batch's returns before any TD error: MODE 1 runs the target pass only and writes
 // ret[b][t] = r + gamma (Q_tot' sqrt(var[b]) + mean[b]) (1 - done) for every sample; ret_ms_step standardises them; MODE 2 runs the online
-// pass against the standardised ret.
+// pass against the standardised ret.  algorithm.td_lambda: MODE 3 runs the target pass only and writes boot[b][t] = Q_tot' (de-standardised as in
+// MODE 1 when ret_ms is set); td_lambda_kernel (dqn.cu) turns it into the λ-returns in ret, and MODE 2 runs the online pass against them.
 template <int HL, int MODE>
 __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p, const float* __restrict__ img, const float* __restrict__ img_tgt) {
   extern __shared__ __align__(16) float qsm[];
@@ -284,6 +287,8 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
       const float tq = unstandardise(ytgt, p.ret_ms[b], p.ret_ms[p.n_stat + b]);
       p.ret[s] = td_target_rn(p.traj.rew[p.traj.step_at(ep, 0, t)], p.gamma, tq, (float)p.traj.done[p.traj.done_at(ep, t + 1)]);
     }
+  } else if constexpr (MODE == 3) {
+    if (live && warp == 0) p.boot[s] = p.ret_ms ? unstandardise(ytgt, p.ret_ms[b], p.ret_ms[p.n_stat + b]) : ytgt;
   } else {
     // ---- online ----
     for (int i = threadIdx.x; i < n4; i += kQmWarps * 32) reinterpret_cast<float4*>(sm.W)[i] = reinterpret_cast<const float4*>(img)[r4 + i];

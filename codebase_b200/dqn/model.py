@@ -9,7 +9,9 @@ owner of device buffers.  There is no CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+import numbers
 import random
+import types
 
 import numpy as np
 import torch
@@ -21,11 +23,26 @@ from ..learner import MAX_AGENTS, NativeLearner, flat_to_state_dict, flatdim, hi
 from ..native_env import TrajStore
 
 
+def td_lambda(cfg):
+    """cfg.td_lambda: None (absent or null: the reference's one-step TD target) or the λ in [0, 1] of the TD(λ) target that replaces it.  Anything
+    else raises ValueError here, before any native call."""
+    lam = getattr(cfg, "td_lambda", None)
+    if lam is None:
+        return None
+    if isinstance(lam, bool) or not isinstance(lam, numbers.Real):
+        raise ValueError(f"algorithm.td_lambda must be null or a number in [0, 1], not {lam!r}")
+    lam = float(lam)
+    if not 0.0 <= lam <= 1.0:
+        raise ValueError(f"algorithm.td_lambda must be in [0, 1], not {lam}")
+    return lam
+
+
 class QNetwork(NativeLearner):
     mixer = 0
     _destroy = "marl_dqn_destroy"
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch=None, max_episode_length=None):
+        self.td_lambda = td_lambda(cfg)
         self.use_rnn = bool(use_rnn)
         self.hidden = hidden_width(layers, "layers", self.use_rnn)
         self._open(obs_space, action_space, cfg, device)
@@ -62,6 +79,14 @@ class QNetwork(NativeLearner):
         self.standardise_returns = bool(getattr(cfg, "standardise_returns", False))   # dqn/model.py:82-84 (VDN: 221-222)
         if self.standardise_returns:
             nat.check(self._lib.marl_dqn_standardise_returns(self._h, C.c_int32(1)), "marl_dqn_standardise_returns")
+        if self.td_lambda is not None:
+            self.set_td_lambda(self.td_lambda)
+
+    def set_td_lambda(self, lam):
+        """TD(λ) targets of `lam` in [0, 1] in place of the one-step target from the next update on (DESIGN.md §4.4d); None: the one-step target again"""
+        lam = td_lambda(types.SimpleNamespace(td_lambda=lam))
+        nat.check(self._lib.marl_dqn_set_td_lambda(self._h, C.c_int32(lam is not None), C.c_float(0.0 if lam is None else lam)), "marl_dqn_set_td_lambda")
+        self.td_lambda = lam
 
     def ret_ms(self):
         """(mean, var, count) of the RunningMeanStd over the TD targets (standardise_returns): one entry per agent; VDN, QMIX: per batch entry."""

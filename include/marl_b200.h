@@ -301,6 +301,12 @@ int marl_dqn_destroy(marl_dqn* q);
  * reshape), so their updates must use batch == max_batch. */
 int marl_dqn_standardise_returns(marl_dqn* q, int32_t enable);
 int marl_dqn_ret_ms_ptrs(marl_dqn* q, float** ret_ms /* mean[n] | var[n] */, double** count, int32_t* n_stat);
+/* algorithm.td_lambda of IDQN, VDN and QMIX (this project's option; the reference has only the one-step target): enable != 0 makes every later
+ * update (marl_dqn_update, _update_grads, _update_n) use the TD(λ) target of `lambda` in [0, 1] over the sampled episode,
+ *   G_t = r_t + γ (1 - d_{t+1}) ((1 - λ f_{t+1}) v_{t+1} + λ f_{t+1} G_{t+1}),  f_T = 0,
+ * with v the learner's bootstrap value (double-Q or max, VDN: summed over agents, QMIX: the target mixer's Q_tot) -- λ = 0 is the one-step target.
+ * Under standardise_returns the statistics absorb G.  enable == 0 restores the one-step target.  λ outside [0, 1] is refused. */
+int marl_dqn_set_td_lambda(marl_dqn* q, int32_t enable, float lambda);
 /* QMixNetwork (marlbase/dqn/model.py:272-443, configs/algorithm/qmix.yaml): with hp.mixer == 2, call once after marl_dqn_create.  The mixing
  * network works on state = the agents' observations concatenated (state_dim = n_agents * in_dim); its parameters are one flat vector in the
  * reference's state_dict order (weight, bias each): hypernet_layers == 2: hyper_w_1.0, hyper_w_1.2, hyper_w_final.0, hyper_w_final.2, hyper_b_1,

@@ -1,0 +1,301 @@
+"""GPU: TD(λ) targets of IDQN, VDN and QMIX (algorithm.td_lambda; col_td_kernel's bootstrap stage, qmix_mix_kernel's MODE 3 and td_lambda_kernel in
+csrc/dqn.cu / csrc/qmix.cuh) against the float64 oracle (tests/td_lambda_ref.py): loss, gradients and parameters after each update of unglued chains
+on ragged episodes -- the tensor-core and the FP32 training pass, GRU agents, both QMIX mixers, double-Q on and off, standardise_returns, truncated
+episodes, parameter sharing, stale tails -- at λ in {0, 0.6, 1} and T at every window edge of the scan up to 513; the update_n chain against its
+loop and the oracle; λ = 0 against the one-step target; and the training drivers end to end."""
+import copy
+import ctypes as C
+import dataclasses
+import types
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import learner_ref as lr
+from oracle import policy_ref
+from oracle import qmix_ref as qr
+from tests import hidden_width_ref as hw
+from tests import qmix_options_ref as qo
+from tests import td_lambda_ref as tl
+from tests.helpers import TIE, NearTie, assert_grad_close, random_store, redraw_on_near_tie, space, traj_store
+
+pytestmark = pytest.mark.gpu
+A = 6
+MIXER = {"idqn": 0, "vdn": 1, "qmix": 2}
+
+
+@dataclasses.dataclass(frozen=True)
+class Case:
+    kind: str = "idqn"
+    lam: float = 0.6
+    N: int = 2
+    D: int = 9
+    T: int = 25
+    B: int = 16
+    H: int = 128
+    rnn: bool = False
+    hl: int = 2
+    sharing: bool = False
+    double_q: bool = True
+    standardise: bool = False
+    tu: float = 2.0
+    tails: str = "ragged"   # ragged: done before T, unfilled tails; truncated: no done flag at all (use_proper_termination); stale: filled again after a gap
+
+
+def _hp(c):
+    return lr.DqnHP(double_q=c.double_q, target_update_interval_or_tau=c.tu, mixer=MIXER[c.kind])
+
+
+def _model(c, lam="case"):
+    from codebase_b200.dqn import model as M
+
+    hp = _hp(c)
+    cfg = types.SimpleNamespace(optimizer="Adam", lr=hp.lr, gamma=hp.gamma, grad_clip=hp.grad_clip, double_q=c.double_q, target_update_interval_or_tau=c.tu,
+                                standardise_returns=c.standardise, td_lambda=c.lam if lam == "case" else lam)
+    obs, act = [space(shape=(c.D,))] * c.N, [space(n=A)] * c.N
+    if c.kind == "qmix":
+        return M.QMixNetwork(obs, act, cfg, [c.H, c.H], c.sharing, c.rnn, True, dict(embed_dim=32, hypernet_layers=c.hl, hypernet_embed=32), "cuda",
+                             max_batch=c.B, max_episode_length=c.T)
+    cls = M.VDNetwork if c.kind == "vdn" else M.QNetwork
+    return cls(obs, act, cfg, [c.H, c.H], c.sharing, c.rnn, True, "cuda", max_batch=c.B, max_episode_length=c.T)
+
+
+def _perturb_target(m):
+    """a target that differs from the online networks, so that the double-Q pick and the target networks matter"""
+    m.theta_tgt.copy_(m.theta + 0.01 * torch.randn_like(m.theta))
+    if m.mixer == 2:
+        m.mix_tgt.copy_(m.mix + 0.01 * torch.randn_like(m.mix))
+    m.params_changed()
+
+
+def _agent_net(c):
+    return [0] * c.N if c.sharing else list(range(c.N))
+
+
+def _oracle(c, m):
+    ms = (lambda: lr.RunningMeanStdRef((c.N,) if c.kind == "idqn" else (1,))) if c.standardise else (lambda: None)
+    if c.kind == "qmix":
+        return qo.QmixOptState(m.theta.cpu().clone(), m.theta_tgt.cpu().clone(), m.mix.cpu().clone(), m.mix_tgt.cpu().clone(), _agent_net(c), c.D, A,
+                               embed_dim=32, hypernet_layers=c.hl, ret_ms=ms())
+    return lr.DqnState(m.theta.cpu().clone(), m.theta_tgt.cpu().clone(), _agent_net(c), c.D, A, ret_ms=ms())
+
+
+def _store(c, seed, cap=None):
+    """cap episodes (default B) in the device layout; VDN and QMIX see the team reward"""
+    rng = np.random.default_rng(seed)
+    s = random_store(rng, cap or c.B, c.N, c.T, c.D, c.kind != "idqn", A=A)
+    if c.tails == "truncated":
+        s["done"][:] = 0
+    elif c.tails == "stale":   # rows marked filled again after an unfilled gap (a re-used slot's stale tail), done flags among them
+        for e in range(0, s["filled"].shape[0], 2):
+            L = int(s["filled"][e].sum())
+            if L + 1 < c.T:
+                s["filled"][e, L + 1:] = 1
+                s["done"][e, L + 1:] = rng.random(c.T - L) < 0.2
+    return s
+
+
+def _update_oracle(c, st, batch, hp):
+    with hw.networks({(c.D, A)} if c.rnn else ()), tl.td_lambda_in(c.lam):
+        return qr.qmix_update(st, batch, hp) if c.kind == "qmix" else lr.dqn_update(st, batch, hp)
+
+
+def _margin(c, st, batch, hp):
+    if not c.double_q:
+        return
+    with hw.networks({(c.D, A)} if c.rnn else ()):
+        margin = lr.double_q_margin(lr.DqnState(st.theta, st.theta_tgt, st.agent_net, c.D, A), batch, hp)
+    if margin < TIE:
+        raise NearTie(f"double-Q argmax margin {margin:.1e}")
+
+
+def _kink(c, st0, batch, hp):
+    def risk():
+        with hw.networks({(c.D, A)} if c.rnn else ()):
+            if c.kind == "qmix":
+                return tl.qmix_kink_risk(st0, batch, hp, c.lam)
+            with tl.td_lambda_in(c.lam):
+                return lr.dqn_kink_risk(st0, batch, hp)
+    return risk
+
+
+def _close(got, want, tol, what):
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    scale = max(1.0, float(np.abs(want).max()))
+    err = float(np.abs(got - want).max())
+    assert err <= tol * scale, f"{what}: max abs error {err:.3e} > {tol:g} x {scale:.3g}"
+
+
+def _check_update(c, m, st, st0, batch, want, met, hp, what):
+    filled = float(batch["filled"].sum())
+    assert abs(float(met[0]) - want["loss"]) <= 2e-5 * max(1.0, abs(want["loss"])), f"loss {float(met[0])} vs {want['loss']}, {what}"
+    assert_grad_close(lr, st0, batch, hp, m.grad[: m.n_params].cpu().numpy() / filled, want["grad"].numpy(), tol=2e-5, what=f"agents' gradient, {what}",
+                      kink_risk=_kink(c, st0, batch, hp))
+    mine = [(m.theta, st.theta, "theta"), (m.theta_tgt, st.theta_tgt, "target")]
+    if c.kind == "qmix":
+        _close(m.mix_grad[: m.n_mix].cpu().numpy() / filled, want["mix_grad"].numpy(), 2e-5, f"mixer gradient, {what}")
+        mine += [(m.mix, st.mix, "mixer"), (m.mix_tgt, st.mix_tgt, "target mixer")]
+    for got, ref, name in mine:
+        assert np.quantile(np.abs(got.cpu().numpy() - ref.numpy()), 0.999) < 2e-5, f"{name} after {what}"
+    if c.standardise:
+        mean, var, count = m.ret_ms()
+        want_mean, want_var = np.broadcast_to(st.ret_ms.mean.numpy(), mean.shape), np.broadcast_to(st.ret_ms.var.numpy(), var.shape)
+        np.testing.assert_allclose(mean.numpy(), want_mean, rtol=1e-5, atol=1e-6, err_msg=f"ret_ms mean, {what}")
+        np.testing.assert_allclose(var.numpy(), want_var, rtol=1e-5, atol=1e-5, err_msg=f"ret_ms var, {what}")
+        assert count == pytest.approx(st.ret_ms.count, rel=1e-12), what
+
+
+def _run_chain(c, n_updates=3):
+    hp = _hp(c)
+    m = _model(c)
+    _perturb_target(m)
+    st = _oracle(c, m)
+    idx = torch.arange(c.B, dtype=torch.int32, device=m.device)
+    for u in range(n_updates):
+        s = _store(c, 1000 * u + c.B + c.T)
+        batch = lr.batch_from_store(s, np.arange(c.B))
+        _margin(c, st, batch, hp)
+        st0 = copy.deepcopy(st)
+        want = _update_oracle(c, st, batch, hp)
+        met = m.update_from_store(traj_store(s, m.device), idx).cpu()
+        _check_update(c, m, st, st0, batch, want, met, hp, f"update {u}")
+    m.close()
+
+
+# ---- 1. unglued chains against the oracle --------------------------------------------------------------------------------------------------------
+CHAIN = {
+    "idqn_tc": Case(),
+    "idqn_tc_lam0": Case(lam=0.0),
+    "idqn_tc_lam1_single_q": Case(lam=1.0, double_q=False),
+    "idqn_tc_standardise_polyak": Case(standardise=True, tu=0.05),
+    "idqn_tc_shared_stale": Case(sharing=True, tails="stale", N=3),
+    "idqn_tc_truncated": Case(tails="truncated", lam=1.0),
+    "idqn_fp32": Case(H=64),
+    "idqn_fp32_standardise_lam1": Case(H=64, standardise=True, lam=1.0, tails="stale"),
+    "vdn": Case(kind="vdn", N=3),
+    "vdn_lam1_standardise": Case(kind="vdn", lam=1.0, standardise=True),
+    "vdn_single_q_truncated": Case(kind="vdn", double_q=False, tails="truncated"),
+    "qmix_h2": Case(kind="qmix"),
+    "qmix_h1": Case(kind="qmix", hl=1, N=3),
+    "qmix_h1_lam0_standardise": Case(kind="qmix", hl=1, lam=0.0, standardise=True),
+    "qmix_h2_lam1_standardise_stale": Case(kind="qmix", lam=1.0, standardise=True, tails="stale"),
+    "qmix_h2_single_q_shared_truncated": Case(kind="qmix", double_q=False, sharing=True, tails="truncated", tu=0.05),
+    "rnn_idqn": Case(rnn=True, T=9, B=8),
+    "rnn_idqn_standardise_lam1": Case(rnn=True, T=9, B=8, lam=1.0, standardise=True),
+    "rnn_vdn": Case(kind="vdn", rnn=True, T=9, B=8, tails="stale"),
+    "rnn_qmix_h1": Case(kind="qmix", hl=1, rnn=True, T=9, B=8),
+    "rnn_qmix_h2_standardise": Case(kind="qmix", rnn=True, T=9, B=8, standardise=True, lam=0.0),
+}
+
+
+@pytest.mark.parametrize("name", list(CHAIN))
+@redraw_on_near_tie
+def test_unglued_chain_matches_oracle(name):
+    """three updates through marl_dqn_update on fresh ragged batches; the device state is never re-synchronised with the oracle"""
+    _run_chain(CHAIN[name])
+
+
+# ---- 2. episode lengths at the scan's window edges (windows of 256 steps) ------------------------------------------------------------------------
+EDGES = [(1, "idqn"), (2, "vdn"), (255, "idqn"), (256, "qmix"), (257, "vdn"), (500, "qmix"), (513, "idqn")]
+
+
+@pytest.mark.parametrize("T,kind", EDGES)
+@redraw_on_near_tie
+def test_episode_lengths_at_window_edges(T, kind):
+    _run_chain(Case(kind=kind, T=T, B=4, N=2, D=7, lam=0.6 if T % 2 else 1.0, tails="stale" if T > 2 else "ragged"), n_updates=2)
+
+
+# ---- 3. update_n: the loop it replaces, bit for bit, and the oracle ------------------------------------------------------------------------------
+SEED = 0x7D1A
+
+
+def _state(m):
+    out = dict(theta=m.theta, theta_tgt=m.theta_tgt, adam_m=m.adam_m, adam_v=m.adam_v, grad=m.grad, metrics=m._metrics)
+    if m.mixer == 2:
+        out.update(mix=m.mix, mix_tgt=m.mix_tgt, mix_m=m.mix_m, mix_v=m.mix_v, mix_grad=m.mix_grad)
+    return {k: v.detach().cpu().clone() for k, v in out.items()}
+
+
+@pytest.mark.parametrize("kind", ["idqn", "vdn", "qmix"])
+@redraw_on_near_tie
+def test_update_n_is_the_loop_it_replaces_and_tracks_the_oracle(kind):
+    from codebase_b200 import _native as nat
+
+    c, K, cap = Case(kind=kind, T=12, B=24, tu=3.0), 4, 64
+    hp = _hp(c)
+    a, b = _model(c), _model(c)
+    _perturb_target(a)
+    for k in ("theta", "theta_tgt") + (("mix", "mix_tgt") if kind == "qmix" else ()):
+        getattr(b, k).copy_(getattr(a, k))
+    b.params_changed()
+    st = _oracle(c, a)
+    s = _store(c, 77, cap)
+    ts = traj_store(s, a.device)
+    a.update_n(ts, c.B, cap, SEED, 0, K)
+    idx = torch.zeros(c.B, dtype=torch.int32, device=b.device)
+    for u in range(K):
+        nat.check(nat.lib().marl_replay_sample(C.c_uint64(SEED), C.c_uint64(u), C.c_int32(c.B), C.c_int32(cap), nat.ptr(idx), nat.stream_ptr()), "marl_replay_sample")
+        ids = policy_ref.replay_sample(SEED, u, c.B, cap)
+        assert np.array_equal(idx.cpu().numpy(), ids), f"replay indices of update {u}"
+        batch = lr.batch_from_store(s, ids)
+        _margin(c, st, batch, hp)
+        st0 = copy.deepcopy(st)
+        want = _update_oracle(c, st, batch, hp)
+        met = b.update_from_store(ts, idx).cpu()
+        _check_update(c, b, st, st0, batch, want, met, hp, f"update {u}")
+    got, ref = _state(a), _state(b)
+    for k in ref:
+        assert torch.equal(got[k], ref[k]), f"{k}: max abs difference {float((got[k].double() - ref[k].double()).abs().max()):.3e}"
+    assert a.updates == b.updates == K
+    a.close(); b.close()
+
+
+# ---- 4. λ = 0 is the one-step target; switching back restores it ---------------------------------------------------------------------------------
+@pytest.mark.parametrize("c", [Case(), Case(H=64), Case(kind="vdn", standardise=True), Case(kind="qmix", hl=1), Case(kind="qmix", standardise=True),
+                               Case(rnn=True, T=9, B=8)], ids=["idqn_tc", "idqn_fp32", "vdn_std", "qmix_h1", "qmix_h2_std", "rnn_idqn"])
+def test_lambda_zero_matches_the_one_step_target(c):
+    """the same update with td_lambda = 0 and td_lambda = null: loss and gradients within 1e-6 relative; then set_td_lambda(None) on the λ handle
+    makes its next update the one-step update again"""
+    a, b = _model(c, lam=0.0), _model(c, lam=None)
+    _perturb_target(a)
+    for k in ("theta", "theta_tgt") + (("mix", "mix_tgt") if c.kind == "qmix" else ()):
+        getattr(b, k).copy_(getattr(a, k))
+    b.params_changed()
+    idx = torch.arange(c.B, dtype=torch.int32, device=a.device)
+    for u in range(2):
+        if u == 1:
+            a.set_td_lambda(None)
+        ts = traj_store(_store(c, 5 + u), a.device)
+        ma, mb = a.update_from_store(ts, idx).cpu().clone(), b.update_from_store(ts, idx).cpu().clone()
+        assert abs(float(ma[0]) - float(mb[0])) <= 1e-6 * max(1.0, abs(float(mb[0]))), (u, float(ma[0]), float(mb[0]))
+        grads = [(a.grad, b.grad)] + ([(a.mix_grad, b.mix_grad)] if c.kind == "qmix" else [])
+        for ga, gb in grads:
+            ga, gb = ga.cpu().double(), gb.cpu().double()
+            assert float((ga - gb).abs().max()) <= 1e-6 * max(1.0, float(gb.abs().max())), (u, float((ga - gb).abs().max()))
+    assert a.td_lambda is None
+    a.close(); b.close()
+
+
+# ---- 5. the drivers -------------------------------------------------------------------------------------------------------------------------------
+# the reference's FileSystemLogger columns of a two-agent DQN-family run: environment_steps first, the rest sorted
+DRIVER_COLS = ["environment_steps", "agent0/mean_episode_returns", "agent0/std_episode_returns", "agent1/mean_episode_returns", "agent1/std_episode_returns",
+               "epsilon", "loss", "mean_episode_length", "mean_episode_returns", "mean_episode_time", "std_episode_length", "std_episode_returns",
+               "std_episode_time", "updates"]
+
+
+@pytest.mark.parametrize("alg,extra", [("idqn", []), ("vdn", ["algorithm.use_proper_termination=True"]), ("qmix", ["algorithm.model.mixing.hypernet_layers=1"])])
+def test_driver_with_td_lambda(tmp_path, monkeypatch, alg, extra):
+    """(QMIX with standardise_returns is left out here: its de-standardised target feeds the running variance back into the next returns and
+    diverges on untrained networks with either target, see tests/test_qmix_options_gpu.py; its updates are pinned against the oracle above.)"""
+    import pandas as pd
+
+    from codebase_b200 import run
+
+    monkeypatch.chdir(tmp_path)
+    run.main([f"+algorithm={alg}", "env.name=lbforaging:Foraging-8x8-2p-3f-v3", "env.time_limit=25", "env.parallel_envs=256", "seed=0",
+              "algorithm.total_steps=60000", "algorithm.eval_interval=20000", "algorithm.batch_size=128", "algorithm.buffer_size=4096",
+              "algorithm.updates_per_iteration=16", "algorithm.td_lambda=0.6", f"run_dir={tmp_path}/out"] + extra)
+    df = pd.read_csv(tmp_path / "out" / "results.csv")
+    assert list(df.columns) == DRIVER_COLS
+    assert len(df) >= 2 and df["updates"].iloc[-1] > 0 and np.isfinite(df["loss"][df["updates"] > 0]).all()
