@@ -28,7 +28,7 @@ __global__ void replay_sample_kernel(uint64_t seed, uint64_t update_idx, int bat
 // ---- TD error over C columns of G agents (marlbase/dqn/model.py:138-163, VDN 224-269) -----------------------------
 // Column c sums the Q-values and bootstrap values of agents [c G, c G + G) and takes agent c G's reward.  VDN: C = 1, G = N; independent learners
 // (the recurrent pass, whose backward has no TD head of its own; standardise_returns): C = N, G = 1.  One thread per (c, b, t).
-//   STAGE 0: td[c][b][t] = 2 delta filled and the loss statistics.
+//   STAGE 0: td[c][b][t] = dLoss/dQ filled (2 delta; Huber: clamp(delta, -huber, huber)) and the loss statistics.
 //   STAGE 1 (standardise_returns, dqn/model.py:147-158, VDN 256-264: the TD target needs statistics of the whole batch's returns before any loss):
 //            ret = r + gamma (next * sqrt(var) + mean) (1 - done[t + 1]) and chosen = Q(o_t)[a_t], for every (b, t), filled or not, as the
 //            reference.  Columns of the statistics: one per agent (IDQN); the reference's VDN reshapes its (E, B) returns with reshape(-1, B), i.e.
@@ -40,10 +40,11 @@ struct ColTdParams {
   const float* q; const float* tq;  // [N][B][T+1][A]
   TrajView traj; const int32_t* idx; int B, A; float gamma; int double_q;
   int C, G;
+  float huber;       // STAGES 0, 2: algorithm.huber_delta (> 0: the Huber TD loss; <= 0: the squared error)
   const float* ret_ms; int n_stat, stat_per_b;   // STAGE 1 (STAGE 3: or NULL): mean[n_stat] | var[n_stat]
   float* ret; float* chosen;                     // STAGES 1, 2, 3: [C][B][T]
   float* boot;       // STAGE 3: [C][B][T]
-  float* td;         // [C][B][T] = 2 * delta * filled
+  float* td;         // [C][B][T] = td_dloss(delta) * filled
   float* loss_part;  // [gridDim][4]
 };
 
@@ -67,7 +68,7 @@ __global__ void __launch_bounds__(256) col_td_kernel(ColTdParams p) {
     const int c = i / (p.B * T), rem = i - c * p.B * T, b = rem / T, t = rem - b * T;
     const size_t ep = (size_t)p.idx[b];
     if constexpr (STAGE == 2) {
-      p.td[i] = td_error(p.chosen[i], p.ret[i], (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill);
+      p.td[i] = td_error(p.chosen[i], p.ret[i], (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill, p.huber);
     } else {
       float chosen = 0.f, next = 0.f;
       for (int a = c * p.G; a < (c + 1) * p.G; ++a) {
@@ -78,7 +79,7 @@ __global__ void __launch_bounds__(256) col_td_kernel(ColTdParams p) {
       }
       const float rew = p.traj.rew[p.traj.step_at(ep, c * p.G, t)], done1 = (float)p.traj.done[p.traj.done_at(ep, t + 1)];
       if constexpr (STAGE == 0) {
-        p.td[i] = td_error(chosen, td_target(rew, p.gamma, next, done1), (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill);
+        p.td[i] = td_error(chosen, td_target(rew, p.gamma, next, done1), (float)p.traj.filled[p.traj.filled_at(ep, t)], c == 0, loss, fill, p.huber);
       } else if constexpr (STAGE == 1) {
         const int col = p.stat_per_b ? b : c;
         p.ret[i] = td_target_rn(rew, p.gamma, unstandardise(next, p.ret_ms[col], p.ret_ms[p.n_stat + col]), done1);
@@ -188,6 +189,8 @@ struct marl_dqn : LearnerHandle {
   float *ret = nullptr, *chosen = nullptr;
   // algorithm.td_lambda (marl_dqn_set_td_lambda): λ-returns in place of the one-step target; boot: the bootstrap values v_{t+1} per (column, b, t)
   bool td_lambda_on = false; float td_lambda = 0.f; float* boot = nullptr;
+  // algorithm.huber_delta (marl_dqn_set_huber_delta): the Huber TD loss's delta; 0: the reference's squared error
+  float huber = 0.f;
   // QMIX (hp.mixer == 2): the mixing network's parameters / Adam state / gradient (+ 4 statistics), per-sample records, chunked partial sums, tile list
   QmixLayout ql = {}; float *mix = nullptr, *mix_tgt = nullptr, *mix_m = nullptr, *mix_v = nullptr, *mix_grad = nullptr, *mix_rec = nullptr, *mix_part = nullptr, *mix_img = nullptr, *mix_img_tgt = nullptr;
   QmixTile* mix_tiles = nullptr; int mix_n_tiles = 0; QmixMicro* mix_micro = nullptr; int mix_n_micro = 0; bool mix_wgrad_tiles = false;
@@ -316,6 +319,16 @@ int marl_dqn_set_td_lambda(marl_dqn* h, int32_t enable, float lambda) {
   }
   h->td_lambda_on = enable != 0;
   h->td_lambda = enable ? lambda : 0.f;
+  return MARL_OK;
+}
+
+/* algorithm.huber_delta: enable != 0 replaces the squared TD error of every later update (marl_dqn_update*, update_n, the fused tail) by
+ * torch.nn.functional.huber_loss with delta = `delta` > 0 (DESIGN.md §4.4e); enable == 0 restores the squared error.  Every TD head takes delta
+ * as a run-time argument, so nothing is allocated and every path stays the one it was. */
+int marl_dqn_set_huber_delta(marl_dqn* h, int32_t enable, float delta) {
+  MARL_REQUIRE(!enable || (delta > 0.f && isfinite(delta)), "marl_dqn_set_huber_delta: delta %g must be a finite number > 0", (double)delta);
+  MARL_REQUIRE(h != nullptr, "marl_dqn_set_huber_delta: NULL handle");
+  h->huber = enable ? delta : 0.f;
   return MARL_OK;
 }
 
@@ -524,7 +537,7 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
   if (h->hp.mixer == 2) {  // QMIX: the mixer turns the agents' Q-values into the TD error and hands dL/dq_a back per agent (qmix.cuh)
     QmixParams qp; memset(&qp, 0, sizeof(qp));
     qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = src.idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
-    qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
+    qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.huber = h->huber; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
     qp.loss_part = loss_part;
     const int Sn = batch * T, qb = (Sn + kQmTS - 1) / kQmTS, n = h->ql.n, hl = h->ql.hl;
     qmix_pack_kernel<<<dim3((n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
@@ -565,7 +578,7 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
   const bool vdn = h->hp.mixer == 1;
   ColTdParams cp; memset(&cp, 0, sizeof(cp));
   cp.q = h->q_all; cp.tq = h->tq; cp.traj = src.traj; cp.idx = src.idx; cp.B = batch; cp.A = h->ns.out;
-  cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.C = vdn ? 1 : h->ns.n_agents; cp.G = vdn ? h->ns.n_agents : 1;
+  cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.huber = h->huber; cp.C = vdn ? 1 : h->ns.n_agents; cp.G = vdn ? h->ns.n_agents : 1;
   cp.td = h->td; cp.loss_part = loss_part;
   const int blocks = (cp.C * batch * T + 255) / 256;
   if (h->td_lambda_on) {   // bootstrap values + chosen Q, λ-return scan, [RunningMeanStd step], TD error on the (standardised) returns
@@ -673,7 +686,7 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   cudaEvent_t* ev = h->timing && h->ev_used < kTimingPairs ? &h->ev[4 * h->ev_used] : nullptr;
   TrainParams tp; memset(&tp, 0, sizeof(tp));
   tp.plan = plan; tp.src = src; tp.theta = h->theta; tp.lay = h->ns.lay; tp.tq = h->tq;
-  tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = h->loss_part;
+  tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.huber = h->huber; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = h->loss_part;
   int n_loss_parts = h->rnn ? 0 : plan.cta_begin[plan.n_nets];
   // The target network on every gathered row (dqn/model.py:132-134) runs inside the tensor-core training forward when that pipeline runs with the
   // tensor-core forward on (an FP32 target forward gives other bits).  Otherwise it is a forward of its own; several ranks with the split exchange:

@@ -139,6 +139,7 @@ struct TrainParams {
   const float* td_ext;    // precomputed 2*delta*filled (VDN: per (b, t), [B][T]; standardise_returns: per (agent, b, t) with td_agent_stride = B*T); NULL: the head computes it
   int td_agent_stride;
   float gamma; int double_q;
+  float huber;            // algorithm.huber_delta (> 0: the Huber TD loss of dqn_heads.cuh; <= 0: the squared error)
   // kHeadA2cCritic: parts = (0, sum filled on agent 0, 0, sum adv^2*filled); writes adv = returns - V
   const float* returns;   // [N][B][T] n-step returns
   float* adv_out;         // [N][B][T]

@@ -235,7 +235,7 @@ __device__ __forceinline__ void head_dqn(const TrainParams& p, const RowCtx& c, 
     g = p.td_ext[(size_t)c.agent * p.td_agent_stride + (size_t)c.b * c.T + c.tt];
   } else {
     const float* tq = p.tq + (row_index(c.agent, c.b, c.tt, c.B, c.T + 1) + 1) * c.A;   // the next row's target outputs
-    g = td_error(q[act], td_target(c.rew, p.gamma, next_value(qn, tq, c.A, p.double_q), c.done1), c.filled, c.agent == 0, st[0], st[1]);
+    g = td_error(q[act], td_target(c.rew, p.gamma, next_value(qn, tq, c.A, p.double_q), c.done1), c.filled, c.agent == 0, st[0], st[1], p.huber);
   }
 #pragma unroll
   for (int o = 0; o < kOutPad; ++o) dq[o] = (o == act) ? g : 0.f;

@@ -85,9 +85,10 @@ struct QmixParams {
   QmixLayout L;
   const float* q; const float* tq;   // [N][B][T+1][A] online / target Q-values of every gathered row
   TrajView traj; const int32_t* idx; int B, A, D; float gamma; int double_q;
+  float huber;        // algorithm.huber_delta (> 0: the Huber TD loss of dqn_heads.cuh; <= 0: the squared error)
   const float* mix; const float* mix_tgt;
   float* rec;         // [R][B*T]
-  float* td;          // [N][B][T] = dL/dq_a (un-normalised: x 2 delta filled)
+  float* td;          // [N][B][T] = dL/dq_a (un-normalised: x td_dloss(delta) filled)
   float* loss_part;   // [gridDim][4]
   // standardise_returns (two launches around ret_ms_step): the target pass writes ret[b][t], the online pass reads it back standardised
   const float* ret_ms; int n_stat;   // mean[n_stat] | var[n_stat], one column per batch entry (MODE 3: NULL without standardise_returns)
@@ -301,7 +302,7 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
     float ret;
     if constexpr (MODE == 2) ret = live ? p.ret[s] : 0.f;
     else ret = live ? td_target(p.traj.rew[p.traj.step_at(ep, 0, t)], p.gamma, ytgt, (float)p.traj.done[p.traj.done_at(ep, t + 1)]) : 0.f;
-    const float delta = live ? y - ret : 0.f, dy = 2.f * delta * filled;
+    const float delta = live ? y - ret : 0.f, dy = td_dloss(delta, p.huber) * filled;
     float* rc = p.rec + s;   // this sample's column of the field-major record
     if (live) {
       // the layers' inputs (x, h1, h2) -> record; rows are shared out over the warps
@@ -350,7 +351,7 @@ __global__ void __launch_bounds__(kQmWarps * 32, 2) qmix_mix_kernel(QmixParams p
     }
     // loss statistics of the tile (warp 0 holds every sample once)
     if (warp == 0) {
-      float loss = delta * delta * filled, fill = filled;
+      float loss = td_loss(delta, p.huber) * filled, fill = filled;
 #pragma unroll
       for (int off = 16; off > 0; off >>= 1) { loss += __shfl_xor_sync(0xFFFFFFFFu, loss, off); fill += __shfl_xor_sync(0xFFFFFFFFu, fill, off); }
       if (lane == 0) { p.loss_part[4 * blockIdx.x] = loss; p.loss_part[4 * blockIdx.x + 1] = fill; p.loss_part[4 * blockIdx.x + 2] = 0.f; p.loss_part[4 * blockIdx.x + 3] = 0.f; }

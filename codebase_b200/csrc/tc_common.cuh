@@ -306,7 +306,7 @@ struct TcTrainParams {
   // [rows][x_pitch] gathered observation rows, x_pitch = 8 ceil(D / 8) (zero beyond D): the dH1 kernel reads them for dW1 and the
   // weight-gradient kernel for H1, without chasing the episode index again
   float* xg; int x_pitch;
-  const float* tq; const float* td_ext; int td_agent_stride; float gamma; int double_q;
+  const float* tq; const float* td_ext; int td_agent_stride; float gamma; int double_q; float huber;
   float* scratch; int scratch_pitch; float* loss_part;
   // training forward only: the target network's images (NULL: the forward runs the online network alone) and where its outputs go (tq's
   // [rows][out] layout); q_out (NULL: none) receives the online outputs in the same layout, for an external TD head

@@ -259,7 +259,7 @@ __device__ __forceinline__ float td_grad(const TcTrainParams& p, size_t d, int a
   const float* q = p.rec + d * kRowRec;
   const float* qn = q + kRowRec;                 // the next row of the same episode
   const float* tq = p.tq + (d + 1) * A;          // target outputs share the [agent][unit][T + 1] row layout
-  return td_error(q[act], td_target(rew, p.gamma, next_value(qn, tq, A, p.double_q), done1), filled, agent == 0, s0, s1);
+  return td_error(q[act], td_target(rew, p.gamma, next_value(qn, tq, A, p.double_q), done1), filled, agent == 0, s0, s1, p.huber);
 }
 
 // One staging phase of the dW1 product: warpgroup `owner` stages its two chunks of a tile, c and c + 1 (its 64 rows of dH1 from the accumulator
@@ -620,7 +620,7 @@ static TcTrainParams tc_params(const TrainParams& tp, const TcBuffers& buf) {
   TcTrainParams p; memset(&p, 0, sizeof(p));
   p.plan = tp.plan; p.src = tp.src; p.lay = tp.lay; p.images = buf.image; p.bwd_images = buf.bwd_image;
   p.h2g = buf.h2; p.rec = buf.rec; p.xg = buf.x; p.x_pitch = 8 * ((tp.src.D + 7) / 8); p.rows = buf.rows;
-  p.tq = tp.tq; p.td_ext = tp.td_ext; p.td_agent_stride = tp.td_agent_stride; p.gamma = tp.gamma; p.double_q = tp.double_q;
+  p.tq = tp.tq; p.td_ext = tp.td_ext; p.td_agent_stride = tp.td_agent_stride; p.gamma = tp.gamma; p.double_q = tp.double_q; p.huber = tp.huber;
   p.scratch = tp.scratch; p.scratch_pitch = tp.scratch_pitch; p.loss_part = tp.loss_part;
   return p;
 }

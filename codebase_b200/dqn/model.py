@@ -9,6 +9,7 @@ owner of device buffers.  There is no CPU fallback.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import numbers
 import random
 import types
@@ -37,12 +38,27 @@ def td_lambda(cfg):
     return lam
 
 
+def huber_delta(cfg):
+    """cfg.huber_delta: None (absent or null: the reference's squared TD error) or the finite delta > 0 of the Huber TD loss that replaces it.
+    Anything else raises ValueError here, before any native call."""
+    delta = getattr(cfg, "huber_delta", None)
+    if delta is None:
+        return None
+    if isinstance(delta, bool) or not isinstance(delta, numbers.Real):
+        raise ValueError(f"algorithm.huber_delta must be null or a finite number > 0, not {delta!r}")
+    delta = float(delta)
+    if not (math.isfinite(delta) and delta > 0.0):
+        raise ValueError(f"algorithm.huber_delta must be a finite number > 0, not {delta}")
+    return delta
+
+
 class QNetwork(NativeLearner):
     mixer = 0
     _destroy = "marl_dqn_destroy"
 
     def __init__(self, obs_space, action_space, cfg, layers, parameter_sharing, use_rnn, use_orthogonal_init, device, max_batch=None, max_episode_length=None):
         self.td_lambda = td_lambda(cfg)
+        self.huber_delta = huber_delta(cfg)
         self.use_rnn = bool(use_rnn)
         self.hidden = hidden_width(layers, "layers", self.use_rnn)
         self._open(obs_space, action_space, cfg, device)
@@ -81,12 +97,22 @@ class QNetwork(NativeLearner):
             nat.check(self._lib.marl_dqn_standardise_returns(self._h, C.c_int32(1)), "marl_dqn_standardise_returns")
         if self.td_lambda is not None:
             self.set_td_lambda(self.td_lambda)
+        if self.huber_delta is not None:
+            self.set_huber_delta(self.huber_delta)
 
     def set_td_lambda(self, lam):
         """TD(λ) targets of `lam` in [0, 1] in place of the one-step target from the next update on (DESIGN.md §4.4d); None: the one-step target again"""
         lam = td_lambda(types.SimpleNamespace(td_lambda=lam))
         nat.check(self._lib.marl_dqn_set_td_lambda(self._h, C.c_int32(lam is not None), C.c_float(0.0 if lam is None else lam)), "marl_dqn_set_td_lambda")
         self.td_lambda = lam
+
+    def set_huber_delta(self, delta):
+        """The Huber TD loss with `delta` (a finite number > 0) in place of the squared TD error from the next update on (DESIGN.md §4.4e); None:
+        the squared error again"""
+        delta = huber_delta(types.SimpleNamespace(huber_delta=delta))
+        nat.check(self._lib.marl_dqn_set_huber_delta(self._h, C.c_int32(delta is not None), C.c_float(0.0 if delta is None else delta)),
+                  "marl_dqn_set_huber_delta")
+        self.huber_delta = delta
 
     def ret_ms(self):
         """(mean, var, count) of the RunningMeanStd over the TD targets (standardise_returns): one entry per agent; VDN, QMIX: per batch entry."""

@@ -307,6 +307,12 @@ int marl_dqn_ret_ms_ptrs(marl_dqn* q, float** ret_ms /* mean[n] | var[n] */, dou
  * with v the learner's bootstrap value (double-Q or max, VDN: summed over agents, QMIX: the target mixer's Q_tot) -- λ = 0 is the one-step target.
  * Under standardise_returns the statistics absorb G.  enable == 0 restores the one-step target.  λ outside [0, 1] is refused. */
 int marl_dqn_set_td_lambda(marl_dqn* q, int32_t enable, float lambda);
+/* algorithm.huber_delta of IDQN, VDN and QMIX (this project's option; the reference has only the squared TD error): enable != 0 makes every later
+ * update (marl_dqn_update, _update_grads, _update_n) use torch.nn.functional.huber_loss(Q, y, delta = `delta`) per TD error d = Q - y in place of
+ * mse_loss: 0.5 d² for |d| < delta, else delta (|d| - 0.5 delta), gradient clamp(d, -delta, delta).  The logged loss is the Huber mean.  For a
+ * large delta this is half the squared error and half its gradient.  enable == 0 restores the squared error.  A delta that is not a finite
+ * number > 0 is refused. */
+int marl_dqn_set_huber_delta(marl_dqn* q, int32_t enable, float delta);
 /* QMixNetwork (marlbase/dqn/model.py:272-443, configs/algorithm/qmix.yaml): with hp.mixer == 2, call once after marl_dqn_create.  The mixing
  * network works on state = the agents' observations concatenated (state_dim = n_agents * in_dim); its parameters are one flat vector in the
  * reference's state_dict order (weight, bias each): hypernet_layers == 2: hyper_w_1.0, hyper_w_1.2, hyper_w_final.0, hyper_w_final.2, hyper_b_1,
