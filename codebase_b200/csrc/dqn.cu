@@ -338,6 +338,12 @@ int marl_dqn_ret_ms_ptrs(marl_dqn* h, float** ret_ms, double** count, int32_t* n
   return MARL_OK;
 }
 
+int marl_dqn_scratch_ptrs(marl_dqn* h, float** boot, float** ret, float** chosen, float** td) {
+  MARL_REQUIRE(h != nullptr, "marl_dqn_scratch_ptrs: NULL handle");
+  if (boot) *boot = h->boot; if (ret) *ret = h->ret; if (chosen) *chosen = h->chosen; if (td) *td = h->td;
+  return MARL_OK;
+}
+
 /* QMixNetwork.__init__ (dqn/model.py:365-379): the mixing network over the concatenated observations (state_dim = N * in_dim).  Parameters are
  * initialised by the caller through marl_dqn_qmix_ptrs (nn.Linear defaults), then marl_dqn_sync_target copies them to the target mixer. */
 typedef void (*QmixMixFn)(QmixParams, const float*, const float*);

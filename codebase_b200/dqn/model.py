@@ -121,6 +121,14 @@ class QNetwork(NativeLearner):
         ms = nat.device_view(pm.value, 2 * n.value, self.device).cpu()
         return ms[: n.value], ms[n.value:], float(nat.device_view(pc.value, 1, self.device, "<f8").cpu()[0])
 
+    def scratch(self, B, T):
+        """(bootstrap values, TD targets, chosen Q, dLoss/dQ) of the last update's external TD head, each [C,B,T] (C = N for IDQN, 1 for VDN and
+        QMIX; QMIX's dLoss/dQ is per agent, [N,B,T]) or None where the handle has no such buffer -- device views for tests."""
+        ptrs = [C.c_void_p() for _ in range(4)]
+        nat.check(self._lib.marl_dqn_scratch_ptrs(self._h, *[C.byref(p) for p in ptrs]), "marl_dqn_scratch_ptrs")
+        cols = [1 if self.mixer else self.n_agents] * 3 + [1 if self.mixer == 1 else self.n_agents]
+        return tuple(None if p.value is None else nat.device_view(p.value, c * B * T, self.device).view(c, B, T) for p, c in zip(ptrs, cols))
+
     # ---- reference API ------------------------------------------------------------------------------------------
     def init_hiddens(self, batch_size):
         return self._hiddens(self.use_rnn, batch_size, self.hidden)

@@ -301,6 +301,10 @@ int marl_dqn_destroy(marl_dqn* q);
  * reshape), so their updates must use batch == max_batch. */
 int marl_dqn_standardise_returns(marl_dqn* q, int32_t enable);
 int marl_dqn_ret_ms_ptrs(marl_dqn* q, float** ret_ms /* mean[n] | var[n] */, double** count, int32_t* n_stat);
+/* device scratch of the last update's external TD head (parity tests), NULL where not allocated: bootstrap values v_{t+1} (td_lambda), TD targets
+ * (standardised under standardise_returns), chosen Q-values, each [C][B][T] with C = n_agents (IDQN) or 1 (VDN, QMIX; QMIX leaves chosen
+ * unwritten); and dLoss/dQ of the taken actions: IDQN, VDN [C][B][T], QMIX per agent [N][B][T] */
+int marl_dqn_scratch_ptrs(marl_dqn* q, float** boot, float** ret, float** chosen, float** td);
 /* algorithm.td_lambda of IDQN, VDN and QMIX (this project's option; the reference has only the one-step target): enable != 0 makes every later
  * update (marl_dqn_update, _update_grads, _update_n) use the TD(λ) target of `lambda` in [0, 1] over the sampled episode,
  *   G_t = r_t + γ (1 - d_{t+1}) ((1 - λ f_{t+1}) v_{t+1} + λ f_{t+1} G_{t+1}),  f_T = 0,

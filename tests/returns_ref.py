@@ -4,6 +4,9 @@
 - The per-row bar: every return is judged against its own no-cancellation scale S_t, not against the batch's largest |R|.
 - The cases of tests/test_returns_edges_gpu.py and their batches: dones and reward spikes placed on the split's boundaries.
 - A plain float32 recursion and mutations of it (tests/test_returns_edges.py shows the bar passes the one and fails the others).
+- The DQN family's TD(λ) scan (td_lambda_kernel, the same split): its bar and scale, the cases of tests/test_td_target_edges_gpu.py and their
+  batches (cuts, stale restarts, dones and spikes on the edges), ret_ms_step's choice of moment kernel, and the scan's float32 recursion and its
+  mutations (tests/test_td_target_edges.py).
 """
 from __future__ import annotations
 
@@ -301,3 +304,198 @@ class StatsRef:
     @property
     def count(self):
         return self.rms.count
+
+
+# ---- the DQN family's TD(λ) targets (td_lambda_kernel, col_td_kernel and ret_ms_step, csrc/dqn.cu) --------------------------------------------------
+# td_lambda_kernel splits each (column, episode) sequence as lambda_returns_kernel does: windows of LAM_WINDOW steps right to left, lanes of
+# LAM_CHUNK; it runs TDL_WARPS sequences per block.  col_td_kernel, which writes the bootstrap values and the TD error, and its block_loss_part run
+# one thread per (c, b, t) in blocks of COL_BLOCK.
+TDL_WARPS = 8                       # kTdlWarps
+COL_BLOCK = 256                     # col_td_kernel's block
+RET_COLS_N, RET_COLS_PT = 64, 1024  # ret_ms_step takes ret_moments_cols_kernel when N > 64 and P·T <= 1024
+
+
+def td_tau(T, gamma, lam):
+    """the TD(λ) target's bar: 16 float32 roundings of every term along the horizon min(T, 1/(1 - γλ)), never below 2e-5 -- twice tau's.  The
+    rounding of float32(γλ) compounds along the chain (about horizon / 2 roundings on the farthest terms, which a plain float32 recursion shows
+    at 20 u for a horizon of 17), and each step rounds b_t = r_t + (γ (1 - d_{t+1})) ((1 - λ f_{t+1}) v_{t+1}) four times."""
+    return 2 * tau(T, gamma, lam)
+
+
+def td_columns(kind, N):
+    """C of a DQN-family learner: IDQN one column per agent, VDN and QMIX one column of the team"""
+    return N if kind == "idqn" else 1
+
+
+def ret_ms_path(kind, N, B, T):
+    """the moment kernel ret_ms_step launches for a standardised update: VDN and QMIX keep one statistic per batch entry (N = B columns of P = 1
+    episode of T returns), IDQN one per agent (N columns of P = B episodes)"""
+    n, P = (B, 1) if kind != "idqn" else (N, B)
+    return "cols" if n > RET_COLS_N and P * T <= RET_COLS_PT else "grid"
+
+
+def td_lambda_scale(rew, done, filled, boot, lam, gamma):
+    """S_t = |r_t| + γ (1 - d_{t+1}) (|1 - λ f_{t+1}| |v_{t+1}| + λ f_{t+1} S_{t+1}), f_T = 0, float64: the TD(λ) target's terms without
+    cancellation, cut at the first unfilled row as the target is.  rew, filled, boot (T, ...) with boot[t] = v_{t+1}; done (T+1, ...)"""
+    r, v = np.abs(np.asarray(rew, np.float64)), np.abs(np.asarray(boot, np.float64))
+    d, f = np.asarray(done, np.float64), np.asarray(filled, np.float64)
+    T = r.shape[0]
+    out, nxt = np.zeros_like(r), np.zeros_like(r[0])
+    for t in reversed(range(T)):
+        f1 = f[t + 1] if t + 1 < T else 0.0
+        nxt = r[t] + gamma * (1.0 - d[t + 1]) * (np.abs(1.0 - lam * f1) * v[t] + lam * f1 * nxt)
+        out[t] = nxt
+    return out
+
+
+def td_rows(T):
+    """the rows that get an event: every window edge w0 - 1, w0, w0 + 1, each window's lane edge and its neighbours, and T - 1 (inside [1, T))"""
+    out = []
+    for w0 in edges(T):
+        out += [w0 - 1, w0, w0 + 1]
+    for w0, length in windows(T):
+        x = lane_edge(w0, length)
+        if x is not None:
+            out += [x - 1, x, x + 1]
+    out.append(T - 1)
+    return sorted({x for x in out if 1 <= x < T})
+
+
+TD_EVENTS = ("cut", "done", "stale")
+
+
+def td_episodes(T):
+    """the scripted episodes of a TD(λ) case, (kind, row): one filled to T without a done flag, one terminated at T, and per row x of td_rows(T)
+    - cut: filled up to x (x is the first unfilled row), no done flag: a truncated episode;
+    - done: terminated at x (done[x] = 1), unfilled from x;
+    - stale: filled up to x - 2, row x - 1 unfilled, filled again from x (a re-used slot's stale tail restarts at x), random done flags in it."""
+    return [("full", T), ("done", T)] + [(k, x) for x in td_rows(T) for k in TD_EVENTS]
+
+
+def td_batch(rng, T, N, B, A=6, D=D):
+    """a device-layout store of B episodes: the first len(td_episodes(T)) are scripted, the rest end at random steps; rewards as lambda_batch's
+    (sparse and dense, spikes on the window and lane edges); VDN and QMIX read agent 0's reward"""
+    obs = (rng.integers(-1, 8, size=(B, N, T + 1, D)) / 4.0).astype(np.float32)
+    act = rng.integers(0, A, size=(B, N, T)).astype(np.int32)
+    sparse = (rng.random((B, N, T)) < 0.2) * rng.random((B, N, T)) * 0.1
+    dense = rng.standard_normal((B, N, T)) * 0.1
+    parity = (np.arange(B)[:, None] + np.arange(N)[None, :]) % 2
+    rew = np.where(parity[:, :, None] == 0, sparse, dense)
+    sp = spikes_at(T)
+    rew[:, :, sp] += rng.uniform(5.0, 10.0, size=(B, N, len(sp)))
+    done = np.zeros((B, T + 1), np.uint8); filled = np.zeros((B, T), np.uint8)
+    eps = td_episodes(T)
+    for e in range(B):
+        kind, x = eps[e] if e < len(eps) else (("done", "cut")[e % 2], int(rng.integers(1, T + 1)))
+        if kind == "stale":
+            filled[e, : max(x - 1, 0)] = 1
+            filled[e, x:] = 1
+            done[e, x + 1:] = rng.random(T - x) < 0.2
+        else:
+            filled[e, :x] = 1
+            done[e, x] = kind == "done"
+    return dict(obs=obs, act=act, rew=rew.astype(np.float32), done=done, filled=filled)
+
+
+def td_sequences(s, C):
+    """(rew, done, filled) of a device-layout store in time-major float64, (T, C, B) and done (T+1, C, B): column c reads agent c's reward (C = 1:
+    agent 0's), every column of an episode its done and filled flags"""
+    rew = s["rew"][:, :C].astype(np.float64).transpose(2, 1, 0)
+    B, T = s["filled"].shape
+    done = np.broadcast_to(s["done"].astype(np.float64).T[:, None, :], (T + 1, C, B))
+    filled = np.broadcast_to(s["filled"].astype(np.float64).T[:, None, :], (T, C, B))
+    return rew, done, filled
+
+
+def td_case_B(T, C, cb8, cbt=None):
+    """the fewest episodes >= len(td_episodes(T)) with C·B ≡ cb8 (mod 8) and, when given, C·B·T ≡ cbt (mod COL_BLOCK)"""
+    B = len(td_episodes(T))
+    while (C * B) % 8 != cb8 or (cbt is not None and (C * B * T) % COL_BLOCK != cbt):
+        B += 1
+    return B
+
+
+# (T, kind, N, C·B mod 8 or None for C·B < 8, C·B·T mod 256 or None): every T mod 256 in {1, 7, 8, 9, 255, 0}, 1 to 5 windows
+TD_CASES = [(1, "idqn", 2, None, None), (7, "vdn", 2, 1, 255), (9, "qmix", 2, 7, None), (255, "idqn", 3, 0, None), (256, "qmix", 2, 1, 0),
+            (257, "vdn", 2, 7, 255), (263, "idqn", 3, 1, None), (264, "qmix", 3, 0, None), (265, "vdn", 2, 1, 1), (511, "qmix", 2, 7, None),
+            (512, "idqn", 3, 7, None), (769, "vdn", 2, 0, None), (1024, "qmix", 2, 1, None), (1025, "idqn", 3, 1, None)]
+
+
+def td_case(T, kind, N, cb8, cbt):
+    """(C, B) of a TD(λ) case; C·B < 8: three episodes of one row (T = 1 has no edge rows)"""
+    C = td_columns(kind, N)
+    return C, (3 if cb8 is None else td_case_B(T, C, cb8, cbt))
+
+
+def td_reaches(T, kind, N, B, standardise=False):
+    """the boundaries a TD(λ) case reaches, by the mirror of the split"""
+    C = td_columns(kind, N)
+    ws = windows(T)
+    got = {f"windows={len(ws)}", f"CB%8={(C * B) % 8}", f"T%256={T % LAM_WINDOW}"}
+    if C * B < 8:
+        got.add("CB<8")
+    if (C * B) % TDL_WARPS and C * B > TDL_WARPS:
+        got.add("partial last block")
+    if (C * B * T) % COL_BLOCK in (COL_BLOCK - 1, 0, 1):
+        got.add(f"CBT%256={(C * B * T) % COL_BLOCK}")
+    eps = td_episodes(T)[:B]
+    first_unfilled = {x for k, x in eps if k in ("cut", "done") and x < T} | {x - 1 for k, x in eps if k == "stale"}
+    restarts = {x for k, x in eps if k == "stale"}
+    dones = {x for k, x in eps if k == "done"}
+    for w0 in edges(T):
+        for name, rows in (("cut", first_unfilled), ("restart", restarts), ("done", dones)):
+            got |= {f"{name} at w0{k:+d}" if k else f"{name} at w0" for k in (-1, 0, 1) if w0 + k in rows}
+    for w0, length in ws:
+        x = lane_edge(w0, length)
+        if x is not None:
+            for name, rows in (("cut", first_unfilled), ("restart", restarts), ("done", dones)):
+                if x in rows:
+                    got.add(f"{name} at a lane edge")
+    if standardise:
+        got.add(f"ret_ms {ret_ms_path(kind, N, B, T)}")
+    return got
+
+
+def td_f32_recursion(rew, done, filled, boot, lam, gamma, next_of=None, f_from_t=False, ignore_cut_at=()):
+    """td_lambda_kernel's arithmetic done sequentially in float32: a_t = float32(γλ) (1 - d_{t+1}) f_{t+1}, b_t = r_t + (γ (1 - d_{t+1})) ((1 - λ
+    f_{t+1}) v_{t+1}), G_t = b_t + a_t G_{t+1}.  Mutations: next_of {t: callable(G) -> the value used as G_{t+1}}; f_from_t: f_{t+1} read as f_t;
+    ignore_cut_at: steps t whose f_{t+1} is taken as 1"""
+    g, l_ = np.float32(gamma), np.float32(lam)
+    gl = np.float32(float(g) * float(l_))
+    r, v = np.asarray(rew, np.float32), np.asarray(boot, np.float32)
+    d, f = np.asarray(done, np.float32), np.asarray(filled, np.float32)
+    T = r.shape[0]
+    G = np.zeros((T + 1,) + r.shape[1:], np.float32)
+    one = np.float32(1.0)
+    for t in reversed(range(T)):
+        live = one - d[t + 1]
+        f1 = (f[t] if f_from_t else f[t + 1]) if t + 1 < T else np.zeros_like(r[0])
+        if t in ignore_cut_at:
+            f1 = np.ones_like(f1)
+        a = gl * live * f1
+        b = r[t] + (g * live) * ((one - l_ * f1) * v[t])
+        nxt = next_of[t](G) if next_of and t in next_of else G[t + 1]
+        G[t] = b + a * nxt
+    return G[:T]
+
+
+def td_mutations(T, cut_rows):
+    """{name: td_f32_recursion keyword arguments} of td_lambda_kernel's plausible defects that apply at T (cut_rows: the first unfilled rows present)"""
+    out = {"f_{t+1} read as f_t": dict(f_from_t=True)} if cut_rows else {}
+    es = edges(T)
+    if es:
+        E = es[-1]
+        out["carry between windows dropped"] = dict(next_of={w0 - 1: lambda G: np.zeros_like(G[0]) for w0 in es})
+        out["window edge shifted by one"] = dict(next_of={E - 1: lambda G, x=min(E + 1, T): G[x]})
+        hit = [w0 - 1 for w0 in es if w0 in cut_rows]
+        if hit:
+            out["cut ignored on a window's last step"] = dict(ignore_cut_at=hit)
+    wrong = {}
+    for w0, length in windows(T):   # every lane but the last two takes G after the lane two to its right; lanes 30 and 31 the carry
+        for lane in range(32):
+            lo, hi = lane * LAM_CHUNK, min(lane * LAM_CHUNK + LAM_CHUNK, length)
+            if lo < hi and hi < length:
+                wrong[w0 + hi - 1] = lambda G, x=w0 + min((lane + 2) * LAM_CHUNK, length) if lane < 30 else w0 + length: G[x]
+    if wrong:
+        out["a lane's incoming G from two lanes over"] = dict(next_of=wrong)
+    return out

@@ -148,6 +148,9 @@ CHAIN = {
     "h1_std_n2_d15_polyak": Case(hl=1, N=2, D=15, E=64, T=25, B=17, standardise=True, tu=0.05),
     "h2_std_n3_d9_shared": Case(hl=2, N=3, D=9, E=64, T=6, B=19, sharing=True, standardise=True),
     "h1_std_n4_d27_single_q": Case(hl=1, N=4, D=27, E=64, T=6, B=11, double_q=False, standardise=True, tu=3.0),
+    # above 64 batch entries: ret_moments_cols_kernel takes the moments of the 128 statistics columns, for either mixer
+    "h1_std_b128_single_q": Case(hl=1, N=2, D=9, E=64, T=10, B=128, double_q=False, standardise=True, tu=3.0),
+    "h2_std_b128_single_q": Case(hl=2, N=2, D=9, E=64, T=10, B=128, double_q=False, standardise=True, tu=3.0),
 }
 
 
@@ -324,7 +327,10 @@ def test_driver_one_layer_standardised_and_eval(tmp_path, monkeypatch):
     """The driver trains with both options and its checkpoint plays in codebase_b200.eval.  The loss value is not asserted: the reference's
     de-standardised target (Q' sqrt(var) + mean) feeds the running variance back into the next returns, and on untrained networks that loop grows
     the statistics geometrically (tests/qmix_options_ref.py reaches an infinite variance after ~20 updates of random episodes; this run's loss was NaN
-    after 8 updates).  The arithmetic of each update is pinned against the oracle and the reference above."""
+    after 8 updates).  The arithmetic of each update is pinned against the oracle and the reference above.  This run's batch of 128 takes
+    ret_moments_cols_kernel for the statistics' moments; that kernel is not the cause: tests/test_td_target_edges_gpu.py holds its running
+    statistics and standardised returns to float64 at 65 and 128 batch entries, and the B = 128 cases of CHAIN hold whole standardised updates to
+    the oracle."""
     import os
 
     from codebase_b200 import eval as ev

@@ -1,8 +1,10 @@
 """GPU: TD(λ) targets of IDQN, VDN and QMIX (algorithm.td_lambda; col_td_kernel's bootstrap stage, qmix_mix_kernel's MODE 3 and td_lambda_kernel in
 csrc/dqn.cu / csrc/qmix.cuh) against the float64 oracle (tests/td_lambda_ref.py): loss, gradients and parameters after each update of unglued chains
 on ragged episodes -- the tensor-core and the FP32 training pass, GRU agents, both QMIX mixers, double-Q on and off, standardise_returns, truncated
-episodes, parameter sharing, stale tails -- at λ in {0, 0.6, 1} and T at every window edge of the scan up to 513; the update_n chain against its
-loop and the oracle; λ = 0 against the one-step target; and the training drivers end to end."""
+episodes, parameter sharing, stale tails -- at λ in {0, 0.6, 1} and T in {1, 2, 255, 256, 257, 264, 500, 513, 769} (264 and 769 standardised at 65
+and 72 batch entries); the update_n chain against its loop and the oracle; λ = 0 against the one-step target; and the training drivers end to end.
+These are whole updates against the oracle with an aggregate bar; tests/test_td_target_edges_gpu.py holds every target per row at the scan's
+window and lane boundaries."""
 import copy
 import ctypes as C
 import dataclasses
@@ -196,14 +198,18 @@ def test_unglued_chain_matches_oracle(name):
     _run_chain(CHAIN[name])
 
 
-# ---- 2. episode lengths at the scan's window edges (windows of 256 steps) ------------------------------------------------------------------------
-EDGES = [(1, "idqn"), (2, "vdn"), (255, "idqn"), (256, "qmix"), (257, "vdn"), (500, "qmix"), (513, "idqn")]
+# ---- 2. episode lengths around the scan's window edges (windows of 256 steps) ---------------------------------------------------------------------
+EDGES = [(1, "idqn"), (2, "vdn"), (255, "idqn"), (256, "qmix"), (257, "vdn"), (500, "qmix"), (513, "idqn"), (264, "vdn"), (769, "qmix")]
+# standardised at more than 64 batch entries (ret_moments_cols_kernel below 1025 returns per entry): T = 264 ends its last window at a lane edge
+WIDE = {264: 65, 769: 72}
 
 
 @pytest.mark.parametrize("T,kind", EDGES)
 @redraw_on_near_tie
 def test_episode_lengths_at_window_edges(T, kind):
-    _run_chain(Case(kind=kind, T=T, B=4, N=2, D=7, lam=0.6 if T % 2 else 1.0, tails="stale" if T > 2 else "ragged"), n_updates=2)
+    B = WIDE.get(T, 4)
+    _run_chain(Case(kind=kind, T=T, B=B, N=2, D=7, lam=0.6 if T % 2 else 1.0, tails="stale" if T > 2 else "ragged", standardise=T in WIDE,
+                    double_q=T not in WIDE), n_updates=2)
 
 
 # ---- 3. update_n: the loop it replaces, bit for bit, and the oracle ------------------------------------------------------------------------------

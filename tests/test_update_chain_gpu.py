@@ -59,6 +59,8 @@ CASES = {
     "idqn4_two_kernel_tail": Case(N=4, B=48, T=12),
     # running return statistics carried across fused updates (VDN keeps one per batch entry: batch = max_batch)
     "vdn2_standardise_returns": Case(mixer=1, B=48, standardise=True),
+    # the same above 64 batch entries: one statistics column per entry of 25 returns, whose moments ret_moments_cols_kernel takes
+    "vdn2_standardise_returns_b128": Case(mixer=1, B=128, standardise=True),
     # the mixer's gradient and Adam step next to the fused tail; hard syncs of the target mixer (single-Q: a double-Q chain of this length tied in
     # 3 of 5 initialisations; tests/test_qmix.py compares the mixer's double-Q target with the oracle)
     "qmix2": Case(mixer=2, B=32, K=8, T=10),
