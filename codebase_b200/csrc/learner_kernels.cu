@@ -783,13 +783,9 @@ static StepFn step_fn(int opt) {
   return fns[opt];
 }
 
-// Fused tail; returns MARL_EINVAL without launching when no co-resident grid covers the parameters (the caller then uses the two
-// kernels).  The hand-made grid barrier needs every block resident at once, so the block shape follows from the device: capacity =
-// SMs x (blocks of 1024 threads per SM, from the occupancy API of the instantiation that will run: 1 at these kernels' register counts),
-// pb = parameters per block = ceil(n / capacity) rounded up to a warp multiple, ns = slices = 1024 / pb.
-// xp: NULL or world == 1 -> single GPU; else the exchange over peer memory (xp->epoch is advanced here).
-int reduce_adam_shape(int n, int n_sm, bool xchg, int opt, int* pb_out, int* ns_out) {
-  MARL_REQUIRE(opt >= 0 && opt < kNumOpt, "reduce_adam_shape: optimizer kind %d unknown", opt);
+// blocks of the fused tail per SM (-1: none fit), from the occupancy API, cached per (xchg, opt)
+static int tail_occupancy(bool xchg, int opt, int* oc_out) {
+  MARL_REQUIRE(opt >= 0 && opt < kNumOpt, "tail_occupancy: optimizer kind %d unknown", opt);
   static int occ[2][kNumOpt] = {};
   int& oc = occ[xchg][opt];
   if (oc == 0) {
@@ -805,6 +801,18 @@ int reduce_adam_shape(int n, int n_sm, bool xchg, int opt, int* pb_out, int* ns_
     }
     oc = o > 0 ? o : -1;
   }
+  *oc_out = oc;
+  return MARL_OK;
+}
+
+// Fused tail; returns MARL_EINVAL without launching when no co-resident grid covers the parameters (the caller then uses the two
+// kernels).  The hand-made grid barrier needs every block resident at once, so the block shape follows from the device: capacity =
+// SMs x (blocks of 1024 threads per SM, from the occupancy API of the instantiation that will run: 1 at these kernels' register counts),
+// pb = parameters per block = ceil(n / capacity) rounded up to a warp multiple, ns = slices = 1024 / pb.
+// xp: NULL or world == 1 -> single GPU; else the exchange over peer memory (xp->epoch is advanced here).
+int reduce_adam_shape(int n, int n_sm, bool xchg, int opt, int* pb_out, int* ns_out) {
+  int oc = 0;
+  if (int rc = tail_occupancy(xchg, opt, &oc)) return rc;
   if (oc < 1) return MARL_EINVAL;
   const int capacity = n_sm * oc;
   const int pb = ((n + capacity - 1) / capacity + 31) / 32 * 32;
@@ -869,3 +877,78 @@ int launch_adam(const AdamParams& p, int opt, cudaStream_t st) {
 }
 
 }  // namespace marl
+
+// ---- test hooks: the update tail alone, through the launchers above -----------------------------------------------------------------------
+using namespace marl;
+extern "C" {
+int marl_debug_tail_shape(int32_t n, int32_t opt_kind, int32_t device, int32_t* pb, int32_t* ns, int32_t* capacity) {
+  MARL_REQUIRE(pb != nullptr && ns != nullptr && capacity != nullptr, "marl_debug_tail_shape: NULL output");
+  MARL_REQUIRE(n >= 1, "marl_debug_tail_shape: n = %d must be positive", (int)n);
+  MARL_REQUIRE(opt_kind >= 0 && opt_kind < kNumOpt, "marl_debug_tail_shape: optimizer kind %d unknown", (int)opt_kind);
+  if (int rc = check_device(device)) return rc;
+  int n_sm = 0, oc = 0;
+  MARL_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
+  if (int rc = tail_occupancy(false, opt_kind, &oc)) return rc;
+  *capacity = n_sm * (oc > 0 ? oc : 0);
+  int b = 0, s = 0;
+  if (reduce_adam_shape(n, n_sm, false, opt_kind, &b, &s) != MARL_OK) {
+    set_error("marl_debug_tail_shape: no fused block shape covers %d parameters with capacity %d: the two-kernel tail", (int)n, (int)*capacity);
+    return MARL_EINVAL;
+  }
+  *pb = b; *ns = s;
+  return MARL_OK;
+}
+
+int marl_debug_tail_run(const marl_debug_tail* t, const marl_optimizer* opt, int32_t path, int32_t device, void* stream) {
+  MARL_REQUIRE(t != nullptr, "marl_debug_tail_run: NULL arguments");
+  if (int rc = check_optimizer(opt, "marl_debug_tail_run")) return rc;
+  MARL_REQUIRE(path >= 0 && path <= 2, "marl_debug_tail_run: path %d unknown (0 fused, 1 two kernels with sums of squares, 2 without)", (int)path);
+  MARL_REQUIRE(t->n_nets >= 1 && t->n_nets <= MARL_MAX_AGENTS, "marl_debug_tail_run: n_nets %d out of range (1..%d)", (int)t->n_nets, MARL_MAX_AGENTS);
+  MARL_REQUIRE(t->P >= 1 && (int64_t)t->n_nets * t->P <= (1 << 28), "marl_debug_tail_run: P = %d out of range", (int)t->P);
+  MARL_REQUIRE(t->scratch_pitch >= t->P, "marl_debug_tail_run: scratch_pitch %d below P = %d", (int)t->scratch_pitch, (int)t->P);
+  MARL_REQUIRE(t->cta_begin[0] >= 0, "marl_debug_tail_run: cta_begin[0] = %d is negative", (int)t->cta_begin[0]);
+  for (int k = 0; k < t->n_nets; ++k)
+    MARL_REQUIRE(t->cta_begin[k + 1] >= t->cta_begin[k], "marl_debug_tail_run: cta_begin decreases at network %d", k);
+  MARL_REQUIRE(t->n_loss_parts >= 0 && (t->n_loss_parts == 0 || t->loss_part != nullptr), "marl_debug_tail_run: n_loss_parts %d / loss_part", (int)t->n_loss_parts);
+  MARL_REQUIRE(t->stats_accumulate == 0 || t->stats_accumulate == 1, "marl_debug_tail_run: stats_accumulate must be 0 or 1");
+  const int n = t->n_nets * t->P;
+  MARL_REQUIRE(t->target_mode >= 0 && t->target_mode <= 2, "marl_debug_tail_run: target_mode %d unknown (0 none, 1 hard, 2 Polyak)", (int)t->target_mode);
+  MARL_REQUIRE(t->tgt_begin >= 0 && t->tgt_n >= 0 && t->tgt_begin + t->tgt_n <= n, "marl_debug_tail_run: target slice [%d, %d) outside [0, %d)", (int)t->tgt_begin,
+               (int)(t->tgt_begin + t->tgt_n), n);
+  MARL_REQUIRE(t->target_mode == 0 || t->theta_tgt != nullptr, "marl_debug_tail_run: NULL theta_tgt");
+  MARL_REQUIRE(t->step >= 1, "marl_debug_tail_run: step %lld must be >= 1", (long long)t->step);
+  MARL_REQUIRE(t->scratch != nullptr && t->grad != nullptr && t->sumsq != nullptr && t->theta != nullptr && t->m != nullptr && t->v != nullptr,
+               "marl_debug_tail_run: NULL buffer");
+  MARL_REQUIRE(((uintptr_t)t->grad & 15) == 0, "marl_debug_tail_run: grad must be 16-byte aligned (adam_kernel reads it as float4)");
+  if (int rc = check_device(device)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  ReduceParams rp; memset(&rp, 0, sizeof(rp));
+  rp.scratch = t->scratch; rp.loss_part = t->loss_part; rp.n_nets = t->n_nets; rp.P = t->P; rp.scratch_pitch = t->scratch_pitch;
+  memcpy(rp.cta_begin, t->cta_begin, sizeof(rp.cta_begin));
+  rp.n_loss_parts = t->n_loss_parts; rp.grad = t->grad; rp.stats = t->grad + n; rp.stats_accumulate = t->stats_accumulate;
+  rp.sumsq_part = path == 2 ? nullptr : t->sumsq;
+  AdamParams ap; memset(&ap, 0, sizeof(ap));
+  ap.theta = t->theta; ap.theta_tgt = t->theta_tgt; ap.m = t->m; ap.v = t->v; ap.grad = t->grad; ap.n = n;
+  ap.tgt_begin = t->tgt_begin; ap.tgt_n = t->tgt_n; ap.target_mode = t->target_mode; ap.tau = t->tau;
+  ap.grad_clip = t->grad_clip; ap.loss_out = t->loss_out;
+  set_step_consts(ap, *opt, t->lr, t->step);
+  if (path != 0) {
+    if (path == 1) { ap.sumsq_part = t->sumsq; ap.n_sumsq = (n + 63) / 64; }
+    if (int rc = launch_grad_reduce(rp, st)) return rc;
+    return launch_adam(ap, opt->kind, st);
+  }
+  int n_sm = 0, pb = 0, ns = 0;
+  MARL_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
+  MARL_REQUIRE(reduce_adam_shape(n, n_sm, false, opt->kind, &pb, &ns) == MARL_OK,
+               "marl_debug_tail_run: the fused tail has no co-resident block shape for %d parameters on %d SMs", n, n_sm);
+  // a fresh barrier counter: the state a handle's first update sees
+  unsigned long long* barrier = nullptr;
+  unsigned long long epoch = 0;
+  MARL_CUDA_TRY(cudaMallocAsync((void**)&barrier, 2 * sizeof(unsigned long long), st));
+  MARL_CUDA_TRY(cudaMemsetAsync(barrier, 0, 2 * sizeof(unsigned long long), st));
+  SampleParams sp; memset(&sp, 0, sizeof(sp));
+  const int rc = launch_reduce_adam(rp, ap, opt->kind, nullptr, sp, barrier, &epoch, n_sm, st);
+  MARL_CUDA_TRY(cudaFreeAsync(barrier, st));
+  return rc;
+}
+}  // extern "C"

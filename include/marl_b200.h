@@ -333,6 +333,27 @@ int marl_debug_qmix_coverage(int32_t n_agents, int32_t state_dim, int32_t embed_
 /* The same self-check for either hypernetwork form (hypernet_layers 1 or 2; anything else is refused).  marl_debug_qmix_coverage is this with 2. */
 int marl_debug_qmix_coverage_layers(int32_t n_agents, int32_t state_dim, int32_t embed_dim, int32_t hypernet_layers, int32_t hypernet_embed,
                                     int32_t* counts, int64_t cap, int64_t* n_params);
+/* The tail every learner's update ends in (tests/test_optimizer_tail_gpu.py): the reduction of the per-CTA gradient partials, the clip, the optimiser
+ * step and the target update, alone, through the launchers the learners use.
+ * marl_debug_tail_shape: the fused tail's block shape for n parameters on `device` -- MARL_OK and pb (parameters per block), ns (CTA slices),
+ * capacity (SMs x blocks per SM); MARL_EINVAL (capacity still written) when the learners would take the two-kernel tail. */
+int marl_debug_tail_shape(int32_t n, int32_t opt_kind, int32_t device, int32_t* pb, int32_t* ns, int32_t* capacity);
+typedef struct {
+  int32_t n_nets, P, scratch_pitch, cta_begin[MARL_MAX_AGENTS + 1];   /* CTAs [cta_begin[k], cta_begin[k+1]) hold network k's partials */
+  const float* scratch;   /* device [cta_begin[n_nets]][scratch_pitch] per-CTA partial gradient sums */
+  const float* loss_part; /* device [n_loss_parts][4] per-CTA loss statistics */
+  int32_t n_loss_parts, stats_accumulate;   /* stats_accumulate: add the statistics to grad[n .. n+4) instead of overwriting them */
+  float* grad;            /* device [n_nets*P + 4], 16-byte aligned: the reduced gradient and the 4 statistics */
+  float* sumsq;           /* device [ceil(n_nets*P / 64) + 1] per-block sums of squares */
+  float *theta, *theta_tgt, *m, *v;   /* device [n_nets*P]; theta_tgt[0 .. tgt_n) mirrors theta[tgt_begin ..) */
+  int32_t tgt_begin, tgt_n, target_mode; float tau;   /* target_mode 0 none, 1 hard copy, 2 Polyak with tau */
+  float lr, grad_clip; int64_t step;   /* grad_clip <= 0: off; step = 1, 2, ... (bias corrections) */
+  float* loss_out;        /* device [6] as marl_dqn_update's, or NULL */
+} marl_debug_tail;
+/* path 0: reduce_adam_kernel<0> with a fresh barrier counter (MARL_EINVAL without launching when no co-resident shape exists);
+ *      1: grad_reduce_kernel + adam_kernel with the per-block sums of squares (the DQN family's fallback);
+ *      2: the same without them (actor-critic learners, marl_dqn_update_apply, the QMIX mixer's step) */
+int marl_debug_tail_run(const marl_debug_tail* t, const marl_optimizer* opt, int32_t path, int32_t device, void* stream);
 int marl_dqn_qmix_ptrs(marl_dqn* q, float** mix, float** mix_tgt, float** adam_m, float** adam_v, float** grad, int64_t* n_params);
 int marl_dqn_param_ptrs(marl_dqn* q, float** theta, float** theta_tgt, float** adam_m, float** adam_v, float** grad,
                         int64_t* n_params);
