@@ -619,9 +619,11 @@ static bool dqn_tc_train(const marl_dqn* h) { return !h->rnn && tc_backward_enab
 
 // The tensor-core pipeline's buffers (allocated on first use) and current online images
 static int dqn_tc_prepare(marl_dqn* h, TcBuffers& tb, cudaStream_t st) {
+  // H2 slabs of every row split of up to `rows` rows over at most n_sm CTAs (the per-CTA gradient scratch has n_sm rows): tc_train.cu, h2_slab
+  const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), h2_tiles = (rows + 63) / 64 + (size_t)h->n_sm;
   if (!h->tc_h2) {  // intermediates of the tensor-core pipeline, allocated on first use (observation rows at pitch 8 ceil(in / 8))
-    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), F = sizeof(float);
-    if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h2, rows * kHidden * F},
+    const size_t F = sizeof(float);
+    if (int rc = alloc_buffers(h, "marl_dqn_update", {{&h->tc_h2, h2_tiles * 64 * kHidden * F},
                                                       {&h->tc_rec, rows * 32 /* kRowRec */ * F}, {&h->tc_x, rows * ((h->ns.in + 7) / 8 * 8) * F},
                                                       {&h->image_bwd, ((size_t)h->ns.n_nets * tc_bwd_image_bytes() / 4 + 4) * F}}))
       return rc;
@@ -630,7 +632,7 @@ static int dqn_tc_prepare(marl_dqn* h, TcBuffers& tb, cudaStream_t st) {
     if (int rc = launch_pack_weights(h->theta, h->ns.lay, h->ns.n_nets, h->image, st, h->image_bwd)) return rc;
     h->image_current = h->bwd_image_current = true;
   }
-  tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h2 = h->tc_h2; tb.rec = h->tc_rec; tb.x = h->tc_x; tb.rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1);
+  tb.image = h->image; tb.bwd_image = h->image_bwd; tb.h2 = h->tc_h2; tb.h2_tiles = h2_tiles; tb.rec = h->tc_rec; tb.x = h->tc_x;
   return MARL_OK;
 }
 

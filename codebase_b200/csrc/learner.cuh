@@ -310,10 +310,10 @@ int launch_tc_forward(const FwdParams& p, const uint8_t* images, cudaStream_t st
 // ---- tensor-core training pipeline (tc_train.cu) ----------------------------------------------------------------------------
 struct TcBuffers {
   uint8_t* image; uint8_t* bwd_image;       // packed online-network images (forward K-major, backward K-major W2^T)
-  float* h2;                                // [128][rows] (feature-major) H2 activations
+  float* h2;                                // H2 activations in fragment order: [h2_tiles][16][128] float4, a slab of 64-row tiles per CTA
+  size_t h2_tiles;                          // allocated 64-row tiles of h2 (ceil(rows / 64) + grid hold any row split: tc_train.cu, h2_slab)
   float* rec;                               // [rows][kRowRec] row records (tc_train.cu)
   float* x;                                 // [rows][8 ceil(in / 8)] gathered observation rows
-  size_t rows;                              // allocated rows
 };
 int tc_train_init();
 // the training forward (tc_dqn_fwd_kernel): the online network, and with tgt_images the target network on the same rows into tq_out; q_out (optional):

@@ -299,9 +299,9 @@ struct TcTrainParams {
   RowPlan plan; RowSource src; NetLayout lay;
   const uint8_t* images;      // forward images [n_nets][kImageBytes]
   const uint8_t* bwd_images;  // backward images [n_nets][kBwdImageBytes]
-  // H2: feature-major [128][rows] (the weight-gradient kernel stages 32 consecutive rows of one feature per warp instruction); H1 is not stored:
-  // the weight-gradient kernel rebuilds it from xg (layer1_tile)
-  float* h2g; size_t rows;
+  // H2 in the forward's accumulator-fragment order, one slab of 64-row tiles per CTA (tc_train.cu: h2_slab); H1 is not stored: the
+  // weight-gradient kernel rebuilds it from xg (layer1_tile)
+  float4* h2s;
   float* rec;                 // [rows][kRowRec] row records
   // [rows][x_pitch] gathered observation rows, x_pitch = 8 ceil(D / 8) (zero beyond D): the dH1 kernel reads them for dW1 and the
   // weight-gradient kernel for H1, without chasing the episode index again

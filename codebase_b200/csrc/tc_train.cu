@@ -2,8 +2,9 @@
 //
 // Same arithmetic as train_kernel<KP, kHeadDqn> (QNetwork._compute_loss + backward, marlbase/dqn/model.py:118-168), split where a
 // weight gradient needs the rows of many tiles as its K dimension (tf32 wgmma reads both shared-memory operands K-major only):
-//   tc_dqn_fwd_kernel   online forward (A operand in registers, weights = K-major image), head on the CUDA cores; stores H2 (FP32,
-//                        feature-major), the gathered observation row, the row's outputs and the ReLU masks of H1 / H2 (row record);
+//   tc_dqn_fwd_kernel   online forward (A operand in registers, weights = K-major image), head on the CUDA cores; stores H2 (FP32, in
+//                        accumulator-fragment order: h2_slab), the gathered observation row, the row's outputs and the ReLU masks of H1 / H2
+//                        (row record);
 //                        then, on the same rows, the target network's forward (the TD target's bootstrap values)
 //   tc_dh1_kernel       TD head (needs the next row's outputs, hence after the forward) -> dLoss/dq[act] and the loss statistics;
 //                        dH1 = (dH2 x W2) * relu'(H1) with dH2[r][j] = g_r W3[act_r][j] relu'(H2[r][j]) built in registers (the TD loss touches
@@ -57,15 +58,16 @@ __device__ __forceinline__ void store_frag_masks(const float (&v)[64], long long
   if (d0 >= 0) rec[(size_t)d0 * kRowRec + mask + quad_lane] = __uint_as_float(m0);
   if (d1 >= 0) rec[(size_t)d1 * kRowRec + mask + quad_lane] = __uint_as_float(m1);
 }
-// store a 64 x 128 fragment feature-major (dst[j * rows + row]) and its ReLU mask words
-__device__ __forceinline__ void store_frag_fm(float* dst, size_t rows, const float (&v)[64], long long d0, long long d1, int quad_lane, float* rec, int mask) {
-#pragma unroll
-  for (int i = 0; i < 64; ++i) {
-    const long long d = (i & 2) ? d1 : d0;
-    if (d >= 0) dst[(size_t)frag_col(i, quad_lane) * rows + (size_t)d] = v[i];
-  }
-  store_frag_masks(v, d0, d1, quad_lane, rec, mask);
+// H2 in the forward's accumulator-fragment order.  CTA b owns a slab of 64-row tiles starting at tile h2_slab(b); its tile k (rows
+// row_begin + 64 k, + 64) holds element group n (0..15: elements 4 n .. 4 n + 3, i.e. columns 8 n + 2 q, + 1 of rows 16 w + g and + 8) of thread
+// u (0..127) of the warpgroup that ran it as the float4 ((h2_slab(b) + k) * 16 + n) * 128 + u.  A warp's store is then 512 contiguous bytes, and
+// the weight-gradient kernel's chunk c (tile c / 2, threads [64 (c % 2), + 64)) is 16 KB in one piece.  The slab starts at the CTA's first row
+// over all networks, in tiles, plus its index: every CTA of n rows has at least ceil(n / 64) tiles before the next CTA's slab, whatever the
+// plan, so ceil(rows / 64) + grid tiles hold any split of `rows` rows (TcBuffers::h2_tiles).  Rows past row_end are written, never staged.
+__device__ __forceinline__ size_t h2_slab(const RowPlan& p, int net, int row_begin) {
+  return (size_t)(((long long)p.slot_begin[net] * p.units_per_agent * p.unit_rows + row_begin) / kWgRows) + blockIdx.x;
 }
+constexpr int kH2TileF4 = 16 * 128;   // float4 per 64-row tile
 
 // Shared memory of the training forward: the online image at 0, then the target network's W1 hi | lo (1024-byte aligned, as the swizzled panels
 // need) and its b1 | b2 | b3 | FP32 W3, then the mbarriers.  The target's W2 has no room of its own: it is loaded over the online W2 once every
@@ -129,7 +131,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
     }
   };
   bool first = true;
-  for (int vr0 = row_begin + kWgRows * wg; vr0 < row_end; vr0 += kTileRows) {
+  float4* const h2s = p.h2s + h2_slab(p.plan, net, row_begin) * kH2TileF4 + (t & 127);
+  int it = 0;   // this warpgroup's phase-A tile count so far (probe slots 1 + 3 it .. 3 + 3 it of warpgroup 0's first five tiles)
+  for (int vr0 = row_begin + kWgRows * wg; vr0 < row_end; vr0 += kTileRows, ++it) {
+    if (it < 5) TSG(g_ts_fwd, 1 + 3 * it);
     const int r0 = vr0 + 16 * wq + g, r1 = r0 + 8;
     size_t d0u = 0, d1u = 0;
     int agent, unit, off, ep;
@@ -160,10 +165,16 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       layer_rs<16>(acc, hi, lo, sb + kOffW2Hi, sb + kOffW2Lo, 16);
     }
+    if (it < 5) TSG(g_ts_fwd, 2 + 3 * it);
     if (tgt && vr0 + kTileRows >= row_end) online_w2_done();   // this warpgroup's last phase-A tile
     float q0[kOutPad], q1[kOutPad];
     head_quad(acc, b2, w3f, A, tq, q0, q1);   // acc = H2 from here
-    store_frag_fm(p.h2g, p.rows, acc, d0, d1, tq, p.rec, kRecMask2);
+    {
+      float4* h2 = h2s + (size_t)((vr0 - row_begin) / kWgRows) * kH2TileF4;
+#pragma unroll
+      for (int n = 0; n < 16; ++n) h2[n * 128] = make_float4(acc[4 * n], acc[4 * n + 1], acc[4 * n + 2], acc[4 * n + 3]);
+    }
+    store_frag_masks(acc, d0, d1, tq, p.rec, kRecMask2);
     const long long d = tq == 0 ? d0 : d1;
     if (tq < 2 && d >= 0) {
       float* o = p.rec + (size_t)d * kRowRec;
@@ -174,6 +185,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dqn_fwd_kernel(TcTrainParams
         if (p.q_out != nullptr && a < A) p.q_out[(size_t)d * A + a] = v;
       }
     }
+    if (it < 5) TSG(g_ts_fwd, 3 + 3 * it);
   }
   if (!tgt) { TSG(g_ts_fwd, 31); return; }
   if (row_begin + kWgRows * wg >= row_end) online_w2_done();   // no phase-A tile (warpgroup 1 of a CTA of at most 64 rows)
@@ -440,13 +452,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dh1_kernel(TcTrainParams p) 
 // =====================================================================================================================
 //   dW2 | db2 [j2][j1 | 1] += dH2^T x [H1 | 1]^T   (A: 128 lines, B: 136 lines, line 128 = ones)
 //   dW3^T [j][a]           += H2^T x dq^T          (B: 8 lines, dq[r][a] = g_r at a = act_r)
-// Warpgroup w accumulates the M rows [64 w, 64 w + 64) of both.  A2, A3 and B3 are staged per chunk by all eight warps, lane = row; H1 is rebuilt
-// per 64 rows (two chunks) by the warpgroup that ran those rows in the forward (layer1_tile on the W1 panels of the forward image) and staged
-// from its accumulator fragments into two B2 buffers, one per chunk.
-// The FP32 copy of W3 has rows of kW3Pitch = 129 floats: the 32 lanes of a staging warp read W3[act][j] at one j and their rows' actions, and with
-// a pitch of 128 every action would sit in the same bank (up to A-way conflicts on 16 loads per thread and chunk); with 129 they are distinct.
+// Warpgroup w accumulates the M rows [64 w, 64 w + 64) of both.  A2 and A3 are staged per chunk by all eight warps from the forward's fragment
+// order of H2 (h2_slab): thread t loads element groups n = 4 (t / 64) + m (m < 4) of forward thread u = 64 (c % 2) + t % 64, four 16-byte loads
+// of rows cr and cr + 8 (cr = 16 (warp % 2) + lane / 4), columns 8 n + 2 (lane % 4) and + 1; under line_off the 32 lanes of a staging store hit
+// 32 distinct banks.  B3 and db3 are staged lane = row, and the fragment rows take g and act from those lanes by shuffle.  H1 is rebuilt per 64
+// rows (two chunks) by the warpgroup that ran those rows in the forward (layer1_tile on the W1 panels of the forward image) and staged from its
+// accumulator fragments into two B2 buffers, one per chunk.
+// The FP32 copy of W3 has rows of kW3Pitch = 136 floats, read as float2 (columns 8 n + 2 q, + 1): the four lanes of a row cover eight banks from
+// 8 act on, so the four rows of a half-warp sit in distinct banks unless two actions differ by 4 (2-way); with a pitch of 128 every action would
+// sit in the same banks (up to 4-way).
 constexpr int kB2Bytes = 2 * 136 * kLine;                                  // one chunk of [H1 | 1], hi | lo
-constexpr int kW3Pitch = kHidden + 1;
+constexpr int kW3Pitch = kHidden + 8;
 constexpr int kSA2 = 0, kSB2 = kSA2 + 2 * 128 * kLine, kSA3 = kSB2 + 2 * kB2Bytes, kSB3 = kSA3 + 2 * 128 * kLine, kSW1 = kSB3 + 2 * 8 * kLine;
 constexpr int kSW3 = kSW1 + (kOffW2Hi - kOffW1Hi);                         // behind the W1 hi | lo panels of the forward image
 constexpr int kSB1 = kSW3 + (kOutPad * kW3Pitch * 4 + 15) / 16 * 16, kSBar = kSB1 + kHidden * 4;
@@ -507,24 +523,27 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
   float db3 = 0.f;   // warp a, lane 0: sum of dq[.][a]
   bool first = true;
   const int n_chunks = (row_end - row_begin + kChunk - 1) / kChunk;
+  // this thread's H2 of chunk 0: element groups 4 (t / 64) + m of forward thread t % 64 of tile 0 (chunk c: + tile c / 2, + 64 (c % 2) threads)
+  const float4* const h2s = p.h2s + h2_slab(p.plan, net, row_begin) * kH2TileF4 + 4 * (t >> 6) * 128 + (t & 63);
+  const int cr = 16 * (warp & 1) + g;   // this thread's fragment rows of every chunk: cr and cr + 8
   int c = 0;
   do {   // n_chunks >= 1: with a zero-trip path (a for loop) ptxas serialises every wgmma of the kernel (C7515)
     TSG(g_ts_dw, 2 + c);   // chunk c: slots 2-29 (chunks past 27 land on 30 / 31, which the epilogue writes again)
-    // ---- this thread's row (lane) and features (warp + 8 i) of the chunk -> registers; their loads overlap the previous chunk's MMAs
+    // ---- the chunk's rows' g and act (lane = row) and this thread's H2 fragment -> registers; their loads overlap the previous chunk's MMAs
     const int vr = row_begin + c * kChunk + lane;
-    float h2v[16], gr = 0.f;
+    float gr = 0.f;
     int act = 0;
+    if (vr < row_end) {
+      int agent, unit, off;
+      decode_row(p.plan, net, vr, agent, unit, off);
+      const float* rp = p.rec + row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows) * kRowRec;
+      gr = rp[kRecG]; act = __float_as_int(rp[kRecAct]);
+    }
+    float4 h2q[4];
     {
-      long long d = -1;
-      if (vr < row_end) {
-        int agent, unit, off;
-        decode_row(p.plan, net, vr, agent, unit, off);
-        d = (long long)row_index(agent, unit, off, p.plan.units_per_agent, p.plan.unit_rows);
-        const float* rp = p.rec + (size_t)d * kRowRec;
-        gr = rp[kRecG]; act = __float_as_int(rp[kRecAct]);
-      }
+      const float4* src = h2s + (size_t)(c >> 1) * kH2TileF4 + 64 * (c & 1);
 #pragma unroll
-      for (int i = 0; i < 16; ++i) h2v[i] = d >= 0 ? p.h2g[(size_t)(warp + 8 * i) * p.rows + (size_t)d] : 0.f;
+      for (int m = 0; m < 4; ++m) h2q[m] = src[m * 128];
     }
     // ---- H1 of chunks c and c + 1 (even c): the 64 rows of warpgroup (c / 2) % 2 of tile c / 4, as the forward computed them
     const bool rebuild = (c & 1) == 0 && wg == ((c >> 1) & 1);
@@ -540,11 +559,21 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dw_kernel(TcTrainParams p) {
     }
     __syncthreads();   // both warpgroups are done reading the previous chunk
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const int j = warp + 8 * i;
-      const float dh2 = h2v[i] > 0.f ? gr * w3f[act * kW3Pitch + j] : 0.f;
-      stage_hl(smem + kSA2, 128, j, lane, dh2);
-      stage_hl(smem + kSA3, 128, j, lane, h2v[i]);
+    for (int k = 0; k < 2; ++k) {   // row cr + 8 k of the chunk: H2 (0 past the CTA's rows) and dH2 = g W3[act][j] relu'(H2)
+      const int r = cr + 8 * k;
+      const bool live = row_begin + c * kChunk + r < row_end;
+      const float g_r = __shfl_sync(0xFFFFFFFFu, gr, r);
+      const int act_r = __shfl_sync(0xFFFFFFFFu, act, r);
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {
+        const int j = 8 * (4 * (t >> 6) + m) + 2 * tq;
+        const float2 w = *reinterpret_cast<const float2*>(w3f + act_r * kW3Pitch + j);
+        const float h0 = live ? (k ? h2q[m].z : h2q[m].x) : 0.f, h1v = live ? (k ? h2q[m].w : h2q[m].y) : 0.f;
+        stage_hl(smem + kSA2, 128, j, r, h0 > 0.f ? g_r * w.x : 0.f);
+        stage_hl(smem + kSA2, 128, j + 1, r, h1v > 0.f ? g_r * w.y : 0.f);
+        stage_hl(smem + kSA3, 128, j, r, h0);
+        stage_hl(smem + kSA3, 128, j + 1, r, h1v);
+      }
     }
     {
       const float dq = act == warp ? gr : 0.f;   // warp = output a
@@ -619,7 +648,7 @@ int tc_train_init() {
 static TcTrainParams tc_params(const TrainParams& tp, const TcBuffers& buf) {
   TcTrainParams p; memset(&p, 0, sizeof(p));
   p.plan = tp.plan; p.src = tp.src; p.lay = tp.lay; p.images = buf.image; p.bwd_images = buf.bwd_image;
-  p.h2g = buf.h2; p.rec = buf.rec; p.xg = buf.x; p.x_pitch = 8 * ((tp.src.D + 7) / 8); p.rows = buf.rows;
+  p.h2s = reinterpret_cast<float4*>(buf.h2); p.rec = buf.rec; p.xg = buf.x; p.x_pitch = 8 * ((tp.src.D + 7) / 8);
   p.tq = tp.tq; p.td_ext = tp.td_ext; p.td_agent_stride = tp.td_agent_stride; p.gamma = tp.gamma; p.double_q = tp.double_q; p.huber = tp.huber;
   p.scratch = tp.scratch; p.scratch_pitch = tp.scratch_pitch; p.loss_part = tp.loss_part;
   return p;
@@ -630,6 +659,11 @@ int launch_tc_dqn_forward(const TrainParams& tp, const TcBuffers& buf, const uin
   MARL_REQUIRE(tp.lay.in < kMaxObsDim, "tensor-core backward: observation width %d needs a spare column for the bias trick (max %d)", tp.lay.in, kMaxObsDim - 1);
   MARL_REQUIRE(tp.src.mode == 1, "tensor-core backward: rows must be gathered from the trajectory store (mode %d)", tp.src.mode);
   MARL_REQUIRE(tgt_images == nullptr || tq_out != nullptr, "tensor-core training forward: target images without an output buffer");
+  {
+    const RowPlan& pl = tp.plan;
+    const size_t tiles = ((size_t)pl.slot_begin[pl.n_nets] * pl.units_per_agent * pl.unit_rows + kWgRows - 1) / kWgRows + pl.cta_begin[pl.n_nets];
+    MARL_REQUIRE(tiles <= buf.h2_tiles, "tensor-core training forward: the H2 slabs need %zu tiles, %zu allocated", tiles, buf.h2_tiles);
+  }
   TcTrainParams p = tc_params(tp, buf);
   p.tgt_images = tgt_images; p.tq_out = tq_out; p.q_out = q_out;
   return with_k1(tp.src.D, [&](auto k1) {
