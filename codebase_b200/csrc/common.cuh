@@ -138,6 +138,5 @@ int destroy_handle(H* h) {
 int check_device(int device);
 int tc_forward_enabled();
 int tc_backward_enabled();
-int tc_split_exchange_enabled();
 
 }  // namespace marl

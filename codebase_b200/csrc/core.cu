@@ -1,7 +1,6 @@
 // core.cu -- error reporting and device checks shared by every entry point of libmarlb200.
 #include "tc_common.cuh"
 #include <string.h>
-#include <stdlib.h>
 
 namespace marl {
 
@@ -33,10 +32,7 @@ int check_device(int device) {
   return MARL_OK;
 }
 
-static int env_int(const char* name, int dflt) { const char* v = getenv(name); return v && *v ? atoi(v) : dflt; }
 static int g_tc_forward = 1, g_tc_backward = 1;
-static int g_split_exchange = env_int("MARL_SPLIT_EXCHANGE", 0);
-int tc_split_exchange_enabled() { return g_split_exchange; }
 int tc_forward_enabled() { return g_tc_forward; }
 int tc_backward_enabled() { return g_tc_backward; }
 
@@ -49,9 +45,6 @@ extern "C" {
 int marl_set_option(const char* name, int32_t value) {
   if (name && strcmp(name, "tensor_core_forward") == 0) { marl::g_tc_forward = value ? 1 : 0; return MARL_OK; }
   if (name && strcmp(name, "tensor_core_backward") == 0) { marl::g_tc_backward = value ? 1 : 0; return MARL_OK; }
-  /* several ranks: 0 (default) = the gradient exchange inside one fused reduce + Adam kernel; 1 = split into a push kernel and a finishing kernel with the
-   * next update's target forward between them (hides the peer round trip but costs a launch) */
-  if (name && strcmp(name, "split_exchange") == 0) { marl::g_split_exchange = value ? 1 : 0; return MARL_OK; }
   marl::set_error("marl_set_option: unknown option '%s'", name ? name : "(null)");
   return MARL_EINVAL;
 }

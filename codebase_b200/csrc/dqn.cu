@@ -174,8 +174,6 @@ struct marl_dqn : LearnerHandle {
   float *tc_h2 = nullptr, *tc_rec = nullptr, *tc_x = nullptr;
   bool tgt_image_current = false;
   unsigned long long* grid_barrier = nullptr; unsigned long long grid_epoch = 0;   // arrival counter of the fused reduce + Adam kernel
-  unsigned long long push_epoch = 0;   // arrival counter of the push kernel (split exchange)
-  bool tq_ahead = false;               // the target forward of the NEXT update has already been launched (between push and finish)
   // gradient exchange over peer memory (several ranks, one process per GPU): own buffer + the peers' buffers opened through CUDA IPC
   XchgParams xchg = {}; float* xbuf = nullptr; void* peer_base[kMaxRanks] = {};
   // online images: valid = a full pack happened and every later change of theta came from adam_kernel (which updates them in place)
@@ -232,7 +230,7 @@ static int dqn_create(const marl_mlp_cfg* cfg, const marl_dqn_hp* hp, int32_t ma
   if (!rc) rc = dqn_grow_loss_part(h, (size_t)h->n_sm + (size_t)(rnn ? cfg->n_agents : 1) * max_batch * max_T / 256 + 2, who);
   if (!rc)
     rc = alloc_buffers(h, who, {{&h->tq, rows * cfg->out_dim * F}, {&h->loss_dev, 8 * F}, {&h->sumsq, ((size_t)(h->n_params + 63) / 64 + 1) * F},
-                                {&h->grid_barrier, 4 * F}});   // two zero-initialised 64-bit counters (grid barrier, push arrivals)
+                                {&h->grid_barrier, sizeof(unsigned long long)}});   // the grid barrier's zero-initialised 64-bit arrival counter
   // online Q-values of every row for the external TD heads (VDN, QMIX; the recurrent pass always hands the TD error to its backward) and the TD
   // error: VDN one entry per (b, t), QMIX and the recurrent pass one per (agent, b, t)
   if (!rc && (hp->mixer != 0 || rnn))
@@ -272,6 +270,23 @@ int marl_dqn_destroy(marl_dqn* h) {
   return destroy_handle(h);
 }
 
+// (column, b, t) entries of the external TD head at max_batch and max_T: one column per agent (IDQN), one of all agents (VDN, QMIX)
+static size_t dqn_head_entries(const marl_dqn* h) { return (size_t)(h->hp.mixer != 0 ? 1 : h->ns.n_agents) * h->max_batch * h->max_T; }
+
+// The external TD head's buffers (standardise_returns, algorithm.td_lambda), each allocated where missing: returns and chosen Q-values per entry,
+// the online Q-values of every row, the TD error (IDQN's MLP path has none yet; every other learner's was sized at create: QMIX's and the recurrent
+// pass's per agent) and room for the head's loss statistics, one block per 256 entries (QMIX: per tile, sized by marl_dqn_qmix_init).
+static int dqn_external_buffers(marl_dqn* h, const char* who) {
+  const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), cbt = dqn_head_entries(h), F = sizeof(float);
+  if (!h->ret)
+    if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
+  if (!h->q_all)
+    if (int rc = alloc_buffers(h, who, {{&h->q_all, rows * h->ns.out * F}})) return rc;
+  if (!h->td)
+    if (int rc = alloc_buffers(h, who, {{&h->td, cbt * F}})) return rc;
+  return dqn_grow_loss_part(h, (size_t)h->n_sm + cbt / 256 + 2, who);
+}
+
 /* cfg.standardise_returns (dqn/model.py:82-84, 221-222, 357-358): RunningMeanStd over the TD targets, one column per agent (VDN and QMIX: per
  * batch entry, see the kernels above and qmix.cuh); mean 0, var 1, count 1e-4 on first enable. */
 int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
@@ -279,43 +294,23 @@ int marl_dqn_standardise_returns(marl_dqn* h, int32_t enable) {
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   if (enable && !h->ret_ms) {
     const char* who = "marl_dqn_standardise_returns";
-    const int n = h->hp.mixer != 0 ? h->max_batch : h->ns.n_agents, C = h->hp.mixer != 0 ? 1 : h->ns.n_agents;
-    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), cbt = (size_t)C * h->max_batch * h->max_T, F = sizeof(float);
-    if (!h->ret)   // (marl_dqn_set_td_lambda may have allocated them)
-      if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
-    if (!h->q_all)
-      if (int rc = alloc_buffers(h, who, {{&h->q_all, rows * h->ns.out * F}})) return rc;
-    if (!h->td || (h->hp.mixer == 0 && !h->rnn)) {
-      free_buffer(h, &h->td);
-      if (int rc = alloc_buffers(h, who, {{&h->td, cbt * F}})) return rc;
-    }
-    // the per-update loss statistics of this path come from one block per 256 (c, b, t) entries (QMIX: per tile, sized by marl_dqn_qmix_init)
-    if (int rc = dqn_grow_loss_part(h, (size_t)h->n_sm + cbt / 256 + 2, who)) return rc;
-    if (int rc = enable_ret_stats(h, n, who)) return rc;
+    if (int rc = dqn_external_buffers(h, who)) return rc;
+    if (int rc = enable_ret_stats(h, h->hp.mixer != 0 ? h->max_batch : h->ns.n_agents, who)) return rc;
   }
   h->standardise = enable ? 1 : 0;
   return MARL_OK;
 }
 /* algorithm.td_lambda: enable != 0 replaces the one-step TD target of every later update (marl_dqn_update*, update_n, the fused tail) by the λ-return
  * of `lambda` in [0, 1] over the sampled episode (DESIGN.md §4.4d); enable == 0 restores the one-step target.  The first enable allocates the
- * bootstrap values, returns, chosen Q-values, TD error, the online Q-values of every row and the loss statistics' room -- the external TD head's
- * buffers, which IDQN then takes on every path. */
+ * bootstrap values and the rest of the external TD head's buffers, which IDQN then takes on every path. */
 int marl_dqn_set_td_lambda(marl_dqn* h, int32_t enable, float lambda) {
   MARL_REQUIRE(!enable || (lambda >= 0.f && lambda <= 1.f), "marl_dqn_set_td_lambda: lambda %g is outside [0, 1]", (double)lambda);
   MARL_REQUIRE(h != nullptr, "marl_dqn_set_td_lambda: NULL handle");
   MARL_CUDA_TRY(cudaSetDevice(h->device));
   if (enable && !h->boot) {
     const char* who = "marl_dqn_set_td_lambda";
-    const int C = h->hp.mixer != 0 ? 1 : h->ns.n_agents;
-    const size_t rows = (size_t)h->ns.n_agents * h->max_batch * (h->max_T + 1), cbt = (size_t)C * h->max_batch * h->max_T, F = sizeof(float);
-    if (!h->ret)
-      if (int rc = alloc_buffers(h, who, {{&h->ret, cbt * F}, {&h->chosen, cbt * F}})) return rc;
-    if (!h->q_all)
-      if (int rc = alloc_buffers(h, who, {{&h->q_all, rows * h->ns.out * F}})) return rc;
-    if (!h->td)   // IDQN's MLP path has none yet; every other learner's was sized at create
-      if (int rc = alloc_buffers(h, who, {{&h->td, cbt * F}})) return rc;
-    if (int rc = dqn_grow_loss_part(h, (size_t)h->n_sm + cbt / 256 + 2, who)) return rc;
-    if (int rc = alloc_buffers(h, who, {{&h->boot, cbt * F}})) return rc;
+    if (int rc = dqn_external_buffers(h, who)) return rc;
+    if (int rc = alloc_buffers(h, who, {{&h->boot, dqn_head_entries(h) * sizeof(float)}})) return rc;
   }
   h->td_lambda_on = enable != 0;
   h->td_lambda = enable ? lambda : 0.f;
@@ -521,52 +516,62 @@ int marl_replay_sample(uint64_t seed, uint64_t update_idx, int32_t batch, int32_
 
 static bool dqn_external_head(const marl_dqn* h) { return h->hp.mixer != 0 || h->rnn || h->standardise || h->td_lambda_on; }
 
-// algorithm.td_lambda: the λ-returns of C columns (reward of agent c G) from h->boot into h->ret
-static int dqn_td_lambda(const marl_dqn* h, const RowSource& src, int C, int G, int batch, cudaStream_t st) {
-  TdLambdaParams lp; lp.boot = h->boot; lp.traj = src.traj; lp.idx = src.idx; lp.C = C; lp.G = G; lp.B = batch; lp.ret = h->ret;
-  lp.gamma = h->hp.gamma; lp.lambda = h->td_lambda; lp.gl = (float)((double)h->hp.gamma * (double)h->td_lambda);
-  MARL_CUDA_TRY(launch_td_lambda(lp, st));
-  return MARL_OK;
-}
-
-// The external TD head, for the cases the training pass's own head does not cover (QMIX, standardise_returns, VDN, the recurrent pass): the online
-// forward on every row (forward = false: the fused training forward has already written q_all), then dL/dQ of the taken actions into td, which
-// becomes tp.td_ext (per agent at tp.td_agent_stride; VDN: per (b, t), stride 0), and the head's loss statistics into loss_part blocks
-// [n_loss_parts, ...), which n_loss_parts is advanced past.
+// The external TD head, for the cases the training pass's own head does not cover (QMIX, standardise_returns, td_lambda, VDN, the recurrent pass):
+// the online forward on every row (forward = false: the fused training forward has already written q_all), then dL/dQ of the taken actions into td,
+// which becomes tp.td_ext (per agent at tp.td_agent_stride; VDN: per (b, t), stride 0), and the head's loss statistics into loss_part blocks
+// [n_loss_parts, ...), which n_loss_parts is advanced past.  The TD error comes from col_td_kernel over C columns of G agents (VDN: one column of all
+// agents; independent learners: one column per agent) or, for QMIX, from the mixer (qmix.cuh: one column of all agents, agent 0's reward), which
+// hands dL/dq_a back per agent.  Both run the same stage sequence.
 static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, int batch, TrainParams& tp, int& n_loss_parts, bool forward, cudaStream_t st) {
   if (!dqn_external_head(h)) return MARL_OK;
   if (forward)
     if (int rc = dqn_forward(h, plan, src, false, h->q_all, h->gru_save, st)) return rc;
   const int T = src.traj.T;
+  const bool qmix = h->hp.mixer == 2, per_b = h->hp.mixer != 0;   // per_b: the return statistics keep one column per batch entry
+  const int C = per_b ? 1 : h->ns.n_agents, G = h->ns.n_agents / C;
+  const float* ret_ms = h->standardise ? h->ret_ms : nullptr;   // stage 1 needs it; stage 3 de-standardises its bootstrap values exactly when it is set
+  const int n_stat = h->standardise ? h->n_stat : 0;
   float* loss_part = h->loss_part + 4 * (size_t)n_loss_parts;
-  tp.td_ext = h->td;
-  if (h->hp.mixer == 2) {  // QMIX: the mixer turns the agents' Q-values into the TD error and hands dL/dq_a back per agent (qmix.cuh)
-    QmixParams qp; memset(&qp, 0, sizeof(qp));
+  QmixParams qp; memset(&qp, 0, sizeof(qp));
+  ColTdParams cp; memset(&cp, 0, sizeof(cp));
+  int blocks = 0;
+  if (qmix) {
     qp.L = h->ql; qp.q = h->q_all; qp.tq = h->tq; qp.traj = src.traj; qp.idx = src.idx; qp.B = batch; qp.A = h->ns.out; qp.D = h->ns.in;
     qp.gamma = h->hp.gamma; qp.double_q = h->hp.double_q; qp.huber = h->huber; qp.mix = h->mix; qp.mix_tgt = h->mix_tgt; qp.rec = h->mix_rec; qp.td = h->td;
-    qp.loss_part = loss_part;
-    const int Sn = batch * T, qb = (Sn + kQmTS - 1) / kQmTS, n = h->ql.n, hl = h->ql.hl;
-    qmix_pack_kernel<<<dim3((n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
-    if (h->td_lambda_on) {   // target pass -> bootstrap values, λ-return scan (one column, agent 0's reward), [RunningMeanStd step], online pass
-      qp.ret = h->ret; qp.boot = h->boot;
-      if (h->standardise) { qp.ret_ms = h->ret_ms; qp.n_stat = h->n_stat; }
-      qmix_mix_fn(hl, 3)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
-      if (int rc = dqn_td_lambda(h, src, 1, h->ns.n_agents, batch, st)) return rc;
-      if (h->standardise) {
-        RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T; rp.N = batch; rp.P = 1;
-        MARL_CUDA_TRY(ret_ms_step(rp, st));
-      }
-      qmix_mix_fn(hl, 2)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
-    } else if (h->standardise) {   // target pass -> returns, RunningMeanStd step (one column per batch entry), online pass on the standardised returns
-      qp.ret_ms = h->ret_ms; qp.n_stat = h->n_stat; qp.ret = h->ret;
-      qmix_mix_fn(hl, 1)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
-      RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T; rp.N = batch; rp.P = 1;
-      MARL_CUDA_TRY(ret_ms_step(rp, st));
-      qmix_mix_fn(hl, 2)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
-    } else {
-      qmix_mix_fn(hl, 0)<<<qb, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+    qp.loss_part = loss_part; qp.ret_ms = ret_ms; qp.n_stat = n_stat; qp.ret = h->ret; qp.boot = h->boot;
+    blocks = (batch * T + kQmTS - 1) / kQmTS;
+    qmix_pack_kernel<<<dim3((h->ql.n + 255) / 256, 2), 256, 0, st>>>(h->ql, h->mix, h->mix_tgt, h->mix_img, h->mix_img_tgt);
+  } else {
+    cp.q = h->q_all; cp.tq = h->tq; cp.traj = src.traj; cp.idx = src.idx; cp.B = batch; cp.A = h->ns.out;
+    cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.huber = h->huber; cp.C = C; cp.G = G;
+    cp.ret_ms = ret_ms; cp.n_stat = n_stat; cp.stat_per_b = per_b; cp.ret = h->ret; cp.chosen = h->chosen; cp.boot = h->boot;
+    cp.td = h->td; cp.loss_part = loss_part;
+    blocks = (C * batch * T + 255) / 256;
+  }
+  static void (*const col_td_fns[4])(ColTdParams) = {col_td_kernel<0>, col_td_kernel<1>, col_td_kernel<2>, col_td_kernel<3>};
+  const auto stage = [&](int S) {
+    if (qmix) qmix_mix_fn(h->ql.hl, S)<<<blocks, kQmWarps * 32, qm_smem_bytes(h->ql), st>>>(qp, h->mix_img, h->mix_img_tgt);
+    else col_td_fns[S]<<<blocks, 256, 0, st>>>(cp);
+  };
+  if (h->td_lambda_on || h->standardise) {
+    // λ: bootstrap values (+ chosen Q), the λ-return scan; else the one-step returns (+ chosen Q).  Then [RunningMeanStd step], TD error on the returns
+    stage(h->td_lambda_on ? 3 : 1);
+    if (h->td_lambda_on) {
+      TdLambdaParams lp; lp.boot = h->boot; lp.traj = src.traj; lp.idx = src.idx; lp.C = C; lp.G = G; lp.B = batch; lp.ret = h->ret;
+      lp.gamma = h->hp.gamma; lp.lambda = h->td_lambda; lp.gl = (float)((double)h->hp.gamma * (double)h->td_lambda);
+      MARL_CUDA_TRY(launch_td_lambda(lp, st));
     }
-    const int want = h->mix_wgrad_tiles ? kQmixChunks : 2 * h->n_sm;
+    if (h->standardise) {
+      RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T;
+      rp.N = per_b ? batch : C; rp.P = per_b ? 1 : batch;
+      MARL_CUDA_TRY(ret_ms_step(rp, st));
+    }
+    stage(2);
+  } else {
+    stage(0);
+  }
+  if (qmix) {   // the mixer's weight gradient: per-chunk partial sums, then their reduction (with the head's loss statistics)
+    const int Sn = batch * T, n = h->ql.n, want = h->mix_wgrad_tiles ? kQmixChunks : 2 * h->n_sm;
     const int chunk_len = (((Sn + want - 1) / want) + 31) & ~31, chunks = (Sn + chunk_len - 1) / chunk_len;
     if (h->mix_wgrad_tiles) {
       qmix_wgrad_kernel<<<dim3(h->mix_n_tiles, chunks), 256, 0, st>>>(h->mix_rec, Sn, h->mix_tiles, chunk_len, h->mix_part, n);
@@ -574,43 +579,12 @@ static int dqn_td_head(marl_dqn* h, const RowPlan& plan, const RowSource& src, i
       for (int round = 0; round * kQmMicroPerRound < h->mix_n_micro; ++round)
         qmix_wgrad2_kernel<<<chunks, 256, (size_t)(h->ql.R + 2) * kQmP * sizeof(float), st>>>(h->mix_rec, Sn, h->ql.R, h->mix_micro, h->mix_n_micro, round, chunk_len, h->mix_part, n);
     }
-    qmix_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(h->mix_part, chunks, n, h->mix_grad, qp.loss_part, qb);
-    MARL_CUDA_TRY(cudaGetLastError());
-    n_loss_parts += qb;
-    tp.td_agent_stride = batch * T;
-    return MARL_OK;
-  }
-  // VDN: one column of all agents; independent learners: one column per agent
-  const bool vdn = h->hp.mixer == 1;
-  ColTdParams cp; memset(&cp, 0, sizeof(cp));
-  cp.q = h->q_all; cp.tq = h->tq; cp.traj = src.traj; cp.idx = src.idx; cp.B = batch; cp.A = h->ns.out;
-  cp.gamma = h->hp.gamma; cp.double_q = h->hp.double_q; cp.huber = h->huber; cp.C = vdn ? 1 : h->ns.n_agents; cp.G = vdn ? h->ns.n_agents : 1;
-  cp.td = h->td; cp.loss_part = loss_part;
-  const int blocks = (cp.C * batch * T + 255) / 256;
-  if (h->td_lambda_on) {   // bootstrap values + chosen Q, λ-return scan, [RunningMeanStd step], TD error on the (standardised) returns
-    cp.ret = h->ret; cp.chosen = h->chosen; cp.boot = h->boot; cp.stat_per_b = vdn;
-    if (h->standardise) { cp.ret_ms = h->ret_ms; cp.n_stat = h->n_stat; }
-    col_td_kernel<3><<<blocks, 256, 0, st>>>(cp);
-    if (int rc = dqn_td_lambda(h, src, cp.C, cp.G, batch, st)) return rc;
-    if (h->standardise) {
-      RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T;
-      if (vdn) { rp.N = batch; rp.P = 1; } else { rp.N = cp.C; rp.P = batch; }
-      MARL_CUDA_TRY(ret_ms_step(rp, st));
-    }
-    col_td_kernel<2><<<blocks, 256, 0, st>>>(cp);
-  } else if (h->standardise) {   // returns + chosen Q, RunningMeanStd step, TD error on the standardised returns
-    cp.ret_ms = h->ret_ms; cp.n_stat = h->n_stat; cp.stat_per_b = vdn; cp.ret = h->ret; cp.chosen = h->chosen;
-    col_td_kernel<1><<<blocks, 256, 0, st>>>(cp);
-    RetMsParams rp; rp.ret = h->ret; rp.part = h->ret_part; rp.ret_ms = h->ret_ms; rp.count = h->ret_count; rp.T = T;
-    if (vdn) { rp.N = batch; rp.P = 1; } else { rp.N = cp.C; rp.P = batch; }
-    MARL_CUDA_TRY(ret_ms_step(rp, st));
-    col_td_kernel<2><<<blocks, 256, 0, st>>>(cp);
-  } else {
-    col_td_kernel<0><<<blocks, 256, 0, st>>>(cp);
+    qmix_reduce_kernel<<<(n + 255) / 256, 256, 0, st>>>(h->mix_part, chunks, n, h->mix_grad, loss_part, blocks);
   }
   MARL_CUDA_TRY(cudaGetLastError());
   n_loss_parts += blocks;
-  tp.td_agent_stride = vdn ? 0 : batch * T;
+  tp.td_ext = h->td;
+  tp.td_agent_stride = h->hp.mixer == 1 ? 0 : batch * T;
   return MARL_OK;
 }
 
@@ -697,13 +671,11 @@ static int dqn_grads(marl_dqn* h, const marl_traj_view* traj, const int32_t* epi
   tp.gamma = h->hp.gamma; tp.double_q = h->hp.double_q; tp.huber = h->huber; tp.scratch = h->scratch; tp.scratch_pitch = h->scratch_pitch; tp.loss_part = h->loss_part;
   int n_loss_parts = h->rnn ? 0 : plan.cta_begin[plan.n_nets];
   // The target network on every gathered row (dqn/model.py:132-134) runs inside the tensor-core training forward when that pipeline runs with the
-  // tensor-core forward on (an FP32 target forward gives other bits).  Otherwise it is a forward of its own; several ranks with the split exchange:
-  // the previous update launched it between its push and its finish.
-  if (!h->tq_ahead && dqn_tc_train(h) && tc_forward_enabled()) {
+  // tensor-core forward on (an FP32 target forward gives other bits).  Otherwise it is a forward of its own.
+  if (dqn_tc_train(h) && tc_forward_enabled()) {
     if (int rc = dqn_fused_pass(h, plan, src, batch, tp, n_loss_parts, ev, st)) return rc;
   } else {
-    if (h->tq_ahead) h->tq_ahead = false;
-    else if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, st)) return rc;
+    if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, st)) return rc;
     if (ev && h->rnn) cudaEventRecord(ev[0], st);
     if (int rc = dqn_td_head(h, plan, src, batch, tp, n_loss_parts, true, st)) return rc;
     if (ev && !h->rnn) cudaEventRecord(ev[0], st);
@@ -778,23 +750,6 @@ static int dqn_update(marl_dqn* h, const marl_traj_view* traj, const int32_t* ep
   // one kernel for reduce + clip + Adam when its grid fits the GPU in one wave, else the two kernels
   SampleParams sp; memset(&sp, 0, sizeof(sp));
   if (next != nullptr) sp = *next;
-  // Several ranks: the exchange costs a round trip over NVLink (push, flags, poll: 7-10 us per update when exposed).  Split it -- push the local sums
-  // first, then launch the NEXT update's target forward (it needs theta_tgt and the next indices, which the push kernel draws, not this update's Adam
-  // step), then wait for the peers and finish: the wait hides under ~17 us of forward.  Not when this step rewrites theta_tgt.  Off by default: on two
-  // GPUs the extra launch (prologue, second pass over the Adam state) cost more than the hidden wait saved (120.9 vs 116.8 us per update).
-  if (h->xchg.world > 1 && tc_split_exchange_enabled()) {
-    if (launch_reduce_push(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->push_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
-      if (next != nullptr && ap.target_mode == 0 && !dqn_external_head(h)) {
-        const RowPlan plan = episode_plan(h->ns, batch, traj->T, h->n_sm);
-        const RowSource src = episode_rows(traj, next->idx, h->ns.n_agents, h->ns.in);
-        if (int rc = dqn_forward(h, plan, src, true, h->tq, nullptr, (cudaStream_t)stream)) return rc;
-        h->tq_ahead = true;
-      }
-      if (int rc = launch_adam_finish(rp, ap, h->opt.kind, &h->xchg, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream)) return rc;
-      if (fused_out) *fused_out = true;
-      return qmix_adam(h, ap, (cudaStream_t)stream);
-    }
-  }
   if (launch_reduce_adam(rp, ap, h->opt.kind, &h->xchg, sp, h->grid_barrier, &h->grid_epoch, h->n_sm, (cudaStream_t)stream) == MARL_OK) {
     if (fused_out) *fused_out = true;
     return qmix_adam(h, ap, (cudaStream_t)stream);
@@ -858,10 +813,9 @@ int marl_dqn_params_changed(marl_dqn* h) {
 }
 
 /* Per-kernel split of the launches timed by the last marl_dqn_timing(1) .. marl_dqn_timing(0) window: summed CUDA-event durations of
- * the three kernels of the tensor-core training pass (training forward, dH1 + TD head, weight gradients).  With the tensor-core forward on
- * (and no split exchange), slot 0 is the forward of both the online and the target network, and for VDN, QMIX and standardise_returns slot 1
- * includes the external TD head that runs between the forward and the dH1 kernel.  *count = 0 when the window ran the single fused FP32
- * kernel instead. */
+ * the three kernels of the tensor-core training pass (training forward, dH1 + TD head, weight gradients).  With the tensor-core forward on,
+ * slot 0 is the forward of both the online and the target network, and for VDN, QMIX and standardise_returns slot 1 includes the external TD
+ * head that runs between the forward and the dH1 kernel.  *count = 0 when the window ran the single fused FP32 kernel instead. */
 int marl_dqn_timing_kernels(marl_dqn* h, float* ms3, int32_t* count) {
   MARL_REQUIRE(h != nullptr && ms3 != nullptr, "marl_dqn_timing_kernels: NULL argument");
   MARL_REQUIRE(!h->timing, "marl_dqn_timing_kernels: call marl_dqn_timing(q, 0, ...) first");

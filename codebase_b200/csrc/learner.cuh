@@ -206,10 +206,6 @@ struct SampleParams { uint64_t seed, update_idx; int batch, n_valid; int32_t* id
 // opt: the OptKind of the step
 int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
                        unsigned long long* epoch, int n_sm, cudaStream_t st);
-int launch_reduce_push(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
-                       unsigned long long* push_epoch, int n_sm, cudaStream_t st);
-int launch_adam_finish(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, unsigned long long* barrier, unsigned long long* epoch, int n_sm,
-                       cudaStream_t st);
 int launch_adam(const AdamParams& p, int opt, cudaStream_t st);
 // can the fused tail with optimiser `opt` cover n parameters with one co-resident wave on n_sm SMs?  (pb, ns: the block shape it would use)
 int reduce_adam_shape(int n, int n_sm, bool xchg, int opt, int* pb, int* ns);

@@ -517,10 +517,7 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* barrier, unsign
 
 TSG_DEFINE(g_ts_adam)
 TSG_GETTER(tsg_adam, g_ts_adam)
-// MODE 0: one GPU.  1: several ranks, exchange inside this kernel (push, grid barrier, flags, poll, sum).  2 + 3: the same exchange split over two
-// launches so that the wait for the peers hides under other work (the next update's target forward runs between them): 2 = reduce + push; the LAST
-// block to finish its pushes publishes this rank's epoch flags (an arrival counter, nobody spins) and the next update's replay indices are drawn here;
-// 3 = poll the local flags, sum the ranks' copies, clip + Adam.
+// MODE 0: one GPU.  1: several ranks, exchange inside this kernel (push, grid barrier, flags, poll, sum).
 template <int MODE, int OPT>
 __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams rp, AdamParams ap, XchgParams xp, SampleParams sp, int pb, int ns,
                                                                     unsigned long long* barrier, unsigned long long target) {
@@ -536,7 +533,7 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
   pdl_launch_dependents();
   TSG(g_ts_adam, 1);
   float s = 0.f;
-  if (MODE != 3 && i < n) {
+  if (i < n) {
     const int net = i / rp.P, j = i - net * rp.P;
     const int c0 = rp.cta_begin[net], c1 = rp.cta_begin[net + 1];
     const float* base = rp.scratch + j;
@@ -552,28 +549,28 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
   }
   // this thread's optimiser state: the loads fly under the reductions and barriers below
   float m_i = 0.f, v_i = 0.f, th_i = 0.f;
-  if (MODE != 2 && q == 0 && i < ap.n) { m_i = ap.m[i]; v_i = ap.v[i]; th_i = ap.theta[i]; }   // (loads an optimiser does not use are dead code)
+  if (q == 0 && i < ap.n) { m_i = ap.m[i]; v_i = ap.v[i]; th_i = ap.theta[i]; }   // (loads an optimiser does not use are dead code)
   part[q][lane] = s;
   __syncthreads();
   TSG(g_ts_adam, 2);
   float g = 0.f;
   // this rank's copy inside rank r's buffer: base_r + ((epoch & 1) * world + rank) * slot_floats
   const size_t push_off = XCHG ? ((size_t)(xp.epoch & 1ULL) * xp.world + xp.rank) * xp.slot_floats : 0;
-  if (MODE != 3 && q == 0) {
+  if (q == 0) {
     g = part[0][lane];
     for (int k = 1; k < ns; ++k) g += part[k][lane];
     if (i >= n) g = 0.f;
     else if (XCHG) { for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + i] = g; }   // local sums -> every rank (own included)
     else rp.grad[i] = g;
   }
-  if (XCHG && MODE != 3) {   // the second buffer's local sums -> every rank (grid-stride: any n_extra fits)
+  if (XCHG) {   // the second buffer's local sums -> every rank (grid-stride: any n_extra fits)
     for (int k = blockIdx.x * (int)blockDim.x + t; k < xp.n_extra; k += (int)(gridDim.x * blockDim.x)) {
       const float e = xp.extra[k];
       for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + n + k] = e;
     }
   }
   // the four loss statistics: one warp each of block 0, fixed order
-  if (MODE != 3 && blockIdx.x == 0 && t >= pb && t < pb + 128) {   // (the launcher guarantees ns >= 2 and pb >= 128)
+  if (blockIdx.x == 0 && t >= pb && t < pb + 128) {   // (the launcher guarantees ns >= 2 and pb >= 128)
     const int which = (t - pb) >> 5, l = t & 31;
     float x = 0.f;
     for (int c = l; c < rp.n_loss_parts; c += 32) x += rp.loss_part[4 * c + which];
@@ -584,32 +581,10 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
       if (XCHG) { for (int r = 0; r < xp.world; ++r) xp.peers[r][push_off + n + xp.n_extra + which] = x; } else rp.stats[which] = x;
     }
   }
-  if (MODE == 2) {
-    // ---- push only: this block's pushes become visible system-wide, it arrives; the last block to arrive publishes the epoch.  `barrier` + 1 is this
-    // kernel's own arrival counter (never reset: `target` is its value once this launch has fully arrived)
-    if (sp.idx != nullptr) {   // replay indices of the NEXT update: its target forward runs before the finishing kernel
-      for (int k = blockIdx.x * (int)blockDim.x + t; k < sp.batch; k += (int)(gridDim.x * blockDim.x)) {
-        const u32x4 b = philox4x32_10((uint32_t)sp.update_idx, (uint32_t)(sp.update_idx >> 32), (uint32_t)(k >> 2), 0u, (uint32_t)sp.seed, (uint32_t)(sp.seed >> 32) ^ kTagSample);
-        sp.idx[k] = (int32_t)bounded(pick(b, k & 3), (uint32_t)sp.n_valid);
-      }
-    }
-    __syncthreads();
-    if (t == 0) {
-      __threadfence_system();
-      const unsigned long long arrived = atomicAdd(barrier + 1, 1ULL) + 1ULL;
-      if (arrived == target) {
-        __threadfence_system();
-        for (int r = 0; r < xp.world; ++r) st_release_sys(xp.peer_flags[r] + xp.rank, xp.epoch);   // my flag on every rank
-      }
-    }
-    return;
-  }
   if (XCHG) {
     // ---- exchange: local sums visible system-wide -> publish the epoch -> wait for every peer -> sum in rank order -----------------
-    if (MODE == 1) {
-      grid_barrier(barrier, target - gridDim.x, true);   // every block's pushes are ordered before the flags (system-scope fences)
-      if (blockIdx.x == 0 && t < xp.world) st_release_sys(xp.peer_flags[t] + xp.rank, xp.epoch);   // my flag on rank t
-    }
+    grid_barrier(barrier, target - gridDim.x, true);   // every block's pushes are ordered before the flags (system-scope fences)
+    if (blockIdx.x == 0 && t < xp.world) st_release_sys(xp.peer_flags[t] + xp.rank, xp.epoch);   // my flag on rank t
     if (t < xp.world) {   // local polling only; bounded: a rank that died / skipped an update must not hang this GPU for ever
       const long long t0 = clock64();
       while (ld_acquire_sys(xp.own_flags + t) < xp.epoch) {
@@ -630,7 +605,6 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
       if (blockIdx.x == 0) { rp.stats[t] = x; if (xp.n_extra > 0) xp.extra[xp.n_extra + t] = x; }
     }
     // the second buffer's all-rank sum, in rank order, in place: every block has pushed (read) its entries before the grid barrier above
-    // (MODE 1) or in the previous launch (MODE 3)
     for (int k = blockIdx.x * (int)blockDim.x + t; k < xp.n_extra; k += (int)(gridDim.x * blockDim.x)) {
       float e = 0.f;
       for (int r = 0; r < xp.world; ++r) e += ld_relaxed_sys(mine + (size_t)r * xp.slot_floats + n + k);
@@ -688,7 +662,7 @@ __global__ void __launch_bounds__(kFusedThreads) reduce_adam_kernel(ReduceParams
   }
   // replay indices of the NEXT update (marl_dqn_update_n): np.random.randint(0, len(rb), batch) from the Philox stream -- every reader of
   // the current indices has completed (this kernel runs after the weight-gradient kernel), and the next sample launch is saved
-  if (MODE != 3 && sp.idx != nullptr) {
+  if (sp.idx != nullptr) {
     for (int k = blockIdx.x * (int)blockDim.x + t; k < sp.batch; k += (int)(gridDim.x * blockDim.x)) {
       const u32x4 b = philox4x32_10((uint32_t)sp.update_idx, (uint32_t)(sp.update_idx >> 32), (uint32_t)(k >> 2), 0u, (uint32_t)sp.seed, (uint32_t)(sp.seed >> 32) ^ kTagSample);
       sp.idx[k] = (int32_t)bounded(pick(b, k & 3), (uint32_t)sp.n_valid);
@@ -760,8 +734,7 @@ int launch_grad_reduce(const ReduceParams& p, cudaStream_t st) {
   return MARL_OK;
 }
 
-// Every instantiation of the two step kernels, by (mode, optimiser).  Mode 2 (push only) returns before the step: one instantiation serves
-// every optimiser.
+// Every instantiation of the two step kernels, by (mode, optimiser).
 using TailFn = void (*)(ReduceParams, AdamParams, XchgParams, SampleParams, int, int, unsigned long long*, unsigned long long);
 template <int MODE>
 static TailFn tail_fn_mode(int opt) {
@@ -769,14 +742,7 @@ static TailFn tail_fn_mode(int opt) {
                                       reduce_adam_kernel<MODE, kOptAdagrad>, reduce_adam_kernel<MODE, kOptSgd>};
   return fns[opt];
 }
-static TailFn tail_fn(int mode, int opt) {
-  switch (mode) {
-    case 0: return tail_fn_mode<0>(opt);
-    case 1: return tail_fn_mode<1>(opt);
-    case 2: return reduce_adam_kernel<2, kOptAdam>;
-    default: return tail_fn_mode<3>(opt);
-  }
-}
+static TailFn tail_fn(bool xchg, int opt) { return xchg ? tail_fn_mode<1>(opt) : tail_fn_mode<0>(opt); }
 using StepFn = void (*)(AdamParams);
 static StepFn step_fn(int opt) {
   static const StepFn fns[kNumOpt] = {adam_kernel<kOptAdam>, adam_kernel<kOptAdamW>, adam_kernel<kOptRmsprop>, adam_kernel<kOptAdagrad>, adam_kernel<kOptSgd>};
@@ -790,15 +756,7 @@ static int tail_occupancy(bool xchg, int opt, int* oc_out) {
   int& oc = occ[xchg][opt];
   if (oc == 0) {
     int o = 0;
-    if (xchg) {   // the split form shares the block shape: the smaller occupancy of the three variants counts
-      int o1 = 0, o2 = 0, o3 = 0;
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o1, tail_fn(1, opt), kFusedThreads, 0));
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o2, tail_fn(2, opt), kFusedThreads, 0));
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o3, tail_fn(3, opt), kFusedThreads, 0));
-      o = o1 < o2 ? o1 : o2; o = o < o3 ? o : o3;
-    } else {
-      MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, tail_fn(0, opt), kFusedThreads, 0));
-    }
+    MARL_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, tail_fn(xchg, opt), kFusedThreads, 0));
     oc = o > 0 ? o : -1;
   }
   *oc_out = oc;
@@ -835,38 +793,9 @@ int launch_reduce_adam(const ReduceParams& rp, const AdamParams& ap, int opt, Xc
   if (xchg) {
     xp->epoch += 1;
     x = *xp;
-    *epoch += 2ULL * (unsigned long long)grid;               // two arrival rounds
-    MARL_CUDA_TRY(launch_pdl(tail_fn(1, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
-  } else {
-    *epoch += (unsigned long long)grid;
-    MARL_CUDA_TRY(launch_pdl(tail_fn(0, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
   }
-  return MARL_OK;
-}
-
-// The exchange split over two launches (several ranks): launch_reduce_push, then whatever should hide the wait for the peers, then launch_adam_finish.
-// barrier[0] counts the finishing kernel's grid-barrier arrivals, barrier[1] the pushing kernel's block arrivals (epoch / push_epoch: their values once
-// the respective launch has fully arrived).
-int launch_reduce_push(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, const SampleParams& sp, unsigned long long* barrier,
-                       unsigned long long* push_epoch, int n_sm, cudaStream_t st) {
-  const int n = rp.n_nets * rp.P;
-  int pb = 0, ns = 0;
-  if (xp == nullptr || xp->world <= 1 || ap.n != n || reduce_adam_shape(n, n_sm, true, opt, &pb, &ns) != MARL_OK) return MARL_EINVAL;
-  const int grid = (n + pb - 1) / pb;
-  xp->epoch += 1;
-  *push_epoch += (unsigned long long)grid;
-  MARL_CUDA_TRY(launch_pdl(tail_fn(2, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, *xp, sp, pb, ns, barrier, *push_epoch));
-  return MARL_OK;
-}
-int launch_adam_finish(const ReduceParams& rp, const AdamParams& ap, int opt, XchgParams* xp, unsigned long long* barrier, unsigned long long* epoch, int n_sm,
-                       cudaStream_t st) {
-  const int n = rp.n_nets * rp.P;
-  int pb = 0, ns = 0;
-  if (xp == nullptr || xp->world <= 1 || reduce_adam_shape(n, n_sm, true, opt, &pb, &ns) != MARL_OK) return MARL_EINVAL;
-  const int grid = (n + pb - 1) / pb;
-  SampleParams none; memset(&none, 0, sizeof(none));
-  *epoch += (unsigned long long)grid;                          // one arrival round
-  MARL_CUDA_TRY(launch_pdl(tail_fn(3, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, *xp, none, pb, ns, barrier, *epoch));
+  *epoch += (xchg ? 2ULL : 1ULL) * (unsigned long long)grid;   // arrival rounds: the exchange adds one before the flags
+  MARL_CUDA_TRY(launch_pdl(tail_fn(xchg, opt), dim3(grid), dim3(pb * ns), 0, st, rp, ap, x, sp, pb, ns, barrier, *epoch));
   return MARL_OK;
 }
 
@@ -944,8 +873,8 @@ int marl_debug_tail_run(const marl_debug_tail* t, const marl_optimizer* opt, int
   // a fresh barrier counter: the state a handle's first update sees
   unsigned long long* barrier = nullptr;
   unsigned long long epoch = 0;
-  MARL_CUDA_TRY(cudaMallocAsync((void**)&barrier, 2 * sizeof(unsigned long long), st));
-  MARL_CUDA_TRY(cudaMemsetAsync(barrier, 0, 2 * sizeof(unsigned long long), st));
+  MARL_CUDA_TRY(cudaMallocAsync((void**)&barrier, sizeof(unsigned long long), st));
+  MARL_CUDA_TRY(cudaMemsetAsync(barrier, 0, sizeof(unsigned long long), st));
   SampleParams sp; memset(&sp, 0, sizeof(sp));
   const int rc = launch_reduce_adam(rp, ap, opt->kind, nullptr, sp, barrier, &epoch, n_sm, st);
   MARL_CUDA_TRY(cudaFreeAsync(barrier, st));

@@ -33,8 +33,7 @@ extern "C" {
 int marl_version(void);
 const char* marl_last_error(void);
 /* Process-wide options: "tensor_core_forward" 1 (default) = forward-only passes on the tensor cores (wgmma) with the 3xTF32 split, 0 = FP32 FFMA;
- * "tensor_core_backward" 1 = the DQN-family training pass runs as the three-kernel wgmma pipeline (tc_train.cu), 0 = fused FP32 kernel;
- * "split_exchange" (several ranks) 1 = gradient exchange split around the next update's target forward. */
+ * "tensor_core_backward" 1 = the DQN-family training pass runs as the three-kernel wgmma pipeline (tc_train.cu), 0 = fused FP32 kernel. */
 int marl_set_option(const char* name, int32_t value);
 /* Profiling builds (-DMARL_TC_TIMESTAMPS): timeline probes of kernel `which` as uint64 [160 CTAs][32 slots][globaltimer ns, clock64] into HOST
  * memory; product builds return MARL_EINVAL. */
